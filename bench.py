@@ -2,7 +2,7 @@
 """bench.py -- BA solver iterations/s on synthetic sliding windows (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W [--batch B] [--iters I] [--impl reference]
-                    [--cams mono|stereo|quad] [--rho-sweep] [--swarm-agents A --swarms S]
+                    [--cams mono|stereo|quad] [--rho-sweep] [--swarm-agents A --swarms S] [--dump-outputs DIR]
 
 A "step" = one solve of `iters` trust-region iterations (fixed schedule, convergence exits off so the
 work per step is constant) on every window of the batch.  An iteration = one trust-region step attempt:
@@ -17,6 +17,9 @@ carries (a) `latency_b1`: one window through the reference-style reset -> add ->
 handle on one GPU (ADMM, consensus reduced on the device) next to the CPU path with 4 threads and with all cores.
 N>1 (configs[2], [3]): N-drone swarms, one agent per GPU, ADMM with the NCCL consensus exchange per sub-step; every rank
 solves its agent's window of B swarms.  `--cams quad --rho-sweep` is config 4's quadcam / rho sweep mode.
+`--dump-outputs DIR` writes what the last timed step solved (the windows' poses, speed/biases, inverse depths and final
+costs, float64 .npy; every window up to 64 MB, a fixed seeded sample of windows beyond, listed in windows.npy) to DIR, so
+that two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import contextlib
@@ -102,6 +105,18 @@ class ClockSampler:
                     reasons.add(nm)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": float(max(mx)) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def gpu_identity(index=0):
+    """Card name and power limit: a measured number belongs with what it was measured on."""
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power = [x.strip() for x in q.split(",")]
+        return {"name": name, "power_limit": power}
+    except Exception:
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit": None}
 
 
 @contextlib.contextmanager
@@ -287,13 +302,14 @@ def run_reference(args, rank, world):
 # ------------------------------------------------------------------------------------------------ our arm: helpers
 def timed_solves(solver, probs, iters, steps, warmup, barrier=None, step_barrier=None):
     """Device-resident throughput: problem already in HBM, only the (small) state is restored per step.
-    -> (device seconds summed over steps [CUDA events on the solver stream], wall seconds)"""
+    -> (device seconds summed over steps [CUDA events on the solver stream], wall seconds, reports of the last step)"""
     for _ in range(warmup):
         reset_state(solver, probs); solver.solve_fixed(iters)
     if barrier:
         barrier()
     t0 = time.perf_counter()
     dev_ms = 0.0
+    reps = None
     for _ in range(steps):
         reset_state(solver, probs)
         if step_barrier:
@@ -302,7 +318,30 @@ def timed_solves(solver, probs, iters, steps, warmup, barrier=None, step_barrier
         dev_ms += reps[0].total_time * 1e3
     if barrier:
         barrier()
-    return dev_ms * 1e-3, time.perf_counter() - t0
+    return dev_ms * 1e-3, time.perf_counter() - t0, reps
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(path, solver, probs, reps):
+    """The solved state of the windows as the caller of the timed path reads it back, windows concatenated in order:
+    every window while that fits in DUMP_LIMIT_BYTES, otherwise a fixed, seeded sample of windows (windows.npy lists
+    which, in both cases)."""
+    per_window = [8 * (7 * len(p["frame_ids"]) + 9 * len(p["sb_ids"]) + len(p["lm_ids"]) + 2) for p in probs]
+    budget = DUMP_LIMIT_BYTES - 4096   # the .npy headers
+    win = np.arange(len(probs))
+    if sum(per_window) > budget:
+        n = int(budget // max(per_window))
+        win = np.sort(np.random.default_rng(0).choice(len(probs), size=n, replace=False))
+    os.makedirs(path, exist_ok=True)
+    out = {"poses": [solver.get_blocks(i, abi.POSE, probs[i]["frame_ids"]) for i in win],
+           "speed_bias": [solver.get_blocks(i, abi.SPEED_BIAS, probs[i]["sb_ids"]) for i in win],
+           "inv_depth": [solver.get_blocks(i, abi.LANDMARK, probs[i]["lm_ids"]).reshape(-1) for i in win]}
+    for k, v in out.items():
+        np.save(os.path.join(path, k + ".npy"), np.concatenate(v).astype(np.float64))
+    np.save(os.path.join(path, "final_cost.npy"), np.array([reps[i].final_cost for i in win], dtype=np.float64))
+    np.save(os.path.join(path, "windows.npy"), win.astype(np.float64))
 
 
 def latency_b1(local_rank, iters, cams):
@@ -362,7 +401,7 @@ def swarm_one_gpu(args, local_rank, n_agents, n_swarms, iters, steps, warmup, cp
         out["final_cost_mean"] = float(np.mean([r.final_cost for r in reps]))
         s.close()
         return out
-    dev_s, wall_s = timed_solves(s, probs, iters, steps, warmup)
+    dev_s, wall_s, _ = timed_solves(s, probs, iters, steps, warmup)
     out["value"] = len(probs) * iters * steps / dev_s
     out["ms_per_step"] = dev_s / steps * 1e3
     reset_state(s, probs)
@@ -518,8 +557,10 @@ def run_ours(args, rank, world, local_rank):
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    t_dev, wall = timed_solves(solver, probs, iters, args.steps, args.warmup, barrier, barrier if swarm else None)
+    t_dev, wall, last_reps = timed_solves(solver, probs, iters, args.steps, args.warmup, barrier, barrier if swarm else None)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, f"rank{rank}"), solver, probs, last_reps)
     tt = torch.tensor([wall, t_dev], dtype=torch.float64, device="cuda")
     if dist is not None:
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
@@ -616,17 +657,9 @@ def run_ours(args, rank, world, local_rank):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6650 GB/s"
+    peak = float(peaks.get("hbm_gbs", 3350.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "H100 SXM data sheet, 3350 GB/s"
     dom = max(kt, key=kt.get)
     proj_gbs = B * proj_bytes / (kt["proj_lin"] * 1e-3) / 1e9
-    traffic = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        traffic = tj.get("proj_lin_pp_bytes_per_launch", tj.get("proj_lin_bytes_per_launch"))
-        if traffic is not None:
-            traffic = float(traffic) * B / float(tj.get("batch", B))   # captured at another batch size: scale per window
-    except Exception:
-        pass
     extra = {}
     if world == 1:
         # CPU baseline on rank 0, bounded sample, one thread (ceres_options.num_threads = 1)
@@ -659,7 +692,7 @@ def run_ours(args, rank, world, local_rank):
                                 f"W1 single-drone 11-frame/300-landmark windows ({args.cams}; configs[1]); batch of {B} independent windows per GPU, "
                                 f"{iters} trust-region iterations per solve, fixed schedule"),
                    "windows_per_gpu": B, "iters_per_solve": iters, "frames": 11, "landmarks": 300, "residual_blocks": len(probs[0]["obs"]) + 11,
-                   "l2_policy": "inputs larger than L2 (batch working set >> 126 MB)" if B >= 128 else "batch smaller than L2",
+                   "l2_policy": "inputs larger than L2 (batch working set >> 50 MB)" if B >= 128 else "batch smaller than L2",
                    "wall_ms_per_step": wall_max * 1e3 / args.steps, "bytes_iter_per_window": int(bi),
                    "weak_scaling_note": ("the per-GPU work GROWS with N: an agent's window holds 11 own + 11 (N-1) remote pose blocks and the cross-drone observations, so "
                                          "value(N) / (N value(1)) mixes hardware scaling with a larger problem per GPU") if swarm else None},
@@ -669,11 +702,12 @@ def run_ours(args, rank, world, local_rank):
                 "ms_per_step_breakdown": e2e_breakdown,
                 "note": "every step runs the full C-ABI sequence from HOST buffers: d2ba_reset + set_blocks/add_proj/add_imu/set_prior_info + d2ba_finalize (order, tile plan, pinned H2D) + d2ba_solve_fixed + d2ba_get_blocks (D2H), driven by the C++ harness; with handles_in_flight > 1 consecutive steps overlap on independent handles"},
         "roofline": {"bound": "hbm", "kernel": "k_proj_lin_pp (reprojection linearisation + group J^T J)", "achieved": proj_gbs, "peak": peak, "unit": "GB/s", "frac": proj_gbs / peak,
-                     "traffic": traffic, "peak_source": peak_src, "dominant_kernel_by_time": dom,
+                     "peak_source": peak_src, "dominant_kernel_by_time": dom,
                      "algorithmic_bytes_per_launch": int(B * proj_bytes), "kernel_ms_per_iteration": kt,
                      "whole_iteration_frac": B * bi / (sum(kt.values()) * 1e-3) / 1e9 / peak},
         "cpu_baseline": cpu_baseline,
         "clocks": clocks,
+        "gpu": gpu_identity(local_rank),
     }
     if parity is not None:
         line["parity_check"] = parity
@@ -690,19 +724,24 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--batch", type=int, default=592)   # 4 x 148 SMs: whole waves of the one-CTA-per-window kernels
+    ap.add_argument("--batch", type=int, default=528)   # 4 x 132 SMs (H100 SXM): whole waves of the one-CTA-per-window kernels
     ap.add_argument("--iters", type=int, default=8)
     ap.add_argument("--cpu-windows", type=int, default=96)
     ap.add_argument("--admm-steps", type=int, default=4)
     ap.add_argument("--cams", default="mono", choices=["mono", "stereo", "quad"])
     ap.add_argument("--rho-sweep", action="store_true")
     ap.add_argument("--swarm-agents", type=int, default=4)   # north-star leg at N=1: 4-agent swarms on one GPU
-    ap.add_argument("--swarms", type=int, default=148)
+    ap.add_argument("--swarms", type=int, default=132)
     ap.add_argument("--handles", type=int, default=4)
     ap.add_argument("--host-threads", type=int, default=0, help="feeding / planning threads per stage of the e2e leg (0 = min(cores, 32))")
     ap.add_argument("--no-extras", action="store_true", help="N=1: skip the latency_b1 / swarm_1gpu legs")
     ap.add_argument("--impl", default="ours")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's solved state to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's solved state; the reference arm has none")
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     # watchdog: a rank stuck in a collective must not hang the launcher -- dump every thread's Python stack and exit
     import faulthandler

@@ -1,4 +1,4 @@
-"""Builds libd2ba.so (sm_100a) in-tree with nvcc.  `python -m d2slam_b200.build`."""
+"""Builds libd2ba.so (sm_90a) in-tree with nvcc.  `python -m d2slam_b200.build`."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ OUT = os.environ.get("D2BA_OUT") or os.path.join(HERE, "libd2ba.so")
 SOURCES = ["d2ba_kernels.cu", "d2ba_host.cu", "d2ba_margin.cu", "d2pgo.cu"]
 EXTRA_DEPS = ["d2ba_harness.cpp"]
 HEADERS = ["d2ba_types.cuh", "d2ba_math.cuh", "d2ba_proj.cuh", os.path.join("..", "..", "include", "d2ba.h"), os.path.join("..", "..", "include", "d2pgo.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -41,7 +41,7 @@ def build(force=False, verbose=False):
         if p.returncode != 0:
             sys.stderr.write("\n".join(log))
             raise RuntimeError(f"nvcc failed on {s}")
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT] + objs + ["-lcudart", "-ldl"]
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", OUT] + objs + ["-lcudart", "-ldl"]
     subprocess.check_call(link)
     # host-side harness (C++ stand-in for the D2Estimator call sequence), links against libd2ba.so
     harness = os.path.join(HERE, "libd2ba_harness.so")

@@ -841,7 +841,9 @@ int d2ba_finalize(d2ba_handle *h) {
   size_t total_obs = 0;
   for (int i = 0; i < nw; i++) total_obs += h->win[i].obs.size();
   const int tiles_est = (int)(total_obs / kTile) + nw;
-  const int tpj_target = std::max(1, std::min(8, tiles_est / (148 * 8)));
+  int n_sm = 132;   // H100 SXM; the device's own count when it can be read
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->cfg.device);
+  const int tpj_target = std::max(1, std::min(8, tiles_est / (n_sm * 8)));
   // ---- pass A (parallel): columns, pair-major order, groups, tiles, jobs, Schur tiles
   parallel_for(nw, [&](int wi) {
     HostWin &w = h->win[wi];

@@ -1,4 +1,4 @@
-// d2ba_kernels.cu -- sm_100a kernels of the sliding-window BA solver (DESIGN.md section 4).
+// d2ba_kernels.cu -- sm_90a kernels of the sliding-window BA solver (DESIGN.md section 4).
 //
 //   k_state_prep      rotation matrices of every six-dof block
 //   k_imu_prep        IMU sqrt-information U = chol(cov^-1)^T            (imu_factor.h:29)
@@ -1513,8 +1513,8 @@ __global__ void __launch_bounds__(kCholThreads) k_chol(Dev d, int max_rows) {
 //   (3) trailing update on the fp64 tensor cores: 8x8 output tiles, two DMMA m8n8k4 per tile, operands from a
 //       transposed copy of the panel; the tile column of the next panel first, then warp 0 factors the next
 //       diagonal block while the other warps update the rest.
-// Then blocked back substitution, all from shared memory.  (Measured on B200: DFMA latency 8.7 cycles, DMMA 26,
-// shuffle 30, dependent LDS ~30; DMMA and DFMA have the same peak, so the tensor-core form wins on issue slots.)
+// Then blocked back substitution, all from shared memory.  (H100's fp64 tensor-core peak is twice its DFMA peak, and
+// one DMMA m8n8k4 (256 FMAs per warp) does the work of 8 DFMA per lane, so the tensor-core form wins on issue slots.)
 constexpr int kCsThreads = 512;
 constexpr int kCsNB = 8;
 __host__ __device__ inline int chol_smem_ld(int n) { return (n + 1) & ~1; }

@@ -1,4 +1,4 @@
-// d2ba_types.cuh -- device-visible data layout of libd2ba (sm_100a).
+// d2ba_types.cuh -- device-visible data layout of libd2ba (sm_90a).
 //
 // HBM layout (DESIGN.md section 3).  One handle holds B windows; every array below is a single
 // allocation shared by all windows, indexed through the per-window WinDesc offsets so that one

@@ -25,7 +25,7 @@ def lib():
     if _LIB is None:
         p = lib_path()
         if not os.path.exists(p):
-            raise RuntimeError(f"{p} not built: run `python -m d2slam_b200.build` (nvcc, sm_100a). No CPU fallback exists.")
+            raise RuntimeError(f"{p} not built: run `python -m d2slam_b200.build` (nvcc, sm_90a). No CPU fallback exists.")
         # torch bundles the NCCL the library dlopens lazily; make it discoverable without importing torch
         if "D2BA_NCCL_LIB" not in os.environ:
             try:

@@ -1,5 +1,5 @@
 /*
- * d2ba.h -- C ABI of libd2ba.so: the Blackwell-native sliding-window visual-inertial
+ * d2ba.h -- C ABI of libd2ba.so: the Hopper-native (sm_90a) sliding-window visual-inertial
  * bundle-adjustment solver that replaces the Ceres-backed hot path of D2SLAM's d2vins.
  *
  * Drop-in boundary (SURVEY.md section 8b).  Each entry point names the reference

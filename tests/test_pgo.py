@@ -1,11 +1,16 @@
 """Pose-graph path (include/d2pgo.h, BASELINE config 5 / SURVEY 8f rank 3): factor restatement vs finite differences,
 g2o round trip in the reference's multi-agent id convention, edge sharding == full product (gloo-free numpy check),
 and on the GPU: per-edge residual / Jacobians and the converged solution against the scipy oracle."""
+import hashlib
+import os
+
 import numpy as np
 import pytest
 
 from d2slam_b200 import pgo, synth
 from oracle import pgo_oracle as po
+
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_cases.npz")
 
 
 def small_graph(seed=1, n_agents=3, n=40, loops=120):
@@ -91,47 +96,53 @@ def test_pgo_converged_solution_matches_sparse_direct_oracle():
     assert e1 < 0.5 * e0
 
 
-@pytest.mark.gpu
-def test_pgo_edges_on_device_match_the_reference_functor():
-    """Device residual / tangent Jacobians of every sampled edge vs the reference's own RelPoseFactorAD functor (shipped
-    oracle/_ref/libd2ref.so: doubles for the residual, dual numbers for the exact ambient Jacobians)."""
-    from oracle import ref
-    if not ref.available():
-        pytest.skip("oracle/_ref/libd2ref.so not shipped")
-    from test_ref_pin import plus_jacobian
+def relpose_graph():
     g = small_graph(seed=8)
     rng = np.random.default_rng(1)
     S = g["sqrt_info"].reshape(-1, 6, 6) + 0.5 * rng.normal(size=(len(g["ea"]), 6, 6))      # full square-root information
+    return g, S
+
+
+def g2o_agents_graph():
+    g = small_graph(seed=2, n_agents=3, n=12, loops=20)
+    rng = np.random.default_rng(0)
+    S = g["sqrt_info"].reshape(-1, 6, 6) + 0.3 * rng.normal(size=(len(g["ea"]), 6, 6))        # full information matrices
+    return g, S
+
+
+def g2o_written_graph():
+    g = small_graph(seed=3, n_agents=1, n=15, loops=10)
+    S = g["sqrt_info"].reshape(-1, 6, 6)
+    return g, np.einsum("eki,ekj->eij", S, S)
+
+
+@pytest.mark.gpu
+def test_pgo_edges_on_device_match_the_reference_functor():
+    """Device residual / tangent Jacobians of every sampled edge vs the reference's own RelPoseFactorAD functor (doubles for
+    the residual, dual numbers for the exact ambient Jacobians), frozen in tests/golden/ref_cases.npz."""
+    gold = np.load(GOLD)
+    g, S = relpose_graph()
     s = pgo.PgoSolver()
     s.set_poses(g["ids"], g["init"], g["fixed"]); s.add_edges(g["id_a"], g["id_b"], g["rel"], S.reshape(-1, 36))
     dev = s.debug_edges()
-    for e in range(0, len(dev), 5):
-        a, b = g["ea"][e], g["eb"][e]
-        r, Ja, Jb = ref.relpose_ad_eval(g["init"][a], g["init"][b], g["rel"][e], S[e])
-        want = np.concatenate([r, (Ja @ plus_jacobian(g["init"][a])).ravel(), (Jb @ plus_jacobian(g["init"][b])).ravel()])
+    assert len(dev) == len(g["ea"])
+    for e, want in zip(gold["relpose_idx"], gold["relpose_want"]):
         assert np.abs(dev[e] - want).max() <= 1e-11 * max(1.0, np.abs(want).max()), e
-
-
-def _ref_or_skip():
-    from oracle import ref
-    if not ref.available():
-        pytest.skip("oracle/_ref/libd2ref.so not built and no reference tree")
-    return ref
 
 
 def test_g2o_written_here_is_read_by_the_reference_reader(tmp_path):
     """pgo.write_g2o_agents (one `<agent>.g2o` per agent, chr('a' + agent) in the top byte of every vertex id) -> the reference's
-    OWN read_g2o_agent (d2pgo/test/posegraph_g2o.cpp, compiled unmodified into oracle/_ref) on every file: agents, keyframe ids,
-    poses, relative poses and information matrices come back exactly; the max_agent_id filter drops the same edges as ours."""
-    ref = _ref_or_skip()
-    g = small_graph(seed=2, n_agents=3, n=12, loops=20)
-    rng = np.random.default_rng(0)
-    S = g["sqrt_info"].reshape(-1, 6, 6) + 0.3 * rng.normal(size=(len(g["ea"]), 6, 6))        # full information matrices
+    OWN read_g2o_agent (d2pgo/test/posegraph_g2o.cpp) on every file, its results frozen in tests/golden/ref_cases.npz together
+    with the SHA-256 of the files it read: the files written now are those files, and agents, keyframe ids, poses, relative
+    poses and information matrices come back exactly; the max_agent_id filter drops the same edges as ours."""
+    gold = np.load(GOLD)
+    g, S = g2o_agents_graph()
     info = np.einsum("eki,ekj->eij", S, S)
     agents = pgo.write_g2o_agents(str(tmp_path), g["ids"], g["init"], g["id_a"], g["id_b"], g["rel"], S.reshape(-1, 36))
     assert agents == [0, 1, 2]
     for a in agents:
-        r = ref.g2o_read(str(tmp_path / f"{a}.g2o"), max_agent_id=len(agents) - 1)
+        assert hashlib.sha256((tmp_path / f"{a}.g2o").read_bytes()).hexdigest() == str(gold[f"g2o_agent{a}_sha256"])
+        r = {k: gold[f"g2o_agent{a}_{k}"] for k in ("v_agent", "v_id", "v_pose", "e_agent_a", "e_id_a", "e_agent_b", "e_id_b", "e_rel", "e_info")}
         v = (g["ids"] // 1_000_000) == a; e = (g["id_a"] // 1_000_000) == a
         assert np.all(r["v_agent"] == a) and np.array_equal(np.sort(r["v_id"]), np.sort(g["ids"][v] % 1_000_000))
         order = np.argsort(r["v_id"]); mine = np.argsort(g["ids"][v])
@@ -141,8 +152,8 @@ def test_g2o_written_here_is_read_by_the_reference_reader(tmp_path):
         assert np.abs(r["e_rel"] - g["rel"][e]).max() <= 1e-15
         assert np.abs(r["e_info"] - info[e]).max() <= 1e-12 * np.abs(info).max()
         # the agent filter (posegraph_g2o.cpp:72-74, 112-114): with max_agent_id = 0 only agent 0's own edges survive
-        r0 = ref.g2o_read(str(tmp_path / f"{a}.g2o"), max_agent_id=0); m0 = pgo.read_g2o(str(tmp_path / f"{a}.g2o"), max_agent_id=0)
-        assert len(r0["v_id"]) == len(m0["ids"]) and len(r0["e_id_a"]) == len(m0["id_a"])
+        m0 = pgo.read_g2o(str(tmp_path / f"{a}.g2o"), max_agent_id=0)
+        assert list(gold[f"g2o_agent{a}_n_filtered"]) == [len(m0["ids"]), len(m0["id_a"])]
     h = pgo.read_g2o_agents(str(tmp_path), 3)
     assert np.array_equal(np.sort(h["ids"]), np.sort(g["ids"])) and len(h["id_a"]) == len(g["id_a"])
     h2 = pgo.read_g2o_agents(str(tmp_path), 2)
@@ -150,13 +161,12 @@ def test_g2o_written_here_is_read_by_the_reference_reader(tmp_path):
 
 
 def test_g2o_written_by_the_reference_is_read_here(tmp_path):
-    """The reference's write_result_to_g2o (plain keyframe ids, default ostream precision: 6 significant digits) -> pgo.read_g2o."""
-    ref = _ref_or_skip()
-    g = small_graph(seed=3, n_agents=1, n=15, loops=10)
-    S = g["sqrt_info"].reshape(-1, 6, 6); info = np.einsum("eki,ekj->eij", S, S)
-    path = str(tmp_path / "out.g2o")
-    ref.g2o_write(path, g["ids"], g["init"], g["id_a"], g["id_b"], g["rel"], info)
-    h = pgo.read_g2o(path)
+    """The reference's write_result_to_g2o (plain keyframe ids, default ostream precision: 6 significant digits), its output
+    frozen in tests/golden/ref_cases.npz -> pgo.read_g2o."""
+    g, info = g2o_written_graph()
+    path = tmp_path / "out.g2o"
+    path.write_bytes(np.load(GOLD)["g2o_written"].tobytes())
+    h = pgo.read_g2o(str(path))
     assert np.array_equal(h["ids"], g["ids"]) and np.array_equal(h["id_a"], g["id_a"]) and np.array_equal(h["id_b"], g["id_b"])
     assert np.abs(h["poses"][:, :3] - g["init"][:, :3]).max() <= 1e-5 * max(1.0, np.abs(g["init"][:, :3]).max()) and np.abs(h["poses"][:, 3:] - g["init"][:, 3:]).max() <= 1e-5
     assert np.abs(h["rel"] - g["rel"]).max() <= 1e-5 * max(1.0, np.abs(g["rel"]).max())

@@ -67,12 +67,12 @@ int main() {
   const int it = 20000;
   run("dfma ILP1 1 warp", [](double *o, int i, long long *c, int t, int b) { k_dfma<1><<<b, t>>>(o, i, c); }, 1, 32, 1, it);
   run("dfma ILP8 1 warp", [](double *o, int i, long long *c, int t, int b) { k_dfma<8><<<b, t>>>(o, i, c); }, 8, 32, 1, it);
-  run("dfma ILP8 16 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dfma<8><<<b, t>>>(o, i, c); }, 8, 512, 148, it);
-  run("dfma ILP8 32 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dfma<8><<<b, t>>>(o, i, c); }, 8, 1024, 148, it);
+  run("dfma ILP8 16 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dfma<8><<<b, t>>>(o, i, c); }, 8, 512, 132, it);
+  run("dfma ILP8 32 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dfma<8><<<b, t>>>(o, i, c); }, 8, 1024, 132, it);
   run("dmma ILP1 1 warp", [](double *o, int i, long long *c, int t, int b) { k_dmma<1><<<b, t>>>(o, i, c); }, 8, 32, 1, it);
   run("dmma ILP4 1 warp", [](double *o, int i, long long *c, int t, int b) { k_dmma<4><<<b, t>>>(o, i, c); }, 32, 32, 1, it);
-  run("dmma ILP4 16 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dmma<4><<<b, t>>>(o, i, c); }, 32, 512, 148, it);
-  run("dmma ILP4 32 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dmma<4><<<b, t>>>(o, i, c); }, 32, 1024, 148, it);
+  run("dmma ILP4 16 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dmma<4><<<b, t>>>(o, i, c); }, 32, 512, 132, it);
+  run("dmma ILP4 32 warps/SM", [](double *o, int i, long long *c, int t, int b) { k_dmma<4><<<b, t>>>(o, i, c); }, 32, 1024, 132, it);
   run("shfl chain", [](double *o, int i, long long *c, int t, int b) { k_shfl<<<b, t>>>(o, i, c); }, 1, 32, 1, it);
   run("rsqrt(f32 seed + 2 newton)", [](double *o, int i, long long *c, int t, int b) { k_rsqrt<<<b, t>>>(o, i, c); }, 1, 32, 1, it);
   run("lds dependent chain", [](double *o, int i, long long *c, int t, int b) { k_lds<<<b, t>>>(o, i, c); }, 1, 32, 1, it);

@@ -7,9 +7,9 @@ so = os.path.join(ROOT, "d2slam_b200", "libd2ba.so")
 KERNELS = ["k_proj_lin_pp", "k_lm_gather16", "k_schur_small", "k_schur", "k_chol_smem", "k_sb_elim", "k_leaf_elim", "k_leaf_back", "k_imu_lin", "k_step"]
 sass = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
 funcs = re.split(r"\n\s*Function : ", sass)
-out = [f"# cuobjdump -sass {os.path.relpath(so, ROOT)} (sm_100a), per-kernel instruction histogram of the mnemonics that matter\n",
+out = [f"# cuobjdump -sass {os.path.relpath(so, ROOT)} (sm_90a), per-kernel instruction histogram of the mnemonics that matter\n",
        "# DMMA = fp64 tensor-core mma.sync m8n8k4; UBLKCP = cp.async.bulk (TMA bulk copy); SYNCS = mbarrier; LDGSTS = cp.async;\n",
-       "# RED/ATOMG = L2 reductions; DFMA/DADD/DMUL = fp64 pipe.  tcgen05 (UTC*MMA) has no f64 kind: none expected.\n\n"]
+       "# RED/ATOMG = L2 reductions; DFMA/DADD/DMUL = fp64 pipe.  wgmma (HGMMA) has no f64 kind: none expected.\n\n"]
 for fn in funcs[1:]:
     name = fn.split("\n", 1)[0].strip()
     short = next((k for k in KERNELS if re.search(rf"\d+{k}(E|I)", name)), None)
