@@ -1,10 +1,12 @@
 // d2pgo.cu -- pose-graph optimisation on the GPU (include/d2pgo.h): relative-pose factors, matrix-free block-Jacobi PCG,
 // Levenberg-Marquardt outer loop, edge-sharded multi-GPU with one NCCL all-reduce per CG iteration.
 //
-// Factor: D2Common::RelPoseFactorAD (d2common/include/d2common/solver/RelPoseFactor.hpp:68-135), restated in pgo_edge_eval
+// Factors: D2Common::RelPoseFactorAD (d2common/include/d2common/solver/RelPoseFactor.hpp:68-135), restated in pgo_edge_eval
 // below with analytic exact derivatives in the tangent of the right-multiplicative pose retraction
 // (pose_local_parameterization.cpp:13-38).  (The header's hand-differentiated RelPoseFactor :8-66, used when
 // pgo_use_autodiff is off, drops q_rel from its rotation blocks -- its Jacobian is exact only for identity relative rotation.)
+// And RelPoseFactor4D (:196-238), d2pgo's default 4-DoF configuration, in pgo_edge_eval_4d.  One solver serves both: every
+// kernel is a template over an edge policy (PgoEdge6 / PgoEdge4) that fixes the block size D and the retraction.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -34,17 +36,17 @@ struct PgoScalars {      // device-resident CG state that is not a per-block par
 
 struct PgoDev {
   int n_pose, n_edge;
-  const double *x;        // [N][8] poses the edges are linearised at
+  const double *x;        // [N][8] poses the edges are linearised at: [x y z qx qy qz qw 0] (6-DoF) or [x y z yaw 0 0 0 0] (4-DoF)
   const unsigned char *fixed;
   const int *ea, *eb;     // [E] pose indices
-  const double *rel;      // [E][8]
-  const double *sinfo;    // [E][36] sqrt information, row-major
-  double *lin;            // [78][E] field-major: r(6), J0 (6x6 row-major), J1 (6x6)
-  double *g, *D;          // [6N], [N][36]
-  double *Minv;           // [N][36]
-  double *dx, *r, *z, *p, *Ap;   // [6N]
-  double *damp;           // [6N] lambda diag(D) + 1e-12
-  double *t;              // [12][E] per edge: J0^T (J p) (6), J1^T (J p) (6)
+  const double *rel;      // [E][8] measurements, same layouts as x
+  const double *sinfo;    // [E][D*D] sqrt information, row-major
+  double *lin;            // [D + 2 D^2][E] field-major: r(D), J0 (DxD row-major), J1 (DxD)
+  double *g, *D;          // [D N], [N][D*D]
+  double *Minv;           // [N][D*D]
+  double *dx, *r, *z, *p, *Ap;   // [D N]
+  double *damp;           // [D N] lambda diag(D) + 1e-12
+  double *t;              // [2D][E] per edge: J0^T (J p) (D), J1^T (J p) (D)
   const int *inc_ptr, *inc;   // incidence lists: pose i -> (edge << 1 | side) of this rank's edges, ascending
   double *rz_part, *rr_part;  // [2][nbp] per-block partials, ping-pong on the iteration parity
   double *pAp_part;           // [nbp]
@@ -90,6 +92,50 @@ D2BA_DEV void pgo_edge_eval(const double *p0, const double *p1, const double *re
   }
 }
 
+// Utility::NormalizeAngle (d2common/include/d2common/utils.hpp:251-257): a - 2 pi floor((a + pi) / 2 pi), in [-pi, pi)
+D2BA_DEV double pgo_normalize_angle(double a) { return a - 2.0 * M_PI * floor((a + M_PI) / (2.0 * M_PI)); }
+
+// RelPoseFactor4D (RelPoseFactor.hpp:216-227 + Utility::poseError4D, utils.hpp:240-280; d2pgo's default pgo_pose_dof =
+// PGO_POSE_4D): poses [x y z yaw], v = p_b - p_a,
+//   r = S [ p_meas - Rz(-yaw_a) v ; N(yaw_meas - N(yaw_b - yaw_a)) ]   with the full 4x4 S, and the exact Jacobians
+//   d/d p_a = S [Rz(-yaw_a); 0],  d/d yaw_a = S [Rz'(-yaw_a) v; 1],  d/d p_b = S [-Rz(-yaw_a); 0],  d/d yaw_b = S [0; -1]
+// (PosAngleManifold's tangent is the 4-vector itself).  The CPU oracle states the same lines (edge_eval_4d).
+D2BA_DEV void pgo_edge_eval_4d(const double *pa, const double *pb, const double *rel, const double *S, double *r, double *J0, double *J1) {
+  double s, c;
+  sincos(-pa[3], &s, &c);
+  const double v[3] = {pb[0] - pa[0], pb[1] - pa[1], pb[2] - pa[2]};
+  const double raw[4] = {rel[0] - (c * v[0] - s * v[1]), rel[1] - (s * v[0] + c * v[1]), rel[2] - v[2],
+                         pgo_normalize_angle(rel[3] - pgo_normalize_angle(pb[3] - pa[3]))};
+  for (int i = 0; i < 4; i++) { double t = 0; for (int k = 0; k < 4; k++) t += S[i * 4 + k] * raw[k]; r[i] = t; }
+  if (!J0) return;
+  // A0 = [Rz | Rz' v ; 0 0 0 1], A1 = [-Rz | 0 ; 0 0 0 -1]; Rz' = d Rz(t) / dt at t = -yaw_a
+  const double A0[16] = {c, -s, 0.0, -s * v[0] - c * v[1],
+                         s, c, 0.0, c * v[0] - s * v[1],
+                         0.0, 0.0, 1.0, 0.0,
+                         0.0, 0.0, 0.0, 1.0};
+  for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) {
+    double t0 = 0;
+    for (int k = 0; k < 4; k++) t0 += S[i * 4 + k] * A0[k * 4 + j];
+    J0[i * 4 + j] = t0;
+    J1[i * 4 + j] = j < 3 ? -t0 : -S[i * 4 + 3];   // S A1: the position columns are those of S A0 negated
+  }
+}
+
+// Edge-evaluation policies: block size D of the tangent, stored pose width NX (of the 8 doubles per pose) and the retraction.
+struct PgoEdge6 {   // RelPoseFactorAD on [x y z qx qy qz qw], PoseLocalParameterization::Plus
+  static constexpr int D = 6, NX = 7;
+  D2BA_DEV static void eval(const double *p0, const double *p1, const double *rel, const double *S, double *r, double *J0, double *J1) { pgo_edge_eval(p0, p1, rel, S, r, J0, J1); }
+  D2BA_DEV static void plus(const double *x, const double *dx, double *o) { pose_plus(x, dx, o); }
+};
+struct PgoEdge4 {   // RelPoseFactor4D on [x y z yaw], PosAngleManifold::Plus (angle_manifold.h:39-68): x + dx, yaw normalised
+  static constexpr int D = 4, NX = 4;
+  D2BA_DEV static void eval(const double *p0, const double *p1, const double *rel, const double *S, double *r, double *J0, double *J1) { pgo_edge_eval_4d(p0, p1, rel, S, r, J0, J1); }
+  D2BA_DEV static void plus(const double *x, const double *dx, double *o) {
+    for (int k = 0; k < 3; k++) o[k] = x[k] + dx[k];
+    o[3] = pgo_normalize_angle(x[3] + dx[3]);
+  }
+};
+
 // Fixed-order sum of n per-block partials, the same value in every thread of every block (so that all blocks -- and all
 // ranks, which hold identical vectors -- take the same branch without a single-thread "decide" kernel in between).
 D2BA_DEV double total_of(const double *part, int n, double *red) {
@@ -105,20 +151,22 @@ D2BA_DEV double total_of(const double *part, int n, double *red) {
 }
 
 // linearise every local edge at d.x: lin records [r | J0 | J1] and per-block cost partials (summed in fixed order by k_pgo_sum)
+template <class P>
 __global__ void __launch_bounds__(128) k_pgo_lin(PgoDev d, double *cost_part, int want_jac) {
+  constexpr int D = P::D, DD = D * D;
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   __shared__ double red[40];
   double c = 0.0;
   if (e < d.n_edge) {
     const int a = d.ea[e], b = d.eb[e];
-    double r[6], J0[36], J1[36];
-    pgo_edge_eval(d.x + (size_t)a * 8, d.x + (size_t)b * 8, d.rel + (size_t)e * 8, d.sinfo + (size_t)e * 36, r, want_jac ? J0 : nullptr, J1);
-    for (int k = 0; k < 6; k++) c += 0.5 * r[k] * r[k];
+    double r[D], J0[DD], J1[DD];
+    P::eval(d.x + (size_t)a * 8, d.x + (size_t)b * 8, d.rel + (size_t)e * 8, d.sinfo + (size_t)e * DD, r, want_jac ? J0 : nullptr, J1);
+    for (int k = 0; k < D; k++) c += 0.5 * r[k] * r[k];
     if (want_jac) {
-      double *o = d.lin + e;   // field-major [78][E]: consecutive edges (threads) touch consecutive addresses
+      double *o = d.lin + e;   // field-major [D + 2 D^2][E]: consecutive edges (threads) touch consecutive addresses
       const size_t E = (size_t)d.n_edge;
-      for (int k = 0; k < 6; k++) o[k * E] = r[k];
-      for (int k = 0; k < 36; k++) { o[(6 + k) * E] = J0[k]; o[(42 + k) * E] = J1[k]; }
+      for (int k = 0; k < D; k++) o[k * E] = r[k];
+      for (int k = 0; k < DD; k++) { o[(D + k) * E] = J0[k]; o[(D + DD + k) * E] = J1[k]; }
     }
   }
   c = block_sum(c, red);
@@ -132,52 +180,57 @@ __global__ void k_pgo_sum(const double *part, int n, double *out) {
 
 // gradient g_i = sum J^T r and block diagonal D_i = sum J^T J over the edges incident to pose i, in the fixed order of the
 // incidence list (no atomics: bitwise reproducible)
-__global__ void __launch_bounds__(128) k_pgo_gD(PgoDev d, double *g, double *D) {
+template <class P>
+__global__ void __launch_bounds__(128) k_pgo_gD(PgoDev d, double *g, double *Dg) {
+  constexpr int D = P::D, DD = D * D;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= d.n_pose) return;
-  double gi[6] = {0, 0, 0, 0, 0, 0}, Di[36];
-  for (int k = 0; k < 36; k++) Di[k] = 0.0;
+  double gi[D], Di[DD];
+  for (int k = 0; k < D; k++) gi[k] = 0.0;
+  for (int k = 0; k < DD; k++) Di[k] = 0.0;
   if (!d.fixed[i])
     for (int q = d.inc_ptr[i]; q < d.inc_ptr[i + 1]; q++) {
       const int c = d.inc[q];
       const size_t E = (size_t)d.n_edge;
-      const double *o = d.lin + (c >> 1), *J = o + (size_t)(6 + 36 * (c & 1)) * E;
-      for (int k = 0; k < 6; k++) {
+      const double *o = d.lin + (c >> 1), *J = o + (size_t)(D + DD * (c & 1)) * E;
+      for (int k = 0; k < D; k++) {
         const double rk = o[k * E];
-        double row[6];
-        for (int a = 0; a < 6; a++) { row[a] = J[(size_t)(k * 6 + a) * E]; gi[a] += row[a] * rk; }
-        for (int a = 0; a < 6; a++) for (int b = 0; b < 6; b++) Di[a * 6 + b] += row[a] * row[b];
+        double row[D];
+        for (int a = 0; a < D; a++) { row[a] = J[(size_t)(k * D + a) * E]; gi[a] += row[a] * rk; }
+        for (int a = 0; a < D; a++) for (int b = 0; b < D; b++) Di[a * D + b] += row[a] * row[b];
       }
     }
-  for (int k = 0; k < 6; k++) g[(size_t)i * 6 + k] = gi[k];
-  for (int k = 0; k < 36; k++) D[(size_t)i * 36 + k] = Di[k];
+  for (int k = 0; k < D; k++) g[(size_t)i * D + k] = gi[k];
+  for (int k = 0; k < DD; k++) Dg[(size_t)i * DD + k] = Di[k];
 }
 
-// block-Jacobi preconditioner: Minv = (D + lambda diag(D))^-1 per free pose (6x6 Cholesky, one thread per pose); also the
+// block-Jacobi preconditioner: Minv = (D + lambda diag(D))^-1 per free pose (DxD Cholesky, one thread per pose); also the
 // damping diagonal lambda diag(D) + 1e-12 the products add
-__global__ void k_pgo_precond(PgoDev d, const double *D, double lambda) {
+template <class P>
+__global__ void k_pgo_precond(PgoDev d, const double *Dg, double lambda) {
+  constexpr int D = P::D, DD = D * D;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= d.n_pose) return;
-  double *M = d.Minv + (size_t)i * 36;
-  if (d.fixed[i]) { for (int k = 0; k < 36; k++) M[k] = 0.0; for (int k = 0; k < 6; k++) d.damp[(size_t)i * 6 + k] = 0.0; return; }
-  double A[36], Li[36];
-  for (int k = 0; k < 36; k++) A[k] = D[(size_t)i * 36 + k];
-  for (int k = 0; k < 6; k++) { const double dk = lambda * A[k * 7] + 1e-12; d.damp[(size_t)i * 6 + k] = dk; A[k * 7] += dk; }
-  for (int j = 0; j < 6; j++) {   // Cholesky, lower
-    double s = A[j * 6 + j];
-    for (int k = 0; k < j; k++) s -= A[j * 6 + k] * A[j * 6 + k];
+  double *M = d.Minv + (size_t)i * DD;
+  if (d.fixed[i]) { for (int k = 0; k < DD; k++) M[k] = 0.0; for (int k = 0; k < D; k++) d.damp[(size_t)i * D + k] = 0.0; return; }
+  double A[DD], Li[DD];
+  for (int k = 0; k < DD; k++) A[k] = Dg[(size_t)i * DD + k];
+  for (int k = 0; k < D; k++) { const double dk = lambda * A[k * (D + 1)] + 1e-12; d.damp[(size_t)i * D + k] = dk; A[k * (D + 1)] += dk; }
+  for (int j = 0; j < D; j++) {   // Cholesky, lower
+    double s = A[j * D + j];
+    for (int k = 0; k < j; k++) s -= A[j * D + k] * A[j * D + k];
     s = sqrt(s > 0.0 ? s : 1e-300);
-    A[j * 6 + j] = s;
-    for (int r = j + 1; r < 6; r++) { double t = A[r * 6 + j]; for (int k = 0; k < j; k++) t -= A[r * 6 + k] * A[j * 6 + k]; A[r * 6 + j] = t / s; }
+    A[j * D + j] = s;
+    for (int r = j + 1; r < D; r++) { double t = A[r * D + j]; for (int k = 0; k < j; k++) t -= A[r * D + k] * A[j * D + k]; A[r * D + j] = t / s; }
   }
-  for (int c = 0; c < 6; c++) {   // L^-1 column by column
-    for (int r = 0; r < 6; r++) {
+  for (int c = 0; c < D; c++) {   // L^-1 column by column
+    for (int r = 0; r < D; r++) {
       double t = r == c ? 1.0 : 0.0;
-      for (int k = 0; k < r; k++) t -= A[r * 6 + k] * Li[k * 6 + c];
-      Li[r * 6 + c] = t / A[r * 6 + r];
+      for (int k = 0; k < r; k++) t -= A[r * D + k] * Li[k * D + c];
+      Li[r * D + c] = t / A[r * D + r];
     }
   }
-  for (int r = 0; r < 6; r++) for (int c = 0; c < 6; c++) { double t = 0; for (int k = 0; k < 6; k++) t += Li[k * 6 + r] * Li[k * 6 + c]; M[r * 6 + c] = t; }
+  for (int r = 0; r < D; r++) for (int c = 0; c < D; c++) { double t = 0; for (int k = 0; k < D; k++) t += Li[k * D + r] * Li[k * D + c]; M[r * D + c] = t; }
 }
 
 // ---- conjugate gradients.  One iteration = three kernels (the three grid-wide dependencies of CG):
@@ -197,11 +250,14 @@ D2BA_DEV CgView cg_view(const PgoDev &d, int par, double tol2, double *red) {
   v.done = s->done || !(v.rr_cur > tol2 * s->bb) || !(v.rz_cur > 0.0) || !isfinite(v.rz_cur);
   return v;
 }
+template <int D>
 D2BA_DEV void cg_p_new(const PgoDev &d, int i, double beta, double *p) {
-  for (int k = 0; k < 6; k++) p[k] = d.z[(size_t)i * 6 + k] + beta * d.p[(size_t)i * 6 + k];   // p holds 0 before the first iteration
+  for (int k = 0; k < D; k++) p[k] = d.z[(size_t)i * D + k] + beta * d.p[(size_t)i * D + k];   // p holds 0 before the first iteration
 }
 
+template <class P>
 __global__ void __launch_bounds__(128) k_pgo_cg_edge(PgoDev d, int par, double tol2) {
+  constexpr int D = P::D, DD = D * D;
   __shared__ double red[40];
   const CgView v = cg_view(d, par, tol2, red);
   if (v.done) return;
@@ -210,22 +266,24 @@ __global__ void __launch_bounds__(128) k_pgo_cg_edge(PgoDev d, int par, double t
   const double beta = v.first ? 0.0 : v.rz_cur / v.rz_prev;
   const int a = d.ea[e], b = d.eb[e];
   const size_t E = (size_t)d.n_edge;
-  const double *J0 = d.lin + 6 * E + e, *J1 = J0 + 36 * E;
-  double pa[6], pb[6], ya[6] = {0, 0, 0, 0, 0, 0}, yb[6] = {0, 0, 0, 0, 0, 0};
-  cg_p_new(d, a, beta, pa); cg_p_new(d, b, beta, pb);
+  const double *J0 = d.lin + D * E + e, *J1 = J0 + DD * E;
+  double pa[D], pb[D], ya[D], yb[D];
+  for (int q = 0; q < D; q++) { ya[q] = 0.0; yb[q] = 0.0; }
+  cg_p_new<D>(d, a, beta, pa); cg_p_new<D>(d, b, beta, pb);
   // t = J0 pa + J1 pb, then this edge's two contributions J0^T t, J1^T t (the Jacobians are read once, coalesced; the
-  // per-pose kernel only sums six numbers per incident edge)
-  for (int k = 0; k < 6; k++) {
-    double j0[6], j1[6], tk = 0;
-    for (int q = 0; q < 6; q++) { j0[q] = J0[(size_t)(k * 6 + q) * E]; j1[q] = J1[(size_t)(k * 6 + q) * E]; tk += j0[q] * pa[q] + j1[q] * pb[q]; }
-    for (int q = 0; q < 6; q++) { ya[q] += j0[q] * tk; yb[q] += j1[q] * tk; }
+  // per-pose kernel only sums D numbers per incident edge)
+  for (int k = 0; k < D; k++) {
+    double j0[D], j1[D], tk = 0;
+    for (int q = 0; q < D; q++) { j0[q] = J0[(size_t)(k * D + q) * E]; j1[q] = J1[(size_t)(k * D + q) * E]; tk += j0[q] * pa[q] + j1[q] * pb[q]; }
+    for (int q = 0; q < D; q++) { ya[q] += j0[q] * tk; yb[q] += j1[q] * tk; }
   }
-  for (int q = 0; q < 6; q++) { d.t[(size_t)q * E + e] = ya[q]; d.t[(size_t)(6 + q) * E + e] = yb[q]; }
+  for (int q = 0; q < D; q++) { d.t[(size_t)q * E + e] = ya[q]; d.t[(size_t)(D + q) * E + e] = yb[q]; }
 }
 
 // LOCAL: this rank's edges only, no damping / p.Ap yet (the all-reduce of Ap comes first; k_pgo_cg_pAp follows)
-template <bool LOCAL>
+template <class P, bool LOCAL>
 __global__ void __launch_bounds__(128) k_pgo_cg_pose(PgoDev d, int par, double tol2) {
+  constexpr int D = P::D;
   __shared__ double red[40];
   const CgView v = cg_view(d, par, tol2, red);
   if (v.done) return;
@@ -233,42 +291,45 @@ __global__ void __launch_bounds__(128) k_pgo_cg_pose(PgoDev d, int par, double t
   double s = 0.0;
   if (i < d.n_pose) {
     const double beta = v.first ? 0.0 : v.rz_cur / v.rz_prev;
-    double p[6], y[6] = {0, 0, 0, 0, 0, 0};
-    cg_p_new(d, i, beta, p);
+    double p[D], y[D];
+    for (int k = 0; k < D; k++) y[k] = 0.0;
+    cg_p_new<D>(d, i, beta, p);
     if (!d.fixed[i])
       for (int q = d.inc_ptr[i]; q < d.inc_ptr[i + 1]; q++) {
         const int c = d.inc[q];
         const size_t E = (size_t)d.n_edge;
-        const double *t = d.t + (size_t)(6 * (c & 1)) * E + (c >> 1);
-        for (int a = 0; a < 6; a++) y[a] += t[a * E];
+        const double *t = d.t + (size_t)(D * (c & 1)) * E + (c >> 1);
+        for (int a = 0; a < D; a++) y[a] += t[a * E];
       }
-    for (int k = 0; k < 6; k++) {
-      d.p[(size_t)i * 6 + k] = p[k];
-      if (!LOCAL) { y[k] += d.damp[(size_t)i * 6 + k] * p[k]; s += p[k] * y[k]; }
-      d.Ap[(size_t)i * 6 + k] = y[k];
+    for (int k = 0; k < D; k++) {
+      d.p[(size_t)i * D + k] = p[k];
+      if (!LOCAL) { y[k] += d.damp[(size_t)i * D + k] * p[k]; s += p[k] * y[k]; }
+      d.Ap[(size_t)i * D + k] = y[k];
     }
   }
   if (!LOCAL) { s = block_sum(s, red); if (threadIdx.x == 0) d.pAp_part[blockIdx.x] = s; }
 }
-template __global__ void k_pgo_cg_pose<true>(PgoDev, int, double);
-template __global__ void k_pgo_cg_pose<false>(PgoDev, int, double);
 
+template <class P>
 __global__ void __launch_bounds__(128) k_pgo_cg_pAp(PgoDev d, int par, double tol2) {   // multi-rank: after the all-reduce of Ap
+  constexpr int D = P::D;
   __shared__ double red[40];
   const CgView v = cg_view(d, par, tol2, red);
   if (v.done) return;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double s = 0.0;
   if (i < d.n_pose)
-    for (int k = 0; k < 6; k++) {
-      const double pk = d.p[(size_t)i * 6 + k], y = d.Ap[(size_t)i * 6 + k] + d.damp[(size_t)i * 6 + k] * pk;
-      d.Ap[(size_t)i * 6 + k] = y; s += pk * y;
+    for (int k = 0; k < D; k++) {
+      const double pk = d.p[(size_t)i * D + k], y = d.Ap[(size_t)i * D + k] + d.damp[(size_t)i * D + k] * pk;
+      d.Ap[(size_t)i * D + k] = y; s += pk * y;
     }
   s = block_sum(s, red);
   if (threadIdx.x == 0) d.pAp_part[blockIdx.x] = s;
 }
 
+template <class P>
 __global__ void __launch_bounds__(128) k_pgo_cg_step(PgoDev d, int par, double tol2) {
+  constexpr int D = P::D, DD = D * D;
   __shared__ double red[40];
   const CgView v = cg_view(d, par, tol2, red);
   if (v.done) { if (blockIdx.x == 0 && threadIdx.x == 0) d.s->done = 1; return; }
@@ -277,14 +338,14 @@ __global__ void __launch_bounds__(128) k_pgo_cg_step(PgoDev d, int par, double t
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double rz = 0, rr = 0;
   if (i < d.n_pose && !d.fixed[i]) {
-    double r[6];
-    for (int k = 0; k < 6; k++) {
-      d.dx[(size_t)i * 6 + k] += alpha * d.p[(size_t)i * 6 + k];
-      r[k] = d.r[(size_t)i * 6 + k] - alpha * d.Ap[(size_t)i * 6 + k];
-      d.r[(size_t)i * 6 + k] = r[k];
+    double r[D];
+    for (int k = 0; k < D; k++) {
+      d.dx[(size_t)i * D + k] += alpha * d.p[(size_t)i * D + k];
+      r[k] = d.r[(size_t)i * D + k] - alpha * d.Ap[(size_t)i * D + k];
+      d.r[(size_t)i * D + k] = r[k];
     }
-    const double *M = d.Minv + (size_t)i * 36;
-    for (int k = 0; k < 6; k++) { double t = 0; for (int q = 0; q < 6; q++) t += M[k * 6 + q] * r[q]; d.z[(size_t)i * 6 + k] = t; rz += r[k] * t; rr += r[k] * r[k]; }
+    const double *M = d.Minv + (size_t)i * DD;
+    for (int k = 0; k < D; k++) { double t = 0; for (int q = 0; q < D; q++) t += M[k * D + q] * r[q]; d.z[(size_t)i * D + k] = t; rz += r[k] * t; rr += r[k] * r[k]; }
   }
   rz = block_sum(rz, red); rr = block_sum(rr, red);
   if (threadIdx.x == 0) {
@@ -294,17 +355,19 @@ __global__ void __launch_bounds__(128) k_pgo_cg_step(PgoDev d, int par, double t
 }
 
 // CG start: dx = 0, r = -g, z = Minv r, p = 0 (the first k_pgo_cg_edge forms p = z); partials into the parity-1 slots
+template <class P>
 __global__ void __launch_bounds__(128) k_pgo_cg_init(PgoDev d, const double *g) {
+  constexpr int D = P::D, DD = D * D;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   __shared__ double red[40];
   double rz = 0, rr = 0;
   if (i < d.n_pose) {
-    double r[6], z[6];
-    for (int k = 0; k < 6; k++) r[k] = d.fixed[i] ? 0.0 : -g[(size_t)i * 6 + k];
-    const double *M = d.Minv + (size_t)i * 36;
-    for (int k = 0; k < 6; k++) { double t = 0; for (int q = 0; q < 6; q++) t += M[k * 6 + q] * r[q]; z[k] = t; }
-    for (int k = 0; k < 6; k++) {
-      d.dx[(size_t)i * 6 + k] = 0.0; d.r[(size_t)i * 6 + k] = r[k]; d.z[(size_t)i * 6 + k] = z[k]; d.p[(size_t)i * 6 + k] = 0.0;
+    double r[D], z[D];
+    for (int k = 0; k < D; k++) r[k] = d.fixed[i] ? 0.0 : -g[(size_t)i * D + k];
+    const double *M = d.Minv + (size_t)i * DD;
+    for (int k = 0; k < D; k++) { double t = 0; for (int q = 0; q < D; q++) t += M[k * D + q] * r[q]; z[k] = t; }
+    for (int k = 0; k < D; k++) {
+      d.dx[(size_t)i * D + k] = 0.0; d.r[(size_t)i * D + k] = r[k]; d.z[(size_t)i * D + k] = z[k]; d.p[(size_t)i * D + k] = 0.0;
       rz += r[k] * z[k]; rr += r[k] * r[k];
     }
   }
@@ -317,16 +380,18 @@ __global__ void k_pgo_cg_init2(PgoDev d) {   // |b|^2 and the counters
   if (threadIdx.x == 0) { d.s->bb = bb; d.s->done = 0; d.s->iters = 0; }
 }
 
-// candidate poses: x_out = x (+) dx   (PoseLocalParameterization::Plus)
+// candidate poses: x_out = x (+) dx   (PoseLocalParameterization::Plus / PosAngleManifold::Plus); unused slots zero
+template <class P>
 __global__ void k_pgo_retract(PgoDev d, double *x_out) {
+  constexpr int NX = P::NX;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= d.n_pose) return;
   const double *x = d.x + (size_t)i * 8;
-  double o[7];
-  if (d.fixed[i]) { for (int k = 0; k < 7; k++) o[k] = x[k]; }
-  else pose_plus(x, d.dx + (size_t)i * 6, o);
-  for (int k = 0; k < 7; k++) x_out[(size_t)i * 8 + k] = o[k];
-  x_out[(size_t)i * 8 + 7] = 0.0;
+  double o[NX];
+  if (d.fixed[i]) { for (int k = 0; k < NX; k++) o[k] = x[k]; }
+  else P::plus(x, d.dx + (size_t)i * P::D, o);
+  for (int k = 0; k < NX; k++) x_out[(size_t)i * 8 + k] = o[k];
+  for (int k = NX; k < 8; k++) x_out[(size_t)i * 8 + k] = 0.0;
 }
 
 template <typename T> struct Buf {
@@ -338,12 +403,13 @@ template <typename T> struct Buf {
 
 struct d2pgo_handle {
   d2pgo_config cfg;
+  int dof = 6;              // pose block size: 6 (RelPoseFactorAD on SE(3)) or 4 (RelPoseFactor4D on [x y z yaw])
   std::string err;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::vector<int64_t> ids; std::unordered_map<int64_t, int> index;
-  std::vector<double> poses; std::vector<unsigned char> fixed;
-  std::vector<int> ea, eb; std::vector<double> rel, sinfo;
+  std::vector<double> poses; std::vector<unsigned char> fixed;   // [N][8], the device layout of PgoDev::x
+  std::vector<int> ea, eb; std::vector<double> rel, sinfo;         // rel [E][8], sinfo [E][dof^2]
   Buf<double> d_x[2], d_rel, d_sinfo, d_lin[2], d_g[2], d_D[2], d_Minv, d_dx, d_r, d_z, d_p, d_Ap, d_cost, d_damp, d_t, d_part, d_cost_part;
   Buf<unsigned char> d_fixed; Buf<int> d_ea, d_eb, d_inc_ptr, d_inc; Buf<PgoScalars> d_s;
   cudaGraphExec_t cg_graph[2] = {nullptr, nullptr};   // 16 CG iterations on the linearisation buffer 0 / 1 (single rank)
@@ -353,6 +419,48 @@ struct d2pgo_handle {
 };
 
 #define PCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return 100 + (int)e_; } } while (0)
+
+// the 6-DoF and the 4-DoF entry points each serve one kind of handle
+static int pgo_want_dof(d2pgo_handle *h, int dof, const char *what) {
+  if (h->dof == dof) return 0;
+  h->err = std::string(what) + ": the handle was created with pose_dof = " + std::to_string(h->dof) + "; use the " +
+           (h->dof == 4 ? "d2pgo_*_4d" : "6-DoF d2pgo_*") + " entry points";
+  return 5;
+}
+
+static int pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *poses, int width, const uint8_t *fixed, const char *what) {
+  h->ids.assign(ids, ids + n); h->index.clear(); h->poses.assign((size_t)n * 8, 0.0); h->fixed.assign(n, 0);
+  for (int i = 0; i < n; i++) {
+    if (!h->index.emplace(ids[i], i).second) { h->err = std::string(what) + ": duplicate pose id"; return 2; }
+    memcpy(&h->poses[(size_t)i * 8], poses + (size_t)i * width, (size_t)width * 8);
+    h->fixed[i] = fixed ? fixed[i] : 0;
+  }
+  h->ea.clear(); h->eb.clear(); h->rel.clear(); h->sinfo.clear(); h->uploaded = false;
+  return 0;
+}
+
+static int pgo_add_edges(d2pgo_handle *h, int32_t n, const int64_t *id_a, const int64_t *id_b, const double *rel, int width, const double *sqrt_info, const char *what) {
+  const int DD = h->dof * h->dof;
+  for (int e = 0; e < n; e++) {
+    auto a = h->index.find(id_a[e]), b = h->index.find(id_b[e]);
+    if (a == h->index.end() || b == h->index.end()) { h->err = std::string(what) + ": unknown pose id"; return 2; }
+    h->ea.push_back(a->second); h->eb.push_back(b->second);
+    for (int k = 0; k < width; k++) h->rel.push_back(rel[(size_t)e * width + k]);
+    for (int k = width; k < 8; k++) h->rel.push_back(0.0);
+    for (int k = 0; k < DD; k++) h->sinfo.push_back(sqrt_info[(size_t)e * DD + k]);
+  }
+  h->uploaded = false;
+  return 0;
+}
+
+static int pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out, int width, const char *what) {
+  for (int i = 0; i < n; i++) {
+    auto it = h->index.find(ids[i]);
+    if (it == h->index.end()) { h->err = std::string(what) + ": unknown id"; return 2; }
+    memcpy(out + (size_t)i * width, &h->poses[(size_t)it->second * 8], (size_t)width * 8);
+  }
+  return 0;
+}
 
 extern "C" {
 
@@ -365,11 +473,16 @@ int d2pgo_default_config(d2pgo_config *c) {
 
 int d2pgo_create(const d2pgo_config *cfg, d2pgo_handle **out) {
   if (!cfg || !out) return 1;
+  if (cfg->pose_dof != 0 && cfg->pose_dof != 6 && cfg->pose_dof != 4) {
+    fprintf(stderr, "d2pgo_create: pose_dof = %d (0 or 6: 6-DoF poses, 4: [x y z yaw] poses)\n", (int)cfg->pose_dof);
+    return 2;
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) { fprintf(stderr, "d2pgo_create: no CUDA device (there is no CPU fallback)\n"); return 3; }
   if (cfg->device < 0 || cfg->device >= ndev || cudaSetDevice(cfg->device) != cudaSuccess) return 4;
   d2pgo_handle *h = new d2pgo_handle();
   h->cfg = *cfg;
+  h->dof = cfg->pose_dof == 4 ? 4 : 6;
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { delete h; return 6; }
   cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1);
   *out = h;
@@ -394,28 +507,26 @@ const char *d2pgo_last_error(const d2pgo_handle *h) { return h ? h->err.c_str() 
 
 int d2pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *poses7, const uint8_t *fixed) {
   if (!h || n <= 0) return 1;
-  h->ids.assign(ids, ids + n); h->index.clear(); h->poses.assign((size_t)n * 8, 0.0); h->fixed.assign(n, 0);
-  for (int i = 0; i < n; i++) {
-    if (!h->index.emplace(ids[i], i).second) { h->err = "set_poses: duplicate pose id"; return 2; }
-    memcpy(&h->poses[(size_t)i * 8], poses7 + (size_t)i * 7, 56);
-    h->fixed[i] = fixed ? fixed[i] : 0;
-  }
-  h->ea.clear(); h->eb.clear(); h->rel.clear(); h->sinfo.clear(); h->uploaded = false;
-  return 0;
+  if (int rc = pgo_want_dof(h, 6, "set_poses")) return rc;
+  return pgo_set_poses(h, n, ids, poses7, 7, fixed, "set_poses");
+}
+
+int d2pgo_set_poses_4d(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *poses4, const uint8_t *fixed) {
+  if (!h || n <= 0) return 1;
+  if (int rc = pgo_want_dof(h, 4, "set_poses_4d")) return rc;
+  return pgo_set_poses(h, n, ids, poses4, 4, fixed, "set_poses_4d");
 }
 
 int d2pgo_add_edges(d2pgo_handle *h, int32_t n, const int64_t *id_a, const int64_t *id_b, const double *rel7, const double *sqrt_info36) {
   if (!h) return 1;
-  for (int e = 0; e < n; e++) {
-    auto a = h->index.find(id_a[e]), b = h->index.find(id_b[e]);
-    if (a == h->index.end() || b == h->index.end()) { h->err = "add_edges: unknown pose id"; return 2; }
-    h->ea.push_back(a->second); h->eb.push_back(b->second);
-    for (int k = 0; k < 7; k++) h->rel.push_back(rel7[(size_t)e * 7 + k]);
-    h->rel.push_back(0.0);
-    for (int k = 0; k < 36; k++) h->sinfo.push_back(sqrt_info36[(size_t)e * 36 + k]);
-  }
-  h->uploaded = false;
-  return 0;
+  if (int rc = pgo_want_dof(h, 6, "add_edges")) return rc;
+  return pgo_add_edges(h, n, id_a, id_b, rel7, 7, sqrt_info36, "add_edges");
+}
+
+int d2pgo_add_edges_4d(d2pgo_handle *h, int32_t n, const int64_t *id_a, const int64_t *id_b, const double *rel4, const double *sqrt_info16) {
+  if (!h) return 1;
+  if (int rc = pgo_want_dof(h, 4, "add_edges_4d")) return rc;
+  return pgo_add_edges(h, n, id_a, id_b, rel4, 4, sqrt_info16, "add_edges_4d");
 }
 
 int d2pgo_comm_init(d2pgo_handle *h, const uint8_t unique_id[128], int32_t rank, int32_t nranks) {
@@ -426,17 +537,20 @@ int d2pgo_comm_init(d2pgo_handle *h, const uint8_t unique_id[128], int32_t rank,
   return 0;
 }
 
+}  // extern "C"
+
 static void pgo_drop_graphs(d2pgo_handle *h) {
   for (int b = 0; b < 2; b++) if (h->cg_graph[b]) { cudaGraphExecDestroy(h->cg_graph[b]); h->cg_graph[b] = nullptr; }
 }
 
 static int pgo_upload(d2pgo_handle *h) {
   const size_t N = h->ids.size(), E = h->ea.size(), nbp = (N + 127) / 128, nbe = (E + 127) / 128;
+  const size_t D = h->dof, DD = D * D;
   pgo_drop_graphs(h);
-  for (int b = 0; b < 2; b++) { PCK(h->d_x[b].alloc(N * 8)); PCK(h->d_g[b].alloc(N * 6)); PCK(h->d_D[b].alloc(N * 36)); PCK(h->d_lin[b].alloc(E * 78)); }
-  PCK(h->d_rel.alloc(E * 8)); PCK(h->d_sinfo.alloc(E * 36)); PCK(h->d_Minv.alloc(N * 36));
-  PCK(h->d_dx.alloc(N * 6)); PCK(h->d_r.alloc(N * 6)); PCK(h->d_z.alloc(N * 6)); PCK(h->d_p.alloc(N * 6)); PCK(h->d_Ap.alloc(N * 6)); PCK(h->d_cost.alloc(2));
-  PCK(h->d_damp.alloc(N * 6)); PCK(h->d_t.alloc(E * 12)); PCK(h->d_part.alloc(5 * nbp)); PCK(h->d_cost_part.alloc(nbe + 1));
+  for (int b = 0; b < 2; b++) { PCK(h->d_x[b].alloc(N * 8)); PCK(h->d_g[b].alloc(N * D)); PCK(h->d_D[b].alloc(N * DD)); PCK(h->d_lin[b].alloc(E * (D + 2 * DD))); }
+  PCK(h->d_rel.alloc(E * 8)); PCK(h->d_sinfo.alloc(E * DD)); PCK(h->d_Minv.alloc(N * DD));
+  PCK(h->d_dx.alloc(N * D)); PCK(h->d_r.alloc(N * D)); PCK(h->d_z.alloc(N * D)); PCK(h->d_p.alloc(N * D)); PCK(h->d_Ap.alloc(N * D)); PCK(h->d_cost.alloc(2));
+  PCK(h->d_damp.alloc(N * D)); PCK(h->d_t.alloc(E * 2 * D)); PCK(h->d_part.alloc(5 * nbp)); PCK(h->d_cost_part.alloc(nbe + 1));
   PCK(h->d_fixed.alloc(N)); PCK(h->d_ea.alloc(E)); PCK(h->d_eb.alloc(E)); PCK(h->d_s.alloc(1)); PCK(h->d_inc_ptr.alloc(N + 1)); PCK(h->d_inc.alloc(2 * E));
   // incidence lists (pose -> its edges, ascending edge order): the fixed summation order of every product
   std::vector<int> ptr(N + 1, 0), inc(2 * E);
@@ -450,7 +564,7 @@ static int pgo_upload(d2pgo_handle *h) {
   if (E) {
     PCK(cudaMemcpyAsync(h->d_inc.p, inc.data(), 2 * E * 4, cudaMemcpyHostToDevice, h->stream));
     PCK(cudaMemcpyAsync(h->d_ea.p, h->ea.data(), E * 4, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(h->d_eb.p, h->eb.data(), E * 4, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(h->d_rel.p, h->rel.data(), E * 64, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(h->d_sinfo.p, h->sinfo.data(), E * 288, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_rel.p, h->rel.data(), E * 64, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(h->d_sinfo.p, h->sinfo.data(), E * DD * 8, cudaMemcpyHostToDevice, h->stream));
   }
   PCK(cudaStreamSynchronize(h->stream));   // ptr / inc go out of scope
   h->uploaded = true;
@@ -467,16 +581,18 @@ static PgoDev pgo_view(d2pgo_handle *h, int cur) {
 }
 
 // cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks
+template <class P>
 static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
+  constexpr int D = P::D;
   PgoDev d = pgo_view(h, b);
   const size_t N = h->ids.size();
   const int nbe = (d.n_edge + 127) / 128;
-  if (d.n_edge > 0) k_pgo_lin<<<nbe, 128, 0, h->stream>>>(d, h->d_cost_part.p, want_jac);
+  if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, h->stream>>>(d, h->d_cost_part.p, want_jac);
   k_pgo_sum<<<1, 128, 0, h->stream>>>(h->d_cost_part.p, nbe, h->d_cost.p);
-  if (want_jac) k_pgo_gD<<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p);
+  if (want_jac) k_pgo_gD<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p);
   if (h->comm) {
     if (nccl_allreduce_f64(h->comm, h->d_cost.p, 1, h->stream)) { h->err = "ncclAllReduce(cost) failed"; return 40; }
-    if (want_jac && (nccl_allreduce_f64(h->comm, h->d_g[b].p, N * 6, h->stream) || nccl_allreduce_f64(h->comm, h->d_D[b].p, N * 36, h->stream))) { h->err = "ncclAllReduce(g, D) failed"; return 40; }
+    if (want_jac && (nccl_allreduce_f64(h->comm, h->d_g[b].p, N * D, h->stream) || nccl_allreduce_f64(h->comm, h->d_D[b].p, N * D * D, h->stream))) { h->err = "ncclAllReduce(g, D) failed"; return 40; }
   }
   PCK(cudaMemcpyAsync(cost, h->d_cost.p, 8, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
@@ -485,26 +601,27 @@ static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
 
 constexpr int kCgChunk = 16;   // CG iterations between two looks at the convergence flag (one graph launch on a single rank)
 
+template <class P>
 static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, double tol2) {
   const int ge = (d.n_edge + 127) / 128;
   for (int k = 0; k < kCgChunk; k++) {
     const int par = k & 1;
-    if (d.n_edge > 0) k_pgo_cg_edge<<<ge, 128, 0, h->stream>>>(d, par, tol2);
+    if (d.n_edge > 0) k_pgo_cg_edge<P><<<ge, 128, 0, h->stream>>>(d, par, tol2);
     if (h->comm) {
-      k_pgo_cg_pose<true><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+      k_pgo_cg_pose<P, true><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
       // every rank holds the same r, z, p (the all-reduced products are bitwise identical), so all of them reach the same
       // `done` decision at the same iteration and the collective below is always matched
-      if (nccl_allreduce_f64(h->comm, d.Ap, (size_t)d.n_pose * 6, h->stream)) { h->err = "ncclAllReduce(Ap) failed"; return 40; }
-      k_pgo_cg_pAp<<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
-    } else k_pgo_cg_pose<false><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
-    k_pgo_cg_step<<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+      if (nccl_allreduce_f64(h->comm, d.Ap, (size_t)d.n_pose * P::D, h->stream)) { h->err = "ncclAllReduce(Ap) failed"; return 40; }
+      k_pgo_cg_pAp<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+    } else k_pgo_cg_pose<P, false><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+    k_pgo_cg_step<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
   }
   return 0;
 }
 
-int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
-  if (!h || h->ids.empty()) return 1;
-  cudaSetDevice(h->cfg.device);
+// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4)
+template <class P>
+static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
   const int N = (int)h->ids.size();
@@ -513,15 +630,15 @@ int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   PCK(cudaEventRecord(h->ev0, h->stream));
   int cur = 0;                    // buffer (poses, lin records, g, D) of the accepted point
   double cost = 0, lambda = h->cfg.lambda0;
-  if ((rc = pgo_linearize(h, cur, 1, &cost))) return rc;
+  if ((rc = pgo_linearize<P>(h, cur, 1, &cost))) return rc;
   R.initial_cost = cost;
   const double tol2 = h->cfg.pcg_tolerance * h->cfg.pcg_tolerance;
   if (tol2 != h->graph_tol2) { pgo_drop_graphs(h); h->graph_tol2 = tol2; }
   for (int it = 0; it < h->cfg.max_iterations; it++) {
     PgoDev d = pgo_view(h, cur);
     // (J^T J + lambda diag D) dx = -g by block-Jacobi preconditioned CG; J^T J is never formed
-    k_pgo_precond<<<gp, 128, 0, h->stream>>>(d, h->d_D[cur].p, lambda);
-    k_pgo_cg_init<<<gp, 128, 0, h->stream>>>(d, h->d_g[cur].p);
+    k_pgo_precond<P><<<gp, 128, 0, h->stream>>>(d, h->d_D[cur].p, lambda);
+    k_pgo_cg_init<P><<<gp, 128, 0, h->stream>>>(d, h->d_g[cur].p);
     k_pgo_cg_init2<<<1, 128, 0, h->stream>>>(d);
     PgoScalars s; memset(&s, 0, sizeof s);
     for (int k = 0; k < h->cfg.pcg_max_iterations; k += kCgChunk) {
@@ -529,20 +646,20 @@ int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
         if (!h->cg_graph[cur]) {
           cudaGraph_t g;
           PCK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-          pgo_cg_chunk(h, d, tol2);
+          pgo_cg_chunk<P>(h, d, tol2);
           PCK(cudaStreamEndCapture(h->stream, &g));
           PCK(cudaGraphInstantiate(&h->cg_graph[cur], g, 0));
           cudaGraphDestroy(g);
         }
         PCK(cudaGraphLaunch(h->cg_graph[cur], h->stream));
-      } else if ((rc = pgo_cg_chunk(h, d, tol2))) return rc;
+      } else if ((rc = pgo_cg_chunk<P>(h, d, tol2))) return rc;
       PCK(cudaMemcpyAsync(&s, h->d_s.p, sizeof s, cudaMemcpyDeviceToHost, h->stream));
       PCK(cudaStreamSynchronize(h->stream));
       if (s.done) break;   // identical on every rank (see pgo_cg_chunk)
     }
-    k_pgo_retract<<<gp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
+    k_pgo_retract<P><<<gp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
     double cand = 0;
-    if ((rc = pgo_linearize(h, 1 - cur, 1, &cand))) return rc;
+    if ((rc = pgo_linearize<P>(h, 1 - cur, 1, &cand))) return rc;
     R.pcg_iterations += s.iters; R.iterations++;
     if (cand < cost && isfinite(cand)) {
       const double rel_dec = (cost - cand) / (cost > 0 ? cost : 1.0);
@@ -564,14 +681,24 @@ int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   return 0;
 }
 
+extern "C" {
+
+int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
+  if (!h || h->ids.empty()) return 1;
+  cudaSetDevice(h->cfg.device);
+  return h->dof == 4 ? pgo_solve<PgoEdge4>(h, rep) : pgo_solve<PgoEdge6>(h, rep);
+}
+
 int d2pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out) {
   if (!h) return 1;
-  for (int i = 0; i < n; i++) {
-    auto it = h->index.find(ids[i]);
-    if (it == h->index.end()) { h->err = "get_poses: unknown id"; return 2; }
-    memcpy(out + (size_t)i * 7, &h->poses[(size_t)it->second * 8], 56);
-  }
-  return 0;
+  if (int rc = pgo_want_dof(h, 6, "get_poses")) return rc;
+  return pgo_get_poses(h, n, ids, out, 7, "get_poses");
+}
+
+int d2pgo_get_poses_4d(d2pgo_handle *h, int32_t n, const int64_t *ids, double *poses4_out) {
+  if (!h) return 1;
+  if (int rc = pgo_want_dof(h, 4, "get_poses_4d")) return rc;
+  return pgo_get_poses(h, n, ids, poses4_out, 4, "get_poses_4d");
 }
 
 int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles) {
@@ -579,13 +706,13 @@ int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles) {
   cudaSetDevice(h->cfg.device);
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
-  const size_t E = h->ea.size();
-  if ((size_t)out_doubles < E * 78) { h->err = "debug_edges: buffer too small"; return 2; }
+  const size_t E = h->ea.size(), W = (size_t)h->dof + 2 * (size_t)h->dof * h->dof;   // 78 (6-DoF) or 36 (4-DoF) per edge
+  if ((size_t)out_doubles < E * W) { h->err = "debug_edges: buffer too small"; return 2; }
   double cost;
-  if ((rc = pgo_linearize(h, 0, 1, &cost))) return rc;
-  std::vector<double> tmp(E * 78);
-  PCK(cudaMemcpy(tmp.data(), h->d_lin[0].p, E * 78 * 8, cudaMemcpyDeviceToHost));
-  for (size_t e = 0; e < E; e++) for (int k = 0; k < 78; k++) out[e * 78 + k] = tmp[(size_t)k * E + e];   // device layout is field-major
+  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4>(h, 0, 1, &cost) : pgo_linearize<PgoEdge6>(h, 0, 1, &cost))) return rc;
+  std::vector<double> tmp(E * W);
+  PCK(cudaMemcpy(tmp.data(), h->d_lin[0].p, E * W * 8, cudaMemcpyDeviceToHost));
+  for (size_t e = 0; e < E; e++) for (size_t k = 0; k < W; k++) out[e * W + k] = tmp[k * E + e];   // device layout is field-major
   return 0;
 }
 

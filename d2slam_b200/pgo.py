@@ -3,7 +3,11 @@
 
 g2o convention (d2pgo/test/posegraph_g2o.cpp:27-39, 57-232): `VERTEX_SE3:QUAT id x y z qx qy qz qw`,
 `EDGE_SE3:QUAT id_a id_b x y z qx qy qz qw <21 upper-triangular information entries>`; for multi-agent files the top byte of
-a vertex id carries chr('a' + agent) (gtsam Symbol style) and the low 56 bits the keyframe index."""
+a vertex id carries chr('a' + agent) (gtsam Symbol style) and the low 56 bits the keyframe index.
+
+4-DoF (d2pgo's default pgo_pose_dof = PGO_POSE_4D): `PgoSolver(pose_dof=4)` with set_poses_4d / add_edges_4d / get_poses_4d
+on [x y z yaw] poses; poses_to_4d / poses_from_4d convert to and from 7-vector poses the way d2pgo does, pose_graph_to_4d
+builds 4-DoF inputs from a make_pose_graph graph."""
 import ctypes as C
 
 import numpy as np
@@ -12,7 +16,7 @@ from .solver import lib as _lib
 
 
 class PgoConfig(C.Structure):
-    _fields_ = [("device", C.c_int32), ("max_iterations", C.c_int32), ("pcg_max_iterations", C.c_int32), ("reserved", C.c_int32),
+    _fields_ = [("device", C.c_int32), ("max_iterations", C.c_int32), ("pcg_max_iterations", C.c_int32), ("pose_dof", C.c_int32),
                 ("pcg_tolerance", C.c_double), ("lambda0", C.c_double), ("function_tolerance", C.c_double)]
 
 
@@ -22,7 +26,10 @@ class PgoReport(C.Structure):
 
 
 PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_last_error", "d2pgo_set_poses", "d2pgo_add_edges",
-                "d2pgo_comm_init", "d2pgo_solve", "d2pgo_get_poses", "d2pgo_debug_edges"]
+                "d2pgo_comm_init", "d2pgo_solve", "d2pgo_get_poses", "d2pgo_debug_edges", "d2pgo_set_poses_4d", "d2pgo_add_edges_4d",
+                "d2pgo_get_poses_4d"]
+_CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
+                  4: "bad device index"}
 
 
 def _p(a):
@@ -41,7 +48,7 @@ class PgoSolver:
         self.h = C.c_void_p()
         rc = L.d2pgo_create(C.byref(self.cfg), C.byref(self.h))
         if rc:
-            raise RuntimeError(f"d2pgo_create failed rc={rc} (CUDA device required; no CPU fallback)")
+            raise RuntimeError(f"d2pgo_create failed rc={rc}: {_CREATE_ERRORS.get(rc, 'CUDA device required; no CPU fallback')}")
         self.n_edges = 0
 
     def _chk(self, rc, what):
@@ -70,6 +77,20 @@ class PgoSolver:
         self._chk(_lib().d2pgo_add_edges(self.h, C.c_int32(len(id_a)), _p(id_a), _p(id_b), _p(rel), _p(si)), "add_edges")
         self.n_edges += len(id_a)
 
+    def set_poses_4d(self, ids, poses4, fixed=None):
+        """[x y z yaw] poses of a pose_dof = 4 solver."""
+        ids = np.ascontiguousarray(ids, np.int64); poses4 = np.ascontiguousarray(poses4, np.float64)
+        f = None if fixed is None else np.ascontiguousarray(fixed, np.uint8)
+        self._chk(_lib().d2pgo_set_poses_4d(self.h, C.c_int32(len(ids)), _p(ids), _p(poses4), _p(f)), "set_poses_4d")
+        self.n_edges = 0
+
+    def add_edges_4d(self, id_a, id_b, rel4, sqrt_info16):
+        """rel4 = [x y z yaw] measurements (RelPoseFactor4D), sqrt_info16 = 4x4 square-root information per edge."""
+        id_a = np.ascontiguousarray(id_a, np.int64); id_b = np.ascontiguousarray(id_b, np.int64)
+        rel4 = np.ascontiguousarray(rel4, np.float64); si = np.ascontiguousarray(sqrt_info16, np.float64)
+        self._chk(_lib().d2pgo_add_edges_4d(self.h, C.c_int32(len(id_a)), _p(id_a), _p(id_b), _p(rel4), _p(si)), "add_edges_4d")
+        self.n_edges += len(id_a)
+
     def comm_init(self, unique_id, rank, nranks):
         uid = (C.c_uint8 * 128)(*unique_id)
         self._chk(_lib().d2pgo_comm_init(self.h, uid, C.c_int32(rank), C.c_int32(nranks)), "comm_init")
@@ -84,8 +105,14 @@ class PgoSolver:
         self._chk(_lib().d2pgo_get_poses(self.h, C.c_int32(len(ids)), _p(ids), _p(out)), "get_poses")
         return out
 
+    def get_poses_4d(self, ids):
+        ids = np.ascontiguousarray(ids, np.int64); out = np.zeros((len(ids), 4))
+        self._chk(_lib().d2pgo_get_poses_4d(self.h, C.c_int32(len(ids)), _p(ids), _p(out)), "get_poses_4d")
+        return out
+
     def debug_edges(self):
-        out = np.zeros((max(self.n_edges, 1), 78))
+        """Per local edge: r | J_a | J_b at the current poses, 78 doubles (6-DoF) or 36 (pose_dof = 4)."""
+        out = np.zeros((max(self.n_edges, 1), 36 if self.cfg.pose_dof == 4 else 78))
         self._chk(_lib().d2pgo_debug_edges(self.h, _p(out), C.c_int64(out.size)), "debug_edges")
         return out[: self.n_edges]
 
@@ -172,6 +199,80 @@ def make_pose_graph(seed=0, n_agents=8, poses_per_agent=1250, loops=30000, sigma
             init[s + k, :3] = init[s + k - 1, :3] + _qrot(init[s + k - 1, 3:7], r[:3]); q = _qmul(init[s + k - 1, 3:7], r[3:7]); init[s + k, 3:7] = q / np.linalg.norm(q)
     fixed = np.zeros(N, np.uint8); fixed[0] = 1; init[0] = gt[0]
     return dict(ids=ids, gt=gt, init=init, fixed=fixed, id_a=ids[ea], id_b=ids[eb], rel=rel, sqrt_info=si.reshape(E, 36), agent=agent, ea=ea, eb=eb)
+
+
+# ------------------------------------------------------------------------------------------------ 4-DoF poses
+def normalize_angle(a):
+    """Utility::NormalizeAngle (utils.hpp:251-257): a - 2 pi floor((a + pi) / 2 pi), in [-pi, pi)."""
+    return a - 2.0 * np.pi * np.floor((a + np.pi) / (2.0 * np.pi))
+
+
+def quat_yaw(q):
+    """Yaw of [qx qy qz qw] quaternions: the z angle of the z-y-x Euler decomposition, atan2(2(w z + x y), 1 - 2(y^2 + z^2)).
+    ASSUMED to be Swarm::Pose::yaw (swarm_msgs is not in the reference tree); the same formula pins RelPoseFactor4D's
+    measurement yaw to the reference functor."""
+    q = np.asarray(q, np.float64)
+    x, y, z, w = q[..., 0], q[..., 1], q[..., 2], q[..., 3]
+    return np.arctan2(2 * (w * z + x * y), 1 - 2 * (y * y + z * z))
+
+
+def _qyaw(yaw):
+    yaw = np.asarray(yaw, np.float64)
+    z = np.zeros_like(yaw)
+    return np.stack([z, z, np.sin(yaw / 2), np.cos(yaw / 2)], axis=-1)
+
+
+def poses_to_4d(poses7):
+    """[x y z qx qy qz qw] -> [x y z yaw], as PGOState::addFrame's 4-DoF branch takes a frame (pgostate.hpp:31-33,
+    Swarm::Pose::to_vector_xyzyaw; yaw by quat_yaw, the ASSUMED Swarm::Pose::yaw)."""
+    p = np.asarray(poses7, np.float64)
+    return np.concatenate([p[..., :3], quat_yaw(p[..., 3:7])[..., None]], axis=-1)
+
+
+def poses_from_4d(x4, ego_poses7):
+    """Solved [x y z yaw] -> [x y z qx qy qz qw] with the ego pose's roll and pitch put back, as D2PGO::getOptimizedTrajs does
+    for 4-DoF (d2pgo.cpp:640-645): q = Rz(yaw) (yaw_only(q_ego)^-1 q_ego)."""
+    x4 = np.asarray(x4, np.float64); qe = np.asarray(ego_poses7, np.float64)[..., 3:7]
+    tilt = _qmul(_qconj(_qyaw(quat_yaw(qe))), qe)
+    q = _qmul(_qyaw(x4[..., 3]), tilt)
+    return np.concatenate([x4[..., :3], q / np.linalg.norm(q, axis=-1, keepdims=True)], axis=-1)
+
+
+def pose_graph_to_4d(g, seed=0, sigma_t=0.05, sigma_yaw=np.deg2rad(1.0)):
+    """4-DoF inputs from a make_pose_graph graph: the same ground truth (as [x y z yaw]) and the same edge topology, measurements
+    Rz(-yaw_a)(p_b - p_a) + noise and N(yaw_b - yaw_a + noise), diagonal square-root information, initial guess chained from the
+    odometry edges per agent (first pose of every agent from ground truth + noise), pose 0 fixed at ground truth.
+    Returns dict(ids, gt, init, fixed, id_a, id_b, ea, eb, rel, sqrt_info, agent) with 4-vectors and [E, 16] sqrt_info."""
+    rng = np.random.default_rng(seed)
+    gt = poses_to_4d(g["gt"]); ea = np.asarray(g["ea"]); eb = np.asarray(g["eb"]); agent = np.asarray(g["agent"])
+    E = len(ea)
+    c, s = np.cos(-gt[ea, 3]), np.sin(-gt[ea, 3]); v = gt[eb, :3] - gt[ea, :3]
+    rel = np.zeros((E, 4))
+    rel[:, 0] = c * v[:, 0] - s * v[:, 1] + rng.normal(0, sigma_t, E)
+    rel[:, 1] = s * v[:, 0] + c * v[:, 1] + rng.normal(0, sigma_t, E)
+    rel[:, 2] = v[:, 2] + rng.normal(0, sigma_t, E)
+    rel[:, 3] = normalize_angle(gt[eb, 3] - gt[ea, 3] + rng.normal(0, sigma_yaw, E))
+    si = np.zeros((E, 4, 4)); si[:, [0, 1, 2], [0, 1, 2]] = 1.0 / sigma_t; si[:, 3, 3] = 1.0 / sigma_yaw
+    # odometry edges: e -> (i, i + 1) within one agent; each pose after an agent's first has exactly one (make_pose_graph lists
+    # them first)
+    odo = np.full(len(gt), -1)
+    n_odo = len(gt) - len(np.unique(agent))
+    assert np.all(eb[:n_odo] == ea[:n_odo] + 1) and np.all(agent[ea[:n_odo]] == agent[eb[:n_odo]])
+    odo[eb[:n_odo]] = np.arange(n_odo)
+    init = gt.copy()
+    for a in np.unique(agent):
+        idx = np.nonzero(agent == a)[0]; s0 = idx[0]
+        e = odo[idx[1:]]
+        assert np.all(e >= 0)
+        init[s0, :3] += rng.normal(0, 0.2, 3)
+        yaw = init[s0, 3] + np.concatenate([[0.0], np.cumsum(rel[e, 3])])
+        c, s = np.cos(yaw[:-1]), np.sin(yaw[:-1])
+        step = np.stack([c * rel[e, 0] - s * rel[e, 1], s * rel[e, 0] + c * rel[e, 1], rel[e, 2]], axis=1)
+        init[idx, :3] = init[s0, :3] + np.concatenate([np.zeros((1, 3)), np.cumsum(step, axis=0)])
+        init[idx, 3] = normalize_angle(yaw)
+    fixed = np.zeros(len(gt), np.uint8); fixed[0] = 1; init[0] = gt[0]
+    return dict(ids=np.asarray(g["ids"]), gt=gt, init=init, fixed=fixed, id_a=np.asarray(g["id_a"]), id_b=np.asarray(g["id_b"]), ea=ea, eb=eb,
+                rel=rel, sqrt_info=si.reshape(E, 16), agent=agent)
 
 
 # ------------------------------------------------------------------------------------------------ g2o files
