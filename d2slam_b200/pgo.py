@@ -7,7 +7,10 @@ a vertex id carries chr('a' + agent) (gtsam Symbol style) and the low 56 bits th
 
 4-DoF (d2pgo's default pgo_pose_dof = PGO_POSE_4D): `PgoSolver(pose_dof=4)` with set_poses_4d / add_edges_4d / get_poses_4d
 on [x y z yaw] poses; poses_to_4d / poses_from_4d convert to and from 7-vector poses the way d2pgo does, pose_graph_to_4d
-builds 4-DoF inputs from a make_pose_graph graph."""
+builds 4-DoF inputs from a make_pose_graph graph.
+
+PCM (d2pgo's enable_pcm): `PgoSolver.pcm` rejects inconsistent loop closures before they are added (include/d2pgo.h
+d2pgo_pcm); make_pcm_case builds its inputs from a make_pose_graph graph, with injected gross outliers."""
 import ctypes as C
 
 import numpy as np
@@ -25,9 +28,18 @@ class PgoReport(C.Structure):
                 ("initial_cost", C.c_double), ("final_cost", C.c_double), ("device_ms", C.c_double)]
 
 
+class PcmConfig(C.Structure):
+    _fields_ = [("pcm_thres", C.c_double), ("pos_covariance_per_meter", C.c_double), ("yaw_covariance_per_meter", C.c_double)]
+
+
+class PcmReport(C.Structure):
+    _fields_ = [("groups", C.c_int32), ("inliers", C.c_int32), ("pairs_tested", C.c_int64), ("consistent_pairs", C.c_int64),
+                ("clique_rounds", C.c_int64), ("device_ms", C.c_double), ("pair_ms", C.c_double), ("clique_ms", C.c_double)]
+
+
 PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_last_error", "d2pgo_set_poses", "d2pgo_add_edges",
                 "d2pgo_comm_init", "d2pgo_solve", "d2pgo_get_poses", "d2pgo_debug_edges", "d2pgo_set_poses_4d", "d2pgo_add_edges_4d",
-                "d2pgo_get_poses_4d"]
+                "d2pgo_get_poses_4d", "d2pgo_default_pcm_config", "d2pgo_pcm", "d2pgo_debug_pcm_smd", "d2pgo_debug_pcm_clique"]
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
 
@@ -115,6 +127,44 @@ class PgoSolver:
         out = np.zeros((max(self.n_edges, 1), 36 if self.cfg.pose_dof == 4 else 78))
         self._chk(_lib().d2pgo_debug_edges(self.h, _p(out), C.c_int64(out.size)), "debug_edges")
         return out[: self.n_edges]
+
+    def pcm(self, frame_ids, frame_agent, ego_poses7, kf_a, kf_b, rel7, sqrt_info36, **cfg):
+        """Loop-closure outlier rejection (d2pgo's enable_pcm; include/d2pgo.h d2pgo_pcm): boolean inlier mask over the loops.
+        cfg overrides PcmConfig fields (pcm_thres, pos_covariance_per_meter, yaw_covariance_per_meter); the report of the
+        call is kept in self.pcm_report.  The handle's poses and edges are not touched."""
+        c = PcmConfig()
+        _lib().d2pgo_default_pcm_config(C.byref(c))
+        for k, v in cfg.items():
+            setattr(c, k, v)
+        fid = np.ascontiguousarray(frame_ids, np.int64); fag = np.ascontiguousarray(frame_agent, np.int32)
+        ego = np.ascontiguousarray(ego_poses7, np.float64).reshape(-1, 7)
+        ka = np.ascontiguousarray(kf_a, np.int64); kb = np.ascontiguousarray(kf_b, np.int64)
+        rel = np.ascontiguousarray(rel7, np.float64).reshape(-1, 7); si = np.ascontiguousarray(sqrt_info36, np.float64).reshape(-1, 36)
+        out = np.zeros(max(len(ka), 1), np.uint8); r = PcmReport()
+        self._chk(_lib().d2pgo_pcm(self.h, C.byref(c), C.c_int32(len(fid)), _p(fid), _p(fag), _p(ego), C.c_int32(len(ka)), _p(ka), _p(kb), _p(rel), _p(si),
+                                   _p(out), C.byref(r)), "pcm")
+        self.pcm_report = r
+        return out[: len(ka)].astype(bool)
+
+    def debug_pcm_smd(self):
+        """smd of every tested loop pair (i, j < i) of the last pcm() call, group-major (include/d2pgo.h)."""
+        out = np.zeros(max(int(self.pcm_report.pairs_tested), 1))
+        self._chk(_lib().d2pgo_debug_pcm_smd(self.h, _p(out), C.c_int64(out.size)), "debug_pcm_smd")
+        return out[: int(self.pcm_report.pairs_tested)]
+
+    def debug_pcm_clique(self, adj):
+        """The device clique kernel alone on a symmetric boolean adjacency [n, n] -> boolean membership [n]."""
+        words = pcm_pack_bits(adj)
+        n = len(words); member = np.zeros(max(n, 1), np.uint8); size = C.c_int32()
+        self._chk(_lib().d2pgo_debug_pcm_clique(self.h, C.c_int32(n), _p(words), _p(member), C.byref(size)), "debug_pcm_clique")
+        return member[:n].astype(bool)
+
+
+def pcm_pack_bits(adj):
+    """Boolean [n, n] -> uint32 rows [n, ceil(n / 32)], bit j of row i = word j // 32, bit j % 32 (d2pgo_debug_pcm_clique)."""
+    adj = np.asarray(adj, bool); n = len(adj); W = (n + 31) // 32
+    pad = np.zeros((n, W * 32), bool); pad[:, :n] = adj
+    return np.ascontiguousarray((pad.reshape(n, W, 32).astype(np.uint64) << np.arange(32, dtype=np.uint64)).sum(-1).astype(np.uint32))
 
 
 # ------------------------------------------------------------------------------------------------ synthetic graphs
@@ -273,6 +323,40 @@ def pose_graph_to_4d(g, seed=0, sigma_t=0.05, sigma_yaw=np.deg2rad(1.0)):
     fixed = np.zeros(len(gt), np.uint8); fixed[0] = 1; init[0] = gt[0]
     return dict(ids=np.asarray(g["ids"]), gt=gt, init=init, fixed=fixed, id_a=np.asarray(g["id_a"]), id_b=np.asarray(g["id_b"]), ea=ea, eb=eb,
                 rel=rel, sqrt_info=si.reshape(E, 16), agent=agent)
+
+
+# ------------------------------------------------------------------------------------------------ PCM cases
+def _odometry_chain(g):
+    """Per-agent ego trajectories: the first pose of every agent from ground truth, then the odometry edges composed."""
+    gt = np.asarray(g["gt"]); agent = np.asarray(g["agent"]); ea = np.asarray(g["ea"]); eb = np.asarray(g["eb"]); rel = np.asarray(g["rel"])
+    n_odo = len(gt) - len(np.unique(agent))
+    assert np.all(eb[:n_odo] == ea[:n_odo] + 1)
+    ego = gt.copy()
+    for e in range(n_odo):
+        a, b = ea[e], eb[e]
+        ego[b, :3] = ego[a, :3] + _qrot(ego[a, 3:7], rel[e, :3]); q = _qmul(ego[a, 3:7], rel[e, 3:7]); ego[b, 3:7] = q / np.linalg.norm(q)
+    return ego, n_odo
+
+
+def make_pcm_case(g, outlier_frac=0.05, seed=0):
+    """A PCM input from a make_pose_graph graph: frames = every pose with its agent and its ego pose (the agent's odometry
+    chain), loops = the edges after the odometry edges, `rel_bad` = the same loops with a fraction turned into gross
+    outliers (2-10 m of translation in a random direction and 20-180 degrees of yaw, random sign), `outlier` = which,
+    `bad_dt` / `bad_yaw` = the perturbations of the outliers in loop order (to corrupt 4-DoF measurements the same way)."""
+    rng = np.random.default_rng(seed)
+    ego, n_odo = _odometry_chain(g)
+    ids = np.asarray(g["ids"]); agent = np.asarray(g["agent"]).astype(np.int32)
+    rel = np.array(g["rel"][n_odo:]); L = len(rel)
+    bad = np.zeros(L, bool); bad[rng.choice(L, int(round(outlier_frac * L)), replace=False)] = True
+    k = int(bad.sum())
+    d = rng.normal(size=(k, 3)); d /= np.linalg.norm(d, axis=1, keepdims=True)
+    rel_bad = rel.copy()
+    rel_bad[bad, :3] += d * rng.uniform(2.0, 10.0, (k, 1))
+    yaw = rng.uniform(np.deg2rad(20), np.pi, k) * rng.choice([-1.0, 1.0], k)
+    q = _qmul(rel_bad[bad, 3:7], _qyaw(yaw)); rel_bad[bad, 3:7] = q / np.linalg.norm(q, axis=1, keepdims=True)
+    return dict(frame_ids=ids, frame_agent=agent, ego=ego, kf_a=np.asarray(g["id_a"][n_odo:]), kf_b=np.asarray(g["id_b"][n_odo:]), rel=rel,
+                rel_bad=rel_bad, sqrt_info=np.asarray(g["sqrt_info"][n_odo:]), outlier=bad, bad_dt=d * np.linalg.norm(rel_bad[bad, :3] - rel[bad, :3], axis=1, keepdims=True),
+                bad_yaw=yaw, n_odo=n_odo)
 
 
 # ------------------------------------------------------------------------------------------------ g2o files

@@ -14,6 +14,8 @@
  *   d2pgo_add_edges_4d            <- setupLoopFactors / setupEgoMotionFactors, 4-DoF branches (d2pgo/src/d2pgo.cpp:422-423,
  *                                    496-500): one RelPoseFactor4D per edge (RelPoseFactor.hpp:196-238)
  *   d2pgo_get_poses_4d            <- syncFromState: the optimised [x y z yaw] blocks
+ *   d2pgo_pcm                     <- SwarmLocalOutlierRejection::OutlierRejectionLoopEdges (enable_pcm), the loops it keeps
+ *                                    being those setupLoopFactors receives (d2pgo/src/d2pgo.cpp:177-186, :276-282)
  *
  * Scope note: the reference solves the multi-agent graph with ARock (asynchronous dual updates, ARock.cpp:140-328) around
  * per-agent ceres problems; BASELINE's config asks for a *distributed Gauss-Newton* on the 8 GPUs of one box.  Here every
@@ -79,6 +81,51 @@ int d2pgo_get_poses_4d(d2pgo_handle *h, int32_t n, const int64_t *ids, double *p
 /* parity hook: residual and the two tangent Jacobians of every local edge at the current poses, row-major:
  * 6-DoF out[n_edges][78] = r(6) | J_a (6x6) | J_b (6x6);  4-DoF out[n_edges][36] = r(4) | J_a (4x4) | J_b (4x4) */
 int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles);
+
+/* ---- loop-closure outlier rejection: pairwise-consistency maximisation (PCM)
+ *   d2pgo_pcm  <- SwarmLocalOutlierRejection::OutlierRejectionLoopEdges with redundant = true, incremental_pcm = false,
+ *                 is_4dof = (pose_dof == 4), fed every loop once in the order given
+ *                 (d2pgo/src/swarm_outlier_rejection/swarm_outlier_rejection.cpp:46-303; called by D2PGO::solve_single /
+ *                 solve_multi before setupLoopFactors, d2pgo/src/d2pgo.cpp:177-186, :276-282, when enable_pcm is set)
+ *   clique     <- FMC::maxCliqueHeu (d2pgo/third_party/fast_max-clique_finder/src/findCliqueHeu.cpp:124-243)
+ * Loops are grouped by the unordered pair of drone ids (a drone with itself included).  Within a group every loop i is tested
+ * against every earlier loop j: err = odom_a p2 odom_b^-1 rel_i^-1 with p2 = rel_j, odom_a = odom(a_i -> a_j), odom_b =
+ * odom(b_i -> b_j) when the two loops name the drones in the same order, and p2 = rel_j^-1, odom_a = odom(a_i -> b_j), odom_b =
+ * odom(b_i -> a_j) when swapped; smd = log(err)^T Sigma^-1 log(err), Sigma = cov_i + cov_j + cov(odom_a) + cov(odom_b), and the
+ * two loops are consistent iff smd < (float)pcm_thres.  A loop is an inlier iff it is in its group's FMC clique.
+ * odom(f -> g) = DeltaPose(ego_f, ego_g) (yaw only on a 4-DoF handle: (Rz(-yaw_f)(p_g - p_f), Rz(yaw_g - yaw_f))) with the
+ * diagonal covariance (pos_covariance_per_meter len + yaw_covariance_per_meter len^2 / 2) I3, yaw_covariance_per_meter len I3
+ * at the path length len along the drone's keyframes between f and g (a drone's keyframes in the order given).
+ * cov_i = (S^T S)^-1 of the loop's 6x6 square-root information; log = [t ; rotation vector].
+ * The handle's poses and edges are not touched: add the inliers with d2pgo_add_edges[_4d].  Deterministic (bitwise the same
+ * mask on every call and every rank).  A group holds at most 32768 loops. */
+typedef struct d2pgo_pcm_config {
+  double pcm_thres;                  /* consistency threshold on smd; rounded to float like the reference's field (1.635) */
+  double pos_covariance_per_meter;   /* ego-motion model (d2pgo_config.h defaults 4e-3, 4e-5)                          */
+  double yaw_covariance_per_meter;
+} d2pgo_pcm_config;
+
+typedef struct d2pgo_pcm_report {
+  int32_t groups;                    /* drone pairs with at least one loop                                              */
+  int32_t inliers;
+  int64_t pairs_tested;              /* sum over groups of L (L - 1) / 2                                                */
+  int64_t consistent_pairs;
+  int64_t clique_rounds;             /* greedy picks made by the clique kernel, seeds examined again included           */
+  double device_ms, pair_ms, clique_ms;   /* whole call on the device; its consistency part; its clique part          */
+} d2pgo_pcm_report;
+
+int d2pgo_default_pcm_config(d2pgo_pcm_config *cfg);
+/* frames: every keyframe a loop names, with its drone and ego (odometry) pose [x y z qx qy qz qw]; loops: keyframe ids,
+ * rel7 = T_a^-1 T_b, sqrt_info36 row-major.  inlier_out[n_loops] = 1 / 0.  Returns non-zero (d2pgo_last_error says why) on
+ * an unknown or duplicate keyframe id, a non-finite or non-positive threshold, or a group of more than 32768 loops. */
+int d2pgo_pcm(d2pgo_handle *h, const d2pgo_pcm_config *cfg, int32_t n_frames, const int64_t *frame_ids, const int32_t *frame_agent,
+              const double *ego_poses7, int32_t n_loops, const int64_t *kf_a, const int64_t *kf_b, const double *rel7,
+              const double *sqrt_info36, uint8_t *inlier_out, d2pgo_pcm_report *report);
+/* parity hooks.  smd of every tested pair (i, j < i) of the last d2pgo_pcm call: groups in order of their first loop, rows i
+ * ascending, j ascending (report.pairs_tested doubles).  The clique kernel alone on a caller-given symmetric adjacency without
+ * self loops, adj[n][ceil(n / 32)] words, bit j of row i = word j / 32, bit j % 32: member_out[n], size_out = clique size. */
+int d2pgo_debug_pcm_smd(d2pgo_handle *h, double *out, int64_t out_doubles);
+int d2pgo_debug_pcm_clique(d2pgo_handle *h, int32_t n, const uint32_t *adj, uint8_t *member_out, int32_t *size_out);
 
 #ifdef __cplusplus
 }
