@@ -7,6 +7,8 @@
 // pgo_use_autodiff is off, drops q_rel from its rotation blocks -- its Jacobian is exact only for identity relative rotation.)
 // And RelPoseFactor4D (:196-238), d2pgo's default 4-DoF configuration, in pgo_edge_eval_4d.  One solver serves both: every
 // kernel is a template over an edge policy (PgoEdge6 / PgoEdge4) that fixes the block size D and the retraction.
+// Unary gravity priors (GravityPriorPerturbAD, d2pgo's enable_gravity_prior) on 6-DoF poses in pgo_gravity_eval: the kernels
+// that sum per-pose terms take a GRAV flag, so the instantiations without priors are the kernels of a graph of edges alone.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -54,6 +56,16 @@ struct PgoDev {
   double *pAp_part;           // [nbp]
   int nbp;                    // pose blocks of 128
   PgoScalars *s;
+};
+
+// gravity priors of this rank (6-DoF only).  A separate, last kernel parameter: read by the GRAV = true instantiations only, it
+// leaves the parameter layout of the edge-only kernels as it was.
+struct PgoPriorDev {
+  int n_prior;
+  const int *pose;            // [G] pose index of each prior
+  const int *prior_of;        // [N] the prior of each pose, -1 = none
+  const double *u, *S;        // [G][3] u_ego = R(q_ego)^T e3, [G][9] S row-major
+  double *lin;                // [12][G] field-major: r(3), J_theta (3x3 row-major)
 };
 
 // RelPoseFactorAD (RelPoseFactor.hpp:68-135; the reference's default 6-DoF factor, pgo_use_autodiff = true in
@@ -138,6 +150,22 @@ struct PgoEdge4 {   // RelPoseFactor4D on [x y z yaw], PosAngleManifold::Plus (a
   }
 };
 
+// GravityPriorPerturbAD (GravityPrior.hpp:8-46, added per frame by D2PGO::setupGravityPriorFactors, d2pgo.cpp:530-559):
+// u = R(q)^T e3 (the third row of R), r = S^T (u - u_ego) -- the reference forms the row R.row(2) - R_ego.row(2) and applies
+// S on the right.  In the tangent of the right-multiplicative retraction: dr/d dtheta = S^T [u]x, dr/d dp = 0 (rank 2: yaw
+// about gravity stays free).  The reference's chart q0 (x) quatfromRotationVector(theta) has the same value and derivative at
+// theta = 0; inside |theta| < 1e-2 it uses the unnormalised [1, theta/2], which this evaluation at the exact pose does not.
+D2BA_DEV void pgo_gravity_eval(const double *x, const double *ue, const double *S, double *r, double *J) {
+  double R[9];
+  q2R(qload(x + 3), R);
+  const double u[3] = {R[6], R[7], R[8]};
+  const double du[3] = {u[0] - ue[0], u[1] - ue[1], u[2] - ue[2]};
+  for (int i = 0; i < 3; i++) r[i] = S[i] * du[0] + S[3 + i] * du[1] + S[6 + i] * du[2];
+  if (!J) return;
+  const double K[9] = {0.0, -u[2], u[1], u[2], 0.0, -u[0], -u[1], u[0], 0.0};   // [u]x
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) J[i * 3 + j] = S[i] * K[j] + S[3 + i] * K[3 + j] + S[6 + i] * K[6 + j];
+}
+
 // Fixed-order sum of n per-block partials, the same value in every thread of every block (so that all blocks -- and all
 // ranks, which hold identical vectors -- take the same branch without a single-thread "decide" kernel in between).
 D2BA_DEV double total_of(const double *part, int n, double *red) {
@@ -174,6 +202,55 @@ __global__ void __launch_bounds__(128) k_pgo_lin(PgoDev d, double *cost_part, in
   c = block_sum(c, red);
   if (threadIdx.x == 0) cost_part[blockIdx.x] = c;
 }
+// linearise every local gravity prior at d.x: glin records [r | J_theta]; cost partials go after the edges' (k_pgo_sum)
+__global__ void __launch_bounds__(128) k_pgo_prior_lin(PgoDev d, double *cost_part, int want_jac, PgoPriorDev pr) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  __shared__ double red[40];
+  double c = 0.0;
+  if (k < pr.n_prior) {
+    double r[3], J[9];
+    pgo_gravity_eval(d.x + (size_t)pr.pose[k] * 8, pr.u + (size_t)k * 3, pr.S + (size_t)k * 9, r, J);   // J always: keeps r, J in registers
+    for (int a = 0; a < 3; a++) c += 0.5 * r[a] * r[a];
+    if (want_jac) {
+      double *o = pr.lin + k;
+      const size_t G = (size_t)pr.n_prior;
+      for (int a = 0; a < 3; a++) o[a * G] = r[a];
+      for (int a = 0; a < 9; a++) o[(3 + a) * G] = J[a];
+    }
+  }
+  c = block_sum(c, red);
+  if (threadIdx.x == 0) cost_part[blockIdx.x] = c;
+}
+
+// pose i's gravity prior, after its edges: g += J^T r, D += J^T J on the rotation block (D = 6 only)
+template <int D>
+D2BA_DEV void prior_gD(const PgoPriorDev &pr, int i, double *gi, double *Di) {
+  const int k = pr.prior_of[i];
+  if (k < 0) return;
+  const size_t G = (size_t)pr.n_prior;
+  const double *o = pr.lin + k;
+  for (int a = 0; a < 3; a++) {
+    const double ra = o[a * G];
+    double row[3];
+    for (int b = 0; b < 3; b++) { row[b] = o[(3 + a * 3 + b) * G]; gi[3 + b] += row[b] * ra; }
+    for (int b = 0; b < 3; b++) for (int c = 0; c < 3; c++) Di[(3 + b) * D + 3 + c] += row[b] * row[c];
+  }
+}
+
+// pose i's gravity prior in a CG product: y += J^T (J p) on the rotation block
+template <int D>
+D2BA_DEV void prior_Ap(const PgoPriorDev &pr, int i, const double *p, double *y) {
+  const int k = pr.prior_of[i];
+  if (k < 0) return;
+  const size_t G = (size_t)pr.n_prior;
+  const double *J = pr.lin + (size_t)3 * G + k;
+  for (int a = 0; a < 3; a++) {
+    double j[3], t = 0.0;
+    for (int b = 0; b < 3; b++) { j[b] = J[(size_t)(a * 3 + b) * G]; t += j[b] * p[3 + b]; }
+    for (int b = 0; b < 3; b++) y[3 + b] += j[b] * t;
+  }
+}
+
 __global__ void k_pgo_sum(const double *part, int n, double *out) {
   __shared__ double red[40];
   const double v = total_of(part, n, red);
@@ -181,16 +258,17 @@ __global__ void k_pgo_sum(const double *part, int n, double *out) {
 }
 
 // gradient g_i = sum J^T r and block diagonal D_i = sum J^T J over the edges incident to pose i, in the fixed order of the
-// incidence list (no atomics: bitwise reproducible)
-template <class P>
-__global__ void __launch_bounds__(128) k_pgo_gD(PgoDev d, double *g, double *Dg) {
+// incidence list (no atomics: bitwise reproducible); with GRAV, the pose's gravity prior after its edges
+template <class P, bool GRAV>
+__global__ void __launch_bounds__(128) k_pgo_gD(PgoDev d, double *g, double *Dg, PgoPriorDev pr) {
   constexpr int D = P::D, DD = D * D;
+  static_assert(!GRAV || D == 6, "gravity priors act on 6-DoF poses");
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= d.n_pose) return;
   double gi[D], Di[DD];
   for (int k = 0; k < D; k++) gi[k] = 0.0;
   for (int k = 0; k < DD; k++) Di[k] = 0.0;
-  if (!d.fixed[i])
+  if (!d.fixed[i]) {
     for (int q = d.inc_ptr[i]; q < d.inc_ptr[i + 1]; q++) {
       const int c = d.inc[q];
       const size_t E = (size_t)d.n_edge;
@@ -202,6 +280,8 @@ __global__ void __launch_bounds__(128) k_pgo_gD(PgoDev d, double *g, double *Dg)
         for (int a = 0; a < D; a++) for (int b = 0; b < D; b++) Di[a * D + b] += row[a] * row[b];
       }
     }
+    if constexpr (GRAV) prior_gD<D>(pr, i, gi, Di);
+  }
   for (int k = 0; k < D; k++) g[(size_t)i * D + k] = gi[k];
   for (int k = 0; k < DD; k++) Dg[(size_t)i * DD + k] = Di[k];
 }
@@ -282,10 +362,12 @@ __global__ void __launch_bounds__(128) k_pgo_cg_edge(PgoDev d, int par, double t
   for (int q = 0; q < D; q++) { d.t[(size_t)q * E + e] = ya[q]; d.t[(size_t)(D + q) * E + e] = yb[q]; }
 }
 
-// LOCAL: this rank's edges only, no damping / p.Ap yet (the all-reduce of Ap comes first; k_pgo_cg_pAp follows)
-template <class P, bool LOCAL>
-__global__ void __launch_bounds__(128) k_pgo_cg_pose(PgoDev d, int par, double tol2) {
+// LOCAL: this rank's edges only, no damping / p.Ap yet (the all-reduce of Ap comes first; k_pgo_cg_pAp follows).
+// GRAV: the pose's gravity prior after its edges.
+template <class P, bool LOCAL, bool GRAV>
+__global__ void __launch_bounds__(128) k_pgo_cg_pose(PgoDev d, int par, double tol2, PgoPriorDev pr) {
   constexpr int D = P::D;
+  static_assert(!GRAV || D == 6, "gravity priors act on 6-DoF poses");
   __shared__ double red[40];
   const CgView v = cg_view(d, par, tol2, red);
   if (v.done) return;
@@ -296,13 +378,15 @@ __global__ void __launch_bounds__(128) k_pgo_cg_pose(PgoDev d, int par, double t
     double p[D], y[D];
     for (int k = 0; k < D; k++) y[k] = 0.0;
     cg_p_new<D>(d, i, beta, p);
-    if (!d.fixed[i])
+    if (!d.fixed[i]) {
       for (int q = d.inc_ptr[i]; q < d.inc_ptr[i + 1]; q++) {
         const int c = d.inc[q];
         const size_t E = (size_t)d.n_edge;
         const double *t = d.t + (size_t)(D * (c & 1)) * E + (c >> 1);
         for (int a = 0; a < D; a++) y[a] += t[a * E];
       }
+      if constexpr (GRAV) prior_Ap<D>(pr, i, p, y);
+    }
     for (int k = 0; k < D; k++) {
       d.p[(size_t)i * D + k] = p[k];
       if (!LOCAL) { y[k] += d.damp[(size_t)i * D + k] * p[k]; s += p[k] * y[k]; }
@@ -682,6 +766,8 @@ struct d2pgo_handle {
   std::vector<int64_t> ids; std::unordered_map<int64_t, int> index;
   std::vector<double> poses; std::vector<unsigned char> fixed;   // [N][8], the device layout of PgoDev::x
   std::vector<int> ea, eb; std::vector<double> rel, sinfo;         // rel [E][8], sinfo [E][dof^2]
+  std::vector<int> gp_pose; std::vector<double> gp_u, gp_S;        // gravity priors: pose index, u_ego [G][3], S [G][9]
+  Buf<double> d_gp_u, d_gp_S, d_glin[2]; Buf<int> d_gp_pose, d_prior_of;
   Buf<double> d_x[2], d_rel, d_sinfo, d_lin[2], d_g[2], d_D[2], d_Minv, d_dx, d_r, d_z, d_p, d_Ap, d_cost, d_damp, d_t, d_part, d_cost_part;
   Buf<unsigned char> d_fixed; Buf<int> d_ea, d_eb, d_inc_ptr, d_inc; Buf<PgoScalars> d_s;
   cudaGraphExec_t cg_graph[2] = {nullptr, nullptr};   // 16 CG iterations on the linearisation buffer 0 / 1 (single rank)
@@ -709,6 +795,7 @@ static int pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const d
     h->fixed[i] = fixed ? fixed[i] : 0;
   }
   h->ea.clear(); h->eb.clear(); h->rel.clear(); h->sinfo.clear(); h->uploaded = false;
+  h->gp_pose.clear(); h->gp_u.clear(); h->gp_S.clear();
   return 0;
 }
 
@@ -771,6 +858,7 @@ int d2pgo_destroy(d2pgo_handle *h) {
   h->d_damp.release(); h->d_t.release(); h->d_part.release(); h->d_cost_part.release(); h->d_inc_ptr.release(); h->d_inc.release();
   h->d_rel.release(); h->d_sinfo.release(); h->d_Minv.release(); h->d_dx.release(); h->d_r.release(); h->d_z.release(); h->d_p.release();
   h->d_Ap.release(); h->d_cost.release(); h->d_fixed.release(); h->d_ea.release(); h->d_eb.release(); h->d_s.release();
+  h->d_gp_u.release(); h->d_gp_S.release(); h->d_glin[0].release(); h->d_glin[1].release(); h->d_gp_pose.release(); h->d_prior_of.release();
   h->pcm.release();
   cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1); cudaStreamDestroy(h->stream);
   delete h;
@@ -824,7 +912,8 @@ static int pgo_upload(d2pgo_handle *h) {
   for (int b = 0; b < 2; b++) { PCK(h->d_x[b].alloc(N * 8)); PCK(h->d_g[b].alloc(N * D)); PCK(h->d_D[b].alloc(N * DD)); PCK(h->d_lin[b].alloc(E * (D + 2 * DD))); }
   PCK(h->d_rel.alloc(E * 8)); PCK(h->d_sinfo.alloc(E * DD)); PCK(h->d_Minv.alloc(N * DD));
   PCK(h->d_dx.alloc(N * D)); PCK(h->d_r.alloc(N * D)); PCK(h->d_z.alloc(N * D)); PCK(h->d_p.alloc(N * D)); PCK(h->d_Ap.alloc(N * D)); PCK(h->d_cost.alloc(2));
-  PCK(h->d_damp.alloc(N * D)); PCK(h->d_t.alloc(E * 2 * D)); PCK(h->d_part.alloc(5 * nbp)); PCK(h->d_cost_part.alloc(nbe + 1));
+  const size_t G = h->gp_pose.size(), nbg = (G + 127) / 128;
+  PCK(h->d_damp.alloc(N * D)); PCK(h->d_t.alloc(E * 2 * D)); PCK(h->d_part.alloc(5 * nbp)); PCK(h->d_cost_part.alloc(nbe + nbg + 1));
   PCK(h->d_fixed.alloc(N)); PCK(h->d_ea.alloc(E)); PCK(h->d_eb.alloc(E)); PCK(h->d_s.alloc(1)); PCK(h->d_inc_ptr.alloc(N + 1)); PCK(h->d_inc.alloc(2 * E));
   // incidence lists (pose -> its edges, ascending edge order): the fixed summation order of every product
   std::vector<int> ptr(N + 1, 0), inc(2 * E);
@@ -840,7 +929,18 @@ static int pgo_upload(d2pgo_handle *h) {
     PCK(cudaMemcpyAsync(h->d_ea.p, h->ea.data(), E * 4, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(h->d_eb.p, h->eb.data(), E * 4, cudaMemcpyHostToDevice, h->stream));
     PCK(cudaMemcpyAsync(h->d_rel.p, h->rel.data(), E * 64, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(h->d_sinfo.p, h->sinfo.data(), E * DD * 8, cudaMemcpyHostToDevice, h->stream));
   }
-  PCK(cudaStreamSynchronize(h->stream));   // ptr / inc go out of scope
+  std::vector<int> prior_of;
+  if (G) {   // gravity priors: records and the per-pose index
+    PCK(h->d_gp_pose.alloc(G)); PCK(h->d_gp_u.alloc(G * 3)); PCK(h->d_gp_S.alloc(G * 9)); PCK(h->d_prior_of.alloc(N));
+    for (int b = 0; b < 2; b++) PCK(h->d_glin[b].alloc(G * 12));
+    prior_of.assign(N, -1);
+    for (size_t k = 0; k < G; k++) prior_of[h->gp_pose[k]] = (int)k;
+    PCK(cudaMemcpyAsync(h->d_gp_pose.p, h->gp_pose.data(), G * 4, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_gp_u.p, h->gp_u.data(), G * 24, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_gp_S.p, h->gp_S.data(), G * 72, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_prior_of.p, prior_of.data(), N * 4, cudaMemcpyHostToDevice, h->stream));
+  }
+  PCK(cudaStreamSynchronize(h->stream));   // ptr / inc / prior_of go out of scope
   h->uploaded = true;
   return 0;
 }
@@ -854,16 +954,25 @@ static PgoDev pgo_view(d2pgo_handle *h, int cur) {
   return d;
 }
 
-// cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks
-template <class P>
+static PgoPriorDev pgo_prior_view(d2pgo_handle *h, int cur) {
+  PgoPriorDev pr;
+  pr.n_prior = (int)h->gp_pose.size(); pr.pose = h->d_gp_pose.p; pr.prior_of = h->d_prior_of.p; pr.u = h->d_gp_u.p; pr.S = h->d_gp_S.p; pr.lin = h->d_glin[cur].p;
+  return pr;
+}
+
+// cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks.  GRAV: this
+// rank has gravity priors (their cost partials follow the edges', their terms enter g and D after each pose's edges).
+template <class P, bool GRAV>
 static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
   constexpr int D = P::D;
   PgoDev d = pgo_view(h, b);
+  const PgoPriorDev pr = pgo_prior_view(h, b);
   const size_t N = h->ids.size();
-  const int nbe = (d.n_edge + 127) / 128;
+  const int nbe = (d.n_edge + 127) / 128, nbg = GRAV ? (pr.n_prior + 127) / 128 : 0;
   if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, h->stream>>>(d, h->d_cost_part.p, want_jac);
-  k_pgo_sum<<<1, 128, 0, h->stream>>>(h->d_cost_part.p, nbe, h->d_cost.p);
-  if (want_jac) k_pgo_gD<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p);
+  if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, h->stream>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
+  k_pgo_sum<<<1, 128, 0, h->stream>>>(h->d_cost_part.p, nbe + nbg, h->d_cost.p);
+  if (want_jac) k_pgo_gD<P, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
   if (h->comm) {
     if (nccl_allreduce_f64(h->comm, h->d_cost.p, 1, h->stream)) { h->err = "ncclAllReduce(cost) failed"; return 40; }
     if (want_jac && (nccl_allreduce_f64(h->comm, h->d_g[b].p, N * D, h->stream) || nccl_allreduce_f64(h->comm, h->d_D[b].p, N * D * D, h->stream))) { h->err = "ncclAllReduce(g, D) failed"; return 40; }
@@ -875,26 +984,26 @@ static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
 
 constexpr int kCgChunk = 16;   // CG iterations between two looks at the convergence flag (one graph launch on a single rank)
 
-template <class P>
-static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, double tol2) {
+template <class P, bool GRAV>
+static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr, double tol2) {
   const int ge = (d.n_edge + 127) / 128;
   for (int k = 0; k < kCgChunk; k++) {
     const int par = k & 1;
     if (d.n_edge > 0) k_pgo_cg_edge<P><<<ge, 128, 0, h->stream>>>(d, par, tol2);
     if (h->comm) {
-      k_pgo_cg_pose<P, true><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+      k_pgo_cg_pose<P, true, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
       // every rank holds the same r, z, p (the all-reduced products are bitwise identical), so all of them reach the same
       // `done` decision at the same iteration and the collective below is always matched
       if (nccl_allreduce_f64(h->comm, d.Ap, (size_t)d.n_pose * P::D, h->stream)) { h->err = "ncclAllReduce(Ap) failed"; return 40; }
       k_pgo_cg_pAp<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
-    } else k_pgo_cg_pose<P, false><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+    } else k_pgo_cg_pose<P, false, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
     k_pgo_cg_step<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
   }
   return 0;
 }
 
-// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4)
-template <class P>
+// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4) and by 6-DoF graphs with gravity priors (GRAV)
+template <class P, bool GRAV>
 static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
@@ -904,12 +1013,13 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   PCK(cudaEventRecord(h->ev0, h->stream));
   int cur = 0;                    // buffer (poses, lin records, g, D) of the accepted point
   double cost = 0, lambda = h->cfg.lambda0;
-  if ((rc = pgo_linearize<P>(h, cur, 1, &cost))) return rc;
+  if ((rc = pgo_linearize<P, GRAV>(h, cur, 1, &cost))) return rc;
   R.initial_cost = cost;
   const double tol2 = h->cfg.pcg_tolerance * h->cfg.pcg_tolerance;
   if (tol2 != h->graph_tol2) { pgo_drop_graphs(h); h->graph_tol2 = tol2; }
   for (int it = 0; it < h->cfg.max_iterations; it++) {
     PgoDev d = pgo_view(h, cur);
+    const PgoPriorDev pr = pgo_prior_view(h, cur);
     // (J^T J + lambda diag D) dx = -g by block-Jacobi preconditioned CG; J^T J is never formed
     k_pgo_precond<P><<<gp, 128, 0, h->stream>>>(d, h->d_D[cur].p, lambda);
     k_pgo_cg_init<P><<<gp, 128, 0, h->stream>>>(d, h->d_g[cur].p);
@@ -920,20 +1030,20 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
         if (!h->cg_graph[cur]) {
           cudaGraph_t g;
           PCK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-          pgo_cg_chunk<P>(h, d, tol2);
+          pgo_cg_chunk<P, GRAV>(h, d, pr, tol2);
           PCK(cudaStreamEndCapture(h->stream, &g));
           PCK(cudaGraphInstantiate(&h->cg_graph[cur], g, 0));
           cudaGraphDestroy(g);
         }
         PCK(cudaGraphLaunch(h->cg_graph[cur], h->stream));
-      } else if ((rc = pgo_cg_chunk<P>(h, d, tol2))) return rc;
+      } else if ((rc = pgo_cg_chunk<P, GRAV>(h, d, pr, tol2))) return rc;
       PCK(cudaMemcpyAsync(&s, h->d_s.p, sizeof s, cudaMemcpyDeviceToHost, h->stream));
       PCK(cudaStreamSynchronize(h->stream));
       if (s.done) break;   // identical on every rank (see pgo_cg_chunk)
     }
     k_pgo_retract<P><<<gp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
     double cand = 0;
-    if ((rc = pgo_linearize<P>(h, 1 - cur, 1, &cand))) return rc;
+    if ((rc = pgo_linearize<P, GRAV>(h, 1 - cur, 1, &cand))) return rc;
     R.pcg_iterations += s.iters; R.iterations++;
     if (cand < cost && isfinite(cand)) {
       const double rel_dec = (cost - cand) / (cost > 0 ? cost : 1.0);
@@ -960,7 +1070,8 @@ extern "C" {
 int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h || h->ids.empty()) return 1;
   cudaSetDevice(h->cfg.device);
-  return h->dof == 4 ? pgo_solve<PgoEdge4>(h, rep) : pgo_solve<PgoEdge6>(h, rep);
+  if (h->dof == 4) return pgo_solve<PgoEdge4, false>(h, rep);
+  return h->gp_pose.empty() ? pgo_solve<PgoEdge6, false>(h, rep) : pgo_solve<PgoEdge6, true>(h, rep);
 }
 
 int d2pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out) {
@@ -983,10 +1094,69 @@ int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles) {
   const size_t E = h->ea.size(), W = (size_t)h->dof + 2 * (size_t)h->dof * h->dof;   // 78 (6-DoF) or 36 (4-DoF) per edge
   if ((size_t)out_doubles < E * W) { h->err = "debug_edges: buffer too small"; return 2; }
   double cost;
-  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4>(h, 0, 1, &cost) : pgo_linearize<PgoEdge6>(h, 0, 1, &cost))) return rc;
+  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4, false>(h, 0, 1, &cost) : pgo_linearize<PgoEdge6, false>(h, 0, 1, &cost))) return rc;
   std::vector<double> tmp(E * W);
   PCK(cudaMemcpy(tmp.data(), h->d_lin[0].p, E * W * 8, cudaMemcpyDeviceToHost));
   for (size_t e = 0; e < E; e++) for (size_t k = 0; k < W; k++) out[e * W + k] = tmp[k * E + e];   // device layout is field-major
+  return 0;
+}
+
+int d2pgo_add_gravity_priors(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *ego_poses7, const double *sqrt_info9) {
+  if (!h) return 1;
+  if (h->dof != 6) {
+    h->err = "add_gravity_priors: the handle was created with pose_dof = 4; gravity priors act on 6-DoF poses (d2pgo skips them for 4-DoF)";
+    return 5;
+  }
+  if (n < 0 || (n > 0 && (!ids || !ego_poses7 || !sqrt_info9))) { h->err = "add_gravity_priors: negative count or null argument"; return 1; }
+  // validate the whole batch before taking any of it
+  std::vector<char> taken(h->ids.size(), 0);
+  for (int p : h->gp_pose) taken[p] = 1;
+  std::vector<int> pose(n);
+  for (int k = 0; k < n; k++) {
+    const std::string which = "add_gravity_priors: prior " + std::to_string(k) + " (pose id " + std::to_string(ids[k]) + ")";
+    auto it = h->index.find(ids[k]);
+    if (it == h->index.end()) { h->err = which + ": unknown pose id"; return 2; }
+    if (taken[it->second]) { h->err = which + ": the pose already has a gravity prior"; return 2; }
+    taken[it->second] = 1; pose[k] = it->second;
+    bool finite = true;
+    for (int j = 0; j < 7; j++) finite = finite && std::isfinite(ego_poses7[(size_t)k * 7 + j]);
+    for (int j = 0; j < 9; j++) finite = finite && std::isfinite(sqrt_info9[(size_t)k * 9 + j]);
+    if (!finite) { h->err = which + ": non-finite ego pose or sqrt information"; return 2; }
+    const double *q = ego_poses7 + (size_t)k * 7 + 3;
+    if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) { h->err = which + ": zero ego quaternion"; return 2; }
+  }
+  for (int k = 0; k < n; k++) {
+    // u_ego = R(q_ego)^T e3: the third row of the normalised ego attitude's rotation matrix (Swarm::Pose::R, Eigen's polynomial)
+    const double *e = ego_poses7 + (size_t)k * 7 + 3;
+    const double s = 1.0 / std::sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2] + e[3] * e[3]);
+    const double x = e[0] * s, y = e[1] * s, z = e[2] * s, w = e[3] * s;
+    const double tx = 2 * x, ty = 2 * y, tz = 2 * z;
+    h->gp_pose.push_back(pose[k]);
+    h->gp_u.push_back(tz * x - ty * w); h->gp_u.push_back(tz * y + tx * w); h->gp_u.push_back(1 - (tx * x + ty * y));
+    for (int j = 0; j < 9; j++) h->gp_S.push_back(sqrt_info9[(size_t)k * 9 + j]);
+  }
+  if (n > 0) h->uploaded = false;
+  return 0;
+}
+
+int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles) {
+  if (!h) return 1;
+  if (h->dof != 6) { h->err = "debug_gravity_priors: the handle was created with pose_dof = 4 (no gravity priors)"; return 5; }
+  const size_t G = h->gp_pose.size();
+  if ((size_t)out_doubles < G * 21) { h->err = "debug_gravity_priors: buffer too small: " + std::to_string(G * 21) + " doubles needed"; return 2; }
+  if (!G) return 0;
+  cudaSetDevice(h->cfg.device);
+  int rc;
+  if (!h->uploaded && (rc = pgo_upload(h))) return rc;
+  double cost;
+  if ((rc = pgo_linearize<PgoEdge6, true>(h, 0, 1, &cost))) return rc;
+  std::vector<double> tmp(G * 12);
+  PCK(cudaMemcpy(tmp.data(), h->d_glin[0].p, G * 12 * 8, cudaMemcpyDeviceToHost));
+  for (size_t k = 0; k < G; k++) {   // device layout is field-major [12][G]: r(3), J_theta (3x3)
+    double *o = out + k * 21;
+    for (int a = 0; a < 3; a++) o[a] = tmp[a * G + k];
+    for (int a = 0; a < 3; a++) for (int b = 0; b < 6; b++) o[3 + a * 6 + b] = b < 3 ? 0.0 : tmp[(3 + a * 3 + b - 3) * G + k];
+  }
   return 0;
 }
 

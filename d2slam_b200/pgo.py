@@ -10,7 +10,11 @@ on [x y z yaw] poses; poses_to_4d / poses_from_4d convert to and from 7-vector p
 builds 4-DoF inputs from a make_pose_graph graph.
 
 PCM (d2pgo's enable_pcm): `PgoSolver.pcm` rejects inconsistent loop closures before they are added (include/d2pgo.h
-d2pgo_pcm); make_pcm_case builds its inputs from a make_pose_graph graph, with injected gross outliers."""
+d2pgo_pcm); make_pcm_case builds its inputs from a make_pose_graph graph, with injected gross outliers.
+
+Gravity prior (d2pgo's enable_gravity_prior, 6-DoF): `PgoSolver.add_gravity_priors` ties each pose's roll and pitch to the
+gravity direction of its frame's ego (VIO) pose (include/d2pgo.h d2pgo_add_gravity_priors); make_gravity_case builds ego poses
+for a make_pose_graph graph."""
 import ctypes as C
 
 import numpy as np
@@ -39,7 +43,9 @@ class PcmReport(C.Structure):
 
 PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_last_error", "d2pgo_set_poses", "d2pgo_add_edges",
                 "d2pgo_comm_init", "d2pgo_solve", "d2pgo_get_poses", "d2pgo_debug_edges", "d2pgo_set_poses_4d", "d2pgo_add_edges_4d",
-                "d2pgo_get_poses_4d", "d2pgo_default_pcm_config", "d2pgo_pcm", "d2pgo_debug_pcm_smd", "d2pgo_debug_pcm_clique"]
+                "d2pgo_get_poses_4d", "d2pgo_default_pcm_config", "d2pgo_pcm", "d2pgo_debug_pcm_smd", "d2pgo_debug_pcm_clique",
+                "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors"]
+GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
 
@@ -62,6 +68,7 @@ class PgoSolver:
         if rc:
             raise RuntimeError(f"d2pgo_create failed rc={rc}: {_CREATE_ERRORS.get(rc, 'CUDA device required; no CPU fallback')}")
         self.n_edges = 0
+        self.n_priors = 0
 
     def _chk(self, rc, what):
         if rc:
@@ -82,6 +89,7 @@ class PgoSolver:
         f = None if fixed is None else np.ascontiguousarray(fixed, np.uint8)
         self._chk(_lib().d2pgo_set_poses(self.h, C.c_int32(len(ids)), _p(ids), _p(poses), _p(f)), "set_poses")
         self.n_edges = 0
+        self.n_priors = 0
 
     def add_edges(self, id_a, id_b, rel, sqrt_info):
         id_a = np.ascontiguousarray(id_a, np.int64); id_b = np.ascontiguousarray(id_b, np.int64)
@@ -95,6 +103,7 @@ class PgoSolver:
         f = None if fixed is None else np.ascontiguousarray(fixed, np.uint8)
         self._chk(_lib().d2pgo_set_poses_4d(self.h, C.c_int32(len(ids)), _p(ids), _p(poses4), _p(f)), "set_poses_4d")
         self.n_edges = 0
+        self.n_priors = 0
 
     def add_edges_4d(self, id_a, id_b, rel4, sqrt_info16):
         """rel4 = [x y z yaw] measurements (RelPoseFactor4D), sqrt_info16 = 4x4 square-root information per edge."""
@@ -102,6 +111,21 @@ class PgoSolver:
         rel4 = np.ascontiguousarray(rel4, np.float64); si = np.ascontiguousarray(sqrt_info16, np.float64)
         self._chk(_lib().d2pgo_add_edges_4d(self.h, C.c_int32(len(id_a)), _p(id_a), _p(id_b), _p(rel4), _p(si)), "add_edges_4d")
         self.n_edges += len(id_a)
+
+    def add_gravity_priors(self, ids, ego_poses7, sqrt_info=None):
+        """One gravity prior per id (d2pgo's setupGravityPriorFactors): r = S^T (R_i^T e3 - R_ego^T e3) with the frame's ego pose
+        [x y z qx qy qz qw]; sqrt_info = [n, 3, 3] (or [n, 9]) S, None = GRAVITY_SQRT_INFO * I3 for every prior.  6-DoF only."""
+        ids = np.ascontiguousarray(ids, np.int64); ego = np.ascontiguousarray(np.asarray(ego_poses7, np.float64).reshape(-1, 7))
+        S = np.tile(GRAVITY_SQRT_INFO * np.eye(3), (len(ids), 1, 1)) if sqrt_info is None else np.asarray(sqrt_info, np.float64)
+        S = np.ascontiguousarray(S.reshape(-1, 9))
+        self._chk(_lib().d2pgo_add_gravity_priors(self.h, C.c_int32(len(ids)), _p(ids), _p(ego), _p(S)), "add_gravity_priors")
+        self.n_priors += len(ids)
+
+    def debug_gravity_priors(self):
+        """Per local gravity prior at the current poses: r (3) | J (3 x 6 in the tangent [dp, dtheta]), 21 doubles."""
+        out = np.zeros((max(self.n_priors, 1), 21))
+        self._chk(_lib().d2pgo_debug_gravity_priors(self.h, _p(out), C.c_int64(out.size)), "debug_gravity_priors")
+        return out[: self.n_priors]
 
     def comm_init(self, unique_id, rank, nranks):
         uid = (C.c_uint8 * 128)(*unique_id)
@@ -357,6 +381,22 @@ def make_pcm_case(g, outlier_frac=0.05, seed=0):
     return dict(frame_ids=ids, frame_agent=agent, ego=ego, kf_a=np.asarray(g["id_a"][n_odo:]), kf_b=np.asarray(g["id_b"][n_odo:]), rel=rel,
                 rel_bad=rel_bad, sqrt_info=np.asarray(g["sqrt_info"][n_odo:]), outlier=bad, bad_dt=d * np.linalg.norm(rel_bad[bad, :3] - rel[bad, :3], axis=1, keepdims=True),
                 bad_yaw=yaw, n_odo=n_odo)
+
+
+# ------------------------------------------------------------------------------------------------ gravity priors
+def make_gravity_case(g, sigma_tilt=np.deg2rad(0.5), seed=0):
+    """Ego (VIO) poses for gravity priors on a make_pose_graph graph: position and yaw from the agent's odometry chain
+    (_odometry_chain), roll and pitch from the ground truth turned by a random rotation of sigma_tilt per axis -- the gravity
+    direction a VIO front end observes.  The graph's own odometry drifts in roll and pitch, which the priors correct.
+    Returns dict(ids, ego) with ego [N, 7]."""
+    rng = np.random.default_rng(seed)
+    chain, _ = _odometry_chain(g)
+    gt = np.asarray(g["gt"])
+    tilt = _qmul(_qconj(_qyaw(quat_yaw(gt[:, 3:7]))), gt[:, 3:7])                 # ground-truth roll and pitch (zero yaw)
+    tilt = _qmul(tilt, _qexp(rng.normal(0.0, sigma_tilt, (len(gt), 3))))
+    q = _qmul(_qyaw(quat_yaw(chain[:, 3:7])), tilt)
+    ego = np.concatenate([chain[:, :3], q / np.linalg.norm(q, axis=1, keepdims=True)], axis=1)
+    return dict(ids=np.asarray(g["ids"]), ego=ego)
 
 
 # ------------------------------------------------------------------------------------------------ g2o files

@@ -16,6 +16,8 @@
  *   d2pgo_get_poses_4d            <- syncFromState: the optimised [x y z yaw] blocks
  *   d2pgo_pcm                     <- SwarmLocalOutlierRejection::OutlierRejectionLoopEdges (enable_pcm), the loops it keeps
  *                                    being those setupLoopFactors receives (d2pgo/src/d2pgo.cpp:177-186, :276-282)
+ *   d2pgo_add_gravity_priors      <- setupGravityPriorFactors (enable_gravity_prior): GravityPriorPerturbAD per frame
+ *                                    (d2pgo/src/d2pgo.cpp:530-559, GravityPrior.hpp:8-46)
  *
  * Scope note: the reference solves the multi-agent graph with ARock (asynchronous dual updates, ARock.cpp:140-328) around
  * per-agent ceres problems; BASELINE's config asks for a *distributed Gauss-Newton* on the 8 GPUs of one box.  Here every
@@ -81,6 +83,26 @@ int d2pgo_get_poses_4d(d2pgo_handle *h, int32_t n, const int64_t *ids, double *p
 /* parity hook: residual and the two tangent Jacobians of every local edge at the current poses, row-major:
  * 6-DoF out[n_edges][78] = r(6) | J_a (6x6) | J_b (6x6);  4-DoF out[n_edges][36] = r(4) | J_a (4x4) | J_b (4x4) */
 int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles);
+
+/* ---- gravity prior (enable_gravity_prior, 6-DoF handles)
+ *   d2pgo_add_gravity_priors <- D2PGO::setupGravityPriorFactors (d2pgo/src/d2pgo.cpp:530-559, called by solve_single /
+ *                               solve_multi at :216-218, :304-306): one GravityPriorPerturbAD per frame
+ *                               (d2common/include/d2common/solver/GravityPrior.hpp:8-46)
+ * Per prior: pose i, its frame's ego (VIO) pose q_ego and a 3x3 S (row-major; d2pgo passes gravity_sqrt_info I3, 10 in the
+ * shipped configs).  u = R(q_i)^T e3 (the third row of R_i), u_ego = R(q_ego)^T e3, and
+ *     r = S^T (u - u_ego)      (the reference's row R_i.row(2) - R_ego.row(2) with applyOnTheRight(S))
+ * with the tangent Jacobian dr/d dtheta = S^T [u]x, dr/d dp = 0: it ties roll and pitch to the observed gravity direction and
+ * leaves yaw free.  Evaluated at the exact pose; the reference's perturbation chart q0 (x) quatfromRotationVector(theta) agrees
+ * at theta = 0 and wherever |theta| >= 1e-2 (inside, its unnormalised [1, theta/2] is off by O(|theta|^2)).  A pose may carry
+ * one prior; a fixed pose's prior only adds to the cost.  d2pgo_set_poses removes every prior.  With a communicator attached,
+ * each rank passes ITS shard of the priors (each prior on exactly one rank).  Costs in d2pgo_report include the priors.
+ * Returns 5 on a 4-DoF handle (d2pgo skips the prior for 4-DoF, d2pgo.cpp:531-533); 2 on an unknown id, a second prior on a
+ * pose, a non-finite value or a zero ego quaternion (nothing of the call is kept); 1 on a null argument or n < 0.
+ * d2pgo_last_error says why.  n = 0 changes nothing. */
+int d2pgo_add_gravity_priors(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *ego_poses7, const double *sqrt_info9);
+/* parity hook: per local prior at the current poses, in the order added, out[n_priors][21] = r(3) | J (3x6 row-major in the
+ * tangent [dp, dtheta]; the position columns are zero) */
+int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles);
 
 /* ---- loop-closure outlier rejection: pairwise-consistency maximisation (PCM)
  *   d2pgo_pcm  <- SwarmLocalOutlierRejection::OutlierRejectionLoopEdges with redundant = true, incremental_pcm = false,

@@ -1,6 +1,7 @@
 """torchrun worker: the pose graph's edges sharded over the ranks (e % world), J^T J p all-reduced over NCCL inside
 libd2ba (include/d2pgo.h) -- every rank must end on the single-rank solution (rank 0 also solves the whole graph alone).
---dof 4 runs the same check on the graph's 4-DoF version (pgo.pose_graph_to_4d, RelPoseFactor4D)."""
+--dof 4 runs the same check on the graph's 4-DoF version (pgo.pose_graph_to_4d, RelPoseFactor4D).  --gravity adds a gravity
+prior on every pose (pgo.make_gravity_case, full S), the priors split over the ranks like the edges (k % world)."""
 import argparse
 import os
 import sys
@@ -23,17 +24,27 @@ def pose_errors(x, y, dof):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--dof", type=int, choices=(6, 4), default=6)
-    dof = ap.parse_args().dof
+    ap.add_argument("--gravity", action="store_true", help="6-DoF with a gravity prior on every pose")
+    args = ap.parse_args()
+    dof = args.dof
+    if args.gravity and dof != 6:
+        ap.error("--gravity needs --dof 6")
     rank = int(os.environ["RANK"]); world = int(os.environ["WORLD_SIZE"]); lr = int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(lr)
     dist.init_process_group("nccl", device_id=torch.device("cuda", lr))
     g = pgo.make_pose_graph(seed=11, n_agents=4, poses_per_agent=80, loops=400)
     if dof == 4:
         g = pgo.pose_graph_to_4d(g, seed=11)
+    if args.gravity:
+        ego = pgo.make_gravity_case(g, seed=11)["ego"]
+        gS = pgo.GRAVITY_SQRT_INFO * np.eye(3) + 2.0 * np.random.default_rng(11).normal(size=(len(g["ids"]), 3, 3))
     kw = dict(device=lr, max_iterations=25, pcg_max_iterations=800, pcg_tolerance=1e-10, lambda0=0.0, function_tolerance=1e-13, pose_dof=dof)
 
-    def load(s, sel):
-        if dof == 4:
+    def load(s, sel, gsel=None):
+        if args.gravity:
+            s.set_poses(g["ids"], g["init"], g["fixed"]); s.add_edges(g["id_a"][sel], g["id_b"][sel], g["rel"][sel], g["sqrt_info"][sel])
+            s.add_gravity_priors(g["ids"][gsel], ego[gsel], gS[gsel])
+        elif dof == 4:
             s.set_poses_4d(g["ids"], g["init"], g["fixed"]); s.add_edges_4d(g["id_a"][sel], g["id_b"][sel], g["rel"][sel], g["sqrt_info"][sel])
         else:
             s.set_poses(g["ids"], g["init"], g["fixed"]); s.add_edges(g["id_a"][sel], g["id_b"][sel], g["rel"][sel], g["sqrt_info"][sel])
@@ -42,7 +53,7 @@ def main():
         return s.get_poses_4d(g["ids"]) if dof == 4 else s.get_poses(g["ids"])
     sel = np.arange(rank, len(g["id_a"]), world)
     s = pgo.PgoSolver(**kw)
-    load(s, sel)
+    load(s, sel, np.arange(rank, len(g["ids"]), world))
     uid = torch.zeros(128, dtype=torch.uint8, device="cuda")
     if rank == 0:
         uid.copy_(torch.tensor(list(comm_unique_id()), dtype=torch.uint8))
@@ -56,10 +67,10 @@ def main():
     ok = same and rep.final_cost < rep.initial_cost
     if rank == 0:
         s1 = pgo.PgoSolver(**kw)
-        load(s1, np.arange(len(g["id_a"])))
+        load(s1, np.arange(len(g["id_a"])), np.arange(len(g["ids"])))
         r1 = s1.solve()
         dp, dr = pose_errors(x, poses(s1), dof)
-        print(f"pgo multi ({dof}-DoF): cost {rep.final_cost:.9e} vs single {r1.final_cost:.9e}; pose diff {dp:.3e} m {dr:.3e} rad; lm its {rep.iterations}/{r1.iterations}; ranks identical {same}")
+        print(f"pgo multi ({dof}-DoF{' + gravity priors' if args.gravity else ''}): cost {rep.final_cost:.9e} vs single {r1.final_cost:.9e}; pose diff {dp:.3e} m {dr:.3e} rad; lm its {rep.iterations}/{r1.iterations}; ranks identical {same}")
         ok = ok and abs(rep.final_cost - r1.final_cost) <= 1e-9 * r1.final_cost and dp <= 1e-6 and dr <= 1e-6
     flag = torch.tensor([1 if ok else 0], device="cuda"); dist.all_reduce(flag, op=dist.ReduceOp.MIN)
     if rank == 0:
