@@ -30,8 +30,6 @@ void launch_imu_prep(const Dev &d, const double *packed, double *full, int n_imu
 void launch_prior_prep(const Dev &d, cudaStream_t s);
 void launch_misc_lin(const Dev &d, int eval_cur, int max_prior_m, cudaStream_t s);
 void launch_imu_lin(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s);
-void launch_imu_raw(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s);   // the two halves of launch_imu_lin
-void launch_imu_acc(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s);
 int configure_kernels(int max_rows, int max_nc, int max_prior_m);
 int configure_gather(int max_ldw);
 void launch_proj_lin(const Dev &d, int variant, int eval_cur, int job_begin, int job_count, cudaStream_t s);
@@ -250,7 +248,7 @@ struct d2ba_handle {
   std::vector<HostWin> win;
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaStream_t side = nullptr;                 // second lane of the iteration: IMU chain beside the reprojection kernels, sb elimination beside the landmark gather
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_misc = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool two_lanes = true;                       // D2BA_ONE_LANE=1: everything on `stream` (A/B)
   cudaEvent_t ev_copy = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -265,7 +263,7 @@ struct d2ba_handle {
   DBuf<double> d_x6[2], d_R6[2], d_xsb[2], d_xlm[2], d_xtd[2];
   DBuf<int> d_col6, d_colsb, d_tile_grp, d_obs_lm, d_lm_ptr, d_obs_slot, d_slot6, d_lm_win, d_blk_win, d_sb_win, d_tile_win;
   DBuf<Group> d_grp; DBuf<Job> d_job; DBuf<ImuDesc> d_imu; DBuf<PriorBlk> d_prior_blk;
-  DBuf<double> d_obs, d_rec[2], d_imu_c, d_imu_pk, d_imu_U, d_imu_raw, d_prior_J, d_prior_e0, d_prior_A, d_z6, d_tilde6, d_lm_ref, d_sb_ref, d_td_ref,
+  DBuf<double> d_obs, d_rec[2], d_imu_c, d_imu_pk, d_imu_U, d_prior_J, d_prior_e0, d_prior_A, d_z6, d_tilde6, d_lm_ref, d_sb_ref, d_td_ref,
       d_cons, d_H[2], d_gc[2], d_Wt, d_dinv, d_hl, d_gl, d_S, d_gred, d_D2c, d_gn_c, d_gn_l, d_step_c, d_step_l, d_wu, d_uc, d_D2l, d_dbg;
   DBuf<SchurTileH> d_schur; DBuf<int> d_schur_chunks; DBuf<Leaf> d_leaf; DBuf<HSeg> d_hseg; DBuf<unsigned long long> d_lm_mask; DBuf<double> d_leafL; DBuf<int> d_leaf_lm;
   int n_schur0 = 0, n_leaf_total = 0, max_hub = 0; size_t leaf_smem = 0, cfg_leaf_smem = 0, leafb_smem = 0, cfg_leafb_smem = 0;
@@ -387,7 +385,7 @@ int d2ba_create(const d2ba_config *cfg, d2ba_handle **out) {
   cudaEventCreateWithFlags(&h->ev_it[0], cudaEventDisableTiming); cudaEventCreateWithFlags(&h->ev_it[1], cudaEventDisableTiming);
   cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking); cudaEventCreateWithFlags(&h->ev_copy, cudaEventDisableTiming);
   cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking);
-  cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming); cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming); cudaEventCreateWithFlags(&h->ev_misc, cudaEventDisableTiming);
+  cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming); cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming);
   { const char *e = getenv("D2BA_ONE_LANE"); h->two_lanes = !(e && e[0] == '1'); }
   memset(&h->dev, 0, sizeof(h->dev));
   *out = h;
@@ -407,7 +405,7 @@ int d2ba_destroy(d2ba_handle *h) {
   for (int b = 0; b < 2; b++) { h->d_x6[b].release(); h->d_R6[b].release(); h->d_xsb[b].release(); h->d_xlm[b].release(); h->d_xtd[b].release(); h->d_rec[b].release(); h->d_H[b].release(); h->d_gc[b].release(); }
   h->d_col6.release(); h->d_colsb.release(); h->d_tile_grp.release(); h->d_obs_lm.release(); h->d_lm_ptr.release(); h->d_obs_slot.release();
   h->d_slot6.release(); h->d_lm_win.release(); h->d_blk_win.release(); h->d_sb_win.release(); h->d_tile_win.release();
-  h->d_grp.release(); h->d_job.release(); h->d_imu.release(); h->d_prior_blk.release(); h->d_obs.release(); h->d_imu_c.release(); h->d_imu_pk.release(); h->d_imu_U.release(); h->d_imu_raw.release();
+  h->d_grp.release(); h->d_job.release(); h->d_imu.release(); h->d_prior_blk.release(); h->d_obs.release(); h->d_imu_c.release(); h->d_imu_pk.release(); h->d_imu_U.release();
   h->d_prior_J.release(); h->d_prior_e0.release(); h->d_prior_A.release(); h->d_z6.release(); h->d_tilde6.release(); h->d_lm_ref.release(); h->d_sb_ref.release();
   h->d_td_ref.release(); h->d_cons.release(); h->d_Wt.release(); h->d_dinv.release(); h->d_hl.release(); h->d_gl.release(); h->d_S.release(); h->d_gred.release();
   h->d_D2c.release(); h->d_gn_c.release(); h->d_gn_l.release(); h->d_step_c.release(); h->d_step_l.release(); h->d_wu.release(); h->d_uc.release(); h->d_D2l.release(); h->d_dbg.release(); h->d_schur.release(); h->d_schur_chunks.release(); h->d_leaf.release(); h->d_hseg.release(); h->d_lm_mask.release(); h->d_leafL.release(); h->d_leaf_lm.release();
@@ -415,7 +413,7 @@ int d2ba_destroy(d2ba_handle *h) {
   cudaStreamSynchronize(h->copy_stream);
   for (auto &w : h->win) { w.rawj.release(); w.anch.release(); w.d_rawj.release(); w.d_anch.release(); w.rawjm.release(); w.anchm.release(); w.d_rawjm.release(); w.d_anchm.release(); }
   cudaStreamDestroy(h->copy_stream); cudaEventDestroy(h->ev_copy);
-  cudaStreamSynchronize(h->side); cudaStreamDestroy(h->side); cudaEventDestroy(h->ev_fork); cudaEventDestroy(h->ev_join); cudaEventDestroy(h->ev_misc);
+  cudaStreamSynchronize(h->side); cudaStreamDestroy(h->side); cudaEventDestroy(h->ev_fork); cudaEventDestroy(h->ev_join);
   d2ba_release_staging(h);
   cudaEventDestroy(h->ev_it[0]); cudaEventDestroy(h->ev_it[1]);
   cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1); cudaEventDestroy(h->evf0); cudaEventDestroy(h->evf1); cudaEventDestroy(h->evf2);
@@ -1376,7 +1374,6 @@ int d2ba_finalize(d2ba_handle *h) {
   launch_build_tiles(h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, off_tile, h->stream);
   CK(h->d_imu_U.alloc((size_t)off_imu * 225));
   if ((rc = alloc_zero(h, h->d_imu_c, (size_t)off_imu * kImuStride))) return rc;   // expanded from the packed upload by k_imu_unpack (launch_imu_prep)
-  if ((rc = alloc_zero(h, h->d_imu_raw, (size_t)off_imu * 465))) return rc;   // structural zeros of the raw Jacobians are never rewritten
   CK(h->d_prior_A.alloc((size_t)off_pJ));
   CK(h->d_z6.alloc((size_t)off6 * 8)); CK(h->d_tilde6.alloc((size_t)off6 * 6)); CK(h->d_lm_ref.alloc(offlm)); CK(h->d_sb_ref.alloc((size_t)offsb * 9));
   CK(h->d_td_ref.alloc(nw));
@@ -1396,7 +1393,7 @@ int d2ba_finalize(d2ba_handle *h) {
   D.col6 = h->d_col6.p; D.colsb = h->d_colsb.p; D.grp = h->d_grp.p; D.job = h->d_job.p; D.n_job = n_jobs;
   D.lm_mask = h->d_lm_mask.p; D.hseg = h->d_hseg.p; D.leaf = h->d_leaf.p; D.n_leaf_total = h->n_leaf_total; { int np_ = 0; for (int q = 0; q < nw; q++) if (plan[q].d.n_leaf == 0) np_++; D.n_plain_win = np_; } D.leafL = h->d_leafL.p; D.schur_chunks = h->d_schur_chunks.p; D.leaf_lm = h->d_leaf_lm.p;
   D.tile_grp = h->d_tile_grp.p; D.obs = h->d_obs.p; D.obs_lm = h->d_obs_lm.p; D.lm_ptr = h->d_lm_ptr.p; D.obs_slot = h->d_obs_slot.p;
-  D.imu = h->d_imu.p; D.imu_c = h->d_imu_c.p; D.imu_U = h->d_imu_U.p; D.imu_raw = h->d_imu_raw.p; D.prior_blk = h->d_prior_blk.p; D.prior_J = h->d_prior_J.p;
+  D.imu = h->d_imu.p; D.imu_c = h->d_imu_c.p; D.imu_U = h->d_imu_U.p; D.prior_blk = h->d_prior_blk.p; D.prior_J = h->d_prior_J.p;
   D.prior_e0 = h->d_prior_e0.p; D.prior_A = h->d_prior_A.p; D.slot6 = h->d_slot6.p; D.z6 = h->d_z6.p; D.tilde6 = h->d_tilde6.p;
   D.lm_ref = h->d_lm_ref.p; D.sb_ref = h->d_sb_ref.p; D.td_ref = h->d_td_ref.p; D.cons_buf = h->d_cons.p; D.n_slots = h->n_slots;
   D.Wt = h->d_Wt.p; D.dinv = h->d_dinv.p; D.hl = h->d_hl.p; D.gl = h->d_gl.p; D.S = h->d_S.p; D.gred = h->d_gred.p; D.D2c = h->d_D2c.p;
@@ -1501,18 +1498,13 @@ static int upload_state(d2ba_handle *h) {
 }
 
 static void enqueue_linearize(d2ba_handle *h, int eval_cur) {
-  // two lanes: the IMU chain (latency bound, ~10 factors per window) runs beside k_misc_lin / the reprojection kernels
-  // (bandwidth bound).  Order kept: k_misc_lin zero-fills the written runs of Hcc and stores cand_cost_misc before
-  // k_imu_lin and k_proj_lin add to them.
+  // k_misc_lin zero-fills the written runs of Hcc and stores cand_cost_misc before k_imu_lin and k_proj_lin add to them.
+  // Two lanes after it: the IMU factors (one warp each) run beside the reprojection kernels and fill their tails.
+  launch_misc_lin(h->dev, eval_cur, h->max_prior_m, h->stream);
   const bool fork = h->two_lanes && h->n_imu_total > 0;
   if (fork) {
     cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0);
-    launch_imu_raw(h->dev, eval_cur, h->n_imu_total, h->side);
-  }
-  launch_misc_lin(h->dev, eval_cur, h->max_prior_m, h->stream);
-  if (fork) {
-    cudaEventRecord(h->ev_misc, h->stream); cudaStreamWaitEvent(h->side, h->ev_misc, 0);
-    launch_imu_acc(h->dev, eval_cur, h->n_imu_total, h->side);
+    launch_imu_lin(h->dev, eval_cur, h->n_imu_total, h->side);
     cudaEventRecord(h->ev_join, h->side);
   } else launch_imu_lin(h->dev, eval_cur, h->n_imu_total, h->stream);
   for (int v = 0; v < 6; v++) launch_proj_lin(h->dev, v, eval_cur, h->job_begin[v], h->job_count[v], h->stream);

@@ -3,7 +3,8 @@
 //   k_state_prep      rotation matrices of every six-dof block
 //   k_imu_prep        IMU sqrt-information U = chol(cov^-1)^T            (imu_factor.h:29)
 //   k_prior_prep      A' = J_lin^T J_lin of the marginalisation prior
-//   k_misc_lin        IMU + prior + ADMM terms -> Hcc, gc, cost          (one CTA / window)
+//   k_misc_lin        zero Hcc, gc; prior + ADMM terms -> Hcc, gc, cost  (one CTA / window)
+//   k_imu_lin         IMU factors -> Hcc, gc, cost                       (one warp / factor)
 //   k_proj_lin<..>    fused reprojection residual + Jacobian + Huber + DMMA J^T J accumulation
 //   k_lm_gather       per-landmark reduction -> scaled coupling rows Wt, h, g
 //   k_schur           S = Hcc + mu D^2 - Wt^T Wt  (fp64 tensor-core SYRK) + bordered rhs row
@@ -105,45 +106,71 @@ __global__ void k_prior_prep(Dev d) {
 // IMU raw residual (15) and raw Jacobian (15 x 30: pose_i 6 | sb_i 9 | pose_j 6 | sb_j 9) before the
 // sqrt-information is applied.  Same terms as IMUFactor::Evaluate (d2vins/src/factors/imu_factor.h:41-213)
 // and IntegrationBase::evaluate (d2common/include/d2common/integration_base.h:201-227).
-__device__ void imu_raw(const double *c, const double *pi, const double *si, const double *pj, const double *sj,
-                        double g, double *res, double *J /*15x30 zeroed*/) {
+// Split so that a warp evaluates one factor lane-parallel: every lane runs the shared prefix (imu_prefix), then lane k
+// forms the k-th of the kImuBlocks non-zero 3x3 blocks (imu_block).
+//
+// The constants a factor reads (kImuConst doubles): c[0..16] = sum_dt, dp, dq, dv, ba, bg, then rows 0..8 (dp, dq, dv)
+// x columns 9..14 (ba, bg) of the pre-integration Jacobian, 6 per row.  imu_const_src maps them into the kImuStride record.
+constexpr int kImuConst = 17 + 54;
+constexpr int kImuBlocks = 18;
+D2BA_DEV int imu_const_src(int t) { return t < 17 ? t : 17 + ((t - 17) / 6) * 15 + 9 + (t - 17) % 6; }
+
+struct ImuLin {   // what the Jacobian blocks are formed from
+  double Ri[9], ra1[3], ra2[3], dt;
+  Q4 Qi, Qj, Dq, cq;
+};
+
+// prefix of the evaluation; writes the raw residual to res when res != nullptr
+D2BA_DEV void imu_prefix(const double *c, const double *pi, const double *si, const double *pj, const double *sj, double g,
+                         ImuLin &L, double *res) {
   const double dt = c[0];
-  const double *dp = c + 1, *dq = c + 4, *dv = c + 8, *ba0 = c + 11, *bg0 = c + 14, *Jp = c + 17;
-  Q4 Qi = qload(pi + 3), Qj = qload(pj + 3), Dq = qload(dq);
-  double Ri[9];
-  q2R(Qi, Ri);
-  auto jb = [&](int r, int col, double *o) {
+  const double *dp = c + 1, *dq = c + 4, *dv = c + 8, *ba0 = c + 11, *bg0 = c + 14, *B = c + 17;
+  auto jb = [&](int r, int q, double *o) {   // 3x3 block at rows r.., bias columns q.. (0 = ba, 3 = bg)
 #pragma unroll
     for (int a = 0; a < 3; a++)
 #pragma unroll
-      for (int b = 0; b < 3; b++) o[a * 3 + b] = Jp[(r + a) * 15 + col + b];
+      for (int b = 0; b < 3; b++) o[a * 3 + b] = B[(r + a) * 6 + q + b];
   };
+  L.dt = dt;
+  L.Qi = qload(pi + 3); L.Qj = qload(pj + 3); L.Dq = qload(dq);
+  q2R(L.Qi, L.Ri);
   double dp_dba[9], dp_dbg[9], dq_dbg[9], dv_dba[9], dv_dbg[9];
-  jb(0, 9, dp_dba); jb(0, 12, dp_dbg); jb(3, 12, dq_dbg); jb(6, 9, dv_dba); jb(6, 12, dv_dbg);
+  jb(0, 0, dp_dba); jb(0, 3, dp_dbg); jb(3, 3, dq_dbg); jb(6, 0, dv_dba); jb(6, 3, dv_dbg);
   double dba[3] = {si[3] - ba0[0], si[4] - ba0[1], si[5] - ba0[2]};
   double dbg[3] = {si[6] - bg0[0], si[7] - bg0[1], si[8] - bg0[2]};
   double th[3], t1[3], t2[3];
   mv3(dq_dbg, dbg, th);
-  Q4 cq = qmul(Dq, Q4{0.5 * th[0], 0.5 * th[1], 0.5 * th[2], 1.0});
+  L.cq = qmul(L.Dq, Q4{0.5 * th[0], 0.5 * th[1], 0.5 * th[2], 1.0});
+  double G[3] = {0, 0, g};
+  double a1[3], a2[3];
+  for (int k = 0; k < 3; k++) { a1[k] = 0.5 * G[k] * dt * dt + pj[k] - pi[k] - si[k] * dt; a2[k] = G[k] * dt + sj[k] - si[k]; }
+  mtv3(L.Ri, a1, L.ra1); mtv3(L.Ri, a2, L.ra2);
+  if (!res) return;
   double cv[3], cp[3];
   mv3(dv_dba, dba, t1); mv3(dv_dbg, dbg, t2);
   for (int k = 0; k < 3; k++) cv[k] = dv[k] + t1[k] + t2[k];
   mv3(dp_dba, dba, t1); mv3(dp_dbg, dbg, t2);
   for (int k = 0; k < 3; k++) cp[k] = dp[k] + t1[k] + t2[k];
-  double G[3] = {0, 0, g};
-  double a1[3], a2[3], ra1[3], ra2[3];
-  for (int k = 0; k < 3; k++) { a1[k] = 0.5 * G[k] * dt * dt + pj[k] - pi[k] - si[k] * dt; a2[k] = G[k] * dt + sj[k] - si[k]; }
-  mtv3(Ri, a1, ra1); mtv3(Ri, a2, ra2);
-  Q4 qij = qmul(qinv(Qi), Qj);
-  Q4 er = qmul(qinv(cq), qij);
-  for (int k = 0; k < 3; k++) { res[k] = ra1[k] - cp[k]; res[6 + k] = ra2[k] - cv[k]; res[9 + k] = sj[3 + k] - si[3 + k]; res[12 + k] = sj[6 + k] - si[6 + k]; }
+  Q4 qij = qmul(qinv(L.Qi), L.Qj);
+  Q4 er = qmul(qinv(L.cq), qij);
+  for (int k = 0; k < 3; k++) { res[k] = L.ra1[k] - cp[k]; res[6 + k] = L.ra2[k] - cv[k]; res[9 + k] = sj[3 + k] - si[3 + k]; res[12 + k] = sj[6 + k] - si[6 + k]; }
   res[3] = 2 * er.x; res[4] = 2 * er.y; res[5] = 2 * er.z;
-  if (!J) return;
+}
+
+// the k-th non-zero 3x3 block of the raw Jacobian, written into J (15 x 30 row-major; the other entries are left alone)
+D2BA_DEV void imu_block(int k, const ImuLin &L, const double *c, double *J) {
+  const double *B = c + 17;
   auto put = [&](int r, int col, const double *m, double s) {
 #pragma unroll
     for (int a = 0; a < 3; a++)
 #pragma unroll
       for (int b = 0; b < 3; b++) J[(r + a) * 30 + col + b] = s * m[a * 3 + b];
+  };
+  auto putc = [&](int r, int col, int q, double s) {   // a bias block of the pre-integration Jacobian (rows r.., columns q..)
+#pragma unroll
+    for (int a = 0; a < 3; a++)
+#pragma unroll
+      for (int b = 0; b < 3; b++) J[(r + a) * 30 + col + b] = s * B[(r + a) * 6 + q + b];
   };
   auto skewm = [&](const double *v, double *o) { o[0] = 0; o[1] = -v[2]; o[2] = v[1]; o[3] = v[2]; o[4] = 0; o[5] = -v[0]; o[6] = -v[1]; o[7] = v[0]; o[8] = 0; };
   // bottom-right 3x3 of Qleft(a) (and of Qleft(a) Qright(b)), both after positify (utils.hpp:85-104)
@@ -151,41 +178,53 @@ __device__ void imu_raw(const double *c, const double *pi, const double *si, con
     a = qpos(a);
     o[0] = a.w; o[1] = -a.z; o[2] = a.y; o[3] = a.z; o[4] = a.w; o[5] = -a.x; o[6] = -a.y; o[7] = a.x; o[8] = a.w;
   };
-  double RiT[9] = {Ri[0], Ri[3], Ri[6], Ri[1], Ri[4], Ri[7], Ri[2], Ri[5], Ri[8]};
-  double S[9], M[9], I3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-  // pose_i (cols 0..5)
-  put(0, 0, RiT, -1.0);
-  skewm(ra1, S); put(0, 3, S, 1.0);
-  {
-    Q4 a = qpos(qmul(qinv(Qj), Qi)), b = qpos(cq);
-    double L3[9], R3[9];
-    qleft3(a, L3);
-    R3[0] = b.w; R3[1] = b.z; R3[2] = -b.y; R3[3] = -b.z; R3[4] = b.w; R3[5] = b.x; R3[6] = b.y; R3[7] = -b.x; R3[8] = b.w;
-    mm3(L3, R3, M);
-    double av[3] = {a.x, a.y, a.z}, bv[3] = {b.x, b.y, b.z};
-    for (int r = 0; r < 3; r++) for (int cc = 0; cc < 3; cc++) M[r * 3 + cc] -= av[r] * bv[cc];
-    put(3, 3, M, -1.0);
+  const double *Ri = L.Ri;
+  const double RiT[9] = {Ri[0], Ri[3], Ri[6], Ri[1], Ri[4], Ri[7], Ri[2], Ri[5], Ri[8]};
+  const double I3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  double S[9], M[9];
+  switch (k) {
+    // pose_i (cols 0..5)
+    case 0: put(0, 0, RiT, -1.0); break;
+    case 1: skewm(L.ra1, S); put(0, 3, S, 1.0); break;
+    case 2: {
+      Q4 a = qpos(qmul(qinv(L.Qj), L.Qi)), b = qpos(L.cq);
+      double L3[9], R3[9];
+      qleft3(a, L3);
+      R3[0] = b.w; R3[1] = b.z; R3[2] = -b.y; R3[3] = -b.z; R3[4] = b.w; R3[5] = b.x; R3[6] = b.y; R3[7] = -b.x; R3[8] = b.w;
+      mm3(L3, R3, M);
+      double av[3] = {a.x, a.y, a.z}, bv[3] = {b.x, b.y, b.z};
+      for (int r = 0; r < 3; r++) for (int cc = 0; cc < 3; cc++) M[r * 3 + cc] -= av[r] * bv[cc];
+      put(3, 3, M, -1.0);
+    } break;
+    case 3: skewm(L.ra2, S); put(6, 3, S, 1.0); break;
+    // sb_i (cols 6..14): V 6, BA 9, BG 12
+    case 4: put(0, 6, RiT, -L.dt); break;
+    case 5: putc(0, 9, 0, -1.0); break;    // dp_dba
+    case 6: putc(0, 12, 3, -1.0); break;   // dp_dbg
+    case 7: {
+      double L3[9], dq_dbg[9];
+      qleft3(qmul(qmul(qinv(L.Qj), L.Qi), L.Dq), L3);  // uncorrected delta_q (imu_factor.h:159)
+      for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) dq_dbg[a * 3 + b] = B[(3 + a) * 6 + 3 + b];
+      mm3(L3, dq_dbg, M);
+      put(3, 12, M, -1.0);
+    } break;
+    case 8: put(6, 6, RiT, -1.0); break;
+    case 9: putc(6, 9, 0, -1.0); break;    // dv_dba
+    case 10: putc(6, 12, 3, -1.0); break;  // dv_dbg
+    case 11: put(9, 9, I3, -1.0); break;
+    case 12: put(12, 12, I3, -1.0); break;
+    // pose_j (cols 15..20)
+    case 13: put(0, 15, RiT, 1.0); break;
+    case 14: {
+      double L3[9];
+      qleft3(qmul(qmul(qinv(L.cq), qinv(L.Qi)), L.Qj), L3);
+      put(3, 18, L3, 1.0);
+    } break;
+    // sb_j (cols 21..29)
+    case 15: put(6, 21, RiT, 1.0); break;
+    case 16: put(9, 24, I3, 1.0); break;
+    default: put(12, 27, I3, 1.0); break;
   }
-  skewm(ra2, S); put(6, 3, S, 1.0);
-  // sb_i (cols 6..14): V 6, BA 9, BG 12
-  put(0, 6, RiT, -dt); put(0, 9, dp_dba, -1.0); put(0, 12, dp_dbg, -1.0);
-  {
-    double L3[9];
-    qleft3(qmul(qmul(qinv(Qj), Qi), Dq), L3);  // uncorrected delta_q (imu_factor.h:159)
-    mm3(L3, dq_dbg, M);
-    put(3, 12, M, -1.0);
-  }
-  put(6, 6, RiT, -1.0); put(6, 9, dv_dba, -1.0); put(6, 12, dv_dbg, -1.0);
-  put(9, 9, I3, -1.0); put(12, 12, I3, -1.0);
-  // pose_j (cols 15..20)
-  put(0, 15, RiT, 1.0);
-  {
-    double L3[9];
-    qleft3(qmul(qmul(qinv(cq), qinv(Qi)), Qj), L3);
-    put(3, 18, L3, 1.0);
-  }
-  // sb_j (cols 21..29)
-  put(6, 21, RiT, 1.0); put(9, 24, I3, 1.0); put(12, 27, I3, 1.0);
 }
 
 D2BA_DEV void prior_dx_pose(const double *x, const double *x0, double *dx) {  // prior_factor.cpp:57-68
@@ -211,11 +250,10 @@ D2BA_DEV void cons_eval(const double *x, const double *z, const double *tl, doub
   L3[0] = p.w; L3[1] = -p.z; L3[2] = p.y; L3[3] = p.z; L3[4] = p.w; L3[5] = -p.x; L3[6] = -p.y; L3[7] = p.x; L3[8] = p.w;
 }
 
-// One CTA per window: zero Hcc/gc of the evaluated buffer, then add IMU, prior and ADMM terms.
-// Runs before k_proj_lin (which adds the reprojection blocks with atomics).
-constexpr int kMiscThreads = 256;
-constexpr int kMiscImuChunk = 12;
-__global__ void __launch_bounds__(kMiscThreads, 4) k_misc_lin(Dev d, int eval_cur) {
+// One CTA per window: zero Hcc/gc of the evaluated buffer, then add the prior and ADMM terms.
+// Runs before k_imu_lin and k_proj_lin (which add the IMU and reprojection blocks with atomics).
+constexpr int kMiscThreads = 128;
+__global__ void __launch_bounds__(kMiscThreads, 5) k_misc_lin(Dev d, int eval_cur) {
   const int wi = blockIdx.x;
   const WinDesc &w = d.win[wi];
   Ctl *ctl = d.ctl + wi;
@@ -233,27 +271,25 @@ __global__ void __launch_bounds__(kMiscThreads, 4) k_misc_lin(Dev d, int eval_cu
   const double *xlm = d.xlm[buf] + w.offlm;
   const int *col6 = d.col6 + w.off6;
   const int *colsb = d.colsb + w.offsb;
-#ifdef D2BA_MISC_TIMING
-  long long mk[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}; long long mq = clock64();
-#define MLAP(k) do { __syncthreads(); long long t_ = clock64(); mk[k] += t_ - mq; mq = t_; } while (0)
-#else
-#define MLAP(k) do { } while (0)
-#endif
-  // ---- zero + IMU factors.  The raw residual / Jacobian of a factor is one long dependent chain (one lane per
-  //      factor, all in warp 0); the other warps zero H / g and stage the sqrt-information meanwhile.  U J and
-  //      [J r]^T [J r] then run on the fp64 tensor cores (m8n8k4), 8x8 output tiles spread over the warps.
   double cost = 0.0;
-  // zero only the runs of Hcc some factor writes (lower triangle; the rest stays at the zero of the finalize-time memset)
-  auto zero_H = [&](int t0, int tn) {
+  // zero only the runs of Hcc some factor writes (lower triangle; the rest stays at the zero of the finalize-time memset).
+  // A warp loads 32 runs at once and zeroes them one after another, its lanes on consecutive columns, so every store
+  // instruction writes contiguous doubles.
+  {
     const HSeg *sg = d.hseg + w.off_hseg;
-    for (int e = t0; e < w.n_hseg; e += tn) {
-      const HSeg q = sg[e];
-      double *p = H + (size_t)q.row * ld + q.c0;
-      for (int k = 0; k < q.len; k++) p[k] = 0.0;
+    const int warp = tid >> 5, lane = tid & 31, nw = nt >> 5;
+    for (int e0 = warp * 32; e0 < w.n_hseg; e0 += nw * 32) {
+      const int cnt = min(32, w.n_hseg - e0);
+      HSeg q = {0, 0, 0};
+      if (lane < cnt) q = sg[e0 + lane];
+      for (int j = 0; j < cnt; j++) {
+        const int row = __shfl_sync(0xffffffffu, q.row, j), c0 = __shfl_sync(0xffffffffu, q.c0, j), len = __shfl_sync(0xffffffffu, q.len, j);
+        double *p = H + (size_t)row * ld + c0;
+        for (int k = lane; k < len; k += 32) p[k] = 0.0;
+      }
     }
-    for (int e = t0; e < n; e += tn) g[e] = 0.0;
-  };
-  zero_H(tid, nt);
+    for (int e = tid; e < n; e += nt) g[e] = 0.0;
+  }
   __syncthreads();
   // ---- prior: r = e0 + J dx ; H += J^T J ; g += J^T r
   if (w.prior_m > 0) {
@@ -261,8 +297,8 @@ __global__ void __launch_bounds__(kMiscThreads, 4) k_misc_lin(Dev d, int eval_cu
     double *dx = Jr, *r = Jr + m;
     int *cmap = reinterpret_cast<int *>(Jr + 2 * m);
     const PriorBlk *pb = d.prior_blk + w.off_prior_blk;
-    if (tid < w.prior_nblk) {
-      const PriorBlk &b = pb[tid];
+    for (int k = tid; k < w.prior_nblk; k += nt) {
+      const PriorBlk &b = pb[k];
       int col;
       if (b.kind == 0 || b.kind == 1) { prior_dx_pose(x6 + b.index * 8, b.x0, dx + b.off); col = col6[b.index]; }
       else if (b.kind == 2) { for (int q = 0; q < 9; q++) dx[b.off + q] = xsb[b.index * 9 + q] - b.x0[q]; col = colsb[b.index]; }
@@ -299,7 +335,6 @@ __global__ void __launch_bounds__(kMiscThreads, 4) k_misc_lin(Dev d, int eval_cu
     }
     __syncthreads();
   }
-  MLAP(5);
   // ---- ADMM terms (ConsensusSolver::updateTilde, ConsensusSolver.cpp:108-164)
   if (w.admm_on) {
     const int *slot = d.slot6 + w.off6;
@@ -348,60 +383,38 @@ __global__ void __launch_bounds__(kMiscThreads, 4) k_misc_lin(Dev d, int eval_cu
   }
   cost = block_sum(cost, red);
   if (tid == 0) { ctl->cand_cost_misc = cost; }
-#ifdef D2BA_MISC_TIMING
-  MLAP(6);
-  if (wi == 0 && tid == 0) printf("misc timing: zero %lld uload %lld imu_raw %lld UJ %lld JtJ %lld prior %lld tail %lld\n", mk[0], mk[1], mk[2], mk[3], mk[4], mk[5], mk[6]);
-#endif
 }
 
 // ------------------------------------------------------------------------------------------------
-// IMU factors: one WARP per factor over the whole batch (a window has only ~10 of them, so one CTA per window left the
-// SMs mostly idle during the long dependent chain of the raw residual / Jacobian).  Lane 0 evaluates the raw terms
-// (imu_raw), the warp then forms U [J r] and [J r]^T [J r] on the fp64 tensor cores (m8n8k4) and adds the lower triangle
-// into Hcc / gc with L2 reductions.  Runs after k_misc_lin (which zeroed the written runs of Hcc) and adds its cost to it.
-// k_imu_raw: one THREAD per factor -- the raw residual / Jacobian is one long dependent instruction stream, identical for every
-// factor, so 32 factors run it in lockstep per warp (one warp per factor would issue the same stream 32 times).  Output to
-// a global scratch [factor][465] whose never-written entries stay at the zero of the finalize-time memset.
-__global__ void __launch_bounds__(32) k_imu_raw(Dev d, int eval_cur, int n_imu_total) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= n_imu_total) return;
-  const ImuDesc im = d.imu[f];
-  const WinDesc &w = d.win[im.win];
-  const Ctl *ctl = d.ctl + im.win;
-  if (ctl->done || (!eval_cur && !ctl->step_valid)) return;
-  const int buf = eval_cur ? ctl->cur : 1 - ctl->cur;
-  const double *x6 = d.x6[buf] + (size_t)w.off6 * 8, *xsb = d.xsb[buf] + (size_t)w.offsb * 9;
-  double *raw = d.imu_raw + (size_t)f * (15 * 30 + 15);
-  imu_raw(d.imu_c + (size_t)f * kImuStride, x6 + im.pi * 8, xsb + im.si * 9, x6 + im.pj * 8, xsb + im.sj * 9, d.prm.gravity, raw + 450, raw);
-}
+// IMU factors: one WARP per factor over the whole batch (a window has only ~10 of them).  imu_stage evaluates the raw
+// [J r] lane-parallel into shared memory and forms U [J r] on the fp64 tensor cores (m8n8k4); k_imu_lin then forms
+// [J r]^T [J r] the same way and adds the lower triangle into Hcc / gc with L2 reductions.  Runs after k_misc_lin (which
+// zeroed the written runs of Hcc and stored the window's cost) and adds to both.
 constexpr int kImuWarps = 4;
 constexpr int kImuF = 15 * 30 + 15;   // doubles per factor for (J, r)
-constexpr int kImuWarpDoubles = 2 * kImuF + 225 + 1;   // raw, U [J r], sqrt-information
-__global__ void __launch_bounds__(kImuWarps * 32) k_imu_lin(Dev d, int eval_cur, int n_imu_total) {
-  extern __shared__ double sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int f = blockIdx.x * kImuWarps + warp;
-  if (f >= n_imu_total) return;
-  const ImuDesc im = d.imu[f];
-  const int wi = im.win;
-  const WinDesc &w = d.win[wi];
-  Ctl *ctl = d.ctl + wi;
-  if (ctl->done || (!eval_cur && !ctl->step_valid)) return;
-  const int buf = eval_cur ? ctl->cur : 1 - ctl->cur;
-  double *raw = sm + (size_t)warp * kImuWarpDoubles, *fin = raw + kImuF, *Us = fin + kImuF;
-  const int ld = w.ldh;
-  double *H = d.Hcc[buf] + w.offH, *g = d.gc[buf] + w.offc;
-  const int *col6 = d.col6 + w.off6, *colsb = d.colsb + w.offsb;
-  // raw (J, r) of k_imu_raw and the sqrt-information: coalesced, all in flight
+constexpr int kImuWarpDoubles = 2 * kImuF + 225 + 1;   // raw, U [J r] (the constants before it), sqrt-information
+
+// One warp: factor f at state buffer buf -> fin = U [J | r] (15 x 30 whitened Jacobian, then the 15 whitened residuals).
+// raw / fin: kImuF doubles each, Us: 225.  The debug view (k_imu_debug) runs this same path.
+D2BA_DEV void imu_stage(const Dev &d, const ImuDesc &im, int f, int buf, int lane, double *raw, double *fin, double *Us) {
+  const WinDesc &w = d.win[im.win];
+  const double *x6 = d.x6[buf] + (size_t)w.off6 * 8, *xsb = d.xsb[buf] + (size_t)w.offsb * 9;
+  double *cs = fin;   // the factor's constants, staged where U [J r] goes once they are used
   {
-    const double *Ug = d.imu_U + (size_t)f * 225, *rg = d.imu_raw + (size_t)f * kImuF;
+    const double *Ug = d.imu_U + (size_t)f * 225, *cg = d.imu_c + (size_t)f * kImuStride;
     for (int e = lane; e < 225; e += 32) cp_async8(Us + e, Ug + e);
-    for (int e = lane; e < kImuF; e += 32) cp_async8(raw + e, rg + e);
+    for (int e = lane; e < kImuConst; e += 32) cp_async8(cs + e, cg + imu_const_src(e));
+    for (int e = lane; e < 450; e += 32) raw[e] = 0.0;
     cp_async_wait_all();
   }
-  const int cols[4] = {col6[im.pi], colsb[im.si], col6[im.pj], colsb[im.sj]};
-  const double *U = Us;
   __syncwarp();
+  {
+    ImuLin L;
+    imu_prefix(cs, x6 + im.pi * 8, xsb + im.si * 9, x6 + im.pj * 8, xsb + im.sj * 9, d.prm.gravity, L, lane == kImuBlocks ? raw + 450 : nullptr);
+    if (lane < kImuBlocks) imu_block(lane, L, cs, raw);
+  }
+  __syncwarp();
+  const double *U = Us;
   const int g4 = lane >> 2, q4 = lane & 3;
   // fin = U [Jraw | rraw]: 2 x 4 output tiles, K = 15 (4 k-steps, the 16th masked)
   for (int job = 0; job < 8; job++) {
@@ -424,10 +437,30 @@ __global__ void __launch_bounds__(kImuWarps * 32) k_imu_lin(Dev d, int eval_cur,
     }
   }
   __syncwarp();
+}
+
+__global__ void __launch_bounds__(kImuWarps * 32, 4) k_imu_lin(Dev d, int eval_cur, int n_imu_total) {
+  extern __shared__ double sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int f = blockIdx.x * kImuWarps + warp;
+  if (f >= n_imu_total) return;
+  const ImuDesc im = d.imu[f];
+  const int wi = im.win;
+  const WinDesc &w = d.win[wi];
+  Ctl *ctl = d.ctl + wi;
+  if (ctl->done || (!eval_cur && !ctl->step_valid)) return;
+  const int buf = eval_cur ? ctl->cur : 1 - ctl->cur;
+  double *raw = sm + (size_t)warp * kImuWarpDoubles, *fin = raw + kImuF, *Us = fin + kImuF;
+  const int ld = w.ldh;
+  double *H = d.Hcc[buf] + w.offH, *g = d.gc[buf] + w.offc;
+  const int *col6 = d.col6 + w.off6, *colsb = d.colsb + w.offsb;
+  const int cpi = col6[im.pi], csi = colsb[im.si], cpj = col6[im.pj], csj = colsb[im.sj];
+  imu_stage(d, im, f, buf, lane, raw, fin, Us);
+  const int g4 = lane >> 2, q4 = lane & 3;
   auto gcol = [&](int a) -> int {  // local 0..29 -> reduced column
-    const int b = a < 6 ? 0 : (a < 15 ? 1 : (a < 21 ? 2 : 3));
+    const int c = a < 6 ? cpi : (a < 15 ? csi : (a < 21 ? cpj : csj));
     const int o = a < 6 ? a : (a < 15 ? a - 6 : (a < 21 ? a - 15 : a - 21));
-    return cols[b] < 0 ? -1 : cols[b] + o;
+    return c < 0 ? -1 : c + o;
   };
   // [J r]^T [J r]: 4 x 4 output tiles (rows a < 30; column 30 is the gradient), lower triangle kept
   for (int job = 0; job < 16; job++) {
@@ -899,25 +932,16 @@ __global__ void k_proj_debug(Dev d, double *out /*[tiles*32][81]*/, int n_tiles_
   }
 }
 
-// debug: whitened residual + Jacobian of every IMU factor (one thread per factor), same imu_raw as k_misc_lin
-__global__ void k_imu_debug(Dev d, double *out /*[n_imu_total][465]*/, const int *imu_win, int n_imu_total) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+// debug: whitened residual + Jacobian of every IMU factor, through the path k_imu_lin runs (imu_stage, one warp per factor)
+__global__ void __launch_bounds__(kImuWarps * 32) k_imu_debug(Dev d, double *out /*[n_imu_total][465]*/, const int *imu_win, int n_imu_total) {
+  extern __shared__ double sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int f = blockIdx.x * kImuWarps + warp;
   if (f >= n_imu_total) return;
-  const int wi = imu_win[f];
-  const WinDesc &w = d.win[wi];
-  const int buf = d.ctl[wi].cur;
-  const double *x6 = d.x6[buf] + (size_t)w.off6 * 8, *xsb = d.xsb[buf] + (size_t)w.offsb * 9;
-  const ImuDesc &im = d.imu[f];
-  double raw[465];
-  for (int i = 0; i < 465; i++) raw[i] = 0.0;
-  imu_raw(d.imu_c + (size_t)f * kImuStride, x6 + im.pi * 8, xsb + im.si * 9, x6 + im.pj * 8, xsb + im.sj * 9, d.prm.gravity, raw + 450, raw);
-  const double *U = d.imu_U + (size_t)f * 225;
+  double *raw = sm + (size_t)warp * kImuWarpDoubles, *fin = raw + kImuF, *Us = fin + kImuF;
+  imu_stage(d, d.imu[f], f, d.ctl[imu_win[f]].cur, lane, raw, fin, Us);
   double *o = out + (size_t)f * 465;
-  for (int i = 0; i < 15; i++) {
-    double s = 0; for (int k = 0; k < 15; k++) s += U[i * 15 + k] * raw[450 + k];
-    o[i] = s;
-    for (int j = 0; j < 30; j++) { double a = 0; for (int k = 0; k < 15; k++) a += U[i * 15 + k] * raw[k * 30 + j]; o[15 + i * 30 + j] = a; }
-  }
+  for (int e = lane; e < 465; e += 32) o[e] = e < 15 ? fin[450 + e] : fin[e - 15];
 }
 __global__ void k_cons_debug(Dev d, double *out /*[n6_total][62]*/, const int *blk_win, int n6_total) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -934,7 +958,9 @@ __global__ void k_cons_debug(Dev d, double *out /*[n6_total][62]*/, const int *b
   for (int i = 0; i < 6; i++) { o[14 + i] = tl[i]; o[20 + i] = r[i]; }
   for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) { o[26 + i * 6 + j] = wT * Rz[j * 3 + i]; o[26 + (3 + i) * 6 + 3 + j] = wq * L3[i * 3 + j]; }
 }
-void launch_imu_debug(const Dev &d, double *out, const int *imu_win, int n, cudaStream_t s) { if (n > 0) k_imu_debug<<<(n + 31) / 32, 32, 0, s>>>(d, out, imu_win, n); }
+void launch_imu_debug(const Dev &d, double *out, const int *imu_win, int n, cudaStream_t s) {
+  if (n > 0) k_imu_debug<<<(n + kImuWarps - 1) / kImuWarps, kImuWarps * 32, (size_t)kImuWarps * kImuWarpDoubles * 8, s>>>(d, out, imu_win, n);
+}
 void launch_cons_debug(const Dev &d, double *out, const int *blk_win, int n, cudaStream_t s) { if (n > 0) k_cons_debug<<<(n + 63) / 64, 64, 0, s>>>(d, out, blk_win, n); }
 
 // ------------------------------------------------------------------------------------------------
@@ -2770,7 +2796,7 @@ int launch_marg_reduce(const double *S, int ld, int n, const int *keep_idx, int 
 void launch_state_prep(const Dev &d, int n6_total, int buf, cudaStream_t s) {
   if (n6_total > 0) k_state_prep<<<(n6_total + 127) / 128, 128, 0, s>>>(d, n6_total, buf);
 }
-// packed upload record (kImuPack) -> the full constant record imu_raw / k_imu_prep index (kImuStride); entries the factor
+// packed upload record (kImuPack) -> the full constant record imu_stage / k_imu_prep index (kImuStride); entries the factor
 // never reads stay at the zero of the finalize-time memset
 __global__ void k_imu_unpack(const double *pk, double *full, int n_imu) {
   const int f = blockIdx.x, t = threadIdx.x;
@@ -2794,15 +2820,8 @@ void launch_imu_prep(const Dev &d, const double *packed, double *full, int n_imu
 void launch_prior_prep(const Dev &d, cudaStream_t s) { k_prior_prep<<<d.n_win, 256, 0, s>>>(d); }
 
 size_t misc_smem_bytes(int max_prior_m) { return (size_t)(40 + 3 * max_prior_m + 8) * 8; }
-void launch_imu_raw(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s) {
-  if (n_imu_total > 0) k_imu_raw<<<(n_imu_total + 31) / 32, 32, 0, s>>>(d, eval_cur, n_imu_total);
-}
-void launch_imu_acc(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s) {
-  if (n_imu_total > 0) k_imu_lin<<<(n_imu_total + kImuWarps - 1) / kImuWarps, kImuWarps * 32, (size_t)kImuWarps * kImuWarpDoubles * 8, s>>>(d, eval_cur, n_imu_total);
-}
 void launch_imu_lin(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s) {
-  launch_imu_raw(d, eval_cur, n_imu_total, s);
-  launch_imu_acc(d, eval_cur, n_imu_total, s);
+  if (n_imu_total > 0) k_imu_lin<<<(n_imu_total + kImuWarps - 1) / kImuWarps, kImuWarps * 32, (size_t)kImuWarps * kImuWarpDoubles * 8, s>>>(d, eval_cur, n_imu_total);
 }
 void launch_misc_lin(const Dev &d, int eval_cur, int max_prior_m, cudaStream_t s) {
   k_misc_lin<<<d.n_win, kMiscThreads, misc_smem_bytes(max_prior_m), s>>>(d, eval_cur);

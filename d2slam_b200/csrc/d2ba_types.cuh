@@ -176,7 +176,6 @@ struct Dev {
   const ImuDesc *imu;
   const double *imu_c;  // [NIMU][kImuStride]
   double *imu_U;        // [NIMU][225] sqrt_info
-  double *imu_raw;      // [NIMU][465] raw Jacobian (15 x 30) + residual (15) of the current linearisation (k_imu_raw -> k_imu_lin)
   // prior
   const PriorBlk *prior_blk;
   const double *prior_J;  // m x m
