@@ -36,7 +36,7 @@ void launch_proj_lin(const Dev &d, int variant, int eval_cur, int job_begin, int
 void launch_proj_debug(const Dev &d, double *out, int n_tiles, const int *tile_win, cudaStream_t s);
 void launch_imu_debug(const Dev &d, double *out, const int *imu_win, int n, cudaStream_t s);
 void launch_cons_debug(const Dev &d, double *out, const int *blk_win, int n, cudaStream_t s);
-void launch_lm_gather(const Dev &d, const int *lm_win, int n_lm_total, int max_ldw, int any_compact, int any_wide, cudaStream_t s);
+void launch_lm_gather(const Dev &d, const int *lm_win, int n_lm_total, int max_ldw, int any_compact, int any_wide, int n_chunk12, cudaStream_t s);
 void launch_schur(const Dev &d, const void *tiles, int n_tiles, cudaStream_t s);
 int configure_leaf_elim(size_t smem);
 void launch_leaf_elim(const Dev &d, size_t smem, cudaStream_t s);
@@ -265,7 +265,7 @@ struct d2ba_handle {
   DBuf<Group> d_grp; DBuf<Job> d_job; DBuf<ImuDesc> d_imu; DBuf<PriorBlk> d_prior_blk;
   DBuf<double> d_obs, d_rec[2], d_imu_c, d_imu_pk, d_imu_U, d_prior_J, d_prior_e0, d_prior_A, d_z6, d_tilde6, d_lm_ref, d_sb_ref, d_td_ref,
       d_cons, d_H[2], d_gc[2], d_Wt, d_dinv, d_hl, d_gl, d_S, d_gred, d_D2c, d_gn_c, d_gn_l, d_step_c, d_step_l, d_wu, d_uc, d_D2l, d_dbg;
-  DBuf<SchurTileH> d_schur; DBuf<int> d_schur_chunks; DBuf<Leaf> d_leaf; DBuf<HSeg> d_hseg; DBuf<unsigned long long> d_lm_mask; DBuf<double> d_leafL; DBuf<int> d_leaf_lm;
+  DBuf<SchurTileH> d_schur; DBuf<int> d_schur_chunks; DBuf<Leaf> d_leaf; DBuf<HSeg> d_hseg; DBuf<unsigned long long> d_lm_mask; DBuf<double> d_leafL; DBuf<int> d_leaf_lm; DBuf<int4> d_g12;
   int n_schur0 = 0, n_leaf_total = 0, max_hub = 0; size_t leaf_smem = 0, cfg_leaf_smem = 0, leafb_smem = 0, cfg_leafb_smem = 0;
   DBuf<int> d_pr_m, d_pr_info, d_tile_src; DBuf<long long> d_pr_oJ, d_pr_ov, d_raw_off;
   int cfg_max_rows = -1, cfg_max_nc = -1, cfg_max_prior = -1, cfg_max_ldw = -1;
@@ -275,12 +275,13 @@ struct d2ba_handle {
   std::vector<Group> h_grp;
   std::vector<int> h_tile_win;
   int n_used = 0, n6_total = 0, nsb_total = 0, nl_total = 0, n_tiles = 0, n_imu_total = 0, n_schur = 0;
-  int job_begin[6] = {0, 0, 0, 0, 0, 0}, job_count[6] = {0, 0, 0, 0, 0, 0};
+  int job_begin[8] = {0, 0, 0, 0, 0, 0, 0, 0}, job_count[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   int max_rows = 1, max_nc = 1, max_prior_m = 0, max_ldw = 8, n_slots = 0;
   int max_n_smem = 0, max_rows_glob = 1; bool any_chol_glob = false; int cfg_max_n_smem = -1;
   int max_ldw_small = 0, cfg_max_ldw_small = -1;
   int max_row_tiles = 1;
   int any_compact = 0, any_wide = 0;   // record widths present (which gather kernels to launch)
+  int n_g12 = 0;                       // k_lm_gather12 chunks (windows with 96-byte records)
   size_t sbb_smem = 0, cfg_sbb_smem = 0;   // k_sb_back dynamic shared memory
   size_t sbe_smem = 0, cfg_sbe_smem = 0;   // speed-bias elimination: dynamic shared memory of k_sb_elim (0 = no window uses it)
   int64_t totLE = 0;
@@ -297,6 +298,7 @@ struct d2ba_handle {
   bool force_full_S = false;     // the Schur kernels must write the complete reduced system (marginalization reads it)
   bool no_leaf = false;          // D2BA_NO_LEAF=1: keep remote-frame blocks in the dense part (A/B switch)
   bool no_sb_elim = false;       // D2BA_NO_SB_ELIM=1: keep the dense Cholesky of the whole reduced system (A/B switch for tests / profiling)
+  bool rec128 = false;           // D2BA_REC128=1: 128-byte records and k_lm_gather16 in every window that would use 96-byte ones (A/B switch)
   double host_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // wall-clock phases of the last d2ba_finalize (d2ba_debug_host_times)
   double solve_ms[4] = {0, 0, 0, 0};             // host wall-clock of the last solve: enqueue, wait for the device, write-back
   std::atomic<long long> h2d_bytes_add;          // bytes d2ba_add_proj put on the copy stream since the last reset
@@ -371,6 +373,7 @@ int d2ba_create(const d2ba_config *cfg, d2ba_handle **out) {
   d2ba_handle *h = new d2ba_handle();
   { const char *e = getenv("D2BA_NO_SB_ELIM"); h->no_sb_elim = e && e[0] == '1'; }
   { const char *e = getenv("D2BA_NO_LEAF"); h->no_leaf = e && e[0] == '1'; }
+  { const char *e = getenv("D2BA_REC128"); h->rec128 = e && e[0] == '1'; }
   h->cfg = *cfg;
   if (h->cfg.max_windows < 1) h->cfg.max_windows = 1;
   if (h->cfg.initial_trust_region_radius <= 0) h->cfg.initial_trust_region_radius = 1e4;
@@ -408,7 +411,7 @@ int d2ba_destroy(d2ba_handle *h) {
   h->d_grp.release(); h->d_job.release(); h->d_imu.release(); h->d_prior_blk.release(); h->d_obs.release(); h->d_imu_c.release(); h->d_imu_pk.release(); h->d_imu_U.release();
   h->d_prior_J.release(); h->d_prior_e0.release(); h->d_prior_A.release(); h->d_z6.release(); h->d_tilde6.release(); h->d_lm_ref.release(); h->d_sb_ref.release();
   h->d_td_ref.release(); h->d_cons.release(); h->d_Wt.release(); h->d_dinv.release(); h->d_hl.release(); h->d_gl.release(); h->d_S.release(); h->d_gred.release();
-  h->d_D2c.release(); h->d_gn_c.release(); h->d_gn_l.release(); h->d_step_c.release(); h->d_step_l.release(); h->d_wu.release(); h->d_uc.release(); h->d_D2l.release(); h->d_dbg.release(); h->d_schur.release(); h->d_schur_chunks.release(); h->d_leaf.release(); h->d_hseg.release(); h->d_lm_mask.release(); h->d_leafL.release(); h->d_leaf_lm.release();
+  h->d_D2c.release(); h->d_gn_c.release(); h->d_gn_l.release(); h->d_step_c.release(); h->d_step_l.release(); h->d_wu.release(); h->d_uc.release(); h->d_D2l.release(); h->d_dbg.release(); h->d_schur.release(); h->d_schur_chunks.release(); h->d_leaf.release(); h->d_hseg.release(); h->d_lm_mask.release(); h->d_leafL.release(); h->d_leaf_lm.release(); h->d_g12.release();
   h->d_pr_m.release(); h->d_pr_info.release(); h->d_pr_oJ.release(); h->d_pr_ov.release(); h->d_tile_src.release(); h->d_raw_off.release();
   cudaStreamSynchronize(h->copy_stream);
   for (auto &w : h->win) { w.rawj.release(); w.anch.release(); w.d_rawj.release(); w.d_anch.release(); w.rawjm.release(); w.anchm.release(); w.d_rawjm.release(); w.d_anchm.release(); }
@@ -742,13 +745,14 @@ struct WinPlan {
   WinDesc d;
   std::vector<Group> groups;
   std::vector<int> grp_begin, grp_cnt, grp_tile0;   // sorted-obs range and first (window-local) tile of each group
-  std::vector<Job> jobs[6];                         // tile_begin window-local, grp window-local
+  std::vector<Job> jobs[8];                         // tile_begin window-local, grp window-local; index = launch_proj_lin variant
   std::vector<SchurTileH> schur[2];                  // stage 0 (tiles with leaf columns), stage 1 (hub x hub)
   std::vector<int> schur_chunks;                     // chunk lists, window-local offsets in SchurTile::cb
   std::vector<uint64_t> hruns; std::vector<Leaf> leaves; std::vector<HSeg> hseg; std::vector<unsigned long long> lm_mask; std::vector<int> leaf_lm; int leaf_lm_off = 0;
   int n_tiles = 0, n_lmobs = 0;
-  int job_off[6] = {0, 0, 0, 0, 0, 0};
+  int job_off[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   int schur_off[2] = {0, 0}, chunk_off = 0;
+  std::vector<int4> g12; int g12_off = 0;          // k_lm_gather12 chunks {window, first, end landmark, 0} (rec_stride == 12)
 };
 
 template <typename F>
@@ -776,7 +780,7 @@ struct Staging {   // every array finalize uploads lives in ONE pinned arena -> 
   HView<long long> raw_off;
   HView<long long> pr_offJ, pr_offv;
   HView<Group> grp; HView<Job> job; HView<ImuDesc> imu; HView<PriorBlk> pblk; HView<SchurTileH> schur;
-  HView<int> schur_chunks, leaf_lm; HView<Leaf> leaf; HView<HSeg> hseg; HView<unsigned long long> lm_mask;
+  HView<int> schur_chunks, leaf_lm; HView<Leaf> leaf; HView<HSeg> hseg; HView<unsigned long long> lm_mask; HView<int4> g12;
   template <typename T> void reserve(HView<T> &v, size_t count) { v.n = count; v.off = cursor; cursor += (count * sizeof(T) + 255) & ~(size_t)255; }
   template <typename T> void place(HView<T> &v) { v.p = (T *)(arena.p + v.off); }
 };
@@ -993,7 +997,7 @@ int d2ba_finalize(d2ba_handle *h) {
     // landmark masks: W-space column tiles (32 columns) a landmark's coupling row touches; the rhs column n_lc always
     pl.lm_mask.assign(nl, 1ull << (w.n_lc / 32));
     auto mark = [&](int lm, int col, int width) { if (col >= 0) pl.lm_mask[lm] |= (1ull << (col / 32)) | (1ull << ((col + width - 1) / 32)); };
-    bool any_wide = false;
+    bool any_wide = false, all_pp = true;
     size_t k = 0; int tile_run = 0;
     while (k < M) {
       size_t e = k;
@@ -1019,6 +1023,7 @@ int d2ba_finalize(d2ba_handle *h) {
       g.shift0 = (!g.need_td && o0.type != D2BA_PROJ_DEPTH_PRIOR && w.td_min == w.td_max && w.td_min == w.td) ? 1 : 0;
       if (variant == 0 && !g.need_ext && (o0.type == D2BA_PROJ_2F1C || o0.type == D2BA_PROJ_2F2C) && ns == 2 && g.slot_src[0] == 0 && g.slot_src[1] == 1)
         variant = g.shift0 ? 4 : 5;
+      if (variant < 4) all_pp = false;
       const int cnt = (int)(e - k), ntile = (cnt + kTile - 1) / kTile;
       const int gi = (int)pl.groups.size();
       pl.groups.push_back(g); pl.grp_begin.push_back((int)k); pl.grp_cnt.push_back(cnt); pl.grp_tile0.push_back(tile_run);
@@ -1090,6 +1095,34 @@ int d2ba_finalize(d2ba_handle *h) {
       d.row_tiles = rt;
     }
     d.rec_stride = any_wide ? 32 : 16;
+    pl.g12.clear();
+    if (!any_wide && all_pp && !h->rec128 && d.n_leaf == 0 && d.gather_nosync) {
+      // 96-byte records + k_lm_gather12: every record comes from k_proj_lin_pp (two free poses: slot 1's position block is
+      // minus slot 0's), and per landmark the slot-0 column is unique (gather_nosync), the slot-1 columns are pairwise
+      // distinct and there are at most 32 records (one lane each)
+      std::vector<int> cnt(nl, 0);
+      std::vector<uint64_t> lc; lc.reserve(M);
+      for (int gi = 0; gi < (int)pl.groups.size(); gi++)
+        for (int q = pl.grp_begin[gi]; q < pl.grp_begin[gi] + pl.grp_cnt[gi]; q++) {
+          const int lm = w.obs[w.order[q]].lm;
+          cnt[lm]++;
+          lc.push_back(((uint64_t)lm << 32) | (uint32_t)pl.groups[gi].slot_col[1]);
+        }
+      bool ok = true;
+      for (int l = 0; l < nl && ok; l++) ok = cnt[l] <= 32;
+      if (ok) { std::sort(lc.begin(), lc.end()); ok = std::adjacent_find(lc.begin(), lc.end()) == lc.end(); }
+      if (ok) {
+        d.rec_stride = 12;
+        pl.jobs[6].swap(pl.jobs[4]); pl.jobs[7].swap(pl.jobs[5]);   // k_proj_lin_pp<SHIFT0, 96-byte records>
+        // chunks of whole landmarks: at most 32 records and 31 landmarks (lane #landmarks holds the end pointer)
+        for (int l = 0; l < nl;) {
+          const int l0 = l;
+          int r = 0;
+          while (l < nl && l - l0 < 31 && r + cnt[l] <= 32) r += cnt[l++];
+          pl.g12.push_back(make_int4(wi, l0, l, 0));
+        }
+      }
+    }
     pl.n_lmobs = (int)M;
     d.schur_small = (d.n_lc + 1 <= 96) ? 1 : 0;
     d.hub_small = (d.n_leaf > 0 && d.n_hub + 1 <= 96) ? 1 : 0;
@@ -1181,9 +1214,9 @@ int d2ba_finalize(d2ba_handle *h) {
   h->max_row_tiles = 1; h->max_n_smem = 0; h->max_rows_glob = 1; h->any_chol_glob = false; h->max_ldw_small = 0; h->any_compact = h->any_wide = 0; h->sbe_smem = 0; h->sbb_smem = 0;
   int64_t offLE = 0;
   int off6 = 0, offsb = 0, offlm = 0, off_tile = 0, off_grp = 0, off_imu = 0, off_lmptr = 0, off_pblk = 0, n_schur = 0, n_sch[2] = {0, 0}, n_chunks = 0, off_leaf = 0, off_hseg = 0, n_leaf_lm = 0;
-  int64_t offLL = 0; size_t leaf_smem = 0, leafb_smem = 0; int max_hub = 0;
+  int64_t offLL = 0; size_t leaf_smem = 0, leafb_smem = 0; int max_hub = 0, n_g12 = 0;
   int64_t offH = 0, offW = 0, offc = 0, off_lmobs = 0, off_pJ = 0, off_pv = 0, off_rec = 0; long long off_raw = 0;
-  int njobs[6] = {0, 0, 0, 0, 0, 0};
+  int njobs[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   bool any_info = false;
   for (int wi = 0; wi < nw; wi++) {
     HostWin &w = h->win[wi]; WinPlan &pl = plan[wi]; WinDesc &d = pl.d;
@@ -1196,7 +1229,7 @@ int d2ba_finalize(d2ba_handle *h) {
     d.offH = offH; offH += (int64_t)(d.n_c + 1) * d.ldh;
     d.offW = offW; offW += (int64_t)std::max(d.wt_rows, 32) * d.ldw;
     d.offc = offc; offc += roundup(d.n_c + 1, 4);
-    for (int v = 0; v < 6; v++) { pl.job_off[v] = njobs[v]; njobs[v] += (int)pl.jobs[v].size(); }
+    for (int v = 0; v < 8; v++) { pl.job_off[v] = njobs[v]; njobs[v] += (int)pl.jobs[v].size(); }
     for (int sg = 0; sg < 2; sg++) { pl.schur_off[sg] = n_sch[sg]; n_sch[sg] += (int)pl.schur[sg].size(); }
     pl.chunk_off = n_chunks; n_chunks += (int)pl.schur_chunks.size();
     pl.leaf_lm_off = n_leaf_lm; n_leaf_lm += (int)pl.leaf_lm.size();
@@ -1208,7 +1241,8 @@ int d2ba_finalize(d2ba_handle *h) {
     h->max_prior_m = std::max(h->max_prior_m, d.prior_m);
     if (d.schur_small) h->max_ldw_small = std::max(h->max_ldw_small, d.ldw);
     if (d.hub_small) h->max_ldw_small = std::max(h->max_ldw_small, roundup(d.n_hub + 1, 8));
-    if (d.rec_stride == 16) h->any_compact = 1; else h->any_wide = 1;
+    if (d.rec_stride == 16) h->any_compact = 1; else if (d.rec_stride == 32) h->any_wide = 1;
+    pl.g12_off = n_g12; n_g12 += (int)pl.g12.size();
     if (d.sb_elim) {
       d.offLE = offLE; offLE += (int64_t)d.n_sbe * 171;
       h->sbe_smem = std::max(h->sbe_smem, sb_elim_smem(roundup(d.n_hub + 1, 8), d.n_c, d.n_sbe)); h->sbb_smem = std::max(h->sbb_smem, sb_back_smem(d.n_hub, d.n_sbe));
@@ -1221,8 +1255,8 @@ int d2ba_finalize(d2ba_handle *h) {
     }
     if (w.prior_m > 0 && w.prior_is_info) any_info = true;
   }
-  int jbase[6]; { int r = 0; for (int v = 0; v < 6; v++) { jbase[v] = r; h->job_begin[v] = r; h->job_count[v] = njobs[v]; r += njobs[v]; } }
-  const int n_jobs = jbase[5] + njobs[5];
+  int jbase[8]; { int r = 0; for (int v = 0; v < 8; v++) { jbase[v] = r; h->job_begin[v] = r; h->job_count[v] = njobs[v]; r += njobs[v]; } }
+  const int n_jobs = jbase[7] + njobs[7];
   h->n6_total = off6; h->nsb_total = offsb; h->nl_total = offlm; h->n_tiles = off_tile; h->n_imu_total = off_imu; n_schur = n_sch[0] + n_sch[1]; h->n_schur = n_schur; h->n_schur0 = n_sch[0];
   h->n_leaf_total = off_leaf; h->leaf_smem = leaf_smem; h->leafb_smem = leafb_smem; h->max_hub = max_hub;
   h->totH = offH; h->totW = offW; h->totc = offc; h->totLE = offLE;
@@ -1233,14 +1267,14 @@ int d2ba_finalize(d2ba_handle *h) {
   st.reserve(st.lm_win, offlm); st.reserve(st.tile_grp, off_tile); st.reserve(st.tile_win, off_tile); st.reserve(st.obs_lm, (size_t)off_tile * kTile);
   st.reserve(st.tile_src, (size_t)off_tile * kTile); st.reserve(st.raw_off, 4 * (size_t)nw); st.reserve(st.lm_ptr, off_lmptr); st.reserve(st.obs_slot, (size_t)off_tile * kTile);
   st.reserve(st.grp, off_grp); st.reserve(st.job, n_jobs); st.reserve(st.imu, off_imu); st.reserve(st.imu_c, (size_t)off_imu * kImuPack);
-  st.reserve(st.pblk, off_pblk); st.reserve(st.prior_J, (size_t)off_pJ); st.reserve(st.prior_e0, (size_t)off_pv); st.reserve(st.schur, n_schur); st.reserve(st.schur_chunks, n_chunks); st.reserve(st.leaf, off_leaf); st.reserve(st.hseg, off_hseg); st.reserve(st.lm_mask, offlm); st.reserve(st.leaf_lm, n_leaf_lm);
+  st.reserve(st.pblk, off_pblk); st.reserve(st.prior_J, (size_t)off_pJ); st.reserve(st.prior_e0, (size_t)off_pv); st.reserve(st.schur, n_schur); st.reserve(st.schur_chunks, n_chunks); st.reserve(st.leaf, off_leaf); st.reserve(st.hseg, off_hseg); st.reserve(st.lm_mask, offlm); st.reserve(st.leaf_lm, n_leaf_lm); st.reserve(st.g12, n_g12);
   st.reserve(st.pr_m, nw); st.reserve(st.pr_info, nw); st.reserve(st.pr_offJ, nw); st.reserve(st.pr_offv, nw);
   bool ok = st.arena.resize(st.cursor + 256);
   if (ok) {
     st.place(st.win); st.place(st.x6); st.place(st.xsb); st.place(st.xlm); st.place(st.xtd); st.place(st.col6); st.place(st.colsb); st.place(st.slot6);
     st.place(st.blk_win); st.place(st.sb_win); st.place(st.lm_win); st.place(st.tile_grp); st.place(st.tile_win); st.place(st.obs_lm); st.place(st.tile_src);
     st.place(st.raw_off); st.place(st.lm_ptr); st.place(st.obs_slot); st.place(st.grp); st.place(st.job); st.place(st.imu); st.place(st.imu_c); st.place(st.pblk);
-    st.place(st.prior_J); st.place(st.prior_e0); st.place(st.schur); st.place(st.schur_chunks); st.place(st.leaf); st.place(st.hseg); st.place(st.lm_mask); st.place(st.leaf_lm); st.place(st.pr_m); st.place(st.pr_info); st.place(st.pr_offJ); st.place(st.pr_offv);
+    st.place(st.prior_J); st.place(st.prior_e0); st.place(st.schur); st.place(st.schur_chunks); st.place(st.leaf); st.place(st.hseg); st.place(st.lm_mask); st.place(st.leaf_lm); st.place(st.g12); st.place(st.pr_m); st.place(st.pr_info); st.place(st.pr_offJ); st.place(st.pr_offv);
   }
   if (!ok) return fail(h, 24, "pinned staging allocation failed");
   lap(1);
@@ -1291,7 +1325,7 @@ int d2ba_finalize(d2ba_handle *h) {
     }
     // a landmark's records in ascending tile-position order (deterministic reduction order): positions increase with sorted index
     for (size_t k = 0; k < w.order.size(); k++) { const HObs &o = w.obs[w.order[k]]; oslot[w.sorted_pos[k]] = cursor[o.lm]++; }
-    for (int v = 0; v < 6; v++)
+    for (int v = 0; v < 8; v++)
       for (size_t j = 0; j < pl.jobs[v].size(); j++) {
         Job jb = pl.jobs[v][j]; jb.grp += d.off_grp; jb.tile_begin += d.off_tile;
         st.job.p[jbase[v] + pl.job_off[v] + j] = jb;
@@ -1303,6 +1337,7 @@ int d2ba_finalize(d2ba_handle *h) {
     for (size_t t = 0; t < pl.leaf_lm.size(); t++) st.leaf_lm.p[pl.leaf_lm_off + t] = pl.leaf_lm[t];
     for (size_t t = 0; t < pl.hseg.size(); t++) st.hseg.p[d.off_hseg + t] = pl.hseg[t];
     for (int l = 0; l < d.nl; l++) st.lm_mask.p[d.offlm + l] = pl.lm_mask[l];
+    for (size_t t = 0; t < pl.g12.size(); t++) st.g12.p[pl.g12_off + t] = pl.g12[t];
     for (int i = 0; i < d.n_imu; i++) {
       const HImu &m = w.imu[i];
       st.imu.p[d.off_imu + i] = ImuDesc{m.pi, m.si, m.pj, m.sj, wi};
@@ -1362,7 +1397,7 @@ int d2ba_finalize(d2ba_handle *h) {
       (rc = up(h, h->d_grp, st.grp)) || (rc = up(h, h->d_job, st.job)) || (rc = up(h, h->d_imu, st.imu)) || (rc = up(h, h->d_imu_pk, st.imu_c)) ||
       (rc = up(h, h->d_prior_blk, st.pblk)) || (rc = up(h, h->d_prior_J, st.prior_J)) || (rc = up(h, h->d_prior_e0, st.prior_e0)) ||
       (rc = up(h, h->d_schur, st.schur)) || (rc = up(h, h->d_schur_chunks, st.schur_chunks)) || (rc = up(h, h->d_leaf, st.leaf)) || (rc = up(h, h->d_leaf_lm, st.leaf_lm)) ||
-      (rc = up(h, h->d_hseg, st.hseg)) || (rc = up(h, h->d_lm_mask, st.lm_mask)))
+      (rc = up(h, h->d_hseg, st.hseg)) || (rc = up(h, h->d_lm_mask, st.lm_mask)) || (rc = up(h, h->d_g12, st.g12)))
     return rc;
   // the device builds the tiles from the raw records
   CK(h->d_obs.alloc((size_t)off_tile * kTile * kObsFields));
@@ -1392,6 +1427,7 @@ int d2ba_finalize(d2ba_handle *h) {
   for (int b = 0; b < 2; b++) { D.x6[b] = h->d_x6[b].p; D.R6[b] = h->d_R6[b].p; D.xsb[b] = h->d_xsb[b].p; D.xlm[b] = h->d_xlm[b].p; D.xtd[b] = h->d_xtd[b].p; D.rec[b] = h->d_rec[b].p; D.Hcc[b] = h->d_H[b].p; D.gc[b] = h->d_gc[b].p; }
   D.col6 = h->d_col6.p; D.colsb = h->d_colsb.p; D.grp = h->d_grp.p; D.job = h->d_job.p; D.n_job = n_jobs;
   D.lm_mask = h->d_lm_mask.p; D.hseg = h->d_hseg.p; D.leaf = h->d_leaf.p; D.n_leaf_total = h->n_leaf_total; { int np_ = 0; for (int q = 0; q < nw; q++) if (plan[q].d.n_leaf == 0) np_++; D.n_plain_win = np_; } D.leafL = h->d_leafL.p; D.schur_chunks = h->d_schur_chunks.p; D.leaf_lm = h->d_leaf_lm.p;
+  D.g12_chunk = h->d_g12.p; h->n_g12 = n_g12;
   D.tile_grp = h->d_tile_grp.p; D.obs = h->d_obs.p; D.obs_lm = h->d_obs_lm.p; D.lm_ptr = h->d_lm_ptr.p; D.obs_slot = h->d_obs_slot.p;
   D.imu = h->d_imu.p; D.imu_c = h->d_imu_c.p; D.imu_U = h->d_imu_U.p; D.prior_blk = h->d_prior_blk.p; D.prior_J = h->d_prior_J.p;
   D.prior_e0 = h->d_prior_e0.p; D.prior_A = h->d_prior_A.p; D.slot6 = h->d_slot6.p; D.z6 = h->d_z6.p; D.tilde6 = h->d_tilde6.p;
@@ -1507,7 +1543,7 @@ static void enqueue_linearize(d2ba_handle *h, int eval_cur) {
     launch_imu_lin(h->dev, eval_cur, h->n_imu_total, h->side);
     cudaEventRecord(h->ev_join, h->side);
   } else launch_imu_lin(h->dev, eval_cur, h->n_imu_total, h->stream);
-  for (int v = 0; v < 6; v++) launch_proj_lin(h->dev, v, eval_cur, h->job_begin[v], h->job_count[v], h->stream);
+  for (int v = 0; v < 8; v++) launch_proj_lin(h->dev, v, eval_cur, h->job_begin[v], h->job_count[v], h->stream);
   if (fork) cudaStreamWaitEvent(h->stream, h->ev_join, 0);
 }
 
@@ -1532,7 +1568,7 @@ static void enqueue_iteration(d2ba_handle *h) {
   // reads or writes: second lane
   const bool fork = h->two_lanes && h->sbe_smem > 0;
   if (fork) { cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0); launch_sb_elim(h->dev, h->sbe_smem, h->side); cudaEventRecord(h->ev_join, h->side); }
-  launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->stream);
+  launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->n_g12, h->stream);
   if (fork) cudaStreamWaitEvent(h->stream, h->ev_join, 0);
   else if (h->sbe_smem > 0) launch_sb_elim(h->dev, h->sbe_smem, h->stream);   // Y rows into Wt: the Schur kernels subtract them too
   enqueue_schur(h);
@@ -1740,9 +1776,13 @@ int d2ba_debug_linearize(d2ba_handle *h) {
   if (h->state_dirty) { int rc = upload_state(h); if (rc) return rc; }
   h->dev.prm.fixed_mode = 1; h->dev.prm.max_iter = 1;
   launch_tr_reset(h->dev, 1, h->stream);
+  if (h->any_admm) {   // ADMM terms as at the start of a solve (z = x, tilde = 0, references = state), not whatever the buffers held
+    launch_cons_init(h->dev, h->n6_total, h->stream);
+    launch_cons_refs(h->dev, h->nsb_total, h->nl_total, h->d_sb_win.p, h->d_lm_win.p, h->stream);
+  }
   enqueue_linearize(h, 1);
   launch_control(h->dev, 1, h->stream);
-  launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->stream);
+  launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->n_g12, h->stream);
   // debug view: the landmark-only Schur complement (eliminated speed-bias rows zeroed), kept un-factored in d_dbg
   if (h->sbe_smem > 0) launch_zero_sb_rows(h->dev, h->stream);
   if (h->n_leaf_total > 0) launch_zero_leaf_rows(h->dev, h->stream);
@@ -1997,7 +2037,7 @@ int d2ba_marginalize(d2ba_handle *h, int32_t window, int32_t n_remove, const int
   launch_tr_reset(t->dev, 1, t->stream);
   enqueue_linearize(t, 1);
   launch_control(t->dev, 1, t->stream);
-  launch_lm_gather(t->dev, t->d_lm_win.p, t->nl_total, t->max_row_tiles * 32, t->any_compact, t->any_wide, t->stream);
+  launch_lm_gather(t->dev, t->d_lm_win.p, t->nl_total, t->max_row_tiles * 32, t->any_compact, t->any_wide, t->n_g12, t->stream);
   if (t->max_ldw_small > 0) launch_schur_small(t->dev, t->max_ldw_small, t->stream);
   launch_schur(t->dev, t->d_schur.p, t->n_schur, t->stream);
   // eliminate the removed camera columns
@@ -2044,7 +2084,7 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
   cudaEventCreate(&evs[0]); cudaEventCreate(&evs[1]);
   for (int i = 0; i < 12; i++) ms_out[i] = 0;
   for (int it = 0; it < iters; it++) {
-    cudaEventRecord(ev[0], h->stream); launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->stream);
+    cudaEventRecord(ev[0], h->stream); launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->n_g12, h->stream);
     cudaEventRecord(evs[0], h->stream); if (h->sbe_smem > 0) launch_sb_elim(h->dev, h->sbe_smem, h->stream);
     cudaEventRecord(ev[1], h->stream);
     cudaEventRecord(evl[0], h->stream);
@@ -2056,7 +2096,7 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
     cudaEventRecord(evl[2], h->stream); if (h->n_leaf_total > 0) launch_leaf_back(h->dev, h->leafb_smem, h->stream);
     cudaEventRecord(ev[3], h->stream); launch_step(h->dev, h->max_nc, h->stream);
     cudaEventRecord(ev[4], h->stream); launch_misc_lin(h->dev, 0, h->max_prior_m, h->stream); launch_imu_lin(h->dev, 0, h->n_imu_total, h->stream);
-    cudaEventRecord(ev[5], h->stream); for (int v = 0; v < 6; v++) launch_proj_lin(h->dev, v, 0, h->job_begin[v], h->job_count[v], h->stream);
+    cudaEventRecord(ev[5], h->stream); for (int v = 0; v < 8; v++) launch_proj_lin(h->dev, v, 0, h->job_begin[v], h->job_count[v], h->stream);
     cudaEventRecord(ev[6], h->stream); launch_control(h->dev, 0, h->stream);
     cudaEventRecord(ev[7], h->stream);
     CK(cudaStreamSynchronize(h->stream));

@@ -705,14 +705,15 @@ template __global__ void k_proj_lin<4, 4>(Dev, int, int, int);
 #ifndef D2BA_PP_BLOCKS
 #define D2BA_PP_BLOCKS 4
 #endif
-// The 128-byte landmark records of a tile are staged in shared memory (16-byte units, XOR-swizzled) and written out four
-// whole records per store instruction: a lane storing its own record touched 32 different lines per instruction, eight
-// times per tile -- that, not DRAM, kept L1/TEX at 70 %.  The landmark index / inverse depth of the next tile are
+// The landmark records of a tile are staged in shared memory (16-byte units, swizzled) and written out whole records per
+// store instruction (four of 128 bytes, or five of 96 bytes in windows with rec_stride == 12): a lane storing its own
+// record touched 32 different lines per instruction, eight times per tile -- that, not DRAM, kept L1/TEX at 70 %.  The landmark index / inverse depth of the next tile are
 // fetched during the arithmetic and the DMMA pass of the current one.
 constexpr int kPpRows = 13;                          // staged Jacobian rows: 12 + residual (rows 13..15 of the MMA tile read as zero)
 constexpr int kPpWarpDoubles = GC_SIZE + kPpRows * (kTile * 2 + 4) + kTile * 16;
 static size_t proj_pp_smem() { return (size_t)4 * kPpWarpDoubles * 8; }
-template <bool SHIFT0>
+// REC12: the jobs' windows use 96-byte records (rec_stride == 12, decided per window at finalize); else rec_stride 16 / 32.
+template <bool SHIFT0, bool REC12>
 __global__ void __launch_bounds__(128, D2BA_PP_BLOCKS) k_proj_lin_pp(Dev d, int eval_cur, int job_begin, int job_count) {
   constexpr int LDJ = kTile * 2 + 4, RCOL = 12;
   extern __shared__ __align__(16) double sm[];
@@ -815,7 +816,17 @@ __global__ void __launch_bounds__(128, D2BA_PP_BLOCKS) k_proj_lin_pp(Dev d, int 
     Js[RCOL * LDJ + lane] = r0; Js[RCOL * LDJ + kTile + lane] = r1;
     // records are stored landmark-major (obs_slot: tile slot -> position in the landmark's run), so the per-landmark
     // reduction streams them; padding lanes (slot -1) never write
-    {
+    if (REC12) {
+      // 96-byte record {h, g, cols, a[0..5], b[0..2]}: a = pose_i's coupling block, b = pose_j's rotation entries (its
+      // position entries are -a[0..2]); [32 records][6 x 16 B], unit c of record r at r * 6 + (c + (r >> 2 & 1)) % 6
+      // (conflict-free: the eight lanes of a 16-byte phase hit eight different bank groups)
+      double2 *sr = stg + lane * 6;
+      const int rot = (lane >> 2) & 1;
+      sr[rot] = make_double2(jl[0] * jl[0] + jl[1] * jl[1], jl[0] * r0 + jl[1] * r1);
+      sr[1 + rot] = make_double2(__hiloint2double(g.slot_col[0], g.slot_col[1]), wi[0]);
+      sr[2 + rot] = make_double2(wi[1], wi[2]); sr[3 + rot] = make_double2(wi[3], wi[4]); sr[4 + rot] = make_double2(wi[5], wjr[0]);
+      sr[rot ? 0 : 5] = make_double2(wjr[1], wjr[2]);
+    } else {
       double2 *sr = stg + lane * 8;
       const int sw = lane & 7;
       sr[0 ^ sw] = make_double2(jl[0] * jl[0] + jl[1] * jl[1], jl[0] * r0 + jl[1] * r1);
@@ -828,17 +839,31 @@ __global__ void __launch_bounds__(128, D2BA_PP_BLOCKS) k_proj_lin_pp(Dev d, int 
     lam = lm >= 0 ? xlm[lm] : 1.0;                    // next tile's inverse depth: in flight during the MMA pass
     __syncwarp();
     {
-      // four whole records per store instruction: lanes 8k .. 8k+7 write the 128 contiguous bytes of record 4 j + k
       double *recs = d.rec[buf] + (size_t)w.off_rec;
-      const int c = lane & 7, stride = w.rec_stride;
+      if (REC12) {
+        // five whole records per store instruction: lanes 6k .. 6k+5 (k < 5) write the 96 contiguous bytes of record 5 j + k
+        const int k = lane / 6, c = lane - 6 * k;
 #pragma unroll
-      for (int j = 0; j < 8; j++) {
-        const int r = 4 * j + (lane >> 3);
-        const int slot = __shfl_sync(0xffffffffu, my_slot, r);
-        if (slot >= 0) {
-          double2 *dst = reinterpret_cast<double2 *>(recs + (size_t)slot * stride);
-          dst[c] = stg[r * 8 + (c ^ (r & 7))];
-          if (stride == 32 && c == 0) dst[14] = make_double2(__hiloint2double(-1, -1), __hiloint2double(-1, -1));
+        for (int j = 0; j < 7; j++) {
+          const int r = 5 * j + k;
+          const int slot = __shfl_sync(0xffffffffu, my_slot, r & 31);
+          if (k < 5 && r < kTile && slot >= 0) {
+            const int p = c + ((r >> 2) & 1);
+            reinterpret_cast<double2 *>(recs + (size_t)slot * 12)[c] = stg[r * 6 + (p == 6 ? 0 : p)];
+          }
+        }
+      } else {
+        // four whole records per store instruction: lanes 8k .. 8k+7 write the 128 contiguous bytes of record 4 j + k
+        const int c = lane & 7, stride = w.rec_stride;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          const int r = 4 * j + (lane >> 3);
+          const int slot = __shfl_sync(0xffffffffu, my_slot, r);
+          if (slot >= 0) {
+            double2 *dst = reinterpret_cast<double2 *>(recs + (size_t)slot * stride);
+            dst[c] = stg[r * 8 + (c ^ (r & 7))];
+            if (stride == 32 && c == 0) dst[14] = make_double2(__hiloint2double(-1, -1), __hiloint2double(-1, -1));
+          }
         }
       }
     }
@@ -879,8 +904,10 @@ __global__ void __launch_bounds__(128, D2BA_PP_BLOCKS) k_proj_lin_pp(Dev d, int 
     }
   }
 }
-template __global__ void k_proj_lin_pp<true>(Dev, int, int, int);
-template __global__ void k_proj_lin_pp<false>(Dev, int, int, int);
+template __global__ void k_proj_lin_pp<true, false>(Dev, int, int, int);
+template __global__ void k_proj_lin_pp<false, false>(Dev, int, int, int);
+template __global__ void k_proj_lin_pp<true, true>(Dev, int, int, int);
+template __global__ void k_proj_lin_pp<false, true>(Dev, int, int, int);
 
 // debug: raw (un-robustified) residual + full 3x26 Jacobian per observation tile slot
 __global__ void k_proj_debug(Dev d, double *out /*[tiles*32][81]*/, int n_tiles_total, const int *tile_win) {
@@ -978,7 +1005,7 @@ __global__ void __launch_bounds__(kGatherWarps * 32) k_lm_gather(Dev d, const in
   if (gl_idx >= n_lm_total) return;
   const int wi = lm_win[gl_idx];
   const WinDesc &w = d.win[wi];
-  if (w.rec_stride == 16) return;   // compact windows: k_lm_gather16
+  if (w.rec_stride != 32) return;   // compact windows: k_lm_gather16 / k_lm_gather12
   Ctl *ctl = d.ctl + wi;
   if (ctl->done || ctl->reuse) return;
   const int buf = ctl->cur;
@@ -1058,7 +1085,7 @@ __global__ void __launch_bounds__(kG16Lm * 16) k_lm_gather16(Dev d, const int *l
   if (gl_idx >= n_lm_total) return;
   const int wi = lm_win[gl_idx];
   const WinDesc &w = d.win[wi];
-  if (w.rec_stride != 16) return;
+  if (w.rec_stride != 16) return;   // 96-byte records: k_lm_gather12
   Ctl *ctl = d.ctl + wi;
   if (ctl->done || ctl->reuse) return;
   const int buf = ctl->cur;
@@ -1138,6 +1165,92 @@ __global__ void __launch_bounds__(kG16Lm * 16) k_lm_gather16(Dev d, const int *l
     d.hl[w.offlm + l] = h; d.gl[w.offlm + l] = g; d.dinv[w.offlm + l] = di; d.wu[w.offlm + l] = wu; d.D2l[w.offlm + l] = dl2;
     if (!(hp > 0.0)) ctl->chol_fail = 1;
     atomicMax(&ctl->gmax_l_bits, (unsigned long long)__double_as_longlong(fabs(g)));
+  }
+}
+
+// 96-byte-record windows (rec_stride == 12, host-checked: every residual is a two-free-pose factor of k_proj_lin_pp, no
+// leaves, per landmark one anchor column, pairwise distinct observing columns and at most 32 records).  A landmark's row
+// then has one summed block (the anchor's six columns, with h and g); every observing block comes from exactly one record.
+// One lane per record: a warp takes a host-built chunk of whole landmarks (Dev::g12_chunk: window, first, end landmark)
+// whose records fit in 32 lanes.  Lane j < #landmarks owns landmark l0 + j and sums h, g and the anchor block over its
+// records in record order (the order of k_lm_gather16, so these sums and the scaled row are bitwise the same); every
+// record lane stores its own observing block.  Row columns no record names are never written: they keep the zero of
+// the finalize-time memset.
+constexpr int kG12Warps = 8;
+__global__ void __launch_bounds__(kG12Warps * 32) k_lm_gather12(Dev d, int n_chunk) {
+  __shared__ double sv[kG12Warps][9][32];      // per record lane: h, g, a[0..5], observing block . u_c
+  __shared__ double sdi[kG12Warps][32];        // per record lane: 1/sqrt(h') of its landmark
+  __shared__ int srow[kG12Warps][32];          // per record lane: its landmark (window-local)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ci = blockIdx.x * kG12Warps + warp;
+  if (ci >= n_chunk) return;
+  const int4 ck = d.g12_chunk[ci];
+  Ctl *ctl = d.ctl + ck.x;
+  if (ctl->done || ctl->reuse) return;
+  const WinDesc &w = d.win[ck.x];
+  const int buf = ctl->cur;
+  const int *ptr = d.lm_ptr + w.off_lmptr;
+  const int nlm = ck.z - ck.y;
+  const int rb = lane <= nlm ? ptr[ck.y + lane] : 0;   // lane j <= nlm: first record of landmark l0 + j
+  const int r0 = __shfl_sync(0xffffffffu, rb, 0), nrec = __shfl_sync(0xffffffffu, rb, nlm) - r0;
+  const int re = __shfl_down_sync(0xffffffffu, rb, 1);
+  const double *uc = d.uc + w.offc;
+  double ob[6];
+  int ca = -1, cj = -1;
+  if (lane < nrec) {
+    const double2 *rp = reinterpret_cast<const double2 *>(d.rec[buf] + (size_t)w.off_rec + (size_t)(r0 + lane) * 12);
+    const double2 u0 = rp[0], u1 = rp[1], u2 = rp[2], u3 = rp[3], u4 = rp[4], u5 = rp[5];
+    ca = __double2hiint(u1.x); cj = __double2loint(u1.x);
+    ob[0] = -u1.y; ob[1] = -u2.x; ob[2] = -u2.y; ob[3] = u4.y; ob[4] = u5.x; ob[5] = u5.y;
+    double wp = 0.0;
+#pragma unroll
+    for (int k = 0; k < 6; k++) wp += ob[k] * uc[cj + k];
+    double *s = &sv[warp][0][lane];
+    s[0] = u0.x; s[32] = u0.y; s[64] = u1.y; s[96] = u2.x; s[128] = u2.y; s[160] = u3.x; s[192] = u3.y; s[224] = u4.x; s[256] = wp;
+  }
+  __syncwarp();
+  const int kb = lane < nlm ? rb - r0 : 0, ke = lane < nlm ? re - r0 : 0;
+  const int cal = __shfl_sync(0xffffffffu, ca, kb & 31);   // the landmark's anchor column (one per landmark, host-checked)
+  if (lane < nlm) {
+    const int l = ck.y + lane;
+    double h = 0, g = 0, a[6] = {0, 0, 0, 0, 0, 0}, wu = 0;
+    for (int k = kb; k < ke; k++) {
+      h += sv[warp][0][k]; g += sv[warp][1][k];
+#pragma unroll
+      for (int q = 0; q < 6; q++) a[q] += sv[warp][2 + q][k];
+      wu += sv[warp][8][k];
+    }
+    if (w.admm_on) {
+      const double rl = d.prm.rho_landmark;
+      h += rl * rl;
+      g += rl * rl * (d.xlm[buf][w.offlm + l] - d.lm_ref[w.offlm + l]);
+    }
+    const double dl2 = d2_of(h);
+    const double hp = h + ctl->mu * dl2;
+    const double di = 1.0 / sqrt(hp);
+    double *Wt = d.Wt + w.offW + (size_t)l * w.ldw;
+    Wt[w.n_lc] = g * di;
+    if (ke > kb) {
+#pragma unroll
+      for (int q = 0; q < 6; q++) { Wt[cal + q] = a[q] * di; wu += a[q] * uc[cal + q]; }
+    }
+    for (int k = kb; k < ke; k++) { sdi[warp][k] = di; srow[warp][k] = l; }
+    d.hl[w.offlm + l] = h; d.gl[w.offlm + l] = g; d.dinv[w.offlm + l] = di; d.wu[w.offlm + l] = wu; d.D2l[w.offlm + l] = dl2;
+    if (!(hp > 0.0)) ctl->chol_fail = 1;
+    atomicMax(&ctl->gmax_l_bits, (unsigned long long)__double_as_longlong(fabs(g)));
+  }
+  __syncwarp();
+  if (lane < nrec) {
+    const double di = sdi[warp][lane];
+    double *dst = d.Wt + w.offW + (size_t)srow[warp][lane] * w.ldw + cj;
+    // 0.0 + v: the row entry k_lm_gather16 forms from its zeroed row buffer (turns -0 into +0)
+    if ((cj & 1) == 0) {
+#pragma unroll
+      for (int k = 0; k < 3; k++) reinterpret_cast<double2 *>(dst)[k] = make_double2((0.0 + ob[2 * k]) * di, (0.0 + ob[2 * k + 1]) * di);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 6; k++) dst[k] = (0.0 + ob[k]) * di;
+    }
   }
 }
 
@@ -2836,16 +2949,15 @@ int configure_kernels(int max_rows, int max_nc, int max_prior_m) {
   e = raise_smem_limit(k_proj_lin<4, 2>, (size_t)(proj_smem<4, 2>())); if (e) return e;
   e = raise_smem_limit(k_proj_lin<2, 4>, (size_t)(proj_smem<2, 4>())); if (e) return e;
   e = raise_smem_limit(k_proj_lin<4, 4>, (size_t)(proj_smem<4, 4>())); if (e) return e;
-  e = raise_smem_limit(k_proj_lin_pp<true>, proj_pp_smem()); if (e) return e;
-  e = raise_smem_limit(k_proj_lin_pp<false>, proj_pp_smem()); if (e) return e;
+  e = raise_smem_limit(k_proj_lin_pp<true, false>, proj_pp_smem()); if (e) return e;
+  e = raise_smem_limit(k_proj_lin_pp<false, false>, proj_pp_smem()); if (e) return e;
+  e = raise_smem_limit(k_proj_lin_pp<true, true>, proj_pp_smem()); if (e) return e;
+  e = raise_smem_limit(k_proj_lin_pp<false, true>, proj_pp_smem()); if (e) return e;
   // 4 x 51 KB per SM needs the large shared-memory carveout
-  cudaFuncSetAttribute(k_proj_lin_pp<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(k_proj_lin_pp<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-#if D2BA_PP_BLOCKS > 4
-  // 37 KB per CTA: the large shared-memory carveout lets the register file, not the L1 split, set the occupancy
-  cudaFuncSetAttribute(k_proj_lin_pp<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(k_proj_lin_pp<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-#endif
+  cudaFuncSetAttribute(k_proj_lin_pp<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_proj_lin_pp<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_proj_lin_pp<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_proj_lin_pp<false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 
   size_t chol = (size_t)(kNB * (max_rows + 4) + 2 * max_rows + 16 + 16 * 32 + kNB * (kNB + 1)) * 8;
   e = raise_smem_limit(k_chol, (size_t)(chol)); if (e) return e;
@@ -2872,19 +2984,22 @@ void launch_proj_lin(const Dev &d, int variant, int eval_cur, int job_begin, int
     case 1: k_proj_lin<4, 2><<<grid, 128, proj_smem<4, 2>(), s>>>(d, eval_cur, job_begin, job_count); break;
     case 2: k_proj_lin<2, 4><<<grid, 128, proj_smem<2, 4>(), s>>>(d, eval_cur, job_begin, job_count); break;
     case 3: k_proj_lin<4, 4><<<grid, 128, proj_smem<4, 4>(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 4: k_proj_lin_pp<true><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 5: k_proj_lin_pp<false><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+    case 4: k_proj_lin_pp<true, false><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+    case 5: k_proj_lin_pp<false, false><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+    case 6: k_proj_lin_pp<true, true><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+    case 7: k_proj_lin_pp<false, true><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
   }
 }
 void launch_proj_debug(const Dev &d, double *out, int n_tiles, const int *tile_win, cudaStream_t s) {
   if (n_tiles > 0) k_proj_debug<<<n_tiles, 32, 0, s>>>(d, out, n_tiles, tile_win);
 }
-void launch_lm_gather(const Dev &d, const int *lm_win, int n_lm_total, int max_ldw, int any_compact, int any_wide, cudaStream_t s) {
+void launch_lm_gather(const Dev &d, const int *lm_win, int n_lm_total, int max_ldw, int any_compact, int any_wide, int n_chunk12, cudaStream_t s) {
   if (n_lm_total <= 0) return;
   if (any_wide)
     k_lm_gather<<<(n_lm_total + kGatherWarps - 1) / kGatherWarps, kGatherWarps * 32, (size_t)kGatherWarps * max_ldw * 8, s>>>(d, lm_win, n_lm_total, max_ldw);
   if (any_compact)
     k_lm_gather16<<<(n_lm_total + kG16Lm - 1) / kG16Lm, kG16Lm * 16, (size_t)kG16Lm * max_ldw * 8, s>>>(d, lm_win, n_lm_total, max_ldw);
+  if (n_chunk12 > 0) k_lm_gather12<<<(n_chunk12 + kG12Warps - 1) / kG12Warps, kG12Warps * 32, 0, s>>>(d, n_chunk12);
 }
 void launch_schur_small(const Dev &d, int max_ldw, cudaStream_t s) {
   k_schur_small<<<d.n_win, kSsThreads, (size_t)(2 * 32 * (max_ldw + 4) + 40) * 8, s>>>(d);

@@ -80,7 +80,7 @@ struct WinDesc {
   int off_tile, n_tile;
   int off_grp, n_grp;
   int off_imu, n_imu;
-  int rec_stride;              // doubles per landmark-side record (16 or 32)
+  int rec_stride;              // doubles per landmark-side record (12, 16 or 32)
   int64_t off_rec;             // offset of the window's records (doubles)
   int64_t offH;                // Hcc / S offset (doubles)
   int64_t offW;                // Wt offset (doubles)
@@ -172,6 +172,7 @@ struct Dev {
   const int *schur_chunks;
   const int *leaf_lm;
   const int *obs_slot;  // [T][32] position of the observation's record in its landmark's run (window-local), -1 = padding
+  const int4 *g12_chunk;  // k_lm_gather12 work list: {window, first landmark, end landmark, 0} (window-local), <= 32 records each
   // imu
   const ImuDesc *imu;
   const double *imu_c;  // [NIMU][kImuStride]
