@@ -22,7 +22,7 @@ TERM_NO_CONVERGENCE, TERM_FUNCTION_TOL, TERM_GRADIENT_TOL, TERM_PARAMETER_TOL, T
 
 # d2ba_debug_item
 (DBG_N_CAM, DBG_HCC, DBG_GC, DBG_HLL, DBG_GL, DBG_W, DBG_COST, DBG_S, DBG_N_LC, DBG_OBS_INDEX,
- DBG_COL_OF_BLOCK, DBG_PROJ_RESJAC, DBG_STEP, DBG_GN_STEP, DBG_IMU_RESJAC, DBG_CONS_RESJAC) = range(16)
+ DBG_COL_OF_BLOCK, DBG_PROJ_RESJAC, DBG_STEP, DBG_GN_STEP, DBG_IMU_RESJAC, DBG_CONS_RESJAC, DBG_SOLVE_PATH) = range(17)
 
 
 class Config(C.Structure):

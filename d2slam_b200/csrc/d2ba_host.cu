@@ -44,8 +44,13 @@ void launch_leaf_back(const Dev &d, size_t smem, cudaStream_t s);
 size_t leaf_back_smem(int n, int n_hub);
 int configure_leaf_back(size_t smem);
 void launch_zero_leaf_rows(const Dev &d, cudaStream_t s);
-void launch_schur_small(const Dev &d, int max_ldw, cudaStream_t s);
+void launch_schur_small(const Dev &d, int max_ldw, int with_fused, cudaStream_t s);
 int configure_schur_small(int max_ldw);
+bool solve_small_fits(int ldw);
+size_t solve_small_smem(int ldw, int n_lc, int n_c, int nb);
+int configure_solve_small(size_t smem);
+void launch_solve_small(const Dev &d, size_t smem, cudaStream_t s);
+int solve_small_occupancy(size_t smem);
 void launch_chol(const Dev &d, int max_rows, cudaStream_t s);
 size_t chol_smem_need(int n);
 int configure_chol_smem(int max_n);
@@ -76,6 +81,11 @@ void launch_prior_from_info(int n_win, int max_m, const int *m_of, const long lo
 }  // namespace d2ba
 
 using namespace d2ba;
+
+// k_solve_small is used when at least this many eligible windows per SM share a handle (see d2ba_finalize).  Tail of the
+// bench iteration in a graph replay, fused over separate kernels (H100 80GB HBM3, 700 W, tools/solve_tail_probe.py):
+// 1.29x at 1 window per SM, 1.11x at 2, 0.90x at 3, 0.84x at 4.
+constexpr int kFusedMinWindowsPerSM = 3;
 
 namespace {
 
@@ -284,6 +294,10 @@ struct d2ba_handle {
   int n_g12 = 0;                       // k_lm_gather12 chunks (windows with 96-byte records)
   size_t sbb_smem = 0, cfg_sbb_smem = 0;   // k_sb_back dynamic shared memory
   size_t sbe_smem = 0, cfg_sbe_smem = 0;   // speed-bias elimination: dynamic shared memory of k_sb_elim (0 = no window uses it)
+  // one-kernel reduced-system solve (k_solve_small) of the windows with WinDesc::fused_solve; the separate kernels are
+  // launched only when some window still needs them
+  int n_fused = 0; size_t fused_smem = 0, cfg_fused_smem = 0;
+  bool ss_unfused = false, cs_unfused = false, sbb_unfused = false;
   int64_t totLE = 0;
   DBuf<double> d_sbLE;
   int64_t totH = 0, totW = 0, totc = 0;
@@ -299,6 +313,7 @@ struct d2ba_handle {
   bool no_leaf = false;          // D2BA_NO_LEAF=1: keep remote-frame blocks in the dense part (A/B switch)
   bool no_sb_elim = false;       // D2BA_NO_SB_ELIM=1: keep the dense Cholesky of the whole reduced system (A/B switch for tests / profiling)
   bool rec128 = false;           // D2BA_REC128=1: 128-byte records and k_lm_gather16 in every window that would use 96-byte ones (A/B switch)
+  bool no_fused_solve = false;   // D2BA_NO_FUSED_SOLVE=1: the separate Schur / Cholesky / back-substitution / step kernels everywhere (A/B switch)
   double host_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // wall-clock phases of the last d2ba_finalize (d2ba_debug_host_times)
   double solve_ms[4] = {0, 0, 0, 0};             // host wall-clock of the last solve: enqueue, wait for the device, write-back
   std::atomic<long long> h2d_bytes_add;          // bytes d2ba_add_proj put on the copy stream since the last reset
@@ -374,6 +389,7 @@ int d2ba_create(const d2ba_config *cfg, d2ba_handle **out) {
   { const char *e = getenv("D2BA_NO_SB_ELIM"); h->no_sb_elim = e && e[0] == '1'; }
   { const char *e = getenv("D2BA_NO_LEAF"); h->no_leaf = e && e[0] == '1'; }
   { const char *e = getenv("D2BA_REC128"); h->rec128 = e && e[0] == '1'; }
+  { const char *e = getenv("D2BA_NO_FUSED_SOLVE"); h->no_fused_solve = e && e[0] == '1'; }
   h->cfg = *cfg;
   if (h->cfg.max_windows < 1) h->cfg.max_windows = 1;
   if (h->cfg.initial_trust_region_radius <= 0) h->cfg.initial_trust_region_radius = 1e4;
@@ -1135,6 +1151,8 @@ int d2ba_finalize(d2ba_handle *h) {
       d.sb_elim = ok ? 1 : 0;
       // the dense Cholesky only sees the hub of the pose part then: decide its kernel with that size
       if (ok || d.n_leaf > 0) d.chol_smem = (chol_smem_need(d.n_hub) <= (size_t)232448 - 16) ? 1 : 0;
+      // single-drone window whose whole reduced-system solve fits one CTA (k_solve_small)
+      d.fused_solve = (!h->no_fused_solve && d.n_leaf == 0 && d.sb_elim && d.schur_small && d.chol_smem && solve_small_fits(d.ldw)) ? 1 : 0;
       // rows of Wt the Schur kernels sum over: landmark rows, then the eliminated speed-bias rows, then the leaves' rows
       int rows = nl + (ok ? 9 * nb : 0);
       for (Leaf &lf : pl.leaves) { lf.row0 = rows; rows += lf.n; }
@@ -1208,10 +1226,20 @@ int d2ba_finalize(d2ba_handle *h) {
       if (!d.sb_elim) for (int tm = t_lo; tm <= t_hi; tm++) for (int tn = 0; tn <= tm; tn++) pl.schur[1].push_back(SchurTileH{wi, 1, tm, tn, 0, 0});
     }
   });
+  {   // k_solve_small pays off through the wave count: it runs each window with 4 warps where the separate kernels have 8,
+      // and wins only once those kernels need more than one wave (k_step: 3 CTAs per SM).  Smaller batches (the
+      // one-window latency case) keep the separate kernels.
+    int n_sm = 0;
+    if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->cfg.device) != cudaSuccess || n_sm < 1) n_sm = 1;
+    int n_elig = 0;
+    for (int wi = 0; wi < nw; wi++) n_elig += plan[wi].d.fused_solve;
+    if (n_elig < kFusedMinWindowsPerSM * n_sm) for (int wi = 0; wi < nw; wi++) plan[wi].d.fused_solve = 0;
+  }
   lap(0);
   // ---- serial prefix sums
   h->n_used = nw; h->max_rows = 1; h->max_nc = 1; h->max_prior_m = 0; h->max_ldw = 8; h->n_slots = 0; h->any_admm = false;
   h->max_row_tiles = 1; h->max_n_smem = 0; h->max_rows_glob = 1; h->any_chol_glob = false; h->max_ldw_small = 0; h->any_compact = h->any_wide = 0; h->sbe_smem = 0; h->sbb_smem = 0;
+  h->n_fused = 0; h->fused_smem = 0; h->ss_unfused = h->cs_unfused = h->sbb_unfused = false;
   int64_t offLE = 0;
   int off6 = 0, offsb = 0, offlm = 0, off_tile = 0, off_grp = 0, off_imu = 0, off_lmptr = 0, off_pblk = 0, n_schur = 0, n_sch[2] = {0, 0}, n_chunks = 0, off_leaf = 0, off_hseg = 0, n_leaf_lm = 0;
   int64_t offLL = 0; size_t leaf_smem = 0, leafb_smem = 0; int max_hub = 0, n_g12 = 0;
@@ -1249,6 +1277,12 @@ int d2ba_finalize(d2ba_handle *h) {
     }
     { const int ndense = (d.sb_elim || d.n_leaf > 0) ? d.n_hub : d.n_c;
       if (d.chol_smem) h->max_n_smem = std::max(h->max_n_smem, ndense); else { h->any_chol_glob = true; h->max_rows_glob = std::max(h->max_rows_glob, ndense + 1); } }
+    if (d.fused_solve) { h->n_fused++; h->fused_smem = std::max(h->fused_smem, solve_small_smem(d.ldw, d.n_lc, d.n_c, d.n_sbe)); }
+    else {
+      if (d.schur_small || d.hub_small) h->ss_unfused = true;
+      if (d.chol_smem) h->cs_unfused = true;
+      if (d.sb_elim) h->sbb_unfused = true;
+    }
     if (w.admm) {
       if (h->any_admm && h->n_slots != w.n_slots) return fail(h, 26, "finalize: every window of a handle must name the same n_slots_global (the all-reduce count)");
       h->any_admm = true; h->n_slots = w.n_slots;
@@ -1426,7 +1460,7 @@ int d2ba_finalize(d2ba_handle *h) {
   D.win = h->d_win.p; D.ctl = h->d_ctl.p; D.n_win = nw;
   for (int b = 0; b < 2; b++) { D.x6[b] = h->d_x6[b].p; D.R6[b] = h->d_R6[b].p; D.xsb[b] = h->d_xsb[b].p; D.xlm[b] = h->d_xlm[b].p; D.xtd[b] = h->d_xtd[b].p; D.rec[b] = h->d_rec[b].p; D.Hcc[b] = h->d_H[b].p; D.gc[b] = h->d_gc[b].p; }
   D.col6 = h->d_col6.p; D.colsb = h->d_colsb.p; D.grp = h->d_grp.p; D.job = h->d_job.p; D.n_job = n_jobs;
-  D.lm_mask = h->d_lm_mask.p; D.hseg = h->d_hseg.p; D.leaf = h->d_leaf.p; D.n_leaf_total = h->n_leaf_total; { int np_ = 0; for (int q = 0; q < nw; q++) if (plan[q].d.n_leaf == 0) np_++; D.n_plain_win = np_; } D.leafL = h->d_leafL.p; D.schur_chunks = h->d_schur_chunks.p; D.leaf_lm = h->d_leaf_lm.p;
+  D.lm_mask = h->d_lm_mask.p; D.hseg = h->d_hseg.p; D.leaf = h->d_leaf.p; D.n_leaf_total = h->n_leaf_total; { int np_ = 0; for (int q = 0; q < nw; q++) if (plan[q].d.n_leaf == 0 && !plan[q].d.fused_solve) np_++; D.n_plain_win = np_; } D.leafL = h->d_leafL.p; D.schur_chunks = h->d_schur_chunks.p; D.leaf_lm = h->d_leaf_lm.p;
   D.g12_chunk = h->d_g12.p; h->n_g12 = n_g12;
   D.tile_grp = h->d_tile_grp.p; D.obs = h->d_obs.p; D.obs_lm = h->d_obs_lm.p; D.lm_ptr = h->d_lm_ptr.p; D.obs_slot = h->d_obs_slot.p;
   D.imu = h->d_imu.p; D.imu_c = h->d_imu_c.p; D.imu_U = h->d_imu_U.p; D.prior_blk = h->d_prior_blk.p; D.prior_J = h->d_prior_J.p;
@@ -1472,6 +1506,10 @@ int d2ba_finalize(d2ba_handle *h) {
   if (h->max_n_smem > 0 && h->cfg_max_n_smem != h->max_n_smem) {
     if (configure_chol_smem(h->max_n_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_chol_smem) failed");
     h->cfg_max_n_smem = h->max_n_smem;
+  }
+  if (h->fused_smem > 0 && h->cfg_fused_smem < h->fused_smem) {
+    if (configure_solve_small(h->fused_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_solve_small) failed");
+    h->cfg_fused_smem = h->fused_smem;
   }
   launch_state_prep(D, h->n6_total, 0, h->stream);
   launch_imu_prep(D, h->d_imu_pk.p, h->d_imu_c.p, h->n_imu_total, h->stream);
@@ -1552,15 +1590,20 @@ static void enqueue_schur(d2ba_handle *h) {
   // (the leaf kernel forms its own part of the reduced system from Hcc and its landmarks' rows: the stage-0 tiles are
   //  only launched for the debug view of S)
   if (h->n_leaf_total > 0) launch_leaf_elim(h->dev, h->leaf_smem, h->stream);
-  if (h->max_ldw_small > 0) launch_schur_small(h->dev, h->max_ldw_small, h->stream);
+  if (h->ss_unfused) launch_schur_small(h->dev, h->max_ldw_small, 0, h->stream);
   if (h->n_schur > h->n_schur0) launch_schur(h->dev, h->d_schur.p + h->n_schur0, h->n_schur - h->n_schur0, h->stream);
 }
 // dense Cholesky of the hub, then the eliminated parts' back substitutions
 static void enqueue_solve_reduced(d2ba_handle *h) {
-  if (h->max_n_smem > 0) launch_chol_smem(h->dev, h->max_n_smem, h->stream);
+  if (h->cs_unfused) launch_chol_smem(h->dev, h->max_n_smem, h->stream);
   if (h->any_chol_glob) launch_chol(h->dev, h->max_rows_glob, h->stream);
-  if (h->sbe_smem > 0) launch_sb_back(h->dev, h->sbb_smem, h->stream);
+  if (h->sbb_unfused) launch_sb_back(h->dev, h->sbb_smem, h->stream);
   if (h->n_leaf_total > 0) launch_leaf_back(h->dev, h->leafb_smem, h->stream);
+}
+// the step: k_solve_small does the whole reduced-system solve and the step of its windows, k_step the others'
+static void enqueue_step(d2ba_handle *h) {
+  if (h->n_fused > 0) launch_solve_small(h->dev, h->fused_smem, h->stream);
+  launch_step(h->dev, h->max_nc, h->stream);
 }
 
 static void enqueue_iteration(d2ba_handle *h) {
@@ -1573,7 +1616,7 @@ static void enqueue_iteration(d2ba_handle *h) {
   else if (h->sbe_smem > 0) launch_sb_elim(h->dev, h->sbe_smem, h->stream);   // Y rows into Wt: the Schur kernels subtract them too
   enqueue_schur(h);
   enqueue_solve_reduced(h);
-  launch_step(h->dev, h->max_nc, h->stream);
+  enqueue_step(h);
   enqueue_linearize(h, 0);
   launch_control(h->dev, 0, h->stream);
 }
@@ -1786,7 +1829,7 @@ int d2ba_debug_linearize(d2ba_handle *h) {
   // debug view: the landmark-only Schur complement (eliminated speed-bias rows zeroed), kept un-factored in d_dbg
   if (h->sbe_smem > 0) launch_zero_sb_rows(h->dev, h->stream);
   if (h->n_leaf_total > 0) launch_zero_leaf_rows(h->dev, h->stream);
-  if (h->max_ldw_small > 0) launch_schur_small(h->dev, h->max_ldw_small, h->stream);
+  if (h->max_ldw_small > 0) launch_schur_small(h->dev, h->max_ldw_small, 1, h->stream);   // k_solve_small's windows too
   launch_schur(h->dev, h->d_schur.p, h->n_schur, h->stream);   // both stages back to back: no eliminated rows in this view
   CK(h->d_dbg.alloc((size_t)h->totH));
   CK(cudaMemcpyAsync(h->d_dbg.p, h->d_S.p, (size_t)h->totH * 8, cudaMemcpyDeviceToDevice, h->stream));
@@ -1795,7 +1838,7 @@ int d2ba_debug_linearize(d2ba_handle *h) {
     enqueue_schur(h);
   }
   enqueue_solve_reduced(h);
-  launch_step(h->dev, h->max_nc, h->stream);
+  enqueue_step(h);   // the fused solve the iteration runs: DBG_GN_STEP / DBG_STEP show what it computed
   CK(cudaMemcpyAsync(h->h_ctl.p, h->d_ctl.p, sizeof(Ctl) * h->n_used, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   CK(cudaGetLastError());
@@ -1818,6 +1861,7 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
   switch (item) {
     case D2BA_DBG_N_CAM: { int64_t v = n; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
     case D2BA_DBG_N_LC: { int64_t v = nlc; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
+    case D2BA_DBG_SOLVE_PATH: { int64_t v = d.fused_solve ? 1 : 0; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
     case D2BA_DBG_HCC: {   // Hcc is stored lower-triangular in device column order: symmetric, canonical order out
       auto H = fetch(h->d_H[cur].p + d.offH, (size_t)n * ld);
       std::vector<double> o((size_t)n * n);
@@ -2038,7 +2082,7 @@ int d2ba_marginalize(d2ba_handle *h, int32_t window, int32_t n_remove, const int
   enqueue_linearize(t, 1);
   launch_control(t->dev, 1, t->stream);
   launch_lm_gather(t->dev, t->d_lm_win.p, t->nl_total, t->max_row_tiles * 32, t->any_compact, t->any_wide, t->n_g12, t->stream);
-  if (t->max_ldw_small > 0) launch_schur_small(t->dev, t->max_ldw_small, t->stream);
+  if (t->max_ldw_small > 0) launch_schur_small(t->dev, t->max_ldw_small, 1, t->stream);
   launch_schur(t->dev, t->d_schur.p, t->n_schur, t->stream);
   // eliminate the removed camera columns
   DBuf<int> d_keep, d_rem, d_flag; DBuf<double> d_A, d_b;
@@ -2066,7 +2110,21 @@ int d2ba_marginalize(d2ba_handle *h, int32_t window, int32_t n_remove, const int
 // Per-kernel device time of the iteration sequence (CUDA events on the solver stream, no graph):
 // ms_out[0..6] = lm_gather, schur, chol, step, misc_lin, proj_lin, control, summed over `iters` iterations;
 // ms_out[7] = number of iterations timed; ms_out[8], [9] = the speed-bias elimination / back-substitution share of the
-// chol bucket.  Used by bench.py for the roofline of the dominant kernel.
+// chol bucket.  Used by bench.py for the roofline of the dominant kernel.  k_solve_small (the whole reduced-system
+// solve and step of the windows with fused_solve) is timed in the step bucket; the schur, chol and back-substitution
+// buckets then hold only the other windows' kernels.
+int d2ba_debug_solve_occupancy(d2ba_handle *h, int32_t *ctas_per_sm) {
+  if (!h || !ctas_per_sm) return 1;
+  cudaSetDevice(h->cfg.device);
+  if (!h->finalized) { int rc = d2ba_finalize(h); if (rc) return rc; }
+  *ctas_per_sm = 0;
+  if (h->n_fused == 0) return 0;
+  const int n = solve_small_occupancy(h->fused_smem);
+  if (n < 0) return fail(h, 5, "cudaOccupancyMaxActiveBlocksPerMultiprocessor(k_solve_small) failed");
+  *ctas_per_sm = n;
+  return 0;
+}
+
 int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
   if (!h) return 1;
   cudaSetDevice(h->cfg.device);
@@ -2090,11 +2148,11 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
     cudaEventRecord(evl[0], h->stream);
     if (h->n_leaf_total > 0) launch_leaf_elim(h->dev, h->leaf_smem, h->stream);
     cudaEventRecord(evl[1], h->stream);
-    if (h->max_ldw_small > 0) launch_schur_small(h->dev, h->max_ldw_small, h->stream);
+    if (h->ss_unfused) launch_schur_small(h->dev, h->max_ldw_small, 0, h->stream);
     if (h->n_schur > h->n_schur0) launch_schur(h->dev, h->d_schur.p + h->n_schur0, h->n_schur - h->n_schur0, h->stream);
-    cudaEventRecord(ev[2], h->stream); if (h->max_n_smem > 0) launch_chol_smem(h->dev, h->max_n_smem, h->stream); if (h->any_chol_glob) launch_chol(h->dev, h->max_rows_glob, h->stream); cudaEventRecord(evs[1], h->stream); if (h->sbe_smem > 0) launch_sb_back(h->dev, h->sbb_smem, h->stream);
+    cudaEventRecord(ev[2], h->stream); if (h->cs_unfused) launch_chol_smem(h->dev, h->max_n_smem, h->stream); if (h->any_chol_glob) launch_chol(h->dev, h->max_rows_glob, h->stream); cudaEventRecord(evs[1], h->stream); if (h->sbb_unfused) launch_sb_back(h->dev, h->sbb_smem, h->stream);
     cudaEventRecord(evl[2], h->stream); if (h->n_leaf_total > 0) launch_leaf_back(h->dev, h->leafb_smem, h->stream);
-    cudaEventRecord(ev[3], h->stream); launch_step(h->dev, h->max_nc, h->stream);
+    cudaEventRecord(ev[3], h->stream); enqueue_step(h);
     cudaEventRecord(ev[4], h->stream); launch_misc_lin(h->dev, 0, h->max_prior_m, h->stream); launch_imu_lin(h->dev, 0, h->n_imu_total, h->stream);
     cudaEventRecord(ev[5], h->stream); for (int v = 0; v < 8; v++) launch_proj_lin(h->dev, v, 0, h->job_begin[v], h->job_count[v], h->stream);
     cudaEventRecord(ev[6], h->stream); launch_control(h->dev, 0, h->stream);

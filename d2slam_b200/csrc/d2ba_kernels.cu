@@ -10,6 +10,7 @@
 //   k_schur           S = Hcc + mu D^2 - Wt^T Wt  (fp64 tensor-core SYRK) + bordered rhs row
 //   k_chol            blocked bordered Cholesky + back substitution        (one CTA / window)
 //   k_step            landmark back-substitution, Cauchy point, dogleg, retraction
+//   k_solve_small     Schur + Cholesky + speed-bias back-substitution + step of a single-drone window in one CTA
 //   k_control         accept / reject, radius, convergence
 //   k_cons_*          ADMM consensus pack / apply
 #include <cuda_runtime.h>
@@ -1356,12 +1357,22 @@ __global__ void __launch_bounds__(128) k_schur(Dev d, const SchurTile *tiles) {
 // The Wt chunk is staged once per 32 landmarks and shared by all blocks; each warp owns up to kSsMaxB blocks.
 constexpr int kSsThreads = 256;
 constexpr int kSsMaxB = 10;   // 12*13/2 = 78 lower blocks over 8 warps
-__global__ void __launch_bounds__(kSsThreads, 2) k_schur_small(Dev d) {
-  const int wi = blockIdx.x;
+// Dispatch to f(integral_constant<Q>) for the run-time nq in [1, MAXB] (nothing for 0).
+template <int Q, int MAXB, class F>
+D2BA_DEV void dispatch_nq(int nq, F &&f) {
+  if constexpr (Q <= MAXB) {
+    if (nq == Q) f(std::integral_constant<int, Q>());
+    else dispatch_nq<Q + 1, MAXB>(nq, f);
+  }
+}
+// Body shared by k_schur_small and k_solve_small: NT threads, each warp owns up to MAXB of the 8x8 blocks (the host keeps
+// the block count <= MAXB * NT / 32).  The reduced system goes to S with leading dimension lds (global S, or the matrix of
+// the shared-memory Cholesky); the staging buffers live at sm.  Returns this window's share of u^T H u in every thread.
+template <int NT, int MAXB>
+D2BA_DEV double schur_small_body(const Dev &d, int wi, double *sm, double *redq, double *Sg, int lds) {
+  constexpr int NW = NT / 32;
   const WinDesc &w = d.win[wi];
-  if (!w.schur_small && !w.hub_small) return;
-  Ctl *ctl = d.ctl + wi;
-  if (ctl->done || ctl->reuse) return;
+  const Ctl *ctl = d.ctl + wi;
   const int buf = ctl->cur;
   // window of W-space columns this kernel forms: everything (single-drone window) or the hub [hub0, n_lc] behind the leaves;
   // below, nlc / ldw / the pointers are all relative to that window
@@ -1371,27 +1382,25 @@ __global__ void __launch_bounds__(kSsThreads, 2) k_schur_small(Dev d) {
   const double *H = d.Hcc[buf] + w.offH + (size_t)c0 * ld + c0;
   const double *gcv = d.gc[buf] + w.offc + c0;
   const double *ucv = d.uc + w.offc + c0, *D2v = d.D2c + w.offc + c0;
-  double *S = d.S + w.offH + (size_t)c0 * ld + c0;
+  double *S = Sg;
   const double *Wt = d.Wt + w.offW + c0;
-  extern __shared__ double sm[];
   const int ldws = ldw + 4;
   double *Ws = sm;                            // 2 buffers x 32 x ldws (TMA bulk staged)
-  double *redq = sm + 2 * 32 * ldws;          // 40
   __shared__ unsigned long long bar[2];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, kq = lane & 3, cr = lane >> 2;
   const int nb8 = ldw >> 3, nblk = nb8 * (nb8 + 1) / 2;
-  int bi[kSsMaxB], bj[kSsMaxB];
-  double acc[kSsMaxB][2];
+  int bi[MAXB], bj[MAXB];
+  double acc[MAXB][2];
 #pragma unroll
-  for (int q = 0; q < kSsMaxB; q++) {
-    int t = warp + q * 8;
+  for (int q = 0; q < MAXB; q++) {
+    int t = warp + q * NW;
     int i = (int)((sqrtf(8.0f * t + 1.0f) - 1.0f) * 0.5f);
     while ((i + 1) * (i + 2) / 2 <= t) i++;
     while (i * (i + 1) / 2 > t) i--;
     bi[q] = i; bj[q] = t - i * (i + 1) / 2;
     acc[q][0] = 0.0; acc[q][1] = 0.0;
   }
-  const int nq = warp < nblk ? (nblk - 1 - warp) / 8 + 1 : 0;   // blocks owned by this warp (t = warp, warp + 8, ...)
+  const int nq = warp < nblk ? (nblk - 1 - warp) / NW + 1 : 0;   // blocks owned by this warp (t = warp, warp + NW, ...)
   double uhu = 0.0;
   if (nlc > 0) {
     const int nchunk = w.wt_rows / 32;   // landmark rows, then the eliminated speed-bias rows Y
@@ -1424,25 +1433,14 @@ __global__ void __launch_bounds__(kSsThreads, 2) k_schur_small(Dev d) {
           for (int q = 0; q < nq_c; q++) dmma(acc[q][0], acc[q][1], fa[q], fb[q]);
         }
       };
-      switch (nq) {
-        case 1: body(std::integral_constant<int, 1>()); break;
-        case 2: body(std::integral_constant<int, 2>()); break;
-        case 3: body(std::integral_constant<int, 3>()); break;
-        case 4: body(std::integral_constant<int, 4>()); break;
-        case 5: body(std::integral_constant<int, 5>()); break;
-        case 6: body(std::integral_constant<int, 6>()); break;
-        case 7: body(std::integral_constant<int, 7>()); break;
-        case 8: body(std::integral_constant<int, 8>()); break;
-        case 9: body(std::integral_constant<int, 9>()); break;
-        case 10: body(std::integral_constant<int, 10>()); break;
-        default: break;
-      }
+      dispatch_nq<1, MAXB>(nq, body);
       __syncthreads();
       if (tid == 0 && c + 2 < nchunk) { fence_proxy_async(); issue(c + 2, b); }
     }
+    // (every warp is past its last read of the staging buffers: S may overwrite them when it lives in shared memory)
 #pragma unroll
-    for (int q = 0; q < kSsMaxB; q++) {
-      if (warp + q * 8 >= nblk) continue;
+    for (int q = 0; q < MAXB; q++) {
+      if (warp + q * NW >= nblk) continue;
 #pragma unroll
       for (int e = 0; e < 2; e++) {
         const int m = bi[q] * 8 + cr, c = bj[q] * 8 + kq * 2 + e;
@@ -1451,9 +1449,9 @@ __global__ void __launch_bounds__(kSsThreads, 2) k_schur_small(Dev d) {
           double hv = H[(size_t)m * ld + c];
           uhu += (m == c ? 1.0 : 2.0) * hv * ucv[m] * ucv[c];
           if (m == c) hv += mu * D2v[m];
-          S[(size_t)m * ld + c] = hv - v;
+          S[(size_t)m * lds + c] = hv - v;
         } else if (m == nlc && c < nlc) {
-          S[(size_t)(w.sb_elim ? nlc : n) * ld + c] = gcv[c] - v;   // rhs row of the system the Cholesky will see
+          S[(size_t)(w.sb_elim ? nlc : n) * lds + c] = gcv[c] - v;   // rhs row of the system the Cholesky will see
         }
       }
     }
@@ -1461,17 +1459,31 @@ __global__ void __launch_bounds__(kSsThreads, 2) k_schur_small(Dev d) {
   // rows of the speed-bias part (no landmark coupling) and the rest of the rhs row; when the shared-memory
   // Cholesky owns this window it reads them straight from Hcc instead (saves the copy through S)
   const int nrow = (w.chol_smem || w.sb_elim) ? 0 : n - nlc;
-  for (int e = tid; e < nrow * n; e += kSsThreads) {
+  for (int e = tid; e < nrow * n; e += NT) {
     const int i = nlc + e / n, j = e % n;
     if (j > i) continue;
     double v = H[(size_t)i * ld + j];
     uhu += (i == j ? 1.0 : 2.0) * v * ucv[i] * ucv[j];
     if (i == j) v += mu * D2v[i];
-    S[(size_t)i * ld + j] = v;
+    S[(size_t)i * lds + j] = v;
   }
-  if (!w.chol_smem && !w.sb_elim) for (int j = nlc + tid; j < n; j += kSsThreads) S[(size_t)n * ld + j] = gcv[j];
-  uhu = block_sum(uhu, redq);
-  if (tid == 0) atomicAdd(&ctl->uHu_cam, uhu);
+  if (!w.chol_smem && !w.sb_elim) for (int j = nlc + tid; j < n; j += NT) S[(size_t)n * lds + j] = gcv[j];
+  return block_sum(uhu, redq);
+}
+
+// with_fused: also the windows k_solve_small owns (the debug view of the un-factored S)
+__global__ void __launch_bounds__(kSsThreads, 2) k_schur_small(Dev d, int with_fused) {
+  const int wi = blockIdx.x;
+  const WinDesc &w = d.win[wi];
+  if (!w.schur_small && !w.hub_small) return;
+  if (w.fused_solve && !with_fused) return;
+  Ctl *ctl = d.ctl + wi;
+  if (ctl->done || ctl->reuse) return;
+  extern __shared__ double sm[];
+  const int c0 = w.hub_small ? w.hub0 : 0, ldw = w.hub_small ? ((w.n_lc - c0 + 1 + 7) & ~7) : w.ldw;
+  double *redq = sm + 2 * 32 * (ldw + 4);   // 40, behind the staging buffers
+  const double uhu = schur_small_body<kSsThreads, kSsMaxB>(d, wi, sm, redq, d.S + w.offH + (size_t)c0 * w.ldh + c0, w.ldh);
+  if (threadIdx.x == 0) atomicAdd(&ctl->uHu_cam, uhu);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1737,13 +1749,12 @@ D2BA_DEV void chol_tile8(double *A, int ld, const double *P, int ldp, int gi0, i
   }
 }
 
-__global__ void __launch_bounds__(kCsThreads) k_chol_smem(Dev d) {
-  const int wi = blockIdx.x;
+// Body shared by k_chol_smem and k_solve_small.  in_smem: the bordered matrix is already at sm (k_solve_small's Schur
+// phase wrote it there), skip the load.  Returns true (in every thread) on a bad pivot, after setting ctl->chol_fail;
+// otherwise the pose part of the GN step is in gn_c.
+D2BA_DEV bool chol_smem_body(const Dev &d, int wi, double *sm, bool in_smem) {
   const WinDesc &w = d.win[wi];
-  if (!w.chol_smem) return;
   Ctl *ctl = d.ctl + wi;
-  if (ctl->done || ctl->reuse || ctl->chol_fail) return;
-  extern __shared__ __align__(16) double sm[];
   // after the speed-bias elimination (k_sb_elim + Schur) only the landmark-coupled part is left: S rows 0..n_lc (rhs)
   // ... and after the leaf elimination only the hub [hub0, n_lc) of it
   const bool reduced = w.sb_elim != 0 || w.n_leaf > 0;
@@ -1769,7 +1780,7 @@ __global__ void __launch_bounds__(kCsThreads) k_chol_smem(Dev d) {
   // load the lower triangle (+ rhs row) with one TMA bulk copy per row, all in flight at once.  Rows of the
   // landmark-coupled part come from the Schur kernel's S; when that was the one-CTA kernel the speed-bias rows are
   // taken from Hcc directly (+ mu D^2 on the diagonal, added below) and their share of u^T H u is accumulated here.
-  {
+  if (!in_smem) {
     __shared__ __align__(8) unsigned long long bar;
     const int nlc = w.n_lc, cur = ctl->cur;
     const bool direct = !reduced && w.schur_small != 0;
@@ -1869,7 +1880,7 @@ __global__ void __launch_bounds__(kCsThreads) k_chol_smem(Dev d) {
     __syncthreads();
     TLAP(6);
   }
-  if (fail) { if (tid == 0) ctl->chol_fail = 1; return; }
+  if (fail) { if (tid == 0) ctl->chol_fail = 1; return true; }
   // ---- back substitution L^T x = y (y = row n), 32-column blocks from the end
   double *xs = P;                 // n
   double *redb = P + n + 1;       // 16 x 32
@@ -1913,6 +1924,17 @@ __global__ void __launch_bounds__(kCsThreads) k_chol_smem(Dev d) {
     printf("chol timing tid %d n %d: load %lld diag0 %lld trsm %lld trsm_bar %lld look+bar %lld work3b %lld bar3b %lld back_partial %lld back_tri %lld tail %lld\n", tid, n,
            tk[0], tk[1], tk[2], tk[3], tk[4], tk[5], tk[6], tk[7], tk[8], tk[9]);
 #endif
+  return false;
+}
+
+__global__ void __launch_bounds__(kCsThreads) k_chol_smem(Dev d) {
+  const int wi = blockIdx.x;
+  const WinDesc &w = d.win[wi];
+  if (!w.chol_smem || w.fused_solve) return;
+  const Ctl *ctl = d.ctl + wi;
+  if (ctl->done || ctl->reuse || ctl->chol_fail) return;
+  extern __shared__ __align__(16) double sm[];
+  chol_smem_body(d, wi, sm, false);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2132,13 +2154,9 @@ __global__ void __launch_bounds__(kSeThreads, 4) k_sb_elim(Dev d) {
 // warp 0 then runs the short recursion out of shared memory.
 constexpr int kSbBackThreads = 256;
 __host__ __device__ inline size_t sb_back_smem_bytes(int nlc, int nb) { return (size_t)(((nlc + 31) & ~31) + 9 * nb + 171 * nb) * 8; }
-__global__ void __launch_bounds__(kSbBackThreads) k_sb_back(Dev d) {
-  const int wi = blockIdx.x;
+// Body shared by k_sb_back and k_solve_small (gn_c holds the pose part of the step).
+D2BA_DEV void sb_back_body(const Dev &d, int wi, double *sm) {
   const WinDesc &w = d.win[wi];
-  if (!w.sb_elim) return;
-  Ctl *ctl = d.ctl + wi;
-  if (ctl->done || ctl->reuse || ctl->chol_fail) return;
-  extern __shared__ double sm[];
   const int c0 = w.hub0, nh = w.n_lc - c0, nlc = w.n_lc, nb = w.n_sbe, ldy = w.ldw;   // Y lives in the hub columns [hub0, n_lc] of its rows
   double *xp = sm;                       // n_hub (padded to 32)
   double *rhs = sm + ((nh + 31) & ~31);  // 9 nb : z - Y x_p
@@ -2194,6 +2212,16 @@ __global__ void __launch_bounds__(kSbBackThreads) k_sb_back(Dev d) {
     xn = x;
     if (lane < 9) gn[nlc + 9 * k + lane] = -x;
   }
+}
+
+__global__ void __launch_bounds__(kSbBackThreads) k_sb_back(Dev d) {
+  const int wi = blockIdx.x;
+  const WinDesc &w = d.win[wi];
+  if (!w.sb_elim || w.fused_solve) return;
+  const Ctl *ctl = d.ctl + wi;
+  if (ctl->done || ctl->reuse || ctl->chol_fail) return;
+  extern __shared__ double sm[];
+  sb_back_body(d, wi, sm);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2443,14 +2471,11 @@ __global__ void k_zero_leaf_rows(Dev d) {
 // ------------------------------------------------------------------------------------------------
 // Step kernel: one CTA per window.
 constexpr int kStepThreads = 256;
+// Body shared by k_step and k_solve_small; sm holds 40 + 3 max_nc doubles.
 template <bool LEAF>   // LEAF: windows with leaves (block-sparse landmark rows); the other instantiation handles the dense rows
-__global__ void __launch_bounds__(kStepThreads, LEAF ? 4 : 3) k_step(Dev d, int max_nc) {
-  const int wi = blockIdx.x;
+D2BA_DEV void step_body(const Dev &d, int wi, double *sm, int max_nc) {
   const WinDesc &w = d.win[wi];
-  if ((w.n_leaf != 0) != LEAF) return;
   Ctl *ctl = d.ctl + wi;
-  if (ctl->done) return;
-  extern __shared__ double sm[];
   double *red = sm;               // 40
   double *uc = sm + 40;           // n_c : g / D^2
   double *dcs = uc + max_nc;      // n_c : GN camera step
@@ -2606,6 +2631,58 @@ __global__ void __launch_bounds__(kStepThreads, LEAF ? 4 : 3) k_step(Dev d, int 
     ctl->x_norm2 = xn; ctl->dx_norm2 = dxn; ctl->model_change = model_change; ctl->step_norm = step_norm;
     ctl->step_valid = 1; ctl->cand_cost_proj = 0.0; ctl->cand_cost_misc = 0.0;
   }
+}
+
+template <bool LEAF>
+__global__ void __launch_bounds__(kStepThreads, LEAF ? 4 : 3) k_step(Dev d, int max_nc) {
+  const int wi = blockIdx.x;
+  const WinDesc &w = d.win[wi];
+  if ((w.n_leaf != 0) != LEAF) return;
+  if (!LEAF && w.fused_solve) return;
+  if (d.ctl[wi].done) return;
+  extern __shared__ double sm[];
+  step_body<LEAF>(d, wi, sm, max_nc);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Reduced-system solve of a single-drone window in one CTA (WinDesc::fused_solve: no leaves, speed-bias elimination,
+// one-CTA Schur and shared-memory Cholesky, at most kSolveMaxB 8x8 blocks per warp).  The four phases are the bodies of
+// k_schur_small -> k_chol_smem -> k_sb_back -> k_step<false>, back to back on one window:
+//   (1) Schur: S = Hcc_pp + mu D^2 - Wt^T Wt - Y^T Y and its rhs row, written straight into the shared-memory matrix of
+//       the Cholesky (the Wt staging buffers and that matrix are never live together and share one region);
+//   (2) bordered Cholesky + back substitution in place: pose part of the GN step;
+//   (3) speed-bias back substitution;
+//   (4) landmark back substitution, dogleg, model change, retraction into the candidate buffers.
+// A rejected step (reuse), a finished window and a failed speed-bias elimination skip (1)-(3), as the separate kernels do.
+// 4 warps and <= 56 KB of shared memory: 4 CTAs per SM, so the 528 windows of 132 SMs run in one wave.
+constexpr int kSolveThreads = 128;
+constexpr int kSolveMaxB = 12;   // 9*10/2 = 45 lower blocks (ldw <= 72) over 4 warps
+__host__ __device__ inline size_t solve_small_smem_bytes(int ldw, int n_lc, int n_c, int nb) {
+  size_t b = (size_t)2 * 32 * (ldw + 4) * 8;
+  b = std::max(b, chol_smem_bytes(n_lc));
+  b = std::max(b, sb_back_smem_bytes(n_lc, nb));
+  return std::max(b, (size_t)(40 + 3 * n_c) * 8);
+}
+__global__ void __launch_bounds__(kSolveThreads, 4) k_solve_small(Dev d) {
+  const int wi = blockIdx.x;
+  const WinDesc &w = d.win[wi];
+  if (!w.fused_solve) return;
+  Ctl *ctl = d.ctl + wi;
+  if (ctl->done) return;
+  extern __shared__ __align__(16) double sm[];
+  __shared__ double red[40];
+  if (!ctl->reuse && !ctl->chol_fail) {
+    const double uhu = schur_small_body<kSolveThreads, kSolveMaxB>(d, wi, sm, red, sm, chol_smem_ld(w.n_lc));
+    // k_sb_elim has added its share already and nothing else writes the window's uHu_cam now: a plain add
+    if (threadIdx.x == 0) ctl->uHu_cam += uhu;
+    __syncthreads();
+    if (!chol_smem_body(d, wi, sm, true)) {
+      __syncthreads();   // gn_c (pose part) and the shared memory of phase 2
+      sb_back_body(d, wi, sm);
+    }
+    __syncthreads();
+  }
+  step_body<false>(d, wi, sm, w.n_c);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3001,8 +3078,18 @@ void launch_lm_gather(const Dev &d, const int *lm_win, int n_lm_total, int max_l
     k_lm_gather16<<<(n_lm_total + kG16Lm - 1) / kG16Lm, kG16Lm * 16, (size_t)kG16Lm * max_ldw * 8, s>>>(d, lm_win, n_lm_total, max_ldw);
   if (n_chunk12 > 0) k_lm_gather12<<<(n_chunk12 + kG12Warps - 1) / kG12Warps, kG12Warps * 32, 0, s>>>(d, n_chunk12);
 }
-void launch_schur_small(const Dev &d, int max_ldw, cudaStream_t s) {
-  k_schur_small<<<d.n_win, kSsThreads, (size_t)(2 * 32 * (max_ldw + 4) + 40) * 8, s>>>(d);
+void launch_schur_small(const Dev &d, int max_ldw, int with_fused, cudaStream_t s) {
+  k_schur_small<<<d.n_win, kSsThreads, (size_t)(2 * 32 * (max_ldw + 4) + 40) * 8, s>>>(d, with_fused);
+}
+// the 8x8 blocks of the lower triangle fit the accumulators of k_solve_small's warps
+bool solve_small_fits(int ldw) { const int nb8 = ldw / 8; return nb8 * (nb8 + 1) / 2 <= kSolveMaxB * (kSolveThreads / 32); }
+size_t solve_small_smem(int ldw, int n_lc, int n_c, int nb) { return solve_small_smem_bytes(ldw, n_lc, n_c, nb); }
+int configure_solve_small(size_t smem) { return (int)raise_smem_limit(k_solve_small, smem); }
+void launch_solve_small(const Dev &d, size_t smem, cudaStream_t s) { k_solve_small<<<d.n_win, kSolveThreads, smem, s>>>(d); }
+int solve_small_occupancy(size_t smem) {
+  int n = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_solve_small, kSolveThreads, smem) != cudaSuccess) return -1;
+  return n;
 }
 int configure_schur_small(int max_ldw) {
   return (int)raise_smem_limit(k_schur_small, (size_t)((2 * 32 * (max_ldw + 4) + 40) * 8));
@@ -3048,6 +3135,7 @@ void launch_chol(const Dev &d, int max_rows, cudaStream_t s) {
 }
 void launch_step(const Dev &d, int max_nc, cudaStream_t s) {
   // both kinds of windows may share a handle: each instantiation skips the other's windows
+  // (n_plain_win: windows without leaves that k_solve_small does not own)
   if (d.n_leaf_total < 0 || d.n_plain_win > 0) k_step<false><<<d.n_win, kStepThreads, (size_t)(40 + 3 * max_nc) * 8, s>>>(d, max_nc);
   if (d.n_leaf_total > 0) k_step<true><<<d.n_win, kStepThreads, (size_t)(40 + 3 * max_nc) * 8, s>>>(d, max_nc);
 }

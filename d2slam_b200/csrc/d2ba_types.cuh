@@ -105,6 +105,9 @@ struct WinDesc {
   int hub_small;               // leaves present and n_hub + 1 <= 96: the hub x hub part of the reduced system comes from the one-CTA Schur kernel
   int gather_nosync;           // compact records: within a landmark no column block appears at both slot positions (k_lm_gather16 needs no barrier between records)
   int row_tiles;               // most 32-column tiles any landmark's coupling row touches (row buffers of the gather kernels)
+  int fused_solve;             // k_solve_small solves the reduced system (no leaves, sb_elim, schur_small, chol_smem, and
+                               // enough such windows in the handle to fill the GPU: d2ba_finalize); the
+                               // separate Schur / Cholesky / speed-bias back-substitution / step kernels skip the window
 };
 
 struct PriorBlk {
@@ -167,7 +170,7 @@ struct Dev {
   const unsigned long long *lm_mask;  // [NL] bit t set: the landmark's coupling row has entries in W-space columns [32 t, 32 t + 32)
   const HSeg *hseg;
   const Leaf *leaf; int n_leaf_total;
-  int n_plain_win;      // windows without leaves
+  int n_plain_win;      // windows without leaves and without fused_solve (k_step<false>)
   double *leafL;        // per leaf: L, 1/diag(L)
   const int *schur_chunks;
   const int *leaf_lm;

@@ -50,6 +50,7 @@ EXPORTED = [
     "d2ba_set_consensus", "d2ba_comm_unique_id", "d2ba_comm_init", "d2ba_consensus_buffer", "d2ba_finalize",
     "d2ba_solve", "d2ba_solve_fixed", "d2ba_get_blocks", "d2ba_num_windows", "d2ba_marginalize",
     "d2ba_debug_linearize", "d2ba_debug_get", "d2ba_debug_kernel_times", "d2ba_debug_host_times",
+    "d2ba_debug_solve_occupancy",
 ]
 
 
@@ -171,6 +172,12 @@ class Solver:
         refs = refs[: nb.value].copy()
         nx = int(sum(abi.KIND_SIZE[int(k)] for k in refs["kind"]))
         return Aflat[: mm * mm].reshape(mm, mm).copy(), b[:mm].copy(), refs, x0[:nx].copy()
+
+    def solve_occupancy(self):
+        """CTAs per SM of the one-kernel reduced-system solve (0: no window of this handle takes that path)."""
+        n = C.c_int32()
+        self._chk(lib().d2ba_debug_solve_occupancy(self.h, C.byref(n)), "solve_occupancy")
+        return n.value
 
     def kernel_times(self, iters):
         out = np.zeros(12)

@@ -284,9 +284,12 @@ enum d2ba_debug_item {
   D2BA_DBG_GN_STEP = 13,
   D2BA_DBG_IMU_RESJAC = 14,  /* per IMU factor (input order): r[15], J (15 x 30) row-major tangent columns
                                 [pose_i 6 | speed-bias_i 9 | pose_j 6 | speed-bias_j 9], both times sqrt_info        */
-  D2BA_DBG_CONS_RESJAC = 15  /* per six-dof block (poses then extrinsics, input order) 62 doubles: x[7], z[7], tilde[6],
+  D2BA_DBG_CONS_RESJAC = 15, /* per six-dof block (poses then extrinsics, input order) 62 doubles: x[7], z[7], tilde[6],
                                 r[6], J (6 x 6) row-major tangent of ConsenusPoseFactor at the current state; zeros for
                                 blocks outside the consensus set                                                       */
+  D2BA_DBG_SOLVE_PATH = 16   /* int64 scalar: 1 when the window's reduced system is solved by the one-kernel path
+                                (k_solve_small), 0 when by the separate Schur / Cholesky / step kernels (also for
+                                windows that fit the one-kernel path in a handle with fewer than 3 of them per SM)    */
 };
 /* Linearise at the current state (no step) so that the debug items are defined. */
 int d2ba_debug_linearize(d2ba_handle *h);
@@ -295,8 +298,13 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
 /* Device time (ms, CUDA events on the solver stream) of each kernel of the iteration sequence, summed over `iters`
  * iterations: [0] lm_gather (+ sb_elim), [1] reduced system (Schur tiles + leaf elimination), [2] dense Cholesky (+ sb / leaf back
  * substitution), [3] step, [4] misc_lin, [5] proj_lin, [6] control, [7] = iters, and the shares [8] sb_elim (of [0]),
- * [9] sb_back (of [2]), [10] leaf_elim (of [1]), [11] leaf_back (of [2]). */
+ * [9] sb_back (of [2]), [10] leaf_elim (of [1]), [11] leaf_back (of [2]).  The one-kernel solve of the windows with
+ * D2BA_DBG_SOLVE_PATH = 1 (Schur, Cholesky, back substitutions and step) is timed in [3]; [1], [2], [9] then hold only
+ * the other windows' kernels. */
 int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out /* [12] */);
+/* CTAs per SM of the one-kernel solve at this handle's shared-memory size (cudaOccupancyMaxActiveBlocksPerMultiprocessor);
+ * 0 when no window of the finalized handle takes that path. */
+int d2ba_debug_solve_occupancy(d2ba_handle *h, int32_t *ctas_per_sm);
 /* Host wall-clock (ms) of the phases of the last d2ba_finalize: [plan (pair-major order, groups, jobs), prefix sums +
  * staging resize, staging fill, upload enqueue, error check, read-back buffers, device ms of the uploads, device ms of tile build + prep kernels], followed by
  * the thread-summed ms spent inside d2ba_add_proj since the last d2ba_reset: [id lookup, stamp scan, staging copy,
