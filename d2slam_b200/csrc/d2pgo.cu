@@ -15,7 +15,9 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <cmath>
+#include <map>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -480,6 +482,177 @@ __global__ void k_pgo_retract(PgoDev d, double *x_out) {
   for (int k = NX; k < 8; k++) x_out[(size_t)i * 8 + k] = 0.0;
 }
 
+// ---- ARock (d2pgo's pgo_mode 1, ARockSolver / ARockPGO): proximal terms of one agent's local problem and its dual update.
+// A dual (neighbour, frame) holds y_l (sent to the neighbour) and y_r (received); its proximal term pulls the frame's pose, in
+// dual coordinates, towards y_r.  Dual coordinates: 4-DoF the pose [x y z yaw] itself (POSE_4D); 6-DoF [p ; theta] with
+// R = R(q_init) Exp(theta) (POSE_PERTURB_6D, pgostate.hpp:35-46).  The proximal terms run in kernels of their own after the
+// edge / prior kernels (k_pgo_arock_gD after k_pgo_gD, k_pgo_arock_cg_pAp in place of the damping pass), so the kernels of a
+// graph without ARock are untouched.
+struct PgoArockDev {
+  int n_dual;
+  const int *pose;            // [K] pose index of each dual
+  const int *ptr, *of;        // CSR pose -> its duals, ascending dual index
+  const double *yr;           // [K][D] remote duals: the proximal targets
+  double *yl;                 // [K][D] local duals
+  const double *qinit;        // [N][4] attitude the 6-DoF perturbation is taken from (unit, xyzw)
+  double *lin;                // [D + D^2][K] field-major: r(D), J (DxD row-major)
+  double wT, wR;              // residual weights: 4-DoF rho_T, rho_theta (ConsenusPoseFactor4D); 6-DoF sqrt of them (NormalPrior A)
+  double eta;
+};
+
+// theta = Log(q_init^-1 q) (principal, |theta| <= pi) and, with Jinv, J_r^-1(theta) = d theta / d dtheta of the right
+// perturbation q (x) Exp(dtheta): I + [theta]x / 2 + c2 [theta]x^2, c2 = 1/a^2 - (1 + cos a) / (2 a sin a), a = |theta|;
+// with the half-angle quaternion (|v|, w) = (sin a/2, cos a/2) of q_init^-1 q: c2 = 1/a^2 - w / (2 a |v|) (series below 1e-2)
+D2BA_DEV void arock_theta(const double *x, const double *qi, double *th, double *Jinv) {   // x: [x y z qx qy qz qw]
+  Q4 e = qmul(Q4{-qi[0], -qi[1], -qi[2], qi[3]}, qload(x + 3));
+  if (e.w < 0.0) e = Q4{-e.x, -e.y, -e.z, -e.w};
+  const double n = sqrt(e.x * e.x + e.y * e.y + e.z * e.z);
+  const double a = 2.0 * atan2(n, e.w), k = n > 0.0 ? a / n : 2.0 / e.w;
+  th[0] = k * e.x; th[1] = k * e.y; th[2] = k * e.z;
+  if (!Jinv) return;
+  const double a2 = a * a;
+  const double c2 = a < 1e-2 ? 1.0 / 12.0 + a2 / 720.0 + a2 * a2 / 30240.0 : 1.0 / a2 - e.w / (2.0 * a * n);
+  const double K[9] = {0.0, -th[2], th[1], th[2], 0.0, -th[0], -th[1], th[0], 0.0};
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) {
+    double k2 = 0.0;
+    for (int m = 0; m < 3; m++) k2 += K[i * 3 + m] * K[m * 3 + j];
+    Jinv[i * 3 + j] = (i == j ? 1.0 : 0.0) + 0.5 * K[i * 3 + j] + c2 * k2;
+  }
+}
+
+// pose x in dual coordinates (D = 4: the 4-vector; D = 6: [p ; theta])
+template <int D>
+D2BA_DEV void arock_coord(const double *x, const double *qi, double *c) {
+  for (int k = 0; k < 3; k++) c[k] = x[k];
+  if constexpr (D == 4) c[3] = x[3];
+  else arock_theta(x, qi, c + 3, nullptr);
+}
+
+// one proximal term at pose x, target y:
+//   4-DoF ConsenusPoseFactor4D(y, rho_T, rho_theta, norm_yaw) (consenus_factor_4d.h, utils.hpp:267-280):
+//     r = diag(rho_T I3, rho_theta) [y_p - p ; N(N(y_yaw) - yaw)],  J = -diag(rho_T I3, rho_theta)
+//   6-DoF NormalPrior(A, y), A = diag(sqrt(rho_T) I3, sqrt(rho_theta) I3) (ARock.cpp:284-291):
+//     r = A ([p ; theta] - y),  J = A blockdiag(I3, J_r^-1(theta))
+template <int D>
+D2BA_DEV void arock_eval(const double *x, const double *qi, const double *y, double wT, double wR, double *r, double *J) {
+  for (int k = 0; k < D * D; k++) J[k] = 0.0;
+  if constexpr (D == 4) {
+    for (int k = 0; k < 3; k++) { r[k] = wT * (y[k] - x[k]); J[k * 5] = -wT; }
+    r[3] = wR * pgo_normalize_angle(pgo_normalize_angle(y[3]) - x[3]);
+    J[15] = -wR;
+  } else {
+    double th[3], Ji[9];
+    arock_theta(x, qi, th, Ji);
+    for (int k = 0; k < 3; k++) { r[k] = wT * (x[k] - y[k]); r[3 + k] = wR * (th[k] - y[3 + k]); J[k * 7] = wT; }
+    for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) J[(3 + i) * 6 + 3 + j] = wR * Ji[i * 3 + j];
+  }
+}
+
+// linearise every proximal term at d.x: records [r | J]; cost partials go after the edges' and the priors' (k_pgo_sum)
+template <int D>
+__global__ void __launch_bounds__(128) k_pgo_arock_lin(PgoDev d, double *cost_part, PgoArockDev a) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  __shared__ double red[40];
+  double c = 0.0;
+  if (k < a.n_dual) {
+    const int i = a.pose[k];
+    double r[D], J[D * D];
+    arock_eval<D>(d.x + (size_t)i * 8, a.qinit + (size_t)i * 4, a.yr + (size_t)k * D, a.wT, a.wR, r, J);
+    for (int q = 0; q < D; q++) c += 0.5 * r[q] * r[q];
+    double *o = a.lin + k;
+    const size_t K = (size_t)a.n_dual;
+    for (int q = 0; q < D; q++) o[q * K] = r[q];
+    for (int q = 0; q < D * D; q++) o[(D + q) * K] = J[q];
+  }
+  c = block_sum(c, red);
+  if (threadIdx.x == 0) cost_part[blockIdx.x] = c;
+}
+
+// after k_pgo_gD: g_i += sum J^T r, D_i += sum J^T J over pose i's duals, in dual order (free poses only)
+template <int D>
+__global__ void __launch_bounds__(128) k_pgo_arock_gD(PgoDev d, double *g, double *Dg, PgoArockDev a) {
+  constexpr int DD = D * D;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= d.n_pose || d.fixed[i] || a.ptr[i] == a.ptr[i + 1]) return;
+  double gi[D], Di[DD];
+  for (int k = 0; k < D; k++) gi[k] = g[(size_t)i * D + k];
+  for (int k = 0; k < DD; k++) Di[k] = Dg[(size_t)i * DD + k];
+  const size_t K = (size_t)a.n_dual;
+  for (int q = a.ptr[i]; q < a.ptr[i + 1]; q++) {
+    const double *o = a.lin + a.of[q];
+    for (int k = 0; k < D; k++) {
+      const double rk = o[k * K];
+      double row[D];
+      for (int b = 0; b < D; b++) { row[b] = o[(D + k * D + b) * K]; gi[b] += row[b] * rk; }
+      for (int b = 0; b < D; b++) for (int c = 0; c < D; c++) Di[b * D + c] += row[b] * row[c];
+    }
+  }
+  for (int k = 0; k < D; k++) g[(size_t)i * D + k] = gi[k];
+  for (int k = 0; k < DD; k++) Dg[(size_t)i * DD + k] = Di[k];
+}
+
+// after k_pgo_cg_pose<P, LOCAL = true>: Ap_i += sum J^T (J p_i) over pose i's duals, then the damping and the partials of
+// p.Ap (what k_pgo_cg_pAp does for a multi-rank graph)
+template <class P>
+__global__ void __launch_bounds__(128) k_pgo_arock_cg_pAp(PgoDev d, int par, double tol2, PgoArockDev a) {
+  constexpr int D = P::D;
+  __shared__ double red[40];
+  const CgView v = cg_view(d, par, tol2, red);
+  if (v.done) return;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  double s = 0.0;
+  if (i < d.n_pose) {
+    double p[D], y[D];
+    for (int k = 0; k < D; k++) { p[k] = d.p[(size_t)i * D + k]; y[k] = d.Ap[(size_t)i * D + k]; }
+    if (!d.fixed[i]) {
+      const size_t K = (size_t)a.n_dual;
+      for (int q = a.ptr[i]; q < a.ptr[i + 1]; q++) {
+        const double *J = a.lin + (size_t)D * K + a.of[q];
+        for (int k = 0; k < D; k++) {
+          double j[D], t = 0.0;
+          for (int b = 0; b < D; b++) { j[b] = J[(size_t)(k * D + b) * K]; t += j[b] * p[b]; }
+          for (int b = 0; b < D; b++) y[b] += j[b] * t;
+        }
+      }
+    }
+    for (int k = 0; k < D; k++) {
+      y[k] += d.damp[(size_t)i * D + k] * p[k];
+      s += p[k] * y[k];
+      d.Ap[(size_t)i * D + k] = y[k];
+    }
+  }
+  s = block_sum(s, red);
+  if (threadIdx.x == 0) d.pAp_part[blockIdx.x] = s;
+}
+
+// updateDualStates (ARock.cpp:50-81) per dual at the solved poses x: y_l -= eta ((y_l + y_r) / 2 - x), x in dual coordinates,
+// the operations in the reference's order and rounding (no contraction); 4-DoF: y_l's yaw normalised only once outside +-pi
+template <int D>
+__global__ void k_pgo_arock_update(const double *x, PgoArockDev a) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= a.n_dual) return;
+  const int i = a.pose[k];
+  double c[D];
+  arock_coord<D>(x + (size_t)i * 8, a.qinit + (size_t)i * 4, c);
+  double *yl = a.yl + (size_t)k * D;
+  const double *yr = a.yr + (size_t)k * D;
+  for (int q = 0; q < D; q++) {
+    const double avg = __ddiv_rn(__dadd_rn(yl[q], yr[q]), 2.0);
+    yl[q] = __dsub_rn(yl[q], __dmul_rn(__dsub_rn(avg, c[q]), a.eta));
+  }
+  if constexpr (D == 4) if (yl[3] > M_PI || yl[3] < -M_PI) yl[3] = pgo_normalize_angle(yl[3]);
+}
+
+// every pose in dual coordinates, [N][D] (the value a dual created by scanning starts from)
+template <int D>
+__global__ void k_pgo_arock_coord(int n, const double *x, const double *qinit, double *out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double c[D];
+  arock_coord<D>(x + (size_t)i * 8, qinit + (size_t)i * 4, c);
+  for (int k = 0; k < D; k++) out[(size_t)i * D + k] = c[k];
+}
+
 template <typename T> struct Buf {
   T *p = nullptr; size_t n = 0;
   cudaError_t alloc(size_t c) { if (c <= n && p) return cudaSuccess; if (p) cudaFree(p); p = nullptr; n = 0; cudaError_t e = cudaMalloc(&p, (c ? c : 1) * sizeof(T)); if (e == cudaSuccess) n = c; return e; }
@@ -775,6 +948,18 @@ struct d2pgo_handle {
   bool uploaded = false;
   void *comm = nullptr; int rank = 0, nranks = 1;
   PcmBufs pcm;   // d2pgo_pcm's device buffers (independent of the poses and edges above)
+  // ARock (d2pgo_arock_enable): owner agent and 6-DoF q_init per pose id, the dual table keyed (neighbour, frame id) in
+  // ascending order, the messages received since the last step, and the device copy of the table (in table order)
+  bool arock = false; d2pgo_arock_config acfg = {};
+  std::unordered_map<int64_t, int32_t> owner; std::unordered_map<int64_t, std::array<double, 4>> qinit;
+  struct Dual { double yl[6], yr[6]; };
+  struct Msg { int32_t sender, target; std::vector<int64_t> frames; std::vector<double> duals; };
+  std::map<std::pair<int32_t, int64_t>, Dual> duals;
+  std::vector<Msg> inbox;
+  Buf<int> d_ak_pose, d_ak_ptr, d_ak_of; Buf<double> d_ak_yr, d_ak_yl, d_ak_qinit, d_ak_lin[2], d_ak_coord;
+  int ak_n = -1;                      // duals on the device, -1 = none synced
+  const void *ak_key[4] = {nullptr, nullptr, nullptr, nullptr};   // buffers the captured CG graphs point at
+  bool graph_ark = false;             // the captured CG graphs carry the proximal terms
 };
 
 #define PCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return 100 + (int)e_; } } while (0)
@@ -796,6 +981,9 @@ static int pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const d
   }
   h->ea.clear(); h->eb.clear(); h->rel.clear(); h->sinfo.clear(); h->uploaded = false;
   h->gp_pose.clear(); h->gp_u.clear(); h->gp_S.clear();
+  for (auto it = h->duals.begin(); it != h->duals.end();)   // ARock duals live on for the frames still present
+    it = h->index.count(it->first.second) ? std::next(it) : h->duals.erase(it);
+  h->ak_n = -1;
   return 0;
 }
 
@@ -860,6 +1048,8 @@ int d2pgo_destroy(d2pgo_handle *h) {
   h->d_Ap.release(); h->d_cost.release(); h->d_fixed.release(); h->d_ea.release(); h->d_eb.release(); h->d_s.release();
   h->d_gp_u.release(); h->d_gp_S.release(); h->d_glin[0].release(); h->d_glin[1].release(); h->d_gp_pose.release(); h->d_prior_of.release();
   h->pcm.release();
+  h->d_ak_pose.release(); h->d_ak_ptr.release(); h->d_ak_of.release(); h->d_ak_yr.release(); h->d_ak_yl.release(); h->d_ak_qinit.release();
+  h->d_ak_lin[0].release(); h->d_ak_lin[1].release(); h->d_ak_coord.release();
   cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1); cudaStreamDestroy(h->stream);
   delete h;
   return 0;
@@ -893,6 +1083,7 @@ int d2pgo_add_edges_4d(d2pgo_handle *h, int32_t n, const int64_t *id_a, const in
 
 int d2pgo_comm_init(d2pgo_handle *h, const uint8_t unique_id[128], int32_t rank, int32_t nranks) {
   if (!h) return 1;
+  if (h->arock) { h->err = "comm_init: the handle is in ARock mode (each agent solves its own sub-graph; edge sharding splits one graph)"; return 5; }
   cudaSetDevice(h->cfg.device);
   if (nccl_comm_init(&h->comm, unique_id, rank, nranks, h->err)) return 3;
   h->rank = rank; h->nranks = nranks;
@@ -960,19 +1151,33 @@ static PgoPriorDev pgo_prior_view(d2pgo_handle *h, int cur) {
   return pr;
 }
 
+static PgoArockDev pgo_arock_view(d2pgo_handle *h, int cur) {
+  PgoArockDev a;
+  a.n_dual = h->ak_n > 0 ? h->ak_n : 0; a.pose = h->d_ak_pose.p; a.ptr = h->d_ak_ptr.p; a.of = h->d_ak_of.p; a.yr = h->d_ak_yr.p; a.yl = h->d_ak_yl.p;
+  a.qinit = h->d_ak_qinit.p; a.lin = h->d_ak_lin[cur].p;
+  const bool six = h->dof == 6;
+  a.wT = six ? std::sqrt(h->acfg.rho_frame_T) : h->acfg.rho_frame_T; a.wR = six ? std::sqrt(h->acfg.rho_frame_theta) : h->acfg.rho_frame_theta;
+  a.eta = h->acfg.eta_k;
+  return a;
+}
+
 // cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks.  GRAV: this
-// rank has gravity priors (their cost partials follow the edges', their terms enter g and D after each pose's edges).
-template <class P, bool GRAV>
+// rank has gravity priors (their cost partials follow the edges', their terms enter g and D after each pose's edges).  ARK:
+// the ARock proximal terms of the synced dual table (cost partials last, g and D after the edges and priors).
+template <class P, bool GRAV, bool ARK = false>
 static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
   constexpr int D = P::D;
   PgoDev d = pgo_view(h, b);
   const PgoPriorDev pr = pgo_prior_view(h, b);
+  const PgoArockDev ak = pgo_arock_view(h, b);
   const size_t N = h->ids.size();
-  const int nbe = (d.n_edge + 127) / 128, nbg = GRAV ? (pr.n_prior + 127) / 128 : 0;
+  const int nbe = (d.n_edge + 127) / 128, nbg = GRAV ? (pr.n_prior + 127) / 128 : 0, nbk = ARK ? (ak.n_dual + 127) / 128 : 0;
   if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, h->stream>>>(d, h->d_cost_part.p, want_jac);
   if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, h->stream>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
-  k_pgo_sum<<<1, 128, 0, h->stream>>>(h->d_cost_part.p, nbe + nbg, h->d_cost.p);
+  if (nbk > 0) k_pgo_arock_lin<D><<<nbk, 128, 0, h->stream>>>(d, h->d_cost_part.p + nbe + nbg, ak);
+  k_pgo_sum<<<1, 128, 0, h->stream>>>(h->d_cost_part.p, nbe + nbg + nbk, h->d_cost.p);
   if (want_jac) k_pgo_gD<P, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+  if (want_jac && nbk > 0) k_pgo_arock_gD<D><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, ak);
   if (h->comm) {
     if (nccl_allreduce_f64(h->comm, h->d_cost.p, 1, h->stream)) { h->err = "ncclAllReduce(cost) failed"; return 40; }
     if (want_jac && (nccl_allreduce_f64(h->comm, h->d_g[b].p, N * D, h->stream) || nccl_allreduce_f64(h->comm, h->d_D[b].p, N * D * D, h->stream))) { h->err = "ncclAllReduce(g, D) failed"; return 40; }
@@ -984,13 +1189,16 @@ static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
 
 constexpr int kCgChunk = 16;   // CG iterations between two looks at the convergence flag (one graph launch on a single rank)
 
-template <class P, bool GRAV>
-static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr, double tol2) {
+template <class P, bool GRAV, bool ARK>
+static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr, const PgoArockDev &ak, double tol2) {
   const int ge = (d.n_edge + 127) / 128;
   for (int k = 0; k < kCgChunk; k++) {
     const int par = k & 1;
     if (d.n_edge > 0) k_pgo_cg_edge<P><<<ge, 128, 0, h->stream>>>(d, par, tol2);
-    if (h->comm) {
+    if constexpr (ARK) {   // an ARock handle has no communicator (d2pgo_comm_init refuses it)
+      k_pgo_cg_pose<P, true, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
+      k_pgo_arock_cg_pAp<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, ak);
+    } else if (h->comm) {
       k_pgo_cg_pose<P, true, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
       // every rank holds the same r, z, p (the all-reduced products are bitwise identical), so all of them reach the same
       // `done` decision at the same iteration and the collective below is always matched
@@ -1002,8 +1210,9 @@ static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr,
   return 0;
 }
 
-// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4) and by 6-DoF graphs with gravity priors (GRAV)
-template <class P, bool GRAV>
+// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4), by 6-DoF graphs with gravity priors (GRAV)
+// and by ARock local problems (ARK: the proximal terms of the synced dual table)
+template <class P, bool GRAV, bool ARK = false>
 static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
@@ -1013,13 +1222,14 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   PCK(cudaEventRecord(h->ev0, h->stream));
   int cur = 0;                    // buffer (poses, lin records, g, D) of the accepted point
   double cost = 0, lambda = h->cfg.lambda0;
-  if ((rc = pgo_linearize<P, GRAV>(h, cur, 1, &cost))) return rc;
+  if ((rc = pgo_linearize<P, GRAV, ARK>(h, cur, 1, &cost))) return rc;
   R.initial_cost = cost;
   const double tol2 = h->cfg.pcg_tolerance * h->cfg.pcg_tolerance;
-  if (tol2 != h->graph_tol2) { pgo_drop_graphs(h); h->graph_tol2 = tol2; }
+  if (tol2 != h->graph_tol2 || ARK != h->graph_ark) { pgo_drop_graphs(h); h->graph_tol2 = tol2; h->graph_ark = ARK; }
   for (int it = 0; it < h->cfg.max_iterations; it++) {
     PgoDev d = pgo_view(h, cur);
     const PgoPriorDev pr = pgo_prior_view(h, cur);
+    const PgoArockDev ak = pgo_arock_view(h, cur);
     // (J^T J + lambda diag D) dx = -g by block-Jacobi preconditioned CG; J^T J is never formed
     k_pgo_precond<P><<<gp, 128, 0, h->stream>>>(d, h->d_D[cur].p, lambda);
     k_pgo_cg_init<P><<<gp, 128, 0, h->stream>>>(d, h->d_g[cur].p);
@@ -1030,20 +1240,20 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
         if (!h->cg_graph[cur]) {
           cudaGraph_t g;
           PCK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-          pgo_cg_chunk<P, GRAV>(h, d, pr, tol2);
+          pgo_cg_chunk<P, GRAV, ARK>(h, d, pr, ak, tol2);
           PCK(cudaStreamEndCapture(h->stream, &g));
           PCK(cudaGraphInstantiate(&h->cg_graph[cur], g, 0));
           cudaGraphDestroy(g);
         }
         PCK(cudaGraphLaunch(h->cg_graph[cur], h->stream));
-      } else if ((rc = pgo_cg_chunk<P, GRAV>(h, d, pr, tol2))) return rc;
+      } else if ((rc = pgo_cg_chunk<P, GRAV, ARK>(h, d, pr, ak, tol2))) return rc;
       PCK(cudaMemcpyAsync(&s, h->d_s.p, sizeof s, cudaMemcpyDeviceToHost, h->stream));
       PCK(cudaStreamSynchronize(h->stream));
       if (s.done) break;   // identical on every rank (see pgo_cg_chunk)
     }
     k_pgo_retract<P><<<gp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
     double cand = 0;
-    if ((rc = pgo_linearize<P, GRAV>(h, 1 - cur, 1, &cand))) return rc;
+    if ((rc = pgo_linearize<P, GRAV, ARK>(h, 1 - cur, 1, &cand))) return rc;
     R.pcg_iterations += s.iters; R.iterations++;
     if (cand < cost && isfinite(cand)) {
       const double rel_dec = (cost - cand) / (cost > 0 ? cost : 1.0);
@@ -1157,6 +1367,242 @@ int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles
     for (int a = 0; a < 3; a++) o[a] = tmp[a * G + k];
     for (int a = 0; a < 3; a++) for (int b = 0; b < 6; b++) o[3 + a * 6 + b] = b < 3 ? 0.0 : tmp[(3 + a * 3 + b - 3) * G + k];
   }
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- ARock host side
+static int arock_fail(d2pgo_handle *h, int rc, const std::string &msg) { h->err = msg; return rc; }
+
+static bool all_finite(const double *v, size_t n) {
+  for (size_t k = 0; k < n; k++) if (!std::isfinite(v[k])) return false;
+  return true;
+}
+
+// poses the local problem uses: those an edge or a gravity prior touches (ARockSolver::all_estimating_params)
+static std::vector<char> arock_in_problem(const d2pgo_handle *h) {
+  std::vector<char> in(h->ids.size(), 0);
+  for (size_t e = 0; e < h->ea.size(); e++) in[h->ea[e]] = in[h->eb[e]] = 1;
+  for (int p : h->gp_pose) in[p] = 1;
+  return in;
+}
+
+// the dual table, in table order, to the device: pose of each dual, the pose -> duals CSR, y_r, y_l, q_init
+static int arock_sync(d2pgo_handle *h) {
+  const size_t N = h->ids.size(), K = h->duals.size(), D = h->dof;
+  std::vector<int> pose(K), ptr(N + 1, 0), of(K);
+  std::vector<double> yr(K * D), yl(K * D), qi(N * 4, 0.0);
+  size_t k = 0;
+  for (const auto &kv : h->duals) {
+    pose[k] = h->index.at(kv.first.second); ptr[pose[k] + 1]++;
+    for (size_t q = 0; q < D; q++) { yr[k * D + q] = kv.second.yr[q]; yl[k * D + q] = kv.second.yl[q]; }
+    k++;
+  }
+  for (size_t i = 0; i < N; i++) ptr[i + 1] += ptr[i];
+  { std::vector<int> fill(ptr.begin(), ptr.end() - 1);
+    for (size_t j = 0; j < K; j++) of[fill[pose[j]]++] = (int)j; }
+  if (D == 6) for (size_t i = 0; i < N; i++) memcpy(&qi[i * 4], h->qinit.at(h->ids[i]).data(), 32);
+  const size_t nbe = (h->ea.size() + 127) / 128, nbg = (h->gp_pose.size() + 127) / 128, nbk = (K + 127) / 128;
+  PCK(h->d_ak_pose.alloc(K)); PCK(h->d_ak_of.alloc(K)); PCK(h->d_ak_ptr.alloc(N + 1)); PCK(h->d_ak_yr.alloc(K * D)); PCK(h->d_ak_yl.alloc(K * D));
+  PCK(h->d_ak_qinit.alloc(N * 4)); PCK(h->d_ak_lin[0].alloc(K * (D + D * D))); PCK(h->d_ak_lin[1].alloc(K * (D + D * D)));
+  PCK(h->d_cost_part.alloc(nbe + nbg + nbk + 1));
+  if (K) {
+    PCK(cudaMemcpyAsync(h->d_ak_pose.p, pose.data(), K * 4, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_ak_of.p, of.data(), K * 4, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_ak_yr.p, yr.data(), K * D * 8, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_ak_yl.p, yl.data(), K * D * 8, cudaMemcpyHostToDevice, h->stream));
+  }
+  PCK(cudaMemcpyAsync(h->d_ak_ptr.p, ptr.data(), (N + 1) * 4, cudaMemcpyHostToDevice, h->stream));
+  PCK(cudaMemcpyAsync(h->d_ak_qinit.p, qi.data(), N * 32, cudaMemcpyHostToDevice, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
+  // the CG graphs hold the dual count and these buffers by value: capture them again when either changed
+  const void *key[4] = {h->d_ak_ptr.p, h->d_ak_of.p, h->d_ak_lin[0].p, h->d_ak_lin[1].p};
+  if ((int)K != h->ak_n || memcmp(key, h->ak_key, sizeof key)) { pgo_drop_graphs(h); memcpy(h->ak_key, key, sizeof key); }
+  h->ak_n = (int)K;
+  return 0;
+}
+
+// every pose at d_x[0] in dual coordinates, [N][D] on the host
+static int arock_coords(d2pgo_handle *h, std::vector<double> &out) {
+  const size_t N = h->ids.size(), D = h->dof;
+  PCK(h->d_ak_coord.alloc(N * D));
+  const int nb = (int)((N + 127) / 128);
+  if (D == 6) k_pgo_arock_coord<6><<<nb, 128, 0, h->stream>>>((int)N, h->d_x[0].p, h->d_ak_qinit.p, h->d_ak_coord.p);
+  else k_pgo_arock_coord<4><<<nb, 128, 0, h->stream>>>((int)N, h->d_x[0].p, h->d_ak_qinit.p, h->d_ak_coord.p);
+  PCK(cudaGetLastError());
+  out.resize(N * D);
+  PCK(cudaMemcpyAsync(out.data(), h->d_ak_coord.p, N * D * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// every pose needs an owner (and, 6-DoF, a q_init) before the table can be built
+static int arock_check_poses(d2pgo_handle *h, const char *what) {
+  if (!h->arock) return arock_fail(h, 5, std::string(what) + ": the handle is not in ARock mode (d2pgo_arock_enable)");
+  for (int64_t id : h->ids) {
+    if (!h->owner.count(id)) return arock_fail(h, 2, std::string(what) + ": pose id " + std::to_string(id) + " has no owner agent (d2pgo_arock_enable)");
+    if (h->dof == 6 && !h->qinit.count(id)) return arock_fail(h, 2, std::string(what) + ": pose id " + std::to_string(id) + " has no q_init (d2pgo_arock_enable)");
+  }
+  return 0;
+}
+
+extern "C" {
+
+int d2pgo_default_arock_config(d2pgo_arock_config *c) {
+  if (!c) return 1;
+  memset(c, 0, sizeof *c);
+  c->self_id = 0; c->dual_state_init_to_zero = 0; c->rho_frame_T = 0.1; c->rho_frame_theta = 0.1; c->eta_k = 0.9;
+  return 0;
+}
+
+int d2pgo_arock_enable(d2pgo_handle *h, const d2pgo_arock_config *cfg, int32_t n, const int64_t *ids, const int32_t *owner, const double *q_init4) {
+  if (!h) return 1;
+  if (!cfg || n < 0 || (n > 0 && (!ids || !owner))) return arock_fail(h, 1, "arock_enable: null argument or negative count");
+  if (h->comm) return arock_fail(h, 5, "arock_enable: the handle has a communicator (edge sharding and ARock are different splits of the graph)");
+  if (!(std::isfinite(cfg->rho_frame_T) && cfg->rho_frame_T >= 0.0 && std::isfinite(cfg->rho_frame_theta) && cfg->rho_frame_theta >= 0.0 && std::isfinite(cfg->eta_k)))
+    return arock_fail(h, 2, "arock_enable: rho_frame_T, rho_frame_theta must be finite and non-negative, eta_k finite");
+  std::vector<std::array<double, 4>> q(n);
+  for (int k = 0; k < n; k++) {
+    auto it = h->index.find(ids[k]);
+    if (it == h->index.end()) return arock_fail(h, 2, "arock_enable: unknown pose id " + std::to_string(ids[k]));
+    const double *src = q_init4 ? q_init4 + (size_t)k * 4 : &h->poses[(size_t)it->second * 8 + 3];
+    if (h->dof == 6) {
+      const double s2 = src[0] * src[0] + src[1] * src[1] + src[2] * src[2] + src[3] * src[3];
+      if (!all_finite(src, 4) || !(s2 > 0.0)) return arock_fail(h, 2, "arock_enable: pose id " + std::to_string(ids[k]) + ": non-finite or zero q_init");
+      const double s = 1.0 / std::sqrt(s2);
+      q[k] = {src[0] * s, src[1] * s, src[2] * s, src[3] * s};
+    }
+  }
+  h->arock = true; h->acfg = *cfg;
+  for (int k = 0; k < n; k++) { h->owner[ids[k]] = owner[k]; if (h->dof == 6) h->qinit[ids[k]] = q[k]; }
+  h->ak_n = -1;
+  return 0;
+}
+
+int d2pgo_arock_receive(d2pgo_handle *h, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int32_t dim, const double *duals) {
+  if (!h) return 1;
+  if (!h->arock) return arock_fail(h, 5, "arock_receive: the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (n < 0 || (n > 0 && (!frame_ids || !duals))) return arock_fail(h, 1, "arock_receive: null argument or negative count");
+  if (dim != h->dof) return arock_fail(h, 2, "arock_receive: duals of dimension " + std::to_string(dim) + " on a handle with pose_dof = " + std::to_string(h->dof));
+  if (sender == h->acfg.self_id) return arock_fail(h, 2, "arock_receive: a message from this agent itself (self_id " + std::to_string(sender) + ")");
+  if (!all_finite(duals, (size_t)n * dim)) return arock_fail(h, 2, "arock_receive: non-finite dual");
+  std::unordered_map<int64_t, int> seen;
+  for (int k = 0; k < n; k++) if (!seen.emplace(frame_ids[k], k).second) return arock_fail(h, 2, "arock_receive: frame id " + std::to_string(frame_ids[k]) + " twice in one message");
+  h->inbox.push_back(d2pgo_handle::Msg{sender, target, std::vector<int64_t>(frame_ids, frame_ids + n), std::vector<double>(duals, duals + (size_t)n * dim)});
+  return 0;
+}
+
+int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
+  if (!h) return 1;
+  if (h->ids.empty()) return arock_fail(h, 1, "arock_step: no poses");
+  if (int rc = arock_check_poses(h, "arock_step")) return rc;
+  cudaSetDevice(h->cfg.device);
+  int rc;
+  if (!h->uploaded && (rc = pgo_upload(h))) return rc;
+  const int D = h->dof, self = h->acfg.self_id;
+  const std::vector<char> in = arock_in_problem(h);
+  // 1. receiveAll / processPGOData (ARockPGO.cpp:13-70), messages in arrival order
+  for (const auto &m : h->inbox)
+    for (size_t k = 0; k < m.frames.size(); k++) {
+      auto it = h->index.find(m.frames[k]);
+      if (it == h->index.end() || !in[it->second]) continue;
+      const auto key = std::make_pair(m.sender, m.frames[k]);
+      auto d = h->duals.find(key);
+      if (m.target != self && d != h->duals.end()) continue;
+      const double *v = &m.duals[k * D];
+      if (d == h->duals.end()) { d2pgo_handle::Dual nd; memset(&nd, 0, sizeof nd); memcpy(nd.yl, v, D * 8); memcpy(nd.yr, v, D * 8); h->duals.emplace(key, nd); }
+      else memcpy(d->second.yr, v, D * 8);
+    }
+  h->inbox.clear();
+  // 2. scanAndCreateDualStates (ARock.cpp:192-208): a dual for every frame of another agent, from x(f) or zero.  The q_init
+  // table goes to the device first (arock_sync) so that the coordinates can be taken there.
+  if ((rc = arock_sync(h))) return rc;
+  std::vector<double> coord;
+  if (!h->acfg.dual_state_init_to_zero && (rc = arock_coords(h, coord))) return rc;
+  bool created = false;
+  for (size_t i = 0; i < h->ids.size(); i++) {
+    const int32_t o = h->owner.at(h->ids[i]);
+    if (!in[i] || o == self) continue;
+    const auto key = std::make_pair(o, h->ids[i]);
+    if (h->duals.count(key)) continue;
+    d2pgo_handle::Dual nd; memset(&nd, 0, sizeof nd);
+    if (!h->acfg.dual_state_init_to_zero) { memcpy(nd.yl, &coord[i * D], D * 8); memcpy(nd.yr, &coord[i * D], D * 8); }
+    h->duals.emplace(key, nd); created = true;
+  }
+  // 3. setDualStateFactors + solveLocalStep: the LM solve with the proximal terms towards y_r
+  if (created && (rc = arock_sync(h))) return rc;
+  if ((rc = D == 4 ? pgo_solve<PgoEdge4, false, true>(h, rep)
+                   : h->gp_pose.empty() ? pgo_solve<PgoEdge6, false, true>(h, rep) : pgo_solve<PgoEdge6, true, true>(h, rep))) return rc;
+  // 4. updateDualStates at the solved poses.  pgo_solve leaves them in buffer 0, by a device-to-device cudaMemcpy when they
+  // were in buffer 1: that copy is not ordered with this handle's non-blocking stream, so wait for it.
+  PCK(cudaStreamSynchronize(0));
+  const PgoArockDev ak = pgo_arock_view(h, 0);
+  if (ak.n_dual > 0) {
+    const int nb = (ak.n_dual + 127) / 128;
+    if (D == 6) k_pgo_arock_update<6><<<nb, 128, 0, h->stream>>>(h->d_x[0].p, ak);
+    else k_pgo_arock_update<4><<<nb, 128, 0, h->stream>>>(h->d_x[0].p, ak);
+    PCK(cudaGetLastError());
+    std::vector<double> yl((size_t)ak.n_dual * D);
+    PCK(cudaMemcpyAsync(yl.data(), h->d_ak_yl.p, yl.size() * 8, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaStreamSynchronize(h->stream));
+    size_t k = 0;
+    for (auto &kv : h->duals) { memcpy(kv.second.yl, &yl[k * D], D * 8); k++; }
+  }
+  return 0;
+}
+
+int d2pgo_arock_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out) {
+  if (!h) return 1;
+  if (!h->arock) return arock_fail(h, 5, "arock_neighbours: the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (!n_out || max_n < 0 || (max_n > 0 && !ids_out)) return arock_fail(h, 1, "arock_neighbours: null argument or negative count");
+  std::vector<int32_t> nb;
+  for (const auto &kv : h->duals) if (nb.empty() || nb.back() != kv.first.first) nb.push_back(kv.first.first);
+  *n_out = (int32_t)nb.size();
+  if ((int32_t)nb.size() > max_n) return arock_fail(h, 2, "arock_neighbours: room for " + std::to_string(max_n) + " ids, " + std::to_string(nb.size()) + " needed");
+  std::copy(nb.begin(), nb.end(), ids_out);
+  return 0;
+}
+
+int d2pgo_arock_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t *n_out, int64_t *frame_ids, double *local_out, double *remote_out) {
+  if (!h) return 1;
+  if (!h->arock) return arock_fail(h, 5, "arock_duals: the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (!n_out || max_n < 0 || (max_n > 0 && (!frame_ids || !local_out))) return arock_fail(h, 1, "arock_duals: null argument or negative count");
+  const int D = h->dof;
+  auto lo = h->duals.lower_bound(std::make_pair(neighbour, INT64_MIN)), hi = h->duals.upper_bound(std::make_pair(neighbour, INT64_MAX));
+  const int32_t cnt = (int32_t)std::distance(lo, hi);
+  *n_out = cnt;
+  if (cnt > max_n) return arock_fail(h, 2, "arock_duals: room for " + std::to_string(max_n) + " duals, " + std::to_string(cnt) + " needed");
+  int k = 0;
+  for (auto it = lo; it != hi; ++it, ++k) {
+    frame_ids[k] = it->first.second;
+    memcpy(local_out + (size_t)k * D, it->second.yl, D * 8);
+    if (remote_out) memcpy(remote_out + (size_t)k * D, it->second.yr, D * 8);
+  }
+  return 0;
+}
+
+int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
+  if (!h) return 1;
+  if (int rc = arock_check_poses(h, "debug_arock_terms")) return rc;
+  const size_t K = h->duals.size(), D = h->dof, W = D + D * D;
+  if ((size_t)out_doubles < K * W) return arock_fail(h, 2, "debug_arock_terms: buffer too small: " + std::to_string(K * W) + " doubles needed");
+  if (!out && K) return arock_fail(h, 1, "debug_arock_terms: null argument");
+  if (!K) return 0;
+  cudaSetDevice(h->cfg.device);
+  int rc;
+  if (!h->uploaded && (rc = pgo_upload(h))) return rc;
+  if ((rc = arock_sync(h))) return rc;
+  const PgoDev d = pgo_view(h, 0);
+  const PgoArockDev ak = pgo_arock_view(h, 0);
+  const int nb = (int)((K + 127) / 128);
+  if (D == 6) k_pgo_arock_lin<6><<<nb, 128, 0, h->stream>>>(d, h->d_cost_part.p, ak);
+  else k_pgo_arock_lin<4><<<nb, 128, 0, h->stream>>>(d, h->d_cost_part.p, ak);
+  PCK(cudaGetLastError());
+  std::vector<double> tmp(K * W);
+  PCK(cudaMemcpyAsync(tmp.data(), ak.lin, K * W * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
+  for (size_t k = 0; k < K; k++) for (size_t q = 0; q < W; q++) out[k * W + q] = tmp[q * K + k];   // device layout is field-major
   return 0;
 }
 

@@ -14,7 +14,10 @@ d2pgo_pcm); make_pcm_case builds its inputs from a make_pose_graph graph, with i
 
 Gravity prior (d2pgo's enable_gravity_prior, 6-DoF): `PgoSolver.add_gravity_priors` ties each pose's roll and pitch to the
 gravity direction of its frame's ego (VIO) pose (include/d2pgo.h d2pgo_add_gravity_priors); make_gravity_case builds ego poses
-for a make_pose_graph graph."""
+for a make_pose_graph graph.
+
+ARock (d2pgo's distributed pgo_mode 1): `ArockAgent` is one agent's handle in ARock mode (include/d2pgo.h d2pgo_arock_*);
+arock_split builds agent s's sub-graph the way D2PGO::solve_multi does, arock_run runs the synchronous broadcast schedule."""
 import ctypes as C
 
 import numpy as np
@@ -36,6 +39,11 @@ class PcmConfig(C.Structure):
     _fields_ = [("pcm_thres", C.c_double), ("pos_covariance_per_meter", C.c_double), ("yaw_covariance_per_meter", C.c_double)]
 
 
+class ArockConfig(C.Structure):
+    _fields_ = [("self_id", C.c_int32), ("dual_state_init_to_zero", C.c_int32), ("rho_frame_T", C.c_double), ("rho_frame_theta", C.c_double),
+                ("eta_k", C.c_double)]
+
+
 class PcmReport(C.Structure):
     _fields_ = [("groups", C.c_int32), ("inliers", C.c_int32), ("pairs_tested", C.c_int64), ("consistent_pairs", C.c_int64),
                 ("clique_rounds", C.c_int64), ("device_ms", C.c_double), ("pair_ms", C.c_double), ("clique_ms", C.c_double)]
@@ -44,7 +52,8 @@ class PcmReport(C.Structure):
 PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_last_error", "d2pgo_set_poses", "d2pgo_add_edges",
                 "d2pgo_comm_init", "d2pgo_solve", "d2pgo_get_poses", "d2pgo_debug_edges", "d2pgo_set_poses_4d", "d2pgo_add_edges_4d",
                 "d2pgo_get_poses_4d", "d2pgo_default_pcm_config", "d2pgo_pcm", "d2pgo_debug_pcm_smd", "d2pgo_debug_pcm_clique",
-                "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors"]
+                "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors", "d2pgo_default_arock_config", "d2pgo_arock_enable",
+                "d2pgo_arock_receive", "d2pgo_arock_step", "d2pgo_arock_neighbours", "d2pgo_arock_duals", "d2pgo_debug_arock_terms"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -175,6 +184,56 @@ class PgoSolver:
         out = np.zeros(max(int(self.pcm_report.pairs_tested), 1))
         self._chk(_lib().d2pgo_debug_pcm_smd(self.h, _p(out), C.c_int64(out.size)), "debug_pcm_smd")
         return out[: int(self.pcm_report.pairs_tested)]
+
+    # ---- ARock (include/d2pgo.h d2pgo_arock_*)
+    @property
+    def dim(self):
+        return 4 if self.cfg.pose_dof == 4 else 6
+
+    def arock_enable(self, ids, owner, q_init=None, **cfg):
+        """ARock mode: owner agent per pose id, 6-DoF q_init [n, 4] (None = the attitudes given to set_poses); cfg overrides
+        ArockConfig fields (self_id, dual_state_init_to_zero, rho_frame_T, rho_frame_theta, eta_k)."""
+        c = ArockConfig()
+        _lib().d2pgo_default_arock_config(C.byref(c))
+        for k, v in cfg.items():
+            setattr(c, k, v)
+        ids = np.ascontiguousarray(ids, np.int64); own = np.ascontiguousarray(owner, np.int32)
+        q = None if q_init is None else np.ascontiguousarray(np.asarray(q_init, np.float64).reshape(-1, 4))
+        self._chk(_lib().d2pgo_arock_enable(self.h, C.byref(c), C.c_int32(len(ids)), _p(ids), _p(own), _p(q)), "arock_enable")
+        self.arock_cfg = c
+
+    def arock_receive(self, sender, target, frame_ids, duals, dim=None):
+        f = np.ascontiguousarray(frame_ids, np.int64); d = np.ascontiguousarray(np.asarray(duals, np.float64).reshape(len(f), -1))
+        self._chk(_lib().d2pgo_arock_receive(self.h, C.c_int32(sender), C.c_int32(target), C.c_int32(len(f)), _p(f),
+                                             C.c_int32(d.shape[1] if dim is None else dim), _p(d)), "arock_receive")
+
+    def arock_step(self):
+        r = PgoReport()
+        self._chk(_lib().d2pgo_arock_step(self.h, C.byref(r)), "arock_step")
+        return r
+
+    def arock_neighbours(self):
+        n = C.c_int32()
+        _lib().d2pgo_arock_neighbours(self.h, 0, C.byref(n), None)
+        out = np.zeros(max(n.value, 1), np.int32)
+        self._chk(_lib().d2pgo_arock_neighbours(self.h, C.c_int32(len(out)), C.byref(n), _p(out)), "arock_neighbours")
+        return out[: n.value]
+
+    def arock_duals(self, neighbour):
+        """(frame ids, y_l [n, D], y_r [n, D]) of the duals held with `neighbour`, frame ids ascending."""
+        n = C.c_int32()
+        _lib().d2pgo_arock_duals(self.h, C.c_int32(neighbour), 0, C.byref(n), None, None, None)
+        m = max(n.value, 1)
+        f = np.zeros(m, np.int64); yl = np.zeros((m, self.dim)); yr = np.zeros((m, self.dim))
+        self._chk(_lib().d2pgo_arock_duals(self.h, C.c_int32(neighbour), C.c_int32(m), C.byref(n), _p(f), _p(yl), _p(yr)), "arock_duals")
+        return f[: n.value], yl[: n.value], yr[: n.value]
+
+    def debug_arock_terms(self, n_duals):
+        """Per dual in table order at the current poses: r (D) | J (D x D), D + D^2 doubles."""
+        D = self.dim
+        out = np.zeros((max(n_duals, 1), D + D * D))
+        self._chk(_lib().d2pgo_debug_arock_terms(self.h, _p(out), C.c_int64(out.size)), "debug_arock_terms")
+        return out[:n_duals]
 
     def debug_pcm_clique(self, adj):
         """The device clique kernel alone on a symmetric boolean adjacency [n, n] -> boolean membership [n]."""
@@ -478,3 +537,106 @@ def read_g2o_agents(directory, agents_num):
     parts = [read_g2o(p, max_agent_id=agents_num - 1) for _, p in files]
     cat = lambda k: np.concatenate([q[k] for q in parts]) if parts else np.zeros(0)
     return dict(ids=cat("ids"), poses=cat("poses"), id_a=cat("id_a"), id_b=cat("id_b"), rel=cat("rel"), sqrt_info=cat("sqrt_info"))
+
+
+# ------------------------------------------------------------------------------------------------ ARock (pgo_mode 1)
+def graph_agents(g):
+    """Owner agent of every pose of a graph dict: g["agent"], or the estimator's frame-id convention id // 1_000_000."""
+    return np.asarray(g["agent"]) if "agent" in g else (np.asarray(g["ids"]) // 1_000_000).astype(np.int64)
+
+
+def arock_split(g, s, main_id=0):
+    """Agent s's sub-graph as D2PGO::solve_multi builds it: s's own ego-motion edges (setupEgoMotionFactors(solver, self_id),
+    d2pgo.cpp:561-567) and every loop whose two frames s knows (setupLoopFactors, :413-466), where s knows its own frames and
+    the frames at the other end of its loops.  An ego-motion edge joins two consecutive frames (in id order) of one agent;
+    every other edge is a loop.  Only main_id's head frame is fixed, and only in main_id's own sub-graph (d2pgo.cpp:602-612).
+    g: dict(ids, init or poses, id_a, id_b, rel, sqrt_info[, agent]) with 7-vector (6-DoF) or 4-vector (4-DoF) poses, e.g.
+    from make_pose_graph, pose_graph_to_4d or read_g2o_agents.  Returns dict(self_id, ids, poses, fixed, owner, id_a, id_b,
+    rel, sqrt_info, edges) with the frames in id order and `edges` the indices of the kept edges in g."""
+    ids = np.asarray(g["ids"]); poses = np.asarray(g["init"] if "init" in g else g["poses"]); agent = graph_agents(g)
+    pos = {int(i): k for k, i in enumerate(ids)}
+    ia = np.array([pos[int(i)] for i in g["id_a"]], np.int64); ib = np.array([pos[int(i)] for i in g["id_b"]], np.int64)
+    # consecutive frames of each agent, in id order
+    nxt = {}
+    for a in np.unique(agent):
+        mine = np.sort(ids[agent == a])
+        nxt.update({int(u): int(v) for u, v in zip(mine[:-1], mine[1:])})
+    ida, idb = ids[ia], ids[ib]
+    ego = np.array([(agent[x] == agent[y]) and (nxt.get(int(u)) == int(v) or nxt.get(int(v)) == int(u)) for x, y, u, v in zip(ia, ib, ida, idb)], bool)
+    own = agent[ia] == s
+    known = set(ids[agent == s].tolist())
+    touch = ~ego & ((agent[ia] == s) | (agent[ib] == s))
+    known |= set(ida[touch].tolist()) | set(idb[touch].tolist())
+    kin = np.array([int(u) in known and int(v) in known for u, v in zip(ida, idb)], bool)
+    keep = np.nonzero((ego & own) | (~ego & kin))[0]
+    used = np.unique(np.concatenate([ia[keep], ib[keep]])) if len(keep) else np.zeros(0, np.int64)
+    used = used[np.argsort(ids[used], kind="stable")]
+    fixed = np.zeros(len(used), np.uint8)
+    if s == main_id:
+        head = ids[agent == s].min()
+        fixed[ids[used] == head] = 1
+    return dict(self_id=int(s), ids=ids[used].astype(np.int64), poses=poses[used].copy(), fixed=fixed, owner=agent[used].astype(np.int32),
+                id_a=ida[keep].astype(np.int64), id_b=idb[keep].astype(np.int64), rel=np.asarray(g["rel"])[keep], sqrt_info=np.asarray(g["sqrt_info"])[keep], edges=keep)
+
+
+class ArockAgent:
+    """One agent of d2pgo's ARock mode on the GPU: a PgoSolver handle with the agent's sub-graph (arock_split) in ARock mode.
+    q_init: 6-DoF attitudes [n, 4] of the sub-graph's frames (None = their initial attitudes); ego_poses: 6-DoF ego poses [n, 7]
+    of the frames for one gravity prior each (d2pgo's enable_gravity_prior; None = no priors); cfg: ArockConfig fields;
+    solver_kw: PgoConfig fields (pose_dof is taken from the poses)."""
+
+    def __init__(self, split, q_init=None, ego_poses=None, solver_kw=None, **cfg):
+        self.split = split; self.self_id = split["self_id"]
+        self.dof = 4 if np.asarray(split["poses"]).shape[1] == 4 else 6
+        self.s = PgoSolver(pose_dof=self.dof, **(solver_kw or {}))
+        if self.dof == 4:
+            self.s.set_poses_4d(split["ids"], split["poses"], split["fixed"]); self.s.add_edges_4d(split["id_a"], split["id_b"], split["rel"], split["sqrt_info"])
+        else:
+            self.s.set_poses(split["ids"], split["poses"], split["fixed"]); self.s.add_edges(split["id_a"], split["id_b"], split["rel"], split["sqrt_info"])
+            if ego_poses is not None:
+                self.s.add_gravity_priors(split["ids"], ego_poses)
+        self.s.arock_enable(split["ids"], split["owner"], q_init, self_id=self.self_id, **cfg)
+
+    def step(self):
+        return self.s.arock_step()
+
+    def messages(self):
+        """broadcastData: one (sender, target, frame ids, y_l) per neighbour, neighbours ascending."""
+        return [(self.self_id, int(n), *self.s.arock_duals(int(n))[:2]) for n in self.s.arock_neighbours()]
+
+    def receive(self, msg):
+        sender, target, frames, duals = msg
+        self.s.arock_receive(sender, target, frames, duals)
+
+    def duals(self):
+        """{(neighbour, frame id): (y_l, y_r)}"""
+        out = {}
+        for n in self.s.arock_neighbours():
+            f, yl, yr = self.s.arock_duals(int(n))
+            out.update({(int(n), int(i)): (a, b) for i, a, b in zip(f, yl, yr)})
+        return out
+
+    def poses(self):
+        ids = self.split["ids"]
+        return self.s.get_poses_4d(ids) if self.dof == 4 else self.s.get_poses(ids)
+
+    def close(self):
+        self.s.close()
+
+
+def arock_run(agents, rounds, after_round=None):
+    """The synchronous broadcast schedule: every round, every agent steps, then every message of the round is delivered to every
+    other agent (in the order of the agents, each agent's messages by neighbour).  after_round(r, agents, reports) is called
+    after each round's delivery.  Returns the per-round lists of step reports."""
+    out = []
+    for r in range(rounds):
+        reps = [a.step() for a in agents]
+        msgs = [m for a in agents for m in a.messages()]
+        for a in agents:
+            for m in msgs:
+                if m[0] != a.self_id:
+                    a.receive(m)
+        out.append(reps)
+        if after_round is not None:
+            after_round(r, agents, reps)
+    return out

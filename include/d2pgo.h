@@ -18,9 +18,11 @@
  *                                    being those setupLoopFactors receives (d2pgo/src/d2pgo.cpp:177-186, :276-282)
  *   d2pgo_add_gravity_priors      <- setupGravityPriorFactors (enable_gravity_prior): GravityPriorPerturbAD per frame
  *                                    (d2pgo/src/d2pgo.cpp:530-559, GravityPrior.hpp:8-46)
+ *   d2pgo_arock_*                 <- ARockPGO, d2pgo's distributed pgo_mode 1 (ARock.cpp:24-314, ARockPGO.cpp:7-104; below)
  *
- * Scope note: the reference solves the multi-agent graph with ARock (asynchronous dual updates, ARock.cpp:140-328) around
- * per-agent ceres problems; BASELINE's config asks for a *distributed Gauss-Newton* on the 8 GPUs of one box.  Here every
+ * Scope note: the reference solves the multi-agent graph with ARock (dual updates around per-agent ceres problems,
+ * ARock.cpp:140-328), which the d2pgo_arock_* entry points reproduce, one handle per agent.  BASELINE's config also asks for
+ * a *distributed Gauss-Newton* on the 8 GPUs of one box, which d2pgo_comm_init provides: every
  * rank holds the whole pose vector (10k poses = 560 KB) and a shard of the edges; one LM iteration = linearise the local
  * edges, block-Jacobi preconditioned conjugate gradients on (J^T J + lambda D) dx = -J^T r with the matrix never formed
  * (y = J^T (J x) per edge), the per-rank partial products summed with one ncclAllReduce per CG iteration over NVLink.
@@ -148,6 +150,66 @@ int d2pgo_pcm(d2pgo_handle *h, const d2pgo_pcm_config *cfg, int32_t n_frames, co
  * self loops, adj[n][ceil(n / 32)] words, bit j of row i = word j / 32, bit j % 32: member_out[n], size_out = clique size. */
 int d2pgo_debug_pcm_smd(d2pgo_handle *h, double *out, int64_t out_doubles);
 int d2pgo_debug_pcm_clique(d2pgo_handle *h, int32_t n, const uint32_t *adj, uint8_t *member_out, int32_t *size_out);
+
+/* ---- ARock distributed mode (d2pgo's pgo_mode 1: PGO_MODE_DISTRIBUTED_AROCK)
+ *   d2pgo_arock_enable     <- ARockPGO construction with ARockSolverConfig (d2common/include/d2common/solver/ARock.hpp:6-19)
+ *   d2pgo_arock_receive    <- ARockPGO::inputDPGOData; processed at the next step as receiveAll / processPGOData
+ *                             (d2pgo/src/ARockPGO.cpp:7-70)
+ *   d2pgo_arock_step       <- one pass of ARockBase::solve_arock with max_steps = 1, as d2pgo_node runs it
+ *                             (d2common/src/solver/ARock.cpp:140-190)
+ *   d2pgo_arock_neighbours,
+ *   d2pgo_arock_duals      <- ARockPGO::broadcastData: one message per neighbour, target = that neighbour (ARockPGO.cpp:72-104)
+ * One handle is one agent (self_id).  Its poses and edges are that agent's sub-graph (D2PGO::solve_multi: its own ego-motion
+ * edges and every loop whose two frames it knows); every pose carries its owner agent.  The dual table is keyed by
+ * (neighbour agent, frame id) and holds a local dual y_l and a remote dual y_r, in dual coordinates:
+ *   4-DoF handles: [x y z yaw] (POSE_4D);
+ *   6-DoF handles: [p ; theta] with R = R(q_init) Exp(theta), theta = Log(q_init^-1 q) the principal log (POSE_PERTURB_6D,
+ *                  d2pgo/src/pgostate.hpp:35-46; the node's perturb_mode).  q_init is the frame's attitude when it was added.
+ * One step:
+ *   1. the received messages in arrival order: for a frame the local problem uses (an edge or a gravity prior touches it),
+ *      if target == self_id or there is no dual (sender, frame) yet: create it with y_l = y_r = the value, or else set y_r;
+ *   2. every frame the local problem uses and another agent d owns gets a dual (d, frame) if it has none, y_l = y_r = the
+ *      frame's pose in dual coordinates (or 0 with dual_state_init_to_zero);
+ *   3. the LM solve of d2pgo_solve over the edges, the gravity priors and one proximal term per dual, towards its y_r:
+ *        4-DoF ConsenusPoseFactor4D (norm_yaw): r = diag(rho_T I3, rho_theta) [y_p - p ; N(N(y_yaw) - yaw)]  (weights rho,
+ *              not sqrt(rho); d2common/include/d2common/solver/consenus_factor_4d.h)
+ *        6-DoF NormalPrior: r = diag(sqrt(rho_T) I3, sqrt(rho_theta) I3) ([p ; theta] - y_r)   (ARock.cpp:284-291)
+ *   4. updateDualStates (ARock.cpp:50-81) on every dual at the solved poses x (in dual coordinates):
+ *        y_l -= eta_k ((y_l + y_r) / 2 - x), and on 4-DoF handles y_l's yaw normalised only when it lies outside [-pi, pi].
+ * Only the fixed flags of d2pgo_set_poses hold the gauge: d2pgo fixes main_id's head frame and nothing else
+ * (d2pgo/src/d2pgo.cpp:602-612).  The report is the local LM solve's (costs include the proximal terms).  d2pgo_set_poses
+ * keeps the duals of the frames still present and every queued message; d2pgo_solve on an ARock handle solves its sub-graph
+ * without proximal terms.  A handle in ARock mode refuses d2pgo_comm_init (5) and a handle with a communicator refuses
+ * d2pgo_arock_enable (5).  Every refusal keeps nothing of the call and sets d2pgo_last_error. */
+typedef struct d2pgo_arock_config {
+  int32_t self_id;
+  int32_t dual_state_init_to_zero;       /* ARockSolverConfig default 0                                              */
+  double rho_frame_T, rho_frame_theta;   /* defaults 0.1 / 0.1; config/realsense_d435/d435_multi.yaml: 0.7 / 0.625   */
+  double eta_k;                          /* default 0.9; d435_multi.yaml: 0.1                                        */
+} d2pgo_arock_config;
+
+int d2pgo_default_arock_config(d2pgo_arock_config *cfg);
+/* owner agent of each pose id (ids must be poses of the handle; a later call adds to or replaces the table and the config).
+ * 6-DoF: q_init4[n][4] (xyzw, normalised here), NULL = the attitude of the pose as d2pgo_set_poses gave it.  Returns 1 on a
+ * null argument or n < 0, 2 on an unknown id, a non-finite or zero q_init or a bad config, 5 with a communicator attached. */
+int d2pgo_arock_enable(d2pgo_handle *h, const d2pgo_arock_config *cfg, int32_t n, const int64_t *ids, const int32_t *owner,
+                       const double *q_init4);
+/* one message (sender, target, frames, duals[n][dim]), queued for the next step; dim must be 4 (4-DoF) or 6 (6-DoF).
+ * Returns 2 on a wrong dim, a non-finite dual, a frame id twice, or sender == self_id; 5 if not in ARock mode. */
+int d2pgo_arock_receive(d2pgo_handle *h, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int32_t dim,
+                        const double *duals);
+/* one ARock step; every pose needs an owner (and, 6-DoF, a q_init) */
+int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *report);
+/* the neighbours the dual table holds, ascending; *n_out = their number (2 if more than max_n) */
+int d2pgo_arock_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out);
+/* the broadcast payload for one neighbour: frame ids ascending, y_l [n][D] and (remote_out may be NULL) y_r [n][D];
+ * *n_out = the count (2 if more than max_n) */
+int d2pgo_arock_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t *n_out, int64_t *frame_ids, double *local_out,
+                      double *remote_out);
+/* parity hook: per dual in table order ((neighbour, frame id) ascending), at the current poses and towards its y_r:
+ * out[n_duals][D + D*D] = r (D) | J (D x D row-major, in the tangent: 4-DoF the 4-vector, 6-DoF [dp, dtheta] of the right
+ * perturbation q (x) Exp(dtheta); the 6-DoF theta block is sqrt(rho_theta) J_r^-1(theta)) */
+int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles);
 
 #ifdef __cplusplus
 }
