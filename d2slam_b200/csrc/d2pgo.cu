@@ -653,6 +653,131 @@ __global__ void k_pgo_arock_coord(int n, const double *x, const double *qinit, d
   for (int k = 0; k < D; k++) out[(size_t)i * D + k] = c[k];
 }
 
+// ---- chordal rotation initialisation (d2pgo_rot_init; RotationInitialization<double>, rotation_initialization_base.hpp).
+// One row system k at a time through the solver above: the "pose" is row k of R_f (x[0..2] of the 8 doubles), an edge's
+// residual S (R_ab^T x_a - x_b) with R_ab the edge's (normalised) quaternion and S = s I3, fixed frames hold their rows as
+// constants.  The residual is linear, so one Gauss-Newton step from x = 0 with CG run to a tight tolerance solves the system.
+D2BA_DEV void rotinit_edge_eval(const double *xa, const double *xb, const double *rel, const double *S, double *r, double *J0, double *J1) {
+  double R[9];
+  q2R(qload(rel + 3), R);
+  const double v[3] = {R[0] * xa[0] + R[3] * xa[1] + R[6] * xa[2] - xb[0],   // R_ab^T x_a - x_b
+                       R[1] * xa[0] + R[4] * xa[1] + R[7] * xa[2] - xb[1],
+                       R[2] * xa[0] + R[5] * xa[1] + R[8] * xa[2] - xb[2]};
+  for (int i = 0; i < 3; i++) r[i] = S[i * 3] * v[0] + S[i * 3 + 1] * v[1] + S[i * 3 + 2] * v[2];
+  if (!J0) return;
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) {
+    J0[i * 3 + j] = S[i * 3] * R[j * 3] + S[i * 3 + 1] * R[j * 3 + 1] + S[i * 3 + 2] * R[j * 3 + 2];   // S R_ab^T
+    J1[i * 3 + j] = -S[i * 3 + j];
+  }
+}
+struct PgoRotRow {   // one row of R per frame, x + dx
+  static constexpr int D = 3, NX = 3;
+  D2BA_DEV static void eval(const double *p0, const double *p1, const double *rel, const double *S, double *r, double *J0, double *J1) { rotinit_edge_eval(p0, p1, rel, S, r, J0, J1); }
+  D2BA_DEV static void plus(const double *x, const double *dx, double *o) { for (int k = 0; k < 3; k++) o[k] = x[k] + dx[k]; }
+};
+
+template <int P, int Q>
+D2BA_DEV void rotinit_order(double *sv, double *A, double *V) {   // columns P < Q of A and V swapped if sv[P] < sv[Q]
+  if (!(sv[P] < sv[Q])) return;
+  double t = sv[P]; sv[P] = sv[Q]; sv[Q] = t;
+  for (int i = 0; i < 3; i++) {
+    t = A[i * 3 + P]; A[i * 3 + P] = A[i * 3 + Q]; A[i * 3 + Q] = t;
+    t = V[i * 3 + P]; V[i * 3 + P] = V[i * 3 + Q]; V[i * 3 + Q] = t;
+  }
+}
+
+// Utility::recoverRotationSVD (d2common/include/d2common/utils.hpp:121-129): R = U diag(1, 1, det(U V^T)) V^T of M = U S V^T,
+// singular values descending (JacobiSVD's order).  One-sided (Hestenes) Jacobi on the columns of M; row-major in and out.
+D2BA_DEV void rotinit_project_svd(const double *M, double *R) {
+  double A[9], V[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  for (int k = 0; k < 9; k++) A[k] = M[k];
+  for (int sweep = 0; sweep < 16; sweep++) {
+    bool rotated = false;
+    for (int pq = 0; pq < 3; pq++) {
+      const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;
+      double al = 0, be = 0, ga = 0;
+      for (int i = 0; i < 3; i++) { al += A[i * 3 + p] * A[i * 3 + p]; be += A[i * 3 + q] * A[i * 3 + q]; ga += A[i * 3 + p] * A[i * 3 + q]; }
+      if (!(fabs(ga) > 2.220446049250313e-16 * sqrt(al * be))) continue;
+      rotated = true;
+      const double zeta = (be - al) / (2.0 * ga);
+      const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+      const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
+      for (int i = 0; i < 3; i++) {
+        const double ap = A[i * 3 + p], aq = A[i * 3 + q], vp = V[i * 3 + p], vq = V[i * 3 + q];
+        A[i * 3 + p] = c * ap - s * aq; A[i * 3 + q] = s * ap + c * aq;
+        V[i * 3 + p] = c * vp - s * vq; V[i * 3 + q] = s * vp + c * vq;
+      }
+    }
+    if (!rotated) break;
+  }
+  // columns in descending singular-value order (compare-and-swap of whole columns: static indices, no local memory)
+  double sv[3];
+  for (int j = 0; j < 3; j++) sv[j] = sqrt(A[j] * A[j] + A[3 + j] * A[3 + j] + A[6 + j] * A[6 + j]);
+  rotinit_order<0, 1>(sv, A, V); rotinit_order<1, 2>(sv, A, V); rotinit_order<0, 1>(sv, A, V);
+  double U[9], W[9];
+  for (int j = 0; j < 3; j++) {
+    const double inv = sv[j] > 0.0 ? 1.0 / sv[j] : 0.0;
+    for (int i = 0; i < 3; i++) { U[i * 3 + j] = A[i * 3 + j] * inv; W[i * 3 + j] = V[i * 3 + j]; }
+  }
+  if (!(sv[2] > 0.0)) {   // rank-deficient M: complete U by the cross product of its first two columns
+    U[2] = U[3] * U[7] - U[6] * U[4]; U[5] = U[6] * U[1] - U[0] * U[7]; U[8] = U[0] * U[4] - U[3] * U[1];
+  }
+  const double detU = U[0] * (U[4] * U[8] - U[5] * U[7]) - U[1] * (U[3] * U[8] - U[5] * U[6]) + U[2] * (U[3] * U[7] - U[4] * U[6]);
+  const double detW = W[0] * (W[4] * W[8] - W[5] * W[7]) - W[1] * (W[3] * W[8] - W[5] * W[6]) + W[2] * (W[3] * W[7] - W[4] * W[6]);
+  const double d = detU * detW < 0.0 ? -1.0 : 1.0;
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++)
+    R[i * 3 + j] = U[i * 3] * W[j * 3] + U[i * 3 + 1] * W[j * 3 + 1] + d * U[i * 3 + 2] * W[j * 3 + 2];
+}
+
+// Eigen's Quaternion(const Matrix3 &) (quaternionbase_assign_impl): the trace branch, else the largest diagonal's
+template <int I>
+D2BA_DEV Q4 rotinit_quat_diag(const double *R) {   // the branch of the largest diagonal entry I
+  constexpr int J = (I + 1) % 3, K = (J + 1) % 3;
+  double q[4];   // x y z w
+  double t = sqrt(R[I * 4] - R[J * 4] - R[K * 4] + 1.0);
+  q[I] = 0.5 * t; t = 0.5 / t;
+  q[3] = (R[K * 3 + J] - R[J * 3 + K]) * t; q[J] = (R[J * 3 + I] + R[I * 3 + J]) * t; q[K] = (R[K * 3 + I] + R[I * 3 + K]) * t;
+  return Q4{q[0], q[1], q[2], q[3]};
+}
+D2BA_DEV Q4 rotinit_quat(const double *R) {
+  const double tr = R[0] + R[4] + R[8];
+  if (tr > 0.0) {
+    double t = sqrt(tr + 1.0);
+    const double w = 0.5 * t;
+    t = 0.5 / t;
+    return Q4{(R[7] - R[5]) * t, (R[2] - R[6]) * t, (R[3] - R[1]) * t, w};
+  }
+  if (R[8] > (R[4] > R[0] ? R[4] : R[0])) return rotinit_quat_diag<2>(R);
+  return R[4] > R[0] ? rotinit_quat_diag<1>(R) : rotinit_quat_diag<0>(R);
+}
+
+// recoverRotationLLT (rotation_initialization_base.hpp:360-389) per solved frame: M = [row 0 ; row 1 ; row 2] from the three
+// row systems' solutions m0..m2 ([N][8], row at +0), its state change |R_before - M|_F / |R_before|_F (R_before: the rotation
+// of the frame's normalised attitude, PGOState's rot state) into per-block partials, and the attitude x[3..6] = quaternion of
+// the projected R.  The position x[0..2] is not written.
+__global__ void __launch_bounds__(128) k_rotinit_project(int n, const int *frame, const double *m0, const double *m1, const double *m2, double *x, double *chg_part) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  __shared__ double red[40];
+  double chg = 0.0;
+  if (j < n) {
+    const size_t i = (size_t)frame[j];
+    double M[9], R0[9], R[9];
+    for (int c = 0; c < 3; c++) { M[c] = m0[i * 8 + c]; M[3 + c] = m1[i * 8 + c]; M[6 + c] = m2[i * 8 + c]; }
+    Q4 q = qload(x + i * 8 + 3);
+    const double qn = sqrt(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+    q = Q4{q.x / qn, q.y / qn, q.z / qn, q.w / qn};
+    q2R(q, R0);
+    double dd = 0.0, nn = 0.0;
+    for (int c = 0; c < 9; c++) { dd += (R0[c] - M[c]) * (R0[c] - M[c]); nn += R0[c] * R0[c]; }
+    chg = sqrt(dd) / sqrt(nn);
+    rotinit_project_svd(M, R);
+    const Q4 o = rotinit_quat(R);
+    x[i * 8 + 3] = o.x; x[i * 8 + 4] = o.y; x[i * 8 + 5] = o.z; x[i * 8 + 6] = o.w;
+  }
+  chg = block_sum(chg, red);
+  if (threadIdx.x == 0) chg_part[blockIdx.x] = chg;
+}
+
 template <typename T> struct Buf {
   T *p = nullptr; size_t n = 0;
   cudaError_t alloc(size_t c) { if (c <= n && p) return cudaSuccess; if (p) cudaFree(p); p = nullptr; n = 0; cudaError_t e = cudaMalloc(&p, (c ? c : 1) * sizeof(T)); if (e == cudaSuccess) n = c; return e; }
@@ -960,6 +1085,7 @@ struct d2pgo_handle {
   int ak_n = -1;                      // duals on the device, -1 = none synced
   const void *ak_key[4] = {nullptr, nullptr, nullptr, nullptr};   // buffers the captured CG graphs point at
   bool graph_ark = false;             // the captured CG graphs carry the proximal terms
+  d2pgo_handle *rot = nullptr;        // d2pgo_rot_init's row systems (dof 3), kept between calls for their buffers
 };
 
 #define PCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return 100 + (int)e_; } } while (0)
@@ -1037,11 +1163,7 @@ int d2pgo_create(const d2pgo_config *cfg, d2pgo_handle **out) {
   return 0;
 }
 
-int d2pgo_destroy(d2pgo_handle *h) {
-  if (!h) return 0;
-  cudaSetDevice(h->cfg.device);
-  cudaStreamSynchronize(h->stream);
-  if (h->comm) nccl_comm_destroy(h->comm);
+static void pgo_release(d2pgo_handle *h) {   // every device buffer and graph of a handle
   for (int b = 0; b < 2; b++) { h->d_x[b].release(); h->d_g[b].release(); h->d_D[b].release(); h->d_lin[b].release(); if (h->cg_graph[b]) cudaGraphExecDestroy(h->cg_graph[b]); }
   h->d_damp.release(); h->d_t.release(); h->d_part.release(); h->d_cost_part.release(); h->d_inc_ptr.release(); h->d_inc.release();
   h->d_rel.release(); h->d_sinfo.release(); h->d_Minv.release(); h->d_dx.release(); h->d_r.release(); h->d_z.release(); h->d_p.release();
@@ -1050,6 +1172,15 @@ int d2pgo_destroy(d2pgo_handle *h) {
   h->pcm.release();
   h->d_ak_pose.release(); h->d_ak_ptr.release(); h->d_ak_of.release(); h->d_ak_yr.release(); h->d_ak_yl.release(); h->d_ak_qinit.release();
   h->d_ak_lin[0].release(); h->d_ak_lin[1].release(); h->d_ak_coord.release();
+}
+
+int d2pgo_destroy(d2pgo_handle *h) {
+  if (!h) return 0;
+  cudaSetDevice(h->cfg.device);
+  cudaStreamSynchronize(h->stream);
+  if (h->comm) nccl_comm_destroy(h->comm);
+  pgo_release(h);
+  if (h->rot) { pgo_release(h->rot); delete h->rot; }
   cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1); cudaStreamDestroy(h->stream);
   delete h;
   return 0;
@@ -1769,6 +1900,215 @@ int d2pgo_debug_pcm_clique(d2pgo_handle *h, int32_t n, const uint32_t *adj, uint
   int c = 0;
   for (int k = 0; k < n; k++) c += member_out[k];
   if (size_out) *size_out = c;
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- chordal rotation initialisation host side (d2pgo_rot_init)
+static int rot_fail(d2pgo_handle *h, int rc, const std::string &msg) { h->err = "rot_init: " + msg; return rc; }
+
+// Eigen's toRotationMatrix polynomial (q2R of d2ba_math.cuh) on the host, row-major, of the normalised quaternion (Swarm::Pose
+// normalises its attitude)
+static void rot_quat_R(const double *q_xyzw, double *R) {
+  const double n = std::sqrt(q_xyzw[0] * q_xyzw[0] + q_xyzw[1] * q_xyzw[1] + q_xyzw[2] * q_xyzw[2] + q_xyzw[3] * q_xyzw[3]);
+  const double x = q_xyzw[0] / n, y = q_xyzw[1] / n, z = q_xyzw[2] / n, w = q_xyzw[3] / n;
+  const double tx = 2 * x, ty = 2 * y, tz = 2 * z, twx = tx * w, twy = ty * w, twz = tz * w;
+  const double txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
+  const double m[9] = {1 - (tyy + tzz), txy - twz, txz + twy, txy + twz, 1 - (txx + tzz), tyz - twx, txz - twy, tyz + twx, 1 - (txx + tyy)};
+  for (int k = 0; k < 9; k++) R[k] = m[k];
+}
+
+static int rot_find(std::vector<int> &uf, int i) {
+  while (uf[i] != i) { uf[i] = uf[uf[i]]; i = uf[i]; }
+  return i;
+}
+
+// one row system on the inner handle r (poses and edges already set): upload, linearise at x = 0 rows, one undamped
+// Gauss-Newton step by the block-Jacobi PCG of d2pgo_solve, x + dx into r->d_x[1]
+static int rot_solve_row(d2pgo_handle *r, double tol2, int max_it, int *iters, double *residual) {
+  typedef PgoRotRow P;
+  int rc;
+  if ((rc = pgo_upload(r))) return rc;
+  d2pgo_handle *h = r;   // PCK reports into the inner handle
+  PgoDev d = pgo_view(r, 0);
+  const PgoPriorDev pr = pgo_prior_view(r, 0);
+  const int gp = d.nbp, ge = (d.n_edge + 127) / 128;
+  if (d.n_edge > 0) k_pgo_lin<P><<<ge, 128, 0, r->stream>>>(d, r->d_cost_part.p, 1);
+  k_pgo_gD<P, false><<<gp, 128, 0, r->stream>>>(d, r->d_g[0].p, r->d_D[0].p, pr);
+  k_pgo_precond<P><<<gp, 128, 0, r->stream>>>(d, r->d_D[0].p, 0.0);
+  k_pgo_cg_init<P><<<gp, 128, 0, r->stream>>>(d, r->d_g[0].p);
+  k_pgo_cg_init2<<<1, 128, 0, r->stream>>>(d);
+  PgoScalars s; memset(&s, 0, sizeof s);
+  for (int k = 0; k < max_it; k += kCgChunk) {
+    if (!r->cg_graph[0]) {
+      cudaGraph_t g;
+      PCK(cudaStreamBeginCapture(r->stream, cudaStreamCaptureModeThreadLocal));
+      for (int c = 0; c < kCgChunk; c++) {
+        const int par = c & 1;
+        if (d.n_edge > 0) k_pgo_cg_edge<P><<<ge, 128, 0, r->stream>>>(d, par, tol2);
+        k_pgo_cg_pose<P, false, false><<<gp, 128, 0, r->stream>>>(d, par, tol2, pr);
+        k_pgo_cg_step<P><<<gp, 128, 0, r->stream>>>(d, par, tol2);
+      }
+      PCK(cudaStreamEndCapture(r->stream, &g));
+      PCK(cudaGraphInstantiate(&r->cg_graph[0], g, 0));
+      cudaGraphDestroy(g);
+    }
+    PCK(cudaGraphLaunch(r->cg_graph[0], r->stream));
+    PCK(cudaMemcpyAsync(&s, r->d_s.p, sizeof s, cudaMemcpyDeviceToHost, r->stream));
+    PCK(cudaStreamSynchronize(r->stream));
+    if (s.done) break;
+  }
+  k_pgo_retract<P><<<gp, 128, 0, r->stream>>>(d, r->d_x[1].p);
+  // the residual of the last CG update: its r.r partials sit in the parity slot of the last iteration (cg_init: slot 1)
+  std::vector<double> part(d.nbp);
+  const int slot = s.iters == 0 ? 1 : (s.iters - 1) & 1;
+  PCK(cudaMemcpyAsync(part.data(), d.rr_part + (size_t)slot * d.nbp, (size_t)d.nbp * 8, cudaMemcpyDeviceToHost, r->stream));
+  PCK(cudaStreamSynchronize(r->stream));
+  double rr = 0.0;
+  for (double v : part) rr += v;
+  *iters = s.iters;
+  *residual = s.bb > 0.0 ? std::sqrt(rr / s.bb) : 0.0;
+  return 0;
+}
+
+extern "C" {
+
+int d2pgo_default_rot_init_config(d2pgo_rot_init_config *c) {
+  if (!c) return 1;
+  memset(c, 0, sizeof *c);
+  c->enable_gravity_prior = 0; c->pcg_max_iterations = 20000; c->gravity_sqrt_info = 10.0; c->pcg_tolerance = 1e-12;
+  return 0;
+}
+
+int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids, const double *ego_poses7,
+                   d2pgo_rot_init_report *report) {
+  if (!h) return 1;
+  if (!cfg || n_ego < 0 || (n_ego > 0 && (!ego_ids || !ego_poses7))) return rot_fail(h, 1, "null argument or negative count");
+  if (h->dof != 6) return rot_fail(h, 5, "the handle was created with pose_dof = 4; rotation initialisation acts on 6-DoF poses");
+  if (h->comm) return rot_fail(h, 5, "a communicator is attached (edge-sharded rotation initialisation is not supported)");
+  if (h->arock) return rot_fail(h, 5, "the handle is in ARock mode (d2pgo runs the distributed RotationInitARock there)");
+  if (h->ids.empty()) return rot_fail(h, 1, "the handle has no poses");
+  if (!(std::isfinite(cfg->pcg_tolerance) && cfg->pcg_tolerance >= 0.0) || cfg->pcg_max_iterations < 0 ||
+      (cfg->enable_gravity_prior && !std::isfinite(cfg->gravity_sqrt_info)))
+    return rot_fail(h, 2, "non-finite or negative pcg_tolerance, gravity_sqrt_info or pcg_max_iterations");
+  const int N = (int)h->ids.size(), E = (int)h->ea.size();
+  const bool grav = cfg->enable_gravity_prior != 0;
+  // the ego attitudes by pose index (gravity rows only)
+  std::vector<int> ego_of(N, -1);
+  for (int k = 0; k < n_ego; k++) {
+    const std::string which = "ego pose " + std::to_string(k) + " (id " + std::to_string(ego_ids[k]) + ")";
+    auto it = h->index.find(ego_ids[k]);
+    if (it == h->index.end()) return rot_fail(h, 2, which + ": unknown pose id");
+    if (ego_of[it->second] >= 0) return rot_fail(h, 2, which + ": duplicate id");
+    ego_of[it->second] = k;
+    if (!all_finite(ego_poses7 + (size_t)k * 7, 7)) return rot_fail(h, 2, which + ": non-finite value");
+    const double *q = ego_poses7 + (size_t)k * 7 + 3;
+    if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return rot_fail(h, 2, which + ": zero quaternion");
+  }
+  // the frames the edges name (all of them: the reference's all_frames, :444-450), the edges that give rows, and the components
+  // of free frames joined by the edges with both ends free; an edge from a fixed frame anchors its free end's component
+  std::vector<char> named(N, 0), anchored(N, 0);
+  std::vector<int> uf(N), used;
+  for (int i = 0; i < N; i++) uf[i] = i;
+  int dropped = 0;
+  for (int e = 0; e < E; e++) {
+    const int a = h->ea[e], b = h->eb[e];
+    named[a] = named[b] = 1;
+    const bool fa = h->fixed[a] != 0, fb = h->fixed[b] != 0;
+    if (a == b || fb) { dropped++; continue; }   // self loop, both fixed, or b fixed with a free (the :84 quirk)
+    const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
+    if (!all_finite(q, 4) || !(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0) || !all_finite(S, 36))
+      return rot_fail(h, 2, "edge " + std::to_string(e) + ": non-finite or zero relative rotation or square-root information");
+    if (fa && !all_finite(&h->poses[(size_t)a * 8 + 3], 4))
+      return rot_fail(h, 2, "edge " + std::to_string(e) + ": non-finite attitude of its fixed frame");
+    used.push_back(e);
+    if (!fa) uf[rot_find(uf, a)] = rot_find(uf, b);
+  }
+  for (int e : used) if (h->fixed[h->ea[e]]) anchored[rot_find(uf, h->eb[e])] = 1;
+  std::vector<int> frames;   // the free frames solved, ascending pose index
+  for (int i = 0; i < N; i++) {
+    if (!named[i] || h->fixed[i]) continue;
+    if (!anchored[rot_find(uf, i)])
+      return rot_fail(h, 2, "frame id " + std::to_string(h->ids[i]) + ": its component of free frames holds no fixed frame (A^T A is singular)");
+    if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return rot_fail(h, 2, "frame id " + std::to_string(h->ids[i]) + ": non-finite attitude");
+    if (grav && ego_of[i] < 0) return rot_fail(h, 2, "frame id " + std::to_string(h->ids[i]) + ": gravity rows are on and the frame has no ego pose");
+    frames.push_back(i);
+  }
+  d2pgo_rot_init_report R; memset(&R, 0, sizeof R);
+  R.frames = (int)frames.size(); R.edges_used = (int)used.size(); R.edges_dropped = dropped;
+  cudaSetDevice(h->cfg.device);
+  PCK(cudaEventRecord(h->ev0, h->stream));
+  std::vector<double> poses = h->poses;
+  if (!frames.empty()) {
+    // the inner handle: nodes = the handle's poses, then (gravity) one fixed virtual node per solved frame holding R_ego^T e3
+    if (!h->rot) { h->rot = new d2pgo_handle(); h->rot->dof = 3; }
+    d2pgo_handle *r = h->rot;
+    r->cfg = h->cfg; r->stream = h->stream;
+    const int G = grav ? (int)frames.size() : 0, Nn = N + G;
+    r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
+    for (int f : frames) r->fixed[f] = 0;
+    r->ea.clear(); r->eb.clear(); r->rel.clear(); r->sinfo.clear();
+    for (int e : used) {
+      r->ea.push_back(h->ea[e]); r->eb.push_back(h->eb[e]);
+      const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
+      const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+      const double rel[8] = {0, 0, 0, q[0] / n, q[1] / n, q[2] / n, q[3] / n, 0};
+      r->rel.insert(r->rel.end(), rel, rel + 8);
+      double s2 = 0.0;   // |S[3:6, 3:6]|_F
+      for (int i = 3; i < 6; i++) for (int j = 3; j < 6; j++) s2 += S[i * 6 + j] * S[i * 6 + j];
+      const double s = std::sqrt(s2), Si[9] = {s, 0, 0, 0, s, 0, 0, 0, s};
+      r->sinfo.insert(r->sinfo.end(), Si, Si + 9);
+    }
+    std::vector<double> Rfix((size_t)N * 9, 0.0);
+    for (int e : used) if (h->fixed[h->ea[e]]) rot_quat_R(&h->poses[(size_t)h->ea[e] * 8 + 3], &Rfix[(size_t)h->ea[e] * 9]);
+    Buf<double> sol[3];
+    const double tol2 = cfg->pcg_tolerance * cfg->pcg_tolerance;
+    int rc = 0;
+    for (int k = 0; k < 3 && !rc; k++) {
+      r->poses.assign((size_t)Nn * 8, 0.0);
+      for (int i = 0; i < N; i++) if (r->fixed[i]) for (int c = 0; c < 3; c++) r->poses[(size_t)i * 8 + c] = Rfix[(size_t)i * 9 + k * 3 + c];
+      if (k == 2 && G) {   // gravity rows g (r_f^2 - R_ego^T e3): an edge from the virtual node with R_ab = I, S = g I3
+        const double g = cfg->gravity_sqrt_info, Si[9] = {g, 0, 0, 0, g, 0, 0, 0, g}, rel[8] = {0, 0, 0, 0, 0, 0, 1, 0};
+        for (int j = 0; j < G; j++) {
+          double Re[9];
+          rot_quat_R(ego_poses7 + (size_t)ego_of[frames[j]] * 7 + 3, Re);
+          for (int c = 0; c < 3; c++) r->poses[(size_t)(N + j) * 8 + c] = Re[6 + c];   // R_ego^T e3 = third row of R_ego
+          r->ea.push_back(N + j); r->eb.push_back(frames[j]);
+          r->rel.insert(r->rel.end(), rel, rel + 8); r->sinfo.insert(r->sinfo.end(), Si, Si + 9);
+        }
+      }
+      if ((rc = rot_solve_row(r, tol2, cfg->pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) break;
+      if (sol[k].alloc((size_t)Nn * 8) != cudaSuccess ||
+          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, (size_t)Nn * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = rot_fail(h, 100, "device buffer for a row system"); break; }
+    }
+    if (rc && rc != 100) h->err = "rot_init: " + r->err;
+    Buf<double> x, part; Buf<int> fr;
+    const int F = (int)frames.size(), nb = (F + 127) / 128;
+    if (!rc && (x.alloc((size_t)N * 8) != cudaSuccess || part.alloc(nb) != cudaSuccess || fr.alloc(F) != cudaSuccess)) rc = rot_fail(h, 100, "device buffers");
+    if (!rc) {
+      double chg = 0.0;
+      cudaMemcpyAsync(x.p, poses.data(), (size_t)N * 64, cudaMemcpyHostToDevice, h->stream);
+      cudaMemcpyAsync(fr.p, frames.data(), (size_t)F * 4, cudaMemcpyHostToDevice, h->stream);
+      k_rotinit_project<<<nb, 128, 0, h->stream>>>(F, fr.p, sol[0].p, sol[1].p, sol[2].p, x.p, part.p);
+      k_pgo_sum<<<1, 128, 0, h->stream>>>(part.p, nb, r->d_cost.p);
+      cudaMemcpyAsync(&chg, r->d_cost.p, 8, cudaMemcpyDeviceToHost, h->stream);
+      cudaMemcpyAsync(poses.data(), x.p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream);
+      const cudaError_t e = cudaStreamSynchronize(h->stream);
+      if (e != cudaSuccess) rc = rot_fail(h, 100 + (int)e, std::string("projection: ") + cudaGetErrorString(e));
+      R.state_changes = chg / F;
+    }
+    for (int k = 0; k < 3; k++) sol[k].release();
+    x.release(); part.release(); fr.release();
+    if (rc) return rc;
+  }
+  PCK(cudaEventRecord(h->ev1, h->stream));
+  PCK(cudaEventSynchronize(h->ev1));
+  float ms = 0; cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+  R.device_ms = ms;
+  h->poses.swap(poses);   // commit: the solved attitudes; the next d2pgo_solve uploads them
+  h->uploaded = false;
+  if (report) *report = R;
   return 0;
 }
 

@@ -17,7 +17,11 @@ gravity direction of its frame's ego (VIO) pose (include/d2pgo.h d2pgo_add_gravi
 for a make_pose_graph graph.
 
 ARock (d2pgo's distributed pgo_mode 1): `ArockAgent` is one agent's handle in ARock mode (include/d2pgo.h d2pgo_arock_*);
-arock_split builds agent s's sub-graph the way D2PGO::solve_multi does, arock_run runs the synchronous broadcast schedule."""
+arock_split builds agent s's sub-graph the way D2PGO::solve_multi does, arock_run runs the synchronous broadcast schedule.
+
+Rotation initialisation (d2pgo's rotInitial, enable_rotation_initialization): `PgoSolver.rot_init` replaces the attitudes of the
+free frames by d2pgo's chordal relaxation from the handle's edges and fixed frames (include/d2pgo.h d2pgo_rot_init), before
+solve()."""
 import ctypes as C
 
 import numpy as np
@@ -44,6 +48,16 @@ class ArockConfig(C.Structure):
                 ("eta_k", C.c_double)]
 
 
+class RotInitConfig(C.Structure):
+    _fields_ = [("enable_gravity_prior", C.c_int32), ("pcg_max_iterations", C.c_int32), ("gravity_sqrt_info", C.c_double),
+                ("pcg_tolerance", C.c_double)]
+
+
+class RotInitReport(C.Structure):
+    _fields_ = [("frames", C.c_int32), ("edges_used", C.c_int32), ("edges_dropped", C.c_int32), ("pcg_iterations", C.c_int32 * 3),
+                ("residual", C.c_double * 3), ("state_changes", C.c_double), ("device_ms", C.c_double)]
+
+
 class PcmReport(C.Structure):
     _fields_ = [("groups", C.c_int32), ("inliers", C.c_int32), ("pairs_tested", C.c_int64), ("consistent_pairs", C.c_int64),
                 ("clique_rounds", C.c_int64), ("device_ms", C.c_double), ("pair_ms", C.c_double), ("clique_ms", C.c_double)]
@@ -53,7 +67,8 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_comm_init", "d2pgo_solve", "d2pgo_get_poses", "d2pgo_debug_edges", "d2pgo_set_poses_4d", "d2pgo_add_edges_4d",
                 "d2pgo_get_poses_4d", "d2pgo_default_pcm_config", "d2pgo_pcm", "d2pgo_debug_pcm_smd", "d2pgo_debug_pcm_clique",
                 "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors", "d2pgo_default_arock_config", "d2pgo_arock_enable",
-                "d2pgo_arock_receive", "d2pgo_arock_step", "d2pgo_arock_neighbours", "d2pgo_arock_duals", "d2pgo_debug_arock_terms"]
+                "d2pgo_arock_receive", "d2pgo_arock_step", "d2pgo_arock_neighbours", "d2pgo_arock_duals", "d2pgo_debug_arock_terms",
+                "d2pgo_default_rot_init_config", "d2pgo_rot_init"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -135,6 +150,23 @@ class PgoSolver:
         out = np.zeros((max(self.n_priors, 1), 21))
         self._chk(_lib().d2pgo_debug_gravity_priors(self.h, _p(out), C.c_int64(out.size)), "debug_gravity_priors")
         return out[: self.n_priors]
+
+    def rot_init(self, ego_ids=None, ego_poses7=None, **cfg):
+        """Chordal rotation initialisation (d2pgo's rotInitial; include/d2pgo.h d2pgo_rot_init): the attitudes of the free frames
+        the edges name become the SO(3) projections of the linear least-squares rotations; positions, fixed frames and frames
+        no edge names are kept.  cfg overrides RotInitConfig fields (enable_gravity_prior, pcg_max_iterations,
+        gravity_sqrt_info, pcg_tolerance); with enable_gravity_prior every free frame an edge names needs an ego pose
+        [x y z qx qy qz qw] in ego_ids / ego_poses7.  6-DoF only.  Returns the report as a dict."""
+        c = RotInitConfig()
+        _lib().d2pgo_default_rot_init_config(C.byref(c))
+        for k, v in cfg.items():
+            setattr(c, k, v)
+        ids = np.zeros(0, np.int64) if ego_ids is None else np.ascontiguousarray(ego_ids, np.int64)
+        ego = np.zeros((0, 7)) if ego_poses7 is None else np.ascontiguousarray(np.asarray(ego_poses7, np.float64).reshape(-1, 7))
+        r = RotInitReport()
+        self._chk(_lib().d2pgo_rot_init(self.h, C.byref(c), C.c_int32(len(ids)), _p(ids), _p(ego), C.byref(r)), "rot_init")
+        return dict(frames=r.frames, edges_used=r.edges_used, edges_dropped=r.edges_dropped, pcg_iterations=list(r.pcg_iterations),
+                    residual=list(r.residual), state_changes=r.state_changes, device_ms=r.device_ms)
 
     def comm_init(self, unique_id, rank, nranks):
         uid = (C.c_uint8 * 128)(*unique_id)

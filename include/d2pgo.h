@@ -211,6 +211,53 @@ int d2pgo_arock_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t
  * perturbation q (x) Exp(dtheta); the 6-DoF theta block is sqrt(rho_theta) J_r^-1(theta)) */
 int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles);
 
+/* ---- chordal rotation initialisation (d2pgo's rotInitial, enable_rotation_initialization = true by default)
+ *   d2pgo_rot_init  <- RotationInitialization<double>::solve on the non-distributed path (RotInit,
+ *                      d2pgo/src/rot_init/rotation_initialization.cpp:21-28; rotation_initialization_base.hpp:440-456),
+ *                      fed every edge of the handle (D2PGO::rotInitial's used_loops, d2pgo/src/d2pgo.cpp:336-361) and the
+ *                      handle's fixed flags (the fixed frame, :346-349)
+ * Unknowns: the three rows r_f^k of R_f of every free frame an edge names (updateFrameIdx, :57-69).  Per edge with rotation
+ * weight s = |S[3:6, 3:6]|_F (the reference replaces each square-root block by its Frobenius norm times I3):
+ *   a, b free, a != b:   s (R_ab^T r_a^k - r_b^k) = 0                     (setupRotInitProblembyLoop, :89-111)
+ *   a fixed, b free:     s r_b^k = s (row k of R_a R_ab)^T                 (setPriorFactorsbyFixedParam, :72-87; ASSUMED: the
+ *                        prior's rotation square root is that of the edge, so these are the edge rows with r_a held)
+ *   a free, b fixed:     no rows -- the reference attaches that prior to frame b, the fixed frame, which has no unknowns (:84)
+ *   both fixed, a == b:  no rows (:96-102)
+ *   enable_gravity_prior: per free frame an edge names, g (r_f^2 - R_ego,f^T e3) = 0, e3 = (0, 0, 1) (:131-144)
+ * The weights are scalar times I3, so the system splits into three 3N x 3N systems, one per k, sharing the edge structure;
+ * the gravity rows enter k = 2 only.  Each is solved by the block-Jacobi PCG of d2pgo_solve (one Gauss-Newton step from zero,
+ * D = 3 per frame) to pcg_tolerance; the reference factorises A^T A (SimplicialLLT, :146-176).  Each free frame then gets
+ * R_f = U diag(1, 1, det(U V^T)) V^T of the SVD of its solved M_f = [r^0 r^1 r^2]^T (recoverRotationLLT :360-389,
+ * Utility::recoverRotationSVD); its attitude becomes the quaternion of R_f (the sign may differ from the reference's) and its
+ * position keeps every bit.  Fixed frames and frames no edge names keep their poses.  The edges, gravity priors and every
+ * other table of the handle are untouched, so d2pgo_solve can follow directly.  Binary64, no atomics, bitwise reproducible.
+ * Refusals keep nothing of the call and set d2pgo_last_error: 5 on a 4-DoF handle (a 4-DoF PGOState has no rotation states,
+ * pgostate.hpp:31-47), with a communicator attached or in ARock mode (the reference runs RotationInitARock there); 2 when a
+ * component of free frames (joined by the edges that give rows) holds no fixed frame -- A^T A is singular there and the
+ * reference asserts (:173); a free frame named only by dropped edges is such a component --, when gravity rows are on and a
+ * free frame lacks an ego pose, and on an unknown or duplicate ego id or a non-finite value; 1 on a null argument or n < 0. */
+typedef struct d2pgo_rot_init_config {
+  int32_t enable_gravity_prior;   /* RotInitConfig::enable_gravity_prior (d2pgo_config.h:11; d2pgo_test.cpp turns it on)   */
+  int32_t pcg_max_iterations;     /* per row system k (default 20000)                                                       */
+  double gravity_sqrt_info;       /* RotInitConfig default 10                                                               */
+  double pcg_tolerance;           /* relative residual |A^T A x - A^T b| / |A^T b| at which CG stops (default 1e-12)        */
+} d2pgo_rot_init_config;
+
+typedef struct d2pgo_rot_init_report {
+  int32_t frames;                 /* free frames solved                                                                     */
+  int32_t edges_used, edges_dropped;   /* dropped: b fixed with a free, both fixed, self loops                              */
+  int32_t pcg_iterations[3];      /* per row system k                                                                       */
+  double residual[3];             /* relative residual reached per row system (CG recurrence)                               */
+  double state_changes;           /* mean over free frames of |R_before - M_f|_F / |R_before|_F (SolverReport, :376-388)    */
+  double device_ms;
+} d2pgo_rot_init_report;
+
+int d2pgo_default_rot_init_config(d2pgo_rot_init_config *cfg);
+/* ego attitudes are read only with enable_gravity_prior (every free frame an edge touches needs one): ego_poses7[n_ego][7] of
+ * the frames ego_ids, [x y z qx qy qz qw] (the attitude is normalised).  report may be NULL. */
+int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids,
+                   const double *ego_poses7, d2pgo_rot_init_report *report);
+
 #ifdef __cplusplus
 }
 #endif
