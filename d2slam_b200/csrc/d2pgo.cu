@@ -24,6 +24,7 @@
 
 #include "../../include/d2pgo.h"
 #include "d2ba_math.cuh"
+#include "d2pgo_chol.cuh"
 
 namespace d2ba {
 // NCCL through the dlopen'ed entry points of d2ba_host.cu
@@ -1086,6 +1087,8 @@ struct d2pgo_handle {
   const void *ak_key[4] = {nullptr, nullptr, nullptr, nullptr};   // buffers the captured CG graphs point at
   bool graph_ark = false;             // the captured CG graphs carry the proximal terms
   d2pgo_handle *rot = nullptr;        // d2pgo_rot_init's row systems (dof 3), kept between calls for their buffers
+  int linear_solver = D2PGO_LINEAR_PCG;   // d2pgo_set_linear_solver
+  d2pgo_chol::Numeric *chol = nullptr;    // the sparse Cholesky's analysis and device state (d2pgo_chol.cu)
 };
 
 #define PCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return 100 + (int)e_; } } while (0)
@@ -1181,6 +1184,7 @@ int d2pgo_destroy(d2pgo_handle *h) {
   if (h->comm) nccl_comm_destroy(h->comm);
   pgo_release(h);
   if (h->rot) { pgo_release(h->rot); delete h->rot; }
+  delete h->chol;
   cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1); cudaStreamDestroy(h->stream);
   delete h;
   return 0;
@@ -1215,6 +1219,7 @@ int d2pgo_add_edges_4d(d2pgo_handle *h, int32_t n, const int64_t *id_a, const in
 int d2pgo_comm_init(d2pgo_handle *h, const uint8_t unique_id[128], int32_t rank, int32_t nranks) {
   if (!h) return 1;
   if (h->arock) { h->err = "comm_init: the handle is in ARock mode (each agent solves its own sub-graph; edge sharding splits one graph)"; return 5; }
+  if (h->linear_solver == D2PGO_LINEAR_SPARSE_CHOLESKY) { h->err = "comm_init: the handle solves with the sparse Cholesky, which has no edge-sharded form (d2pgo_set_linear_solver PCG first)"; return 5; }
   cudaSetDevice(h->cfg.device);
   if (nccl_comm_init(&h->comm, unique_id, rank, nranks, h->err)) return 3;
   h->rank = rank; h->nranks = nranks;
@@ -1341,11 +1346,50 @@ static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr,
   return 0;
 }
 
+// the sparse Cholesky's symbolic analysis of the handle's current structure (host only: poses, fixed flags, edge ends), redone
+// when that structure changed; then the size limits, before any device work of the solve
+static int pgo_chol_analyse(d2pgo_handle *h) {
+  if (!h->chol) h->chol = new d2pgo_chol::Numeric();
+  d2pgo_chol::Symbolic &S = h->chol->sym;
+  if (S.D == h->dof && S.fixed == h->fixed && S.ea == h->ea && S.eb == h->eb) return 0;
+  h->chol->release();
+  if (int rc = d2pgo_chol::analyse((int)h->ids.size(), h->fixed.data(), (int)h->ea.size(), h->ea.data(), h->eb.data(), h->dof, S, h->err)) {
+    S = d2pgo_chol::Symbolic();
+    return rc;
+  }
+  return 0;
+}
+
+static int pgo_chol_prepare(d2pgo_handle *h) {
+  if (int rc = pgo_chol_analyse(h)) return rc;
+  const d2pgo_chol::Symbolic &S = h->chol->sym;
+  size_t free_b = 0, total_b = 0;
+  PCK(cudaMemGetInfo(&free_b, &total_b));
+  if (!h->chol->dev_ready) {
+    const std::string why = d2pgo_chol::check_limits(S, free_b);
+    if (!why.empty()) { h->err = why; return 7; }
+  }
+  return 0;
+}
+
+// one exact step (J^T J + lambda diag D + 1e-12) dx = -g at linearisation buffer `cur` into d_dx
+static int pgo_chol_step(d2pgo_handle *h, int cur, double lambda, bool *failed) {
+  d2pgo_chol::Numeric &c = *h->chol;
+  if (!c.dev_ready) if (int rc = c.upload(h->stream, h->err)) return rc;
+  const d2pgo_chol::Lin in{h->d_lin[cur].p, h->d_D[cur].p, h->d_g[cur].p, h->d_fixed.p, h->d_ea.p, h->d_eb.p, h->d_dx.p};
+  return c.step(h->stream, cur, in, lambda, failed, h->err);
+}
+
 // the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4), by 6-DoF graphs with gravity priors (GRAV)
 // and by ARock local problems (ARK: the proximal terms of the synced dual table)
 template <class P, bool GRAV, bool ARK = false>
 static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   int rc;
+  const bool chol = h->linear_solver == D2PGO_LINEAR_SPARSE_CHOLESKY;
+  if (chol) {
+    if ((rc = pgo_chol_prepare(h))) return rc;
+    h->chol->factorizations = h->chol->failed = 0; h->chol->factor_ms = h->chol->solve_ms = 0.0;
+  }
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
   const int N = (int)h->ids.size();
   const int gp = (N + 127) / 128;
@@ -1361,11 +1405,21 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
     PgoDev d = pgo_view(h, cur);
     const PgoPriorDev pr = pgo_prior_view(h, cur);
     const PgoArockDev ak = pgo_arock_view(h, cur);
+    PgoScalars s; memset(&s, 0, sizeof s);
+    if (chol) {   // the exact step from the sparse Cholesky; a failed factorisation is a rejected step
+      bool failed = false;
+      if ((rc = pgo_chol_step(h, cur, lambda, &failed))) return rc;
+      if (failed) {
+        R.iterations++;
+        lambda = lambda > 0 ? lambda * 4.0 : 1e-4;
+        if (lambda > 1e8) break;
+        continue;
+      }
+    } else {
     // (J^T J + lambda diag D) dx = -g by block-Jacobi preconditioned CG; J^T J is never formed
     k_pgo_precond<P><<<gp, 128, 0, h->stream>>>(d, h->d_D[cur].p, lambda);
     k_pgo_cg_init<P><<<gp, 128, 0, h->stream>>>(d, h->d_g[cur].p);
     k_pgo_cg_init2<<<1, 128, 0, h->stream>>>(d);
-    PgoScalars s; memset(&s, 0, sizeof s);
     for (int k = 0; k < h->cfg.pcg_max_iterations; k += kCgChunk) {
       if (!h->comm) {
         if (!h->cg_graph[cur]) {
@@ -1381,6 +1435,7 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
       PCK(cudaMemcpyAsync(&s, h->d_s.p, sizeof s, cudaMemcpyDeviceToHost, h->stream));
       PCK(cudaStreamSynchronize(h->stream));
       if (s.done) break;   // identical on every rank (see pgo_cg_chunk)
+    }
     }
     k_pgo_retract<P><<<gp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
     double cand = 0;
@@ -1735,6 +1790,71 @@ int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
   PCK(cudaStreamSynchronize(h->stream));
   for (size_t k = 0; k < K; k++) for (size_t q = 0; q < W; q++) out[k * W + q] = tmp[q * K + k];   // device layout is field-major
   return 0;
+}
+
+}  // extern "C"
+
+// ---- sparse Cholesky (d2pgo_set_linear_solver) host side
+template <class P, bool GRAV, bool ARK>
+static int pgo_exact_step(d2pgo_handle *h, double lambda, double *out) {
+  int rc;
+  if ((rc = pgo_chol_prepare(h))) return rc;
+  if (!h->uploaded && (rc = pgo_upload(h))) return rc;
+  if (ARK && (rc = arock_sync(h))) return rc;
+  double cost;
+  if ((rc = pgo_linearize<P, GRAV, ARK>(h, 0, 1, &cost))) return rc;
+  bool failed = false;
+  if ((rc = pgo_chol_step(h, 0, lambda, &failed))) return rc;
+  PCK(cudaMemcpy(out, h->d_dx.p, h->ids.size() * (size_t)P::D * 8, cudaMemcpyDeviceToHost));
+  if (failed) { h->err = "debug_exact_step: the factorisation met a non-positive or non-finite pivot"; return 6; }
+  return 0;
+}
+
+extern "C" {
+
+int d2pgo_set_linear_solver(d2pgo_handle *h, int32_t kind) {
+  if (!h) return 1;
+  if (kind != D2PGO_LINEAR_PCG && kind != D2PGO_LINEAR_SPARSE_CHOLESKY) {
+    h->err = "set_linear_solver: unknown kind " + std::to_string(kind) + " (0 = PCG, 1 = sparse Cholesky)";
+    return 2;
+  }
+  if (kind == D2PGO_LINEAR_SPARSE_CHOLESKY && h->comm) {
+    h->err = "set_linear_solver: the handle has a communicator; the sparse Cholesky has no edge-sharded form";
+    return 5;
+  }
+  if (kind == D2PGO_LINEAR_PCG && h->chol) {   // the factor's tables, fronts and graphs are not needed by PCG
+    cudaSetDevice(h->cfg.device);
+    cudaStreamSynchronize(h->stream);
+    delete h->chol;
+    h->chol = nullptr;
+  }
+  h->linear_solver = kind;
+  return 0;
+}
+
+int d2pgo_cholesky_stats(d2pgo_handle *h, d2pgo_cholesky_info *out) {
+  if (!h || !out) return 1;
+  memset(out, 0, sizeof *out);
+  if (h->ids.empty()) return 0;
+  if (int rc = pgo_chol_analyse(h)) return rc;   // analysis only: no device work
+  d2pgo_chol::fill_info(h->chol->sym, out);
+  out->factorizations = h->chol->factorizations; out->failed_factorizations = h->chol->failed;
+  out->factor_ms = h->chol->factor_ms; out->solve_ms = h->chol->solve_ms;
+  return 0;
+}
+
+int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64_t out_doubles) {
+  if (!h) return 1;
+  if (!dx_out || h->ids.empty()) { h->err = "debug_exact_step: null argument or no poses"; return 1; }
+  if ((size_t)out_doubles < h->ids.size() * (size_t)h->dof) { h->err = "debug_exact_step: buffer too small: " + std::to_string(h->ids.size() * h->dof) + " doubles needed"; return 2; }
+  if (!(lambda >= 0.0 && std::isfinite(lambda))) { h->err = "debug_exact_step: lambda must be finite and non-negative"; return 2; }
+  if (h->comm) { h->err = "debug_exact_step: the handle has a communicator"; return 5; }
+  if (h->arock) if (int rc = arock_check_poses(h, "debug_exact_step")) return rc;
+  cudaSetDevice(h->cfg.device);
+  const bool ark = h->arock, grav = !h->gp_pose.empty();
+  if (h->dof == 4) return ark ? pgo_exact_step<PgoEdge4, false, true>(h, lambda, dx_out) : pgo_exact_step<PgoEdge4, false, false>(h, lambda, dx_out);
+  if (grav) return ark ? pgo_exact_step<PgoEdge6, true, true>(h, lambda, dx_out) : pgo_exact_step<PgoEdge6, true, false>(h, lambda, dx_out);
+  return ark ? pgo_exact_step<PgoEdge6, false, true>(h, lambda, dx_out) : pgo_exact_step<PgoEdge6, false, false>(h, lambda, dx_out);
 }
 
 }  // extern "C"

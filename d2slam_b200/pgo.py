@@ -21,7 +21,12 @@ arock_split builds agent s's sub-graph the way D2PGO::solve_multi does, arock_ru
 
 Rotation initialisation (d2pgo's rotInitial, enable_rotation_initialization): `PgoSolver.rot_init` replaces the attitudes of the
 free frames by d2pgo's chordal relaxation from the handle's edges and fixed frames (include/d2pgo.h d2pgo_rot_init), before
-solve()."""
+solve().
+
+Linear solver (the reference's ceres linear_solver_type): `PgoSolver(linear_solver="sparse_cholesky")` takes exact LM steps
+from a GPU supernodal sparse Cholesky (d2pgo's SPARSE_NORMAL_CHOLESKY; include/d2pgo.h d2pgo_set_linear_solver) instead of the
+default truncated block-Jacobi PCG ("pcg"); cholesky_stats() reports the factor's structure and timings, cholesky_symbolic() runs
+the host analysis alone."""
 import ctypes as C
 
 import numpy as np
@@ -58,6 +63,34 @@ class RotInitReport(C.Structure):
                 ("residual", C.c_double * 3), ("state_changes", C.c_double), ("device_ms", C.c_double)]
 
 
+class CholeskyInfo(C.Structure):
+    _fields_ = [("free_poses", C.c_int32), ("block_pairs", C.c_int32), ("nnz_L", C.c_int64), ("nnz_L_stored", C.c_int64),
+                ("supernodes", C.c_int32), ("levels", C.c_int32), ("supernodes_fundamental", C.c_int32), ("levels_fundamental", C.c_int32),
+                ("max_front_rows", C.c_int32), ("max_front_cols", C.c_int32), ("factorizations", C.c_int32),
+                ("failed_factorizations", C.c_int32), ("factor_ms", C.c_double), ("solve_ms", C.c_double)]
+
+
+LINEAR_SOLVERS = {"pcg": 0, "sparse_cholesky": 1}
+
+
+def _info_dict(r):
+    return {k: getattr(r, k) for k, _ in CholeskyInfo._fields_}
+
+
+def cholesky_symbolic(n, fixed, ea, eb, dof=6):
+    """The sparse Cholesky's host analysis alone (no device, no handle; include/d2pgo.h d2pgo_cholesky_symbolic): n poses,
+    fixed flags (None = all free), edge ends as pose indices, block size 4 or 6.  Returns dict(perm = pose of each block
+    column [n_free], sn_ptr = first column of each supernode and the end, sn_parent, **the structure counts)."""
+    f = None if fixed is None else np.ascontiguousarray(fixed, np.uint8)
+    a = np.ascontiguousarray(ea, np.int32); b = np.ascontiguousarray(eb, np.int32)
+    perm = np.zeros(max(n, 1), np.int32); ptr = np.zeros(n + 1, np.int32); par = np.zeros(max(n, 1), np.int32); info = CholeskyInfo()
+    rc = _lib().d2pgo_cholesky_symbolic(C.c_int32(n), _p(f), C.c_int32(len(a)), _p(a), _p(b), C.c_int32(dof), _p(perm), _p(ptr), _p(par), C.byref(info))
+    if rc:
+        raise RuntimeError(f"d2pgo_cholesky_symbolic failed rc={rc}")
+    S = info.supernodes
+    return dict(perm=perm[: info.free_poses].copy(), sn_ptr=ptr[: S + 1].copy(), sn_parent=par[:S].copy(), **_info_dict(info))
+
+
 class PcmReport(C.Structure):
     _fields_ = [("groups", C.c_int32), ("inliers", C.c_int32), ("pairs_tested", C.c_int64), ("consistent_pairs", C.c_int64),
                 ("clique_rounds", C.c_int64), ("device_ms", C.c_double), ("pair_ms", C.c_double), ("clique_ms", C.c_double)]
@@ -68,7 +101,8 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_get_poses_4d", "d2pgo_default_pcm_config", "d2pgo_pcm", "d2pgo_debug_pcm_smd", "d2pgo_debug_pcm_clique",
                 "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors", "d2pgo_default_arock_config", "d2pgo_arock_enable",
                 "d2pgo_arock_receive", "d2pgo_arock_step", "d2pgo_arock_neighbours", "d2pgo_arock_duals", "d2pgo_debug_arock_terms",
-                "d2pgo_default_rot_init_config", "d2pgo_rot_init"]
+                "d2pgo_default_rot_init_config", "d2pgo_rot_init", "d2pgo_set_linear_solver", "d2pgo_cholesky_stats",
+                "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -79,7 +113,7 @@ def _p(a):
 
 
 class PgoSolver:
-    def __init__(self, **kw):
+    def __init__(self, linear_solver="pcg", **kw):
         L = _lib()
         L.d2pgo_last_error.restype = C.c_char_p
         L.d2pgo_last_error.argtypes = [C.c_void_p]
@@ -91,8 +125,31 @@ class PgoSolver:
         rc = L.d2pgo_create(C.byref(self.cfg), C.byref(self.h))
         if rc:
             raise RuntimeError(f"d2pgo_create failed rc={rc}: {_CREATE_ERRORS.get(rc, 'CUDA device required; no CPU fallback')}")
+        self.n_poses = 0
         self.n_edges = 0
         self.n_priors = 0
+        if linear_solver != "pcg":
+            self.set_linear_solver(linear_solver)
+
+    def set_linear_solver(self, kind):
+        """"pcg" (the default) or "sparse_cholesky" (include/d2pgo.h d2pgo_set_linear_solver); ints pass through."""
+        k = LINEAR_SOLVERS.get(kind, kind) if isinstance(kind, str) else int(kind)
+        if isinstance(k, str):
+            raise ValueError(f"unknown linear solver {kind!r}: {sorted(LINEAR_SOLVERS)}")
+        self._chk(_lib().d2pgo_set_linear_solver(self.h, C.c_int32(k)), "set_linear_solver")
+
+    def cholesky_stats(self):
+        """Structure counts of the current graph's sparse Cholesky and the counters of the last solve, as a dict."""
+        r = CholeskyInfo()
+        self._chk(_lib().d2pgo_cholesky_stats(self.h, C.byref(r)), "cholesky_stats")
+        return _info_dict(r)
+
+    def debug_exact_step(self, lam):
+        """The sparse Cholesky's step dx [N, D] for damping lam at the current poses (0 on fixed poses); poses unchanged."""
+        D = 4 if self.cfg.pose_dof == 4 else 6
+        out = np.zeros((self.n_poses, D))
+        self._chk(_lib().d2pgo_debug_exact_step(self.h, C.c_double(lam), _p(out), C.c_int64(out.size)), "debug_exact_step")
+        return out
 
     def _chk(self, rc, what):
         if rc:
@@ -112,6 +169,7 @@ class PgoSolver:
         ids = np.ascontiguousarray(ids, np.int64); poses = np.ascontiguousarray(poses, np.float64)
         f = None if fixed is None else np.ascontiguousarray(fixed, np.uint8)
         self._chk(_lib().d2pgo_set_poses(self.h, C.c_int32(len(ids)), _p(ids), _p(poses), _p(f)), "set_poses")
+        self.n_poses = len(ids)
         self.n_edges = 0
         self.n_priors = 0
 
@@ -126,6 +184,7 @@ class PgoSolver:
         ids = np.ascontiguousarray(ids, np.int64); poses4 = np.ascontiguousarray(poses4, np.float64)
         f = None if fixed is None else np.ascontiguousarray(fixed, np.uint8)
         self._chk(_lib().d2pgo_set_poses_4d(self.h, C.c_int32(len(ids)), _p(ids), _p(poses4), _p(f)), "set_poses_4d")
+        self.n_poses = len(ids)
         self.n_edges = 0
         self.n_priors = 0
 

@@ -258,6 +258,50 @@ int d2pgo_default_rot_init_config(d2pgo_rot_init_config *cfg);
 int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids,
                    const double *ego_poses7, d2pgo_rot_init_report *report);
 
+/* ---- linear solver of the LM steps (the reference's ceres linear_solver_type)
+ *   D2PGO_LINEAR_PCG             the default: (J^T J + lambda diag D) dx = -g by block-Jacobi PCG to pcg_tolerance, at most
+ *                                pcg_max_iterations (a truncated step); the only kind with a communicator and for rot init
+ *   D2PGO_LINEAR_SPARSE_CHOLESKY <- SPARSE_NORMAL_CHOLESKY, which d2pgo uses for every pose graph (d2pgo/src/d2pgo_node.cpp:
+ *                                191-195, and the ARock local solves, :202): the exact step from a supernodal multifrontal
+ *                                Cholesky of H = J^T J + lambda diag(D) + 1e-12 I over the free poses, H being exactly the
+ *                                operator PCG applies (self loops included).  Ordering by nested dissection, once per graph
+ *                                structure on the host; factorisation and triangular solves on the device, binary64, no
+ *                                atomics, bitwise reproducible.  A non-positive or non-finite pivot makes the step a rejected
+ *                                one (lambda -> 4 lambda, or 1e-4 from 0).  pcg_iterations stays 0; pcg_* fields are unused.
+ * The kind applies to d2pgo_solve and d2pgo_arock_step, 4-DoF and 6-DoF, with or without gravity priors; d2pgo_rot_init keeps
+ * PCG.  It may change between solves.  Returns 2 on an unknown kind, 5 for the sparse Cholesky on a handle with a
+ * communicator (and d2pgo_comm_init returns 5 on a sparse-Cholesky handle); a refusal keeps nothing.  A solve refuses (7,
+ * before any device work, d2pgo_last_error says why) a structure with a front above 1024 scalar rows or whose fronts need
+ * more than half the free device memory.  Switching back to PCG frees the factor's device memory and graphs. */
+enum { D2PGO_LINEAR_PCG = 0, D2PGO_LINEAR_SPARSE_CHOLESKY = 1 };
+
+typedef struct d2pgo_cholesky_info {
+  int32_t free_poses;
+  int32_t block_pairs;                    /* distinct pairs of free poses an edge joins (self loops excluded)           */
+  int64_t nnz_L;                          /* D x D blocks of L, diagonal included (the exact symbolic count)             */
+  int64_t nnz_L_stored;                   /* blocks stored after relaxed amalgamation (explicit zeros included)          */
+  int32_t supernodes, levels;             /* of the amalgamated supernodal tree: one launch per level and phase          */
+  int32_t supernodes_fundamental, levels_fundamental;   /* before amalgamation                                          */
+  int32_t max_front_rows, max_front_cols; /* scalar                                                                      */
+  int32_t factorizations, failed_factorizations;       /* during the last solve                                          */
+  double factor_ms, solve_ms;             /* device ms of the factorisations (assembly included) and of the triangular
+                                             solves, summed over the last solve                                          */
+} d2pgo_cholesky_info;
+
+int d2pgo_set_linear_solver(d2pgo_handle *h, int32_t kind);
+/* the structure counts of the handle's current graph (analysed on the host if needed) and the counters of the last solve */
+int d2pgo_cholesky_stats(d2pgo_handle *h, d2pgo_cholesky_info *out);
+/* parity hook: linearise at the current poses (edges, gravity priors, ARock proximal terms towards the duals' y_r), factor
+ * and solve for the given lambda; dx_out[N][D] (0 on fixed poses).  The poses do not move.  Returns 6 (dx_out still written)
+ * when a pivot was not positive. */
+int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64_t out_doubles);
+/* the symbolic analysis alone, no device and no handle: n poses, fixed flags (may be NULL), edge ends, D (4 or 6).
+ * perm_out[n]: the pose of each block column (the first info->free_poses entries), sn_ptr_out[n + 1]: the first column of
+ * each supernode and the end (info->supernodes + 1 entries), sn_parent_out[n]: each supernode's parent, -1 for a root.
+ * Returns 1 on a null argument or negative count, 2 on an edge end out of range or another D. */
+int d2pgo_cholesky_symbolic(int32_t n, const uint8_t *fixed, int32_t n_edges, const int32_t *ea, const int32_t *eb, int32_t dof,
+                            int32_t *perm_out, int32_t *sn_ptr_out, int32_t *sn_parent_out, d2pgo_cholesky_info *info);
+
 #ifdef __cplusplus
 }
 #endif
