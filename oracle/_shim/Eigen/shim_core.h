@@ -36,6 +36,7 @@ template <class X, int BR, int BC> class Block;
 template <class M, int MapOpt = 0, class Stride = void> class Map;
 template <class S, int Opt = 0> class Quaternion;
 template <class Derived> class QuaternionBase;
+template <class M> class JacobiSVD;
 
 template <class T> struct traits<const T> : traits<T> {};
 template <class S, int R, int C, int Opt, int MR, int MC> struct traits<Matrix<S, R, C, Opt, MR, MC>> {
@@ -120,6 +121,7 @@ class MatrixBase {
   PlainObject cwiseAbs() const { PlainObject r(*this); for (int j = 0; j < cols(); j++) for (int i = 0; i < rows(); i++) r.ref(i, j) = std::fabs(coeff(i, j)); return r; }
   Scalar determinant() const;
   PlainObject inverse() const;
+  JacobiSVD<PlainObject> jacobiSvd(int opts = 0) const;
   const Derived &format(const IOFormat &) const { return derived(); }
 
   // ---- assignment helpers
@@ -136,6 +138,7 @@ class MatrixBase {
   Derived &setConstant(const Scalar &v) { for (int j = 0; j < cols(); j++) for (int i = 0; i < rows(); i++) coeffRef(i, j) = v; return derived(); }
   Derived &setIdentity() { for (int j = 0; j < cols(); j++) for (int i = 0; i < rows(); i++) coeffRef(i, j) = i == j ? Scalar(1) : Scalar(0); return derived(); }
   template <class O> void applyOnTheLeft(const MatrixBase<O> &m);
+  template <class O> void applyOnTheRight(const MatrixBase<O> &m);
   shim::CommaInit<Derived> operator<<(const Scalar &v);
 
   // ---- blocks
@@ -255,6 +258,7 @@ class Matrix : public MatrixBase<Matrix<S, R, C, Opt, MR, MC>> {
   const S *data() const { return st.p(); }
   void resize(int r, int c) { st.resize(r, c); }
   void resize(int n) { if (C == 1) st.resize(n, 1); else st.resize(1, n); }
+  void conservativeResize(int n) { if (C == 1) conservativeResize(n, 1); else conservativeResize(1, n); }
   void conservativeResize(int r, int c) { Matrix old(*this); st.resize(r, c); for (int j = 0; j < std::min(c, old.cols()); j++) for (int i = 0; i < std::min(r, old.rows()); i++) ref(i, j) = old.get(i, j); }
 
   Matrix() {}
@@ -391,6 +395,7 @@ template <class A> std::ostream &operator<<(std::ostream &os, const MatrixBase<A
   return os;
 }
 template <class D> template <class O> void MatrixBase<D>::applyOnTheLeft(const MatrixBase<O> &m) { PlainObject t = m * (*this); assign(t); }
+template <class D> template <class O> void MatrixBase<D>::applyOnTheRight(const MatrixBase<O> &m) { PlainObject t = (*this) * m; assign(t); }
 
 namespace shim {
 template <class D> struct CommaInit {
@@ -501,6 +506,47 @@ template <class M> class SelfAdjointEigenSolver {   // cyclic Jacobi; eigenvalue
   ComputationInfo info() const { return inf; }
 };
 
+// JacobiSVD of a square matrix, full U and V, singular values descending like Eigen's: V = eigenvectors of A^T A (cyclic Jacobi
+// above), sigma = sqrt of its eigenvalues, U = A V diag(1 / sigma), completed by Gram-Schmidt where sigma = 0.  (Eigen runs a
+// two-sided Jacobi on A; both give the same factorisation up to the signs of paired columns and rounding.)
+template <class M> class JacobiSVD {
+  typedef typename traits<M>::Scalar S;
+  M U, V; Matrix<S, traits<M>::Rows, 1> sv;
+ public:
+  template <class O> explicit JacobiSVD(const MatrixBase<O> &a0, int = 0) {
+    const int n = a0.rows();
+    assert(a0.cols() == n);
+    Matrix<S, Dynamic, Dynamic> A(a0), AtA = Matrix<S, Dynamic, Dynamic>::Zero(n, n);
+    for (int i = 0; i < n; i++) for (int j = 0; j < n; j++) { S t = 0; for (int k = 0; k < n; k++) t += A(k, i) * A(k, j); AtA(i, j) = t; }
+    SelfAdjointEigenSolver<Matrix<S, Dynamic, Dynamic>> es(AtA);
+    U = M::Zero(n, n); V = M::Zero(n, n); sv.resize_(n, 1);
+    for (int j = 0; j < n; j++) {
+      const int c = n - 1 - j;   // eigenvalues ascending -> singular values descending
+      const S l = es.eigenvalues()(c);
+      sv(j) = l > S(0) ? std::sqrt(l) : S(0);
+      for (int i = 0; i < n; i++) V(i, j) = es.eigenvectors()(i, c);
+    }
+    for (int j = 0; j < n; j++) {
+      S nn = 0;
+      for (int i = 0; i < n; i++) { S t = 0; for (int k = 0; k < n; k++) t += A(i, k) * V(k, j); U(i, j) = t; }
+      if (sv(j) > S(0)) { for (int i = 0; i < n; i++) U(i, j) = U(i, j) / sv(j); continue; }
+      for (int e = 0; e < n; e++) {   // Gram-Schmidt of a unit vector against the columns before j
+        for (int i = 0; i < n; i++) U(i, j) = i == e ? S(1) : S(0);
+        for (int p = 0; p < j; p++) { S d = 0; for (int i = 0; i < n; i++) d += U(i, p) * U(i, j); for (int i = 0; i < n; i++) U(i, j) -= d * U(i, p); }
+        nn = 0; for (int i = 0; i < n; i++) nn += U(i, j) * U(i, j);
+        if (nn > S(1e-6)) break;
+      }
+      for (int i = 0; i < n; i++) U(i, j) = U(i, j) / std::sqrt(nn);
+    }
+  }
+  const M &matrixU() const { return U; }
+  const M &matrixV() const { return V; }
+  const Matrix<S, traits<M>::Rows, 1> &singularValues() const { return sv; }
+};
+template <class D> JacobiSVD<typename MatrixBase<D>::PlainObject> MatrixBase<D>::jacobiSvd(int opts) const {
+  return JacobiSVD<PlainObject>(derived(), opts);
+}
+
 // "Sparse" types with Eigen's interface on DENSE storage (the marginalization code of the reference assembles its Jacobian
 // from triplets and takes a sparse LLT; at oracle sizes a dense matrix computes the same numbers).
 template <class S> struct Triplet {
@@ -519,6 +565,16 @@ template <class S, int Opt = 0, class I = int> class SparseMatrix : public Matri
   template <class It> void setFromTriplets(It b, It e) { this->setZero(); for (It t = b; t != e; ++t) this->ref(t->row(), t->col()) += t->value(); }   // duplicates are summed
   Dense toDense() const { return Dense(*this); }
   int nonZeros() const { int n = 0; for (int j = 0; j < this->cols(); j++) for (int i = 0; i < this->rows(); i++) n += this->get(i, j) != S(0); return n; }
+  int outerSize() const { return this->cols(); }
+  class InnerIterator {   // the non-zero entries of column j, rows ascending
+    const SparseMatrix &m; int j, i;
+    void skip() { while (i < m.rows() && m.get(i, j) == S(0)) i++; }
+   public:
+    InnerIterator(const SparseMatrix &m_, int j_) : m(m_), j(j_), i(0) { skip(); }
+    explicit operator bool() const { return i < m.rows(); }
+    InnerIterator &operator++() { i++; skip(); return *this; }
+    int row() const { return i; } int col() const { return j; } S value() const { return m.get(i, j); }
+  };
 };
 template <class M, int UpLo = 1, class Ord = void> class SimplicialLLT {   // dense Cholesky behind the sparse-solver interface
   typedef typename M::Scalar S;

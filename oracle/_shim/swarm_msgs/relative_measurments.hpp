@@ -1,3 +1,3 @@
-// Stand-in for swarm_msgs/relative_measurments.hpp (un-vendored) -- Swarm::LoopEdge lives in the Pose.h stand-in.
+// Stand-in for swarm_msgs/relative_measurments.hpp (un-vendored) -- Swarm::LoopEdge and Swarm::PosePrior live in Pose.h.
 #pragma once
 #include <swarm_msgs/Pose.h>

@@ -4,7 +4,7 @@ A numpy restatement of SwarmLocalOutlierRejection::OutlierRejectionLoopEdges wit
 (d2pgo/src/swarm_outlier_rejection/swarm_outlier_rejection.cpp:46-303) and of FMC::maxCliqueHeu
 (d2pgo/third_party/fast_max-clique_finder/src/findCliqueHeu.cpp:124-243) on bitsets.  Pinned to the reference's own code by
 tests/test_pgo_pcm.py (live through oracle/_ref/libd2ref_pcm.so, and through tests/golden/ref_pcm.npz).  The ASSUMED swarm_msgs semantics are
-those listed in include/d2pgo.h (d2pgo_pcm) and in oracle/_shim_pcm/swarm_msgs/drone_trajectory.hpp."""
+those listed in include/d2pgo.h (d2pgo_pcm) and in oracle/_shim/swarm_msgs/drone_trajectory.hpp."""
 import numpy as np
 
 from d2slam_b200.pgo import _qconj, _qmul, _qrot, quat_yaw

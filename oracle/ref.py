@@ -1,5 +1,6 @@
 """ctypes front-end of oracle/_ref/libd2ref.so: the REFERENCE's own factor classes (compiled unmodified from
-/root/reference by oracle/Makefile.ref against the stand-in headers of oracle/_shim).
+/root/reference by oracle/Makefile.ref against the stand-in headers of oracle/_shim), and `Pin`, which builds and loads
+every library of oracle/Makefile.ref for its front-end module.
 
 TEST INFRASTRUCTURE ONLY: used by tests/test_ref_pin.py (oracle restatement == reference, and the golden vectors under
 tests/golden/ref_factors.npz) and by tests/golden/make_ref_golden.py.  Nothing under d2slam_b200/ imports it.
@@ -12,36 +13,39 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REF_ROOT = os.environ.get("D2SLAM_REF", "/root/reference")
-_LIB = None
 
 
-def so_path():
-    return os.path.join(_HERE, "_ref", "libd2ref.so")
+class Pin:
+    """One reference pin library, oracle/_ref/<name>, built from the sources under REF_ROOT/<subtree>.  Where the reference
+    tree is absent (the GPU machines) the prebuilt file is used as is.  `setup(lib)` runs once on the freshly loaded library."""
 
+    def __init__(self, name, subtree, setup=None):
+        self.name, self.subtree, self.setup, self._lib = name, subtree, setup, None
 
-def available():
-    return os.path.exists(so_path()) or os.path.isdir(os.path.join(REF_ROOT, "d2vins"))
+    def so_path(self):
+        return os.path.join(_HERE, "_ref", self.name)
 
+    def _buildable(self):
+        return os.path.isdir(os.path.join(REF_ROOT, self.subtree))
 
-def build(force=False):
-    """Compile the reference sources where they lie (only possible where /root/reference exists)."""
-    so = so_path()
-    if os.path.isdir(os.path.join(REF_ROOT, "d2vins")):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "Makefile.ref", "-s", f"REF={REF_ROOT}"] + (["-B"] if force else []))
-    if not os.path.exists(so):
-        raise RuntimeError("oracle/_ref/libd2ref.so missing and the reference tree is not present to build it")
-    return so
+    def available(self):
+        return os.path.exists(self.so_path()) or self._buildable()
 
+    def build(self, force=False):
+        """Compile the library where its reference sources lie (a no-op when it is up to date) and return its path."""
+        so = self.so_path()
+        if self._buildable():
+            subprocess.check_call(["make", "-C", _HERE, "-f", "Makefile.ref", "-s", f"REF={REF_ROOT}", f"_ref/{self.name}"] + (["-B"] if force else []))
+        if not os.path.exists(so):
+            raise RuntimeError(f"oracle/_ref/{self.name} missing and the reference tree is not present to build it")
+        return so
 
-def lib():
-    global _LIB
-    if _LIB is None:
-        _LIB = C.CDLL(build())
-        _LIB.ref_proj_eval.restype = C.c_int
-        _LIB.ref_imu_eval.restype = C.c_int
-        _LIB.ref_consensus_eval.restype = C.c_int
-        configure()
-    return _LIB
+    def lib(self):
+        if self._lib is None:
+            self._lib = C.CDLL(self.build())
+            if self.setup is not None:
+                self.setup(self._lib)
+        return self._lib
 
 
 def _p(a):
@@ -49,7 +53,11 @@ def _p(a):
 
 
 def configure(focal_length=460.0, depth_sqrt_inf=20.0, g_norm=9.805, acc_n=0.1, gyr_n=0.05, acc_w=0.002, gyr_w=0.0004):
-    (_LIB or lib()).ref_configure(*[C.c_double(v) for v in (focal_length, depth_sqrt_inf, g_norm, acc_n, gyr_n, acc_w, gyr_w)])
+    lib().ref_configure(*[C.c_double(v) for v in (focal_length, depth_sqrt_inf, g_norm, acc_n, gyr_n, acc_w, gyr_w)])
+
+
+_PIN = Pin("libd2ref.so", "d2vins", setup=lambda _: configure())
+so_path, available, build, lib = _PIN.so_path, _PIN.available, _PIN.build, _PIN.lib
 
 
 _BLOCKS = {0: (7, 7, 7, 1, 1), 1: (7, 7, 7, 7, 1, 1), 2: (7, 7, 1, 1), 3: (7, 7, 7, 1, 1)}

@@ -1,37 +1,22 @@
 """ctypes binding of oracle/_ref/libd2ref_arock.so: the reference's own ARock loop (d2common/src/solver/ARock.cpp compiled
-unmodified, ARockPGO's message handling restated in oracle/ref_arock_driver.cpp) replaying given local solutions.
+unmodified by oracle/Makefile.ref against the stand-in headers of oracle/_shim, ARockPGO's message handling restated in
+oracle/ref_arock_driver.cpp) replaying given local solutions.
 TEST INFRASTRUCTURE: imported by tests/ only."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle.ref import REF_ROOT
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-LIB = os.path.join(HERE, "_ref", "libd2ref_arock.so")
-_L = None
+from oracle.ref import Pin
 
 
-def build():
-    """Compile the pin library from the reference tree (oracle/Makefile.arock); a no-op when it is up to date."""
-    subprocess.check_call(["make", "-C", HERE, "-s", "-f", "Makefile.arock", f"REF={REF_ROOT}"])
+def _setup(lib):
+    lib.ref_arock_run.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_int,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
 
 
-def available():
-    return os.path.exists(LIB)
-
-
-def _lib():
-    global _L
-    if _L is None:
-        _L = C.CDLL(LIB)
-        _L.ref_arock_run.restype = C.c_int
-        _L.ref_arock_run.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_double, C.c_double, C.c_double, C.c_int,
-                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    return _L
+_PIN = Pin("libd2ref_arock.so", "d2common", setup=_setup)
+so_path, available, build, lib = _PIN.so_path, _PIN.available, _PIN.build, _PIN.lib
 
 
 def run(self_ids, frames, owners, init, solved, rho_T, rho_theta, eta, init_zero=False, max_n=256):
@@ -47,7 +32,7 @@ def run(self_ids, frames, owners, init, solved, rho_T, rho_theta, eta, init_zero
     xs = np.ascontiguousarray(np.stack([np.concatenate(s) for s in solved]), np.float64)
     n = np.zeros(R * A, np.int32); keys = np.zeros((R * A, max_n, 2), np.int64)
     yl = np.zeros((R * A, max_n, D)); yr = np.zeros((R * A, max_n, D)); fac = np.zeros((R * A, max_n, D + D * D))
-    rc = _lib().ref_arock_run(A, D, R, p(sid), rho_T, rho_theta, eta, int(init_zero), p(nf), p(fid), p(own), p(x0), p(xs), max_n,
+    rc = lib().ref_arock_run(A, D, R, p(sid), rho_T, rho_theta, eta, int(init_zero), p(nf), p(fid), p(own), p(x0), p(xs), max_n,
                               p(n), p(keys), p(yl), p(yr), p(fac))
     assert rc == 0 and n.max(initial=0) <= max_n
     out = []

@@ -1,49 +1,16 @@
 """ctypes front-end of oracle/_ref/libd2ref_gravity.so: the REFERENCE's own perturbation-mode PGO functors
-(GravityPriorPerturbAD, RelPoseFactorPerturbAD) included unmodified from the reference tree by oracle/Makefile.gravity against
+(GravityPriorPerturbAD, RelPoseFactorPerturbAD) included unmodified from the reference tree by oracle/Makefile.ref against
 the stand-in headers of oracle/_shim, evaluated with doubles (residual) and dual numbers (Jacobians).
 
 TEST INFRASTRUCTURE ONLY: used by tests/test_pgo_gravity.py (oracle/pgo_gravity_oracle.py == reference) and by
 tests/golden/make_ref_gravity_golden.py.  Nothing under d2slam_b200/ imports it.
 """
-import ctypes as C
-import os
-import subprocess
-
 import numpy as np
 
-from oracle.ref import REF_ROOT
+from oracle.ref import Pin, _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def so_path():
-    return os.path.join(_HERE, "_ref", "libd2ref_gravity.so")
-
-
-def available():
-    return os.path.exists(so_path()) or os.path.isdir(os.path.join(REF_ROOT, "d2common"))
-
-
-def build(force=False):
-    """Compile the reference's functors where they lie (only possible where the reference tree exists)."""
-    so = so_path()
-    if os.path.isdir(os.path.join(REF_ROOT, "d2common")):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "Makefile.gravity", "-s", f"REF={REF_ROOT}"] + (["-B"] if force else []))
-    if not os.path.exists(so):
-        raise RuntimeError("oracle/_ref/libd2ref_gravity.so missing and the reference tree is not present to build it")
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _LIB = C.CDLL(build())
-    return _LIB
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+_PIN = Pin("libd2ref_gravity.so", "d2common")
+so_path, available, build, lib = _PIN.so_path, _PIN.available, _PIN.build, _PIN.lib
 
 
 def _f64(a, n):

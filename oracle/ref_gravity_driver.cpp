@@ -1,5 +1,5 @@
 // ref_gravity_driver.cpp -- C entry points over the REFERENCE's own perturbation-mode PGO functors
-// (oracle/_ref/libd2ref_gravity.so, oracle/Makefile.gravity).
+// (oracle/_ref/libd2ref_gravity.so, oracle/Makefile.ref).
 //
 // TEST INFRASTRUCTURE ONLY.  d2common/include/d2common/solver/GravityPrior.hpp (GravityPriorPerturbAD) and RelPoseFactor.hpp
 // (RelPoseFactorPerturbAD), the functors d2pgo builds in its 6-DoF configuration (perturb_mode = true; d2pgo.cpp:427-433,
@@ -8,34 +8,6 @@
 // q = q0 (x) quatfromRotationVector(theta).  This file only builds the reference's objects from flat arrays and calls them --
 // no factor arithmetic of its own.
 #include <Eigen/Dense>
-
-// GravityPriorPerturbAD maps its residual as Map<Matrix<T, 1, 3>> and calls applyOnTheRight(S) (*this = *this * S, Eigen's
-// documented semantics), which oracle/_shim's Map does not have.  Rather than change the stand-in the other pin libraries are
-// built against, this library gets a partial specialisation of Map for 1x3 row vectors: the primary template's members plus
-// applyOnTheRight, declared before the reference header instantiates the type.
-namespace Eigen {
-template <class S, int MO, class St>
-class Map<Matrix<S, 1, 3>, MO, St> : public MatrixBase<Map<Matrix<S, 1, 3>, MO, St>> {
-  S *p;
-  typedef MatrixBase<Map> Base;
-
- public:
-  typedef S Scalar;
-  explicit Map(const S *ptr) : p(const_cast<S *>(ptr)) {}
-  Map(const Map &) = default;
-  int rows_() const { return 1; }
-  int cols_() const { return 3; }
-  void resize_(int r, int c) { (void)r; (void)c; assert(r == 1 && c == 3); }
-  S get(int i, int j) const { (void)i; return p[j]; }
-  S &ref(int i, int j) { (void)i; return p[j]; }
-  S *data() { return p; }
-  const S *data() const { return p; }
-  template <class O> Map &operator=(const MatrixBase<O> &o) { typename MatrixBase<O>::PlainObject tmp(o); Base::assign(tmp); return *this; }
-  Map &operator=(const Map &o) { typename Base::PlainObject tmp(o); Base::assign(tmp); return *this; }
-  template <class O> void applyOnTheRight(const MatrixBase<O> &m) { typename Base::PlainObject t = (*this) * m; Base::assign(t); }
-};
-}  // namespace Eigen
-
 #include <d2common/solver/GravityPrior.hpp>
 #include <d2common/solver/RelPoseFactor.hpp>
 

@@ -1,11 +1,11 @@
-// ref_pcm_driver.cpp -- C entry points over the REFERENCE's own PCM code (oracle/_ref/libd2ref_pcm.so, oracle/Makefile.pcm).
+// ref_pcm_driver.cpp -- C entry points over the REFERENCE's own PCM code (oracle/_ref/libd2ref_pcm.so, oracle/Makefile.ref).
 //
 // TEST INFRASTRUCTURE ONLY.  d2pgo/src/swarm_outlier_rejection/swarm_outlier_rejection.cpp (SwarmLocalOutlierRejection) and
 // d2pgo/third_party/fast_max-clique_finder/src/*.cpp (FMC) are compiled unmodified; their un-vendored dependencies are the
-// stand-ins of oracle/_shim_pcm and oracle/_shim.  This file only builds the reference's objects from flat arrays and calls
+// stand-ins of oracle/_shim.  This file only builds the reference's objects from flat arrays and calls
 // them -- no PCM arithmetic of its own.  ref_pcm feeds every loop once, in the order given, with redundant = true,
 // incremental_pcm = false and the debug-file paths off; loop `id` = its index.  The smd of every tested pair is read from the
-// Swarm::computeSquaredMahalanobisDistance stand-in (oracle/_shim_pcm/swarm_msgs/drone_trajectory.hpp) in the reference's call
+// Swarm::computeSquaredMahalanobisDistance stand-in (oracle/_shim/swarm_msgs/drone_trajectory.hpp) in the reference's call
 // order: groups in std::map order of (max drone id, min drone id), rows i ascending, j ascending.
 #include <cstdint>
 #include <map>

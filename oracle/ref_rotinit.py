@@ -1,50 +1,18 @@
 """ctypes front-end of oracle/_ref/libd2ref_rotinit.so: the REFERENCE's own chordal rotation initialisation
 (RotationInitialization<double>::solve in d2pgo/src/rot_init/rotation_initialization_base.hpp, with pgostate.hpp and
-utils.hpp) included unmodified from the reference tree by oracle/Makefile.rotinit against the stand-in headers of
-oracle/_shim_rotinit, oracle/_shim_pcm and oracle/_shim.
+utils.hpp) included unmodified from the reference tree by oracle/Makefile.ref against the stand-in headers of oracle/_shim.
 
 TEST INFRASTRUCTURE ONLY: used by tests/test_pgo_rotinit.py (oracle/pgo_rotinit_oracle.py == reference) and by
 tests/golden/make_ref_rotinit_golden.py.  Nothing under d2slam_b200/ imports it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle.ref import REF_ROOT
+from oracle.ref import Pin, _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def so_path():
-    return os.path.join(_HERE, "_ref", "libd2ref_rotinit.so")
-
-
-def available():
-    return os.path.exists(so_path()) or os.path.isdir(os.path.join(REF_ROOT, "d2pgo"))
-
-
-def build(force=False):
-    """Compile the reference's rotation initialisation where it lies (only possible where the reference tree exists)."""
-    so = so_path()
-    if os.path.isdir(os.path.join(REF_ROOT, "d2pgo")):
-        subprocess.check_call(["make", "-C", _HERE, "-f", "Makefile.rotinit", "-s", f"REF={REF_ROOT}"] + (["-B"] if force else []))
-    if not os.path.exists(so):
-        raise RuntimeError("oracle/_ref/libd2ref_rotinit.so missing and the reference tree is not present to build it")
-    return so
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        _LIB = C.CDLL(build())
-    return _LIB
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+_PIN = Pin("libd2ref_rotinit.so", "d2pgo")
+so_path, available, build, lib = _PIN.so_path, _PIN.available, _PIN.build, _PIN.lib
 
 
 def rot_init(ids, poses, fixed, id_a, id_b, rel, sqrt_info, gravity=False, gravity_sqrt_info=10.0, ego_ids=None, ego_poses=None):

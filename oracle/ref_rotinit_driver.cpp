@@ -1,5 +1,5 @@
 // ref_rotinit_driver.cpp -- C entry point over the REFERENCE's own chordal rotation initialisation
-// (oracle/_ref/libd2ref_rotinit.so, oracle/Makefile.rotinit).
+// (oracle/_ref/libd2ref_rotinit.so, oracle/Makefile.ref).
 //
 // TEST INFRASTRUCTURE ONLY.  d2pgo/src/rot_init/rotation_initialization_base.hpp (RotationInitialization<double>, the
 // non-distributed RotInit path of rotation_initialization.cpp:21-28) and d2pgo/src/pgostate.hpp are included unmodified.  This

@@ -15,8 +15,7 @@ import test_pgo_arock as t  # noqa: E402
 from oracle import ref_arock  # noqa: E402
 
 
-def main():
-    ref_arock.build()
+def arrays():
     out = {}
     for name in t.PIN_CASES:
         c = t.pin_case(name)
@@ -36,7 +35,11 @@ def main():
                 out[f"{name}/r{r}/a{a}/keys"] = np.array(g["keys"], np.int64).reshape(-1, 2)
                 for k in ("yl", "yr", "fac"):
                     out[f"{name}/r{r}/a{a}/{k}"] = g[k]
-    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_arock.npz"), **out)
+    return out
+
+
+def main():
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_arock.npz"), **arrays())
 
 
 if __name__ == "__main__":

@@ -13,11 +13,15 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import test_pgo_gravity as t  # noqa: E402
 
 
-def main():
+def arrays():
     cases = t.reference_cases()
     out = {f"case_{k}": v for k, v in cases.items()}
     out.update(t.reference_outputs(cases))
-    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_gravity.npz"), **out)
+    return out
+
+
+def main():
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_gravity.npz"), **arrays())
 
 
 if __name__ == "__main__":

@@ -14,7 +14,7 @@ from oracle import ref_pcm as ref  # noqa: E402
 import test_pgo_pcm as t  # noqa: E402
 
 
-def main():
+def arrays():
     out = {}
     case = t.small_case()
     for k, v in case.items():
@@ -30,7 +30,11 @@ def main():
     cl = [sorted(ref.fmc_heu(a)) for a in graphs]
     out["fmc_size"] = np.array([len(c) for c in cl], np.int32)
     out["fmc_clique"] = np.array(sum(cl, []), np.int32)
-    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_pcm.npz"), **out)
+    return out
+
+
+def main():
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_pcm.npz"), **arrays())
 
 
 if __name__ == "__main__":

@@ -13,11 +13,15 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import test_pgo_rotinit as t  # noqa: E402
 
 
-def main():
+def arrays():
     cases = t.reference_cases()
     out = {f"case_{name}__{f}": np.asarray(c[f]) for name, c in cases.items() for f in t.FIELDS}
     out.update(t.reference_outputs(cases))
-    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_rotinit.npz"), **out)
+    return out
+
+
+def main():
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "ref_rotinit.npz"), **arrays())
 
 
 if __name__ == "__main__":
