@@ -1857,6 +1857,24 @@ int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64
   return ark ? pgo_exact_step<PgoEdge6, false, true>(h, lambda, dx_out) : pgo_exact_step<PgoEdge6, false, false>(h, lambda, dx_out);
 }
 
+int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out, int32_t max_pairs, int32_t *n_pairs_out,
+                                int32_t *pair_ab_out, double *pair_out) {
+  if (!h) return 1;
+  if (!diag_out || !b_out || !n_pairs_out || max_pairs < 0 || (max_pairs > 0 && (!pair_ab_out || !pair_out))) {
+    h->err = "debug_cholesky_system: null argument or negative count";
+    return 1;
+  }
+  const d2pgo_chol::Numeric *c = h->chol;
+  if (!c || !c->has_system || c->sym.D != h->dof || c->sym.fixed != h->fixed || c->sym.ea != h->ea || c->sym.eb != h->eb) {
+    h->err = "debug_cholesky_system: no sparse-Cholesky step on the handle's current structure";
+    return 5;
+  }
+  *n_pairs_out = c->sym.n_pairs;
+  if (max_pairs < c->sym.n_pairs) { h->err = "debug_cholesky_system: room for " + std::to_string(max_pairs) + " pairs, " + std::to_string(c->sym.n_pairs) + " needed"; return 2; }
+  cudaSetDevice(h->cfg.device);
+  return h->chol->system(h->stream, diag_out, b_out, max_pairs, pair_ab_out, pair_out, h->err);
+}
+
 }  // extern "C"
 
 // ---- PCM host side

@@ -574,7 +574,7 @@ void Numeric::release() {
   for (void *p : bufs) cudaFree(p);
   bufs.clear();
   for (auto &e : ev) { if (e) cudaEventDestroy(e); e = nullptr; }
-  dev_ready = false;
+  dev_ready = has_system = false;
 }
 
 int Numeric::upload(cudaStream_t st, std::string &err) {
@@ -650,9 +650,33 @@ int Numeric::step(cudaStream_t st, int par, const Lin &in, double lambda, bool *
   CCK(cudaStreamSynchronize(st));
   float a = 0.f, b = 0.f;
   cudaEventElapsedTime(&a, ev[0], ev[1]); cudaEventElapsedTime(&b, ev[1], ev[2]);
-  factor_ms += a; solve_ms += b; factorizations++;
+  factor_ms += a; solve_ms += b; factorizations++; has_system = true;
   if (h_fail) failed++;
   *failed_out = h_fail != 0;
+  return 0;
+}
+
+int Numeric::system(cudaStream_t st, double *diag, double *b, int max_pairs, int32_t *pair_ab, double *pair_H, std::string &err) {
+  const Symbolic &S = sym;
+  const int D = S.D, DD = D * D, nf = S.n_free, P = std::min(max_pairs, S.n_pairs);
+  std::vector<double> dg((size_t)nf * DD), bv((size_t)nf * D);
+  if (nf) {
+    CCK(cudaMemcpyAsync(dg.data(), d_diagH, dg.size() * 8, cudaMemcpyDeviceToHost, st));
+    CCK(cudaMemcpyAsync(bv.data(), d_b, bv.size() * 8, cudaMemcpyDeviceToHost, st));
+  }
+  if (P > 0) CCK(cudaMemcpyAsync(pair_H, d_pairH, (size_t)P * DD * 8, cudaMemcpyDeviceToHost, st));
+  CCK(cudaStreamSynchronize(st));
+  memset(diag, 0, (size_t)S.n_pose * DD * 8);
+  memset(b, 0, (size_t)S.n_pose * D * 8);
+  for (int j = 0; j < nf; j++) {
+    const int i = S.perm[j];
+    for (int r = 0; r < D; r++) for (int c = 0; c < D; c++) diag[(size_t)i * DD + r * D + c] = dg[(size_t)j * DD + std::max(r, c) * D + std::min(r, c)];
+    for (int r = 0; r < D; r++) b[(size_t)i * D + r] = bv[(size_t)j * D + r];
+  }
+  for (int p = 0; p < P; p++) {
+    const int e = S.pair_edge[S.pair_ptr[p]], lo = S.pair_lo[p];
+    pair_ab[2 * p] = lo; pair_ab[2 * p + 1] = S.ea[e] == lo ? S.eb[e] : S.ea[e];
+  }
   return 0;
 }
 

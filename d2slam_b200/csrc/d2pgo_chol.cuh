@@ -65,6 +65,7 @@ struct Numeric {
   Lin gkey[2] = {};             // the buffers each parity's graphs were captured with
   cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
   double h_lambda = 0.0; int h_fail = 0;
+  bool has_system = false;      // d_pairH / d_diagH / d_b hold the system of a step on these buffers
   // counters of the last solve
   int factorizations = 0, failed = 0; double factor_ms = 0.0, solve_ms = 0.0;
 
@@ -76,6 +77,10 @@ struct Numeric {
   // (H + damping) dx = -g at the buffers `in` (parity `par` picks the captured graphs): *failed = a non-positive or non-finite
   // pivot.  Synchronises the stream.
   int step(cudaStream_t st, int par, const Lin &in, double lambda, bool *failed, std::string &err);
+  // copies of the last step's assembled system by pose index (has_system): diag[n_pose][D*D] (lower triangle as factored,
+  // mirrored; 0 on fixed poses), b[n_pose][D] (0 on fixed poses), the first max_pairs pairs' pose indices pair_ab[][2] (lo, hi)
+  // and blocks pair_H[][D*D] (sum J_lo^T J_hi).  Synchronises the stream.
+  int system(cudaStream_t st, double *diag, double *b, int max_pairs, int32_t *pair_ab, double *pair_H, std::string &err);
 };
 
 }  // namespace d2pgo_chol

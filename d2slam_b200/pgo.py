@@ -102,7 +102,7 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors", "d2pgo_default_arock_config", "d2pgo_arock_enable",
                 "d2pgo_arock_receive", "d2pgo_arock_step", "d2pgo_arock_neighbours", "d2pgo_arock_duals", "d2pgo_debug_arock_terms",
                 "d2pgo_default_rot_init_config", "d2pgo_rot_init", "d2pgo_set_linear_solver", "d2pgo_cholesky_stats",
-                "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic"]
+                "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic", "d2pgo_debug_cholesky_system"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -150,6 +150,17 @@ class PgoSolver:
         out = np.zeros((self.n_poses, D))
         self._chk(_lib().d2pgo_debug_exact_step(self.h, C.c_double(lam), _p(out), C.c_int64(out.size)), "debug_exact_step")
         return out
+
+    def debug_cholesky_system(self):
+        """The system the last sparse-Cholesky step on this handle factored, as the device assembled it (include/d2pgo.h
+        d2pgo_debug_cholesky_system): dict(diag [N, D, D] damped diagonal blocks, b [N, D] = -g (both 0 on fixed poses),
+        pairs [P, 2] pose indices a < b of each distinct free pair, pair_blocks [P, D, D] H_ab)."""
+        D = 4 if self.cfg.pose_dof == 4 else 6
+        P = self.cholesky_stats()["block_pairs"]
+        diag = np.zeros((self.n_poses, D, D)); b = np.zeros((self.n_poses, D))
+        ab = np.zeros((max(P, 1), 2), np.int32); H = np.zeros((max(P, 1), D, D)); n = C.c_int32()
+        self._chk(_lib().d2pgo_debug_cholesky_system(self.h, _p(diag), _p(b), C.c_int32(P), C.byref(n), _p(ab), _p(H)), "debug_cholesky_system")
+        return dict(diag=diag, b=b, pairs=ab[: n.value], pair_blocks=H[: n.value])
 
     def _chk(self, rc, what):
         if rc:

@@ -295,6 +295,14 @@ int d2pgo_cholesky_stats(d2pgo_handle *h, d2pgo_cholesky_info *out);
  * and solve for the given lambda; dx_out[N][D] (0 on fixed poses).  The poses do not move.  Returns 6 (dx_out still written)
  * when a pivot was not positive. */
 int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64_t out_doubles);
+/* parity hook: the system the last sparse-Cholesky step on the handle (d2pgo_debug_exact_step or an LM iteration) assembled on
+ * the device and factored, copied out (no other device work): diag_out[N][D*D] the damped diagonal block of each pose
+ * (row-major, the factored lower triangle mirrored; 0 on fixed poses), b_out[N][D] the right-hand side -g (0 on fixed poses),
+ * and the *n_pairs_out distinct pairs of free poses an edge joins, ascending: pair_ab_out[P][2] their pose indices a < b and
+ * pair_out[P][D*D] the block H_ab = sum of J_a^T J_b over their edges.  Returns 5 when no step was taken on the handle's
+ * current structure, 2 (with *n_pairs_out set) when max_pairs < P. */
+int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out, int32_t max_pairs, int32_t *n_pairs_out,
+                                int32_t *pair_ab_out, double *pair_out);
 /* the symbolic analysis alone, no device and no handle: n poses, fixed flags (may be NULL), edge ends, D (4 or 6).
  * perm_out[n]: the pose of each block column (the first info->free_poses entries), sn_ptr_out[n + 1]: the first column of
  * each supernode and the end (info->supernodes + 1 entries), sn_parent_out[n]: each supernode's parent, -1 for a root.
