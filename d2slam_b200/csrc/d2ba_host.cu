@@ -55,6 +55,7 @@ void launch_chol(const Dev &d, int max_rows, cudaStream_t s);
 size_t chol_smem_need(int n);
 int configure_chol_smem(int max_n);
 void launch_chol_smem(const Dev &d, int max_n, cudaStream_t s);
+int chol_smem_threads(int max_n);
 size_t sb_elim_smem(int ldw, int n_c, int nb);
 size_t sb_back_smem(int nlc, int nb);
 int configure_sb_back(size_t smem);
@@ -173,6 +174,7 @@ struct HostWin {
   std::vector<int> order;            // pair-major order: sorted index -> observation index
   std::vector<int> sorted_pos;       // tile slot (window-local) of the k-th sorted observation
   std::vector<int> canon_of_dev;     // device reduced column -> canonical (insertion-order) column, for the debug views
+  int n_g12 = 0, n_schur_tiles[2] = {0, 0};   // k_lm_gather12 chunks and Schur tiles of stages 0 / 1 (D2BA_DBG_PLAN)
   void clear() {   // keeps every allocation (the estimator re-adds a similar problem for the next solve)
     used = false;
     pose_id.clear(); ext_id.clear(); sb_id.clear(); lm_id.clear();
@@ -841,6 +843,17 @@ int d2ba_finalize(d2ba_handle *h) {
     if (h->win[i].used) { if ((int)i != nw) return fail(h, 20, "windows must be used contiguously from index 0"); nw++; }
   }
   if (nw == 0) return fail(h, 22, "finalize: no window in use");
+  for (int wi = 0; wi < nw; wi++) {
+    // the landmark tile masks (lm_mask, Schur chunk masks) are 64-bit, one bit per 32 columns of [W | rhs]: the rhs
+    // column n_lc must fall in tile 63 or lower.  2047 columns are 341 six-dof blocks.
+    const HostWin &w = h->win[wi];
+    int nlc = (w.has_td && !w.td_c) ? 1 : 0;
+    for (uint8_t c : w.pose_c) nlc += c ? 0 : 6;
+    for (uint8_t c : w.ext_c) nlc += c ? 0 : 6;
+    if (nlc / 32 >= 64)
+      return fail(h, 27, "finalize: window " + std::to_string(wi) + " has " + std::to_string(nlc) +
+                             " landmark-coupled columns; at most 2047 are supported (64-bit landmark tile masks)");
+  }
   Staging &st = *staging_of(h);
   // the pinned staging buffers are rewritten below: wait for the uploads of the previous finalize of this handle
   // (normally long complete -- a solve synchronises the stream); the uploads enqueued by THIS call are not waited for
@@ -1225,6 +1238,7 @@ int d2ba_finalize(d2ba_handle *h) {
       int t_lo = d.n_lc / 32, t_hi = d.n_c / 32;
       if (!d.sb_elim) for (int tm = t_lo; tm <= t_hi; tm++) for (int tn = 0; tn <= tm; tn++) pl.schur[1].push_back(SchurTileH{wi, 1, tm, tn, 0, 0});
     }
+    w.n_g12 = (int)pl.g12.size(); w.n_schur_tiles[0] = (int)pl.schur[0].size(); w.n_schur_tiles[1] = (int)pl.schur[1].size();
   });
   {   // k_solve_small pays off through the wave count: it runs each window with 4 warps where the separate kernels have 8,
       // and wins only once those kernels need more than one wave (k_step: 3 CTAs per SM).  Smaller batches (the
@@ -1862,6 +1876,13 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     case D2BA_DBG_N_CAM: { int64_t v = n; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
     case D2BA_DBG_N_LC: { int64_t v = nlc; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
     case D2BA_DBG_SOLVE_PATH: { int64_t v = d.fused_solve ? 1 : 0; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
+    case D2BA_DBG_PLAN: {   // field order: include/d2ba.h
+      const int64_t v[20] = {d.fused_solve, d.schur_small, d.hub_small, d.chol_smem, h->cs_unfused ? chol_smem_threads(h->max_n_smem) : 0,
+                             d.sb_elim, d.n_sbe, d.n_leaf, d.hub0, d.n_hub,
+                             d.n_lc, d.n_c, d.ldw, d.rec_stride, d.gather_nosync, d.row_tiles,
+                             w->n_g12, d.n_tile, w->n_schur_tiles[0], w->n_schur_tiles[1]};
+      buf.resize(sizeof v); memcpy(buf.data(), v, sizeof v); break;
+    }
     case D2BA_DBG_HCC: {   // Hcc is stored lower-triangular in device column order: symmetric, canonical order out
       auto H = fetch(h->d_H[cur].p + d.offH, (size_t)n * ld);
       std::vector<double> o((size_t)n * n);

@@ -2969,6 +2969,7 @@ cudaError_t raise_smem_limit(K kernel, size_t bytes) {
   if (bytes <= c) return cudaSuccess;
   e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
   if (e == cudaSuccess) c = bytes;
+  else cudaGetLastError();   // the refusal is reported through the return value; a later cudaGetLastError check must not see it again
   return e;
 }
 
@@ -3109,10 +3110,10 @@ size_t chol_smem_need(int n) { return chol_smem_bytes(n); }
 int configure_chol_smem(int max_n) {
   return (int)raise_smem_limit(k_chol_smem, (size_t)(chol_smem_bytes(max_n)));
 }
+// small systems (after the speed-bias elimination): 4 warps per window so that several windows share an SM
+int chol_smem_threads(int max_n) { return max_n <= 96 ? 128 : kCsThreads; }
 void launch_chol_smem(const Dev &d, int max_n, cudaStream_t s) {
-  // small systems (after the speed-bias elimination): 4 warps per window so that several windows share an SM
-  const int threads = max_n <= 96 ? 128 : kCsThreads;
-  k_chol_smem<<<d.n_win, threads, chol_smem_bytes(max_n), s>>>(d);
+  k_chol_smem<<<d.n_win, chol_smem_threads(max_n), chol_smem_bytes(max_n), s>>>(d);
 }
 __global__ void k_zero_sb_rows(Dev d) {
   const WinDesc &w = d.win[blockIdx.x];

@@ -214,6 +214,11 @@ class Solver:
                   "debug_get")
         return out[: need.value // np.dtype(dtype).itemsize]
 
+    def debug_plan(self, window):
+        """The solve plan d2ba_finalize chose for a window (kernel choices and sizes), as a dict keyed by abi.PLAN_FIELDS."""
+        v = self.debug_get(window, abi.DBG_PLAN, np.int64)
+        return dict(zip(abi.PLAN_FIELDS, (int(x) for x in v)))
+
 
 KERNEL_NAMES = ["lm_gather", "schur", "chol", "step", "misc_lin", "proj_lin", "control"]
 

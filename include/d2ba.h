@@ -245,6 +245,8 @@ int d2ba_comm_init(d2ba_handle *h, const uint8_t unique_id[128], int32_t rank, i
 int d2ba_consensus_buffer(d2ba_handle *h, void **dev_ptr, int64_t *n_doubles);
 
 /* ---------------------------------------------------------------- solve + output */
+/* Refuses (27) a window with 2048 or more landmark-coupled columns (free pose / extrinsic blocks x 6, + 1 for a free td),
+ * and (23) a window whose kernels need more shared memory than the device grants; d2ba_reset makes the handle usable again. */
 int d2ba_finalize(d2ba_handle *h);
 int d2ba_solve(d2ba_handle *h, d2ba_report *reports /* [n windows in use], may be NULL */);
 /* Run exactly `iters` trust-region iterations on every window without convergence exits
@@ -287,9 +289,14 @@ enum d2ba_debug_item {
   D2BA_DBG_CONS_RESJAC = 15, /* per six-dof block (poses then extrinsics, input order) 62 doubles: x[7], z[7], tilde[6],
                                 r[6], J (6 x 6) row-major tangent of ConsenusPoseFactor at the current state; zeros for
                                 blocks outside the consensus set                                                       */
-  D2BA_DBG_SOLVE_PATH = 16   /* int64 scalar: 1 when the window's reduced system is solved by the one-kernel path
+  D2BA_DBG_SOLVE_PATH = 16,  /* int64 scalar: 1 when the window's reduced system is solved by the one-kernel path
                                 (k_solve_small), 0 when by the separate Schur / Cholesky / step kernels (also for
                                 windows that fit the one-kernel path in a handle with fewer than 3 of them per SM)    */
+  D2BA_DBG_PLAN = 17         /* int64[20], the window's solve plan as d2ba_finalize chose it: fused_solve, schur_small,
+                                hub_small, chol_smem, k_chol_smem threads of the handle (0: not launched), sb_elim, n_sbe,
+                                n_leaf, hub0, n_hub, n_lc, n_c, ldw, rec_stride, gather_nosync, row_tiles,
+                                k_lm_gather12 chunks, observation tiles, Schur tiles of stage 0, of stage 1; needs no
+                                d2ba_debug_linearize                                                                   */
 };
 /* Linearise at the current state (no step) so that the debug items are defined. */
 int d2ba_debug_linearize(d2ba_handle *h);
