@@ -22,10 +22,15 @@ TERM_NO_CONVERGENCE, TERM_FUNCTION_TOL, TERM_GRADIENT_TOL, TERM_PARAMETER_TOL, T
 
 # d2ba_debug_item
 (DBG_N_CAM, DBG_HCC, DBG_GC, DBG_HLL, DBG_GL, DBG_W, DBG_COST, DBG_S, DBG_N_LC, DBG_OBS_INDEX,
- DBG_COL_OF_BLOCK, DBG_PROJ_RESJAC, DBG_STEP, DBG_GN_STEP, DBG_IMU_RESJAC, DBG_CONS_RESJAC, DBG_SOLVE_PATH, DBG_PLAN) = range(18)
+ DBG_COL_OF_BLOCK, DBG_PROJ_RESJAC, DBG_STEP, DBG_GN_STEP, DBG_IMU_RESJAC, DBG_CONS_RESJAC, DBG_SOLVE_PATH, DBG_PLAN,
+ DBG_LIN_JOBS) = range(19)
 # the int64 fields of DBG_PLAN, in order
 PLAN_FIELDS = ("fused_solve", "schur_small", "hub_small", "chol_smem", "chol_threads", "sb_elim", "n_sbe", "n_leaf", "hub0", "n_hub",
                "n_lc", "n_c", "ldw", "rec_stride", "gather_nosync", "row_tiles", "n_g12", "n_tile", "schur0", "schur1")
+# DBG_LIN_JOBS: the kernel variants in launch_proj_lin's index order, the five counts kept for each, then two scalars
+LIN_VARIANTS = ("proj_lin<2,2>", "proj_lin<4,2>", "proj_lin<2,4>", "proj_lin<4,4>",
+                "pp<true,false>", "pp<false,false>", "pp<true,true>", "pp<false,true>")
+LIN_JOBS_FIELDS = ("groups", "jobs", "tiles", "obs", "max_tiles_per_job")
 
 
 class Config(C.Structure):

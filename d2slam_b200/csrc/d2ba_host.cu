@@ -175,6 +175,7 @@ struct HostWin {
   std::vector<int> sorted_pos;       // tile slot (window-local) of the k-th sorted observation
   std::vector<int> canon_of_dev;     // device reduced column -> canonical (insertion-order) column, for the debug views
   int n_g12 = 0, n_schur_tiles[2] = {0, 0};   // k_lm_gather12 chunks and Schur tiles of stages 0 / 1 (D2BA_DBG_PLAN)
+  int64_t lin_jobs[8][5] = {};                // per launch_proj_lin variant: groups, jobs, tiles, observations, most tiles in one job (D2BA_DBG_LIN_JOBS)
   void clear() {   // keeps every allocation (the estimator re-adds a similar problem for the next solve)
     used = false;
     pose_id.clear(); ext_id.clear(); sb_id.clear(); lm_id.clear();
@@ -294,6 +295,7 @@ struct d2ba_handle {
   int max_row_tiles = 1;
   int any_compact = 0, any_wide = 0;   // record widths present (which gather kernels to launch)
   int n_g12 = 0;                       // k_lm_gather12 chunks (windows with 96-byte records)
+  int tpj_target = 1;                  // observation tiles per reprojection job of the last finalize (D2BA_DBG_LIN_JOBS)
   size_t sbb_smem = 0, cfg_sbb_smem = 0;   // k_sb_back dynamic shared memory
   size_t sbe_smem = 0, cfg_sbe_smem = 0;   // speed-bias elimination: dynamic shared memory of k_sb_elim (0 = no window uses it)
   // one-kernel reduced-system solve (k_solve_small) of the windows with WinDesc::fused_solve; the separate kernels are
@@ -875,6 +877,7 @@ int d2ba_finalize(d2ba_handle *h) {
   int n_sm = 132;   // H100 SXM; the device's own count when it can be read
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->cfg.device);
   const int tpj_target = std::max(1, std::min(8, tiles_est / (n_sm * 8)));
+  h->tpj_target = tpj_target;
   // ---- pass A (parallel): columns, pair-major order, groups, tiles, jobs, Schur tiles
   parallel_for(nw, [&](int wi) {
     HostWin &w = h->win[wi];
@@ -1153,6 +1156,15 @@ int d2ba_finalize(d2ba_handle *h) {
       }
     }
     pl.n_lmobs = (int)M;
+    for (int v = 0; v < 8; v++) {   // the final routing (after the 96-byte record swap): a group's jobs are consecutive
+      int64_t *c = w.lin_jobs[v];
+      for (int q = 0; q < 5; q++) c[q] = 0;
+      for (size_t j = 0; j < pl.jobs[v].size(); j++) {
+        const Job &jb = pl.jobs[v][j];
+        if (j == 0 || pl.jobs[v][j - 1].grp != jb.grp) { c[0]++; c[3] += pl.grp_cnt[jb.grp]; }
+        c[1]++; c[2] += jb.ntiles; c[4] = std::max<int64_t>(c[4], jb.ntiles);
+      }
+    }
     d.schur_small = (d.n_lc + 1 <= 96) ? 1 : 0;
     d.hub_small = (d.n_leaf > 0 && d.n_hub + 1 <= 96) ? 1 : 0;
     {
@@ -1881,6 +1893,12 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
                              d.sb_elim, d.n_sbe, d.n_leaf, d.hub0, d.n_hub,
                              d.n_lc, d.n_c, d.ldw, d.rec_stride, d.gather_nosync, d.row_tiles,
                              w->n_g12, d.n_tile, w->n_schur_tiles[0], w->n_schur_tiles[1]};
+      buf.resize(sizeof v); memcpy(buf.data(), v, sizeof v); break;
+    }
+    case D2BA_DBG_LIN_JOBS: {   // field order: include/d2ba.h
+      int64_t v[42];
+      memcpy(v, w->lin_jobs, sizeof w->lin_jobs);
+      v[40] = motion_needed(*w) ? 1 : 0; v[41] = h->tpj_target;
       buf.resize(sizeof v); memcpy(buf.data(), v, sizeof v); break;
     }
     case D2BA_DBG_HCC: {   // Hcc is stored lower-triangular in device column order: symmetric, canonical order out

@@ -219,6 +219,15 @@ class Solver:
         v = self.debug_get(window, abi.DBG_PLAN, np.int64)
         return dict(zip(abi.PLAN_FIELDS, (int(x) for x in v)))
 
+    def debug_lin_jobs(self, window):
+        """How d2ba_finalize routed a window's reprojection factors: {variant: {field: count}} keyed by abi.LIN_VARIANTS and
+        abi.LIN_JOBS_FIELDS, plus "motion_needed" and "tpj_target"."""
+        v = [int(x) for x in self.debug_get(window, abi.DBG_LIN_JOBS, np.int64)]
+        n = len(abi.LIN_JOBS_FIELDS)
+        out = {name: dict(zip(abi.LIN_JOBS_FIELDS, v[n * i:n * (i + 1)])) for i, name in enumerate(abi.LIN_VARIANTS)}
+        out["motion_needed"], out["tpj_target"] = v[8 * n], v[8 * n + 1]
+        return out
+
 
 KERNEL_NAMES = ["lm_gather", "schur", "chol", "step", "misc_lin", "proj_lin", "control"]
 

@@ -292,11 +292,16 @@ enum d2ba_debug_item {
   D2BA_DBG_SOLVE_PATH = 16,  /* int64 scalar: 1 when the window's reduced system is solved by the one-kernel path
                                 (k_solve_small), 0 when by the separate Schur / Cholesky / step kernels (also for
                                 windows that fit the one-kernel path in a handle with fewer than 3 of them per SM)    */
-  D2BA_DBG_PLAN = 17         /* int64[20], the window's solve plan as d2ba_finalize chose it: fused_solve, schur_small,
+  D2BA_DBG_PLAN = 17,        /* int64[20], the window's solve plan as d2ba_finalize chose it: fused_solve, schur_small,
                                 hub_small, chol_smem, k_chol_smem threads of the handle (0: not launched), sb_elim, n_sbe,
                                 n_leaf, hub0, n_hub, n_lc, n_c, ldw, rec_stride, gather_nosync, row_tiles,
                                 k_lm_gather12 chunks, observation tiles, Schur tiles of stage 0, of stage 1; needs no
                                 d2ba_debug_linearize                                                                   */
+  D2BA_DBG_LIN_JOBS = 18     /* int64[42], how d2ba_finalize routed the window's reprojection factors: for each of the 8
+                                kernel variants (k_proj_lin<2,2>, <4,2>, <2,4>, <4,4>, k_proj_lin_pp<true,false>,
+                                <false,false>, <true,true>, <false,true>) groups, jobs, tiles, observations and the most
+                                tiles in one job; then 1 when the window uploads the motion halves (td - td_i can be
+                                non-zero), and the handle's tiles-per-job target; needs no d2ba_debug_linearize       */
 };
 /* Linearise at the current state (no step) so that the debug items are defined. */
 int d2ba_debug_linearize(d2ba_handle *h);

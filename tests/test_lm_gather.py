@@ -46,24 +46,47 @@ def make_solver(windows, monkeypatch, rec128, **cfg):
     return s
 
 
+GATHERS = ("k_lm_gather12", "k_lm_gather16")
+
+
 def gather_views(windows, monkeypatch, rec128):
-    """DBG_W / DBG_HLL / DBG_GL of every window after one debug linearisation, and the gather kernels it launched."""
+    """DBG_W / DBG_HLL / DBG_GL of every window after one debug linearisation, each window's plan (D2BA_DBG_PLAN), and
+    the gather kernels the linearisation launched.  A kernel counts when its (possibly mangled) name contains the kernel's
+    name.  The device work is bracketed by synchronisations and 50 ms of host time inside the profiled region, so that
+    no kernel record falls outside the profiler's window when the GPU and host clocks are a little apart: the
+    linearisation of three bench windows lasts about a millisecond."""
+    import time
+
+    import torch
     from torch.profiler import ProfilerActivity, profile
     s = make_solver(windows, monkeypatch, rec128)
+    torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        time.sleep(0.05)
         s.debug_linearize()
-    kernels = {e.name.split("(")[0].split("<")[0].replace("void ", "").replace("d2ba::", "").strip() for e in prof.events()}
+        torch.cuda.synchronize()
+        time.sleep(0.05)
+    names = [e.name for e in prof.events()]
     out = [{item: s.debug_get(i, item) for item in VIEWS} for i in range(len(windows))]
+    plans = [s.debug_plan(i) for i in range(len(windows))]
     s.close()
-    return out, {k for k in kernels if k.startswith("k_lm_gather")}
+    return out, plans, {k for k in GATHERS if any(k in n for n in names)}
 
 
 @pytest.mark.parametrize("batch", ["bench", "mixed"])
 def test_rows_bitwise_equal_to_128_byte_records(batch, monkeypatch):
     windows = bench_windows() if batch == "bench" else mixed_windows()
-    new, k_new = gather_views(windows, monkeypatch, rec128=False)
-    old, k_old = gather_views(windows, monkeypatch, rec128=True)
+    new, p_new, k_new = gather_views(windows, monkeypatch, rec128=False)
+    old, p_old, k_old = gather_views(windows, monkeypatch, rec128=True)
+    # the plan: 96-byte records and k_lm_gather12 chunks exactly where D2BA_REC128 is off and the window is eligible
+    eligible = [i for i, p in enumerate(p_new) if p["rec_stride"] == 12]
+    assert eligible == ([0, 1, 2] if batch == "bench" else [0, 1, 5]), [p["rec_stride"] for p in p_new]
+    for i in range(len(windows)):
+        assert (p_new[i]["n_g12"] > 0) == (i in eligible), (i, p_new[i])
+        assert p_old[i]["n_g12"] == 0 and p_old[i]["rec_stride"] == (16 if i in eligible else p_new[i]["rec_stride"]), (i, p_old[i])
+    # the kernels the linearisation launched
     assert "k_lm_gather12" in k_new and "k_lm_gather12" not in k_old, (k_new, k_old)
+    assert "k_lm_gather16" in k_old
     if batch == "mixed":
         assert "k_lm_gather16" in k_new   # the ineligible windows keep their records and kernel
     for i in range(len(windows)):

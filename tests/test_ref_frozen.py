@@ -30,6 +30,7 @@ PINS = {
     "ref_gravity": ("make_ref_gravity_golden", ref_gravity),
     "ref_arock": ("make_ref_arock_golden", ref_arock),
     "ref_rotinit": ("make_ref_rotinit_golden", ref_rotinit),
+    "ref_lin_edges": ("make_ref_lin_edges_golden", ref),
 }
 MARG = re.compile(r"marg(\d+)_(refs|x0|J|e0)")
 
