@@ -11,9 +11,9 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
-#include <map>
 #include <mutex>
 #include <thread>
 #include <string>
@@ -253,6 +253,42 @@ struct HBuf {   // pinned host staging buffer (grows, never shrinks)
   void release() { if (p) cudaFreeHost(p); p = nullptr; cap = n = 0; }
 };
 
+template <typename T>
+struct HView {   // typed slice of the pinned staging arena
+  T *p = nullptr; size_t n = 0, off = 0;
+};
+struct Staging {   // every array finalize uploads lives in ONE pinned arena -> one H2D copy into one device arena
+  HBuf<char> arena; size_t cursor = 0;
+  HView<WinDesc> win; HView<double> x6, xsb, xlm, xtd, imu_c, prior_J, prior_e0;
+  HView<int> col6, colsb, tile_grp, tile_win, obs_lm, tile_src, lm_ptr, obs_slot, slot6, lm_win, blk_win, sb_win, pr_m, pr_info;
+  HView<long long> raw_off, pr_offJ, pr_offv;
+  HView<Group> grp; HView<Job> job; HView<ImuDesc> imu; HView<PriorBlk> pblk; HView<SchurTileH> schur;
+  HView<int> schur_chunks, leaf_lm; HView<Leaf> leaf; HView<HSeg> hseg; HView<unsigned long long> lm_mask; HView<int4> g12;
+  template <typename T> void reserve(HView<T> &v, size_t count) { v.n = count; v.off = cursor; cursor += (count * sizeof(T) + 255) & ~(size_t)255; }
+  template <typename T> void place(HView<T> &v) { v.p = (T *)(arena.p + v.off); }
+};
+
+// What d2ba_finalize derives for the handle as a whole: array totals, the maxima the kernels are sized and configured for,
+// and which kernels the iteration launches.  Value-initialised by every finalize.
+struct LaunchSummary {
+  int n_used = 0, n6_total = 0, nsb_total = 0, nl_total = 0, n_tiles = 0, n_imu_total = 0, n_slots = 0;   // windows, blocks, ...
+  int n_grp = 0, n_lmptr = 0, n_pblk = 0, n_leaf_total = 0, n_hseg = 0, n_leaf_lm = 0, n_chunks = 0, n_g12 = 0;
+  int n_schur = 0, n_schur0 = 0;                     // Schur tiles; the first n_schur0 are stage 0 (leaf columns)
+  int n_jobs = 0, job_begin[8] = {}, job_count[8] = {};   // reprojection jobs per launch_proj_lin variant
+  int tpj_target = 1;                                // observation tiles per reprojection job (D2BA_DBG_LIN_JOBS)
+  int64_t totH = 0, totW = 0, totc = 0, totLE = 0, totLL = 0, tot_rec = 0, tot_pJ = 0, tot_pv = 0;   // doubles
+  int max_nc = 1, max_prior_m = 0, max_row_tiles = 1, max_ldw_small = 0;
+  int max_n_smem = 0, max_rows_glob = 1; bool any_chol_glob = false;   // dense Cholesky: shared-memory / global kernel
+  int any_compact = 0, any_wide = 0;                 // record widths present (which gather kernels to launch)
+  bool any_admm = false, any_info = false;           // consensus terms / a prior given in information form
+  // dynamic shared memory of k_leaf_elim, k_leaf_back, k_sb_elim and k_sb_back (0 = no window uses the kernel)
+  size_t leaf_smem = 0, leafb_smem = 0, sbe_smem = 0, sbb_smem = 0;
+  // one-kernel reduced-system solve (k_solve_small) of the windows with WinDesc::fused_solve; the separate kernels are
+  // launched only when some window still needs them
+  int n_fused = 0; size_t fused_smem = 0;
+  bool ss_unfused = false, cs_unfused = false, sbb_unfused = false;
+};
+
 }  // namespace
 
 struct d2ba_handle {
@@ -262,7 +298,6 @@ struct d2ba_handle {
   cudaStream_t stream = nullptr, copy_stream = nullptr;
   cudaStream_t side = nullptr;                 // second lane of the iteration: IMU chain beside the reprojection kernels, sb elimination beside the landmark gather
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool two_lanes = true;                       // D2BA_ONE_LANE=1: everything on `stream` (A/B)
   cudaEvent_t ev_copy = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   cudaEvent_t ev_it[2] = {nullptr, nullptr};   // solver time budget: iteration k-2 complete
@@ -279,33 +314,17 @@ struct d2ba_handle {
   DBuf<double> d_obs, d_rec[2], d_imu_c, d_imu_pk, d_imu_U, d_prior_J, d_prior_e0, d_prior_A, d_z6, d_tilde6, d_lm_ref, d_sb_ref, d_td_ref,
       d_cons, d_H[2], d_gc[2], d_Wt, d_dinv, d_hl, d_gl, d_S, d_gred, d_D2c, d_gn_c, d_gn_l, d_step_c, d_step_l, d_wu, d_uc, d_D2l, d_dbg;
   DBuf<SchurTileH> d_schur; DBuf<int> d_schur_chunks; DBuf<Leaf> d_leaf; DBuf<HSeg> d_hseg; DBuf<unsigned long long> d_lm_mask; DBuf<double> d_leafL; DBuf<int> d_leaf_lm; DBuf<int4> d_g12;
-  int n_schur0 = 0, n_leaf_total = 0, max_hub = 0; size_t leaf_smem = 0, cfg_leaf_smem = 0, leafb_smem = 0, cfg_leafb_smem = 0;
   DBuf<int> d_pr_m, d_pr_info, d_tile_src; DBuf<long long> d_pr_oJ, d_pr_ov, d_raw_off;
-  int cfg_max_rows = -1, cfg_max_nc = -1, cfg_max_prior = -1, cfg_max_ldw = -1;
+  DBuf<double> d_sbLE;
   Dev dev;
   std::vector<WinDesc> h_win;
   HBuf<Ctl> h_ctl;   // pinned: D2H target of every solve
-  std::vector<Group> h_grp;
-  std::vector<int> h_tile_win;
-  int n_used = 0, n6_total = 0, nsb_total = 0, nl_total = 0, n_tiles = 0, n_imu_total = 0, n_schur = 0;
-  int job_begin[8] = {0, 0, 0, 0, 0, 0, 0, 0}, job_count[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  int max_rows = 1, max_nc = 1, max_prior_m = 0, max_ldw = 8, n_slots = 0;
-  int max_n_smem = 0, max_rows_glob = 1; bool any_chol_glob = false; int cfg_max_n_smem = -1;
-  int max_ldw_small = 0, cfg_max_ldw_small = -1;
-  int max_row_tiles = 1;
-  int any_compact = 0, any_wide = 0;   // record widths present (which gather kernels to launch)
-  int n_g12 = 0;                       // k_lm_gather12 chunks (windows with 96-byte records)
-  int tpj_target = 1;                  // observation tiles per reprojection job of the last finalize (D2BA_DBG_LIN_JOBS)
-  size_t sbb_smem = 0, cfg_sbb_smem = 0;   // k_sb_back dynamic shared memory
-  size_t sbe_smem = 0, cfg_sbe_smem = 0;   // speed-bias elimination: dynamic shared memory of k_sb_elim (0 = no window uses it)
-  // one-kernel reduced-system solve (k_solve_small) of the windows with WinDesc::fused_solve; the separate kernels are
-  // launched only when some window still needs them
-  int n_fused = 0; size_t fused_smem = 0, cfg_fused_smem = 0;
-  bool ss_unfused = false, cs_unfused = false, sbb_unfused = false;
-  int64_t totLE = 0;
-  DBuf<double> d_sbLE;
-  int64_t totH = 0, totW = 0, totc = 0;
-  bool any_admm = false;
+  Staging st;
+  LaunchSummary ls;
+  // what the kernel attributes were last configured for (they outlive a finalize)
+  std::array<int, 3> cfg_kernels = {-1, -1, -1};   // configure_kernels: max_rows_glob, max_nc, max_prior_m
+  int cfg_max_ldw = -1, cfg_max_ldw_small = -1, cfg_max_n_smem = -1;
+  size_t cfg_leaf_smem = 0, cfg_leafb_smem = 0, cfg_sbb_smem = 0, cfg_sbe_smem = 0, cfg_fused_smem = 0;
   // host mirrors of the solved state
   HBuf<double> h_x6[2], h_xsb[2], h_xlm[2], h_xtd[2];   // pinned D2H targets
   // graph cache
@@ -355,12 +374,6 @@ void release_graph(d2ba_handle *h) {
 }
 
 template <typename T>
-int upload(d2ba_handle *h, DBuf<T> &b, const std::vector<T> &v) {
-  CK(b.alloc(v.size()));
-  if (!v.empty()) CK(cudaMemcpyAsync(b.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, h->stream));
-  return 0;
-}
-template <typename T>
 int alloc_zero(d2ba_handle *h, DBuf<T> &b, size_t n) {
   CK(b.alloc(n));
   CK(cudaMemsetAsync(b.p, 0, std::max<size_t>(n, 1) * sizeof(T), h->stream));
@@ -368,8 +381,6 @@ int alloc_zero(d2ba_handle *h, DBuf<T> &b, size_t n) {
 }
 
 }  // namespace
-
-void d2ba_release_staging(d2ba_handle *h);
 
 extern "C" {
 
@@ -409,7 +420,6 @@ int d2ba_create(const d2ba_config *cfg, d2ba_handle **out) {
   cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking); cudaEventCreateWithFlags(&h->ev_copy, cudaEventDisableTiming);
   cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking);
   cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming); cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming);
-  { const char *e = getenv("D2BA_ONE_LANE"); h->two_lanes = !(e && e[0] == '1'); }
   memset(&h->dev, 0, sizeof(h->dev));
   *out = h;
   return 0;
@@ -437,7 +447,7 @@ int d2ba_destroy(d2ba_handle *h) {
   for (auto &w : h->win) { w.rawj.release(); w.anch.release(); w.d_rawj.release(); w.d_anch.release(); w.rawjm.release(); w.anchm.release(); w.d_rawjm.release(); w.d_anchm.release(); }
   cudaStreamDestroy(h->copy_stream); cudaEventDestroy(h->ev_copy);
   cudaStreamSynchronize(h->side); cudaStreamDestroy(h->side); cudaEventDestroy(h->ev_fork); cudaEventDestroy(h->ev_join);
-  d2ba_release_staging(h);
+  h->st.arena.release();
   cudaEventDestroy(h->ev_it[0]); cudaEventDestroy(h->ev_it[1]);
   cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1); cudaEventDestroy(h->evf0); cudaEventDestroy(h->evf1); cudaEventDestroy(h->evf2);
   cudaStreamDestroy(h->stream);
@@ -456,7 +466,7 @@ int d2ba_reset(d2ba_handle *h) {
 }
 
 const char *d2ba_last_error(const d2ba_handle *h) { return h ? h->err.c_str() : "null handle"; }
-int d2ba_num_windows(const d2ba_handle *h) { return h ? h->n_used : 0; }
+int d2ba_num_windows(const d2ba_handle *h) { return h ? h->ls.n_used : 0; }
 
 int d2ba_set_blocks(d2ba_handle *h, int32_t window, int32_t kind, int32_t n, const int64_t *ids, const double *values,
                     const uint8_t *is_const) {
@@ -761,8 +771,23 @@ int d2ba_set_consensus(d2ba_handle *h, int32_t window, int32_t n, const d2ba_blo
 
 namespace {
 
+constexpr int kSmallCols = 96;                         // [W | rhs] at most this wide: the one-CTA dense path (k_schur_small)
+constexpr size_t kElimSmemCap = (size_t)200 * 1024;    // leaf and speed-bias elimination kernels
+constexpr size_t kCholSmemCap = (size_t)232448 - 16;   // k_chol_smem: 16 B of static shared memory (fail flag + mbarrier)
+
+struct PlanOpts {   // the handle's switches the window planner reads
+  bool force_full_S, no_leaf, no_sb_elim, rec128, no_fused_solve;
+  int tpj_target;   // observation tiles per reprojection job
+};
+
+// One window's plan.  The plan_* steps fill it, in order, from the window and PlanOpts alone (no handle, no CUDA call), so
+// pass A runs them for all windows in parallel.
 struct WinPlan {
   WinDesc d;
+  std::vector<int> leaf_of;                          // pose block -> its leaf (-1: hub or constant)
+  bool sb_ok = false;                                // speed-bias part block-tridiagonal and within k_sb_elim's block limit
+  bool any_wide = false, all_pp = true;              // some group needs 4 column slots / every group takes k_proj_lin_pp
+  bool leaves_without_sb_elim = false;               // internal inconsistency: reported by d2ba_last_error, not a failure
   std::vector<Group> groups;
   std::vector<int> grp_begin, grp_cnt, grp_tile0;   // sorted-obs range and first (window-local) tile of each group
   std::vector<Job> jobs[8];                         // tile_begin window-local, grp window-local; index = launch_proj_lin variant
@@ -774,7 +799,6 @@ struct WinPlan {
   int schur_off[2] = {0, 0}, chunk_off = 0;
   std::vector<int4> g12; int g12_off = 0;          // k_lm_gather12 chunks {window, first, end landmark, 0} (rec_stride == 12)
 };
-
 template <typename F>
 void parallel_for(int n, F f) {
   int nt = (int)std::thread::hardware_concurrency();
@@ -788,59 +812,668 @@ void parallel_for(int n, F f) {
   for (int t = 0; t < nt; t++) th.emplace_back([&]() { for (;;) { int i = next.fetch_add(1); if (i >= n) break; f(i); } });
   for (auto &t : th) t.join();
 }
-
-template <typename T>
-struct HView {   // typed slice of the pinned staging arena
-  T *p = nullptr; size_t n = 0, off = 0;
-};
-struct Staging {   // every array finalize uploads lives in ONE pinned arena -> one H2D copy into one device arena
-  HBuf<char> arena; size_t cursor = 0;
-  HView<WinDesc> win; HView<double> x6, xsb, xlm, xtd, imu_c, prior_J, prior_e0;
-  HView<int> col6, colsb, tile_grp, tile_win, obs_lm, tile_src, lm_ptr, obs_slot, slot6, lm_win, blk_win, sb_win, pr_m, pr_info;
-  HView<long long> raw_off;
-  HView<long long> pr_offJ, pr_offv;
-  HView<Group> grp; HView<Job> job; HView<ImuDesc> imu; HView<PriorBlk> pblk; HView<SchurTileH> schur;
-  HView<int> schur_chunks, leaf_lm; HView<Leaf> leaf; HView<HSeg> hseg; HView<unsigned long long> lm_mask; HView<int4> g12;
-  template <typename T> void reserve(HView<T> &v, size_t count) { v.n = count; v.off = cursor; cursor += (count * sizeof(T) + 255) & ~(size_t)255; }
-  template <typename T> void place(HView<T> &v) { v.p = (T *)(arena.p + v.off); }
-};
-std::map<d2ba_handle *, Staging *> g_staging;   // owned per handle, freed in d2ba_destroy
-std::mutex g_staging_mu;
-
-Staging *staging_of(d2ba_handle *h) {
-  std::lock_guard<std::mutex> lk(g_staging_mu);
-  auto it = g_staging.find(h);
-  if (it != g_staging.end()) return it->second;
-  Staging *s = new Staging();
-  g_staging[h] = s;
-  return s;
+// Hcc pattern (lower triangle, block rows): one (row, c0, c1) run per row of a block some factor writes.  One flat list,
+// sorted and merged by plan_hcc: no per-row allocations on this per-solve path.
+void hblock(std::vector<uint64_t> &hruns, int ra, int rs, int ca, int cs) {
+  if (ra < 0 || ca < 0) return;
+  if (ra < ca) { std::swap(ra, ca); std::swap(rs, cs); }
+  for (int r = 0; r < rs; r++) hruns.push_back(((uint64_t)(ra + r) << 40) | ((uint64_t)ca << 20) | (uint64_t)(ca + cs));
 }
-
-template <typename T>
-int up(d2ba_handle *h, DBuf<T> &b, const HView<T> &v) {   // the data travels with the single arena copy
-  b.bind(h->d_arena.p, v.off, v.n);
+// Leaves: connected components (through co-observation) of the free pose blocks that no IMU factor / prior touches -- the
+// remote frames of another drone in a multi-agent window (d2vinsstate.cpp:476-485: no speed-bias).  They couple only to
+// themselves and to the hub (own frames, extrinsics, td), so they are eliminated from the reduced system before the dense
+// Cholesky.
+void find_leaves(const HostWin &w, int nlc_cnt, std::vector<std::vector<int>> &leaves) {
+  const int np = (int)w.pose_id.size(), nl = (int)w.lm_id.size();
+  std::vector<char> hub(np, 0);
+  for (const HImu &m : w.imu) { hub[m.pi] = 1; hub[m.pj] = 1; }
+  for (const HPriorBlk &b : w.prior_blk) if (b.kind == D2BA_POSE) hub[b.index] = 1;
+  std::vector<int> uf(np);
+  for (int i = 0; i < np; i++) uf[i] = i;
+  auto find = [&](int x) { while (uf[x] != x) { uf[x] = uf[uf[x]]; x = uf[x]; } return x; };
+  // two poses belong to one component when some landmark is observed from both (the landmark's elimination couples them)
+  std::vector<int> first_pose(nl, -1);
+  for (const HObs &o : w.obs) {
+    const int ps[2] = {o.pi, o.pj};
+    for (int q = 0; q < 2; q++) {
+      const int pz = ps[q];
+      if (pz < 0 || hub[pz] || w.pose_c[pz]) continue;
+      if (first_pose[o.lm] < 0) { first_pose[o.lm] = pz; continue; }
+      const int a = find(pz), b = find(first_pose[o.lm]);
+      if (a != b) uf[std::max(a, b)] = std::min(a, b);
+    }
+  }
+  std::vector<int> comp_id(np, -1);
+  for (int i = 0; i < np; i++) {
+    if (hub[i] || w.pose_c[i]) continue;
+    const int r = find(i);
+    if (comp_id[r] < 0) { comp_id[r] = (int)leaves.size(); leaves.emplace_back(); }
+    leaves[comp_id[r]].push_back(i);
+  }
+  // a leaf must fit the elimination kernel's shared memory together with its hub coupling; otherwise it stays in the hub
+  int n_hub_cols = nlc_cnt;
+  for (auto &lf : leaves) n_hub_cols -= 6 * (int)lf.size();
+  std::vector<std::vector<int>> kept;
+  for (auto &lf : leaves) {
+    const int nl6 = 6 * (int)lf.size();
+    if (nl6 <= leaf_max_cols() && n_hub_cols >= 1 && leaf_elim_smem(nl6, n_hub_cols) <= kElimSmemCap) kept.push_back(lf);
+    else n_hub_cols += nl6;
+  }
+  // worthwhile only when the hub is a real reduction of the dense part
+  if (kept.empty() || n_hub_cols > 3 * nlc_cnt / 4) kept.clear();
+  leaves.swap(kept);
+}
+// Leaves, speed-bias eligibility, the reduced column order [leaf 0 | leaf 1 | ... | hub poses | ext | td | sb], the debug
+// views' canonical columns and the window's descriptor sizes.
+void plan_columns(HostWin &w, const PlanOpts &o, int wi, WinPlan &pl) {
+  WinDesc &d = pl.d; memset(&d, 0, sizeof d);
+  const int np = (int)w.pose_id.size(), ne = (int)w.ext_id.size(), nsb = (int)w.sb_id.size(), nl = (int)w.lm_id.size();
+  d.np = np; d.ne = ne; d.n6 = np + ne; d.nsb = nsb; d.nl = nl; d.has_td = w.has_td ? 1 : 0;
+  int nsb_free = 0, n6_free = 0;
+  for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) nsb_free++;
+  for (int i = 0; i < np; i++) if (!w.pose_c[i]) n6_free++;
+  for (int i = 0; i < ne; i++) if (!w.ext_c[i]) n6_free++;
+  const bool td_free = w.has_td && !w.td_c;
+  const int nlc_cnt = 6 * n6_free + (td_free ? 1 : 0);
+  {   // speed-bias elimination: needs a block-tridiagonal speed-bias part (IMU factors / prior blocks only between
+      // neighbouring speed-bias blocks); the test does not depend on the column order
+    std::vector<int> pos(nsb, -1);
+    int nb = 0;
+    for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) pos[i] = nb++;
+    pl.sb_ok = !o.force_full_S && !o.no_sb_elim && nb >= 1 && nlc_cnt >= 1;
+    for (size_t a = 0; a < w.imu.size() && pl.sb_ok; a++) {
+      const int pa = pos[w.imu[a].si], pb = pos[w.imu[a].sj];
+      if (pa >= 0 && pb >= 0 && std::abs(pa - pb) > 1) pl.sb_ok = false;
+    }
+    int pmin = 1 << 30, pmax = -1;
+    for (const HPriorBlk &b : w.prior_blk) if (b.kind == D2BA_SPEED_BIAS && pos[b.index] >= 0) { pmin = std::min(pmin, pos[b.index]); pmax = std::max(pmax, pos[b.index]); }
+    if (pmax - pmin > 1 || nb > sb_max_blocks()) pl.sb_ok = false;
+    d.n_sbe = nb;
+  }
+  std::vector<std::vector<int>> leaves;
+  if (!o.force_full_S && !o.no_leaf && (pl.sb_ok || nsb_free == 0) && nlc_cnt + 1 > kSmallCols) find_leaves(w, nlc_cnt, leaves);   // small systems keep the one-CTA dense path
+  pl.leaf_of.assign(np, -1);
+  for (size_t li = 0; li < leaves.size(); li++) for (int i : leaves[li]) pl.leaf_of[i] = (int)li;
+  int c = 0;
+  w.pose_col.assign(np, -1); w.ext_col.assign(ne, -1); w.sb_col.assign(nsb, -1);
+  for (size_t li = 0; li < leaves.size(); li++) {
+    Leaf lf; memset(&lf, 0, sizeof lf);
+    lf.win = wi; lf.col0 = c; lf.n = 6 * (int)leaves[li].size();
+    for (int i : leaves[li]) { w.pose_col[i] = c; c += 6; }
+    pl.leaves.push_back(lf);
+  }
+  d.hub0 = c;
+  for (int i = 0; i < np; i++) if (!w.pose_c[i] && pl.leaf_of[i] < 0) { w.pose_col[i] = c; c += 6; }
+  for (int i = 0; i < ne; i++) if (!w.ext_c[i]) { w.ext_col[i] = c; c += 6; }
+  w.td_col = td_free ? c : -1;
+  if (w.td_col >= 0) c += 1;
+  w.n_lc = c;
+  for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) { w.sb_col[i] = c; c += 9; }
+  w.n_c = c;
+  d.n_hub = w.n_lc - d.hub0; d.n_leaf = (int)leaves.size();
+  {   // canonical (insertion-order) columns for the debug views: canon_of_dev[device column] = column the oracle uses
+    w.canon_of_dev.assign(w.n_c, -1);
+    int cc = 0;
+    for (int i = 0; i < np; i++) if (!w.pose_c[i]) { for (int q = 0; q < 6; q++) w.canon_of_dev[w.pose_col[i] + q] = cc + q; cc += 6; }
+    for (int i = 0; i < ne; i++) if (!w.ext_c[i]) { for (int q = 0; q < 6; q++) w.canon_of_dev[w.ext_col[i] + q] = cc + q; cc += 6; }
+    if (w.td_col >= 0) w.canon_of_dev[w.td_col] = cc++;
+    for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) { for (int q = 0; q < 9; q++) w.canon_of_dev[w.sb_col[i] + q] = cc + q; cc += 9; }
+  }
+  d.td_col = w.td_col; d.n_lc = w.n_lc; d.n_c = w.n_c; d.ldh = std::max(4, roundup(w.n_c, 4));
+  d.ldw = roundup(w.n_lc + 1, 8); d.nl_pad = roundup(nl, 32);
+  d.admm_on = w.admm ? 1 : 0; d.n_imu = (int)w.imu.size();
+  d.prior_m = w.prior_m; d.prior_nblk = (int)w.prior_blk.size();
+}
+// Groups (runs of one key in pair-major order) with their kernel variant and balanced jobs, the landmarks' W-space column
+// tiles (lm_mask) and the groups' Hcc runs.
+void plan_groups(HostWin &w, const PlanOpts &o, int wi, WinPlan &pl) {
+  WinDesc &d = pl.d;
+  const int np = d.np;
+  const size_t M = w.obs.size();
+  // pair-major order: key = (type, pose_i, pose_j, ext_a, ext_b), ties by insertion order.  The number of distinct
+  // keys is small (<= a few hundred), so this is a counting sort: key -> bucket via a flat hash, buckets ordered by key.
+  std::vector<std::pair<uint64_t, uint32_t>> keys(M);   // (key, obs index) in sorted order
+  {
+    FlatMap bucket_of;                                     // key -> bucket id
+    std::vector<uint64_t> bkey; std::vector<uint32_t> bcount;
+    std::vector<uint32_t> ob(M);
+    uint64_t last_key = ~0ull; int last_b = -1;
+    for (size_t k = 0; k < M; k++) {
+      const HObs &x = w.obs[k];
+      const uint64_t key = ((uint64_t)(x.type & 0xF) << 60) | ((uint64_t)((x.pi + 1) & 0x7FFF) << 45) | ((uint64_t)((x.pj + 1) & 0x7FFF) << 30) |
+                           ((uint64_t)((x.ea + 1) & 0x7FFF) << 15) | (uint64_t)((x.eb + 1) & 0x7FFF);
+      int b;
+      if (key == last_key) b = last_b;
+      else {
+        b = bucket_of.find((int64_t)key);
+        if (b < 0) { b = (int)bkey.size(); bucket_of.put((int64_t)key, b); bkey.push_back(key); bcount.push_back(0); }
+        last_key = key; last_b = b;
+      }
+      ob[k] = (uint32_t)b; bcount[b]++;
+    }
+    std::vector<uint32_t> border(bkey.size());
+    for (size_t i = 0; i < border.size(); i++) border[i] = (uint32_t)i;
+    std::sort(border.begin(), border.end(), [&](uint32_t a, uint32_t b) { return bkey[a] < bkey[b]; });
+    std::vector<uint32_t> start(bkey.size());
+    uint32_t run = 0;
+    for (uint32_t bi : border) { start[bi] = run; run += bcount[bi]; }
+    for (size_t k = 0; k < M; k++) { const uint32_t b = ob[k]; keys[start[b]++] = {bkey[b], (uint32_t)k}; }   // stable within a bucket
+  }
+  w.order.resize(M); w.sorted_pos.assign(M, -1);
+  for (size_t k = 0; k < M; k++) w.order[k] = (int)keys[k].second;
+  // landmark masks: W-space column tiles (32 columns) a landmark's coupling row touches; the rhs column n_lc always
+  pl.lm_mask.assign(d.nl, 1ull << (w.n_lc / 32));
+  auto mark = [&](int lm, int col, int width) { if (col >= 0) pl.lm_mask[lm] |= (1ull << (col / 32)) | (1ull << ((col + width - 1) / 32)); };
+  size_t k = 0; int tile_run = 0;
+  while (k < M) {
+    size_t e = k;
+    while (e < M && keys[e].first == keys[k].first) e++;
+    const HObs &o0 = w.obs[w.order[k]];
+    Group g; memset(&g, 0, sizeof g);
+    g.type = o0.type;
+    g.blk[0] = o0.pi; g.blk[1] = o0.pj; g.blk[2] = o0.ea >= 0 ? np + o0.ea : -1; g.blk[3] = o0.eb >= 0 ? np + o0.eb : -1;
+    int cols[4] = {o0.pi >= 0 ? w.pose_col[o0.pi] : -1, o0.pj >= 0 ? w.pose_col[o0.pj] : -1, o0.ea >= 0 ? w.ext_col[o0.ea] : -1,
+                   o0.eb >= 0 ? w.ext_col[o0.eb] : -1};
+    if (o0.type == D2BA_PROJ_DEPTH_PRIOR) { cols[0] = cols[1] = cols[2] = cols[3] = -1; }
+    int ns = 0;
+    for (int s = 0; s < 4; s++) { g.slot_src[s] = -1; g.slot_col[s] = -1; }
+    for (int s = 0; s < 4; s++) if (cols[s] >= 0) { g.slot_src[ns] = s; g.slot_col[ns] = cols[s]; ns++; }
+    g.td_col = (o0.type == D2BA_PROJ_DEPTH_PRIOR) ? -1 : w.td_col;
+    g.need_td = g.td_col >= 0; g.need_ext = 0;
+    for (int s = 0; s < ns; s++) if (g.slot_src[s] >= 2) g.need_ext = 1;
+    g.nct = (ns <= 2 && !g.need_td) ? 2 : 4;
+    g.rows = o0.type == D2BA_PROJ_2F1C_DEPTH ? 3 : (o0.type == D2BA_PROJ_DEPTH_PRIOR ? 1 : 2);
+    if (g.nct == 4) pl.any_wide = true;
+    int variant = (g.nct == 4 ? 1 : 0) + (g.rows == 3 ? 2 : 0);
+    // all shifts zero? (td constant and equal to every observation's stamp)
+    g.shift0 = (!g.need_td && o0.type != D2BA_PROJ_DEPTH_PRIOR && w.td_min == w.td_max && w.td_min == w.td) ? 1 : 0;
+    if (variant == 0 && !g.need_ext && (o0.type == D2BA_PROJ_2F1C || o0.type == D2BA_PROJ_2F2C) && ns == 2 && g.slot_src[0] == 0 && g.slot_src[1] == 1)
+      variant = g.shift0 ? 4 : 5;
+    if (variant < 4) pl.all_pp = false;
+    const int cnt = (int)(e - k), ntile = (cnt + kTile - 1) / kTile;
+    const int gi = (int)pl.groups.size();
+    pl.groups.push_back(g); pl.grp_begin.push_back((int)k); pl.grp_cnt.push_back(cnt); pl.grp_tile0.push_back(tile_run);
+    // pattern of the group's J^T J blocks and of its landmarks' coupling rows
+    for (int a = 0; a < ns; a++) {
+      for (int b = 0; b <= a; b++) hblock(pl.hruns, g.slot_col[a], 6, g.slot_col[b], 6);
+      if (g.td_col >= 0) hblock(pl.hruns, g.td_col, 1, g.slot_col[a], 6);
+    }
+    if (g.td_col >= 0) hblock(pl.hruns, g.td_col, 1, g.td_col, 1);
+    for (size_t q = k; q < e; q++) {
+      const int lm = w.obs[w.order[q]].lm;
+      for (int a = 0; a < ns; a++) mark(lm, g.slot_col[a], 6);
+      mark(lm, g.td_col, 1);
+    }
+    // balanced split of the group's tiles into jobs
+    const int njob = (ntile + o.tpj_target - 1) / o.tpj_target;
+    for (int j = 0; j < njob; j++) {
+      int b = (int)((int64_t)ntile * j / njob), en = (int)((int64_t)ntile * (j + 1) / njob);
+      Job jb; jb.win = wi; jb.grp = gi; jb.tile_begin = tile_run + b; jb.ntiles = en - b;
+      pl.jobs[variant].push_back(jb);
+    }
+    tile_run += ntile;
+    k = e;
+  }
+  pl.n_tiles = tile_run; d.n_tile = tile_run; d.n_grp = (int)pl.groups.size();
+  pl.n_lmobs = (int)M;
+}
+// The landmark gather: barrier-free records, the leaves' landmarks, row tiles, the record width (96-byte records and
+// k_lm_gather12 chunks where they fit) and the final routing of the reprojection jobs (D2BA_DBG_LIN_JOBS).
+void plan_gather(HostWin &w, const PlanOpts &o, int wi, WinPlan &pl) {
+  WinDesc &d = pl.d;
+  const int nl = d.nl;
+  {   // may k_lm_gather16 skip the barrier between records?  Only if, per landmark, no column block shows up at slot 0 of one
+      // record and at slot 1 of another (then every row entry is owned by one lane).  True for the reference's graphs:
+      // slot 0 is the anchor pose of the landmark, the other slot an observing frame.
+    std::vector<int> s0(nl, -1);   // the landmark's slot-0 column
+    bool clash = false;
+    for (int gi = 0; gi < (int)pl.groups.size() && !clash; gi++) {
+      const int c0g = pl.groups[gi].slot_col[0];
+      if (c0g < 0) continue;
+      for (int q = pl.grp_begin[gi]; q < pl.grp_begin[gi] + pl.grp_cnt[gi]; q++) {
+        int &s = s0[w.obs[w.order[q]].lm];
+        if (s == -1) s = c0g; else if (s != c0g) { clash = true; break; }
+      }
+    }
+    for (int gi = 0; gi < (int)pl.groups.size() && !clash; gi++) {
+      const int c1g = pl.groups[gi].slot_col[1];
+      if (c1g < 0) continue;
+      for (int q = pl.grp_begin[gi]; q < pl.grp_begin[gi] + pl.grp_cnt[gi]; q++) if (s0[w.obs[w.order[q]].lm] == c1g) { clash = true; break; }
+    }
+    d.gather_nosync = clash ? 0 : 1;
+  }
+  {   // landmarks of every leaf (ascending, each once) and the widest coupling row in 32-column tiles
+    std::vector<std::vector<int>> per_leaf(pl.leaves.size());
+    if (!pl.leaves.empty()) {   // landmark-major obs order is not given: dedupe per (landmark, leaf) with a stamp matrix
+      std::vector<char> seen((size_t)nl * pl.leaves.size(), 0);
+      for (const HObs &ob : w.obs) {
+        const int ps[2] = {ob.pi, ob.pj};
+        for (int q = 0; q < 2; q++) if (ps[q] >= 0 && pl.leaf_of[ps[q]] >= 0) {
+          char &sn = seen[(size_t)ob.lm * pl.leaves.size() + pl.leaf_of[ps[q]]];
+          if (!sn) { sn = 1; per_leaf[pl.leaf_of[ps[q]]].push_back(ob.lm); }
+        }
+      }
+    }
+    for (size_t li = 0; li < pl.leaves.size(); li++) {
+      std::sort(per_leaf[li].begin(), per_leaf[li].end());
+      pl.leaves[li].lm_begin = (int)pl.leaf_lm.size(); pl.leaves[li].lm_count = (int)per_leaf[li].size();
+      pl.leaf_lm.insert(pl.leaf_lm.end(), per_leaf[li].begin(), per_leaf[li].end());
+    }
+    int rt = 1;
+    if (pl.leaves.empty()) rt = w.n_lc / 32 + 1;
+    else for (int l = 0; l < nl; l++) rt = std::max(rt, __builtin_popcountll(pl.lm_mask[l]));
+    d.row_tiles = rt;
+  }
+  d.rec_stride = pl.any_wide ? 32 : 16;
+  if (!pl.any_wide && pl.all_pp && !o.rec128 && d.n_leaf == 0 && d.gather_nosync) {
+    // 96-byte records + k_lm_gather12: every record comes from k_proj_lin_pp (two free poses: slot 1's position block is
+    // minus slot 0's), and per landmark the slot-0 column is unique (gather_nosync), the slot-1 columns are pairwise
+    // distinct and there are at most 32 records (one lane each)
+    std::vector<int> cnt(nl, 0);
+    std::vector<uint64_t> lc; lc.reserve(w.obs.size());
+    for (int gi = 0; gi < (int)pl.groups.size(); gi++)
+      for (int q = pl.grp_begin[gi]; q < pl.grp_begin[gi] + pl.grp_cnt[gi]; q++) {
+        const int lm = w.obs[w.order[q]].lm;
+        cnt[lm]++;
+        lc.push_back(((uint64_t)lm << 32) | (uint32_t)pl.groups[gi].slot_col[1]);
+      }
+    bool ok = true;
+    for (int l = 0; l < nl && ok; l++) ok = cnt[l] <= 32;
+    if (ok) { std::sort(lc.begin(), lc.end()); ok = std::adjacent_find(lc.begin(), lc.end()) == lc.end(); }
+    if (ok) {
+      d.rec_stride = 12;
+      pl.jobs[6].swap(pl.jobs[4]); pl.jobs[7].swap(pl.jobs[5]);   // k_proj_lin_pp<SHIFT0, 96-byte records>
+      // chunks of whole landmarks: at most 32 records and 31 landmarks (lane #landmarks holds the end pointer)
+      for (int l = 0; l < nl;) {
+        const int l0 = l;
+        int r = 0;
+        while (l < nl && l - l0 < 31 && r + cnt[l] <= 32) r += cnt[l++];
+        pl.g12.push_back(make_int4(wi, l0, l, 0));
+      }
+    }
+  }
+  w.n_g12 = (int)pl.g12.size();
+  for (int v = 0; v < 8; v++) {   // the final routing (after the 96-byte record swap): a group's jobs are consecutive
+    int64_t *c = w.lin_jobs[v];
+    for (int q = 0; q < 5; q++) c[q] = 0;
+    for (size_t j = 0; j < pl.jobs[v].size(); j++) {
+      const Job &jb = pl.jobs[v][j];
+      if (j == 0 || pl.jobs[v][j - 1].grp != jb.grp) { c[0]++; c[3] += pl.grp_cnt[jb.grp]; }
+      c[1]++; c[2] += jb.ntiles; c[4] = std::max<int64_t>(c[4], jb.ntiles);
+    }
+  }
+}
+// The solve path: one-CTA Schur of the whole system or of the hub, speed-bias elimination, shared-memory Cholesky, the
+// one-kernel solve (a candidate: apply_fused_threshold decides for the handle) and the rows of Wt.
+void plan_solve(const HostWin &w, const PlanOpts &o, WinPlan &pl) {
+  WinDesc &d = pl.d;
+  d.schur_small = (d.n_lc + 1 <= kSmallCols) ? 1 : 0;
+  d.hub_small = (d.n_leaf > 0 && d.n_hub + 1 <= kSmallCols) ? 1 : 0;
+  const int nb = d.n_sbe, hubw = roundup(d.n_hub + 1, 8);
+  bool ok = pl.sb_ok && w.n_c == w.n_lc + 9 * nb;
+  if (ok && (sb_elim_smem(hubw, d.n_c, nb) > kElimSmemCap || sb_back_smem(d.n_hub, nb) > kElimSmemCap)) ok = false;
+  pl.leaves_without_sb_elim = !ok && d.n_leaf > 0 && nb > 0;
+  d.sb_elim = ok ? 1 : 0;
+  // with speed-bias or leaf elimination the dense Cholesky only sees the hub of the pose part
+  if (ok || d.n_leaf > 0) d.chol_smem = (chol_smem_need(d.n_hub) <= kCholSmemCap) ? 1 : 0;
+  else d.chol_smem = (!o.force_full_S && w.n_c >= 1 && chol_smem_need(w.n_c) <= kCholSmemCap) ? 1 : 0;
+  // single-drone window whose whole reduced-system solve fits one CTA (k_solve_small)
+  d.fused_solve = (!o.no_fused_solve && d.n_leaf == 0 && d.sb_elim && d.schur_small && d.chol_smem && solve_small_fits(d.ldw)) ? 1 : 0;
+  // rows of Wt the Schur kernels sum over: landmark rows, then the eliminated speed-bias rows, then the leaves' rows
+  int rows = d.nl + (ok ? 9 * nb : 0);
+  for (Leaf &lf : pl.leaves) { lf.row0 = rows; rows += lf.n; }
+  d.wt_rows = roundup(std::max(rows, 1), 32);
+}
+// The remaining Hcc blocks (IMU factors, prior, ADMM terms), then all runs merged into the row segments hseg.
+void plan_hcc(const HostWin &w, WinPlan &pl) {
+  std::vector<uint64_t> &hruns = pl.hruns;
+  for (const HImu &m : w.imu) {
+    const int bc[4] = {w.pose_col[m.pi], w.sb_col[m.si], w.pose_col[m.pj], w.sb_col[m.sj]}, bs[4] = {6, 9, 6, 9};
+    for (int a = 0; a < 4; a++) for (int b = 0; b <= a; b++) hblock(hruns, bc[a], bs[a], bc[b], bs[b]);
+  }
+  {
+    std::vector<std::pair<int, int>> pb;
+    for (const HPriorBlk &b : w.prior_blk) {
+      int col = b.kind == D2BA_POSE ? w.pose_col[b.index] : b.kind == D2BA_EXTRINSIC ? w.ext_col[b.index] : b.kind == D2BA_SPEED_BIAS ? w.sb_col[b.index] : b.kind == D2BA_TD ? w.td_col : -1;
+      if (col >= 0) pb.push_back({col, b.eff});
+    }
+    for (size_t a = 0; a < pb.size(); a++) for (size_t b = 0; b <= a; b++) hblock(hruns, pb[a].first, pb[a].second, pb[b].first, pb[b].second);
+  }
+  if (w.admm) {
+    for (size_t i = 0; i < w.pose_col.size(); i++) if (w.pose_slot[i] >= 0) hblock(hruns, w.pose_col[i], 6, w.pose_col[i], 6);
+    for (size_t i = 0; i < w.ext_col.size(); i++) if (w.ext_slot[i] >= 0) hblock(hruns, w.ext_col[i], 6, w.ext_col[i], 6);
+    for (size_t i = 0; i < w.sb_col.size(); i++) hblock(hruns, w.sb_col[i], 9, w.sb_col[i], 9);
+    if (w.td_col >= 0) hblock(hruns, w.td_col, 1, w.td_col, 1);
+  }
+  std::sort(hruns.begin(), hruns.end());
+  for (size_t q = 0; q < hruns.size();) {
+    const int r = (int)(hruns[q] >> 40);
+    int a = (int)((hruns[q] >> 20) & 0xFFFFF), bnd = (int)(hruns[q] & 0xFFFFF);
+    size_t e2 = q + 1;
+    for (; e2 < hruns.size() && (int)(hruns[e2] >> 40) == r; e2++) {
+      const int c0 = (int)((hruns[e2] >> 20) & 0xFFFFF), c1 = (int)(hruns[e2] & 0xFFFFF);
+      if (c0 <= bnd) { bnd = std::max(bnd, c1); continue; }
+      pl.hseg.push_back(HSeg{r, a, std::min(bnd, r + 1) - a});   // lower triangle only
+      a = c0; bnd = c1;
+    }
+    pl.hseg.push_back(HSeg{r, a, std::min(bnd, r + 1) - a});
+    q = e2;
+  }
+  pl.d.n_hseg = (int)pl.hseg.size();
+}
+// Schur tiles with their 32-row chunk lists.  A chunk of Wt rows takes part in tile (tm, tn) iff some row of it has entries
+// in both column tiles.  Stage 0 = tiles with leaf columns (computed before the leaf elimination, landmark rows only),
+// stage 1 = tiles of the hub x hub part (after it: landmark rows + all eliminated rows).
+void plan_schur_tiles(HostWin &w, int wi, WinPlan &pl) {
+  const WinDesc &d = pl.d;
+  if (!d.schur_small) {
+    const int nl = d.nl, ntw = (d.n_lc + 1 + 31) / 32, nchunk = d.wt_rows / 32;
+    std::vector<unsigned long long> cmask(nchunk, 0ull);
+    for (int l = 0; l < nl; l++) cmask[l / 32] |= pl.lm_mask[l];
+    unsigned long long hubmask = 0ull;
+    for (int t = d.hub0 / 32; t <= d.n_lc / 32; t++) hubmask |= 1ull << t;
+    for (int r = nl; r < d.wt_rows; r++) cmask[r / 32] |= hubmask;   // eliminated rows (and the zero padding): hub columns + rhs
+    const int lm_chunks = (nl + 31) / 32;
+    // tile pattern of Hcc (a tile without chunks still copies Hcc into S)
+    std::vector<char> hpat((size_t)ntw * ntw, 0);
+    for (const HSeg &sg : pl.hseg) if (sg.row < d.n_lc) for (int cidx = sg.c0; cidx < sg.c0 + sg.len; cidx += 1) { hpat[(size_t)(sg.row / 32) * ntw + cidx / 32] = 1; }
+    for (int stage = 0; stage < 2; stage++)
+      for (int tm = 0; tm < ntw && d.n_lc > 0; tm++)
+        for (int tn = 0; tn <= tm; tn++) {
+          const bool in_hub = (tm * 32 + 31 >= d.hub0) && (tn * 32 + 31 >= d.hub0);
+          const bool has_leaf = tn * 32 < d.hub0;
+          if (stage == 0 ? !has_leaf : (!in_hub || d.hub_small)) continue;   // hub_small: k_schur_small forms the hub x hub part
+          SchurTileH t{wi, stage == 0 ? 2 : 0, tm, tn, (int)pl.schur_chunks.size(), 0};   // kind 2: only entries in leaf columns are stored
+          const int kend = stage == 0 ? lm_chunks : nchunk;
+          for (int kc = 0; kc < kend; kc++) if (((cmask[kc] >> tm) & 1ull) && ((cmask[kc] >> tn) & 1ull)) pl.schur_chunks.push_back(kc);
+          t.cn = (int)pl.schur_chunks.size() - t.cb;
+          if (t.cn == 0 && !hpat[(size_t)tm * ntw + tn] && tm != ntw - 1) continue;   // structurally zero tile: never read
+          pl.schur[stage].push_back(t);
+        }
+    int t_lo = d.n_lc / 32, t_hi = d.n_c / 32;
+    if (!d.sb_elim) for (int tm = t_lo; tm <= t_hi; tm++) for (int tn = 0; tn <= tm; tn++) pl.schur[1].push_back(SchurTileH{wi, 1, tm, tn, 0, 0});
+  }
+  w.n_schur_tiles[0] = (int)pl.schur[0].size(); w.n_schur_tiles[1] = (int)pl.schur[1].size();
+}
+// k_solve_small pays off through the wave count: it runs each window with 4 warps where the separate kernels have 8, and
+// wins only once those kernels need more than one wave (k_step: 3 CTAs per SM).  Smaller batches (the one-window latency
+// case) keep the separate kernels.
+void apply_fused_threshold(std::vector<WinPlan> &plan, int n_sm) {
+  int n_elig = 0;
+  for (const WinPlan &pl : plan) n_elig += pl.d.fused_solve;
+  if (n_elig < kFusedMinWindowsPerSM * n_sm) for (WinPlan &pl : plan) pl.d.fused_solve = 0;
+}
+// Serial pass: each window's offsets into the handle-wide arrays, and the launch summary.
+int plan_offsets(d2ba_handle *h, std::vector<WinPlan> &plan, const PlanOpts &o) {
+  LaunchSummary &L = h->ls;
+  L = LaunchSummary();
+  L.n_used = (int)plan.size(); L.tpj_target = o.tpj_target;
+  int n_sch[2] = {0, 0};
+  int64_t off_lmobs = 0;
+  for (int wi = 0; wi < L.n_used; wi++) {
+    const HostWin &w = h->win[wi]; WinPlan &pl = plan[wi]; WinDesc &d = pl.d;
+    d.off6 = L.n6_total; L.n6_total += d.n6; d.offsb = L.nsb_total; L.nsb_total += d.nsb; d.offlm = L.nl_total; L.nl_total += d.nl;
+    d.off_tile = L.n_tiles; L.n_tiles += d.n_tile; d.off_rec = L.tot_rec; L.tot_rec += (int64_t)std::max(pl.n_lmobs, 1) * d.rec_stride;
+    d.off_grp = L.n_grp; L.n_grp += d.n_grp; d.off_imu = L.n_imu_total; L.n_imu_total += d.n_imu;
+    d.off_lmptr = L.n_lmptr; L.n_lmptr += d.nl + 1; d.off_lmobs = off_lmobs; off_lmobs += pl.n_lmobs;
+    d.off_prior_blk = L.n_pblk; L.n_pblk += d.prior_nblk; d.off_prior_J = L.tot_pJ; d.off_prior_v = L.tot_pv;
+    L.tot_pJ += (int64_t)d.prior_m * d.prior_m; L.tot_pv += d.prior_m;
+    d.offH = L.totH; L.totH += (int64_t)(d.n_c + 1) * d.ldh;
+    d.offW = L.totW; L.totW += (int64_t)std::max(d.wt_rows, 32) * d.ldw;
+    d.offc = L.totc; L.totc += roundup(d.n_c + 1, 4);
+    for (int v = 0; v < 8; v++) { pl.job_off[v] = L.job_count[v]; L.job_count[v] += (int)pl.jobs[v].size(); }
+    for (int sg = 0; sg < 2; sg++) { pl.schur_off[sg] = n_sch[sg]; n_sch[sg] += (int)pl.schur[sg].size(); }
+    pl.chunk_off = L.n_chunks; L.n_chunks += (int)pl.schur_chunks.size();
+    pl.leaf_lm_off = L.n_leaf_lm; L.n_leaf_lm += (int)pl.leaf_lm.size();
+    L.max_row_tiles = std::max(L.max_row_tiles, d.row_tiles);
+    d.off_leaf = L.n_leaf_total; L.n_leaf_total += d.n_leaf; d.off_hseg = L.n_hseg; L.n_hseg += d.n_hseg;
+    for (Leaf &lf : pl.leaves) {
+      lf.offL = L.totLL; L.totLL += (int64_t)lf.n * lf.n + lf.n;
+      L.leaf_smem = std::max(L.leaf_smem, leaf_elim_smem(lf.n, d.n_hub)); L.leafb_smem = std::max(L.leafb_smem, leaf_back_smem(lf.n, d.n_hub));
+    }
+    L.max_nc = std::max(L.max_nc, d.n_c); L.max_prior_m = std::max(L.max_prior_m, d.prior_m);
+    if (d.schur_small) L.max_ldw_small = std::max(L.max_ldw_small, d.ldw);
+    if (d.hub_small) L.max_ldw_small = std::max(L.max_ldw_small, roundup(d.n_hub + 1, 8));
+    if (d.rec_stride == 16) L.any_compact = 1; else if (d.rec_stride == 32) L.any_wide = 1;
+    pl.g12_off = L.n_g12; L.n_g12 += (int)pl.g12.size();
+    if (d.sb_elim) {
+      d.offLE = L.totLE; L.totLE += (int64_t)d.n_sbe * 171;
+      L.sbe_smem = std::max(L.sbe_smem, sb_elim_smem(roundup(d.n_hub + 1, 8), d.n_c, d.n_sbe)); L.sbb_smem = std::max(L.sbb_smem, sb_back_smem(d.n_hub, d.n_sbe));
+    }
+    const int ndense = (d.sb_elim || d.n_leaf > 0) ? d.n_hub : d.n_c;
+    if (d.chol_smem) L.max_n_smem = std::max(L.max_n_smem, ndense); else { L.any_chol_glob = true; L.max_rows_glob = std::max(L.max_rows_glob, ndense + 1); }
+    if (d.fused_solve) { L.n_fused++; L.fused_smem = std::max(L.fused_smem, solve_small_smem(d.ldw, d.n_lc, d.n_c, d.n_sbe)); }
+    else {
+      if (d.schur_small || d.hub_small) L.ss_unfused = true;
+      if (d.chol_smem) L.cs_unfused = true;
+      if (d.sb_elim) L.sbb_unfused = true;
+    }
+    if (w.admm) {
+      if (L.any_admm && L.n_slots != w.n_slots) return fail(h, 26, "finalize: every window of a handle must name the same n_slots_global (the all-reduce count)");
+      L.any_admm = true; L.n_slots = w.n_slots;
+    }
+    if (w.prior_m > 0 && w.prior_is_info) L.any_info = true;
+  }
+  for (int v = 0; v < 8; v++) { L.job_begin[v] = L.n_jobs; L.n_jobs += L.job_count[v]; }
+  L.n_schur0 = n_sch[0]; L.n_schur = n_sch[0] + n_sch[1];
   return 0;
 }
-
-}  // namespace
-
-void d2ba_release_staging(d2ba_handle *h) {
-  std::lock_guard<std::mutex> lk(g_staging_mu);
-  auto it = g_staging.find(h);
-  if (it == g_staging.end()) return;
-  Staging *s = it->second;
-  s->arena.release();
-  delete s;
-  g_staging.erase(it);
+// Every staged array in arena order, as f(pinned slice, device view, element count).  This one list sets the arena layout,
+// the slices' places in the pinned arena and the device views' bindings to the device arena.
+template <typename F>
+void for_each_staged(Staging &st, d2ba_handle *h, F f) {
+  const LaunchSummary &L = h->ls;
+  const size_t nw = L.n_used, nobs = (size_t)L.n_tiles * kTile;
+  f(st.win, h->d_win, nw); f(st.x6, h->d_x6[0], (size_t)L.n6_total * 8); f(st.xsb, h->d_xsb[0], (size_t)L.nsb_total * 9);
+  f(st.xlm, h->d_xlm[0], L.nl_total); f(st.xtd, h->d_xtd[0], nw); f(st.col6, h->d_col6, L.n6_total); f(st.colsb, h->d_colsb, L.nsb_total);
+  f(st.slot6, h->d_slot6, L.n6_total); f(st.blk_win, h->d_blk_win, L.n6_total); f(st.sb_win, h->d_sb_win, L.nsb_total);
+  f(st.lm_win, h->d_lm_win, L.nl_total); f(st.tile_grp, h->d_tile_grp, L.n_tiles); f(st.tile_win, h->d_tile_win, L.n_tiles);
+  f(st.obs_lm, h->d_obs_lm, nobs); f(st.tile_src, h->d_tile_src, nobs); f(st.raw_off, h->d_raw_off, 4 * nw); f(st.lm_ptr, h->d_lm_ptr, L.n_lmptr);
+  f(st.obs_slot, h->d_obs_slot, nobs); f(st.grp, h->d_grp, L.n_grp); f(st.job, h->d_job, L.n_jobs); f(st.imu, h->d_imu, L.n_imu_total);
+  f(st.imu_c, h->d_imu_pk, (size_t)L.n_imu_total * kImuPack); f(st.pblk, h->d_prior_blk, L.n_pblk); f(st.prior_J, h->d_prior_J, (size_t)L.tot_pJ);
+  f(st.prior_e0, h->d_prior_e0, (size_t)L.tot_pv); f(st.schur, h->d_schur, L.n_schur); f(st.schur_chunks, h->d_schur_chunks, L.n_chunks);
+  f(st.leaf, h->d_leaf, L.n_leaf_total); f(st.hseg, h->d_hseg, L.n_hseg); f(st.lm_mask, h->d_lm_mask, L.nl_total);
+  f(st.leaf_lm, h->d_leaf_lm, L.n_leaf_lm); f(st.g12, h->d_g12, L.n_g12); f(st.pr_m, h->d_pr_m, nw); f(st.pr_info, h->d_pr_info, nw);
+  f(st.pr_offJ, h->d_pr_oJ, nw); f(st.pr_offv, h->d_pr_ov, nw);
 }
-
-extern "C" {
-
-int d2ba_finalize(d2ba_handle *h) {
-  if (!h) return 1;
-  cudaSetDevice(h->cfg.device);
-  release_graph(h);
-  int nw = 0;
+// Pass B: one window's part of every staged array.
+void stage_window(d2ba_handle *h, Staging &st, WinPlan &pl, int wi) {
+  HostWin &w = h->win[wi]; const WinDesc &d = pl.d;
+  st.win.p[wi] = d;
+  const int np = d.np, ne = d.ne;
+  for (int i = 0; i < np; i++) {
+    double *x = st.x6.p + (size_t)(d.off6 + i) * 8; memcpy(x, &w.pose[7 * i], 56); x[7] = 0;
+    st.col6.p[d.off6 + i] = w.pose_col[i]; st.slot6.p[d.off6 + i] = w.admm ? w.pose_slot[i] : -1; st.blk_win.p[d.off6 + i] = wi;
+  }
+  for (int i = 0; i < ne; i++) {
+    double *x = st.x6.p + (size_t)(d.off6 + np + i) * 8; memcpy(x, &w.ext[7 * i], 56); x[7] = 0;
+    st.col6.p[d.off6 + np + i] = w.ext_col[i]; st.slot6.p[d.off6 + np + i] = w.admm ? w.ext_slot[i] : -1; st.blk_win.p[d.off6 + np + i] = wi;
+  }
+  if (d.nsb) memcpy(st.xsb.p + (size_t)d.offsb * 9, w.sb.data(), (size_t)d.nsb * 72);
+  for (int i = 0; i < d.nsb; i++) { st.colsb.p[d.offsb + i] = w.sb_col[i]; st.sb_win.p[d.offsb + i] = wi; }
+  if (d.nl) memcpy(st.xlm.p + d.offlm, w.lm.data(), (size_t)d.nl * 8);
+  for (int i = 0; i < d.nl; i++) st.lm_win.p[d.offlm + i] = wi;
+  st.xtd.p[wi] = w.td;
+  // tile tables: source record of every tile slot (the device builds the AoSoA constants from the raw records)
+  // + landmark CSR by counting sort
+  int *lmp = st.lm_ptr.p + d.off_lmptr;
+  for (int l = 0; l <= d.nl; l++) lmp[l] = 0;
+  for (const HObs &o : w.obs) lmp[o.lm + 1]++;
+  for (int l = 0; l < d.nl; l++) lmp[l + 1] += lmp[l];
+  std::vector<int> cursor(lmp, lmp + d.nl);
+  int *oslot = st.obs_slot.p + (size_t)d.off_tile * kTile;   // tile slot -> record position (landmark-major), -1 = padding
+  for (int gi = 0; gi < (int)pl.groups.size(); gi++) {
+    st.grp.p[d.off_grp + gi] = pl.groups[gi];
+    const int cnt = pl.grp_cnt[gi], ntile = (cnt + kTile - 1) / kTile, k0 = pl.grp_begin[gi], t0 = pl.grp_tile0[gi];
+    for (int t = 0; t < ntile; t++) {
+      const int gt = d.off_tile + t0 + t;
+      st.tile_grp.p[gt] = d.off_grp + gi; st.tile_win.p[gt] = wi;
+      int *ol = st.obs_lm.p + (size_t)gt * kTile;
+      int *os = st.tile_src.p + (size_t)gt * kTile;
+      for (int lane = 0; lane < kTile; lane++) {
+        const int idx = t * kTile + lane;
+        if (idx < cnt) {
+          const int oi = w.order[k0 + idx];
+          ol[lane] = w.obs[oi].lm; os[lane] = oi;
+          w.sorted_pos[k0 + idx] = (t0 + t) * kTile + lane;
+        } else { ol[lane] = -1; os[lane] = -1; oslot[(size_t)(t0 + t) * kTile + lane] = -1; }
+      }
+    }
+  }
+  // a landmark's records in ascending tile-position order (deterministic reduction order): positions increase with sorted index
+  for (size_t k = 0; k < w.order.size(); k++) { const HObs &o = w.obs[w.order[k]]; oslot[w.sorted_pos[k]] = cursor[o.lm]++; }
+  for (int v = 0; v < 8; v++)
+    for (size_t j = 0; j < pl.jobs[v].size(); j++) {
+      Job jb = pl.jobs[v][j]; jb.grp += d.off_grp; jb.tile_begin += d.off_tile;
+      st.job.p[h->ls.job_begin[v] + pl.job_off[v] + j] = jb;
+    }
+  for (int sg = 0; sg < 2; sg++)
+    for (size_t t = 0; t < pl.schur[sg].size(); t++) { SchurTileH q = pl.schur[sg][t]; q.cb += pl.chunk_off; st.schur.p[(sg ? h->ls.n_schur0 : 0) + pl.schur_off[sg] + t] = q; }
+  for (size_t t = 0; t < pl.schur_chunks.size(); t++) st.schur_chunks.p[pl.chunk_off + t] = pl.schur_chunks[t];
+  for (size_t t = 0; t < pl.leaves.size(); t++) { Leaf lf = pl.leaves[t]; lf.lm_begin += pl.leaf_lm_off; st.leaf.p[d.off_leaf + t] = lf; }
+  for (size_t t = 0; t < pl.leaf_lm.size(); t++) st.leaf_lm.p[pl.leaf_lm_off + t] = pl.leaf_lm[t];
+  for (size_t t = 0; t < pl.hseg.size(); t++) st.hseg.p[d.off_hseg + t] = pl.hseg[t];
+  for (int l = 0; l < d.nl; l++) st.lm_mask.p[d.offlm + l] = pl.lm_mask[l];
+  for (size_t t = 0; t < pl.g12.size(); t++) st.g12.p[pl.g12_off + t] = pl.g12[t];
+  for (int i = 0; i < d.n_imu; i++) {
+    const HImu &m = w.imu[i];
+    st.imu.p[d.off_imu + i] = ImuDesc{m.pi, m.si, m.pj, m.sj, wi};
+    double *pk = st.imu_c.p + (size_t)(d.off_imu + i) * kImuPack;   // packed upload record (d2ba_types.cuh kImuPack)
+    memcpy(pk, m.c, 17 * 8);
+    for (int r = 0; r < 9; r++) memcpy(pk + 17 + r * 6, m.c + 17 + r * 15 + 9, 6 * 8);
+    for (int r = 0, q = 0; r < 15; r++) for (int c = 0; c <= r; c++) pk[71 + q++] = m.c[17 + 225 + r * 15 + c];
+  }
+  st.pr_m.p[wi] = d.prior_m; st.pr_info.p[wi] = (d.prior_m > 0 && w.prior_is_info) ? 1 : 0; st.pr_offJ.p[wi] = d.off_prior_J; st.pr_offv.p[wi] = d.off_prior_v;
+  if (d.prior_m > 0) {
+    memcpy(st.prior_J.p + d.off_prior_J, w.prior_J.data(), (size_t)d.prior_m * d.prior_m * 8);
+    memcpy(st.prior_e0.p + d.off_prior_v, w.prior_e0.data(), (size_t)d.prior_m * 8);
+    for (int i = 0; i < d.prior_nblk; i++) {
+      const HPriorBlk &b = w.prior_blk[i];
+      PriorBlk pb; memset(&pb, 0, sizeof pb);
+      pb.kind = b.kind; pb.off = b.off; pb.eff = b.eff; memcpy(pb.x0, b.x0, sizeof pb.x0);
+      pb.index = (b.kind == D2BA_EXTRINSIC) ? np + b.index : b.index;
+      st.pblk.p[d.off_prior_blk + i] = pb;
+    }
+  }
+}
+// The arena goes to the device in one copy on the solver stream and every staged array's device view is bound to it; then
+// the per-iteration buffers are allocated and the device builds the observation tiles from the raw records.
+int upload_and_bind(d2ba_handle *h, Staging &st) {
+  const LaunchSummary &L = h->ls;
+  const int nw = L.n_used;
+  CK(cudaEventRecord(h->evf0, h->stream));
+  // raw observation records were uploaded as they were added (copy stream); their device addresses ride in the arena
+  bool skipped = false;
+  for (int wi = 0; wi < nw; wi++) {
+    HostWin &w = h->win[wi];
+    if (w.rawj.n != w.obs.size()) return fail(h, 25, "internal: raw / index record count mismatch");
+    st.raw_off.p[4 * wi] = (long long)(uintptr_t)w.d_rawj.p; st.raw_off.p[4 * wi + 1] = (long long)(uintptr_t)w.d_anch.p;
+    const bool mot = motion_needed(w);   // else: k_build_tiles writes zero velocities and td_i = td_j = td
+    if (!mot && w.rawj.n) skipped = true;
+    st.raw_off.p[4 * wi + 2] = mot ? (long long)(uintptr_t)w.d_rawjm.p : 0; st.raw_off.p[4 * wi + 3] = mot ? (long long)(uintptr_t)w.d_anchm.p : 0;
+  }
+  if (st.cursor > h->d_arena.n) {   // growing: views of the old arena die with it
+    CK(cudaStreamSynchronize(h->stream));
+    CK(h->d_arena.alloc(st.cursor + st.cursor / 4 + 256));
+  }
+  CK(cudaMemcpyAsync(h->d_arena.p, st.arena.p, st.cursor, cudaMemcpyHostToDevice, h->stream));
+  h->h2d_bytes_fin = (long long)st.cursor;
+  for_each_staged(st, h, [&](auto &v, auto &b, size_t) { b.bind(h->d_arena.p, v.off, v.n); });
+  CK(h->d_ctl.alloc(nw)); CK(cudaMemsetAsync(h->d_ctl.p, 0, sizeof(Ctl) * nw, h->stream));
+  CK(h->d_x6[1].alloc(st.x6.n)); CK(h->d_xsb[1].alloc(st.xsb.n)); CK(h->d_xlm[1].alloc(st.xlm.n)); CK(h->d_xtd[1].alloc(st.xtd.n));
+  const size_t n6 = L.n6_total, nl = L.nl_total, offH = L.totH, offc = L.totc;
+  for (int b = 0; b < 2; b++) {
+    CK(h->d_R6[b].alloc(n6 * 12)); CK(h->d_rec[b].alloc((size_t)L.tot_rec));
+    CK(h->d_H[b].alloc(offH)); CK(h->d_gc[b].alloc(offc));
+    CK(cudaMemsetAsync(h->d_H[b].p, 0, std::max<size_t>(offH, 1) * 8, h->stream));   // entries no factor writes stay zero
+  }
+  CK(h->d_obs.alloc((size_t)L.n_tiles * kTile * kObsFields));
+  CK(cudaEventRecord(h->ev_copy, h->copy_stream));
+  CK(cudaStreamWaitEvent(h->stream, h->ev_copy, 0));
+  CK(cudaEventRecord(h->evf1, h->stream));
+  h->motion_skipped = skipped;
+  launch_build_tiles(h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, L.n_tiles, h->stream);
+  int rc;
+  CK(h->d_imu_U.alloc((size_t)L.n_imu_total * 225));
+  if ((rc = alloc_zero(h, h->d_imu_c, (size_t)L.n_imu_total * kImuStride))) return rc;   // expanded from the packed upload by k_imu_unpack (launch_imu_prep)
+  CK(h->d_prior_A.alloc((size_t)L.tot_pJ));
+  CK(h->d_z6.alloc(n6 * 8)); CK(h->d_tilde6.alloc(n6 * 6)); CK(h->d_lm_ref.alloc(nl)); CK(h->d_sb_ref.alloc((size_t)L.nsb_total * 9));
+  CK(h->d_td_ref.alloc(nw));
+  if ((rc = alloc_zero(h, h->d_cons, (size_t)std::max(L.n_slots, 1) * 14))) return rc;
+  if ((rc = alloc_zero(h, h->d_Wt, (size_t)L.totW))) return rc;   // padding rows / columns must be zero
+  CK(h->d_dinv.alloc(nl)); CK(h->d_hl.alloc(nl)); CK(h->d_gl.alloc(nl));
+  if ((rc = alloc_zero(h, h->d_S, offH))) return rc;   // tiles outside the structural pattern are never written
+  CK(h->d_leafL.alloc((size_t)std::max<int64_t>(L.totLL, 1)));
+  CK(h->d_gred.alloc(offc)); CK(h->d_D2c.alloc(offc)); CK(h->d_gn_c.alloc(offc)); CK(h->d_gn_l.alloc(nl));
+  CK(h->d_sbLE.alloc((size_t)std::max<int64_t>(L.totLE, 1)));
+  CK(h->d_step_c.alloc(offc)); CK(h->d_step_l.alloc(nl)); CK(h->d_wu.alloc(nl)); CK(h->d_uc.alloc(offc)); CK(h->d_D2l.alloc(nl));
+  return 0;
+}
+// The device view the kernels take by value, and the solver parameters.
+void set_device_view(d2ba_handle *h, const std::vector<WinPlan> &plan) {
+  const LaunchSummary &L = h->ls;
+  Dev &D = h->dev;
+  memset(&D, 0, sizeof D);
+  D.win = h->d_win.p; D.ctl = h->d_ctl.p; D.n_win = L.n_used;
+  for (int b = 0; b < 2; b++) { D.x6[b] = h->d_x6[b].p; D.R6[b] = h->d_R6[b].p; D.xsb[b] = h->d_xsb[b].p; D.xlm[b] = h->d_xlm[b].p; D.xtd[b] = h->d_xtd[b].p; D.rec[b] = h->d_rec[b].p; D.Hcc[b] = h->d_H[b].p; D.gc[b] = h->d_gc[b].p; }
+  D.col6 = h->d_col6.p; D.colsb = h->d_colsb.p; D.grp = h->d_grp.p; D.job = h->d_job.p; D.n_job = L.n_jobs;
+  D.lm_mask = h->d_lm_mask.p; D.hseg = h->d_hseg.p; D.leaf = h->d_leaf.p; D.n_leaf_total = L.n_leaf_total;
+  for (const WinPlan &pl : plan) if (pl.d.n_leaf == 0 && !pl.d.fused_solve) D.n_plain_win++;
+  D.leafL = h->d_leafL.p; D.schur_chunks = h->d_schur_chunks.p; D.leaf_lm = h->d_leaf_lm.p; D.g12_chunk = h->d_g12.p;
+  D.tile_grp = h->d_tile_grp.p; D.obs = h->d_obs.p; D.obs_lm = h->d_obs_lm.p; D.lm_ptr = h->d_lm_ptr.p; D.obs_slot = h->d_obs_slot.p;
+  D.imu = h->d_imu.p; D.imu_c = h->d_imu_c.p; D.imu_U = h->d_imu_U.p; D.prior_blk = h->d_prior_blk.p; D.prior_J = h->d_prior_J.p;
+  D.prior_e0 = h->d_prior_e0.p; D.prior_A = h->d_prior_A.p; D.slot6 = h->d_slot6.p; D.z6 = h->d_z6.p; D.tilde6 = h->d_tilde6.p;
+  D.lm_ref = h->d_lm_ref.p; D.sb_ref = h->d_sb_ref.p; D.td_ref = h->d_td_ref.p; D.cons_buf = h->d_cons.p; D.n_slots = L.n_slots;
+  D.Wt = h->d_Wt.p; D.dinv = h->d_dinv.p; D.hl = h->d_hl.p; D.gl = h->d_gl.p; D.S = h->d_S.p; D.gred = h->d_gred.p; D.D2c = h->d_D2c.p;
+  D.sbLE = h->d_sbLE.p;
+  D.gn_c = h->d_gn_c.p; D.gn_l = h->d_gn_l.p; D.step_c = h->d_step_c.p; D.step_l = h->d_step_l.p; D.wu = h->d_wu.p; D.uc = h->d_uc.p; D.D2l = h->d_D2l.p;
+  SolverParams &P = D.prm;
+  P.sqrt_info_px = h->cfg.focal_length / 1.5; P.depth_sqrt_inf = h->cfg.depth_sqrt_inf; P.gravity = h->cfg.gravity_norm; P.huber = h->cfg.huber_delta;
+  P.rho_T = h->cfg.rho_frame_T; P.rho_theta = h->cfg.rho_frame_theta; P.rho_landmark = h->cfg.rho_landmark; P.relaxation_alpha = h->cfg.relaxation_alpha;
+  P.initial_radius = h->cfg.initial_trust_region_radius; P.max_radius = h->cfg.max_trust_region_radius; P.min_rel_decrease = h->cfg.min_relative_decrease;
+  P.ftol = h->cfg.function_tolerance; P.gtol = h->cfg.gradient_tolerance; P.ptol = h->cfg.parameter_tolerance;
+  P.max_iter = h->cfg.max_num_iterations; P.fixed_mode = 0; P.mu0 = h->mu0;
+}
+// A cached kernel attribute: `configure(need)` runs only when `stale`; `cfg` remembers `need` across finalizes.
+template <typename V, typename F>
+int cached_attr(d2ba_handle *h, V &cfg, const V &need, bool stale, F configure, const char *msg) {
+  if (!stale) return 0;
+  if (configure(need)) return fail(h, 23, msg);
+  cfg = need;
+  return 0;
+}
+int configure_attributes(d2ba_handle *h) {
+  const LaunchSummary &L = h->ls;
+  const std::array<int, 3> kern = {L.max_rows_glob, L.max_nc, L.max_prior_m};
+  const int ldw = L.max_row_tiles * 32;
+  auto kernels = [](const std::array<int, 3> &k) { return configure_kernels(std::max(k[0], 2), k[1], k[2]); };
+  int rc;
+  if ((rc = cached_attr(h, h->cfg_kernels, kern, h->cfg_kernels != kern, kernels, "cudaFuncSetAttribute failed (shared memory request too large?)")) ||
+      (rc = cached_attr(h, h->cfg_max_ldw, ldw, h->cfg_max_ldw < ldw, configure_gather, "cudaFuncSetAttribute(k_lm_gather) failed (landmark-coupled part too wide for the row buffers)")) ||
+      (rc = cached_attr(h, h->cfg_max_ldw_small, L.max_ldw_small, L.max_ldw_small > 0 && h->cfg_max_ldw_small != L.max_ldw_small, configure_schur_small, "cudaFuncSetAttribute(k_schur_small) failed")) ||
+      (rc = cached_attr(h, h->cfg_sbe_smem, L.sbe_smem, L.sbe_smem > 0 && h->cfg_sbe_smem < L.sbe_smem, configure_sb_elim, "cudaFuncSetAttribute(k_sb_elim) failed")) ||
+      (rc = cached_attr(h, h->cfg_sbb_smem, L.sbb_smem, L.sbb_smem > 0 && h->cfg_sbb_smem < L.sbb_smem, configure_sb_back, "cudaFuncSetAttribute(k_sb_back) failed")) ||
+      (rc = cached_attr(h, h->cfg_leaf_smem, L.leaf_smem, L.leaf_smem > 0 && h->cfg_leaf_smem < L.leaf_smem, configure_leaf_elim, "cudaFuncSetAttribute(k_leaf_elim) failed")) ||
+      (rc = cached_attr(h, h->cfg_leafb_smem, L.leafb_smem, L.leafb_smem > 0 && h->cfg_leafb_smem < L.leafb_smem, configure_leaf_back, "cudaFuncSetAttribute(k_leaf_back) failed")) ||
+      (rc = cached_attr(h, h->cfg_max_n_smem, L.max_n_smem, L.max_n_smem > 0 && h->cfg_max_n_smem != L.max_n_smem, configure_chol_smem, "cudaFuncSetAttribute(k_chol_smem) failed")) ||
+      (rc = cached_attr(h, h->cfg_fused_smem, L.fused_smem, L.fused_smem > 0 && h->cfg_fused_smem < L.fused_smem, configure_solve_small, "cudaFuncSetAttribute(k_solve_small) failed")))
+    return rc;
+  return 0;
+}
+// State, IMU and prior preparation on the device, ahead of the first solve.
+int launch_prep(d2ba_handle *h) {
+  const LaunchSummary &L = h->ls;
+  launch_state_prep(h->dev, L.n6_total, 0, h->stream);
+  launch_imu_prep(h->dev, h->d_imu_pk.p, h->d_imu_c.p, L.n_imu_total, h->stream);
+  if (L.any_info)
+    launch_prior_from_info(L.n_used, L.max_prior_m, h->d_pr_m.p, h->d_pr_oJ.p, h->d_pr_ov.p, h->d_pr_info.p, h->d_prior_J.p, h->d_prior_A.p, h->d_prior_e0.p, h->stream);
+  launch_prior_prep(h->dev, h->stream);
+  CK(cudaEventRecord(h->evf2, h->stream));
+  return 0;
+}
+// Windows in use (contiguous from index 0), each narrow enough for the 64-bit landmark tile masks.
+int count_windows(d2ba_handle *h, int &nw) {
+  nw = 0;
   for (size_t i = 0; i < h->win.size(); i++) {
     if (h->win[i].used) { if ((int)i != nw) return fail(h, 20, "windows must be used contiguously from index 0"); nw++; }
   }
@@ -856,695 +1489,68 @@ int d2ba_finalize(d2ba_handle *h) {
       return fail(h, 27, "finalize: window " + std::to_string(wi) + " has " + std::to_string(nlc) +
                              " landmark-coupled columns; at most 2047 are supported (64-bit landmark tile masks)");
   }
-  Staging &st = *staging_of(h);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int d2ba_finalize(d2ba_handle *h) {
+  if (!h) return 1;
+  cudaSetDevice(h->cfg.device);
+  release_graph(h);
+  int nw, rc;
+  if ((rc = count_windows(h, nw))) return rc;
+  Staging &st = h->st;
   // the pinned staging buffers are rewritten below: wait for the uploads of the previous finalize of this handle
-  // (normally long complete -- a solve synchronises the stream); the uploads enqueued by THIS call are not waited for
+  // (normally long complete -- a solve synchronises the stream); the record uploads issued here run beside the planning
   CK(cudaStreamSynchronize(h->stream));
-  { std::lock_guard<std::mutex> lk(h->push_mu); int rcp = flush_pending(h, true); if (rcp) return rcp; }   // the rest of the record uploads run beside the planning below
+  { std::lock_guard<std::mutex> lk(h->push_mu); if ((rc = flush_pending(h, true))) return rc; }
   for (int wi = 0; wi < nw; wi++) {   // motion halves: only where td - td_i can be non-zero (td free, or a stamp that differs from td)
     HostWin &w = h->win[wi];
     if (!motion_needed(w)) continue;
-    int rcp;
-    if ((rcp = push_range(h, w.rawjm, w.d_rawjm, w.pushed_jm)) || (rcp = push_range(h, w.anchm, w.d_anchm, w.pushed_am))) return rcp;
+    if ((rc = push_range(h, w.rawjm, w.d_rawjm, w.pushed_jm)) || (rc = push_range(h, w.anchm, w.d_anchm, w.pushed_am))) return rc;
     w.pushed_jm = w.rawjm.n; w.pushed_am = w.anchm.n;
   }
   auto tp0 = std::chrono::steady_clock::now();
   auto lap = [&](int slot) { auto t = std::chrono::steady_clock::now(); h->host_ms[slot] = std::chrono::duration<double, std::milli>(t - tp0).count(); tp0 = t; };
-  std::vector<WinPlan> plan(nw);
+  // ---- pass A (parallel): each window's plan
+  int n_sm = 0;
+  if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->cfg.device) != cudaSuccess || n_sm < 1) n_sm = 132;   // H100 SXM
   size_t total_obs = 0;
   for (int i = 0; i < nw; i++) total_obs += h->win[i].obs.size();
   const int tiles_est = (int)(total_obs / kTile) + nw;
-  int n_sm = 132;   // H100 SXM; the device's own count when it can be read
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->cfg.device);
-  const int tpj_target = std::max(1, std::min(8, tiles_est / (n_sm * 8)));
-  h->tpj_target = tpj_target;
-  // ---- pass A (parallel): columns, pair-major order, groups, tiles, jobs, Schur tiles
+  const PlanOpts opts{h->force_full_S, h->no_leaf, h->no_sb_elim, h->rec128, h->no_fused_solve, std::max(1, std::min(8, tiles_est / (n_sm * 8)))};
+  std::vector<WinPlan> plan(nw);
   parallel_for(nw, [&](int wi) {
-    HostWin &w = h->win[wi];
-    WinPlan &pl = plan[wi];
-    WinDesc &d = pl.d; memset(&d, 0, sizeof d);
-    const int np = (int)w.pose_id.size(), ne = (int)w.ext_id.size(), nsb = (int)w.sb_id.size(), nl = (int)w.lm_id.size();
-    d.np = np; d.ne = ne; d.n6 = np + ne; d.nsb = nsb; d.nl = nl; d.has_td = w.has_td ? 1 : 0;
-    // ---- leaves: connected components (through co-observation) of the free pose blocks that no IMU factor / prior
-    //      touches -- the remote frames of another drone in a multi-agent window (d2vinsstate.cpp:476-485: no speed-bias).
-    //      They couple only to themselves and to the hub (own frames, extrinsics, td), so they are eliminated from the
-    //      reduced system before the dense Cholesky.  Reduced columns: [leaf 0 | leaf 1 | ... | hub poses | ext | td | sb].
-    std::vector<int> leaf_of(np, -1);
-    std::vector<std::vector<int>> leaves;
-    int nsb_free = 0, n6_free = 0;
-    for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) nsb_free++;
-    for (int i = 0; i < np; i++) if (!w.pose_c[i]) n6_free++;
-    for (int i = 0; i < ne; i++) if (!w.ext_c[i]) n6_free++;
-    const bool td_free = w.has_td && !w.td_c;
-    const int nlc_cnt = 6 * n6_free + (td_free ? 1 : 0), nc_cnt = nlc_cnt + 9 * nsb_free;
-    bool sb_ok;
-    {   // speed-bias elimination: needs a block-tridiagonal speed-bias part (IMU factors / prior blocks only between
-        // neighbouring speed-bias blocks); the test does not depend on the column order
-      std::vector<int> pos(nsb, -1);
-      int nb = 0;
-      for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) pos[i] = nb++;
-      sb_ok = !h->force_full_S && !h->no_sb_elim && nb >= 1 && nlc_cnt >= 1;
-      for (size_t a = 0; a < w.imu.size() && sb_ok; a++) {
-        const int pa = pos[w.imu[a].si], pb = pos[w.imu[a].sj];
-        if (pa >= 0 && pb >= 0 && std::abs(pa - pb) > 1) sb_ok = false;
-      }
-      int pmin = 1 << 30, pmax = -1;
-      for (const HPriorBlk &b : w.prior_blk) if (b.kind == D2BA_SPEED_BIAS && pos[b.index] >= 0) { pmin = std::min(pmin, pos[b.index]); pmax = std::max(pmax, pos[b.index]); }
-      if (pmax - pmin > 1) sb_ok = false;
-      if (sb_ok && nb > sb_max_blocks()) sb_ok = false;
-      d.n_sbe = nb;
-    }
-    if (!h->force_full_S && !h->no_leaf && (sb_ok || nsb_free == 0) && nlc_cnt + 1 > 96) {   // small systems keep the one-CTA dense path (k_schur_small)
-      std::vector<char> hub(np, 0);
-      for (const HImu &m : w.imu) { hub[m.pi] = 1; hub[m.pj] = 1; }
-      for (const HPriorBlk &b : w.prior_blk) if (b.kind == D2BA_POSE) hub[b.index] = 1;
-      std::vector<int> uf(np);
-      for (int i = 0; i < np; i++) uf[i] = i;
-      auto find = [&](int x) { while (uf[x] != x) { uf[x] = uf[uf[x]]; x = uf[x]; } return x; };
-      // two poses belong to one component when some landmark is observed from both (the landmark's elimination couples them)
-      std::vector<int> first_pose(nl, -1);
-      for (const HObs &o : w.obs) {
-        const int ps[2] = {o.pi, o.pj};
-        for (int q = 0; q < 2; q++) {
-          const int pz = ps[q];
-          if (pz < 0 || hub[pz] || w.pose_c[pz]) continue;
-          if (first_pose[o.lm] < 0) { first_pose[o.lm] = pz; continue; }
-          const int a = find(pz), b = find(first_pose[o.lm]);
-          if (a != b) uf[std::max(a, b)] = std::min(a, b);
-        }
-      }
-      std::vector<int> comp_id(np, -1);
-      for (int i = 0; i < np; i++) {
-        if (hub[i] || w.pose_c[i]) continue;
-        const int r = find(i);
-        if (comp_id[r] < 0) { comp_id[r] = (int)leaves.size(); leaves.emplace_back(); }
-        leaves[comp_id[r]].push_back(i);
-      }
-      // a leaf must fit the elimination kernel's shared memory together with its hub coupling; otherwise it stays in the hub
-      int n_hub_cols = nlc_cnt;
-      for (auto &lf : leaves) n_hub_cols -= 6 * (int)lf.size();
-      std::vector<std::vector<int>> kept;
-      for (auto &lf : leaves) {
-        const int nl6 = 6 * (int)lf.size();
-        if (nl6 <= leaf_max_cols() && n_hub_cols >= 1 && leaf_elim_smem(nl6, n_hub_cols) <= (size_t)200 * 1024) kept.push_back(lf);
-        else n_hub_cols += nl6;
-      }
-      // worthwhile only when the hub is a real reduction of the dense part
-      if (kept.empty() || n_hub_cols > 3 * nlc_cnt / 4) kept.clear();
-      leaves.swap(kept);
-      for (size_t li = 0; li < leaves.size(); li++) for (int i : leaves[li]) leaf_of[i] = (int)li;
-    }
-    int c = 0;
-    w.pose_col.assign(np, -1); w.ext_col.assign(ne, -1); w.sb_col.assign(nsb, -1);
-    pl.leaves.clear();
-    for (size_t li = 0; li < leaves.size(); li++) {
-      Leaf lf; memset(&lf, 0, sizeof lf);
-      lf.win = wi; lf.col0 = c; lf.n = 6 * (int)leaves[li].size();
-      for (int i : leaves[li]) { w.pose_col[i] = c; c += 6; }
-      pl.leaves.push_back(lf);
-    }
-    d.hub0 = c;
-    for (int i = 0; i < np; i++) if (!w.pose_c[i] && leaf_of[i] < 0) { w.pose_col[i] = c; c += 6; }
-    for (int i = 0; i < ne; i++) if (!w.ext_c[i]) { w.ext_col[i] = c; c += 6; }
-    w.td_col = td_free ? c : -1;
-    if (w.td_col >= 0) c += 1;
-    w.n_lc = c;
-    for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) { w.sb_col[i] = c; c += 9; }
-    w.n_c = c;
-    d.n_hub = w.n_lc - d.hub0; d.n_leaf = (int)leaves.size();
-    {   // canonical (insertion-order) columns for the debug views: canon_of_dev[device column] = column the oracle uses
-      w.canon_of_dev.assign(w.n_c, -1);
-      int cc = 0;
-      for (int i = 0; i < np; i++) if (!w.pose_c[i]) { for (int q = 0; q < 6; q++) w.canon_of_dev[w.pose_col[i] + q] = cc + q; cc += 6; }
-      for (int i = 0; i < ne; i++) if (!w.ext_c[i]) { for (int q = 0; q < 6; q++) w.canon_of_dev[w.ext_col[i] + q] = cc + q; cc += 6; }
-      if (w.td_col >= 0) w.canon_of_dev[w.td_col] = cc++;
-      for (int i = 0; i < nsb; i++) if (!w.sb_c[i]) { for (int q = 0; q < 9; q++) w.canon_of_dev[w.sb_col[i] + q] = cc + q; cc += 9; }
-    }
-    d.td_col = w.td_col; d.n_lc = w.n_lc; d.n_c = w.n_c; d.ldh = std::max(4, roundup(w.n_c, 4));
-    d.ldw = roundup(w.n_lc + 1, 8); d.nl_pad = roundup(nl, 32);
-    d.admm_on = w.admm ? 1 : 0; d.n_imu = (int)w.imu.size();
-    d.chol_smem = (!h->force_full_S && w.n_c >= 1 && chol_smem_need(w.n_c) <= (size_t)232448 - 16) ? 1 : 0;   // 16 B of static shared memory (fail flag + mbarrier)
-    d.prior_m = w.prior_m; d.prior_nblk = (int)w.prior_blk.size();
-    // pair-major order: key = (type, pose_i, pose_j, ext_a, ext_b), ties by insertion order.  The number of distinct
-    // keys is small (<= a few hundred), so this is a counting sort: key -> bucket via a flat hash, buckets ordered by key.
-    const size_t M = w.obs.size();
-    std::vector<std::pair<uint64_t, uint32_t>> keys(M);   // (key, bucket) then reused as (key, obs index) in sorted order
-    {
-      FlatMap bucket_of;                                     // key -> bucket id
-      std::vector<uint64_t> bkey; std::vector<uint32_t> bcount;
-      std::vector<uint32_t> ob(M);
-      uint64_t last_key = ~0ull; int last_b = -1;
-      for (size_t k = 0; k < M; k++) {
-        const HObs &o = w.obs[k];
-        const uint64_t key = ((uint64_t)(o.type & 0xF) << 60) | ((uint64_t)((o.pi + 1) & 0x7FFF) << 45) | ((uint64_t)((o.pj + 1) & 0x7FFF) << 30) |
-                             ((uint64_t)((o.ea + 1) & 0x7FFF) << 15) | (uint64_t)((o.eb + 1) & 0x7FFF);
-        int b;
-        if (key == last_key) b = last_b;
-        else {
-          b = bucket_of.find((int64_t)key);
-          if (b < 0) { b = (int)bkey.size(); bucket_of.put((int64_t)key, b); bkey.push_back(key); bcount.push_back(0); }
-          last_key = key; last_b = b;
-        }
-        ob[k] = (uint32_t)b; bcount[b]++;
-      }
-      std::vector<uint32_t> border(bkey.size());
-      for (size_t i = 0; i < border.size(); i++) border[i] = (uint32_t)i;
-      std::sort(border.begin(), border.end(), [&](uint32_t a, uint32_t b) { return bkey[a] < bkey[b]; });
-      std::vector<uint32_t> start(bkey.size());
-      uint32_t run = 0;
-      for (uint32_t bi : border) { start[bi] = run; run += bcount[bi]; }
-      for (size_t k = 0; k < M; k++) { const uint32_t b = ob[k]; keys[start[b]++] = {bkey[b], (uint32_t)k}; }   // stable within a bucket
-    }
-    w.order.resize(M); w.sorted_pos.assign(M, -1);
-    for (size_t k = 0; k < M; k++) w.order[k] = (int)keys[k].second;
-    // Hcc pattern (lower triangle, block rows): rows[r] collects the [c0, c1) runs some factor writes
-    // (one flat list of (row, c0, c1) runs, sorted and merged below: no per-row allocations on this per-solve path)
-    std::vector<uint64_t> &hruns = pl.hruns;
-    hruns.clear();
-    auto hblock = [&](int ra, int rs, int ca, int cs) {
-      if (ra < 0 || ca < 0) return;
-      if (ra < ca) { std::swap(ra, ca); std::swap(rs, cs); }
-      for (int r = 0; r < rs; r++) hruns.push_back(((uint64_t)(ra + r) << 40) | ((uint64_t)ca << 20) | (uint64_t)(ca + cs));
-    };
-    // landmark masks: W-space column tiles (32 columns) a landmark's coupling row touches; the rhs column n_lc always
-    pl.lm_mask.assign(nl, 1ull << (w.n_lc / 32));
-    auto mark = [&](int lm, int col, int width) { if (col >= 0) pl.lm_mask[lm] |= (1ull << (col / 32)) | (1ull << ((col + width - 1) / 32)); };
-    bool any_wide = false, all_pp = true;
-    size_t k = 0; int tile_run = 0;
-    while (k < M) {
-      size_t e = k;
-      while (e < M && keys[e].first == keys[k].first) e++;
-      const HObs &o0 = w.obs[w.order[k]];
-      Group g; memset(&g, 0, sizeof g);
-      g.type = o0.type;
-      g.blk[0] = o0.pi; g.blk[1] = o0.pj; g.blk[2] = o0.ea >= 0 ? np + o0.ea : -1; g.blk[3] = o0.eb >= 0 ? np + o0.eb : -1;
-      int cols[4] = {o0.pi >= 0 ? w.pose_col[o0.pi] : -1, o0.pj >= 0 ? w.pose_col[o0.pj] : -1, o0.ea >= 0 ? w.ext_col[o0.ea] : -1,
-                     o0.eb >= 0 ? w.ext_col[o0.eb] : -1};
-      if (o0.type == D2BA_PROJ_DEPTH_PRIOR) { cols[0] = cols[1] = cols[2] = cols[3] = -1; }
-      int ns = 0;
-      for (int s = 0; s < 4; s++) { g.slot_src[s] = -1; g.slot_col[s] = -1; }
-      for (int s = 0; s < 4; s++) if (cols[s] >= 0) { g.slot_src[ns] = s; g.slot_col[ns] = cols[s]; ns++; }
-      g.td_col = (o0.type == D2BA_PROJ_DEPTH_PRIOR) ? -1 : w.td_col;
-      g.need_td = g.td_col >= 0; g.need_ext = 0;
-      for (int s = 0; s < ns; s++) if (g.slot_src[s] >= 2) g.need_ext = 1;
-      g.nct = (ns <= 2 && !g.need_td) ? 2 : 4;
-      g.rows = o0.type == D2BA_PROJ_2F1C_DEPTH ? 3 : (o0.type == D2BA_PROJ_DEPTH_PRIOR ? 1 : 2);
-      if (g.nct == 4) any_wide = true;
-      int variant = (g.nct == 4 ? 1 : 0) + (g.rows == 3 ? 2 : 0);
-      // all shifts zero? (td constant and equal to every observation's stamp)
-      g.shift0 = (!g.need_td && o0.type != D2BA_PROJ_DEPTH_PRIOR && w.td_min == w.td_max && w.td_min == w.td) ? 1 : 0;
-      if (variant == 0 && !g.need_ext && (o0.type == D2BA_PROJ_2F1C || o0.type == D2BA_PROJ_2F2C) && ns == 2 && g.slot_src[0] == 0 && g.slot_src[1] == 1)
-        variant = g.shift0 ? 4 : 5;
-      if (variant < 4) all_pp = false;
-      const int cnt = (int)(e - k), ntile = (cnt + kTile - 1) / kTile;
-      const int gi = (int)pl.groups.size();
-      pl.groups.push_back(g); pl.grp_begin.push_back((int)k); pl.grp_cnt.push_back(cnt); pl.grp_tile0.push_back(tile_run);
-      // pattern of the group's J^T J blocks and of its landmarks' coupling rows
-      for (int a = 0; a < ns; a++) {
-        for (int b = 0; b <= a; b++) hblock(g.slot_col[a], 6, g.slot_col[b], 6);
-        if (g.td_col >= 0) hblock(g.td_col, 1, g.slot_col[a], 6);
-      }
-      if (g.td_col >= 0) hblock(g.td_col, 1, g.td_col, 1);
-      for (size_t q = k; q < e; q++) {
-        const int lm = w.obs[w.order[q]].lm;
-        for (int a = 0; a < ns; a++) mark(lm, g.slot_col[a], 6);
-        mark(lm, g.td_col, 1);
-      }
-      // balanced split of the group's tiles into jobs
-      const int njob = (ntile + tpj_target - 1) / tpj_target;
-      for (int j = 0; j < njob; j++) {
-        int b = (int)((int64_t)ntile * j / njob), en = (int)((int64_t)ntile * (j + 1) / njob);
-        Job jb; jb.win = wi; jb.grp = gi; jb.tile_begin = tile_run + b; jb.ntiles = en - b;
-        pl.jobs[variant].push_back(jb);
-      }
-      tile_run += ntile;
-      k = e;
-    }
-    pl.n_tiles = tile_run; d.n_tile = tile_run; d.n_grp = (int)pl.groups.size();
-    {   // may k_lm_gather16 skip the barrier between records?  Only if, per landmark, no column block shows up at slot 0 of one
-        // record and at slot 1 of another (then every row entry is owned by one lane).  True for the reference's graphs:
-        // slot 0 is the anchor pose of the landmark, the other slot an observing frame.
-      std::vector<int> s0(nl, -1);   // the landmark's slot-0 column (-2: more than one -> keep the barrier)
-      bool clash = false;
-      for (int gi = 0; gi < (int)pl.groups.size() && !clash; gi++) {
-        const int c0g = pl.groups[gi].slot_col[0];
-        if (c0g < 0) continue;
-        for (int q = pl.grp_begin[gi]; q < pl.grp_begin[gi] + pl.grp_cnt[gi]; q++) {
-          int &s = s0[w.obs[w.order[q]].lm];
-          if (s == -1) s = c0g; else if (s != c0g) { clash = true; break; }
-        }
-      }
-      for (int gi = 0; gi < (int)pl.groups.size() && !clash; gi++) {
-        const int c1g = pl.groups[gi].slot_col[1];
-        if (c1g < 0) continue;
-        for (int q = pl.grp_begin[gi]; q < pl.grp_begin[gi] + pl.grp_cnt[gi]; q++) if (s0[w.obs[w.order[q]].lm] == c1g) { clash = true; break; }
-      }
-      d.gather_nosync = clash ? 0 : 1;
-    }
-    {   // landmarks of every leaf (ascending, each once) and the widest coupling row in 32-column tiles
-      pl.leaf_lm.clear();
-      std::vector<std::vector<int>> per_leaf(pl.leaves.size());
-      if (!pl.leaves.empty()) {
-        std::vector<int> last_leaf_of_lm(nl, -1);   // landmark-major obs order is not given: dedupe per (landmark, leaf) with a stamp matrix
-        std::vector<char> seen((size_t)nl * pl.leaves.size(), 0);
-        for (const HObs &o : w.obs) {
-          const int ps[2] = {o.pi, o.pj};
-          for (int q = 0; q < 2; q++) if (ps[q] >= 0 && leaf_of[ps[q]] >= 0) {
-            char &sn = seen[(size_t)o.lm * pl.leaves.size() + leaf_of[ps[q]]];
-            if (!sn) { sn = 1; per_leaf[leaf_of[ps[q]]].push_back(o.lm); }
-          }
-        }
-        (void)last_leaf_of_lm;
-      }
-      for (size_t li = 0; li < pl.leaves.size(); li++) {
-        std::sort(per_leaf[li].begin(), per_leaf[li].end());
-        pl.leaves[li].lm_begin = (int)pl.leaf_lm.size(); pl.leaves[li].lm_count = (int)per_leaf[li].size();
-        pl.leaf_lm.insert(pl.leaf_lm.end(), per_leaf[li].begin(), per_leaf[li].end());
-      }
-      int rt = 1;
-      if (pl.leaves.empty()) rt = w.n_lc / 32 + 1;
-      else for (int l = 0; l < nl; l++) rt = std::max(rt, __builtin_popcountll(pl.lm_mask[l]));
-      d.row_tiles = rt;
-    }
-    d.rec_stride = any_wide ? 32 : 16;
-    pl.g12.clear();
-    if (!any_wide && all_pp && !h->rec128 && d.n_leaf == 0 && d.gather_nosync) {
-      // 96-byte records + k_lm_gather12: every record comes from k_proj_lin_pp (two free poses: slot 1's position block is
-      // minus slot 0's), and per landmark the slot-0 column is unique (gather_nosync), the slot-1 columns are pairwise
-      // distinct and there are at most 32 records (one lane each)
-      std::vector<int> cnt(nl, 0);
-      std::vector<uint64_t> lc; lc.reserve(M);
-      for (int gi = 0; gi < (int)pl.groups.size(); gi++)
-        for (int q = pl.grp_begin[gi]; q < pl.grp_begin[gi] + pl.grp_cnt[gi]; q++) {
-          const int lm = w.obs[w.order[q]].lm;
-          cnt[lm]++;
-          lc.push_back(((uint64_t)lm << 32) | (uint32_t)pl.groups[gi].slot_col[1]);
-        }
-      bool ok = true;
-      for (int l = 0; l < nl && ok; l++) ok = cnt[l] <= 32;
-      if (ok) { std::sort(lc.begin(), lc.end()); ok = std::adjacent_find(lc.begin(), lc.end()) == lc.end(); }
-      if (ok) {
-        d.rec_stride = 12;
-        pl.jobs[6].swap(pl.jobs[4]); pl.jobs[7].swap(pl.jobs[5]);   // k_proj_lin_pp<SHIFT0, 96-byte records>
-        // chunks of whole landmarks: at most 32 records and 31 landmarks (lane #landmarks holds the end pointer)
-        for (int l = 0; l < nl;) {
-          const int l0 = l;
-          int r = 0;
-          while (l < nl && l - l0 < 31 && r + cnt[l] <= 32) r += cnt[l++];
-          pl.g12.push_back(make_int4(wi, l0, l, 0));
-        }
-      }
-    }
-    pl.n_lmobs = (int)M;
-    for (int v = 0; v < 8; v++) {   // the final routing (after the 96-byte record swap): a group's jobs are consecutive
-      int64_t *c = w.lin_jobs[v];
-      for (int q = 0; q < 5; q++) c[q] = 0;
-      for (size_t j = 0; j < pl.jobs[v].size(); j++) {
-        const Job &jb = pl.jobs[v][j];
-        if (j == 0 || pl.jobs[v][j - 1].grp != jb.grp) { c[0]++; c[3] += pl.grp_cnt[jb.grp]; }
-        c[1]++; c[2] += jb.ntiles; c[4] = std::max<int64_t>(c[4], jb.ntiles);
-      }
-    }
-    d.schur_small = (d.n_lc + 1 <= 96) ? 1 : 0;
-    d.hub_small = (d.n_leaf > 0 && d.n_hub + 1 <= 96) ? 1 : 0;
-    {
-      const int nb = d.n_sbe;
-      const int hubw = roundup(d.n_hub + 1, 8);
-      bool ok = sb_ok && w.n_c == w.n_lc + 9 * nb;
-      if (ok && (sb_elim_smem(hubw, d.n_c, nb) > (size_t)200 * 1024 || sb_back_smem(d.n_hub, nb) > (size_t)200 * 1024)) ok = false;
-      if (!ok && d.n_leaf > 0 && nb > 0) { h->err = "internal: leaves without speed-bias elimination"; }
-      d.sb_elim = ok ? 1 : 0;
-      // the dense Cholesky only sees the hub of the pose part then: decide its kernel with that size
-      if (ok || d.n_leaf > 0) d.chol_smem = (chol_smem_need(d.n_hub) <= (size_t)232448 - 16) ? 1 : 0;
-      // single-drone window whose whole reduced-system solve fits one CTA (k_solve_small)
-      d.fused_solve = (!h->no_fused_solve && d.n_leaf == 0 && d.sb_elim && d.schur_small && d.chol_smem && solve_small_fits(d.ldw)) ? 1 : 0;
-      // rows of Wt the Schur kernels sum over: landmark rows, then the eliminated speed-bias rows, then the leaves' rows
-      int rows = nl + (ok ? 9 * nb : 0);
-      for (Leaf &lf : pl.leaves) { lf.row0 = rows; rows += lf.n; }
-      d.wt_rows = roundup(std::max(rows, 1), 32);
-    }
-    // other Hcc blocks: IMU factors, prior, ADMM terms
-    for (const HImu &m : w.imu) {
-      const int bc[4] = {w.pose_col[m.pi], w.sb_col[m.si], w.pose_col[m.pj], w.sb_col[m.sj]}, bs[4] = {6, 9, 6, 9};
-      for (int a = 0; a < 4; a++) for (int b = 0; b <= a; b++) hblock(bc[a], bs[a], bc[b], bs[b]);
-    }
-    {
-      std::vector<std::pair<int, int>> pb;
-      for (const HPriorBlk &b : w.prior_blk) {
-        int col = b.kind == D2BA_POSE ? w.pose_col[b.index] : b.kind == D2BA_EXTRINSIC ? w.ext_col[b.index] : b.kind == D2BA_SPEED_BIAS ? w.sb_col[b.index] : b.kind == D2BA_TD ? w.td_col : -1;
-        if (col >= 0) pb.push_back({col, b.eff});
-      }
-      for (size_t a = 0; a < pb.size(); a++) for (size_t b = 0; b <= a; b++) hblock(pb[a].first, pb[a].second, pb[b].first, pb[b].second);
-    }
-    if (w.admm) {
-      for (int i = 0; i < np; i++) if (w.pose_slot[i] >= 0) hblock(w.pose_col[i], 6, w.pose_col[i], 6);
-      for (int i = 0; i < ne; i++) if (w.ext_slot[i] >= 0) hblock(w.ext_col[i], 6, w.ext_col[i], 6);
-      for (int i = 0; i < nsb; i++) hblock(w.sb_col[i], 9, w.sb_col[i], 9);
-      if (w.td_col >= 0) hblock(w.td_col, 1, w.td_col, 1);
-    }
-    pl.hseg.clear();
-    std::sort(hruns.begin(), hruns.end());
-    for (size_t q = 0; q < hruns.size();) {
-      const int r = (int)(hruns[q] >> 40);
-      int a = (int)((hruns[q] >> 20) & 0xFFFFF), bnd = (int)(hruns[q] & 0xFFFFF);
-      size_t e2 = q + 1;
-      for (; e2 < hruns.size() && (int)(hruns[e2] >> 40) == r; e2++) {
-        const int c0 = (int)((hruns[e2] >> 20) & 0xFFFFF), c1 = (int)(hruns[e2] & 0xFFFFF);
-        if (c0 <= bnd) { bnd = std::max(bnd, c1); continue; }
-        pl.hseg.push_back(HSeg{r, a, std::min(bnd, r + 1) - a});   // lower triangle only
-        a = c0; bnd = c1;
-      }
-      pl.hseg.push_back(HSeg{r, a, std::min(bnd, r + 1) - a});
-      q = e2;
-    }
-    d.n_hseg = (int)pl.hseg.size();
-    if (!d.schur_small) {
-      // ---- Schur tiles with their 32-row chunk lists.  A chunk of Wt rows takes part in tile (tm, tn) iff some row of it
-      //      has entries in both column tiles.  Stage 0 = tiles with leaf columns (computed before the leaf elimination,
-      //      landmark rows only), stage 1 = tiles of the hub x hub part (after it: landmark rows + all eliminated rows).
-      const int ntw = (d.n_lc + 1 + 31) / 32, nchunk = d.wt_rows / 32;
-      std::vector<unsigned long long> cmask(nchunk, 0ull);
-      for (int l = 0; l < nl; l++) cmask[l / 32] |= pl.lm_mask[l];
-      unsigned long long hubmask = 0ull;
-      for (int t = d.hub0 / 32; t <= d.n_lc / 32; t++) hubmask |= 1ull << t;
-      const int first_elim_row = nl;
-      for (int r = nl; r < d.wt_rows; r++) cmask[r / 32] |= hubmask;   // eliminated rows (and the zero padding): hub columns + rhs
-      const int lm_chunks = (nl + 31) / 32;
-      (void)first_elim_row;
-      // tile pattern of Hcc (a tile without chunks still copies Hcc into S)
-      std::vector<char> hpat((size_t)ntw * ntw, 0);
-      for (const HSeg &sg : pl.hseg) if (sg.row < d.n_lc) for (int cidx = sg.c0; cidx < sg.c0 + sg.len; cidx += 1) { hpat[(size_t)(sg.row / 32) * ntw + cidx / 32] = 1; }
-      for (int stage = 0; stage < 2; stage++)
-        for (int tm = 0; tm < ntw && d.n_lc > 0; tm++)
-          for (int tn = 0; tn <= tm; tn++) {
-            const bool in_hub = (tm * 32 + 31 >= d.hub0) && (tn * 32 + 31 >= d.hub0);
-            const bool has_leaf = tn * 32 < d.hub0;
-            if (stage == 0 ? !has_leaf : (!in_hub || d.hub_small)) continue;   // hub_small: k_schur_small forms the hub x hub part
-            SchurTileH t{wi, stage == 0 ? 2 : 0, tm, tn, (int)pl.schur_chunks.size(), 0};   // kind 2: only entries in leaf columns are stored
-            const int kend = stage == 0 ? lm_chunks : nchunk;
-            for (int kc = 0; kc < kend; kc++) if (((cmask[kc] >> tm) & 1ull) && ((cmask[kc] >> tn) & 1ull)) pl.schur_chunks.push_back(kc);
-            t.cn = (int)pl.schur_chunks.size() - t.cb;
-            if (t.cn == 0 && !hpat[(size_t)tm * ntw + tn] && tm != ntw - 1) continue;   // structurally zero tile: never read
-            pl.schur[stage].push_back(t);
-          }
-      int t_lo = d.n_lc / 32, t_hi = d.n_c / 32;
-      if (!d.sb_elim) for (int tm = t_lo; tm <= t_hi; tm++) for (int tn = 0; tn <= tm; tn++) pl.schur[1].push_back(SchurTileH{wi, 1, tm, tn, 0, 0});
-    }
-    w.n_g12 = (int)pl.g12.size(); w.n_schur_tiles[0] = (int)pl.schur[0].size(); w.n_schur_tiles[1] = (int)pl.schur[1].size();
+    HostWin &w = h->win[wi]; WinPlan &pl = plan[wi];
+    plan_columns(w, opts, wi, pl);
+    plan_groups(w, opts, wi, pl);
+    plan_gather(w, opts, wi, pl);
+    plan_solve(w, opts, pl);
+    plan_hcc(w, pl);
+    plan_schur_tiles(w, wi, pl);
   });
-  {   // k_solve_small pays off through the wave count: it runs each window with 4 warps where the separate kernels have 8,
-      // and wins only once those kernels need more than one wave (k_step: 3 CTAs per SM).  Smaller batches (the
-      // one-window latency case) keep the separate kernels.
-    int n_sm = 0;
-    if (cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, h->cfg.device) != cudaSuccess || n_sm < 1) n_sm = 1;
-    int n_elig = 0;
-    for (int wi = 0; wi < nw; wi++) n_elig += plan[wi].d.fused_solve;
-    if (n_elig < kFusedMinWindowsPerSM * n_sm) for (int wi = 0; wi < nw; wi++) plan[wi].d.fused_solve = 0;
-  }
+  apply_fused_threshold(plan, n_sm);
+  for (const WinPlan &pl : plan)
+    if (pl.leaves_without_sb_elim) { std::lock_guard<std::mutex> lk(h->err_mu); h->err = "internal: leaves without speed-bias elimination"; }
   lap(0);
-  // ---- serial prefix sums
-  h->n_used = nw; h->max_rows = 1; h->max_nc = 1; h->max_prior_m = 0; h->max_ldw = 8; h->n_slots = 0; h->any_admm = false;
-  h->max_row_tiles = 1; h->max_n_smem = 0; h->max_rows_glob = 1; h->any_chol_glob = false; h->max_ldw_small = 0; h->any_compact = h->any_wide = 0; h->sbe_smem = 0; h->sbb_smem = 0;
-  h->n_fused = 0; h->fused_smem = 0; h->ss_unfused = h->cs_unfused = h->sbb_unfused = false;
-  int64_t offLE = 0;
-  int off6 = 0, offsb = 0, offlm = 0, off_tile = 0, off_grp = 0, off_imu = 0, off_lmptr = 0, off_pblk = 0, n_schur = 0, n_sch[2] = {0, 0}, n_chunks = 0, off_leaf = 0, off_hseg = 0, n_leaf_lm = 0;
-  int64_t offLL = 0; size_t leaf_smem = 0, leafb_smem = 0; int max_hub = 0, n_g12 = 0;
-  int64_t offH = 0, offW = 0, offc = 0, off_lmobs = 0, off_pJ = 0, off_pv = 0, off_rec = 0; long long off_raw = 0;
-  int njobs[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  bool any_info = false;
-  for (int wi = 0; wi < nw; wi++) {
-    HostWin &w = h->win[wi]; WinPlan &pl = plan[wi]; WinDesc &d = pl.d;
-    d.off6 = off6; off6 += d.n6; d.offsb = offsb; offsb += d.nsb; d.offlm = offlm; offlm += d.nl;
-    d.off_tile = off_tile; off_tile += d.n_tile; d.off_rec = off_rec; off_rec += (int64_t)std::max(pl.n_lmobs, 1) * d.rec_stride;
-    d.off_grp = off_grp; off_grp += d.n_grp; d.off_imu = off_imu; off_imu += d.n_imu;
-    d.off_lmptr = off_lmptr; off_lmptr += d.nl + 1; d.off_lmobs = off_lmobs; off_lmobs += pl.n_lmobs;
-    d.off_prior_blk = off_pblk; off_pblk += d.prior_nblk; d.off_prior_J = off_pJ; d.off_prior_v = off_pv;
-    off_pJ += (int64_t)d.prior_m * d.prior_m; off_pv += d.prior_m;
-    d.offH = offH; offH += (int64_t)(d.n_c + 1) * d.ldh;
-    d.offW = offW; offW += (int64_t)std::max(d.wt_rows, 32) * d.ldw;
-    d.offc = offc; offc += roundup(d.n_c + 1, 4);
-    for (int v = 0; v < 8; v++) { pl.job_off[v] = njobs[v]; njobs[v] += (int)pl.jobs[v].size(); }
-    for (int sg = 0; sg < 2; sg++) { pl.schur_off[sg] = n_sch[sg]; n_sch[sg] += (int)pl.schur[sg].size(); }
-    pl.chunk_off = n_chunks; n_chunks += (int)pl.schur_chunks.size();
-    pl.leaf_lm_off = n_leaf_lm; n_leaf_lm += (int)pl.leaf_lm.size();
-    h->max_row_tiles = std::max(h->max_row_tiles, d.row_tiles);
-    d.off_leaf = off_leaf; off_leaf += d.n_leaf; d.off_hseg = off_hseg; off_hseg += d.n_hseg;
-    for (Leaf &lf : pl.leaves) { lf.offL = offLL; offLL += (int64_t)lf.n * lf.n + lf.n; leaf_smem = std::max(leaf_smem, leaf_elim_smem(lf.n, d.n_hub)); leafb_smem = std::max(leafb_smem, leaf_back_smem(lf.n, d.n_hub)); }
-    max_hub = std::max(max_hub, d.n_hub);
-    h->max_rows = std::max(h->max_rows, d.n_c + 1); h->max_nc = std::max(h->max_nc, d.n_c); h->max_ldw = std::max(h->max_ldw, d.ldw);
-    h->max_prior_m = std::max(h->max_prior_m, d.prior_m);
-    if (d.schur_small) h->max_ldw_small = std::max(h->max_ldw_small, d.ldw);
-    if (d.hub_small) h->max_ldw_small = std::max(h->max_ldw_small, roundup(d.n_hub + 1, 8));
-    if (d.rec_stride == 16) h->any_compact = 1; else if (d.rec_stride == 32) h->any_wide = 1;
-    pl.g12_off = n_g12; n_g12 += (int)pl.g12.size();
-    if (d.sb_elim) {
-      d.offLE = offLE; offLE += (int64_t)d.n_sbe * 171;
-      h->sbe_smem = std::max(h->sbe_smem, sb_elim_smem(roundup(d.n_hub + 1, 8), d.n_c, d.n_sbe)); h->sbb_smem = std::max(h->sbb_smem, sb_back_smem(d.n_hub, d.n_sbe));
-    }
-    { const int ndense = (d.sb_elim || d.n_leaf > 0) ? d.n_hub : d.n_c;
-      if (d.chol_smem) h->max_n_smem = std::max(h->max_n_smem, ndense); else { h->any_chol_glob = true; h->max_rows_glob = std::max(h->max_rows_glob, ndense + 1); } }
-    if (d.fused_solve) { h->n_fused++; h->fused_smem = std::max(h->fused_smem, solve_small_smem(d.ldw, d.n_lc, d.n_c, d.n_sbe)); }
-    else {
-      if (d.schur_small || d.hub_small) h->ss_unfused = true;
-      if (d.chol_smem) h->cs_unfused = true;
-      if (d.sb_elim) h->sbb_unfused = true;
-    }
-    if (w.admm) {
-      if (h->any_admm && h->n_slots != w.n_slots) return fail(h, 26, "finalize: every window of a handle must name the same n_slots_global (the all-reduce count)");
-      h->any_admm = true; h->n_slots = w.n_slots;
-    }
-    if (w.prior_m > 0 && w.prior_is_info) any_info = true;
-  }
-  int jbase[8]; { int r = 0; for (int v = 0; v < 8; v++) { jbase[v] = r; h->job_begin[v] = r; h->job_count[v] = njobs[v]; r += njobs[v]; } }
-  const int n_jobs = jbase[7] + njobs[7];
-  h->n6_total = off6; h->nsb_total = offsb; h->nl_total = offlm; h->n_tiles = off_tile; h->n_imu_total = off_imu; n_schur = n_sch[0] + n_sch[1]; h->n_schur = n_schur; h->n_schur0 = n_sch[0];
-  h->n_leaf_total = off_leaf; h->leaf_smem = leaf_smem; h->leafb_smem = leafb_smem; h->max_hub = max_hub;
-  h->totH = offH; h->totW = offW; h->totc = offc; h->totLE = offLE;
-  // ---- staging sizes
+  // ---- serial prefix sums, staging sizes
+  if ((rc = plan_offsets(h, plan, opts))) return rc;
   st.cursor = 0;
-  st.reserve(st.win, nw); st.reserve(st.x6, (size_t)off6 * 8); st.reserve(st.xsb, (size_t)offsb * 9); st.reserve(st.xlm, offlm); st.reserve(st.xtd, nw);
-  st.reserve(st.col6, off6); st.reserve(st.colsb, offsb); st.reserve(st.slot6, off6); st.reserve(st.blk_win, off6); st.reserve(st.sb_win, offsb);
-  st.reserve(st.lm_win, offlm); st.reserve(st.tile_grp, off_tile); st.reserve(st.tile_win, off_tile); st.reserve(st.obs_lm, (size_t)off_tile * kTile);
-  st.reserve(st.tile_src, (size_t)off_tile * kTile); st.reserve(st.raw_off, 4 * (size_t)nw); st.reserve(st.lm_ptr, off_lmptr); st.reserve(st.obs_slot, (size_t)off_tile * kTile);
-  st.reserve(st.grp, off_grp); st.reserve(st.job, n_jobs); st.reserve(st.imu, off_imu); st.reserve(st.imu_c, (size_t)off_imu * kImuPack);
-  st.reserve(st.pblk, off_pblk); st.reserve(st.prior_J, (size_t)off_pJ); st.reserve(st.prior_e0, (size_t)off_pv); st.reserve(st.schur, n_schur); st.reserve(st.schur_chunks, n_chunks); st.reserve(st.leaf, off_leaf); st.reserve(st.hseg, off_hseg); st.reserve(st.lm_mask, offlm); st.reserve(st.leaf_lm, n_leaf_lm); st.reserve(st.g12, n_g12);
-  st.reserve(st.pr_m, nw); st.reserve(st.pr_info, nw); st.reserve(st.pr_offJ, nw); st.reserve(st.pr_offv, nw);
-  bool ok = st.arena.resize(st.cursor + 256);
-  if (ok) {
-    st.place(st.win); st.place(st.x6); st.place(st.xsb); st.place(st.xlm); st.place(st.xtd); st.place(st.col6); st.place(st.colsb); st.place(st.slot6);
-    st.place(st.blk_win); st.place(st.sb_win); st.place(st.lm_win); st.place(st.tile_grp); st.place(st.tile_win); st.place(st.obs_lm); st.place(st.tile_src);
-    st.place(st.raw_off); st.place(st.lm_ptr); st.place(st.obs_slot); st.place(st.grp); st.place(st.job); st.place(st.imu); st.place(st.imu_c); st.place(st.pblk);
-    st.place(st.prior_J); st.place(st.prior_e0); st.place(st.schur); st.place(st.schur_chunks); st.place(st.leaf); st.place(st.hseg); st.place(st.lm_mask); st.place(st.leaf_lm); st.place(st.g12); st.place(st.pr_m); st.place(st.pr_info); st.place(st.pr_offJ); st.place(st.pr_offv);
-  }
-  if (!ok) return fail(h, 24, "pinned staging allocation failed");
+  for_each_staged(st, h, [&](auto &v, auto &, size_t n) { st.reserve(v, n); });
+  if (!st.arena.resize(st.cursor + 256)) return fail(h, 24, "pinned staging allocation failed");
+  for_each_staged(st, h, [&](auto &v, auto &, size_t) { st.place(v); });
   lap(1);
   // ---- pass B (parallel): fill the staging buffers
-  std::atomic<int> skipped_any{0};
-  parallel_for(nw, [&](int wi) {
-    HostWin &w = h->win[wi]; WinPlan &pl = plan[wi]; const WinDesc &d = pl.d;
-    st.win.p[wi] = d;
-    const int np = d.np, ne = d.ne;
-    for (int i = 0; i < np; i++) {
-      double *x = st.x6.p + (size_t)(d.off6 + i) * 8; memcpy(x, &w.pose[7 * i], 56); x[7] = 0;
-      st.col6.p[d.off6 + i] = w.pose_col[i]; st.slot6.p[d.off6 + i] = w.admm ? w.pose_slot[i] : -1; st.blk_win.p[d.off6 + i] = wi;
-    }
-    for (int i = 0; i < ne; i++) {
-      double *x = st.x6.p + (size_t)(d.off6 + np + i) * 8; memcpy(x, &w.ext[7 * i], 56); x[7] = 0;
-      st.col6.p[d.off6 + np + i] = w.ext_col[i]; st.slot6.p[d.off6 + np + i] = w.admm ? w.ext_slot[i] : -1; st.blk_win.p[d.off6 + np + i] = wi;
-    }
-    if (d.nsb) memcpy(st.xsb.p + (size_t)d.offsb * 9, w.sb.data(), (size_t)d.nsb * 72);
-    for (int i = 0; i < d.nsb; i++) { st.colsb.p[d.offsb + i] = w.sb_col[i]; st.sb_win.p[d.offsb + i] = wi; }
-    if (d.nl) memcpy(st.xlm.p + d.offlm, w.lm.data(), (size_t)d.nl * 8);
-    for (int i = 0; i < d.nl; i++) st.lm_win.p[d.offlm + i] = wi;
-    st.xtd.p[wi] = w.td;
-    // tile tables: source record of every tile slot (the device builds the AoSoA constants from the raw records)
-    // + landmark CSR by counting sort
-    int *lmp = st.lm_ptr.p + d.off_lmptr;
-    for (int l = 0; l <= d.nl; l++) lmp[l] = 0;
-    for (const HObs &o : w.obs) lmp[o.lm + 1]++;
-    for (int l = 0; l < d.nl; l++) lmp[l + 1] += lmp[l];
-    std::vector<int> cursor(lmp, lmp + d.nl);
-    int *oslot = st.obs_slot.p + (size_t)d.off_tile * kTile;   // tile slot -> record position (landmark-major), -1 = padding
-    for (int gi = 0; gi < (int)pl.groups.size(); gi++) {
-      st.grp.p[d.off_grp + gi] = pl.groups[gi];
-      const int cnt = pl.grp_cnt[gi], ntile = (cnt + kTile - 1) / kTile, k0 = pl.grp_begin[gi], t0 = pl.grp_tile0[gi];
-      for (int t = 0; t < ntile; t++) {
-        const int gt = d.off_tile + t0 + t;
-        st.tile_grp.p[gt] = d.off_grp + gi; st.tile_win.p[gt] = wi;
-        int *ol = st.obs_lm.p + (size_t)gt * kTile;
-        int *os = st.tile_src.p + (size_t)gt * kTile;
-        for (int lane = 0; lane < kTile; lane++) {
-          const int idx = t * kTile + lane;
-          if (idx < cnt) {
-            const int oi = w.order[k0 + idx];
-            ol[lane] = w.obs[oi].lm; os[lane] = oi;
-            w.sorted_pos[k0 + idx] = (t0 + t) * kTile + lane;
-          } else { ol[lane] = -1; os[lane] = -1; oslot[(size_t)(t0 + t) * kTile + lane] = -1; }
-        }
-      }
-    }
-    // a landmark's records in ascending tile-position order (deterministic reduction order): positions increase with sorted index
-    for (size_t k = 0; k < w.order.size(); k++) { const HObs &o = w.obs[w.order[k]]; oslot[w.sorted_pos[k]] = cursor[o.lm]++; }
-    for (int v = 0; v < 8; v++)
-      for (size_t j = 0; j < pl.jobs[v].size(); j++) {
-        Job jb = pl.jobs[v][j]; jb.grp += d.off_grp; jb.tile_begin += d.off_tile;
-        st.job.p[jbase[v] + pl.job_off[v] + j] = jb;
-      }
-    for (int sg = 0; sg < 2; sg++)
-      for (size_t t = 0; t < pl.schur[sg].size(); t++) { SchurTileH q = pl.schur[sg][t]; q.cb += pl.chunk_off; st.schur.p[(sg ? n_sch[0] : 0) + pl.schur_off[sg] + t] = q; }
-    for (size_t t = 0; t < pl.schur_chunks.size(); t++) st.schur_chunks.p[pl.chunk_off + t] = pl.schur_chunks[t];
-    for (size_t t = 0; t < pl.leaves.size(); t++) { Leaf lf = pl.leaves[t]; lf.lm_begin += pl.leaf_lm_off; st.leaf.p[d.off_leaf + t] = lf; }
-    for (size_t t = 0; t < pl.leaf_lm.size(); t++) st.leaf_lm.p[pl.leaf_lm_off + t] = pl.leaf_lm[t];
-    for (size_t t = 0; t < pl.hseg.size(); t++) st.hseg.p[d.off_hseg + t] = pl.hseg[t];
-    for (int l = 0; l < d.nl; l++) st.lm_mask.p[d.offlm + l] = pl.lm_mask[l];
-    for (size_t t = 0; t < pl.g12.size(); t++) st.g12.p[pl.g12_off + t] = pl.g12[t];
-    for (int i = 0; i < d.n_imu; i++) {
-      const HImu &m = w.imu[i];
-      st.imu.p[d.off_imu + i] = ImuDesc{m.pi, m.si, m.pj, m.sj, wi};
-      double *pk = st.imu_c.p + (size_t)(d.off_imu + i) * kImuPack;   // packed upload record (d2ba_types.cuh kImuPack)
-      memcpy(pk, m.c, 17 * 8);
-      for (int r = 0; r < 9; r++) memcpy(pk + 17 + r * 6, m.c + 17 + r * 15 + 9, 6 * 8);
-      for (int r = 0, q = 0; r < 15; r++) for (int c = 0; c <= r; c++) pk[71 + q++] = m.c[17 + 225 + r * 15 + c];
-    }
-    st.pr_m.p[wi] = d.prior_m; st.pr_info.p[wi] = (d.prior_m > 0 && w.prior_is_info) ? 1 : 0; st.pr_offJ.p[wi] = d.off_prior_J; st.pr_offv.p[wi] = d.off_prior_v;
-    if (d.prior_m > 0) {
-      memcpy(st.prior_J.p + d.off_prior_J, w.prior_J.data(), (size_t)d.prior_m * d.prior_m * 8);
-      memcpy(st.prior_e0.p + d.off_prior_v, w.prior_e0.data(), (size_t)d.prior_m * 8);
-      for (int i = 0; i < d.prior_nblk; i++) {
-        const HPriorBlk &b = w.prior_blk[i];
-        PriorBlk pb; memset(&pb, 0, sizeof pb);
-        pb.kind = b.kind; pb.off = b.off; pb.eff = b.eff; memcpy(pb.x0, b.x0, sizeof pb.x0);
-        pb.index = (b.kind == D2BA_EXTRINSIC) ? np + b.index : b.index;
-        st.pblk.p[d.off_prior_blk + i] = pb;
-      }
-    }
-  });
+  parallel_for(nw, [&](int wi) { stage_window(h, st, plan[wi], wi); });
   lap(2);
   h->h_win.assign(st.win.p, st.win.p + nw);
-  h->h_grp.assign(st.grp.p, st.grp.p + off_grp);
-  // ---- uploads (pinned -> device, async on the solver stream)
-  int rc;
-  CK(cudaEventRecord(h->evf0, h->stream));
-  // raw observation records were uploaded as they were added (copy stream); their device addresses ride in the arena
-  for (int wi = 0; wi < nw; wi++) {
-    HostWin &w = h->win[wi];
-    if (w.rawj.n != w.obs.size()) return fail(h, 25, "internal: raw / index record count mismatch");
-    st.raw_off.p[4 * wi] = (long long)(uintptr_t)w.d_rawj.p; st.raw_off.p[4 * wi + 1] = (long long)(uintptr_t)w.d_anch.p;
-    const bool mot = motion_needed(w);   // else: k_build_tiles writes zero velocities and td_i = td_j = td
-    if (!mot && w.rawj.n) skipped_any = 1;
-    st.raw_off.p[4 * wi + 2] = mot ? (long long)(uintptr_t)w.d_rawjm.p : 0; st.raw_off.p[4 * wi + 3] = mot ? (long long)(uintptr_t)w.d_anchm.p : 0;
-  }
-  if (st.cursor > h->d_arena.n) {   // growing: views of the old arena die with it
-    CK(cudaStreamSynchronize(h->stream));
-    CK(h->d_arena.alloc(st.cursor + st.cursor / 4 + 256));
-  }
-  CK(cudaMemcpyAsync(h->d_arena.p, st.arena.p, st.cursor, cudaMemcpyHostToDevice, h->stream));
-  h->h2d_bytes_fin = (long long)st.cursor;
-  if ((rc = up(h, h->d_win, st.win))) return rc;
-  CK(h->d_ctl.alloc(nw)); CK(cudaMemsetAsync(h->d_ctl.p, 0, sizeof(Ctl) * nw, h->stream));
-  if ((rc = up(h, h->d_x6[0], st.x6)) || (rc = up(h, h->d_xsb[0], st.xsb)) || (rc = up(h, h->d_xlm[0], st.xlm)) || (rc = up(h, h->d_xtd[0], st.xtd))) return rc;
-  CK(h->d_x6[1].alloc(st.x6.n)); CK(h->d_xsb[1].alloc(st.xsb.n)); CK(h->d_xlm[1].alloc(st.xlm.n)); CK(h->d_xtd[1].alloc(st.xtd.n));
-  const size_t rec_doubles = (size_t)off_rec;
-  for (int b = 0; b < 2; b++) {
-    CK(h->d_R6[b].alloc((size_t)off6 * 12)); CK(h->d_rec[b].alloc(rec_doubles));
-    CK(h->d_H[b].alloc((size_t)offH)); CK(h->d_gc[b].alloc((size_t)offc));
-    CK(cudaMemsetAsync(h->d_H[b].p, 0, std::max<size_t>((size_t)offH, 1) * 8, h->stream));   // entries no factor writes stay zero
-  }
-  if ((rc = up(h, h->d_col6, st.col6)) || (rc = up(h, h->d_colsb, st.colsb)) || (rc = up(h, h->d_tile_grp, st.tile_grp)) ||
-      (rc = up(h, h->d_tile_win, st.tile_win)) || (rc = up(h, h->d_obs_lm, st.obs_lm)) || (rc = up(h, h->d_tile_src, st.tile_src)) ||
-      (rc = up(h, h->d_lm_ptr, st.lm_ptr)) || (rc = up(h, h->d_obs_slot, st.obs_slot)) || (rc = up(h, h->d_slot6, st.slot6)) ||
-      (rc = up(h, h->d_lm_win, st.lm_win)) || (rc = up(h, h->d_blk_win, st.blk_win)) || (rc = up(h, h->d_sb_win, st.sb_win)) ||
-      (rc = up(h, h->d_grp, st.grp)) || (rc = up(h, h->d_job, st.job)) || (rc = up(h, h->d_imu, st.imu)) || (rc = up(h, h->d_imu_pk, st.imu_c)) ||
-      (rc = up(h, h->d_prior_blk, st.pblk)) || (rc = up(h, h->d_prior_J, st.prior_J)) || (rc = up(h, h->d_prior_e0, st.prior_e0)) ||
-      (rc = up(h, h->d_schur, st.schur)) || (rc = up(h, h->d_schur_chunks, st.schur_chunks)) || (rc = up(h, h->d_leaf, st.leaf)) || (rc = up(h, h->d_leaf_lm, st.leaf_lm)) ||
-      (rc = up(h, h->d_hseg, st.hseg)) || (rc = up(h, h->d_lm_mask, st.lm_mask)) || (rc = up(h, h->d_g12, st.g12)))
-    return rc;
-  // the device builds the tiles from the raw records
-  CK(h->d_obs.alloc((size_t)off_tile * kTile * kObsFields));
-  if ((rc = up(h, h->d_raw_off, st.raw_off))) return rc;
-  CK(cudaEventRecord(h->ev_copy, h->copy_stream));
-  CK(cudaStreamWaitEvent(h->stream, h->ev_copy, 0));
-  CK(cudaEventRecord(h->evf1, h->stream));
-  h->motion_skipped = skipped_any.load() != 0;
-  launch_build_tiles(h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, off_tile, h->stream);
-  CK(h->d_imu_U.alloc((size_t)off_imu * 225));
-  if ((rc = alloc_zero(h, h->d_imu_c, (size_t)off_imu * kImuStride))) return rc;   // expanded from the packed upload by k_imu_unpack (launch_imu_prep)
-  CK(h->d_prior_A.alloc((size_t)off_pJ));
-  CK(h->d_z6.alloc((size_t)off6 * 8)); CK(h->d_tilde6.alloc((size_t)off6 * 6)); CK(h->d_lm_ref.alloc(offlm)); CK(h->d_sb_ref.alloc((size_t)offsb * 9));
-  CK(h->d_td_ref.alloc(nw));
-  if ((rc = alloc_zero(h, h->d_cons, (size_t)std::max(h->n_slots, 1) * 14))) return rc;
-  if ((rc = alloc_zero(h, h->d_Wt, (size_t)offW))) return rc;   // padding rows / columns must be zero
-  CK(h->d_dinv.alloc(offlm)); CK(h->d_hl.alloc(offlm)); CK(h->d_gl.alloc(offlm));
-  if ((rc = alloc_zero(h, h->d_S, (size_t)offH))) return rc;   // tiles outside the structural pattern are never written
-  CK(h->d_leafL.alloc((size_t)std::max<int64_t>(offLL, 1)));
-  CK(h->d_gred.alloc((size_t)offc)); CK(h->d_D2c.alloc((size_t)offc)); CK(h->d_gn_c.alloc((size_t)offc)); CK(h->d_gn_l.alloc(offlm));
-  CK(h->d_sbLE.alloc((size_t)std::max<int64_t>(offLE, 1)));
-  CK(h->d_step_c.alloc((size_t)offc)); CK(h->d_step_l.alloc(offlm)); CK(h->d_wu.alloc(offlm)); CK(h->d_uc.alloc((size_t)offc)); CK(h->d_D2l.alloc(offlm));
-  // ---- device view
-  Dev &D = h->dev;
-  memset(&D, 0, sizeof D);
-  D.win = h->d_win.p; D.ctl = h->d_ctl.p; D.n_win = nw;
-  for (int b = 0; b < 2; b++) { D.x6[b] = h->d_x6[b].p; D.R6[b] = h->d_R6[b].p; D.xsb[b] = h->d_xsb[b].p; D.xlm[b] = h->d_xlm[b].p; D.xtd[b] = h->d_xtd[b].p; D.rec[b] = h->d_rec[b].p; D.Hcc[b] = h->d_H[b].p; D.gc[b] = h->d_gc[b].p; }
-  D.col6 = h->d_col6.p; D.colsb = h->d_colsb.p; D.grp = h->d_grp.p; D.job = h->d_job.p; D.n_job = n_jobs;
-  D.lm_mask = h->d_lm_mask.p; D.hseg = h->d_hseg.p; D.leaf = h->d_leaf.p; D.n_leaf_total = h->n_leaf_total; { int np_ = 0; for (int q = 0; q < nw; q++) if (plan[q].d.n_leaf == 0 && !plan[q].d.fused_solve) np_++; D.n_plain_win = np_; } D.leafL = h->d_leafL.p; D.schur_chunks = h->d_schur_chunks.p; D.leaf_lm = h->d_leaf_lm.p;
-  D.g12_chunk = h->d_g12.p; h->n_g12 = n_g12;
-  D.tile_grp = h->d_tile_grp.p; D.obs = h->d_obs.p; D.obs_lm = h->d_obs_lm.p; D.lm_ptr = h->d_lm_ptr.p; D.obs_slot = h->d_obs_slot.p;
-  D.imu = h->d_imu.p; D.imu_c = h->d_imu_c.p; D.imu_U = h->d_imu_U.p; D.prior_blk = h->d_prior_blk.p; D.prior_J = h->d_prior_J.p;
-  D.prior_e0 = h->d_prior_e0.p; D.prior_A = h->d_prior_A.p; D.slot6 = h->d_slot6.p; D.z6 = h->d_z6.p; D.tilde6 = h->d_tilde6.p;
-  D.lm_ref = h->d_lm_ref.p; D.sb_ref = h->d_sb_ref.p; D.td_ref = h->d_td_ref.p; D.cons_buf = h->d_cons.p; D.n_slots = h->n_slots;
-  D.Wt = h->d_Wt.p; D.dinv = h->d_dinv.p; D.hl = h->d_hl.p; D.gl = h->d_gl.p; D.S = h->d_S.p; D.gred = h->d_gred.p; D.D2c = h->d_D2c.p;
-  D.sbLE = h->d_sbLE.p;
-  D.gn_c = h->d_gn_c.p; D.gn_l = h->d_gn_l.p; D.step_c = h->d_step_c.p; D.step_l = h->d_step_l.p; D.wu = h->d_wu.p; D.uc = h->d_uc.p; D.D2l = h->d_D2l.p;
-  SolverParams &P = D.prm;
-  P.sqrt_info_px = h->cfg.focal_length / 1.5; P.depth_sqrt_inf = h->cfg.depth_sqrt_inf; P.gravity = h->cfg.gravity_norm; P.huber = h->cfg.huber_delta;
-  P.rho_T = h->cfg.rho_frame_T; P.rho_theta = h->cfg.rho_frame_theta; P.rho_landmark = h->cfg.rho_landmark; P.relaxation_alpha = h->cfg.relaxation_alpha;
-  P.initial_radius = h->cfg.initial_trust_region_radius; P.max_radius = h->cfg.max_trust_region_radius; P.min_rel_decrease = h->cfg.min_relative_decrease;
-  P.ftol = h->cfg.function_tolerance; P.gtol = h->cfg.gradient_tolerance; P.ptol = h->cfg.parameter_tolerance;
-  P.max_iter = h->cfg.max_num_iterations; P.fixed_mode = 0; P.mu0 = h->mu0;
-  if (h->cfg_max_rows != h->max_rows_glob || h->cfg_max_nc != h->max_nc || h->cfg_max_prior != h->max_prior_m) {
-    if (configure_kernels(std::max(h->max_rows_glob, 2), h->max_nc, h->max_prior_m)) return fail(h, 23, "cudaFuncSetAttribute failed (shared memory request too large?)");
-    h->cfg_max_rows = h->max_rows_glob; h->cfg_max_nc = h->max_nc; h->cfg_max_prior = h->max_prior_m;
-  }
-  if (h->cfg_max_ldw < h->max_row_tiles * 32) {
-    if (configure_gather(h->max_row_tiles * 32)) return fail(h, 23, "cudaFuncSetAttribute(k_lm_gather) failed (landmark-coupled part too wide for the row buffers)");
-    h->cfg_max_ldw = h->max_row_tiles * 32;
-  }
-  if (h->max_ldw_small > 0 && h->cfg_max_ldw_small != h->max_ldw_small) {
-    if (configure_schur_small(h->max_ldw_small)) return fail(h, 23, "cudaFuncSetAttribute(k_schur_small) failed");
-    h->cfg_max_ldw_small = h->max_ldw_small;
-  }
-  if (h->sbe_smem > 0 && h->cfg_sbe_smem < h->sbe_smem) {
-    if (configure_sb_elim(h->sbe_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_sb_elim) failed");
-    h->cfg_sbe_smem = h->sbe_smem;
-  }
-  if (h->sbb_smem > 0 && h->cfg_sbb_smem < h->sbb_smem) {
-    if (configure_sb_back(h->sbb_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_sb_back) failed");
-    h->cfg_sbb_smem = h->sbb_smem;
-  }
-  if (h->leaf_smem > 0 && h->cfg_leaf_smem < h->leaf_smem) {
-    if (configure_leaf_elim(h->leaf_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_leaf_elim) failed");
-    h->cfg_leaf_smem = h->leaf_smem;
-  }
-  if (h->leafb_smem > 0 && h->cfg_leafb_smem < h->leafb_smem) {
-    if (configure_leaf_back(h->leafb_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_leaf_back) failed");
-    h->cfg_leafb_smem = h->leafb_smem;
-  }
-  if (h->max_n_smem > 0 && h->cfg_max_n_smem != h->max_n_smem) {
-    if (configure_chol_smem(h->max_n_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_chol_smem) failed");
-    h->cfg_max_n_smem = h->max_n_smem;
-  }
-  if (h->fused_smem > 0 && h->cfg_fused_smem < h->fused_smem) {
-    if (configure_solve_small(h->fused_smem)) return fail(h, 23, "cudaFuncSetAttribute(k_solve_small) failed");
-    h->cfg_fused_smem = h->fused_smem;
-  }
-  launch_state_prep(D, h->n6_total, 0, h->stream);
-  launch_imu_prep(D, h->d_imu_pk.p, h->d_imu_c.p, h->n_imu_total, h->stream);
-  if (any_info) {
-    if ((rc = up(h, h->d_pr_m, st.pr_m)) || (rc = up(h, h->d_pr_info, st.pr_info)) || (rc = up(h, h->d_pr_oJ, st.pr_offJ)) || (rc = up(h, h->d_pr_ov, st.pr_offv))) return rc;
-    launch_prior_from_info(nw, h->max_prior_m, h->d_pr_m.p, h->d_pr_oJ.p, h->d_pr_ov.p, h->d_pr_info.p, h->d_prior_J.p, h->d_prior_A.p, h->d_prior_e0.p, h->stream);
-  }
-  launch_prior_prep(D, h->stream);
-  CK(cudaEventRecord(h->evf2, h->stream));
+  // ---- uploads (pinned -> device, async on the solver stream), kernel attributes, prep kernels
+  if ((rc = upload_and_bind(h, st))) return rc;
+  set_device_view(h, plan);
+  if ((rc = configure_attributes(h)) || (rc = launch_prep(h))) return rc;
   lap(3);
   CK(cudaGetLastError());
   lap(4);
@@ -1591,71 +1597,77 @@ static int upload_state(d2ba_handle *h) {
   if (!xsb.empty()) CK(cudaMemcpyAsync(h->d_xsb[0].p, xsb.data(), xsb.size() * 8, cudaMemcpyHostToDevice, h->stream));
   if (!xlm.empty()) CK(cudaMemcpyAsync(h->d_xlm[0].p, xlm.data(), xlm.size() * 8, cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(h->d_xtd[0].p, xtd.data(), xtd.size() * 8, cudaMemcpyHostToDevice, h->stream));
-  launch_state_prep(h->dev, h->n6_total, 0, h->stream);
+  launch_state_prep(h->dev, h->ls.n6_total, 0, h->stream);
   CK(cudaStreamSynchronize(h->stream));   // host vectors go out of scope
   h->state_dirty = false;
   return 0;
 }
 
-static void enqueue_linearize(d2ba_handle *h, int eval_cur) {
+// Points of the iteration sequence at which d2ba_debug_kernel_times records an event, in enqueue order.
+enum IterMark { kMkGather, kMkSbElim, kMkSchur, kMkLeafElimEnd, kMkChol, kMkSbBack, kMkLeafBack, kMkStep, kMkLin, kMkProj, kMkControl, kMkEnd, kNumMarks };
+// `ev` (nullptr outside d2ba_debug_kernel_times): one event per IterMark, recorded on the solver stream, and one lane only
+static void iter_mark(d2ba_handle *h, cudaEvent_t *ev, IterMark m) { if (ev) cudaEventRecord(ev[m], h->stream); }
+
+static void enqueue_linearize(d2ba_handle *h, int eval_cur, cudaEvent_t *ev = nullptr) {
   // k_misc_lin zero-fills the written runs of Hcc and stores cand_cost_misc before k_imu_lin and k_proj_lin add to them.
   // Two lanes after it: the IMU factors (one warp each) run beside the reprojection kernels and fill their tails.
-  launch_misc_lin(h->dev, eval_cur, h->max_prior_m, h->stream);
-  const bool fork = h->two_lanes && h->n_imu_total > 0;
+  launch_misc_lin(h->dev, eval_cur, h->ls.max_prior_m, h->stream);
+  const bool fork = !ev && h->ls.n_imu_total > 0;
   if (fork) {
     cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0);
-    launch_imu_lin(h->dev, eval_cur, h->n_imu_total, h->side);
+    launch_imu_lin(h->dev, eval_cur, h->ls.n_imu_total, h->side);
     cudaEventRecord(h->ev_join, h->side);
-  } else launch_imu_lin(h->dev, eval_cur, h->n_imu_total, h->stream);
-  for (int v = 0; v < 8; v++) launch_proj_lin(h->dev, v, eval_cur, h->job_begin[v], h->job_count[v], h->stream);
+  } else launch_imu_lin(h->dev, eval_cur, h->ls.n_imu_total, h->stream);
+  iter_mark(h, ev, kMkProj); for (int v = 0; v < 8; v++) launch_proj_lin(h->dev, v, eval_cur, h->ls.job_begin[v], h->ls.job_count[v], h->stream);
   if (fork) cudaStreamWaitEvent(h->stream, h->ev_join, 0);
 }
 
 // reduced camera system: tiles with leaf columns -> leaf elimination (rows Y behind the landmark rows of Wt) -> hub tiles
-static void enqueue_schur(d2ba_handle *h) {
+static void enqueue_schur(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
   // (the leaf kernel forms its own part of the reduced system from Hcc and its landmarks' rows: the stage-0 tiles are
   //  only launched for the debug view of S)
-  if (h->n_leaf_total > 0) launch_leaf_elim(h->dev, h->leaf_smem, h->stream);
-  if (h->ss_unfused) launch_schur_small(h->dev, h->max_ldw_small, 0, h->stream);
-  if (h->n_schur > h->n_schur0) launch_schur(h->dev, h->d_schur.p + h->n_schur0, h->n_schur - h->n_schur0, h->stream);
+  if (h->ls.n_leaf_total > 0) launch_leaf_elim(h->dev, h->ls.leaf_smem, h->stream);
+  iter_mark(h, ev, kMkLeafElimEnd); if (h->ls.ss_unfused) launch_schur_small(h->dev, h->ls.max_ldw_small, 0, h->stream);
+  if (h->ls.n_schur > h->ls.n_schur0) launch_schur(h->dev, h->d_schur.p + h->ls.n_schur0, h->ls.n_schur - h->ls.n_schur0, h->stream);
 }
 // dense Cholesky of the hub, then the eliminated parts' back substitutions
-static void enqueue_solve_reduced(d2ba_handle *h) {
-  if (h->cs_unfused) launch_chol_smem(h->dev, h->max_n_smem, h->stream);
-  if (h->any_chol_glob) launch_chol(h->dev, h->max_rows_glob, h->stream);
-  if (h->sbb_unfused) launch_sb_back(h->dev, h->sbb_smem, h->stream);
-  if (h->n_leaf_total > 0) launch_leaf_back(h->dev, h->leafb_smem, h->stream);
+static void enqueue_solve_reduced(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
+  if (h->ls.cs_unfused) launch_chol_smem(h->dev, h->ls.max_n_smem, h->stream);
+  if (h->ls.any_chol_glob) launch_chol(h->dev, h->ls.max_rows_glob, h->stream);
+  iter_mark(h, ev, kMkSbBack); if (h->ls.sbb_unfused) launch_sb_back(h->dev, h->ls.sbb_smem, h->stream);
+  iter_mark(h, ev, kMkLeafBack); if (h->ls.n_leaf_total > 0) launch_leaf_back(h->dev, h->ls.leafb_smem, h->stream);
 }
 // the step: k_solve_small does the whole reduced-system solve and the step of its windows, k_step the others'
 static void enqueue_step(d2ba_handle *h) {
-  if (h->n_fused > 0) launch_solve_small(h->dev, h->fused_smem, h->stream);
-  launch_step(h->dev, h->max_nc, h->stream);
+  if (h->ls.n_fused > 0) launch_solve_small(h->dev, h->ls.fused_smem, h->stream);
+  launch_step(h->dev, h->ls.max_nc, h->stream);
 }
 
-static void enqueue_iteration(d2ba_handle *h) {
+static void enqueue_iteration(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
   // the speed-bias elimination (Hcc -> its Y rows behind the landmark rows of Wt) does not touch what the landmark gather
   // reads or writes: second lane
-  const bool fork = h->two_lanes && h->sbe_smem > 0;
-  if (fork) { cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0); launch_sb_elim(h->dev, h->sbe_smem, h->side); cudaEventRecord(h->ev_join, h->side); }
-  launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->n_g12, h->stream);
-  if (fork) cudaStreamWaitEvent(h->stream, h->ev_join, 0);
-  else if (h->sbe_smem > 0) launch_sb_elim(h->dev, h->sbe_smem, h->stream);   // Y rows into Wt: the Schur kernels subtract them too
-  enqueue_schur(h);
-  enqueue_solve_reduced(h);
-  enqueue_step(h);
-  enqueue_linearize(h, 0);
-  launch_control(h->dev, 0, h->stream);
+  const bool fork = !ev && h->ls.sbe_smem > 0;
+  iter_mark(h, ev, kMkGather); if (fork) { cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0); launch_sb_elim(h->dev, h->ls.sbe_smem, h->side); cudaEventRecord(h->ev_join, h->side); }
+  launch_lm_gather(h->dev, h->d_lm_win.p, h->ls.nl_total, h->ls.max_row_tiles * 32, h->ls.any_compact, h->ls.any_wide, h->ls.n_g12, h->stream);
+  iter_mark(h, ev, kMkSbElim); if (fork) cudaStreamWaitEvent(h->stream, h->ev_join, 0);
+  else if (h->ls.sbe_smem > 0) launch_sb_elim(h->dev, h->ls.sbe_smem, h->stream);   // Y rows into Wt: the Schur kernels subtract them too
+  iter_mark(h, ev, kMkSchur); enqueue_schur(h, ev);
+  iter_mark(h, ev, kMkChol); enqueue_solve_reduced(h, ev);
+  iter_mark(h, ev, kMkStep); enqueue_step(h);
+  iter_mark(h, ev, kMkLin); enqueue_linearize(h, 0, ev);
+  iter_mark(h, ev, kMkControl); launch_control(h->dev, 0, h->stream);
+  iter_mark(h, ev, kMkEnd);
 }
 
 static int consensus_exchange(d2ba_handle *h) {
-  CK(cudaMemsetAsync(h->d_cons.p, 0, (size_t)std::max(h->n_slots, 1) * 14 * 8, h->stream));
-  launch_cons_pack(h->dev, h->n6_total, h->d_blk_win.p, h->stream);
+  CK(cudaMemsetAsync(h->d_cons.p, 0, (size_t)std::max(h->ls.n_slots, 1) * 14 * 8, h->stream));
+  launch_cons_pack(h->dev, h->ls.n6_total, h->d_blk_win.p, h->stream);
   if (h->comm) {
-    int r = g_nccl.AllReduce(h->d_cons.p, h->d_cons.p, (size_t)h->n_slots * 14, /*ncclFloat64*/ 8, /*ncclSum*/ 0, h->comm, h->stream);
+    int r = g_nccl.AllReduce(h->d_cons.p, h->d_cons.p, (size_t)h->ls.n_slots * 14, /*ncclFloat64*/ 8, /*ncclSum*/ 0, h->comm, h->stream);
     if (r) return fail(h, 40, std::string("ncclAllReduce: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "error"));
   }
-  launch_cons_apply(h->dev, h->n6_total, h->d_blk_win.p, h->stream);
-  launch_cons_refs(h->dev, h->nsb_total, h->nl_total, h->d_sb_win.p, h->d_lm_win.p, h->stream);
+  launch_cons_apply(h->dev, h->ls.n6_total, h->d_blk_win.p, h->stream);
+  launch_cons_refs(h->dev, h->ls.nsb_total, h->ls.nl_total, h->d_sb_win.p, h->d_lm_win.p, h->stream);
   return 0;
 }
 
@@ -1665,9 +1677,9 @@ static int run_solve(d2ba_handle *h, int fixed_iters, d2ba_report *reports) {
   if (!h->finalized) { int rc = d2ba_finalize(h); if (rc) return rc; }
   if (h->state_dirty) { int rc = upload_state(h); if (rc) return rc; }
   const bool fixed = fixed_iters > 0;
-  const int steps = (h->any_admm && h->cfg.consensus_max_steps > 0) ? h->cfg.consensus_max_steps : 1;
+  const int steps = (h->ls.any_admm && h->cfg.consensus_max_steps > 0) ? h->cfg.consensus_max_steps : 1;
   int iters = fixed ? fixed_iters : h->cfg.max_num_iterations;
-  if (steps > 1 || h->any_admm) iters = std::max(1, iters / steps);   // d2vins_params.cpp:156-158
+  if (steps > 1 || h->ls.any_admm) iters = std::max(1, iters / steps);   // d2vins_params.cpp:156-158
   h->dev.prm.fixed_mode = fixed ? 1 : 0; h->dev.prm.max_iter = iters;
   const int key = (fixed ? 1 : 0) * 100000 + iters;
   if (h->graph_key != key) release_graph(h);
@@ -1675,7 +1687,7 @@ static int run_solve(d2ba_handle *h, int fixed_iters, d2ba_report *reports) {
   auto lap = [&](int k) { auto t = std::chrono::steady_clock::now(); h->solve_ms[k] = std::chrono::duration<double, std::milli>(t - tq).count(); tq = t; };
   CK(cudaEventRecord(h->ev0, h->stream));
   launch_tr_reset(h->dev, 1, h->stream);
-  if (h->any_admm) launch_cons_init(h->dev, h->n6_total, h->stream);
+  if (h->ls.any_admm) launch_cons_init(h->dev, h->ls.n6_total, h->stream);
   // ceres max_solver_time_in_seconds: an iteration is only started while the budget of this (sub-)step lasts.  The
   // iterations are enqueued asynchronously, so the host trails the device by at most two of them: before enqueuing
   // iteration k it waits for iteration k-2 and compares the wall clock.
@@ -1690,7 +1702,7 @@ static int run_solve(d2ba_handle *h, int fixed_iters, d2ba_report *reports) {
   for (int st = 0; st < steps; st++) {
     t_step0 = std::chrono::steady_clock::now();
     if (st > 0) launch_tr_reset(h->dev, 0, h->stream);
-    if (h->any_admm) { int rc = consensus_exchange(h); if (rc) return rc; }
+    if (h->ls.any_admm) { int rc = consensus_exchange(h); if (rc) return rc; }
     enqueue_linearize(h, 1);
     launch_control(h->dev, st == 0 ? 1 : 2, h->stream);
     // A graph pays off when the same structure is solved repeatedly (ADMM sub-steps, re-solves, the device-resident
@@ -1712,7 +1724,7 @@ static int run_solve(d2ba_handle *h, int fixed_iters, d2ba_report *reports) {
   }
   CK(cudaEventRecord(h->ev1, h->stream));
   // read back control blocks and both state buffers (the accepted buffer differs per window)
-  CK(cudaMemcpyAsync(h->h_ctl.p, h->d_ctl.p, sizeof(Ctl) * h->n_used, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(h->h_ctl.p, h->d_ctl.p, sizeof(Ctl) * h->ls.n_used, cudaMemcpyDeviceToHost, h->stream));
   for (int b = 0; b < 2; b++) {
     CK(cudaMemcpyAsync(h->h_x6[b].p, h->d_x6[b].p, h->h_x6[b].n * 8, cudaMemcpyDeviceToHost, h->stream));
     if (h->h_xsb[b].n) CK(cudaMemcpyAsync(h->h_xsb[b].p, h->d_xsb[b].p, h->h_xsb[b].n * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -1812,7 +1824,7 @@ int d2ba_comm_init(d2ba_handle *h, const uint8_t unique_id[128], int32_t rank, i
 }
 int d2ba_consensus_buffer(d2ba_handle *h, void **dev_ptr, int64_t *n_doubles) {
   if (!h || !h->finalized) return 1;
-  *dev_ptr = h->d_cons.p; *n_doubles = (int64_t)h->n_slots * 14;
+  *dev_ptr = h->d_cons.p; *n_doubles = (int64_t)h->ls.n_slots * 14;
   return 0;
 }
 
@@ -1821,9 +1833,9 @@ int d2ba_consensus_buffer(d2ba_handle *h, void **dev_ptr, int64_t *n_doubles) {
 // never needs them (td constant): fetch the motion halves that d2ba_finalize left on the host and rebuild the tiles.
 static int ensure_motion(d2ba_handle *h) {
   if (!h->motion_skipped) return 0;
-  std::vector<long long> off(4 * (size_t)h->n_used);
+  std::vector<long long> off(4 * (size_t)h->ls.n_used);
   CK(cudaMemcpy(off.data(), h->d_raw_off.p, off.size() * 8, cudaMemcpyDeviceToHost));
-  for (int wi = 0; wi < h->n_used; wi++) {
+  for (int wi = 0; wi < h->ls.n_used; wi++) {
     HostWin &w = h->win[wi];
     int rc;
     if ((rc = push_range(h, w.rawjm, w.d_rawjm, w.pushed_jm)) || (rc = push_range(h, w.anchm, w.d_anchm, w.pushed_am))) return rc;
@@ -1832,7 +1844,7 @@ static int ensure_motion(d2ba_handle *h) {
   }
   CK(cudaStreamSynchronize(h->copy_stream));
   CK(cudaMemcpy(h->d_raw_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
-  launch_build_tiles(h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, h->n_tiles, h->stream);
+  launch_build_tiles(h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, h->ls.n_tiles, h->stream);
   h->motion_skipped = false;
   return 0;
 }
@@ -1845,27 +1857,27 @@ int d2ba_debug_linearize(d2ba_handle *h) {
   if (h->state_dirty) { int rc = upload_state(h); if (rc) return rc; }
   h->dev.prm.fixed_mode = 1; h->dev.prm.max_iter = 1;
   launch_tr_reset(h->dev, 1, h->stream);
-  if (h->any_admm) {   // ADMM terms as at the start of a solve (z = x, tilde = 0, references = state), not whatever the buffers held
-    launch_cons_init(h->dev, h->n6_total, h->stream);
-    launch_cons_refs(h->dev, h->nsb_total, h->nl_total, h->d_sb_win.p, h->d_lm_win.p, h->stream);
+  if (h->ls.any_admm) {   // ADMM terms as at the start of a solve (z = x, tilde = 0, references = state), not whatever the buffers held
+    launch_cons_init(h->dev, h->ls.n6_total, h->stream);
+    launch_cons_refs(h->dev, h->ls.nsb_total, h->ls.nl_total, h->d_sb_win.p, h->d_lm_win.p, h->stream);
   }
   enqueue_linearize(h, 1);
   launch_control(h->dev, 1, h->stream);
-  launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->n_g12, h->stream);
+  launch_lm_gather(h->dev, h->d_lm_win.p, h->ls.nl_total, h->ls.max_row_tiles * 32, h->ls.any_compact, h->ls.any_wide, h->ls.n_g12, h->stream);
   // debug view: the landmark-only Schur complement (eliminated speed-bias rows zeroed), kept un-factored in d_dbg
-  if (h->sbe_smem > 0) launch_zero_sb_rows(h->dev, h->stream);
-  if (h->n_leaf_total > 0) launch_zero_leaf_rows(h->dev, h->stream);
-  if (h->max_ldw_small > 0) launch_schur_small(h->dev, h->max_ldw_small, 1, h->stream);   // k_solve_small's windows too
-  launch_schur(h->dev, h->d_schur.p, h->n_schur, h->stream);   // both stages back to back: no eliminated rows in this view
-  CK(h->d_dbg.alloc((size_t)h->totH));
-  CK(cudaMemcpyAsync(h->d_dbg.p, h->d_S.p, (size_t)h->totH * 8, cudaMemcpyDeviceToDevice, h->stream));
-  if (h->sbe_smem > 0 || h->n_leaf_total > 0) {   // now the system the solver factors: Y rows in place, Schur again
-    if (h->sbe_smem > 0) launch_sb_elim(h->dev, h->sbe_smem, h->stream);
+  if (h->ls.sbe_smem > 0) launch_zero_sb_rows(h->dev, h->stream);
+  if (h->ls.n_leaf_total > 0) launch_zero_leaf_rows(h->dev, h->stream);
+  if (h->ls.max_ldw_small > 0) launch_schur_small(h->dev, h->ls.max_ldw_small, 1, h->stream);   // k_solve_small's windows too
+  launch_schur(h->dev, h->d_schur.p, h->ls.n_schur, h->stream);   // both stages back to back: no eliminated rows in this view
+  CK(h->d_dbg.alloc((size_t)h->ls.totH));
+  CK(cudaMemcpyAsync(h->d_dbg.p, h->d_S.p, (size_t)h->ls.totH * 8, cudaMemcpyDeviceToDevice, h->stream));
+  if (h->ls.sbe_smem > 0 || h->ls.n_leaf_total > 0) {   // now the system the solver factors: Y rows in place, Schur again
+    if (h->ls.sbe_smem > 0) launch_sb_elim(h->dev, h->ls.sbe_smem, h->stream);
     enqueue_schur(h);
   }
   enqueue_solve_reduced(h);
   enqueue_step(h);   // the fused solve the iteration runs: DBG_GN_STEP / DBG_STEP show what it computed
-  CK(cudaMemcpyAsync(h->h_ctl.p, h->d_ctl.p, sizeof(Ctl) * h->n_used, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(h->h_ctl.p, h->d_ctl.p, sizeof(Ctl) * h->ls.n_used, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   CK(cudaGetLastError());
   release_graph(h);
@@ -1889,7 +1901,7 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     case D2BA_DBG_N_LC: { int64_t v = nlc; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
     case D2BA_DBG_SOLVE_PATH: { int64_t v = d.fused_solve ? 1 : 0; buf.resize(8); memcpy(buf.data(), &v, 8); break; }
     case D2BA_DBG_PLAN: {   // field order: include/d2ba.h
-      const int64_t v[20] = {d.fused_solve, d.schur_small, d.hub_small, d.chol_smem, h->cs_unfused ? chol_smem_threads(h->max_n_smem) : 0,
+      const int64_t v[20] = {d.fused_solve, d.schur_small, d.hub_small, d.chol_smem, h->ls.cs_unfused ? chol_smem_threads(h->ls.max_n_smem) : 0,
                              d.sb_elim, d.n_sbe, d.n_leaf, d.hub0, d.n_hub,
                              d.n_lc, d.n_c, d.ldw, d.rec_stride, d.gather_nosync, d.row_tiles,
                              w->n_g12, d.n_tile, w->n_schur_tiles[0], w->n_schur_tiles[1]};
@@ -1898,7 +1910,7 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     case D2BA_DBG_LIN_JOBS: {   // field order: include/d2ba.h
       int64_t v[42];
       memcpy(v, w->lin_jobs, sizeof w->lin_jobs);
-      v[40] = motion_needed(*w) ? 1 : 0; v[41] = h->tpj_target;
+      v[40] = motion_needed(*w) ? 1 : 0; v[41] = h->ls.tpj_target;
       buf.resize(sizeof v); memcpy(buf.data(), v, sizeof v); break;
     }
     case D2BA_DBG_HCC: {   // Hcc is stored lower-triangular in device column order: symmetric, canonical order out
@@ -1919,7 +1931,7 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     }
     case D2BA_DBG_COST: { std::vector<double> v(1, h->h_ctl.p[window].cost); put_d(v); break; }
     case D2BA_DBG_S: {
-      if (h->d_dbg.n < (size_t)h->totH) return fail(h, 4, "debug_get(S): call d2ba_debug_linearize first");
+      if (h->d_dbg.n < (size_t)h->ls.totH) return fail(h, 4, "debug_get(S): call d2ba_debug_linearize first");
       auto S = fetch(h->d_dbg.p + d.offH, (size_t)n * ld);
       if (d.sb_elim || (d.schur_small && d.chol_smem)) {
         // the speed-bias rows of such windows never pass through S (k_sb_elim / k_chol_smem read them from Hcc): rebuild them
@@ -1958,8 +1970,8 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     }
     case D2BA_DBG_PROJ_RESJAC: {
       DBuf<double> tmp;
-      if (tmp.alloc((size_t)h->n_tiles * kTile * 81) != cudaSuccess) return fail(h, 5, "debug alloc");
-      launch_proj_debug(h->dev, tmp.p, h->n_tiles, h->d_tile_win.p, h->stream);
+      if (tmp.alloc((size_t)h->ls.n_tiles * kTile * 81) != cudaSuccess) return fail(h, 5, "debug alloc");
+      launch_proj_debug(h->dev, tmp.p, h->ls.n_tiles, h->d_tile_win.p, h->stream);
       cudaStreamSynchronize(h->stream);
       std::vector<double> all((size_t)d.n_tile * kTile * 81);
       if (!all.empty()) cudaMemcpy(all.data(), tmp.p + (size_t)d.off_tile * kTile * 81, all.size() * 8, cudaMemcpyDeviceToHost);
@@ -1971,7 +1983,7 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     case D2BA_DBG_IMU_RESJAC: {
       // imu -> window map built here (debug only)
       std::vector<int> iw;
-      for (int wi2 = 0; wi2 < h->n_used; wi2++) iw.insert(iw.end(), h->h_win[wi2].n_imu, wi2);
+      for (int wi2 = 0; wi2 < h->ls.n_used; wi2++) iw.insert(iw.end(), h->h_win[wi2].n_imu, wi2);
       DBuf<double> tmp; DBuf<int> dw;
       if (tmp.alloc((size_t)std::max<size_t>(iw.size(), 1) * 465) != cudaSuccess || dw.alloc(std::max<size_t>(iw.size(), 1)) != cudaSuccess) return fail(h, 5, "debug alloc");
       if (!iw.empty()) cudaMemcpy(dw.p, iw.data(), iw.size() * sizeof(int), cudaMemcpyHostToDevice);
@@ -1982,8 +1994,8 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     }
     case D2BA_DBG_CONS_RESJAC: {
       DBuf<double> tmp;
-      if (tmp.alloc((size_t)std::max(h->n6_total, 1) * 62) != cudaSuccess) return fail(h, 5, "debug alloc");
-      launch_cons_debug(h->dev, tmp.p, h->d_blk_win.p, h->n6_total, h->stream);
+      if (tmp.alloc((size_t)std::max(h->ls.n6_total, 1) * 62) != cudaSuccess) return fail(h, 5, "debug alloc");
+      launch_cons_debug(h->dev, tmp.p, h->d_blk_win.p, h->ls.n6_total, h->stream);
       cudaStreamSynchronize(h->stream);
       put_d(fetch(tmp.p + (size_t)d.off6 * 62, (size_t)d.n6 * 62));
       tmp.release(); break;
@@ -2120,9 +2132,9 @@ int d2ba_marginalize(d2ba_handle *h, int32_t window, int32_t n_remove, const int
   launch_tr_reset(t->dev, 1, t->stream);
   enqueue_linearize(t, 1);
   launch_control(t->dev, 1, t->stream);
-  launch_lm_gather(t->dev, t->d_lm_win.p, t->nl_total, t->max_row_tiles * 32, t->any_compact, t->any_wide, t->n_g12, t->stream);
-  if (t->max_ldw_small > 0) launch_schur_small(t->dev, t->max_ldw_small, 1, t->stream);
-  launch_schur(t->dev, t->d_schur.p, t->n_schur, t->stream);
+  launch_lm_gather(t->dev, t->d_lm_win.p, t->ls.nl_total, t->ls.max_row_tiles * 32, t->ls.any_compact, t->ls.any_wide, t->ls.n_g12, t->stream);
+  if (t->ls.max_ldw_small > 0) launch_schur_small(t->dev, t->ls.max_ldw_small, 1, t->stream);
+  launch_schur(t->dev, t->d_schur.p, t->ls.n_schur, t->stream);
   // eliminate the removed camera columns
   DBuf<int> d_keep, d_rem, d_flag; DBuf<double> d_A, d_b;
   cudaError_t ce;
@@ -2157,8 +2169,8 @@ int d2ba_debug_solve_occupancy(d2ba_handle *h, int32_t *ctas_per_sm) {
   cudaSetDevice(h->cfg.device);
   if (!h->finalized) { int rc = d2ba_finalize(h); if (rc) return rc; }
   *ctas_per_sm = 0;
-  if (h->n_fused == 0) return 0;
-  const int n = solve_small_occupancy(h->fused_smem);
+  if (h->ls.n_fused == 0) return 0;
+  const int n = solve_small_occupancy(h->ls.fused_smem);
   if (n < 0) return fail(h, 5, "cudaOccupancyMaxActiveBlocksPerMultiprocessor(k_solve_small) failed");
   *ctas_per_sm = n;
   return 0;
@@ -2172,42 +2184,27 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
   h->dev.prm.fixed_mode = 1; h->dev.prm.max_iter = iters;
   release_graph(h);
   launch_tr_reset(h->dev, 1, h->stream);
-  if (h->any_admm) { launch_cons_init(h->dev, h->n6_total, h->stream); int rc = consensus_exchange(h); if (rc) return rc; }
+  if (h->ls.any_admm) { launch_cons_init(h->dev, h->ls.n6_total, h->stream); int rc = consensus_exchange(h); if (rc) return rc; }
   enqueue_linearize(h, 1);
   launch_control(h->dev, 1, h->stream);
-  cudaEvent_t ev[8], evs[2], evl[3];
-  for (int i = 0; i < 3; i++) cudaEventCreate(&evl[i]);
-  for (int i = 0; i < 8; i++) cudaEventCreate(&ev[i]);
-  cudaEventCreate(&evs[0]); cudaEventCreate(&evs[1]);
+  cudaEvent_t ev[kNumMarks];
+  for (cudaEvent_t &e : ev) cudaEventCreate(&e);
+  // ms_out[i] sums the span between two marks ([7] is the iteration count)
+  static const IterMark span[12][2] = {{kMkGather, kMkSchur}, {kMkSchur, kMkChol}, {kMkChol, kMkStep}, {kMkStep, kMkLin}, {kMkLin, kMkProj},
+                                       {kMkProj, kMkControl}, {kMkControl, kMkEnd}, {kMkEnd, kMkEnd}, {kMkSbElim, kMkSchur},
+                                       {kMkSbBack, kMkLeafBack}, {kMkSchur, kMkLeafElimEnd}, {kMkLeafBack, kMkStep}};
   for (int i = 0; i < 12; i++) ms_out[i] = 0;
   for (int it = 0; it < iters; it++) {
-    cudaEventRecord(ev[0], h->stream); launch_lm_gather(h->dev, h->d_lm_win.p, h->nl_total, h->max_row_tiles * 32, h->any_compact, h->any_wide, h->n_g12, h->stream);
-    cudaEventRecord(evs[0], h->stream); if (h->sbe_smem > 0) launch_sb_elim(h->dev, h->sbe_smem, h->stream);
-    cudaEventRecord(ev[1], h->stream);
-    cudaEventRecord(evl[0], h->stream);
-    if (h->n_leaf_total > 0) launch_leaf_elim(h->dev, h->leaf_smem, h->stream);
-    cudaEventRecord(evl[1], h->stream);
-    if (h->ss_unfused) launch_schur_small(h->dev, h->max_ldw_small, 0, h->stream);
-    if (h->n_schur > h->n_schur0) launch_schur(h->dev, h->d_schur.p + h->n_schur0, h->n_schur - h->n_schur0, h->stream);
-    cudaEventRecord(ev[2], h->stream); if (h->cs_unfused) launch_chol_smem(h->dev, h->max_n_smem, h->stream); if (h->any_chol_glob) launch_chol(h->dev, h->max_rows_glob, h->stream); cudaEventRecord(evs[1], h->stream); if (h->sbb_unfused) launch_sb_back(h->dev, h->sbb_smem, h->stream);
-    cudaEventRecord(evl[2], h->stream); if (h->n_leaf_total > 0) launch_leaf_back(h->dev, h->leafb_smem, h->stream);
-    cudaEventRecord(ev[3], h->stream); enqueue_step(h);
-    cudaEventRecord(ev[4], h->stream); launch_misc_lin(h->dev, 0, h->max_prior_m, h->stream); launch_imu_lin(h->dev, 0, h->n_imu_total, h->stream);
-    cudaEventRecord(ev[5], h->stream); for (int v = 0; v < 8; v++) launch_proj_lin(h->dev, v, 0, h->job_begin[v], h->job_count[v], h->stream);
-    cudaEventRecord(ev[6], h->stream); launch_control(h->dev, 0, h->stream);
-    cudaEventRecord(ev[7], h->stream);
+    enqueue_iteration(h, ev);
     CK(cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < 7; i++) { float ms = 0; cudaEventElapsedTime(&ms, ev[i], ev[i + 1]); ms_out[i] += ms; }
-    { float ms = 0; cudaEventElapsedTime(&ms, evs[0], ev[1]); ms_out[8] += ms; cudaEventElapsedTime(&ms, evs[1], evl[2]); ms_out[9] += ms;
-      cudaEventElapsedTime(&ms, evl[0], evl[1]); ms_out[10] += ms; cudaEventElapsedTime(&ms, evl[2], ev[3]); ms_out[11] += ms; }
+    for (int i = 0; i < 12; i++) if (i != 7) { float ms = 0; cudaEventElapsedTime(&ms, ev[span[i][0]], ev[span[i][1]]); ms_out[i] += ms; }
   }
   ms_out[7] = iters;
-  for (int i = 0; i < 8; i++) cudaEventDestroy(ev[i]);
-  cudaEventDestroy(evs[0]); cudaEventDestroy(evs[1]);
-  for (int i = 0; i < 3; i++) cudaEventDestroy(evl[i]);
+  for (cudaEvent_t e : ev) cudaEventDestroy(e);
   CK(cudaGetLastError());
   h->state_dirty = true;
   return 0;
 }
 
 }  // extern "C"
+
