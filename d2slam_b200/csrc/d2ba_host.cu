@@ -11,7 +11,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <array>
 #include <atomic>
 #include <chrono>
 #include <mutex>
@@ -21,65 +20,9 @@
 #include <vector>
 
 #include "../../include/d2ba.h"
+#include "d2ba_launch.cuh"
 #include "d2ba_types.cuh"
 
-namespace d2ba {
-// launchers implemented in d2ba_kernels.cu
-void launch_state_prep(const Dev &d, int n6_total, int buf, cudaStream_t s);
-void launch_imu_prep(const Dev &d, const double *packed, double *full, int n_imu, cudaStream_t s);
-void launch_prior_prep(const Dev &d, cudaStream_t s);
-void launch_misc_lin(const Dev &d, int eval_cur, int max_prior_m, cudaStream_t s);
-void launch_imu_lin(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s);
-int configure_kernels(int max_rows, int max_nc, int max_prior_m);
-int configure_gather(int max_ldw);
-void launch_proj_lin(const Dev &d, int variant, int eval_cur, int job_begin, int job_count, cudaStream_t s);
-void launch_proj_debug(const Dev &d, double *out, int n_tiles, const int *tile_win, cudaStream_t s);
-void launch_imu_debug(const Dev &d, double *out, const int *imu_win, int n, cudaStream_t s);
-void launch_cons_debug(const Dev &d, double *out, const int *blk_win, int n, cudaStream_t s);
-void launch_lm_gather(const Dev &d, const int *lm_win, int n_lm_total, int max_ldw, int any_compact, int any_wide, int n_chunk12, cudaStream_t s);
-void launch_schur(const Dev &d, const void *tiles, int n_tiles, cudaStream_t s);
-int configure_leaf_elim(size_t smem);
-void launch_leaf_elim(const Dev &d, size_t smem, cudaStream_t s);
-void launch_leaf_back(const Dev &d, size_t smem, cudaStream_t s);
-size_t leaf_back_smem(int n, int n_hub);
-int configure_leaf_back(size_t smem);
-void launch_zero_leaf_rows(const Dev &d, cudaStream_t s);
-void launch_schur_small(const Dev &d, int max_ldw, int with_fused, cudaStream_t s);
-int configure_schur_small(int max_ldw);
-bool solve_small_fits(int ldw);
-size_t solve_small_smem(int ldw, int n_lc, int n_c, int nb);
-int configure_solve_small(size_t smem);
-void launch_solve_small(const Dev &d, size_t smem, cudaStream_t s);
-int solve_small_occupancy(size_t smem);
-void launch_chol(const Dev &d, int max_rows, cudaStream_t s);
-size_t chol_smem_need(int n);
-int configure_chol_smem(int max_n);
-void launch_chol_smem(const Dev &d, int max_n, cudaStream_t s);
-int chol_smem_threads(int max_n);
-size_t sb_elim_smem(int ldw, int n_c, int nb);
-size_t sb_back_smem(int nlc, int nb);
-int configure_sb_back(size_t smem);
-void launch_zero_sb_rows(const Dev &d, cudaStream_t s);
-int configure_sb_elim(size_t smem);
-void launch_sb_elim(const Dev &d, size_t smem, cudaStream_t s);
-void launch_sb_back(const Dev &d, size_t smem, cudaStream_t s);
-int sb_max_blocks();
-void launch_step(const Dev &d, int max_nc, cudaStream_t s);
-void launch_control(const Dev &d, int init, cudaStream_t s);
-void launch_tr_reset(const Dev &d, int first, cudaStream_t s);
-void launch_cons_init(const Dev &d, int n6_total, cudaStream_t s);
-void launch_cons_pack(const Dev &d, int n6_total, const int *blk_win, cudaStream_t s);
-void launch_cons_apply(const Dev &d, int n6_total, const int *blk_win, cudaStream_t s);
-void launch_cons_refs(const Dev &d, int nsb_total, int nl_total, const int *sb_win, const int *lm_win, cudaStream_t s);
-typedef SchurTile SchurTileH;
-size_t leaf_elim_smem(int n, int n_hub);
-int leaf_max_cols();
-int launch_marg_reduce(const double *S, int ld, int n, const int *keep_idx, int nk, const int *rem_idx, int nr, double *A, double *b, int *fail_flag,
-                       cudaStream_t s);
-void launch_build_tiles(const long long *raw_off, const int *tile_src, const int *tile_win, const double *xtd, double *obs, int n_tiles, cudaStream_t s);
-void launch_prior_from_info(int n_win, int max_m, const int *m_of, const long long *offJ, const long long *offv, const int *is_info,
-                            double *A, double *V, double *b, cudaStream_t s);
-}  // namespace d2ba
 
 using namespace d2ba;
 
@@ -262,32 +205,12 @@ struct Staging {   // every array finalize uploads lives in ONE pinned arena -> 
   HView<WinDesc> win; HView<double> x6, xsb, xlm, xtd, imu_c, prior_J, prior_e0;
   HView<int> col6, colsb, tile_grp, tile_win, obs_lm, tile_src, lm_ptr, obs_slot, slot6, lm_win, blk_win, sb_win, pr_m, pr_info;
   HView<long long> raw_off, pr_offJ, pr_offv;
-  HView<Group> grp; HView<Job> job; HView<ImuDesc> imu; HView<PriorBlk> pblk; HView<SchurTileH> schur;
+  HView<Group> grp; HView<Job> job; HView<ImuDesc> imu; HView<PriorBlk> pblk; HView<SchurTile> schur;
   HView<int> schur_chunks, leaf_lm; HView<Leaf> leaf; HView<HSeg> hseg; HView<unsigned long long> lm_mask; HView<int4> g12;
   template <typename T> void reserve(HView<T> &v, size_t count) { v.n = count; v.off = cursor; cursor += (count * sizeof(T) + 255) & ~(size_t)255; }
   template <typename T> void place(HView<T> &v) { v.p = (T *)(arena.p + v.off); }
 };
 
-// What d2ba_finalize derives for the handle as a whole: array totals, the maxima the kernels are sized and configured for,
-// and which kernels the iteration launches.  Value-initialised by every finalize.
-struct LaunchSummary {
-  int n_used = 0, n6_total = 0, nsb_total = 0, nl_total = 0, n_tiles = 0, n_imu_total = 0, n_slots = 0;   // windows, blocks, ...
-  int n_grp = 0, n_lmptr = 0, n_pblk = 0, n_leaf_total = 0, n_hseg = 0, n_leaf_lm = 0, n_chunks = 0, n_g12 = 0;
-  int n_schur = 0, n_schur0 = 0;                     // Schur tiles; the first n_schur0 are stage 0 (leaf columns)
-  int n_jobs = 0, job_begin[8] = {}, job_count[8] = {};   // reprojection jobs per launch_proj_lin variant
-  int tpj_target = 1;                                // observation tiles per reprojection job (D2BA_DBG_LIN_JOBS)
-  int64_t totH = 0, totW = 0, totc = 0, totLE = 0, totLL = 0, tot_rec = 0, tot_pJ = 0, tot_pv = 0;   // doubles
-  int max_nc = 1, max_prior_m = 0, max_row_tiles = 1, max_ldw_small = 0;
-  int max_n_smem = 0, max_rows_glob = 1; bool any_chol_glob = false;   // dense Cholesky: shared-memory / global kernel
-  int any_compact = 0, any_wide = 0;                 // record widths present (which gather kernels to launch)
-  bool any_admm = false, any_info = false;           // consensus terms / a prior given in information form
-  // dynamic shared memory of k_leaf_elim, k_leaf_back, k_sb_elim and k_sb_back (0 = no window uses the kernel)
-  size_t leaf_smem = 0, leafb_smem = 0, sbe_smem = 0, sbb_smem = 0;
-  // one-kernel reduced-system solve (k_solve_small) of the windows with WinDesc::fused_solve; the separate kernels are
-  // launched only when some window still needs them
-  int n_fused = 0; size_t fused_smem = 0;
-  bool ss_unfused = false, cs_unfused = false, sbb_unfused = false;
-};
 
 }  // namespace
 
@@ -313,7 +236,7 @@ struct d2ba_handle {
   DBuf<Group> d_grp; DBuf<Job> d_job; DBuf<ImuDesc> d_imu; DBuf<PriorBlk> d_prior_blk;
   DBuf<double> d_obs, d_rec[2], d_imu_c, d_imu_pk, d_imu_U, d_prior_J, d_prior_e0, d_prior_A, d_z6, d_tilde6, d_lm_ref, d_sb_ref, d_td_ref,
       d_cons, d_H[2], d_gc[2], d_Wt, d_dinv, d_hl, d_gl, d_S, d_gred, d_D2c, d_gn_c, d_gn_l, d_step_c, d_step_l, d_wu, d_uc, d_D2l, d_dbg;
-  DBuf<SchurTileH> d_schur; DBuf<int> d_schur_chunks; DBuf<Leaf> d_leaf; DBuf<HSeg> d_hseg; DBuf<unsigned long long> d_lm_mask; DBuf<double> d_leafL; DBuf<int> d_leaf_lm; DBuf<int4> d_g12;
+  DBuf<SchurTile> d_schur; DBuf<int> d_schur_chunks; DBuf<Leaf> d_leaf; DBuf<HSeg> d_hseg; DBuf<unsigned long long> d_lm_mask; DBuf<double> d_leafL; DBuf<int> d_leaf_lm; DBuf<int4> d_g12;
   DBuf<int> d_pr_m, d_pr_info, d_tile_src; DBuf<long long> d_pr_oJ, d_pr_ov, d_raw_off;
   DBuf<double> d_sbLE;
   Dev dev;
@@ -321,10 +244,6 @@ struct d2ba_handle {
   HBuf<Ctl> h_ctl;   // pinned: D2H target of every solve
   Staging st;
   LaunchSummary ls;
-  // what the kernel attributes were last configured for (they outlive a finalize)
-  std::array<int, 3> cfg_kernels = {-1, -1, -1};   // configure_kernels: max_rows_glob, max_nc, max_prior_m
-  int cfg_max_ldw = -1, cfg_max_ldw_small = -1, cfg_max_n_smem = -1;
-  size_t cfg_leaf_smem = 0, cfg_leafb_smem = 0, cfg_sbb_smem = 0, cfg_sbe_smem = 0, cfg_fused_smem = 0;
   // host mirrors of the solved state
   HBuf<double> h_x6[2], h_xsb[2], h_xlm[2], h_xtd[2];   // pinned D2H targets
   // graph cache
@@ -791,7 +710,7 @@ struct WinPlan {
   std::vector<Group> groups;
   std::vector<int> grp_begin, grp_cnt, grp_tile0;   // sorted-obs range and first (window-local) tile of each group
   std::vector<Job> jobs[8];                         // tile_begin window-local, grp window-local; index = launch_proj_lin variant
-  std::vector<SchurTileH> schur[2];                  // stage 0 (tiles with leaf columns), stage 1 (hub x hub)
+  std::vector<SchurTile> schur[2];                  // stage 0 (tiles with leaf columns), stage 1 (hub x hub)
   std::vector<int> schur_chunks;                     // chunk lists, window-local offsets in SchurTile::cb
   std::vector<uint64_t> hruns; std::vector<Leaf> leaves; std::vector<HSeg> hseg; std::vector<unsigned long long> lm_mask; std::vector<int> leaf_lm; int leaf_lm_off = 0;
   int n_tiles = 0, n_lmobs = 0;
@@ -856,7 +775,7 @@ void find_leaves(const HostWin &w, int nlc_cnt, std::vector<std::vector<int>> &l
   std::vector<std::vector<int>> kept;
   for (auto &lf : leaves) {
     const int nl6 = 6 * (int)lf.size();
-    if (nl6 <= leaf_max_cols() && n_hub_cols >= 1 && leaf_elim_smem(nl6, n_hub_cols) <= kElimSmemCap) kept.push_back(lf);
+    if (nl6 <= kLeafMaxCols && n_hub_cols >= 1 && leaf_elim_smem_bytes(nl6, n_hub_cols) <= kElimSmemCap) kept.push_back(lf);
     else n_hub_cols += nl6;
   }
   // worthwhile only when the hub is a real reduction of the dense part
@@ -887,7 +806,7 @@ void plan_columns(HostWin &w, const PlanOpts &o, int wi, WinPlan &pl) {
     }
     int pmin = 1 << 30, pmax = -1;
     for (const HPriorBlk &b : w.prior_blk) if (b.kind == D2BA_SPEED_BIAS && pos[b.index] >= 0) { pmin = std::min(pmin, pos[b.index]); pmax = std::max(pmax, pos[b.index]); }
-    if (pmax - pmin > 1 || nb > sb_max_blocks()) pl.sb_ok = false;
+    if (pmax - pmin > 1 || nb > kSeMaxBlocks) pl.sb_ok = false;
     d.n_sbe = nb;
   }
   std::vector<std::vector<int>> leaves;
@@ -1111,12 +1030,12 @@ void plan_solve(const HostWin &w, const PlanOpts &o, WinPlan &pl) {
   d.hub_small = (d.n_leaf > 0 && d.n_hub + 1 <= kSmallCols) ? 1 : 0;
   const int nb = d.n_sbe, hubw = roundup(d.n_hub + 1, 8);
   bool ok = pl.sb_ok && w.n_c == w.n_lc + 9 * nb;
-  if (ok && (sb_elim_smem(hubw, d.n_c, nb) > kElimSmemCap || sb_back_smem(d.n_hub, nb) > kElimSmemCap)) ok = false;
+  if (ok && (sbe_smem_bytes(hubw, d.n_c, nb) > kElimSmemCap || sb_back_smem_bytes(d.n_hub, nb) > kElimSmemCap)) ok = false;
   pl.leaves_without_sb_elim = !ok && d.n_leaf > 0 && nb > 0;
   d.sb_elim = ok ? 1 : 0;
   // with speed-bias or leaf elimination the dense Cholesky only sees the hub of the pose part
-  if (ok || d.n_leaf > 0) d.chol_smem = (chol_smem_need(d.n_hub) <= kCholSmemCap) ? 1 : 0;
-  else d.chol_smem = (!o.force_full_S && w.n_c >= 1 && chol_smem_need(w.n_c) <= kCholSmemCap) ? 1 : 0;
+  if (ok || d.n_leaf > 0) d.chol_smem = (chol_smem_bytes(d.n_hub) <= kCholSmemCap) ? 1 : 0;
+  else d.chol_smem = (!o.force_full_S && w.n_c >= 1 && chol_smem_bytes(w.n_c) <= kCholSmemCap) ? 1 : 0;
   // single-drone window whose whole reduced-system solve fits one CTA (k_solve_small)
   d.fused_solve = (!o.no_fused_solve && d.n_leaf == 0 && d.sb_elim && d.schur_small && d.chol_smem && solve_small_fits(d.ldw)) ? 1 : 0;
   // rows of Wt the Schur kernels sum over: landmark rows, then the eliminated speed-bias rows, then the leaves' rows
@@ -1183,7 +1102,7 @@ void plan_schur_tiles(HostWin &w, int wi, WinPlan &pl) {
           const bool in_hub = (tm * 32 + 31 >= d.hub0) && (tn * 32 + 31 >= d.hub0);
           const bool has_leaf = tn * 32 < d.hub0;
           if (stage == 0 ? !has_leaf : (!in_hub || d.hub_small)) continue;   // hub_small: k_schur_small forms the hub x hub part
-          SchurTileH t{wi, stage == 0 ? 2 : 0, tm, tn, (int)pl.schur_chunks.size(), 0};   // kind 2: only entries in leaf columns are stored
+          SchurTile t{wi, stage == 0 ? 2 : 0, tm, tn, (int)pl.schur_chunks.size(), 0};   // kind 2: only entries in leaf columns are stored
           const int kend = stage == 0 ? lm_chunks : nchunk;
           for (int kc = 0; kc < kend; kc++) if (((cmask[kc] >> tm) & 1ull) && ((cmask[kc] >> tn) & 1ull)) pl.schur_chunks.push_back(kc);
           t.cn = (int)pl.schur_chunks.size() - t.cb;
@@ -1191,7 +1110,7 @@ void plan_schur_tiles(HostWin &w, int wi, WinPlan &pl) {
           pl.schur[stage].push_back(t);
         }
     int t_lo = d.n_lc / 32, t_hi = d.n_c / 32;
-    if (!d.sb_elim) for (int tm = t_lo; tm <= t_hi; tm++) for (int tn = 0; tn <= tm; tn++) pl.schur[1].push_back(SchurTileH{wi, 1, tm, tn, 0, 0});
+    if (!d.sb_elim) for (int tm = t_lo; tm <= t_hi; tm++) for (int tn = 0; tn <= tm; tn++) pl.schur[1].push_back(SchurTile{wi, 1, tm, tn, 0, 0});
   }
   w.n_schur_tiles[0] = (int)pl.schur[0].size(); w.n_schur_tiles[1] = (int)pl.schur[1].size();
 }
@@ -1229,7 +1148,7 @@ int plan_offsets(d2ba_handle *h, std::vector<WinPlan> &plan, const PlanOpts &o) 
     d.off_leaf = L.n_leaf_total; L.n_leaf_total += d.n_leaf; d.off_hseg = L.n_hseg; L.n_hseg += d.n_hseg;
     for (Leaf &lf : pl.leaves) {
       lf.offL = L.totLL; L.totLL += (int64_t)lf.n * lf.n + lf.n;
-      L.leaf_smem = std::max(L.leaf_smem, leaf_elim_smem(lf.n, d.n_hub)); L.leafb_smem = std::max(L.leafb_smem, leaf_back_smem(lf.n, d.n_hub));
+      L.leaf_smem = std::max(L.leaf_smem, leaf_elim_smem_bytes(lf.n, d.n_hub)); L.leafb_smem = std::max(L.leafb_smem, leaf_back_smem_bytes(lf.n, d.n_hub));
     }
     L.max_nc = std::max(L.max_nc, d.n_c); L.max_prior_m = std::max(L.max_prior_m, d.prior_m);
     if (d.schur_small) L.max_ldw_small = std::max(L.max_ldw_small, d.ldw);
@@ -1238,11 +1157,11 @@ int plan_offsets(d2ba_handle *h, std::vector<WinPlan> &plan, const PlanOpts &o) 
     pl.g12_off = L.n_g12; L.n_g12 += (int)pl.g12.size();
     if (d.sb_elim) {
       d.offLE = L.totLE; L.totLE += (int64_t)d.n_sbe * 171;
-      L.sbe_smem = std::max(L.sbe_smem, sb_elim_smem(roundup(d.n_hub + 1, 8), d.n_c, d.n_sbe)); L.sbb_smem = std::max(L.sbb_smem, sb_back_smem(d.n_hub, d.n_sbe));
+      L.sbe_smem = std::max(L.sbe_smem, sbe_smem_bytes(roundup(d.n_hub + 1, 8), d.n_c, d.n_sbe)); L.sbb_smem = std::max(L.sbb_smem, sb_back_smem_bytes(d.n_hub, d.n_sbe));
     }
     const int ndense = (d.sb_elim || d.n_leaf > 0) ? d.n_hub : d.n_c;
     if (d.chol_smem) L.max_n_smem = std::max(L.max_n_smem, ndense); else { L.any_chol_glob = true; L.max_rows_glob = std::max(L.max_rows_glob, ndense + 1); }
-    if (d.fused_solve) { L.n_fused++; L.fused_smem = std::max(L.fused_smem, solve_small_smem(d.ldw, d.n_lc, d.n_c, d.n_sbe)); }
+    if (d.fused_solve) { L.n_fused++; L.fused_smem = std::max(L.fused_smem, solve_small_smem_bytes(d.ldw, d.n_lc, d.n_c, d.n_sbe)); }
     else {
       if (d.schur_small || d.hub_small) L.ss_unfused = true;
       if (d.chol_smem) L.cs_unfused = true;
@@ -1328,7 +1247,7 @@ void stage_window(d2ba_handle *h, Staging &st, WinPlan &pl, int wi) {
       st.job.p[h->ls.job_begin[v] + pl.job_off[v] + j] = jb;
     }
   for (int sg = 0; sg < 2; sg++)
-    for (size_t t = 0; t < pl.schur[sg].size(); t++) { SchurTileH q = pl.schur[sg][t]; q.cb += pl.chunk_off; st.schur.p[(sg ? h->ls.n_schur0 : 0) + pl.schur_off[sg] + t] = q; }
+    for (size_t t = 0; t < pl.schur[sg].size(); t++) { SchurTile q = pl.schur[sg][t]; q.cb += pl.chunk_off; st.schur.p[(sg ? h->ls.n_schur0 : 0) + pl.schur_off[sg] + t] = q; }
   for (size_t t = 0; t < pl.schur_chunks.size(); t++) st.schur_chunks.p[pl.chunk_off + t] = pl.schur_chunks[t];
   for (size_t t = 0; t < pl.leaves.size(); t++) { Leaf lf = pl.leaves[t]; lf.lm_begin += pl.leaf_lm_off; st.leaf.p[d.off_leaf + t] = lf; }
   for (size_t t = 0; t < pl.leaf_lm.size(); t++) st.leaf_lm.p[pl.leaf_lm_off + t] = pl.leaf_lm[t];
@@ -1392,7 +1311,7 @@ int upload_and_bind(d2ba_handle *h, Staging &st) {
   CK(cudaStreamWaitEvent(h->stream, h->ev_copy, 0));
   CK(cudaEventRecord(h->evf1, h->stream));
   h->motion_skipped = skipped;
-  launch_build_tiles(h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, L.n_tiles, h->stream);
+  launch_build_tiles(L, h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, h->stream);
   int rc;
   CK(h->d_imu_U.alloc((size_t)L.n_imu_total * 225));
   if ((rc = alloc_zero(h, h->d_imu_c, (size_t)L.n_imu_total * kImuStride))) return rc;   // expanded from the packed upload by k_imu_unpack (launch_imu_prep)
@@ -1434,39 +1353,12 @@ void set_device_view(d2ba_handle *h, const std::vector<WinPlan> &plan) {
   P.ftol = h->cfg.function_tolerance; P.gtol = h->cfg.gradient_tolerance; P.ptol = h->cfg.parameter_tolerance;
   P.max_iter = h->cfg.max_num_iterations; P.fixed_mode = 0; P.mu0 = h->mu0;
 }
-// A cached kernel attribute: `configure(need)` runs only when `stale`; `cfg` remembers `need` across finalizes.
-template <typename V, typename F>
-int cached_attr(d2ba_handle *h, V &cfg, const V &need, bool stale, F configure, const char *msg) {
-  if (!stale) return 0;
-  if (configure(need)) return fail(h, 23, msg);
-  cfg = need;
-  return 0;
-}
-int configure_attributes(d2ba_handle *h) {
-  const LaunchSummary &L = h->ls;
-  const std::array<int, 3> kern = {L.max_rows_glob, L.max_nc, L.max_prior_m};
-  const int ldw = L.max_row_tiles * 32;
-  auto kernels = [](const std::array<int, 3> &k) { return configure_kernels(std::max(k[0], 2), k[1], k[2]); };
-  int rc;
-  if ((rc = cached_attr(h, h->cfg_kernels, kern, h->cfg_kernels != kern, kernels, "cudaFuncSetAttribute failed (shared memory request too large?)")) ||
-      (rc = cached_attr(h, h->cfg_max_ldw, ldw, h->cfg_max_ldw < ldw, configure_gather, "cudaFuncSetAttribute(k_lm_gather) failed (landmark-coupled part too wide for the row buffers)")) ||
-      (rc = cached_attr(h, h->cfg_max_ldw_small, L.max_ldw_small, L.max_ldw_small > 0 && h->cfg_max_ldw_small != L.max_ldw_small, configure_schur_small, "cudaFuncSetAttribute(k_schur_small) failed")) ||
-      (rc = cached_attr(h, h->cfg_sbe_smem, L.sbe_smem, L.sbe_smem > 0 && h->cfg_sbe_smem < L.sbe_smem, configure_sb_elim, "cudaFuncSetAttribute(k_sb_elim) failed")) ||
-      (rc = cached_attr(h, h->cfg_sbb_smem, L.sbb_smem, L.sbb_smem > 0 && h->cfg_sbb_smem < L.sbb_smem, configure_sb_back, "cudaFuncSetAttribute(k_sb_back) failed")) ||
-      (rc = cached_attr(h, h->cfg_leaf_smem, L.leaf_smem, L.leaf_smem > 0 && h->cfg_leaf_smem < L.leaf_smem, configure_leaf_elim, "cudaFuncSetAttribute(k_leaf_elim) failed")) ||
-      (rc = cached_attr(h, h->cfg_leafb_smem, L.leafb_smem, L.leafb_smem > 0 && h->cfg_leafb_smem < L.leafb_smem, configure_leaf_back, "cudaFuncSetAttribute(k_leaf_back) failed")) ||
-      (rc = cached_attr(h, h->cfg_max_n_smem, L.max_n_smem, L.max_n_smem > 0 && h->cfg_max_n_smem != L.max_n_smem, configure_chol_smem, "cudaFuncSetAttribute(k_chol_smem) failed")) ||
-      (rc = cached_attr(h, h->cfg_fused_smem, L.fused_smem, L.fused_smem > 0 && h->cfg_fused_smem < L.fused_smem, configure_solve_small, "cudaFuncSetAttribute(k_solve_small) failed")))
-    return rc;
-  return 0;
-}
 // State, IMU and prior preparation on the device, ahead of the first solve.
 int launch_prep(d2ba_handle *h) {
   const LaunchSummary &L = h->ls;
-  launch_state_prep(h->dev, L.n6_total, 0, h->stream);
-  launch_imu_prep(h->dev, h->d_imu_pk.p, h->d_imu_c.p, L.n_imu_total, h->stream);
-  if (L.any_info)
-    launch_prior_from_info(L.n_used, L.max_prior_m, h->d_pr_m.p, h->d_pr_oJ.p, h->d_pr_ov.p, h->d_pr_info.p, h->d_prior_J.p, h->d_prior_A.p, h->d_prior_e0.p, h->stream);
+  launch_state_prep(h->dev, L, h->stream);
+  launch_imu_prep(h->dev, L, h->d_imu_pk.p, h->d_imu_c.p, h->stream);
+  launch_prior_from_info(L, h->d_pr_m.p, h->d_pr_oJ.p, h->d_pr_ov.p, h->d_pr_info.p, h->d_prior_J.p, h->d_prior_A.p, h->d_prior_e0.p, h->stream);
   launch_prior_prep(h->dev, h->stream);
   CK(cudaEventRecord(h->evf2, h->stream));
   return 0;
@@ -1550,7 +1442,8 @@ int d2ba_finalize(d2ba_handle *h) {
   // ---- uploads (pinned -> device, async on the solver stream), kernel attributes, prep kernels
   if ((rc = upload_and_bind(h, st))) return rc;
   set_device_view(h, plan);
-  if ((rc = configure_attributes(h)) || (rc = launch_prep(h))) return rc;
+  if (const char *refused = configure_launches(h->ls)) return fail(h, 23, refused);
+  if ((rc = launch_prep(h))) return rc;
   lap(3);
   CK(cudaGetLastError());
   lap(4);
@@ -1597,7 +1490,7 @@ static int upload_state(d2ba_handle *h) {
   if (!xsb.empty()) CK(cudaMemcpyAsync(h->d_xsb[0].p, xsb.data(), xsb.size() * 8, cudaMemcpyHostToDevice, h->stream));
   if (!xlm.empty()) CK(cudaMemcpyAsync(h->d_xlm[0].p, xlm.data(), xlm.size() * 8, cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(h->d_xtd[0].p, xtd.data(), xtd.size() * 8, cudaMemcpyHostToDevice, h->stream));
-  launch_state_prep(h->dev, h->ls.n6_total, 0, h->stream);
+  launch_state_prep(h->dev, h->ls, h->stream);
   CK(cudaStreamSynchronize(h->stream));   // host vectors go out of scope
   h->state_dirty = false;
   return 0;
@@ -1611,14 +1504,14 @@ static void iter_mark(d2ba_handle *h, cudaEvent_t *ev, IterMark m) { if (ev) cud
 static void enqueue_linearize(d2ba_handle *h, int eval_cur, cudaEvent_t *ev = nullptr) {
   // k_misc_lin zero-fills the written runs of Hcc and stores cand_cost_misc before k_imu_lin and k_proj_lin add to them.
   // Two lanes after it: the IMU factors (one warp each) run beside the reprojection kernels and fill their tails.
-  launch_misc_lin(h->dev, eval_cur, h->ls.max_prior_m, h->stream);
+  launch_misc_lin(h->dev, h->ls, eval_cur, h->stream);
   const bool fork = !ev && h->ls.n_imu_total > 0;
   if (fork) {
     cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0);
-    launch_imu_lin(h->dev, eval_cur, h->ls.n_imu_total, h->side);
+    launch_imu_lin(h->dev, h->ls, eval_cur, h->side);
     cudaEventRecord(h->ev_join, h->side);
-  } else launch_imu_lin(h->dev, eval_cur, h->ls.n_imu_total, h->stream);
-  iter_mark(h, ev, kMkProj); for (int v = 0; v < 8; v++) launch_proj_lin(h->dev, v, eval_cur, h->ls.job_begin[v], h->ls.job_count[v], h->stream);
+  } else launch_imu_lin(h->dev, h->ls, eval_cur, h->stream);
+  iter_mark(h, ev, kMkProj); launch_proj_lin(h->dev, h->ls, eval_cur, h->stream);
   if (fork) cudaStreamWaitEvent(h->stream, h->ev_join, 0);
 }
 
@@ -1626,31 +1519,31 @@ static void enqueue_linearize(d2ba_handle *h, int eval_cur, cudaEvent_t *ev = nu
 static void enqueue_schur(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
   // (the leaf kernel forms its own part of the reduced system from Hcc and its landmarks' rows: the stage-0 tiles are
   //  only launched for the debug view of S)
-  if (h->ls.n_leaf_total > 0) launch_leaf_elim(h->dev, h->ls.leaf_smem, h->stream);
-  iter_mark(h, ev, kMkLeafElimEnd); if (h->ls.ss_unfused) launch_schur_small(h->dev, h->ls.max_ldw_small, 0, h->stream);
-  if (h->ls.n_schur > h->ls.n_schur0) launch_schur(h->dev, h->d_schur.p + h->ls.n_schur0, h->ls.n_schur - h->ls.n_schur0, h->stream);
+  launch_leaf_elim(h->dev, h->ls, h->stream);
+  iter_mark(h, ev, kMkLeafElimEnd); launch_schur_small(h->dev, h->ls, 0, h->stream);
+  launch_schur(h->dev, h->d_schur.p + h->ls.n_schur0, h->ls.n_schur - h->ls.n_schur0, h->stream);
 }
 // dense Cholesky of the hub, then the eliminated parts' back substitutions
 static void enqueue_solve_reduced(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
-  if (h->ls.cs_unfused) launch_chol_smem(h->dev, h->ls.max_n_smem, h->stream);
-  if (h->ls.any_chol_glob) launch_chol(h->dev, h->ls.max_rows_glob, h->stream);
-  iter_mark(h, ev, kMkSbBack); if (h->ls.sbb_unfused) launch_sb_back(h->dev, h->ls.sbb_smem, h->stream);
-  iter_mark(h, ev, kMkLeafBack); if (h->ls.n_leaf_total > 0) launch_leaf_back(h->dev, h->ls.leafb_smem, h->stream);
+  launch_chol_smem(h->dev, h->ls, h->stream);
+  launch_chol(h->dev, h->ls, h->stream);
+  iter_mark(h, ev, kMkSbBack); launch_sb_back(h->dev, h->ls, h->stream);
+  iter_mark(h, ev, kMkLeafBack); launch_leaf_back(h->dev, h->ls, h->stream);
 }
 // the step: k_solve_small does the whole reduced-system solve and the step of its windows, k_step the others'
 static void enqueue_step(d2ba_handle *h) {
-  if (h->ls.n_fused > 0) launch_solve_small(h->dev, h->ls.fused_smem, h->stream);
-  launch_step(h->dev, h->ls.max_nc, h->stream);
+  launch_solve_small(h->dev, h->ls, h->stream);
+  launch_step(h->dev, h->ls, h->stream);
 }
 
 static void enqueue_iteration(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
   // the speed-bias elimination (Hcc -> its Y rows behind the landmark rows of Wt) does not touch what the landmark gather
   // reads or writes: second lane
   const bool fork = !ev && h->ls.sbe_smem > 0;
-  iter_mark(h, ev, kMkGather); if (fork) { cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0); launch_sb_elim(h->dev, h->ls.sbe_smem, h->side); cudaEventRecord(h->ev_join, h->side); }
-  launch_lm_gather(h->dev, h->d_lm_win.p, h->ls.nl_total, h->ls.max_row_tiles * 32, h->ls.any_compact, h->ls.any_wide, h->ls.n_g12, h->stream);
+  iter_mark(h, ev, kMkGather); if (fork) { cudaEventRecord(h->ev_fork, h->stream); cudaStreamWaitEvent(h->side, h->ev_fork, 0); launch_sb_elim(h->dev, h->ls, h->side); cudaEventRecord(h->ev_join, h->side); }
+  launch_lm_gather(h->dev, h->ls, h->d_lm_win.p, h->stream);
   iter_mark(h, ev, kMkSbElim); if (fork) cudaStreamWaitEvent(h->stream, h->ev_join, 0);
-  else if (h->ls.sbe_smem > 0) launch_sb_elim(h->dev, h->ls.sbe_smem, h->stream);   // Y rows into Wt: the Schur kernels subtract them too
+  else launch_sb_elim(h->dev, h->ls, h->stream);   // Y rows into Wt: the Schur kernels subtract them too
   iter_mark(h, ev, kMkSchur); enqueue_schur(h, ev);
   iter_mark(h, ev, kMkChol); enqueue_solve_reduced(h, ev);
   iter_mark(h, ev, kMkStep); enqueue_step(h);
@@ -1659,15 +1552,34 @@ static void enqueue_iteration(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
   iter_mark(h, ev, kMkEnd);
 }
 
+// One fixed iteration's linearisation at the current state, then the full reduced system in d_S, un-factored: the
+// eliminated speed-bias and leaf rows zeroed (the landmark-only Schur complement), every Schur tile of both stages and
+// k_schur_small over every window it serves (d2ba_debug_linearize, d2ba_marginalize).
+static void enqueue_full_schur(d2ba_handle *h) {
+  const LaunchSummary &L = h->ls;
+  h->dev.prm.fixed_mode = 1; h->dev.prm.max_iter = 1;
+  launch_tr_reset(h->dev, 1, h->stream);
+  // ADMM terms as at the start of a solve (z = x, tilde = 0, references = state), not whatever the buffers held
+  launch_cons_init(h->dev, L, h->stream);
+  launch_cons_refs(h->dev, L, h->d_sb_win.p, h->d_lm_win.p, h->stream);
+  enqueue_linearize(h, 1);
+  launch_control(h->dev, 1, h->stream);
+  launch_lm_gather(h->dev, L, h->d_lm_win.p, h->stream);
+  launch_zero_sb_rows(h->dev, L, h->stream);
+  launch_zero_leaf_rows(h->dev, L, h->stream);
+  launch_schur_small(h->dev, L, 1, h->stream);
+  launch_schur(h->dev, h->d_schur.p, L.n_schur, h->stream);
+}
+
 static int consensus_exchange(d2ba_handle *h) {
   CK(cudaMemsetAsync(h->d_cons.p, 0, (size_t)std::max(h->ls.n_slots, 1) * 14 * 8, h->stream));
-  launch_cons_pack(h->dev, h->ls.n6_total, h->d_blk_win.p, h->stream);
+  launch_cons_pack(h->dev, h->ls, h->d_blk_win.p, h->stream);
   if (h->comm) {
     int r = g_nccl.AllReduce(h->d_cons.p, h->d_cons.p, (size_t)h->ls.n_slots * 14, /*ncclFloat64*/ 8, /*ncclSum*/ 0, h->comm, h->stream);
     if (r) return fail(h, 40, std::string("ncclAllReduce: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "error"));
   }
-  launch_cons_apply(h->dev, h->ls.n6_total, h->d_blk_win.p, h->stream);
-  launch_cons_refs(h->dev, h->ls.nsb_total, h->ls.nl_total, h->d_sb_win.p, h->d_lm_win.p, h->stream);
+  launch_cons_apply(h->dev, h->ls, h->d_blk_win.p, h->stream);
+  launch_cons_refs(h->dev, h->ls, h->d_sb_win.p, h->d_lm_win.p, h->stream);
   return 0;
 }
 
@@ -1687,7 +1599,7 @@ static int run_solve(d2ba_handle *h, int fixed_iters, d2ba_report *reports) {
   auto lap = [&](int k) { auto t = std::chrono::steady_clock::now(); h->solve_ms[k] = std::chrono::duration<double, std::milli>(t - tq).count(); tq = t; };
   CK(cudaEventRecord(h->ev0, h->stream));
   launch_tr_reset(h->dev, 1, h->stream);
-  if (h->ls.any_admm) launch_cons_init(h->dev, h->ls.n6_total, h->stream);
+  launch_cons_init(h->dev, h->ls, h->stream);
   // ceres max_solver_time_in_seconds: an iteration is only started while the budget of this (sub-)step lasts.  The
   // iterations are enqueued asynchronously, so the host trails the device by at most two of them: before enqueuing
   // iteration k it waits for iteration k-2 and compares the wall clock.
@@ -1844,7 +1756,7 @@ static int ensure_motion(d2ba_handle *h) {
   }
   CK(cudaStreamSynchronize(h->copy_stream));
   CK(cudaMemcpy(h->d_raw_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
-  launch_build_tiles(h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, h->ls.n_tiles, h->stream);
+  launch_build_tiles(h->ls, h->d_raw_off.p, h->d_tile_src.p, h->d_tile_win.p, h->d_xtd[0].p, h->d_obs.p, h->stream);
   h->motion_skipped = false;
   return 0;
 }
@@ -1855,24 +1767,11 @@ int d2ba_debug_linearize(d2ba_handle *h) {
   if (!h->finalized) { int rc = d2ba_finalize(h); if (rc) return rc; }
   { int rc = ensure_motion(h); if (rc) return rc; }
   if (h->state_dirty) { int rc = upload_state(h); if (rc) return rc; }
-  h->dev.prm.fixed_mode = 1; h->dev.prm.max_iter = 1;
-  launch_tr_reset(h->dev, 1, h->stream);
-  if (h->ls.any_admm) {   // ADMM terms as at the start of a solve (z = x, tilde = 0, references = state), not whatever the buffers held
-    launch_cons_init(h->dev, h->ls.n6_total, h->stream);
-    launch_cons_refs(h->dev, h->ls.nsb_total, h->ls.nl_total, h->d_sb_win.p, h->d_lm_win.p, h->stream);
-  }
-  enqueue_linearize(h, 1);
-  launch_control(h->dev, 1, h->stream);
-  launch_lm_gather(h->dev, h->d_lm_win.p, h->ls.nl_total, h->ls.max_row_tiles * 32, h->ls.any_compact, h->ls.any_wide, h->ls.n_g12, h->stream);
-  // debug view: the landmark-only Schur complement (eliminated speed-bias rows zeroed), kept un-factored in d_dbg
-  if (h->ls.sbe_smem > 0) launch_zero_sb_rows(h->dev, h->stream);
-  if (h->ls.n_leaf_total > 0) launch_zero_leaf_rows(h->dev, h->stream);
-  if (h->ls.max_ldw_small > 0) launch_schur_small(h->dev, h->ls.max_ldw_small, 1, h->stream);   // k_solve_small's windows too
-  launch_schur(h->dev, h->d_schur.p, h->ls.n_schur, h->stream);   // both stages back to back: no eliminated rows in this view
+  enqueue_full_schur(h);   // debug view: the landmark-only Schur complement, kept un-factored in d_dbg
   CK(h->d_dbg.alloc((size_t)h->ls.totH));
   CK(cudaMemcpyAsync(h->d_dbg.p, h->d_S.p, (size_t)h->ls.totH * 8, cudaMemcpyDeviceToDevice, h->stream));
   if (h->ls.sbe_smem > 0 || h->ls.n_leaf_total > 0) {   // now the system the solver factors: Y rows in place, Schur again
-    if (h->ls.sbe_smem > 0) launch_sb_elim(h->dev, h->ls.sbe_smem, h->stream);
+    launch_sb_elim(h->dev, h->ls, h->stream);
     enqueue_schur(h);
   }
   enqueue_solve_reduced(h);
@@ -1971,7 +1870,7 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     case D2BA_DBG_PROJ_RESJAC: {
       DBuf<double> tmp;
       if (tmp.alloc((size_t)h->ls.n_tiles * kTile * 81) != cudaSuccess) return fail(h, 5, "debug alloc");
-      launch_proj_debug(h->dev, tmp.p, h->ls.n_tiles, h->d_tile_win.p, h->stream);
+      launch_proj_debug(h->dev, h->ls, tmp.p, h->d_tile_win.p, h->stream);
       cudaStreamSynchronize(h->stream);
       std::vector<double> all((size_t)d.n_tile * kTile * 81);
       if (!all.empty()) cudaMemcpy(all.data(), tmp.p + (size_t)d.off_tile * kTile * 81, all.size() * 8, cudaMemcpyDeviceToHost);
@@ -1995,7 +1894,7 @@ int d2ba_debug_get(d2ba_handle *h, int32_t window, int32_t item, void *out, int6
     case D2BA_DBG_CONS_RESJAC: {
       DBuf<double> tmp;
       if (tmp.alloc((size_t)std::max(h->ls.n6_total, 1) * 62) != cudaSuccess) return fail(h, 5, "debug alloc");
-      launch_cons_debug(h->dev, tmp.p, h->d_blk_win.p, h->ls.n6_total, h->stream);
+      launch_cons_debug(h->dev, h->ls, tmp.p, h->d_blk_win.p, h->stream);
       cudaStreamSynchronize(h->stream);
       put_d(fetch(tmp.p + (size_t)d.off6 * 62, (size_t)d.n6 * 62));
       tmp.release(); break;
@@ -2127,14 +2026,8 @@ int d2ba_marginalize(d2ba_handle *h, int32_t window, int32_t n_remove, const int
   }
   if ((rc = d2ba_finalize(t))) return fail(h, rc, std::string("marginalize/finalize: ") + t->err);
   if (t->h_win[0].n_c != col) return fail(h, 64, "marginalize: internal column count mismatch");
-  // linearise and eliminate the landmarks (mu = 0)
-  t->dev.prm.fixed_mode = 1; t->dev.prm.max_iter = 1;
-  launch_tr_reset(t->dev, 1, t->stream);
-  enqueue_linearize(t, 1);
-  launch_control(t->dev, 1, t->stream);
-  launch_lm_gather(t->dev, t->d_lm_win.p, t->ls.nl_total, t->ls.max_row_tiles * 32, t->ls.any_compact, t->ls.any_wide, t->ls.n_g12, t->stream);
-  if (t->ls.max_ldw_small > 0) launch_schur_small(t->dev, t->ls.max_ldw_small, 1, t->stream);
-  launch_schur(t->dev, t->d_schur.p, t->ls.n_schur, t->stream);
+  // linearise and eliminate the landmarks (mu = 0); force_full_S: no speed-bias or leaf rows, and no consensus
+  enqueue_full_schur(t);
   // eliminate the removed camera columns
   DBuf<int> d_keep, d_rem, d_flag; DBuf<double> d_A, d_b;
   cudaError_t ce;
@@ -2158,12 +2051,7 @@ int d2ba_marginalize(d2ba_handle *h, int32_t window, int32_t n_remove, const int
   return 0;
 }
 
-// Per-kernel device time of the iteration sequence (CUDA events on the solver stream, no graph):
-// ms_out[0..6] = lm_gather, schur, chol, step, misc_lin, proj_lin, control, summed over `iters` iterations;
-// ms_out[7] = number of iterations timed; ms_out[8], [9] = the speed-bias elimination / back-substitution share of the
-// chol bucket.  Used by bench.py for the roofline of the dominant kernel.  k_solve_small (the whole reduced-system
-// solve and step of the windows with fused_solve) is timed in the step bucket; the schur, chol and back-substitution
-// buckets then hold only the other windows' kernels.
+// CTAs of k_solve_small per SM at the handle's shared-memory size (0 when no window takes the one-kernel solve).
 int d2ba_debug_solve_occupancy(d2ba_handle *h, int32_t *ctas_per_sm) {
   if (!h || !ctas_per_sm) return 1;
   cudaSetDevice(h->cfg.device);
@@ -2176,6 +2064,12 @@ int d2ba_debug_solve_occupancy(d2ba_handle *h, int32_t *ctas_per_sm) {
   return 0;
 }
 
+// Per-kernel device time of the iteration sequence (CUDA events on the solver stream, no graph):
+// ms_out[0..6] = lm_gather, schur, chol, step, misc_lin, proj_lin, control, summed over `iters` iterations;
+// ms_out[7] = number of iterations timed; ms_out[8], [9] = the speed-bias elimination / back-substitution share of the
+// chol bucket.  Used by bench.py for the roofline of the dominant kernel.  k_solve_small (the whole reduced-system
+// solve and step of the windows with fused_solve) is timed in the step bucket; the schur, chol and back-substitution
+// buckets then hold only the other windows' kernels.
 int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
   if (!h) return 1;
   cudaSetDevice(h->cfg.device);
@@ -2184,7 +2078,8 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
   h->dev.prm.fixed_mode = 1; h->dev.prm.max_iter = iters;
   release_graph(h);
   launch_tr_reset(h->dev, 1, h->stream);
-  if (h->ls.any_admm) { launch_cons_init(h->dev, h->ls.n6_total, h->stream); int rc = consensus_exchange(h); if (rc) return rc; }
+  launch_cons_init(h->dev, h->ls, h->stream);
+  if (h->ls.any_admm) { int rc = consensus_exchange(h); if (rc) return rc; }
   enqueue_linearize(h, 1);
   launch_control(h->dev, 1, h->stream);
   cudaEvent_t ev[kNumMarks];

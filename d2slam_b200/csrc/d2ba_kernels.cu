@@ -23,6 +23,7 @@
 #include "../../include/d2ba.h"
 #include "d2ba_math.cuh"
 #include "d2ba_proj.cuh"
+#include "d2ba_launch.cuh"
 #include "d2ba_types.cuh"
 
 namespace d2ba {
@@ -394,6 +395,7 @@ __global__ void __launch_bounds__(kMiscThreads, 5) k_misc_lin(Dev d, int eval_cu
 constexpr int kImuWarps = 4;
 constexpr int kImuF = 15 * 30 + 15;   // doubles per factor for (J, r)
 constexpr int kImuWarpDoubles = 2 * kImuF + 225 + 1;   // raw, U [J r] (the constants before it), sqrt-information
+constexpr size_t kImuSmem = (size_t)kImuWarps * kImuWarpDoubles * 8;   // k_imu_lin / k_imu_debug: one buffer per warp
 
 // One warp: factor f at state buffer buf -> fin = U [J | r] (15 x 30 whitened Jacobian, then the 15 whitened residuals).
 // raw / fin: kImuF doubles each, Us: 225.  The debug view (k_imu_debug) runs this same path.
@@ -987,9 +989,12 @@ __global__ void k_cons_debug(Dev d, double *out /*[n6_total][62]*/, const int *b
   for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) { o[26 + i * 6 + j] = wT * Rz[j * 3 + i]; o[26 + (3 + i) * 6 + 3 + j] = wq * L3[i * 3 + j]; }
 }
 void launch_imu_debug(const Dev &d, double *out, const int *imu_win, int n, cudaStream_t s) {
-  if (n > 0) k_imu_debug<<<(n + kImuWarps - 1) / kImuWarps, kImuWarps * 32, (size_t)kImuWarps * kImuWarpDoubles * 8, s>>>(d, out, imu_win, n);
+  if (n > 0) k_imu_debug<<<(n + kImuWarps - 1) / kImuWarps, kImuWarps * 32, kImuSmem, s>>>(d, out, imu_win, n);
 }
-void launch_cons_debug(const Dev &d, double *out, const int *blk_win, int n, cudaStream_t s) { if (n > 0) k_cons_debug<<<(n + 63) / 64, 64, 0, s>>>(d, out, blk_win, n); }
+void launch_cons_debug(const Dev &d, const LaunchSummary &L, double *out, const int *blk_win, cudaStream_t s) {
+  const int n = L.n6_total;
+  if (n > 0) k_cons_debug<<<(n + 63) / 64, 64, 0, s>>>(d, out, blk_win, n);
+}
 
 // ------------------------------------------------------------------------------------------------
 // Per-landmark reduction, wide records (warp per landmark; compact records: k_lm_gather16 below).  The landmark's
@@ -1666,13 +1671,6 @@ __global__ void __launch_bounds__(kCholThreads) k_chol(Dev d, int max_rows) {
 //       diagonal block while the other warps update the rest.
 // Then blocked back substitution, all from shared memory.  (H100's fp64 tensor-core peak is twice its DFMA peak, and
 // one DMMA m8n8k4 (256 FMAs per warp) does the work of 8 DFMA per lane, so the tensor-core form wins on issue slots.)
-constexpr int kCsThreads = 512;
-constexpr int kCsNB = 8;
-__host__ __device__ inline int chol_smem_ld(int n) { return (n + 1) & ~1; }
-__host__ __device__ inline size_t chol_smem_bytes(int n) {
-  size_t pr = (size_t)kCsNB * ((n + 2) & ~1), need = (size_t)n + 1 + 16 * 32;
-  return ((size_t)(n + 1) * chol_smem_ld(n) + (size_t)((n + 1) & ~1) + (pr > need ? pr : need)) * 8 + 32;   // invd padded to even: P stays 16 B aligned
-}
 // 1/d to full double precision: fp32 MUFU seed + two Newton steps; d must be a normal positive number in float range
 D2BA_DEV double fast_rcp(double d) {
   double r;
@@ -1988,11 +1986,6 @@ D2BA_DEV bool chol_block9(double *Dk, double *invd, int lane) {
 }
 
 constexpr int kSeThreads = 128;    // warp 0: D / E chain, warps 1..3: Y rows
-constexpr int kSeMaxBlocks = 32;   // speed-bias blocks per window (mbarrier table)
-constexpr int kSeSlotRows = 9;
-__host__ __device__ inline size_t sbe_smem_bytes(int ldw, int n_c, int nb) {
-  return ((size_t)3 * kSeSlotRows * ldw + (size_t)nb * 2 * 81 + (size_t)nb * 9 + (size_t)n_c + (size_t)9 * nb + 16) * 8;
-}
 
 __global__ void __launch_bounds__(kSeThreads, 4) k_sb_elim(Dev d) {
   const int wi = blockIdx.x;
@@ -2153,7 +2146,6 @@ __global__ void __launch_bounds__(kSeThreads, 4) k_sb_elim(Dev d) {
 // first.  One CTA per window: all warps form v = Y x_p (coalesced, many loads in flight) and stage the small blocks,
 // warp 0 then runs the short recursion out of shared memory.
 constexpr int kSbBackThreads = 256;
-__host__ __device__ inline size_t sb_back_smem_bytes(int nlc, int nb) { return (size_t)(((nlc + 31) & ~31) + 9 * nb + 171 * nb) * 8; }
 // Body shared by k_sb_back and k_solve_small (gn_c holds the pose part of the step).
 D2BA_DEV void sb_back_body(const Dev &d, int wi, double *sm) {
   const WinDesc &w = d.win[wi];
@@ -2237,13 +2229,6 @@ __global__ void __launch_bounds__(kSbBackThreads) k_sb_back(Dev d) {
 #define D2BA_LEAF_THREADS 256
 #endif
 constexpr int kLeafThreads = D2BA_LEAF_THREADS;
-constexpr int kLeafMaxCols = 96;
-constexpr int kLeafLmChunk = 16;   // landmarks whose coupling rows are staged at a time (a multiple of the MMA k = 4)
-__host__ __device__ inline int leaf_lda(int n) { return n | 1; }   // odd: the one-row-per-thread TRSM walks the rows without bank conflicts (all accesses are scalar)
-__host__ __device__ inline size_t leaf_elim_smem_bytes(int n, int nh) {
-  const int n1 = n + nh + 1;
-  return ((size_t)n1 * leaf_lda(n) + (size_t)((n + 1) & ~1) + (size_t)kCsNB * ((n1 + 1) & ~1) + 64 + (size_t)kLeafLmChunk * n1 + 8) * 8;
-}
 // C(8x8 at rows gi0.., cols gj0..) -= P^T P over the 8 panel columns; rows of the leaf block (gi < n) keep the lower
 // triangle only, the extra rows (gi >= n) all n columns
 D2BA_DEV void leaf_tile8(double *A, int ld, const double *P, int ldp, int gi0, int gj0, int ri, int rj, int pmax, int n1, int n, int lane) {
@@ -2408,7 +2393,6 @@ __global__ void __launch_bounds__(kLeafThreads) k_leaf_elim(Dev d) {
 
 // Leaf part of the Gauss-Newton step: L^T x_b = z_b - Y_b x_hub, one CTA per (window, leaf)
 constexpr int kLeafBackThreads = 128;
-__host__ __device__ inline size_t leaf_back_smem_bytes(int n, int nh) { return ((size_t)n * n + 2 * (size_t)n + (size_t)nh + 8) * 8; }
 __global__ void __launch_bounds__(kLeafBackThreads) k_leaf_back(Dev d) {
   const Leaf lf = d.leaf[blockIdx.x];
   const WinDesc &w = d.win[lf.win];
@@ -2655,14 +2639,6 @@ __global__ void __launch_bounds__(kStepThreads, LEAF ? 4 : 3) k_step(Dev d, int 
 //   (4) landmark back substitution, dogleg, model change, retraction into the candidate buffers.
 // A rejected step (reuse), a finished window and a failed speed-bias elimination skip (1)-(3), as the separate kernels do.
 // 4 warps and <= 56 KB of shared memory: 4 CTAs per SM, so the 528 windows of 132 SMs run in one wave.
-constexpr int kSolveThreads = 128;
-constexpr int kSolveMaxB = 12;   // 9*10/2 = 45 lower blocks (ldw <= 72) over 4 warps
-__host__ __device__ inline size_t solve_small_smem_bytes(int ldw, int n_lc, int n_c, int nb) {
-  size_t b = (size_t)2 * 32 * (ldw + 4) * 8;
-  b = std::max(b, chol_smem_bytes(n_lc));
-  b = std::max(b, sb_back_smem_bytes(n_lc, nb));
-  return std::max(b, (size_t)(40 + 3 * n_c) * 8);
-}
 __global__ void __launch_bounds__(kSolveThreads, 4) k_solve_small(Dev d) {
   const int wi = blockIdx.x;
   const WinDesc &w = d.win[wi];
@@ -2905,8 +2881,9 @@ __global__ void __launch_bounds__(128) k_build_tiles(const long long *raw_off, c
 #pragma unroll
   for (int k = 0; k < kObsFields; k++) ob[k * kTile + lane] = f[k];
 }
-void launch_build_tiles(const long long *raw_off, const int *tile_src, const int *tile_win, const double *xtd, double *obs, int n_tiles, cudaStream_t s) {
-  if (n_tiles > 0) k_build_tiles<<<(n_tiles + 3) / 4, 128, 0, s>>>(raw_off, tile_src, tile_win, xtd, obs, n_tiles);
+void launch_build_tiles(const LaunchSummary &L, const long long *raw_off, const int *tile_src, const int *tile_win, const double *xtd,
+                        double *obs, cudaStream_t s) {
+  if (L.n_tiles > 0) k_build_tiles<<<(L.n_tiles + 3) / 4, 128, 0, s>>>(raw_off, tile_src, tile_win, xtd, obs, L.n_tiles);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2984,9 +2961,6 @@ int launch_marg_reduce(const double *S, int ld, int n, const int *keep_idx, int 
 
 // ------------------------------------------------------------------------------------------------
 // host-callable launchers (keeps <<<>>> syntax inside this translation unit)
-void launch_state_prep(const Dev &d, int n6_total, int buf, cudaStream_t s) {
-  if (n6_total > 0) k_state_prep<<<(n6_total + 127) / 128, 128, 0, s>>>(d, n6_total, buf);
-}
 // packed upload record (kImuPack) -> the full constant record imu_stage / k_imu_prep index (kImuStride); entries the factor
 // never reads stay at the zero of the finalize-time memset
 __global__ void k_imu_unpack(const double *pk, double *full, int n_imu) {
@@ -3004,117 +2978,6 @@ __global__ void k_imu_unpack(const double *pk, double *full, int n_imu) {
   }
   full[(size_t)f * kImuStride + dst] = pk[(size_t)f * kImuPack + t];
 }
-void launch_imu_prep(const Dev &d, const double *packed, double *full, int n_imu, cudaStream_t s) {
-  if (n_imu > 0) k_imu_unpack<<<n_imu, 192, 0, s>>>(packed, full, n_imu);
-  if (n_imu > 0) k_imu_prep<<<(n_imu + 31) / 32, 32, 0, s>>>(d, n_imu);
-}
-void launch_prior_prep(const Dev &d, cudaStream_t s) { k_prior_prep<<<d.n_win, 256, 0, s>>>(d); }
-
-size_t misc_smem_bytes(int max_prior_m) { return (size_t)(40 + 3 * max_prior_m + 8) * 8; }
-void launch_imu_lin(const Dev &d, int eval_cur, int n_imu_total, cudaStream_t s) {
-  if (n_imu_total > 0) k_imu_lin<<<(n_imu_total + kImuWarps - 1) / kImuWarps, kImuWarps * 32, (size_t)kImuWarps * kImuWarpDoubles * 8, s>>>(d, eval_cur, n_imu_total);
-}
-void launch_misc_lin(const Dev &d, int eval_cur, int max_prior_m, cudaStream_t s) {
-  k_misc_lin<<<d.n_win, kMiscThreads, misc_smem_bytes(max_prior_m), s>>>(d, eval_cur);
-}
-
-template <int NCT, int KR>
-static size_t proj_smem() { return (size_t)4 * (GC_SIZE + NCT * 8 * (kTile * KR + 4)) * 8; }
-
-int configure_kernels(int max_rows, int max_nc, int max_prior_m) {
-  cudaError_t e;
-  e = raise_smem_limit(k_proj_lin<2, 2>, (size_t)(proj_smem<2, 2>())); if (e) return e;
-  e = raise_smem_limit(k_proj_lin<4, 2>, (size_t)(proj_smem<4, 2>())); if (e) return e;
-  e = raise_smem_limit(k_proj_lin<2, 4>, (size_t)(proj_smem<2, 4>())); if (e) return e;
-  e = raise_smem_limit(k_proj_lin<4, 4>, (size_t)(proj_smem<4, 4>())); if (e) return e;
-  e = raise_smem_limit(k_proj_lin_pp<true, false>, proj_pp_smem()); if (e) return e;
-  e = raise_smem_limit(k_proj_lin_pp<false, false>, proj_pp_smem()); if (e) return e;
-  e = raise_smem_limit(k_proj_lin_pp<true, true>, proj_pp_smem()); if (e) return e;
-  e = raise_smem_limit(k_proj_lin_pp<false, true>, proj_pp_smem()); if (e) return e;
-  // 4 x 51 KB per SM needs the large shared-memory carveout
-  cudaFuncSetAttribute(k_proj_lin_pp<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(k_proj_lin_pp<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(k_proj_lin_pp<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(k_proj_lin_pp<false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-
-  size_t chol = (size_t)(kNB * (max_rows + 4) + 2 * max_rows + 16 + 16 * 32 + kNB * (kNB + 1)) * 8;
-  e = raise_smem_limit(k_chol, (size_t)(chol)); if (e) return e;
-  size_t st = (size_t)(40 + 3 * max_nc) * 8;
-  e = raise_smem_limit(k_step<false>, (size_t)(st)); if (e) return e;
-  e = raise_smem_limit(k_step<true>, (size_t)(st)); if (e) return e;
-  e = raise_smem_limit(k_misc_lin, (size_t)(misc_smem_bytes(max_prior_m))); if (e) return e;
-  e = raise_smem_limit(k_imu_lin, (size_t)kImuWarps * kImuWarpDoubles * 8); if (e) return e;
-  return 0;
-}
-// the row buffers of the per-landmark gather grow with the landmark-coupled width (multi-agent windows: 6 x 88 poses)
-int configure_gather(int max_ldw) {
-  cudaError_t e;
-  e = raise_smem_limit(k_lm_gather, (size_t)kGatherWarps * max_ldw * 8); if (e) return e;
-  e = raise_smem_limit(k_lm_gather16, (size_t)kG16Lm * max_ldw * 8); if (e) return e;
-  return 0;
-}
-
-void launch_proj_lin(const Dev &d, int variant, int eval_cur, int job_begin, int job_count, cudaStream_t s) {
-  if (job_count <= 0) return;
-  int grid = (job_count + 3) / 4;
-  switch (variant) {
-    case 0: k_proj_lin<2, 2><<<grid, 128, proj_smem<2, 2>(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 1: k_proj_lin<4, 2><<<grid, 128, proj_smem<4, 2>(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 2: k_proj_lin<2, 4><<<grid, 128, proj_smem<2, 4>(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 3: k_proj_lin<4, 4><<<grid, 128, proj_smem<4, 4>(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 4: k_proj_lin_pp<true, false><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 5: k_proj_lin_pp<false, false><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 6: k_proj_lin_pp<true, true><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
-    case 7: k_proj_lin_pp<false, true><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
-  }
-}
-void launch_proj_debug(const Dev &d, double *out, int n_tiles, const int *tile_win, cudaStream_t s) {
-  if (n_tiles > 0) k_proj_debug<<<n_tiles, 32, 0, s>>>(d, out, n_tiles, tile_win);
-}
-void launch_lm_gather(const Dev &d, const int *lm_win, int n_lm_total, int max_ldw, int any_compact, int any_wide, int n_chunk12, cudaStream_t s) {
-  if (n_lm_total <= 0) return;
-  if (any_wide)
-    k_lm_gather<<<(n_lm_total + kGatherWarps - 1) / kGatherWarps, kGatherWarps * 32, (size_t)kGatherWarps * max_ldw * 8, s>>>(d, lm_win, n_lm_total, max_ldw);
-  if (any_compact)
-    k_lm_gather16<<<(n_lm_total + kG16Lm - 1) / kG16Lm, kG16Lm * 16, (size_t)kG16Lm * max_ldw * 8, s>>>(d, lm_win, n_lm_total, max_ldw);
-  if (n_chunk12 > 0) k_lm_gather12<<<(n_chunk12 + kG12Warps - 1) / kG12Warps, kG12Warps * 32, 0, s>>>(d, n_chunk12);
-}
-void launch_schur_small(const Dev &d, int max_ldw, int with_fused, cudaStream_t s) {
-  k_schur_small<<<d.n_win, kSsThreads, (size_t)(2 * 32 * (max_ldw + 4) + 40) * 8, s>>>(d, with_fused);
-}
-// the 8x8 blocks of the lower triangle fit the accumulators of k_solve_small's warps
-bool solve_small_fits(int ldw) { const int nb8 = ldw / 8; return nb8 * (nb8 + 1) / 2 <= kSolveMaxB * (kSolveThreads / 32); }
-size_t solve_small_smem(int ldw, int n_lc, int n_c, int nb) { return solve_small_smem_bytes(ldw, n_lc, n_c, nb); }
-int configure_solve_small(size_t smem) { return (int)raise_smem_limit(k_solve_small, smem); }
-void launch_solve_small(const Dev &d, size_t smem, cudaStream_t s) { k_solve_small<<<d.n_win, kSolveThreads, smem, s>>>(d); }
-int solve_small_occupancy(size_t smem) {
-  int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_solve_small, kSolveThreads, smem) != cudaSuccess) return -1;
-  return n;
-}
-int configure_schur_small(int max_ldw) {
-  return (int)raise_smem_limit(k_schur_small, (size_t)((2 * 32 * (max_ldw + 4) + 40) * 8));
-}
-void launch_schur(const Dev &d, const void *tiles, int n_tiles, cudaStream_t s) {
-  if (n_tiles > 0) k_schur<<<n_tiles, 128, 0, s>>>(d, reinterpret_cast<const SchurTile *>(tiles));
-}
-size_t leaf_elim_smem(int n, int n_hub) { return leaf_elim_smem_bytes(n, n_hub); }
-size_t leaf_back_smem(int n, int n_hub) { return leaf_back_smem_bytes(n, n_hub); }
-int leaf_max_cols() { return kLeafMaxCols; }
-int configure_leaf_elim(size_t smem) { return (int)raise_smem_limit(k_leaf_elim, smem); }
-int configure_leaf_back(size_t smem) { return (int)raise_smem_limit(k_leaf_back, smem); }
-void launch_leaf_elim(const Dev &d, size_t smem, cudaStream_t s) { if (d.n_leaf_total > 0) k_leaf_elim<<<d.n_leaf_total, kLeafThreads, smem, s>>>(d); }
-void launch_leaf_back(const Dev &d, size_t smem, cudaStream_t s) { if (d.n_leaf_total > 0) k_leaf_back<<<d.n_leaf_total, kLeafBackThreads, smem, s>>>(d); }
-void launch_zero_leaf_rows(const Dev &d, cudaStream_t s) { k_zero_leaf_rows<<<d.n_win, 256, 0, s>>>(d); }
-size_t chol_smem_need(int n) { return chol_smem_bytes(n); }
-int configure_chol_smem(int max_n) {
-  return (int)raise_smem_limit(k_chol_smem, (size_t)(chol_smem_bytes(max_n)));
-}
-// small systems (after the speed-bias elimination): 4 warps per window so that several windows share an SM
-int chol_smem_threads(int max_n) { return max_n <= 96 ? 128 : kCsThreads; }
-void launch_chol_smem(const Dev &d, int max_n, cudaStream_t s) {
-  k_chol_smem<<<d.n_win, chol_smem_threads(max_n), chol_smem_bytes(max_n), s>>>(d);
-}
 __global__ void k_zero_sb_rows(Dev d) {
   const WinDesc &w = d.win[blockIdx.x];
   if (!w.sb_elim) return;
@@ -3122,32 +2985,142 @@ __global__ void k_zero_sb_rows(Dev d) {
   const size_t tot = (size_t)(w.wt_rows - w.nl) * w.ldw;
   for (size_t e = threadIdx.x; e < tot; e += blockDim.x) Yg[e] = 0.0;
 }
-void launch_zero_sb_rows(const Dev &d, cudaStream_t s) { k_zero_sb_rows<<<d.n_win, 256, 0, s>>>(d); }
-size_t sb_elim_smem(int ldw, int n_c, int nb) { return sbe_smem_bytes(ldw, n_c, nb); }
-int configure_sb_elim(size_t smem) { return (int)raise_smem_limit(k_sb_elim, (size_t)(smem)); }
-void launch_sb_elim(const Dev &d, size_t smem, cudaStream_t s) { k_sb_elim<<<d.n_win, kSeThreads, smem, s>>>(d); }
-size_t sb_back_smem(int nlc, int nb) { return sb_back_smem_bytes(nlc, nb); }
-int sb_max_blocks() { return kSeMaxBlocks; }
-void launch_sb_back(const Dev &d, size_t smem, cudaStream_t s) { k_sb_back<<<d.n_win, kSbBackThreads, smem, s>>>(d); }
-int configure_sb_back(size_t smem) { return (int)raise_smem_limit(k_sb_back, smem); }
-void launch_chol(const Dev &d, int max_rows, cudaStream_t s) {
-  size_t sm = (size_t)(kNB * (max_rows + 4) + 2 * max_rows + 16 + 16 * 32 + kNB * (kNB + 1)) * 8;
-  k_chol<<<d.n_win, kCholThreads, sm, s>>>(d, max_rows);
+
+// Dynamic shared memory of the launches that size it here (the eliminations and k_solve_small take theirs from the
+// LaunchSummary).  configure_launches raises each kernel's limit with the same function the launch uses.
+template <int NCT, int KR>
+static size_t proj_smem() { return (size_t)4 * (GC_SIZE + NCT * 8 * (kTile * KR + 4)) * 8; }
+static size_t misc_smem_bytes(int max_prior_m) { return (size_t)(40 + 3 * max_prior_m + 8) * 8; }
+static size_t step_smem_bytes(int max_nc) { return (size_t)(40 + 3 * max_nc) * 8; }
+static size_t chol_glob_smem_bytes(int max_rows) { return (size_t)(kNB * (max_rows + 4) + 2 * max_rows + 16 + 16 * 32 + kNB * (kNB + 1)) * 8; }
+static size_t gather_smem_bytes(int rows, int max_ldw) { return (size_t)rows * max_ldw * 8; }   // row buffers of the landmark gathers
+static size_t schur_small_smem_bytes(int max_ldw) { return (size_t)(2 * 32 * (max_ldw + 4) + 40) * 8; }
+
+const char *configure_launches(const LaunchSummary &L) {
+  const char *const refused = "cudaFuncSetAttribute failed (shared memory request too large?)";
+  const size_t pp = proj_pp_smem();
+  if (raise_smem_limit(k_proj_lin<2, 2>, proj_smem<2, 2>()) || raise_smem_limit(k_proj_lin<4, 2>, proj_smem<4, 2>()) ||
+      raise_smem_limit(k_proj_lin<2, 4>, proj_smem<2, 4>()) || raise_smem_limit(k_proj_lin<4, 4>, proj_smem<4, 4>()) ||
+      raise_smem_limit(k_proj_lin_pp<true, false>, pp) || raise_smem_limit(k_proj_lin_pp<false, false>, pp) ||
+      raise_smem_limit(k_proj_lin_pp<true, true>, pp) || raise_smem_limit(k_proj_lin_pp<false, true>, pp))
+    return refused;
+  // 4 x 51 KB per SM needs the large shared-memory carveout
+  cudaFuncSetAttribute(k_proj_lin_pp<true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_proj_lin_pp<false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_proj_lin_pp<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  cudaFuncSetAttribute(k_proj_lin_pp<false, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  // k_chol's limit is raised for at least 2 rows; launch_chol asks for max_rows_glob
+  if (raise_smem_limit(k_chol, chol_glob_smem_bytes(std::max(L.max_rows_glob, 2))) || raise_smem_limit(k_step<false>, step_smem_bytes(L.max_nc)) ||
+      raise_smem_limit(k_step<true>, step_smem_bytes(L.max_nc)) || raise_smem_limit(k_misc_lin, misc_smem_bytes(L.max_prior_m)) ||
+      raise_smem_limit(k_imu_lin, kImuSmem))
+    return refused;
+  // the row buffers of the per-landmark gather grow with the landmark-coupled width (multi-agent windows: 6 x 88 poses)
+  const int ldw = L.max_row_tiles * 32;
+  if (raise_smem_limit(k_lm_gather, gather_smem_bytes(kGatherWarps, ldw)) || raise_smem_limit(k_lm_gather16, gather_smem_bytes(kG16Lm, ldw)))
+    return "cudaFuncSetAttribute(k_lm_gather) failed (landmark-coupled part too wide for the row buffers)";
+  // a summary size of 0 (no window uses the kernel) asks raise_smem_limit for nothing
+  if (L.max_ldw_small > 0 && raise_smem_limit(k_schur_small, schur_small_smem_bytes(L.max_ldw_small))) return "cudaFuncSetAttribute(k_schur_small) failed";
+  if (raise_smem_limit(k_sb_elim, L.sbe_smem)) return "cudaFuncSetAttribute(k_sb_elim) failed";
+  if (raise_smem_limit(k_sb_back, L.sbb_smem)) return "cudaFuncSetAttribute(k_sb_back) failed";
+  if (raise_smem_limit(k_leaf_elim, L.leaf_smem)) return "cudaFuncSetAttribute(k_leaf_elim) failed";
+  if (raise_smem_limit(k_leaf_back, L.leafb_smem)) return "cudaFuncSetAttribute(k_leaf_back) failed";
+  if (L.max_n_smem > 0 && raise_smem_limit(k_chol_smem, chol_smem_bytes(L.max_n_smem))) return "cudaFuncSetAttribute(k_chol_smem) failed";
+  if (raise_smem_limit(k_solve_small, L.fused_smem)) return "cudaFuncSetAttribute(k_solve_small) failed";
+  return nullptr;
 }
-void launch_step(const Dev &d, int max_nc, cudaStream_t s) {
+
+void launch_state_prep(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
+  if (L.n6_total > 0) k_state_prep<<<(L.n6_total + 127) / 128, 128, 0, s>>>(d, L.n6_total, 0);
+}
+void launch_imu_prep(const Dev &d, const LaunchSummary &L, const double *packed, double *full, cudaStream_t s) {
+  const int n_imu = L.n_imu_total;
+  if (n_imu > 0) k_imu_unpack<<<n_imu, 192, 0, s>>>(packed, full, n_imu);
+  if (n_imu > 0) k_imu_prep<<<(n_imu + 31) / 32, 32, 0, s>>>(d, n_imu);
+}
+void launch_prior_prep(const Dev &d, cudaStream_t s) { k_prior_prep<<<d.n_win, 256, 0, s>>>(d); }
+
+void launch_misc_lin(const Dev &d, const LaunchSummary &L, int eval_cur, cudaStream_t s) {
+  k_misc_lin<<<d.n_win, kMiscThreads, misc_smem_bytes(L.max_prior_m), s>>>(d, eval_cur);
+}
+void launch_imu_lin(const Dev &d, const LaunchSummary &L, int eval_cur, cudaStream_t s) {
+  const int n = L.n_imu_total;
+  if (n > 0) k_imu_lin<<<(n + kImuWarps - 1) / kImuWarps, kImuWarps * 32, kImuSmem, s>>>(d, eval_cur, n);
+}
+void launch_proj_lin(const Dev &d, const LaunchSummary &L, int eval_cur, cudaStream_t s) {
+  for (int v = 0; v < 8; v++) {
+    const int job_begin = L.job_begin[v], job_count = L.job_count[v];
+    if (job_count <= 0) continue;
+    const int grid = (job_count + 3) / 4;
+    switch (v) {
+      case 0: k_proj_lin<2, 2><<<grid, 128, proj_smem<2, 2>(), s>>>(d, eval_cur, job_begin, job_count); break;
+      case 1: k_proj_lin<4, 2><<<grid, 128, proj_smem<4, 2>(), s>>>(d, eval_cur, job_begin, job_count); break;
+      case 2: k_proj_lin<2, 4><<<grid, 128, proj_smem<2, 4>(), s>>>(d, eval_cur, job_begin, job_count); break;
+      case 3: k_proj_lin<4, 4><<<grid, 128, proj_smem<4, 4>(), s>>>(d, eval_cur, job_begin, job_count); break;
+      case 4: k_proj_lin_pp<true, false><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+      case 5: k_proj_lin_pp<false, false><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+      case 6: k_proj_lin_pp<true, true><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+      case 7: k_proj_lin_pp<false, true><<<grid, 128, proj_pp_smem(), s>>>(d, eval_cur, job_begin, job_count); break;
+    }
+  }
+}
+void launch_proj_debug(const Dev &d, const LaunchSummary &L, double *out, const int *tile_win, cudaStream_t s) {
+  if (L.n_tiles > 0) k_proj_debug<<<L.n_tiles, 32, 0, s>>>(d, out, L.n_tiles, tile_win);
+}
+void launch_lm_gather(const Dev &d, const LaunchSummary &L, const int *lm_win, cudaStream_t s) {
+  const int n = L.nl_total, ldw = L.max_row_tiles * 32;
+  if (n <= 0) return;
+  if (L.any_wide) k_lm_gather<<<(n + kGatherWarps - 1) / kGatherWarps, kGatherWarps * 32, gather_smem_bytes(kGatherWarps, ldw), s>>>(d, lm_win, n, ldw);
+  if (L.any_compact) k_lm_gather16<<<(n + kG16Lm - 1) / kG16Lm, kG16Lm * 16, gather_smem_bytes(kG16Lm, ldw), s>>>(d, lm_win, n, ldw);
+  if (L.n_g12 > 0) k_lm_gather12<<<(L.n_g12 + kG12Warps - 1) / kG12Warps, kG12Warps * 32, 0, s>>>(d, L.n_g12);
+}
+void launch_sb_elim(const Dev &d, const LaunchSummary &L, cudaStream_t s) { if (L.sbe_smem > 0) k_sb_elim<<<d.n_win, kSeThreads, L.sbe_smem, s>>>(d); }
+void launch_zero_sb_rows(const Dev &d, const LaunchSummary &L, cudaStream_t s) { if (L.sbe_smem > 0) k_zero_sb_rows<<<d.n_win, 256, 0, s>>>(d); }
+void launch_leaf_elim(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
+  if (L.n_leaf_total > 0) k_leaf_elim<<<L.n_leaf_total, kLeafThreads, L.leaf_smem, s>>>(d);
+}
+void launch_zero_leaf_rows(const Dev &d, const LaunchSummary &L, cudaStream_t s) { if (L.n_leaf_total > 0) k_zero_leaf_rows<<<d.n_win, 256, 0, s>>>(d); }
+void launch_schur_small(const Dev &d, const LaunchSummary &L, int with_fused, cudaStream_t s) {
+  if (with_fused ? L.max_ldw_small > 0 : L.ss_unfused)
+    k_schur_small<<<d.n_win, kSsThreads, schur_small_smem_bytes(L.max_ldw_small), s>>>(d, with_fused);
+}
+void launch_schur(const Dev &d, const SchurTile *tiles, int n_tiles, cudaStream_t s) { if (n_tiles > 0) k_schur<<<n_tiles, 128, 0, s>>>(d, tiles); }
+void launch_chol_smem(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
+  if (L.cs_unfused) k_chol_smem<<<d.n_win, chol_smem_threads(L.max_n_smem), chol_smem_bytes(L.max_n_smem), s>>>(d);
+}
+void launch_chol(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
+  if (L.any_chol_glob) k_chol<<<d.n_win, kCholThreads, chol_glob_smem_bytes(L.max_rows_glob), s>>>(d, L.max_rows_glob);
+}
+void launch_sb_back(const Dev &d, const LaunchSummary &L, cudaStream_t s) { if (L.sbb_unfused) k_sb_back<<<d.n_win, kSbBackThreads, L.sbb_smem, s>>>(d); }
+void launch_leaf_back(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
+  if (L.n_leaf_total > 0) k_leaf_back<<<L.n_leaf_total, kLeafBackThreads, L.leafb_smem, s>>>(d);
+}
+void launch_solve_small(const Dev &d, const LaunchSummary &L, cudaStream_t s) { if (L.n_fused > 0) k_solve_small<<<d.n_win, kSolveThreads, L.fused_smem, s>>>(d); }
+int solve_small_occupancy(size_t smem) {
+  int n = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_solve_small, kSolveThreads, smem) != cudaSuccess) return -1;
+  return n;
+}
+void launch_step(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
   // both kinds of windows may share a handle: each instantiation skips the other's windows
   // (n_plain_win: windows without leaves that k_solve_small does not own)
-  if (d.n_leaf_total < 0 || d.n_plain_win > 0) k_step<false><<<d.n_win, kStepThreads, (size_t)(40 + 3 * max_nc) * 8, s>>>(d, max_nc);
-  if (d.n_leaf_total > 0) k_step<true><<<d.n_win, kStepThreads, (size_t)(40 + 3 * max_nc) * 8, s>>>(d, max_nc);
+  if (d.n_leaf_total < 0 || d.n_plain_win > 0) k_step<false><<<d.n_win, kStepThreads, step_smem_bytes(L.max_nc), s>>>(d, L.max_nc);
+  if (d.n_leaf_total > 0) k_step<true><<<d.n_win, kStepThreads, step_smem_bytes(L.max_nc), s>>>(d, L.max_nc);
 }
 void launch_control(const Dev &d, int init, cudaStream_t s) { k_control<<<d.n_win, kCtlThreads, 0, s>>>(d, init); }
 void launch_tr_reset(const Dev &d, int first, cudaStream_t s) { k_tr_reset<<<(d.n_win + 127) / 128, 128, 0, s>>>(d, first); }
-void launch_cons_init(const Dev &d, int n6_total, cudaStream_t s) { if (n6_total > 0) k_cons_init<<<(n6_total + 127) / 128, 128, 0, s>>>(d, n6_total); }
-void launch_cons_pack(const Dev &d, int n6_total, const int *blk_win, cudaStream_t s) { if (n6_total > 0) k_cons_pack<<<(n6_total + 127) / 128, 128, 0, s>>>(d, n6_total, blk_win); }
-void launch_cons_apply(const Dev &d, int n6_total, const int *blk_win, cudaStream_t s) { if (n6_total > 0) k_cons_apply<<<(n6_total + 127) / 128, 128, 0, s>>>(d, n6_total, blk_win); }
-void launch_cons_refs(const Dev &d, int nsb_total, int nl_total, const int *sb_win, const int *lm_win, cudaStream_t s) {
-  int n = nsb_total * 9; if (nl_total > n) n = nl_total; if (d.n_win > n) n = d.n_win;
-  if (n > 0) k_cons_refs<<<(n + 127) / 128, 128, 0, s>>>(d, nsb_total * 9, nl_total, sb_win, lm_win);
+
+void launch_cons_init(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
+  if (L.any_admm && L.n6_total > 0) k_cons_init<<<(L.n6_total + 127) / 128, 128, 0, s>>>(d, L.n6_total);
+}
+void launch_cons_pack(const Dev &d, const LaunchSummary &L, const int *blk_win, cudaStream_t s) {
+  if (L.any_admm && L.n6_total > 0) k_cons_pack<<<(L.n6_total + 127) / 128, 128, 0, s>>>(d, L.n6_total, blk_win);
+}
+void launch_cons_apply(const Dev &d, const LaunchSummary &L, const int *blk_win, cudaStream_t s) {
+  if (L.any_admm && L.n6_total > 0) k_cons_apply<<<(L.n6_total + 127) / 128, 128, 0, s>>>(d, L.n6_total, blk_win);
+}
+void launch_cons_refs(const Dev &d, const LaunchSummary &L, const int *sb_win, const int *lm_win, cudaStream_t s) {
+  int n = L.nsb_total * 9; if (L.nl_total > n) n = L.nl_total; if (d.n_win > n) n = d.n_win;
+  if (L.any_admm && n > 0) k_cons_refs<<<(n + 127) / 128, 128, 0, s>>>(d, L.nsb_total * 9, L.nl_total, sb_win, lm_win);
 }
 
 }  // namespace d2ba

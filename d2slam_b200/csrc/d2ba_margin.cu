@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/d2ba.h"
+#include "d2ba_launch.cuh"
 
 namespace d2ba {
 
@@ -100,9 +101,10 @@ __global__ void __launch_bounds__(kEigThreads) k_prior_from_info(const int *m_of
   }
 }
 
-void launch_prior_from_info(int n_win, int max_m, const int *m_of, const long long *offJ, const long long *offv, const int *is_info,
+void launch_prior_from_info(const LaunchSummary &L, const int *m_of, const long long *offJ, const long long *offv, const int *is_info,
                             double *A, double *V, double *b, cudaStream_t s) {
-  size_t sm = (size_t)(4 * (max_m + 2) + 8) * 8;
-  k_prior_from_info<<<n_win, kEigThreads, sm, s>>>(m_of, offJ, offv, is_info, A, V, b);
+  if (!L.any_info) return;
+  size_t sm = (size_t)(4 * (L.max_prior_m + 2) + 8) * 8;
+  k_prior_from_info<<<L.n_used, kEigThreads, sm, s>>>(m_of, offJ, offv, is_info, A, V, b);
 }
 }  // namespace d2ba

@@ -29,35 +29,35 @@ ETA_FLOOR = 1e-16          # H100 (700 W): device eta <= 2.7e-17 over the catalo
 
 
 # ---------------------------------------------------------------------------------------------------------- shared memory
-# restated from d2slam_b200/csrc/d2ba_kernels.cu; the GPU tests compare every decision that depends on them
-def chol_smem_bytes(n):                 # d2ba_kernels.cu:1672
+# restated from d2slam_b200/csrc/d2ba_launch.cuh and d2ba_kernels.cu; the GPU tests compare every decision that depends on them
+def chol_smem_bytes(n):                 # d2ba_launch.cuh: chol_smem_bytes (kCsNB = 8)
     pr, need = 8 * ((n + 2) & ~1), n + 1 + 16 * 32
     return ((n + 1) * ((n + 1) & ~1) + ((n + 1) & ~1) + max(pr, need)) * 8 + 32
 
 
-def sbe_smem_bytes(ldw, n_c, nb):       # d2ba_kernels.cu:1993
+def sbe_smem_bytes(ldw, n_c, nb):       # d2ba_launch.cuh: sbe_smem_bytes (kSeSlotRows = 9)
     return (3 * 9 * ldw + nb * 2 * 81 + nb * 9 + n_c + 9 * nb + 16) * 8
 
 
-def sb_back_smem_bytes(nlc, nb):        # d2ba_kernels.cu:2156
+def sb_back_smem_bytes(nlc, nb):        # d2ba_launch.cuh: sb_back_smem_bytes
     return (((nlc + 31) & ~31) + 9 * nb + 171 * nb) * 8
 
 
-def leaf_elim_smem_bytes(n, nh):        # d2ba_kernels.cu:2243
+def leaf_elim_smem_bytes(n, nh):        # d2ba_launch.cuh: leaf_elim_smem_bytes, leaf_lda (kLeafLmChunk = 16)
     n1 = n + nh + 1
     return (n1 * (n | 1) + ((n + 1) & ~1) + 8 * ((n1 + 1) & ~1) + 64 + 16 * n1 + 8) * 8
 
 
-def solve_small_fits(ldw):              # d2ba_kernels.cu:3086 (kSolveMaxB = 12, 4 warps)
+def solve_small_fits(ldw):              # d2ba_launch.cuh: solve_small_fits (kSolveMaxB = 12, 4 warps)
     nb8 = ldw // 8
     return nb8 * (nb8 + 1) // 2 <= 12 * 4
 
 
-def chol_global_smem_bytes(max_rows):   # launch_chol / configure_kernels, d2ba_kernels.cu:3040 (kNB = 32)
+def chol_global_smem_bytes(max_rows):   # d2ba_kernels.cu: chol_glob_smem_bytes (kNB = 32)
     return (32 * (max_rows + 4) + 2 * max_rows + 16 + 16 * 32 + 32 * 33) * 8
 
 
-def gather_smem_bytes(max_ldw):         # configure_gather, d2ba_kernels.cu:3052-3053 (kGatherWarps = 8, kG16Lm = 16)
+def gather_smem_bytes(max_ldw):         # d2ba_kernels.cu: gather_smem_bytes (kGatherWarps = 8, kG16Lm = 16)
     return max(8 * max_ldw * 8, 16 * max_ldw * 8)
 
 
@@ -365,7 +365,7 @@ CATALOGUE = {
     "f12_imu_2_4": lambda: _extra_imu(_window(111, 12), 2, 4),
     # k_chol: the largest n_c whose panel fits the shared memory (one frame more is refused)
     "f53": lambda: _window(112, 53, 30),
-    # leaves: <= 96 columns and leaf_elim_smem <= 200 KB; hub <= 3/4 n_lc; hub_small: n_hub + 1 <= 96
+    # leaves: <= 96 columns and leaf_elim_smem_bytes <= 200 KB; hub <= 3/4 n_lc; hub_small: n_hub + 1 <= 96
     "a2_f15": lambda: _remote(113, 2, 15),
     "a2_f16": lambda: _remote(114, 2, 16),
     "a2_f17": lambda: _remote(115, 2, 17),
@@ -398,7 +398,7 @@ LARGE = {
     "a31_f11": (lambda: _remote(131, 31, 11, 320), 0),
     "a32_f11": (lambda: _remote(132, 32, 11, 330), 27),
 }
-# the message of each refusal: the k_chol panel (configure_kernels), the landmark tile masks
+# the message of each refusal: the k_chol panel (configure_launches), the landmark tile masks
 REFUSAL_MESSAGE = {
     "f54": r"rc=23: cudaFuncSetAttribute failed \(shared memory request too large\?\)",
     "a32_f11": r"rc=27: finalize: window 0 has 2112 landmark-coupled columns",
