@@ -9,22 +9,15 @@
 // kernel is a template over an edge policy (PgoEdge6 / PgoEdge4) that fixes the block size D and the retraction.
 // Unary gravity priors (GravityPriorPerturbAD, d2pgo's enable_gravity_prior) on 6-DoF poses in pgo_gravity_eval: the kernels
 // that sum per-pose terms take a GRAV flag, so the instantiations without priors are the kernels of a graph of edges alone.
-#include <cuda_runtime.h>
 #include <math.h>
-#include <stdint.h>
 #include <string.h>
 
 #include <algorithm>
-#include <array>
 #include <cmath>
-#include <map>
-#include <string>
-#include <unordered_map>
-#include <vector>
+#include <type_traits>
 
-#include "../../include/d2pgo.h"
 #include "d2ba_math.cuh"
-#include "d2pgo_chol.cuh"
+#include "d2pgo_handle.cuh"
 
 namespace d2ba {
 // NCCL through the dlopen'ed entry points of d2ba_host.cu
@@ -33,13 +26,9 @@ int nccl_allreduce_f64(void *comm, double *buf, size_t n, cudaStream_t s);
 void nccl_comm_destroy(void *comm);
 }  // namespace d2ba
 using namespace d2ba;
+using namespace d2pgo_host;
 
 namespace {
-
-struct PgoScalars {      // device-resident CG state that is not a per-block partial
-  double bb;             // |b|^2 of the current linear system
-  int done, iters;
-};
 
 struct PgoDev {
   int n_pose, n_edge;
@@ -779,319 +768,7 @@ __global__ void __launch_bounds__(128) k_rotinit_project(int n, const int *frame
   if (threadIdx.x == 0) chg_part[blockIdx.x] = chg;
 }
 
-template <typename T> struct Buf {
-  T *p = nullptr; size_t n = 0;
-  cudaError_t alloc(size_t c) { if (c <= n && p) return cudaSuccess; if (p) cudaFree(p); p = nullptr; n = 0; cudaError_t e = cudaMalloc(&p, (c ? c : 1) * sizeof(T)); if (e == cudaSuccess) n = c; return e; }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
-
-// ---- PCM: pairwise-consistency maximisation over the loop closures (SwarmLocalOutlierRejection, non-incremental, redundant;
-// d2pgo/src/swarm_outlier_rejection/swarm_outlier_rejection.cpp:46-303).  Loops are grouped by the unordered pair of drones;
-// a group's loops occupy consecutive slots in input order.  Per group: a bit-packed adjacency [L][W = ceil(L/32)] words,
-// bit (i, j) = smd(edge1 = max(i, j), edge2 = min(i, j)) < thres, then FMC maxCliqueHeu on it; inlier = in the clique.
-constexpr int kPcmMaxGroup = 32768;   // 128 MB of adjacency bits
-constexpr int kPcmWarps = 8;          // warps of a k_pcm_clique CTA = seeds examined per round
-
-struct PcmDev {
-  const int *g_loop;          // [G+1] slot offsets of the groups
-  const long long *g_word;    // [G+1] adjacency word offsets (sum of L W)
-  const long long *g_smd;     // [G+1] offsets of the tested pairs (sum of L (L-1) / 2)
-  const int *fa, *fb;         // [n] frame index of the loop's two keyframes, by slot
-  const unsigned char *flip;  // [n] drone ids in the opposite order to the other loops of the group with flip = 0
-  const double *rel;          // [n][8] measured T_a^-1 T_b [t, q xyzw], by slot
-  const double *cov;          // [n][21] loop covariance (S^T S)^-1, packed lower triangle, by slot
-  const double *ego;          // [F][8] ego poses
-  const double *path;         // [F] path length of the frame's drone from its first keyframe
-  unsigned *adj; int *deg; double *smd;
-  int is4; double thr, pos_cov, yaw_cov;
-};
-
-struct Pose7 { double t[3]; Q4 q; };
-D2BA_DEV Q4 qnormalized(const Q4 &q) { const double s = 1.0 / sqrt(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w); return Q4{q.x * s, q.y * s, q.z * s, q.w * s}; }
-D2BA_DEV Pose7 p7_load(const double *p) { return Pose7{{p[0], p[1], p[2]}, qnormalized(qload(p + 3))}; }
-D2BA_DEV Pose7 p7_mul(const Pose7 &a, const Pose7 &b) {   // a * b (Swarm::Pose composition; attitude normalised as its constructor does)
-  double R[9], v[3];
-  q2R(a.q, R); mv3(R, b.t, v);
-  return Pose7{{v[0] + a.t[0], v[1] + a.t[1], v[2] + a.t[2]}, qnormalized(qmul(a.q, b.q))};
-}
-D2BA_DEV Pose7 p7_inv(const Pose7 &a) {
-  const Q4 qi = qinv(a.q);
-  double R[9], v[3];
-  q2R(qi, R); mv3(R, a.t, v);
-  return Pose7{{-v[0], -v[1], -v[2]}, qnormalized(qi)};
-}
-D2BA_DEV double quat_yaw(const Q4 &q) { return atan2(2.0 * (q.w * q.z + q.x * q.y), 1.0 - 2.0 * (q.y * q.y + q.z * q.z)); }
-
-// ego motion from frame f to frame g of one drone: DeltaPose(ego_f, ego_g[, yaw only]) and the diagonal of d2pgo's ego-motion
-// covariance (d2pgo.cpp:482-493) at the path length between them (ASSUMED DroneTrajectory::get_relative_pose_by_frame_id)
-D2BA_DEV Pose7 pcm_odom(const PcmDev &d, int f, int g, double *cp, double *cr) {
-  const Pose7 a = p7_load(d.ego + (size_t)f * 8), b = p7_load(d.ego + (size_t)g * 8);
-  const double len = fabs(d.path[g] - d.path[f]);
-  *cp = d.pos_cov * len + 0.5 * d.yaw_cov * len * len;
-  *cr = d.yaw_cov * len;
-  if (!d.is4) return p7_mul(p7_inv(a), b);
-  const double ya = quat_yaw(a.q), dy = quat_yaw(b.q) - ya;
-  double s, c, sh, ch;
-  sincos(ya, &s, &c); sincos(0.5 * dy, &sh, &ch);
-  const double v[3] = {b.t[0] - a.t[0], b.t[1] - a.t[1], b.t[2] - a.t[2]};
-  return Pose7{{c * v[0] + s * v[1], -s * v[0] + c * v[1], v[2]}, qnormalized(Q4{0.0, 0.0, sh, ch})};
-}
-
-// squared Mahalanobis distance of the loop pair (edge1 = slot e1, edge2 = slot e2; swarm_outlier_rejection.cpp:141-199)
-D2BA_DEV double pcm_smd(const PcmDev &d, int e1, int e2) {
-  const bool same = d.flip[e1] == d.flip[e2];   // same_robot_pair 1; otherwise 2
-  Pose7 p2 = p7_load(d.rel + (size_t)e2 * 8);
-  if (!same) p2 = p7_inv(p2);
-  double ca_p, ca_r, cb_p, cb_r;
-  const Pose7 oa = pcm_odom(d, d.fa[e1], same ? d.fa[e2] : d.fb[e2], &ca_p, &ca_r);
-  const Pose7 ob = pcm_odom(d, d.fb[e1], same ? d.fb[e2] : d.fa[e2], &cb_p, &cb_r);
-  const Pose7 err = p7_mul(p7_mul(p7_mul(oa, p2), p7_inv(ob)), p7_inv(p7_load(d.rel + (size_t)e1 * 8)));
-  // log_map (ASSUMED = tangentSpace: [t ; angle-axis], angle = 2 atan2(|v|, |w|), sign of w)
-  double v[6] = {err.t[0], err.t[1], err.t[2], 0.0, 0.0, 0.0};
-  const double n = sqrt(err.q.x * err.q.x + err.q.y * err.q.y + err.q.z * err.q.z);
-  if (n > 0.0) {
-    const double k = 2.0 * atan2(n, fabs(err.q.w)) * (err.q.w < 0.0 ? -1.0 : 1.0) / n;
-    v[3] = k * err.q.x; v[4] = k * err.q.y; v[5] = k * err.q.z;
-  }
-  // Sigma = (cov_1 + cov_2) + (cov(odom_a) + cov(odom_b)), then v^T Sigma^-1 v by Cholesky (packed lower triangle)
-  double A[21];
-  const double *c1 = d.cov + (size_t)e1 * 21, *c2 = d.cov + (size_t)e2 * 21;
-  for (int k = 0; k < 21; k++) A[k] = c1[k] + c2[k];
-  for (int k = 0; k < 6; k++) A[k * (k + 3) / 2] += k < 3 ? ca_p + cb_p : ca_r + cb_r;
-  double y[6], s = 0.0;
-  for (int j = 0; j < 6; j++) {
-    double t = A[j * (j + 1) / 2 + j];
-    for (int k = 0; k < j; k++) t -= A[j * (j + 1) / 2 + k] * A[j * (j + 1) / 2 + k];
-    const double l = sqrt(t);
-    A[j * (j + 1) / 2 + j] = l;
-    for (int r = j + 1; r < 6; r++) {
-      double u = A[r * (r + 1) / 2 + j];
-      for (int k = 0; k < j; k++) u -= A[r * (r + 1) / 2 + k] * A[j * (j + 1) / 2 + k];
-      A[r * (r + 1) / 2 + j] = u / l;
-    }
-    double w = v[j];
-    for (int k = 0; k < j; k++) w -= A[j * (j + 1) / 2 + k] * y[k];
-    y[j] = w / l;
-    s += y[j] * y[j];
-  }
-  return s;
-}
-
-// per drone (one warp each): path length from its first keyframe, in trajectory order, by a fixed-order warp scan
-__global__ void k_pcm_path(int n_drones, const int *traj_ptr, const int *traj, const double *ego, double *path) {
-  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (w >= n_drones) return;
-  const int b = traj_ptr[w], n = traj_ptr[w + 1] - b;
-  double carry = 0.0;
-  for (int base = 0; base < n; base += 32) {
-    const int k = base + lane;
-    double x = 0.0;
-    if (k > 0 && k < n) {
-      const double *p = ego + (size_t)traj[b + k] * 8, *q = ego + (size_t)traj[b + k - 1] * 8;
-      const double dx = p[0] - q[0], dy = p[1] - q[1], dz = p[2] - q[2];
-      x = sqrt(dx * dx + dy * dy + dz * dz);
-    }
-    for (int o = 1; o < 32; o <<= 1) { const double u = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += u; }
-    if (k < n) path[traj[b + k]] = carry + x;
-    carry += __shfl_sync(0xffffffffu, x, 31);
-  }
-}
-
-// per loop slot: measurement in slot order and covariance = (S^T S)^-1 (ASSUMED LoopEdge::getCovariance)
-__global__ void k_pcm_loop(int n, const int *src, const double *rel7, const double *sqrt36, double *rel, double *cov) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= n) return;
-  const size_t s = (size_t)src[e];
-  for (int k = 0; k < 7; k++) rel[(size_t)e * 8 + k] = rel7[s * 7 + k];
-  rel[(size_t)e * 8 + 7] = 0.0;
-  const double *S = sqrt36 + s * 36;
-  double A[36], Li[36];
-  for (int i = 0; i < 6; i++) for (int j = 0; j < 6; j++) { double t = 0; for (int k = 0; k < 6; k++) t += S[k * 6 + i] * S[k * 6 + j]; A[i * 6 + j] = t; }
-  for (int j = 0; j < 6; j++) {   // A = L L^T
-    double t = A[j * 7];
-    for (int k = 0; k < j; k++) t -= A[j * 6 + k] * A[j * 6 + k];
-    A[j * 7] = sqrt(t);
-    for (int r = j + 1; r < 6; r++) { double u = A[r * 6 + j]; for (int k = 0; k < j; k++) u -= A[r * 6 + k] * A[j * 6 + k]; A[r * 6 + j] = u / A[j * 7]; }
-  }
-  for (int c = 0; c < 6; c++)
-    for (int r = 0; r < 6; r++) {
-      double t = r == c ? 1.0 : 0.0;
-      for (int k = c; k < r; k++) t -= A[r * 6 + k] * Li[k * 6 + c];
-      Li[r * 6 + c] = r < c ? 0.0 : t / A[r * 7];
-    }
-  for (int r = 0; r < 6; r++) for (int c = 0; c <= r; c++) {   // (L L^T)^-1 = L^-T L^-1
-    double t = 0;
-    for (int k = r; k < 6; k++) t += Li[k * 6 + r] * Li[k * 6 + c];
-    cov[(size_t)e * 21 + r * (r + 1) / 2 + c] = t;
-  }
-}
-
-D2BA_DEV int pcm_group_of(const long long *off, int G, long long t) {   // the g with off[g] <= t < off[g + 1]
-  int lo = 0, hi = G - 1;
-  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (off[mid] <= t) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
-// one warp per adjacency word (row i, columns 32 w .. 32 w + 31 of a group): the word is a ballot, so no atomics.  Cell (i, j)
-// is the pair with edge1 = max(i, j); the smd of j < i is kept for d2pgo_debug_pcm_smd.
-__global__ void __launch_bounds__(256) k_pcm_pairs(PcmDev d, int G, long long n_words) {
-  const long long t = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (t >= n_words) return;
-  const int g = pcm_group_of(d.g_word, G, t);
-  const int base = d.g_loop[g], L = d.g_loop[g + 1] - base, W = (L + 31) >> 5;
-  const long long local = t - d.g_word[g];
-  const int i = (int)(local / W), j = (int)(local % W) * 32 + lane;
-  bool ok = false;
-  if (j < L && j != i) {
-    const double s = pcm_smd(d, base + max(i, j), base + min(i, j));
-    ok = s < d.thr;
-    if (j < i) d.smd[d.g_smd[g] + (long long)i * (i - 1) / 2 + j] = s;
-  }
-  const unsigned word = __ballot_sync(0xffffffffu, ok);
-  if (lane == 0) d.adj[t] = word;
-}
-
-__global__ void k_pcm_degree(int G, const int *g_loop, const long long *g_word, const unsigned *adj, int *deg) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= g_loop[G]) return;
-  int lo = 0, hi = G - 1;
-  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (g_loop[mid] <= e) lo = mid; else hi = mid - 1; }
-  const int L = g_loop[lo + 1] - g_loop[lo], W = (L + 31) >> 5;
-  const unsigned *row = adj + g_word[lo] + (long long)(e - g_loop[lo]) * W;
-  int c = 0;
-  for (int k = 0; k < W; k++) c += __popc(row[k]);
-  deg[e] = c;
-}
-
-// FMC's greedy from seed s under the running maximum m (findCliqueHeu.cpp:146-239): C = N(s) & {deg >= m}; repeat
-// v = max C, C &= N(v).  One warp; C in shared memory, word k owned by lane k % 32.  Returns the clique size 1 + picks, or 0
-// once the clique can no longer exceed m (1 + picks + |C| <= m): such a seed is never taken, so stopping early changes nothing.
-D2BA_DEV int pcm_greedy(int s, int m, const unsigned *rows, int W, const unsigned *degmask, unsigned *C, int lane, long long *rounds, unsigned char *member) {
-  for (int k = lane; k < W; k += 32) C[k] = rows[(size_t)s * W + k] & degmask[k];
-  if (member && lane == 0) member[s] = 1;
-  int picks = 0;
-  for (;;) {
-    int cnt = 0, hi = -1;
-    for (int k = lane; k < W; k += 32) { const unsigned c = C[k]; cnt += __popc(c); if (c) hi = k * 32 + 31 - __clz(c); }
-    cnt = __reduce_add_sync(0xffffffffu, cnt);
-    hi = __reduce_max_sync(0xffffffffu, hi);
-    if (1 + picks + cnt <= m) return 0;
-    if (cnt == 0) return 1 + picks;
-    if (member && lane == 0) member[hi] = 1;
-    picks++; (*rounds)++;
-    for (int k = lane; k < W; k += 32) C[k] &= rows[(size_t)hi * W + k];
-  }
-}
-
-D2BA_DEV void pcm_degmask(unsigned *degmask, const int *deg, int L, int W, int m) {   // bit u: u < L and deg(u) >= m
-  for (int k = threadIdx.x; k < W; k += blockDim.x) {
-    unsigned w = 0;
-    for (int b = 0; b < 32; b++) { const int u = k * 32 + b; if (u < L && deg[u] >= m) w |= 1u << b; }
-    degmask[k] = w;
-  }
-}
-
-// one CTA per group: FMC maxCliqueHeu, exactly.  Seeds are taken kPcmWarps at a time under the current m; the first of them
-// (by index) whose clique exceeds m commits, and the seeds after it are examined again under the new m.  The committed seed's
-// clique is rebuilt at the end under the m it was found with.  stats[g] = {sum of degrees, greedy rounds}.
-__global__ void __launch_bounds__(kPcmWarps * 32) k_pcm_clique(const int *g_loop, const long long *g_word, const unsigned *adj, const int *deg_all, unsigned char *inlier, long long *stats) {
-  extern __shared__ unsigned pcm_smem[];
-  __shared__ int s_size[kPcmWarps], s_m, s_best, s_best_m, s_next;
-  __shared__ long long s_part[kPcmWarps * 32];
-  const int g = blockIdx.x, base = g_loop[g], L = g_loop[g + 1] - base, W = (L + 31) >> 5;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const unsigned *rows = adj + g_word[g];
-  const int *deg = deg_all + base;
-  unsigned *degmask = pcm_smem, *C = pcm_smem + W * (1 + warp);
-  long long rounds = 0, dsum = 0;
-  for (int k = threadIdx.x; k < L; k += blockDim.x) { inlier[base + k] = 0; dsum += deg[k]; }
-  if (threadIdx.x == 0) { s_m = -1; s_best = -1; s_best_m = -1; }
-  pcm_degmask(degmask, deg, L, W, -1);
-  __syncthreads();
-  for (int s0 = 0; s0 < L;) {
-    const int m = s_m, s = s0 + warp;
-    int size = 0;
-    if (s < L && !(m > deg[s])) size = pcm_greedy(s, m, rows, W, degmask, C, lane, &rounds, nullptr);   // Pruning 1
-    if (lane == 0) s_size[warp] = size;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      s_next = s0 + kPcmWarps;
-      for (int w = 0; w < kPcmWarps; w++)
-        if (s_size[w] > m) { s_best = s0 + w; s_best_m = m; s_m = s_size[w]; s_next = s0 + w + 1; break; }
-    }
-    __syncthreads();
-    if (s_m != m) { pcm_degmask(degmask, deg, L, W, s_m); __syncthreads(); }
-    s0 = s_next;
-    __syncthreads();
-  }
-  if (s_best >= 0) {
-    pcm_degmask(degmask, deg, L, W, s_best_m);
-    __syncthreads();
-    if (warp == 0) { long long dummy = 0; pcm_greedy(s_best, s_best_m, rows, W, degmask, C, lane, &dummy, inlier + base); }
-  }
-  s_part[threadIdx.x] = lane == 0 ? rounds : 0;   // every lane of a warp counted the same rounds
-  __syncthreads();
-  if (threadIdx.x == 0) { long long r = 0; for (int k = 0; k < kPcmWarps * 32; k++) r += s_part[k]; s_part[0] = r; }
-  __syncthreads();
-  const long long r = s_part[0];
-  __syncthreads();
-  s_part[threadIdx.x] = dsum;
-  __syncthreads();
-  if (threadIdx.x == 0) { long long t = 0; for (int k = 0; k < kPcmWarps * 32; k++) t += s_part[k]; stats[2 * g] = t; stats[2 * g + 1] = r; }
-}
-
-struct PcmBufs {
-  Buf<int> g_loop, fa, fb, src, traj_ptr, traj, deg; Buf<long long> g_word, g_smd, stats; Buf<unsigned char> flip, inlier;
-  Buf<double> rel_in, sqrt_in, rel, cov, ego, path, smd; Buf<unsigned> adj;
-  long long n_smd = -1;   // tested pairs of the last d2pgo_pcm call (-1: none yet)
-  cudaEvent_t ev_pair = nullptr;
-  void release() {
-    g_loop.release(); fa.release(); fb.release(); src.release(); traj_ptr.release(); traj.release(); deg.release(); g_word.release(); g_smd.release();
-    stats.release(); flip.release(); inlier.release(); rel_in.release(); sqrt_in.release(); rel.release(); cov.release(); ego.release(); path.release();
-    smd.release(); adj.release();
-    if (ev_pair) cudaEventDestroy(ev_pair);
-    ev_pair = nullptr;
-  }
-};
 }  // namespace
-
-struct d2pgo_handle {
-  d2pgo_config cfg;
-  int dof = 6;              // pose block size: 6 (RelPoseFactorAD on SE(3)) or 4 (RelPoseFactor4D on [x y z yaw])
-  std::string err;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  std::vector<int64_t> ids; std::unordered_map<int64_t, int> index;
-  std::vector<double> poses; std::vector<unsigned char> fixed;   // [N][8], the device layout of PgoDev::x
-  std::vector<int> ea, eb; std::vector<double> rel, sinfo;         // rel [E][8], sinfo [E][dof^2]
-  std::vector<int> gp_pose; std::vector<double> gp_u, gp_S;        // gravity priors: pose index, u_ego [G][3], S [G][9]
-  Buf<double> d_gp_u, d_gp_S, d_glin[2]; Buf<int> d_gp_pose, d_prior_of;
-  Buf<double> d_x[2], d_rel, d_sinfo, d_lin[2], d_g[2], d_D[2], d_Minv, d_dx, d_r, d_z, d_p, d_Ap, d_cost, d_damp, d_t, d_part, d_cost_part;
-  Buf<unsigned char> d_fixed; Buf<int> d_ea, d_eb, d_inc_ptr, d_inc; Buf<PgoScalars> d_s;
-  cudaGraphExec_t cg_graph[2] = {nullptr, nullptr};   // 16 CG iterations on the linearisation buffer 0 / 1 (single rank)
-  double graph_tol2 = -1.0;
-  bool uploaded = false;
-  void *comm = nullptr; int rank = 0, nranks = 1;
-  PcmBufs pcm;   // d2pgo_pcm's device buffers (independent of the poses and edges above)
-  // ARock (d2pgo_arock_enable): owner agent and 6-DoF q_init per pose id, the dual table keyed (neighbour, frame id) in
-  // ascending order, the messages received since the last step, and the device copy of the table (in table order)
-  bool arock = false; d2pgo_arock_config acfg = {};
-  std::unordered_map<int64_t, int32_t> owner; std::unordered_map<int64_t, std::array<double, 4>> qinit;
-  struct Dual { double yl[6], yr[6]; };
-  struct Msg { int32_t sender, target; std::vector<int64_t> frames; std::vector<double> duals; };
-  std::map<std::pair<int32_t, int64_t>, Dual> duals;
-  std::vector<Msg> inbox;
-  Buf<int> d_ak_pose, d_ak_ptr, d_ak_of; Buf<double> d_ak_yr, d_ak_yl, d_ak_qinit, d_ak_lin[2], d_ak_coord;
-  int ak_n = -1;                      // duals on the device, -1 = none synced
-  const void *ak_key[4] = {nullptr, nullptr, nullptr, nullptr};   // buffers the captured CG graphs point at
-  bool graph_ark = false;             // the captured CG graphs carry the proximal terms
-  d2pgo_handle *rot = nullptr;        // d2pgo_rot_init's row systems (dof 3), kept between calls for their buffers
-  int linear_solver = D2PGO_LINEAR_PCG;   // d2pgo_set_linear_solver
-  d2pgo_chol::Numeric *chol = nullptr;    // the sparse Cholesky's analysis and device state (d2pgo_chol.cu)
-};
-
-#define PCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return 100 + (int)e_; } } while (0)
 
 // the 6-DoF and the 4-DoF entry points each serve one kind of handle
 static int pgo_want_dof(d2pgo_handle *h, int dof, const char *what) {
@@ -1161,20 +838,10 @@ int d2pgo_create(const d2pgo_config *cfg, d2pgo_handle **out) {
   h->cfg = *cfg;
   h->dof = cfg->pose_dof == 4 ? 4 : 6;
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { delete h; return 6; }
+  h->own_stream = true;
   cudaEventCreate(&h->ev0); cudaEventCreate(&h->ev1);
   *out = h;
   return 0;
-}
-
-static void pgo_release(d2pgo_handle *h) {   // every device buffer and graph of a handle
-  for (int b = 0; b < 2; b++) { h->d_x[b].release(); h->d_g[b].release(); h->d_D[b].release(); h->d_lin[b].release(); if (h->cg_graph[b]) cudaGraphExecDestroy(h->cg_graph[b]); }
-  h->d_damp.release(); h->d_t.release(); h->d_part.release(); h->d_cost_part.release(); h->d_inc_ptr.release(); h->d_inc.release();
-  h->d_rel.release(); h->d_sinfo.release(); h->d_Minv.release(); h->d_dx.release(); h->d_r.release(); h->d_z.release(); h->d_p.release();
-  h->d_Ap.release(); h->d_cost.release(); h->d_fixed.release(); h->d_ea.release(); h->d_eb.release(); h->d_s.release();
-  h->d_gp_u.release(); h->d_gp_S.release(); h->d_glin[0].release(); h->d_glin[1].release(); h->d_gp_pose.release(); h->d_prior_of.release();
-  h->pcm.release();
-  h->d_ak_pose.release(); h->d_ak_ptr.release(); h->d_ak_of.release(); h->d_ak_yr.release(); h->d_ak_yl.release(); h->d_ak_qinit.release();
-  h->d_ak_lin[0].release(); h->d_ak_lin[1].release(); h->d_ak_coord.release();
 }
 
 int d2pgo_destroy(d2pgo_handle *h) {
@@ -1182,10 +849,6 @@ int d2pgo_destroy(d2pgo_handle *h) {
   cudaSetDevice(h->cfg.device);
   cudaStreamSynchronize(h->stream);
   if (h->comm) nccl_comm_destroy(h->comm);
-  pgo_release(h);
-  if (h->rot) { pgo_release(h->rot); delete h->rot; }
-  delete h->chol;
-  cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1); cudaStreamDestroy(h->stream);
   delete h;
   return 0;
 }
@@ -1228,19 +891,22 @@ int d2pgo_comm_init(d2pgo_handle *h, const uint8_t unique_id[128], int32_t rank,
 
 }  // extern "C"
 
-static void pgo_drop_graphs(d2pgo_handle *h) {
-  for (int b = 0; b < 2; b++) if (h->cg_graph[b]) { cudaGraphExecDestroy(h->cg_graph[b]); h->cg_graph[b] = nullptr; }
+// per-block cost partials of the edges, the gravity priors and the synced duals, in that order
+static int pgo_alloc_cost_part(d2pgo_handle *h) {
+  const size_t nbe = (h->ea.size() + 127) / 128, nbg = (h->gp_pose.size() + 127) / 128, nbk = (size_t)(std::max(h->ak_n, 0) + 127) / 128;
+  PCK(h->d_cost_part.alloc(nbe + nbg + nbk + 1));
+  return 0;
 }
 
 static int pgo_upload(d2pgo_handle *h) {
-  const size_t N = h->ids.size(), E = h->ea.size(), nbp = (N + 127) / 128, nbe = (E + 127) / 128;
+  const size_t N = h->ids.size(), E = h->ea.size(), nbp = (N + 127) / 128;
   const size_t D = h->dof, DD = D * D;
-  pgo_drop_graphs(h);
   for (int b = 0; b < 2; b++) { PCK(h->d_x[b].alloc(N * 8)); PCK(h->d_g[b].alloc(N * D)); PCK(h->d_D[b].alloc(N * DD)); PCK(h->d_lin[b].alloc(E * (D + 2 * DD))); }
   PCK(h->d_rel.alloc(E * 8)); PCK(h->d_sinfo.alloc(E * DD)); PCK(h->d_Minv.alloc(N * DD));
   PCK(h->d_dx.alloc(N * D)); PCK(h->d_r.alloc(N * D)); PCK(h->d_z.alloc(N * D)); PCK(h->d_p.alloc(N * D)); PCK(h->d_Ap.alloc(N * D)); PCK(h->d_cost.alloc(2));
-  const size_t G = h->gp_pose.size(), nbg = (G + 127) / 128;
-  PCK(h->d_damp.alloc(N * D)); PCK(h->d_t.alloc(E * 2 * D)); PCK(h->d_part.alloc(5 * nbp)); PCK(h->d_cost_part.alloc(nbe + nbg + 1));
+  const size_t G = h->gp_pose.size();
+  PCK(h->d_damp.alloc(N * D)); PCK(h->d_t.alloc(E * 2 * D)); PCK(h->d_part.alloc(5 * nbp));
+  if (int rc = pgo_alloc_cost_part(h)) return rc;
   PCK(h->d_fixed.alloc(N)); PCK(h->d_ea.alloc(E)); PCK(h->d_eb.alloc(E)); PCK(h->d_s.alloc(1)); PCK(h->d_inc_ptr.alloc(N + 1)); PCK(h->d_inc.alloc(2 * E));
   // incidence lists (pose -> its edges, ascending edge order): the fixed summation order of every product
   std::vector<int> ptr(N + 1, 0), inc(2 * E);
@@ -1282,13 +948,13 @@ static PgoDev pgo_view(d2pgo_handle *h, int cur) {
 }
 
 static PgoPriorDev pgo_prior_view(d2pgo_handle *h, int cur) {
-  PgoPriorDev pr;
+  PgoPriorDev pr; memset(&pr, 0, sizeof pr);
   pr.n_prior = (int)h->gp_pose.size(); pr.pose = h->d_gp_pose.p; pr.prior_of = h->d_prior_of.p; pr.u = h->d_gp_u.p; pr.S = h->d_gp_S.p; pr.lin = h->d_glin[cur].p;
   return pr;
 }
 
 static PgoArockDev pgo_arock_view(d2pgo_handle *h, int cur) {
-  PgoArockDev a;
+  PgoArockDev a; memset(&a, 0, sizeof a);
   a.n_dual = h->ak_n > 0 ? h->ak_n : 0; a.pose = h->d_ak_pose.p; a.ptr = h->d_ak_ptr.p; a.of = h->d_ak_of.p; a.yr = h->d_ak_yr.p; a.yl = h->d_ak_yl.p;
   a.qinit = h->d_ak_qinit.p; a.lin = h->d_ak_lin[cur].p;
   const bool six = h->dof == 6;
@@ -1297,22 +963,24 @@ static PgoArockDev pgo_arock_view(d2pgo_handle *h, int cur) {
   return a;
 }
 
-// cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks.  GRAV: this
-// rank has gravity priors (their cost partials follow the edges', their terms enter g and D after each pose's edges).  ARK:
-// the ARock proximal terms of the synced dual table (cost partials last, g and D after the edges and priors).
-template <class P, bool GRAV, bool ARK = false>
-static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
+// cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks.  grav: the
+// gravity priors of this rank (6-DoF only; their cost partials follow the edges', their terms enter g and D after each pose's
+// edges).  ark: the ARock proximal terms of the synced dual table (cost partials last, g and D after the edges and priors).
+template <class P>
+static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, bool grav, bool ark, double *cost) {
   constexpr int D = P::D;
   PgoDev d = pgo_view(h, b);
   const PgoPriorDev pr = pgo_prior_view(h, b);
   const PgoArockDev ak = pgo_arock_view(h, b);
   const size_t N = h->ids.size();
-  const int nbe = (d.n_edge + 127) / 128, nbg = GRAV ? (pr.n_prior + 127) / 128 : 0, nbk = ARK ? (ak.n_dual + 127) / 128 : 0;
+  const int nbe = (d.n_edge + 127) / 128, nbg = grav ? (pr.n_prior + 127) / 128 : 0, nbk = ark ? (ak.n_dual + 127) / 128 : 0;
   if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, h->stream>>>(d, h->d_cost_part.p, want_jac);
   if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, h->stream>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
   if (nbk > 0) k_pgo_arock_lin<D><<<nbk, 128, 0, h->stream>>>(d, h->d_cost_part.p + nbe + nbg, ak);
   k_pgo_sum<<<1, 128, 0, h->stream>>>(h->d_cost_part.p, nbe + nbg + nbk, h->d_cost.p);
-  if (want_jac) k_pgo_gD<P, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+  if (want_jac && grav) {
+    if constexpr (D == 6) k_pgo_gD<P, true><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+  } else if (want_jac) k_pgo_gD<P, false><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
   if (want_jac && nbk > 0) k_pgo_arock_gD<D><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, ak);
   if (h->comm) {
     if (nccl_allreduce_f64(h->comm, h->d_cost.p, 1, h->stream)) { h->err = "ncclAllReduce(cost) failed"; return 40; }
@@ -1325,23 +993,76 @@ static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, double *cost) {
 
 constexpr int kCgChunk = 16;   // CG iterations between two looks at the convergence flag (one graph launch on a single rank)
 
-template <class P, bool GRAV, bool ARK>
-static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr, const PgoArockDev &ak, double tol2) {
+// the pose pass of one CG iteration, with the gravity priors' terms when grav (6-DoF only)
+template <class P, bool LOCAL>
+static void pgo_cg_pose(d2pgo_handle *h, const PgoDev &d, int par, double tol2, const PgoPriorDev &pr, bool grav) {
+  if constexpr (P::D == 6) {
+    if (grav) { k_pgo_cg_pose<P, LOCAL, true><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr); return; }
+  }
+  k_pgo_cg_pose<P, LOCAL, false><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
+}
+
+// kCgChunk CG iterations; ark: the proximal terms' damping pass.  The rotation rows (PgoRotRow) solve on one rank without
+// proximal terms, so only their single-rank kernels exist.
+template <class P>
+static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr, const PgoArockDev &ak, double tol2, bool grav, bool ark) {
   const int ge = (d.n_edge + 127) / 128;
   for (int k = 0; k < kCgChunk; k++) {
     const int par = k & 1;
     if (d.n_edge > 0) k_pgo_cg_edge<P><<<ge, 128, 0, h->stream>>>(d, par, tol2);
-    if constexpr (ARK) {   // an ARock handle has no communicator (d2pgo_comm_init refuses it)
-      k_pgo_cg_pose<P, true, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
-      k_pgo_arock_cg_pAp<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, ak);
-    } else if (h->comm) {
-      k_pgo_cg_pose<P, true, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
-      // every rank holds the same r, z, p (the all-reduced products are bitwise identical), so all of them reach the same
-      // `done` decision at the same iteration and the collective below is always matched
-      if (nccl_allreduce_f64(h->comm, d.Ap, (size_t)d.n_pose * P::D, h->stream)) { h->err = "ncclAllReduce(Ap) failed"; return 40; }
-      k_pgo_cg_pAp<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
-    } else k_pgo_cg_pose<P, false, GRAV><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
+    if (!ark && !h->comm) {
+      pgo_cg_pose<P, false>(h, d, par, tol2, pr, grav);
+    } else if constexpr (!std::is_same<P, PgoRotRow>::value) {
+      pgo_cg_pose<P, true>(h, d, par, tol2, pr, grav);
+      if (ark) {   // an ARock handle has no communicator (d2pgo_comm_init refuses it)
+        k_pgo_arock_cg_pAp<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, ak);
+      } else {
+        // every rank holds the same r, z, p (the all-reduced products are bitwise identical), so all of them reach the same
+        // `done` decision at the same iteration and the collective below is always matched
+        if (nccl_allreduce_f64(h->comm, d.Ap, (size_t)d.n_pose * P::D, h->stream)) { h->err = "ncclAllReduce(Ap) failed"; return 40; }
+        k_pgo_cg_pAp<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+      }
+    }
     k_pgo_cg_step<P><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2);
+  }
+  return 0;
+}
+
+// (J^T J + lambda diag D) dx = -g at linearisation buffer `cur` by block-Jacobi preconditioned CG (J^T J is never formed), in
+// chunks of kCgChunk iterations up to max_it, until the convergence flag; *s holds the CG scalars after the last chunk.  On a
+// single rank a chunk is one launch of the buffer's captured graph.  The graph's kernel nodes hold the arguments they were
+// captured with (pointers, counts, weights, tol2), so it is captured again whenever any of those bytes differ.
+template <class P>
+static int pgo_pcg(d2pgo_handle *h, int cur, double lambda, double tol2, int max_it, bool grav, bool ark, PgoScalars *s) {
+  const PgoDev d = pgo_view(h, cur);
+  const PgoPriorDev pr = pgo_prior_view(h, cur);
+  const PgoArockDev ak = pgo_arock_view(h, cur);
+  k_pgo_precond<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_D[cur].p, lambda);
+  k_pgo_cg_init<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[cur].p);
+  k_pgo_cg_init2<<<1, 128, 0, h->stream>>>(d);
+  std::string args((const char *)&d, sizeof d);
+  args.append((const char *)&pr, sizeof pr).append((const char *)&ak, sizeof ak).append((const char *)&tol2, sizeof tol2);
+  args += (char)grav; args += (char)ark;
+  cudaGraphExec_t &graph = h->cg_graph[cur];
+  for (int k = 0; k < max_it; k += kCgChunk) {
+    if (h->comm) {
+      if (int rc = pgo_cg_chunk<P>(h, d, pr, ak, tol2, grav, ark)) return rc;
+    } else {
+      if (!graph || h->cg_args[cur] != args) {
+        if (graph) { cudaGraphExecDestroy(graph); graph = nullptr; }
+        cudaGraph_t g;
+        PCK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
+        pgo_cg_chunk<P>(h, d, pr, ak, tol2, grav, ark);
+        PCK(cudaStreamEndCapture(h->stream, &g));
+        PCK(cudaGraphInstantiate(&graph, g, 0));
+        cudaGraphDestroy(g);
+        h->cg_args[cur] = args;
+      }
+      PCK(cudaGraphLaunch(graph, h->stream));
+    }
+    PCK(cudaMemcpyAsync(s, h->d_s.p, sizeof *s, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaStreamSynchronize(h->stream));
+    if (s->done) break;   // identical on every rank (see pgo_cg_chunk)
   }
   return 0;
 }
@@ -1349,7 +1070,7 @@ static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr,
 // the sparse Cholesky's symbolic analysis of the handle's current structure (host only: poses, fixed flags, edge ends), redone
 // when that structure changed; then the size limits, before any device work of the solve
 static int pgo_chol_analyse(d2pgo_handle *h) {
-  if (!h->chol) h->chol = new d2pgo_chol::Numeric();
+  if (!h->chol) h->chol.reset(new d2pgo_chol::Numeric());
   d2pgo_chol::Symbolic &S = h->chol->sym;
   if (S.D == h->dof && S.fixed == h->fixed && S.ea == h->ea && S.eb == h->eb) return 0;
   h->chol->release();
@@ -1380,31 +1101,26 @@ static int pgo_chol_step(d2pgo_handle *h, int cur, double lambda, bool *failed) 
   return c.step(h->stream, cur, in, lambda, failed, h->err);
 }
 
-// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4), by 6-DoF graphs with gravity priors (GRAV)
-// and by ARock local problems (ARK: the proximal terms of the synced dual table)
-template <class P, bool GRAV, bool ARK = false>
-static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
+// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4), with the handle's gravity priors and, when
+// ark, the ARock proximal terms of the synced dual table
+template <class P>
+static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   int rc;
-  const bool chol = h->linear_solver == D2PGO_LINEAR_SPARSE_CHOLESKY;
+  const bool chol = h->linear_solver == D2PGO_LINEAR_SPARSE_CHOLESKY, grav = !h->gp_pose.empty();
   if (chol) {
     if ((rc = pgo_chol_prepare(h))) return rc;
     h->chol->factorizations = h->chol->failed = 0; h->chol->factor_ms = h->chol->solve_ms = 0.0;
   }
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
   const int N = (int)h->ids.size();
-  const int gp = (N + 127) / 128;
   d2pgo_report R; memset(&R, 0, sizeof R);
   PCK(cudaEventRecord(h->ev0, h->stream));
   int cur = 0;                    // buffer (poses, lin records, g, D) of the accepted point
   double cost = 0, lambda = h->cfg.lambda0;
-  if ((rc = pgo_linearize<P, GRAV, ARK>(h, cur, 1, &cost))) return rc;
+  if ((rc = pgo_linearize<P>(h, cur, 1, grav, ark, &cost))) return rc;
   R.initial_cost = cost;
   const double tol2 = h->cfg.pcg_tolerance * h->cfg.pcg_tolerance;
-  if (tol2 != h->graph_tol2 || ARK != h->graph_ark) { pgo_drop_graphs(h); h->graph_tol2 = tol2; h->graph_ark = ARK; }
   for (int it = 0; it < h->cfg.max_iterations; it++) {
-    PgoDev d = pgo_view(h, cur);
-    const PgoPriorDev pr = pgo_prior_view(h, cur);
-    const PgoArockDev ak = pgo_arock_view(h, cur);
     PgoScalars s; memset(&s, 0, sizeof s);
     if (chol) {   // the exact step from the sparse Cholesky; a failed factorisation is a rejected step
       bool failed = false;
@@ -1415,31 +1131,11 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
         if (lambda > 1e8) break;
         continue;
       }
-    } else {
-    // (J^T J + lambda diag D) dx = -g by block-Jacobi preconditioned CG; J^T J is never formed
-    k_pgo_precond<P><<<gp, 128, 0, h->stream>>>(d, h->d_D[cur].p, lambda);
-    k_pgo_cg_init<P><<<gp, 128, 0, h->stream>>>(d, h->d_g[cur].p);
-    k_pgo_cg_init2<<<1, 128, 0, h->stream>>>(d);
-    for (int k = 0; k < h->cfg.pcg_max_iterations; k += kCgChunk) {
-      if (!h->comm) {
-        if (!h->cg_graph[cur]) {
-          cudaGraph_t g;
-          PCK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-          pgo_cg_chunk<P, GRAV, ARK>(h, d, pr, ak, tol2);
-          PCK(cudaStreamEndCapture(h->stream, &g));
-          PCK(cudaGraphInstantiate(&h->cg_graph[cur], g, 0));
-          cudaGraphDestroy(g);
-        }
-        PCK(cudaGraphLaunch(h->cg_graph[cur], h->stream));
-      } else if ((rc = pgo_cg_chunk<P, GRAV, ARK>(h, d, pr, ak, tol2))) return rc;
-      PCK(cudaMemcpyAsync(&s, h->d_s.p, sizeof s, cudaMemcpyDeviceToHost, h->stream));
-      PCK(cudaStreamSynchronize(h->stream));
-      if (s.done) break;   // identical on every rank (see pgo_cg_chunk)
-    }
-    }
-    k_pgo_retract<P><<<gp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
+    } else if ((rc = pgo_pcg<P>(h, cur, lambda, tol2, h->cfg.pcg_max_iterations, grav, ark, &s))) return rc;
+    const PgoDev d = pgo_view(h, cur);
+    k_pgo_retract<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
     double cand = 0;
-    if ((rc = pgo_linearize<P, GRAV, ARK>(h, 1 - cur, 1, &cand))) return rc;
+    if ((rc = pgo_linearize<P>(h, 1 - cur, 1, grav, ark, &cand))) return rc;
     R.pcg_iterations += s.iters; R.iterations++;
     if (cand < cost && isfinite(cand)) {
       const double rel_dec = (cost - cand) / (cost > 0 ? cost : 1.0);
@@ -1452,9 +1148,9 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
     }
   }
   PCK(cudaEventRecord(h->ev1, h->stream));
+  if (cur != 0) PCK(cudaMemcpyAsync(h->d_x[0].p, h->d_x[1].p, (size_t)N * 64, cudaMemcpyDeviceToDevice, h->stream));   // a following solve starts from buffer 0
   PCK(cudaMemcpyAsync(h->poses.data(), h->d_x[cur].p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
-  if (cur != 0) PCK(cudaMemcpy(h->d_x[0].p, h->d_x[1].p, (size_t)N * 64, cudaMemcpyDeviceToDevice));   // a following solve starts from buffer 0
   float ms = 0; cudaEventElapsedTime(&ms, h->ev0, h->ev1);
   R.final_cost = cost; R.device_ms = ms;
   if (rep) *rep = R;
@@ -1466,8 +1162,7 @@ extern "C" {
 int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h || h->ids.empty()) return 1;
   cudaSetDevice(h->cfg.device);
-  if (h->dof == 4) return pgo_solve<PgoEdge4, false>(h, rep);
-  return h->gp_pose.empty() ? pgo_solve<PgoEdge6, false>(h, rep) : pgo_solve<PgoEdge6, true>(h, rep);
+  return h->dof == 4 ? pgo_solve<PgoEdge4>(h, rep, false) : pgo_solve<PgoEdge6>(h, rep, false);
 }
 
 int d2pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out) {
@@ -1490,9 +1185,10 @@ int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles) {
   const size_t E = h->ea.size(), W = (size_t)h->dof + 2 * (size_t)h->dof * h->dof;   // 78 (6-DoF) or 36 (4-DoF) per edge
   if ((size_t)out_doubles < E * W) { h->err = "debug_edges: buffer too small"; return 2; }
   double cost;
-  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4, false>(h, 0, 1, &cost) : pgo_linearize<PgoEdge6, false>(h, 0, 1, &cost))) return rc;
+  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4>(h, 0, 1, false, false, &cost) : pgo_linearize<PgoEdge6>(h, 0, 1, false, false, &cost))) return rc;
   std::vector<double> tmp(E * W);
-  PCK(cudaMemcpy(tmp.data(), h->d_lin[0].p, E * W * 8, cudaMemcpyDeviceToHost));
+  PCK(cudaMemcpyAsync(tmp.data(), h->d_lin[0].p, E * W * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
   for (size_t e = 0; e < E; e++) for (size_t k = 0; k < W; k++) out[e * W + k] = tmp[k * E + e];   // device layout is field-major
   return 0;
 }
@@ -1545,9 +1241,10 @@ int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
   double cost;
-  if ((rc = pgo_linearize<PgoEdge6, true>(h, 0, 1, &cost))) return rc;
+  if ((rc = pgo_linearize<PgoEdge6>(h, 0, 1, true, false, &cost))) return rc;
   std::vector<double> tmp(G * 12);
-  PCK(cudaMemcpy(tmp.data(), h->d_glin[0].p, G * 12 * 8, cudaMemcpyDeviceToHost));
+  PCK(cudaMemcpyAsync(tmp.data(), h->d_glin[0].p, G * 12 * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
   for (size_t k = 0; k < G; k++) {   // device layout is field-major [12][G]: r(3), J_theta (3x3)
     double *o = out + k * 21;
     for (int a = 0; a < 3; a++) o[a] = tmp[a * G + k];
@@ -1559,8 +1256,6 @@ int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles
 }  // extern "C"
 
 // ---- ARock host side
-static int arock_fail(d2pgo_handle *h, int rc, const std::string &msg) { h->err = msg; return rc; }
-
 static bool all_finite(const double *v, size_t n) {
   for (size_t k = 0; k < n; k++) if (!std::isfinite(v[k])) return false;
   return true;
@@ -1589,10 +1284,8 @@ static int arock_sync(d2pgo_handle *h) {
   { std::vector<int> fill(ptr.begin(), ptr.end() - 1);
     for (size_t j = 0; j < K; j++) of[fill[pose[j]]++] = (int)j; }
   if (D == 6) for (size_t i = 0; i < N; i++) memcpy(&qi[i * 4], h->qinit.at(h->ids[i]).data(), 32);
-  const size_t nbe = (h->ea.size() + 127) / 128, nbg = (h->gp_pose.size() + 127) / 128, nbk = (K + 127) / 128;
   PCK(h->d_ak_pose.alloc(K)); PCK(h->d_ak_of.alloc(K)); PCK(h->d_ak_ptr.alloc(N + 1)); PCK(h->d_ak_yr.alloc(K * D)); PCK(h->d_ak_yl.alloc(K * D));
   PCK(h->d_ak_qinit.alloc(N * 4)); PCK(h->d_ak_lin[0].alloc(K * (D + D * D))); PCK(h->d_ak_lin[1].alloc(K * (D + D * D)));
-  PCK(h->d_cost_part.alloc(nbe + nbg + nbk + 1));
   if (K) {
     PCK(cudaMemcpyAsync(h->d_ak_pose.p, pose.data(), K * 4, cudaMemcpyHostToDevice, h->stream));
     PCK(cudaMemcpyAsync(h->d_ak_of.p, of.data(), K * 4, cudaMemcpyHostToDevice, h->stream));
@@ -1602,11 +1295,8 @@ static int arock_sync(d2pgo_handle *h) {
   PCK(cudaMemcpyAsync(h->d_ak_ptr.p, ptr.data(), (N + 1) * 4, cudaMemcpyHostToDevice, h->stream));
   PCK(cudaMemcpyAsync(h->d_ak_qinit.p, qi.data(), N * 32, cudaMemcpyHostToDevice, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
-  // the CG graphs hold the dual count and these buffers by value: capture them again when either changed
-  const void *key[4] = {h->d_ak_ptr.p, h->d_ak_of.p, h->d_ak_lin[0].p, h->d_ak_lin[1].p};
-  if ((int)K != h->ak_n || memcmp(key, h->ak_key, sizeof key)) { pgo_drop_graphs(h); memcpy(h->ak_key, key, sizeof key); }
   h->ak_n = (int)K;
-  return 0;
+  return pgo_alloc_cost_part(h);
 }
 
 // every pose at d_x[0] in dual coordinates, [N][D] on the host
@@ -1625,10 +1315,10 @@ static int arock_coords(d2pgo_handle *h, std::vector<double> &out) {
 
 // every pose needs an owner (and, 6-DoF, a q_init) before the table can be built
 static int arock_check_poses(d2pgo_handle *h, const char *what) {
-  if (!h->arock) return arock_fail(h, 5, std::string(what) + ": the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (!h->arock) return pgo_fail(h, 5, std::string(what) + ": the handle is not in ARock mode (d2pgo_arock_enable)");
   for (int64_t id : h->ids) {
-    if (!h->owner.count(id)) return arock_fail(h, 2, std::string(what) + ": pose id " + std::to_string(id) + " has no owner agent (d2pgo_arock_enable)");
-    if (h->dof == 6 && !h->qinit.count(id)) return arock_fail(h, 2, std::string(what) + ": pose id " + std::to_string(id) + " has no q_init (d2pgo_arock_enable)");
+    if (!h->owner.count(id)) return pgo_fail(h, 2, std::string(what) + ": pose id " + std::to_string(id) + " has no owner agent (d2pgo_arock_enable)");
+    if (h->dof == 6 && !h->qinit.count(id)) return pgo_fail(h, 2, std::string(what) + ": pose id " + std::to_string(id) + " has no q_init (d2pgo_arock_enable)");
   }
   return 0;
 }
@@ -1644,18 +1334,18 @@ int d2pgo_default_arock_config(d2pgo_arock_config *c) {
 
 int d2pgo_arock_enable(d2pgo_handle *h, const d2pgo_arock_config *cfg, int32_t n, const int64_t *ids, const int32_t *owner, const double *q_init4) {
   if (!h) return 1;
-  if (!cfg || n < 0 || (n > 0 && (!ids || !owner))) return arock_fail(h, 1, "arock_enable: null argument or negative count");
-  if (h->comm) return arock_fail(h, 5, "arock_enable: the handle has a communicator (edge sharding and ARock are different splits of the graph)");
+  if (!cfg || n < 0 || (n > 0 && (!ids || !owner))) return pgo_fail(h, 1, "arock_enable: null argument or negative count");
+  if (h->comm) return pgo_fail(h, 5, "arock_enable: the handle has a communicator (edge sharding and ARock are different splits of the graph)");
   if (!(std::isfinite(cfg->rho_frame_T) && cfg->rho_frame_T >= 0.0 && std::isfinite(cfg->rho_frame_theta) && cfg->rho_frame_theta >= 0.0 && std::isfinite(cfg->eta_k)))
-    return arock_fail(h, 2, "arock_enable: rho_frame_T, rho_frame_theta must be finite and non-negative, eta_k finite");
+    return pgo_fail(h, 2, "arock_enable: rho_frame_T, rho_frame_theta must be finite and non-negative, eta_k finite");
   std::vector<std::array<double, 4>> q(n);
   for (int k = 0; k < n; k++) {
     auto it = h->index.find(ids[k]);
-    if (it == h->index.end()) return arock_fail(h, 2, "arock_enable: unknown pose id " + std::to_string(ids[k]));
+    if (it == h->index.end()) return pgo_fail(h, 2, "arock_enable: unknown pose id " + std::to_string(ids[k]));
     const double *src = q_init4 ? q_init4 + (size_t)k * 4 : &h->poses[(size_t)it->second * 8 + 3];
     if (h->dof == 6) {
       const double s2 = src[0] * src[0] + src[1] * src[1] + src[2] * src[2] + src[3] * src[3];
-      if (!all_finite(src, 4) || !(s2 > 0.0)) return arock_fail(h, 2, "arock_enable: pose id " + std::to_string(ids[k]) + ": non-finite or zero q_init");
+      if (!all_finite(src, 4) || !(s2 > 0.0)) return pgo_fail(h, 2, "arock_enable: pose id " + std::to_string(ids[k]) + ": non-finite or zero q_init");
       const double s = 1.0 / std::sqrt(s2);
       q[k] = {src[0] * s, src[1] * s, src[2] * s, src[3] * s};
     }
@@ -1668,20 +1358,20 @@ int d2pgo_arock_enable(d2pgo_handle *h, const d2pgo_arock_config *cfg, int32_t n
 
 int d2pgo_arock_receive(d2pgo_handle *h, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int32_t dim, const double *duals) {
   if (!h) return 1;
-  if (!h->arock) return arock_fail(h, 5, "arock_receive: the handle is not in ARock mode (d2pgo_arock_enable)");
-  if (n < 0 || (n > 0 && (!frame_ids || !duals))) return arock_fail(h, 1, "arock_receive: null argument or negative count");
-  if (dim != h->dof) return arock_fail(h, 2, "arock_receive: duals of dimension " + std::to_string(dim) + " on a handle with pose_dof = " + std::to_string(h->dof));
-  if (sender == h->acfg.self_id) return arock_fail(h, 2, "arock_receive: a message from this agent itself (self_id " + std::to_string(sender) + ")");
-  if (!all_finite(duals, (size_t)n * dim)) return arock_fail(h, 2, "arock_receive: non-finite dual");
+  if (!h->arock) return pgo_fail(h, 5, "arock_receive: the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (n < 0 || (n > 0 && (!frame_ids || !duals))) return pgo_fail(h, 1, "arock_receive: null argument or negative count");
+  if (dim != h->dof) return pgo_fail(h, 2, "arock_receive: duals of dimension " + std::to_string(dim) + " on a handle with pose_dof = " + std::to_string(h->dof));
+  if (sender == h->acfg.self_id) return pgo_fail(h, 2, "arock_receive: a message from this agent itself (self_id " + std::to_string(sender) + ")");
+  if (!all_finite(duals, (size_t)n * dim)) return pgo_fail(h, 2, "arock_receive: non-finite dual");
   std::unordered_map<int64_t, int> seen;
-  for (int k = 0; k < n; k++) if (!seen.emplace(frame_ids[k], k).second) return arock_fail(h, 2, "arock_receive: frame id " + std::to_string(frame_ids[k]) + " twice in one message");
+  for (int k = 0; k < n; k++) if (!seen.emplace(frame_ids[k], k).second) return pgo_fail(h, 2, "arock_receive: frame id " + std::to_string(frame_ids[k]) + " twice in one message");
   h->inbox.push_back(d2pgo_handle::Msg{sender, target, std::vector<int64_t>(frame_ids, frame_ids + n), std::vector<double>(duals, duals + (size_t)n * dim)});
   return 0;
 }
 
 int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h) return 1;
-  if (h->ids.empty()) return arock_fail(h, 1, "arock_step: no poses");
+  if (h->ids.empty()) return pgo_fail(h, 1, "arock_step: no poses");
   if (int rc = arock_check_poses(h, "arock_step")) return rc;
   cudaSetDevice(h->cfg.device);
   int rc;
@@ -1718,11 +1408,8 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
   }
   // 3. setDualStateFactors + solveLocalStep: the LM solve with the proximal terms towards y_r
   if (created && (rc = arock_sync(h))) return rc;
-  if ((rc = D == 4 ? pgo_solve<PgoEdge4, false, true>(h, rep)
-                   : h->gp_pose.empty() ? pgo_solve<PgoEdge6, false, true>(h, rep) : pgo_solve<PgoEdge6, true, true>(h, rep))) return rc;
-  // 4. updateDualStates at the solved poses.  pgo_solve leaves them in buffer 0, by a device-to-device cudaMemcpy when they
-  // were in buffer 1: that copy is not ordered with this handle's non-blocking stream, so wait for it.
-  PCK(cudaStreamSynchronize(0));
+  if ((rc = D == 4 ? pgo_solve<PgoEdge4>(h, rep, true) : pgo_solve<PgoEdge6>(h, rep, true))) return rc;
+  // 4. updateDualStates at the solved poses, which pgo_solve leaves in buffer 0
   const PgoArockDev ak = pgo_arock_view(h, 0);
   if (ak.n_dual > 0) {
     const int nb = (ak.n_dual + 127) / 128;
@@ -1740,25 +1427,25 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
 
 int d2pgo_arock_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out) {
   if (!h) return 1;
-  if (!h->arock) return arock_fail(h, 5, "arock_neighbours: the handle is not in ARock mode (d2pgo_arock_enable)");
-  if (!n_out || max_n < 0 || (max_n > 0 && !ids_out)) return arock_fail(h, 1, "arock_neighbours: null argument or negative count");
+  if (!h->arock) return pgo_fail(h, 5, "arock_neighbours: the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (!n_out || max_n < 0 || (max_n > 0 && !ids_out)) return pgo_fail(h, 1, "arock_neighbours: null argument or negative count");
   std::vector<int32_t> nb;
   for (const auto &kv : h->duals) if (nb.empty() || nb.back() != kv.first.first) nb.push_back(kv.first.first);
   *n_out = (int32_t)nb.size();
-  if ((int32_t)nb.size() > max_n) return arock_fail(h, 2, "arock_neighbours: room for " + std::to_string(max_n) + " ids, " + std::to_string(nb.size()) + " needed");
+  if ((int32_t)nb.size() > max_n) return pgo_fail(h, 2, "arock_neighbours: room for " + std::to_string(max_n) + " ids, " + std::to_string(nb.size()) + " needed");
   std::copy(nb.begin(), nb.end(), ids_out);
   return 0;
 }
 
 int d2pgo_arock_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t *n_out, int64_t *frame_ids, double *local_out, double *remote_out) {
   if (!h) return 1;
-  if (!h->arock) return arock_fail(h, 5, "arock_duals: the handle is not in ARock mode (d2pgo_arock_enable)");
-  if (!n_out || max_n < 0 || (max_n > 0 && (!frame_ids || !local_out))) return arock_fail(h, 1, "arock_duals: null argument or negative count");
+  if (!h->arock) return pgo_fail(h, 5, "arock_duals: the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (!n_out || max_n < 0 || (max_n > 0 && (!frame_ids || !local_out))) return pgo_fail(h, 1, "arock_duals: null argument or negative count");
   const int D = h->dof;
   auto lo = h->duals.lower_bound(std::make_pair(neighbour, INT64_MIN)), hi = h->duals.upper_bound(std::make_pair(neighbour, INT64_MAX));
   const int32_t cnt = (int32_t)std::distance(lo, hi);
   *n_out = cnt;
-  if (cnt > max_n) return arock_fail(h, 2, "arock_duals: room for " + std::to_string(max_n) + " duals, " + std::to_string(cnt) + " needed");
+  if (cnt > max_n) return pgo_fail(h, 2, "arock_duals: room for " + std::to_string(max_n) + " duals, " + std::to_string(cnt) + " needed");
   int k = 0;
   for (auto it = lo; it != hi; ++it, ++k) {
     frame_ids[k] = it->first.second;
@@ -1772,8 +1459,8 @@ int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
   if (!h) return 1;
   if (int rc = arock_check_poses(h, "debug_arock_terms")) return rc;
   const size_t K = h->duals.size(), D = h->dof, W = D + D * D;
-  if ((size_t)out_doubles < K * W) return arock_fail(h, 2, "debug_arock_terms: buffer too small: " + std::to_string(K * W) + " doubles needed");
-  if (!out && K) return arock_fail(h, 1, "debug_arock_terms: null argument");
+  if ((size_t)out_doubles < K * W) return pgo_fail(h, 2, "debug_arock_terms: buffer too small: " + std::to_string(K * W) + " doubles needed");
+  if (!out && K) return pgo_fail(h, 1, "debug_arock_terms: null argument");
   if (!K) return 0;
   cudaSetDevice(h->cfg.device);
   int rc;
@@ -1795,17 +1482,18 @@ int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
 }  // extern "C"
 
 // ---- sparse Cholesky (d2pgo_set_linear_solver) host side
-template <class P, bool GRAV, bool ARK>
-static int pgo_exact_step(d2pgo_handle *h, double lambda, double *out) {
+template <class P>
+static int pgo_exact_step(d2pgo_handle *h, double lambda, bool ark, double *out) {
   int rc;
   if ((rc = pgo_chol_prepare(h))) return rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
-  if (ARK && (rc = arock_sync(h))) return rc;
+  if (ark && (rc = arock_sync(h))) return rc;
   double cost;
-  if ((rc = pgo_linearize<P, GRAV, ARK>(h, 0, 1, &cost))) return rc;
+  if ((rc = pgo_linearize<P>(h, 0, 1, !h->gp_pose.empty(), ark, &cost))) return rc;
   bool failed = false;
   if ((rc = pgo_chol_step(h, 0, lambda, &failed))) return rc;
-  PCK(cudaMemcpy(out, h->d_dx.p, h->ids.size() * (size_t)P::D * 8, cudaMemcpyDeviceToHost));
+  PCK(cudaMemcpyAsync(out, h->d_dx.p, h->ids.size() * (size_t)P::D * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
   if (failed) { h->err = "debug_exact_step: the factorisation met a non-positive or non-finite pivot"; return 6; }
   return 0;
 }
@@ -1825,8 +1513,7 @@ int d2pgo_set_linear_solver(d2pgo_handle *h, int32_t kind) {
   if (kind == D2PGO_LINEAR_PCG && h->chol) {   // the factor's tables, fronts and graphs are not needed by PCG
     cudaSetDevice(h->cfg.device);
     cudaStreamSynchronize(h->stream);
-    delete h->chol;
-    h->chol = nullptr;
+    h->chol.reset();
   }
   h->linear_solver = kind;
   return 0;
@@ -1851,10 +1538,7 @@ int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64
   if (h->comm) { h->err = "debug_exact_step: the handle has a communicator"; return 5; }
   if (h->arock) if (int rc = arock_check_poses(h, "debug_exact_step")) return rc;
   cudaSetDevice(h->cfg.device);
-  const bool ark = h->arock, grav = !h->gp_pose.empty();
-  if (h->dof == 4) return ark ? pgo_exact_step<PgoEdge4, false, true>(h, lambda, dx_out) : pgo_exact_step<PgoEdge4, false, false>(h, lambda, dx_out);
-  if (grav) return ark ? pgo_exact_step<PgoEdge6, true, true>(h, lambda, dx_out) : pgo_exact_step<PgoEdge6, true, false>(h, lambda, dx_out);
-  return ark ? pgo_exact_step<PgoEdge6, false, true>(h, lambda, dx_out) : pgo_exact_step<PgoEdge6, false, false>(h, lambda, dx_out);
+  return h->dof == 4 ? pgo_exact_step<PgoEdge4>(h, lambda, h->arock, dx_out) : pgo_exact_step<PgoEdge6>(h, lambda, h->arock, dx_out);
 }
 
 int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out, int32_t max_pairs, int32_t *n_pairs_out,
@@ -1864,7 +1548,7 @@ int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out
     h->err = "debug_cholesky_system: null argument or negative count";
     return 1;
   }
-  const d2pgo_chol::Numeric *c = h->chol;
+  const d2pgo_chol::Numeric *c = h->chol.get();
   if (!c || !c->has_system || c->sym.D != h->dof || c->sym.fixed != h->fixed || c->sym.ea != h->ea || c->sym.eb != h->eb) {
     h->err = "debug_cholesky_system: no sparse-Cholesky step on the handle's current structure";
     return 5;
@@ -1877,174 +1561,7 @@ int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out
 
 }  // extern "C"
 
-// ---- PCM host side
-static int pcm_fail(d2pgo_handle *h, int rc, const std::string &msg) { h->err = msg; return rc; }
-
-// FMC on groups already in h->pcm (g_loop, g_word, adj): degrees, one clique CTA per group; inlier flags by slot, stats per group
-static int pcm_run_clique(d2pgo_handle *h, int G, int n, int max_w) {
-  PcmBufs &P = h->pcm;
-  PCK(P.deg.alloc(n)); PCK(P.inlier.alloc(n)); PCK(P.stats.alloc(2 * (size_t)G));
-  if (n > 0) k_pcm_degree<<<(n + 255) / 256, 256, 0, h->stream>>>(G, P.g_loop.p, P.g_word.p, P.adj.p, P.deg.p);
-  if (G > 0) k_pcm_clique<<<G, kPcmWarps * 32, (size_t)(1 + kPcmWarps) * max_w * 4, h->stream>>>(P.g_loop.p, P.g_word.p, P.adj.p, P.deg.p, P.inlier.p, P.stats.p);
-  PCK(cudaGetLastError());
-  return 0;
-}
-
-extern "C" {
-
-int d2pgo_default_pcm_config(d2pgo_pcm_config *c) {
-  if (!c) return 1;
-  memset(c, 0, sizeof *c);
-  c->pcm_thres = 1.635; c->pos_covariance_per_meter = 4e-3; c->yaw_covariance_per_meter = 4e-5;
-  return 0;
-}
-
-int d2pgo_pcm(d2pgo_handle *h, const d2pgo_pcm_config *cfg, int32_t n_frames, const int64_t *frame_ids, const int32_t *frame_agent, const double *ego_poses7,
-              int32_t n_loops, const int64_t *kf_a, const int64_t *kf_b, const double *rel7, const double *sqrt_info36, uint8_t *inlier_out, d2pgo_pcm_report *rep) {
-  if (!h) return 1;
-  if (!cfg || n_frames < 0 || n_loops < 0 || (n_frames && (!frame_ids || !frame_agent || !ego_poses7)) ||
-      (n_loops && (!kf_a || !kf_b || !rel7 || !sqrt_info36 || !inlier_out)))
-    return pcm_fail(h, 1, "pcm: null argument or negative count");
-  // the reference keeps pcm_thres in a float (SwarmLocalOutlierRejectionParams, d2pgo_config.h); the test is smd < that float
-  const double thr = (double)(float)cfg->pcm_thres;
-  if (!(std::isfinite(thr) && thr > 0.0)) return pcm_fail(h, 2, "pcm: pcm_thres must be finite and positive");
-  if (!(std::isfinite(cfg->pos_covariance_per_meter) && cfg->pos_covariance_per_meter >= 0.0 && std::isfinite(cfg->yaw_covariance_per_meter) && cfg->yaw_covariance_per_meter >= 0.0))
-    return pcm_fail(h, 2, "pcm: covariance rates must be finite and non-negative");
-  cudaSetDevice(h->cfg.device);
-  PcmBufs &P = h->pcm;
-  P.n_smd = -1;
-  // keyframes -> (drone, position in its trajectory = order of appearance)
-  std::unordered_map<int64_t, int> fidx;
-  std::unordered_map<int32_t, int> drone_of;
-  std::vector<std::vector<int>> trajs;
-  for (int f = 0; f < n_frames; f++) {
-    if (!fidx.emplace(frame_ids[f], f).second) return pcm_fail(h, 3, "pcm: duplicate keyframe id " + std::to_string(frame_ids[f]));
-    auto it = drone_of.emplace(frame_agent[f], (int)trajs.size());
-    if (it.second) trajs.emplace_back();
-    trajs[it.first->second].push_back(f);
-  }
-  // groups: unordered drone pairs, numbered by first appearance; a group's loops keep their input order
-  std::unordered_map<uint64_t, int> gid;
-  std::vector<int> lg(n_loops), la(n_loops), lb(n_loops), gsize;
-  std::vector<uint64_t> gkey;
-  for (int e = 0; e < n_loops; e++) {
-    auto a = fidx.find(kf_a[e]), b = fidx.find(kf_b[e]);
-    if (a == fidx.end() || b == fidx.end())
-      return pcm_fail(h, 3, "pcm: loop " + std::to_string(e) + " names unknown keyframe id " + std::to_string(a == fidx.end() ? kf_a[e] : kf_b[e]));
-    la[e] = a->second; lb[e] = b->second;
-    const uint32_t x = (uint32_t)frame_agent[la[e]], y = (uint32_t)frame_agent[lb[e]];
-    const uint64_t key = (uint64_t)std::min(x, y) << 32 | std::max(x, y);
-    auto it = gid.emplace(key, (int)gsize.size());
-    if (it.second) { gsize.push_back(0); gkey.push_back(key); }
-    lg[e] = it.first->second; gsize[lg[e]]++;
-  }
-  const int G = (int)gsize.size();
-  std::vector<int> g_loop(G + 1, 0); std::vector<long long> g_word(G + 1, 0), g_smd(G + 1, 0);
-  int max_w = 1;
-  for (int g = 0; g < G; g++) {
-    const long long L = gsize[g], W = (L + 31) / 32;
-    if (L > kPcmMaxGroup)
-      return pcm_fail(h, 4, "pcm: the group of drones " + std::to_string((int32_t)(gkey[g] >> 32)) + " and " + std::to_string((int32_t)(gkey[g] & 0xffffffffu)) + " has " +
-                                std::to_string(L) + " loops; at most " + std::to_string(kPcmMaxGroup) + " are supported");
-    g_loop[g + 1] = g_loop[g] + (int)L; g_word[g + 1] = g_word[g] + L * W; g_smd[g + 1] = g_smd[g] + L * (L - 1) / 2;
-    max_w = std::max(max_w, (int)W);
-  }
-  std::vector<int> src(n_loops), sfa(n_loops), sfb(n_loops), fill(g_loop.begin(), g_loop.end() - 1);
-  std::vector<unsigned char> flip(n_loops);
-  for (int e = 0; e < n_loops; e++) {
-    const int s = fill[lg[e]]++;
-    src[s] = e; sfa[s] = la[e]; sfb[s] = lb[e]; flip[s] = frame_agent[la[e]] > frame_agent[lb[e]];
-  }
-  std::vector<int> traj_ptr(1, 0), traj;
-  for (auto &t : trajs) { traj.insert(traj.end(), t.begin(), t.end()); traj_ptr.push_back((int)traj.size()); }
-  std::vector<double> ego((size_t)n_frames * 8, 0.0);
-  for (int f = 0; f < n_frames; f++) memcpy(&ego[(size_t)f * 8], ego_poses7 + (size_t)f * 7, 56);
-  const size_t n = n_loops, F = n_frames;
-  PCK(P.g_loop.alloc(G + 1)); PCK(P.g_word.alloc(G + 1)); PCK(P.g_smd.alloc(G + 1)); PCK(P.fa.alloc(n)); PCK(P.fb.alloc(n)); PCK(P.src.alloc(n)); PCK(P.flip.alloc(n));
-  PCK(P.rel_in.alloc(n * 7)); PCK(P.sqrt_in.alloc(n * 36)); PCK(P.rel.alloc(n * 8)); PCK(P.cov.alloc(n * 21)); PCK(P.ego.alloc(F * 8)); PCK(P.path.alloc(F));
-  PCK(P.traj_ptr.alloc(traj_ptr.size())); PCK(P.traj.alloc(F)); PCK(P.adj.alloc(g_word[G])); PCK(P.smd.alloc(g_smd[G]));
-  if (!P.ev_pair) PCK(cudaEventCreate(&P.ev_pair));
-  PCK(cudaMemcpyAsync(P.g_loop.p, g_loop.data(), (G + 1) * 4, cudaMemcpyHostToDevice, h->stream));
-  PCK(cudaMemcpyAsync(P.g_word.p, g_word.data(), (G + 1) * 8, cudaMemcpyHostToDevice, h->stream));
-  PCK(cudaMemcpyAsync(P.g_smd.p, g_smd.data(), (G + 1) * 8, cudaMemcpyHostToDevice, h->stream));
-  PCK(cudaMemcpyAsync(P.traj_ptr.p, traj_ptr.data(), traj_ptr.size() * 4, cudaMemcpyHostToDevice, h->stream));
-  if (F) {
-    PCK(cudaMemcpyAsync(P.traj.p, traj.data(), F * 4, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(P.ego.p, ego.data(), F * 64, cudaMemcpyHostToDevice, h->stream));
-  }
-  if (n) {
-    PCK(cudaMemcpyAsync(P.fa.p, sfa.data(), n * 4, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(P.fb.p, sfb.data(), n * 4, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(P.src.p, src.data(), n * 4, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(P.flip.p, flip.data(), n, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(P.rel_in.p, rel7, n * 56, cudaMemcpyHostToDevice, h->stream)); PCK(cudaMemcpyAsync(P.sqrt_in.p, sqrt_info36, n * 288, cudaMemcpyHostToDevice, h->stream));
-  }
-  PcmDev d;
-  d.g_loop = P.g_loop.p; d.g_word = P.g_word.p; d.g_smd = P.g_smd.p; d.fa = P.fa.p; d.fb = P.fb.p; d.flip = P.flip.p; d.rel = P.rel.p; d.cov = P.cov.p;
-  d.ego = P.ego.p; d.path = P.path.p; d.adj = P.adj.p; d.deg = P.deg.p; d.smd = P.smd.p;
-  d.is4 = h->dof == 4; d.thr = thr; d.pos_cov = cfg->pos_covariance_per_meter; d.yaw_cov = cfg->yaw_covariance_per_meter;
-  PCK(cudaEventRecord(h->ev0, h->stream));
-  if (!trajs.empty()) k_pcm_path<<<((int)trajs.size() * 32 + 255) / 256, 256, 0, h->stream>>>((int)trajs.size(), P.traj_ptr.p, P.traj.p, P.ego.p, P.path.p);
-  if (n) {
-    k_pcm_loop<<<((int)n + 127) / 128, 128, 0, h->stream>>>((int)n, P.src.p, P.rel_in.p, P.sqrt_in.p, P.rel.p, P.cov.p);
-    const long long words = g_word[G];
-    k_pcm_pairs<<<(unsigned)((words * 32 + 255) / 256), 256, 0, h->stream>>>(d, G, words);
-  }
-  PCK(cudaGetLastError());
-  PCK(cudaEventRecord(P.ev_pair, h->stream));
-  if (int rc = pcm_run_clique(h, G, (int)n, max_w)) return rc;
-  PCK(cudaEventRecord(h->ev1, h->stream));
-  std::vector<unsigned char> inl(n);
-  std::vector<long long> stats(2 * (size_t)G);
-  if (n) PCK(cudaMemcpyAsync(inl.data(), P.inlier.p, n, cudaMemcpyDeviceToHost, h->stream));
-  if (G) PCK(cudaMemcpyAsync(stats.data(), P.stats.p, 16 * (size_t)G, cudaMemcpyDeviceToHost, h->stream));
-  PCK(cudaStreamSynchronize(h->stream));
-  d2pgo_pcm_report R; memset(&R, 0, sizeof R);
-  for (size_t s = 0; s < n; s++) { inlier_out[src[s]] = inl[s]; R.inliers += inl[s]; }
-  for (int g = 0; g < G; g++) { R.consistent_pairs += stats[2 * g] / 2; R.clique_rounds += stats[2 * g + 1]; }
-  R.groups = G; R.pairs_tested = g_smd[G];
-  float ms = 0, mp = 0;
-  cudaEventElapsedTime(&ms, h->ev0, h->ev1); cudaEventElapsedTime(&mp, h->ev0, P.ev_pair);
-  R.device_ms = ms; R.pair_ms = mp; R.clique_ms = ms - mp;
-  P.n_smd = g_smd[G];
-  if (rep) *rep = R;
-  return 0;
-}
-
-int d2pgo_debug_pcm_smd(d2pgo_handle *h, double *out, int64_t out_doubles) {
-  if (!h) return 1;
-  PcmBufs &P = h->pcm;
-  if (P.n_smd < 0) return pcm_fail(h, 2, "debug_pcm_smd: no successful d2pgo_pcm call on this handle");
-  if (out_doubles < P.n_smd) return pcm_fail(h, 2, "debug_pcm_smd: buffer too small: " + std::to_string(P.n_smd) + " doubles needed");
-  cudaSetDevice(h->cfg.device);
-  if (P.n_smd) PCK(cudaMemcpy(out, P.smd.p, (size_t)P.n_smd * 8, cudaMemcpyDeviceToHost));
-  return 0;
-}
-
-int d2pgo_debug_pcm_clique(d2pgo_handle *h, int32_t n, const uint32_t *adj, uint8_t *member_out, int32_t *size_out) {
-  if (!h) return 1;
-  if (n < 0 || (n && (!adj || !member_out))) return pcm_fail(h, 1, "debug_pcm_clique: null argument or negative count");
-  if (n > kPcmMaxGroup) return pcm_fail(h, 4, "debug_pcm_clique: at most " + std::to_string(kPcmMaxGroup) + " vertices are supported");
-  cudaSetDevice(h->cfg.device);
-  PcmBufs &P = h->pcm;
-  const long long W = (n + 31) / 32;
-  const int g_loop[2] = {0, n}; const long long g_word[2] = {0, n * W};
-  P.n_smd = -1;   // the buffers below are shared with d2pgo_pcm
-  PCK(P.g_loop.alloc(2)); PCK(P.g_word.alloc(2)); PCK(P.adj.alloc(n * W));
-  PCK(cudaMemcpyAsync(P.g_loop.p, g_loop, 8, cudaMemcpyHostToDevice, h->stream));
-  PCK(cudaMemcpyAsync(P.g_word.p, g_word, 16, cudaMemcpyHostToDevice, h->stream));
-  if (n) PCK(cudaMemcpyAsync(P.adj.p, adj, (size_t)(n * W) * 4, cudaMemcpyHostToDevice, h->stream));
-  if (int rc = pcm_run_clique(h, n ? 1 : 0, n, (int)std::max(W, 1LL))) return rc;
-  if (n) PCK(cudaMemcpyAsync(member_out, P.inlier.p, n, cudaMemcpyDeviceToHost, h->stream));
-  PCK(cudaStreamSynchronize(h->stream));
-  int c = 0;
-  for (int k = 0; k < n; k++) c += member_out[k];
-  if (size_out) *size_out = c;
-  return 0;
-}
-
-}  // extern "C"
-
 // ---- chordal rotation initialisation host side (d2pgo_rot_init)
-static int rot_fail(d2pgo_handle *h, int rc, const std::string &msg) { h->err = "rot_init: " + msg; return rc; }
 
 // Eigen's toRotationMatrix polynomial (q2R of d2ba_math.cuh) on the host, row-major, of the normalised quaternion (Swarm::Pose
 // normalises its attitude)
@@ -2062,47 +1579,24 @@ static int rot_find(std::vector<int> &uf, int i) {
   return i;
 }
 
-// one row system on the inner handle r (poses and edges already set): upload, linearise at x = 0 rows, one undamped
-// Gauss-Newton step by the block-Jacobi PCG of d2pgo_solve, x + dx into r->d_x[1]
-static int rot_solve_row(d2pgo_handle *r, double tol2, int max_it, int *iters, double *residual) {
+// one row system on the inner handle h (poses and edges already set; errors are reported there): upload, linearise at
+// x = 0 rows, one undamped Gauss-Newton step by the block-Jacobi PCG of d2pgo_solve, x + dx into h->d_x[1]
+static int rot_solve_row(d2pgo_handle *h, double tol2, int max_it, int *iters, double *residual) {
   typedef PgoRotRow P;
   int rc;
-  if ((rc = pgo_upload(r))) return rc;
-  d2pgo_handle *h = r;   // PCK reports into the inner handle
-  PgoDev d = pgo_view(r, 0);
-  const PgoPriorDev pr = pgo_prior_view(r, 0);
-  const int gp = d.nbp, ge = (d.n_edge + 127) / 128;
-  if (d.n_edge > 0) k_pgo_lin<P><<<ge, 128, 0, r->stream>>>(d, r->d_cost_part.p, 1);
-  k_pgo_gD<P, false><<<gp, 128, 0, r->stream>>>(d, r->d_g[0].p, r->d_D[0].p, pr);
-  k_pgo_precond<P><<<gp, 128, 0, r->stream>>>(d, r->d_D[0].p, 0.0);
-  k_pgo_cg_init<P><<<gp, 128, 0, r->stream>>>(d, r->d_g[0].p);
-  k_pgo_cg_init2<<<1, 128, 0, r->stream>>>(d);
+  if ((rc = pgo_upload(h))) return rc;
+  const PgoDev d = pgo_view(h, 0);
+  const PgoPriorDev pr = pgo_prior_view(h, 0);
+  if (d.n_edge > 0) k_pgo_lin<P><<<(d.n_edge + 127) / 128, 128, 0, h->stream>>>(d, h->d_cost_part.p, 1);
+  k_pgo_gD<P, false><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[0].p, h->d_D[0].p, pr);
   PgoScalars s; memset(&s, 0, sizeof s);
-  for (int k = 0; k < max_it; k += kCgChunk) {
-    if (!r->cg_graph[0]) {
-      cudaGraph_t g;
-      PCK(cudaStreamBeginCapture(r->stream, cudaStreamCaptureModeThreadLocal));
-      for (int c = 0; c < kCgChunk; c++) {
-        const int par = c & 1;
-        if (d.n_edge > 0) k_pgo_cg_edge<P><<<ge, 128, 0, r->stream>>>(d, par, tol2);
-        k_pgo_cg_pose<P, false, false><<<gp, 128, 0, r->stream>>>(d, par, tol2, pr);
-        k_pgo_cg_step<P><<<gp, 128, 0, r->stream>>>(d, par, tol2);
-      }
-      PCK(cudaStreamEndCapture(r->stream, &g));
-      PCK(cudaGraphInstantiate(&r->cg_graph[0], g, 0));
-      cudaGraphDestroy(g);
-    }
-    PCK(cudaGraphLaunch(r->cg_graph[0], r->stream));
-    PCK(cudaMemcpyAsync(&s, r->d_s.p, sizeof s, cudaMemcpyDeviceToHost, r->stream));
-    PCK(cudaStreamSynchronize(r->stream));
-    if (s.done) break;
-  }
-  k_pgo_retract<P><<<gp, 128, 0, r->stream>>>(d, r->d_x[1].p);
+  if ((rc = pgo_pcg<P>(h, 0, 0.0, tol2, max_it, false, false, &s))) return rc;
+  k_pgo_retract<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_x[1].p);
   // the residual of the last CG update: its r.r partials sit in the parity slot of the last iteration (cg_init: slot 1)
   std::vector<double> part(d.nbp);
   const int slot = s.iters == 0 ? 1 : (s.iters - 1) & 1;
-  PCK(cudaMemcpyAsync(part.data(), d.rr_part + (size_t)slot * d.nbp, (size_t)d.nbp * 8, cudaMemcpyDeviceToHost, r->stream));
-  PCK(cudaStreamSynchronize(r->stream));
+  PCK(cudaMemcpyAsync(part.data(), d.rr_part + (size_t)slot * d.nbp, (size_t)d.nbp * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
   double rr = 0.0;
   for (double v : part) rr += v;
   *iters = s.iters;
@@ -2122,14 +1616,14 @@ int d2pgo_default_rot_init_config(d2pgo_rot_init_config *c) {
 int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids, const double *ego_poses7,
                    d2pgo_rot_init_report *report) {
   if (!h) return 1;
-  if (!cfg || n_ego < 0 || (n_ego > 0 && (!ego_ids || !ego_poses7))) return rot_fail(h, 1, "null argument or negative count");
-  if (h->dof != 6) return rot_fail(h, 5, "the handle was created with pose_dof = 4; rotation initialisation acts on 6-DoF poses");
-  if (h->comm) return rot_fail(h, 5, "a communicator is attached (edge-sharded rotation initialisation is not supported)");
-  if (h->arock) return rot_fail(h, 5, "the handle is in ARock mode (d2pgo runs the distributed RotationInitARock there)");
-  if (h->ids.empty()) return rot_fail(h, 1, "the handle has no poses");
+  if (!cfg || n_ego < 0 || (n_ego > 0 && (!ego_ids || !ego_poses7))) return pgo_fail(h, 1, "rot_init: null argument or negative count");
+  if (h->dof != 6) return pgo_fail(h, 5, "rot_init: the handle was created with pose_dof = 4; rotation initialisation acts on 6-DoF poses");
+  if (h->comm) return pgo_fail(h, 5, "rot_init: a communicator is attached (edge-sharded rotation initialisation is not supported)");
+  if (h->arock) return pgo_fail(h, 5, "rot_init: the handle is in ARock mode (d2pgo runs the distributed RotationInitARock there)");
+  if (h->ids.empty()) return pgo_fail(h, 1, "rot_init: the handle has no poses");
   if (!(std::isfinite(cfg->pcg_tolerance) && cfg->pcg_tolerance >= 0.0) || cfg->pcg_max_iterations < 0 ||
       (cfg->enable_gravity_prior && !std::isfinite(cfg->gravity_sqrt_info)))
-    return rot_fail(h, 2, "non-finite or negative pcg_tolerance, gravity_sqrt_info or pcg_max_iterations");
+    return pgo_fail(h, 2, "rot_init: non-finite or negative pcg_tolerance, gravity_sqrt_info or pcg_max_iterations");
   const int N = (int)h->ids.size(), E = (int)h->ea.size();
   const bool grav = cfg->enable_gravity_prior != 0;
   // the ego attitudes by pose index (gravity rows only)
@@ -2137,12 +1631,12 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
   for (int k = 0; k < n_ego; k++) {
     const std::string which = "ego pose " + std::to_string(k) + " (id " + std::to_string(ego_ids[k]) + ")";
     auto it = h->index.find(ego_ids[k]);
-    if (it == h->index.end()) return rot_fail(h, 2, which + ": unknown pose id");
-    if (ego_of[it->second] >= 0) return rot_fail(h, 2, which + ": duplicate id");
+    if (it == h->index.end()) return pgo_fail(h, 2, "rot_init: " + which + ": unknown pose id");
+    if (ego_of[it->second] >= 0) return pgo_fail(h, 2, "rot_init: " + which + ": duplicate id");
     ego_of[it->second] = k;
-    if (!all_finite(ego_poses7 + (size_t)k * 7, 7)) return rot_fail(h, 2, which + ": non-finite value");
+    if (!all_finite(ego_poses7 + (size_t)k * 7, 7)) return pgo_fail(h, 2, "rot_init: " + which + ": non-finite value");
     const double *q = ego_poses7 + (size_t)k * 7 + 3;
-    if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return rot_fail(h, 2, which + ": zero quaternion");
+    if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return pgo_fail(h, 2, "rot_init: " + which + ": zero quaternion");
   }
   // the frames the edges name (all of them: the reference's all_frames, :444-450), the edges that give rows, and the components
   // of free frames joined by the edges with both ends free; an edge from a fixed frame anchors its free end's component
@@ -2157,9 +1651,9 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
     if (a == b || fb) { dropped++; continue; }   // self loop, both fixed, or b fixed with a free (the :84 quirk)
     const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
     if (!all_finite(q, 4) || !(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0) || !all_finite(S, 36))
-      return rot_fail(h, 2, "edge " + std::to_string(e) + ": non-finite or zero relative rotation or square-root information");
+      return pgo_fail(h, 2, "rot_init: edge " + std::to_string(e) + ": non-finite or zero relative rotation or square-root information");
     if (fa && !all_finite(&h->poses[(size_t)a * 8 + 3], 4))
-      return rot_fail(h, 2, "edge " + std::to_string(e) + ": non-finite attitude of its fixed frame");
+      return pgo_fail(h, 2, "rot_init: edge " + std::to_string(e) + ": non-finite attitude of its fixed frame");
     used.push_back(e);
     if (!fa) uf[rot_find(uf, a)] = rot_find(uf, b);
   }
@@ -2168,9 +1662,9 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
   for (int i = 0; i < N; i++) {
     if (!named[i] || h->fixed[i]) continue;
     if (!anchored[rot_find(uf, i)])
-      return rot_fail(h, 2, "frame id " + std::to_string(h->ids[i]) + ": its component of free frames holds no fixed frame (A^T A is singular)");
-    if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return rot_fail(h, 2, "frame id " + std::to_string(h->ids[i]) + ": non-finite attitude");
-    if (grav && ego_of[i] < 0) return rot_fail(h, 2, "frame id " + std::to_string(h->ids[i]) + ": gravity rows are on and the frame has no ego pose");
+      return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": its component of free frames holds no fixed frame (A^T A is singular)");
+    if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": non-finite attitude");
+    if (grav && ego_of[i] < 0) return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": gravity rows are on and the frame has no ego pose");
     frames.push_back(i);
   }
   d2pgo_rot_init_report R; memset(&R, 0, sizeof R);
@@ -2180,9 +1674,9 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
   std::vector<double> poses = h->poses;
   if (!frames.empty()) {
     // the inner handle: nodes = the handle's poses, then (gravity) one fixed virtual node per solved frame holding R_ego^T e3
-    if (!h->rot) { h->rot = new d2pgo_handle(); h->rot->dof = 3; }
-    d2pgo_handle *r = h->rot;
-    r->cfg = h->cfg; r->stream = h->stream;
+    if (!h->rot) { h->rot.reset(new d2pgo_handle()); h->rot->dof = 3; }
+    d2pgo_handle *r = h->rot.get();
+    r->cfg = h->cfg; r->stream = h->stream;   // borrowed: r->own_stream stays false
     const int G = grav ? (int)frames.size() : 0, Nn = N + G;
     r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
     for (int f : frames) r->fixed[f] = 0;
@@ -2218,12 +1712,12 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
       }
       if ((rc = rot_solve_row(r, tol2, cfg->pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) break;
       if (sol[k].alloc((size_t)Nn * 8) != cudaSuccess ||
-          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, (size_t)Nn * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = rot_fail(h, 100, "device buffer for a row system"); break; }
+          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, (size_t)Nn * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = pgo_fail(h, 100, "rot_init: device buffer for a row system"); break; }
     }
     if (rc && rc != 100) h->err = "rot_init: " + r->err;
     Buf<double> x, part; Buf<int> fr;
     const int F = (int)frames.size(), nb = (F + 127) / 128;
-    if (!rc && (x.alloc((size_t)N * 8) != cudaSuccess || part.alloc(nb) != cudaSuccess || fr.alloc(F) != cudaSuccess)) rc = rot_fail(h, 100, "device buffers");
+    if (!rc && (x.alloc((size_t)N * 8) != cudaSuccess || part.alloc(nb) != cudaSuccess || fr.alloc(F) != cudaSuccess)) rc = pgo_fail(h, 100, "rot_init: device buffers");
     if (!rc) {
       double chg = 0.0;
       cudaMemcpyAsync(x.p, poses.data(), (size_t)N * 64, cudaMemcpyHostToDevice, h->stream);
@@ -2233,11 +1727,9 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
       cudaMemcpyAsync(&chg, r->d_cost.p, 8, cudaMemcpyDeviceToHost, h->stream);
       cudaMemcpyAsync(poses.data(), x.p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream);
       const cudaError_t e = cudaStreamSynchronize(h->stream);
-      if (e != cudaSuccess) rc = rot_fail(h, 100 + (int)e, std::string("projection: ") + cudaGetErrorString(e));
+      if (e != cudaSuccess) rc = pgo_fail(h, 100 + (int)e, std::string("rot_init: projection: ") + cudaGetErrorString(e));
       R.state_changes = chg / F;
     }
-    for (int k = 0; k < 3; k++) sol[k].release();
-    x.release(); part.release(); fr.release();
     if (rc) return rc;
   }
   PCK(cudaEventRecord(h->ev1, h->stream));

@@ -1,0 +1,77 @@
+// d2pgo_handle.cuh -- what the pose-graph solver (d2pgo.cu) and PCM (d2pgo_pcm.cu) share: the handle behind include/d2pgo.h,
+// its self-freeing device buffers, and the error helpers.
+#pragma once
+#include <array>
+#include <map>
+#include <memory>
+#include <unordered_map>
+
+#include "d2pgo_chol.cuh"   // and with it cuda_runtime.h, <string>, <vector> and include/d2pgo.h
+
+namespace d2pgo_host {
+
+// a device array that only grows, freed with its owner
+template <typename T> struct Buf {
+  T *p = nullptr; size_t n = 0;
+  Buf() = default;
+  Buf(const Buf &) = delete;
+  Buf &operator=(const Buf &) = delete;
+  ~Buf() { if (p) cudaFree(p); }
+  cudaError_t alloc(size_t c) { if (c <= n && p) return cudaSuccess; if (p) cudaFree(p); p = nullptr; n = 0; cudaError_t e = cudaMalloc(&p, (c ? c : 1) * sizeof(T)); if (e == cudaSuccess) n = c; return e; }
+};
+
+struct PgoScalars {      // device-resident CG state that is not a per-block partial
+  double bb;             // |b|^2 of the current linear system
+  int done, iters;
+};
+
+struct PcmBufs;                                               // d2pgo_pcm.cu
+struct PcmBufsFree { void operator()(PcmBufs *p) const; };    // defined beside PcmBufs
+
+}  // namespace d2pgo_host
+
+struct d2pgo_handle {
+  template <typename T> using Buf = d2pgo_host::Buf<T>;
+  d2pgo_config cfg;
+  int dof = 6;              // pose block size: 6 (RelPoseFactorAD on SE(3)) or 4 (RelPoseFactor4D on [x y z yaw])
+  std::string err;
+  cudaStream_t stream = nullptr;
+  bool own_stream = false;  // d2pgo_create's handles; the rotation-init inner handle (rot) runs on its outer handle's stream
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  std::vector<int64_t> ids; std::unordered_map<int64_t, int> index;
+  std::vector<double> poses; std::vector<unsigned char> fixed;   // [N][8], the device layout of PgoDev::x
+  std::vector<int> ea, eb; std::vector<double> rel, sinfo;         // rel [E][8], sinfo [E][dof^2]
+  std::vector<int> gp_pose; std::vector<double> gp_u, gp_S;        // gravity priors: pose index, u_ego [G][3], S [G][9]
+  Buf<double> d_gp_u, d_gp_S, d_glin[2]; Buf<int> d_gp_pose, d_prior_of;
+  Buf<double> d_x[2], d_rel, d_sinfo, d_lin[2], d_g[2], d_D[2], d_Minv, d_dx, d_r, d_z, d_p, d_Ap, d_cost, d_damp, d_t, d_part, d_cost_part;
+  Buf<unsigned char> d_fixed; Buf<int> d_ea, d_eb, d_inc_ptr, d_inc; Buf<d2pgo_host::PgoScalars> d_s;
+  cudaGraphExec_t cg_graph[2] = {nullptr, nullptr};   // kCgChunk CG iterations on the linearisation buffer 0 / 1 (single rank)
+  std::string cg_args[2];                             // the bytes of the kernel arguments each graph was captured with
+  bool uploaded = false;
+  void *comm = nullptr; int rank = 0, nranks = 1;
+  std::unique_ptr<d2pgo_host::PcmBufs, d2pgo_host::PcmBufsFree> pcm;   // d2pgo_pcm's device buffers, from its first call
+  // ARock (d2pgo_arock_enable): owner agent and 6-DoF q_init per pose id, the dual table keyed (neighbour, frame id) in
+  // ascending order, the messages received since the last step, and the device copy of the table (in table order)
+  bool arock = false; d2pgo_arock_config acfg = {};
+  std::unordered_map<int64_t, int32_t> owner; std::unordered_map<int64_t, std::array<double, 4>> qinit;
+  struct Dual { double yl[6], yr[6]; };
+  struct Msg { int32_t sender, target; std::vector<int64_t> frames; std::vector<double> duals; };
+  std::map<std::pair<int32_t, int64_t>, Dual> duals;
+  std::vector<Msg> inbox;
+  Buf<int> d_ak_pose, d_ak_ptr, d_ak_of; Buf<double> d_ak_yr, d_ak_yl, d_ak_qinit, d_ak_lin[2], d_ak_coord;
+  int ak_n = -1;                      // duals on the device, -1 = none synced
+  std::unique_ptr<d2pgo_handle> rot;  // d2pgo_rot_init's row systems (dof 3), kept between calls for their buffers
+  int linear_solver = D2PGO_LINEAR_PCG;   // d2pgo_set_linear_solver
+  std::unique_ptr<d2pgo_chol::Numeric> chol;   // the sparse Cholesky's analysis and device state (d2pgo_chol.cu)
+
+  ~d2pgo_handle() {   // the device buffers free themselves
+    for (cudaGraphExec_t g : cg_graph) if (g) cudaGraphExecDestroy(g);
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (own_stream) cudaStreamDestroy(stream);
+  }
+};
+
+#define PCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return 100 + (int)e_; } } while (0)
+
+inline int pgo_fail(d2pgo_handle *h, int rc, const std::string &msg) { h->err = msg; return rc; }

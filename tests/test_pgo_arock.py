@@ -438,8 +438,8 @@ PARENT = "9392526"   # the last commit before ARock: its d2pgo.cu kernels are th
 
 
 def test_kernels_without_arock_compile_to_the_same_sass_as_before():
-    """Every kernel of d2pgo.cu as it was before ARock compiles to the same instructions now (the proximal terms live in
-    kernels of their own).  Needs the git history and the CUDA toolkit; skipped without them."""
+    """Every kernel of d2pgo.cu as it was before ARock compiles to the same instructions now, in d2pgo.cu or d2pgo_pcm.cu (the
+    proximal terms live in kernels of their own).  Needs the git history and the CUDA toolkit; skipped without them."""
     import shutil
     import subprocess
     import tempfile
@@ -447,7 +447,8 @@ def test_kernels_without_arock_compile_to_the_same_sass_as_before():
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if not (shutil.which("git") and shutil.which("cuobjdump") and os.path.exists(nvcc)):
         pytest.skip("git, nvcc or cuobjdump unavailable")
-    build.build(force=not os.path.exists(os.path.join(ROOT, "d2slam_b200", "build", "d2pgo.o")))
+    objs = [os.path.join(ROOT, "d2slam_b200", "build", o) for o in ("d2pgo.o", "d2pgo_pcm.o")]   # PCM's kernels have their own file
+    build.build(force=not all(os.path.exists(o) for o in objs))
     with tempfile.TemporaryDirectory() as td:
         files = {"d2slam_b200/csrc/d2pgo.cu": "x/csrc/d2pgo.cu", "d2slam_b200/csrc/d2ba_math.cuh": "x/csrc/d2ba_math.cuh", "include/d2pgo.h": "include/d2pgo.h"}
         for src, dst in files.items():
@@ -461,7 +462,10 @@ def test_kernels_without_arock_compile_to_the_same_sass_as_before():
         subprocess.check_call([nvcc] + flags + ["-c", os.path.join(td, "x", "csrc", "d2pgo.cu"), "-o", obj])
         sys.path.insert(0, os.path.join(ROOT, "tools"))
         import sass_diff
-        old, new = sass_diff.kernels(obj), sass_diff.kernels(os.path.join(ROOT, "d2slam_b200", "build", "d2pgo.o"))
+        old = sass_diff.kernels(obj)
+        new = {}
+        for o in objs:
+            new.update(sass_diff.kernels(o))
     assert len(old) == 31
     assert [k for k in old if new.get(k) != old[k]] == []
     assert sum("k_pgo_arock" in k for k in new) == 10

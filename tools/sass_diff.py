@@ -1,13 +1,14 @@
 """Compare the SASS of every kernel of one object (or library) with the same kernel in another:
 `python tools/sass_diff.py OLD NEW` lists the kernels of OLD that NEW lacks or compiles to different instructions, and exits
-non-zero if there is any.  Kernel names are compared with the per-file hash of the anonymous namespace taken out (it changes
-whenever the source file does).  Build OLD from the earlier source with the flags of d2slam_b200/build.py, e.g.
+non-zero if there is any.  Kernel names are compared with the anonymous namespace's per-file name and its length taken out
+(the name changes whenever the source file does, and it names the file, so a kernel moved to another file keeps its name).
+Build OLD from the earlier source with the flags of d2slam_b200/build.py, e.g.
 `nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr -c d2pgo.cu`."""
 import re
 import subprocess
 import sys
 
-_ANON = re.compile(r"_GLOBAL__N__[0-9a-f]+_\d+_[A-Za-z0-9_]+?_[0-9a-f]{8}")
+_ANON = re.compile(r"\d+_GLOBAL__N__[0-9a-f]+_\d+_[A-Za-z0-9_]+?_[0-9a-f]{8}")
 
 
 def kernels(path):
