@@ -1,14 +1,15 @@
 """CPU oracle of the 4-DoF pose-graph path (TEST INFRASTRUCTURE: imported by tests/ and tools/ only).
 
-The batched linearisation and the scipy sparse-direct Gauss-Newton of pgo_oracle.py for d2pgo's default configuration,
-RelPoseFactor4D on [x y z yaw] poses (pgo_pose_dof = PGO_POSE_4D).  Factor level pinned: edges_eval_4d is the per-edge
-pgo_oracle.edge_eval_4d batched (tests/test_pgo_4dof.py), and edge_eval_4d is pinned to the reference functor
-(tests/test_ref_pin.py, tests/golden/ref_factors.npz); the minimiser is a restatement (same optimum, not ceres' iterates)."""
+The batched linearisation of pgo_oracle.py for d2pgo's default configuration, RelPoseFactor4D on [x y z yaw] poses
+(pgo_pose_dof = PGO_POSE_4D), minimised by the scipy sparse-direct Gauss-Newton of pgo_lsq.py.  Factor level pinned:
+edges_eval_4d is the per-edge pgo_oracle.edge_eval_4d batched (tests/test_pgo_4dof.py), and edge_eval_4d is pinned to the
+reference functor (tests/test_ref_pin.py, tests/golden/ref_factors.npz); the minimiser is a restatement (same optimum, not
+ceres' iterates)."""
 import numpy as np
-import scipy.sparse as sp
-import scipy.sparse.linalg as spla
 
-from oracle.pgo_oracle import normalize_angle
+from oracle.pgo_lsq import gauss_newton, normalize_angle
+
+
 def edges_eval_4d(poses, ea, eb, rel, S):
     """edge_eval_4d for all edges at once (same formulas, numpy-batched): poses [N,4], rel [E,4] = [p_meas, yaw_meas], S [E,4,4]
     -> r [E,4], J0 [E,4,4], J1 [E,4,4]."""
@@ -31,27 +32,11 @@ def cost_4d(poses, ea, eb, rel, S):
 
 
 def solve_4d(poses, fixed, ea, eb, rel, sqrt_info, iters=30, ftol=1e-12):
-    """solve() for the 4-DoF problem: Gauss-Newton with a sparse direct solve, retraction of PosAngleManifold::Plus
-    (angle_manifold.h:39-68: x + dx, yaw normalised to [-pi, pi)); returns (poses, costs)."""
-    x = np.array(poses, float); N = len(x); S = np.asarray(sqrt_info).reshape(-1, 4, 4)
-    free = np.nonzero(np.asarray(fixed) == 0)[0]; col = -np.ones(N, int); col[free] = np.arange(len(free)) * 4
-    costs = []
-    ea = np.asarray(ea); eb = np.asarray(eb); rel = np.asarray(rel, float)
-    E = len(ea); rr, cc = np.meshgrid(np.arange(4), np.arange(4), indexing="ij")
-    for it in range(iters):
-        r_e, J0, J1 = edges_eval_4d(x, ea, eb, rel, S)                   # == edge_eval_4d per edge (tests/test_pgo_4dof.py)
-        r_all = r_e.ravel()
-        rows, cols, vals = [], [], []
-        for blk, J in ((ea, J0), (eb, J1)):
-            keep = col[blk] >= 0
-            e_idx = np.nonzero(keep)[0]
-            rows.append((4 * e_idx[:, None, None] + rr[None]).ravel()); cols.append((col[blk[keep]][:, None, None] + cc[None]).ravel()); vals.append(J[keep].ravel())
-        J = sp.csr_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(4 * E, 4 * len(free)))
-        c = 0.5 * float(r_all @ r_all); costs.append(c)
-        if it and abs(costs[-2] - c) <= ftol * max(c, 1e-300):
-            break
-        H = (J.T @ J).tocsc(); g = J.T @ r_all
-        dx = spla.spsolve(H + 1e-12 * sp.identity(H.shape[0], format="csc"), -g).reshape(-1, 4)
-        x[free, :3] += dx[:, :3]
-        x[free, 3] = normalize_angle(x[free, 3] + dx[:, 3])
-    return x, costs
+    """solve() for the 4-DoF problem: Gauss-Newton with a sparse direct solve (pgo_lsq.gauss_newton), retraction of
+    PosAngleManifold::Plus (pgo_lsq.retract); returns (poses, costs)."""
+    ea = np.asarray(ea); eb = np.asarray(eb); rel = np.asarray(rel, float); S = np.asarray(sqrt_info).reshape(-1, 4, 4)
+
+    def blocks(x):
+        r, J0, J1 = edges_eval_4d(x, ea, eb, rel, S)                     # == edge_eval_4d per edge (tests/test_pgo_4dof.py)
+        return [(r, [(ea, J0), (eb, J1)])]
+    return gauss_newton(poses, fixed, blocks, iters, ftol)

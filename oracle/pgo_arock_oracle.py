@@ -6,7 +6,7 @@ d2pgo_node runs it, with ARockPGO's message handling (d2pgo/src/ARockPGO.cpp:13-
      problem uses: if t == self or there is no dual (d, f) yet, create it with y_l = y_r = the value, or else set y_r;
   2. scanAndCreateDualStates (:192-208): a dual (owner, f) for every frame of another agent, from x(f) (or zero);
   3. setDualStateFactors (:256-314) + the local solve: the agent's edges (and gravity priors) plus one proximal term per dual
-     towards y_r, solved to convergence by sparse-direct Gauss-Newton (pgo4d_oracle / pgo_oracle / pgo_gravity_oracle rows);
+     towards y_r, solved to convergence by pgo_lsq's sparse-direct Gauss-Newton;
   4. updateDualStates (:24-84): y_l -= eta ((y_l + y_r) / 2 - x), 4-DoF yaw normalised only outside [-pi, pi];
   5. broadcastData: one message per neighbour, target = that neighbour, the y_l of its duals.
 Dual coordinates: 4-DoF [x y z yaw] (POSE_4D); 6-DoF [p ; theta], theta = Log(q_init^-1 q) (POSE_PERTURB_6D).  Proximal terms:
@@ -15,13 +15,12 @@ Dual coordinates: 4-DoF [x y z yaw] (POSE_4D); 6-DoF [p ; theta], theta = Log(q_
 Jacobian A blockdiag(I3, J_r^-1(theta)) of the right perturbation q (x) Exp(dtheta).  arock_run is the synchronous schedule
 (every agent steps, then every message goes to every other agent).  The dual table is ordered by (neighbour, frame id)."""
 import numpy as np
-import scipy.sparse as sp
-import scipy.sparse.linalg as spla
 
 from d2slam_b200 import synth
 from oracle.pgo4d_oracle import edges_eval_4d
 from oracle.pgo_gravity_oracle import priors_eval
-from oracle.pgo_oracle import _vqmul, _vskew, edges_eval, normalize_angle
+from oracle.pgo_lsq import gauss_newton, normalize_angle
+from oracle.pgo_oracle import _vqmul, _vskew, edges_eval
 
 
 def theta_of(q, q_init):
@@ -79,44 +78,21 @@ def update_duals(yl, yr, c, eta):
 def local_solve(x, fixed, ea, eb, rel, S, dual_pose, q_init_d, yr, rho_T, rho_theta, priors=None, iters=50, ftol=1e-15):
     """Gauss-Newton with a sparse direct solve over the edges, the gravity priors (6-DoF; priors = (idx, u_ego, S3)) and the
     proximal terms (dual k on pose dual_pose[k] towards yr[k]); to convergence.  Returns (poses, costs)."""
-    x = np.array(x, np.float64); N, W = x.shape; D = 4 if W == 4 else 6
-    free = np.nonzero(np.asarray(fixed) == 0)[0]; col = -np.ones(N, int); col[free] = np.arange(len(free)) * D
+    x = np.asarray(x, np.float64); D = 4 if x.shape[1] == 4 else 6
     ea = np.asarray(ea); eb = np.asarray(eb); rel = np.asarray(rel, np.float64); S = np.asarray(S, np.float64).reshape(-1, D, D)
     dual_pose = np.asarray(dual_pose, int)
-    costs = []
-    for it in range(iters):
-        blocks = []                                   # (row offset, residual [M, D'], [(pose idx [M], J [M, D', D])])
+
+    def blocks(x):
         r_e, J0, J1 = (edges_eval_4d if D == 4 else edges_eval)(x, ea, eb, rel, S)
-        blocks.append((r_e, [(ea, J0), (eb, J1)]))
+        out = [(r_e, [(ea, J0), (eb, J1)])]
         if priors is not None and len(priors[0]):
             r_g, Jg = priors_eval(x, priors[0], priors[1], priors[2])
-            blocks.append((r_g, [(np.asarray(priors[0]), Jg)]))
+            out.append((r_g, [(np.asarray(priors[0]), Jg)]))
         if len(dual_pose):
             r_k, J_k = prox_eval(x[dual_pose], q_init_d, yr, rho_T, rho_theta)
-            blocks.append((r_k, [(dual_pose, J_k)]))
-        rows, cols, vals, res = [], [], [], []
-        off = 0
-        for r_b, parts in blocks:
-            m, dr = r_b.shape
-            rb, cb = np.meshgrid(np.arange(dr), np.arange(D), indexing="ij")
-            for idx, J in parts:
-                keep = col[idx] >= 0
-                e_idx = np.nonzero(keep)[0]
-                rows.append((off + dr * e_idx[:, None, None] + rb[None]).ravel()); cols.append((col[idx[keep]][:, None, None] + cb[None]).ravel()); vals.append(J[keep].ravel())
-            res.append(r_b.ravel()); off += m * dr
-        r_all = np.concatenate(res)
-        Jm = sp.csr_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(off, D * len(free)))
-        c = 0.5 * float(r_all @ r_all); costs.append(c)
-        if it and abs(costs[-2] - c) <= ftol * max(c, 1e-300):
-            break
-        H = (Jm.T @ Jm).tocsc(); g = Jm.T @ r_all
-        dx = spla.spsolve(H + 1e-12 * sp.identity(H.shape[0], format="csc"), -g).reshape(-1, D)
-        if D == 4:
-            x[free, :3] += dx[:, :3]; x[free, 3] = normalize_angle(x[free, 3] + dx[:, 3])
-        else:
-            for k, i in enumerate(free):
-                x[i] = synth.pose_plus(x[i], dx[k])
-    return x, costs
+            out.append((r_k, [(dual_pose, J_k)]))
+        return out
+    return gauss_newton(x, fixed, blocks, iters, ftol)
 
 
 class OracleAgent:

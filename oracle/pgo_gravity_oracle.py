@@ -8,13 +8,11 @@ D2Common::GravityPriorPerturbAD residual (d2common/include/d2common/solver/Gravi
 (the reference forms the row R_i.row(2) - R_ego.row(2) and calls applyOnTheRight(S)).  In the tangent of the
 right-multiplicative pose retraction (q <- q (x) [1, dtheta / 2], p <- p + dp): dr/ddtheta = S^T [u]x, dr/ddp = 0; rank 2, yaw
 about gravity stays free.  Factor level PINNED: gravity_eval is compared with the reference's own functor compiled into
-oracle/_ref/libd2ref_gravity.so (tests/test_pgo_gravity.py, tests/golden/ref_gravity.npz).  solve_gravity is the sparse-direct
-Gauss-Newton of pgo_oracle.solve with the priors' rows appended (same optimum as ceres, not its iterates)."""
+oracle/_ref/libd2ref_gravity.so (tests/test_pgo_gravity.py, tests/golden/ref_gravity.npz).  solve_gravity is pgo_lsq's
+sparse-direct Gauss-Newton over the edges and the priors (same optimum as ceres, not its iterates)."""
 import numpy as np
-import scipy.sparse as sp
-import scipy.sparse.linalg as spla
 
-from d2slam_b200 import synth
+from oracle.pgo_lsq import assemble, free_columns, gauss_newton
 from oracle.pgo_oracle import _vrot, _vskew, edges_eval
 
 
@@ -55,56 +53,32 @@ def cost_gravity(poses, ea, eb, rel, sqrt_info, idx, u_ego, S):
     return 0.5 * float(np.sum(re * re) + np.sum(rg * rg))
 
 
-def _system(x, col, ea, eb, rel, S6, idx, u_ego, S3):
-    """Stacked residual and sparse Jacobian (free-pose tangent columns) of edges + priors."""
-    nfree = int((col >= 0).sum())
-    r_e, J0, J1 = edges_eval(x, ea, eb, rel, S6)
-    E = len(ea); rr6, cc6 = np.meshgrid(np.arange(6), np.arange(6), indexing="ij")
-    rows, cols, vals = [], [], []
-    for blk, J in ((ea, J0), (eb, J1)):
-        keep = col[blk] >= 0
-        e_idx = np.nonzero(keep)[0]
-        rows.append((6 * e_idx[:, None, None] + rr6[None]).ravel()); cols.append((col[blk[keep]][:, None, None] + cc6[None]).ravel()); vals.append(J[keep].ravel())
-    G = len(idx)
-    r_all = r_e.ravel()
-    if G:
-        r_g, Jg = priors_eval(x, idx, u_ego, S3)
-        rr3, cc3 = np.meshgrid(np.arange(3), np.arange(6), indexing="ij")
-        keep = col[idx] >= 0
-        g_idx = np.nonzero(keep)[0]
-        rows.append((6 * E + 3 * g_idx[:, None, None] + rr3[None]).ravel()); cols.append((col[idx[keep]][:, None, None] + cc3[None]).ravel()); vals.append(Jg[keep].ravel())
-        r_all = np.concatenate([r_all, r_g.ravel()])
-    J = sp.csr_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(6 * E + 3 * G, 6 * nfree))
-    return r_all, J
+def _blocks_at(ea, eb, rel, sqrt_info, idx, u_ego, S):
+    """x -> the residual blocks of the edges and (if any) the priors at poses x (pgo_lsq's layout)."""
+    ea = np.asarray(ea); eb = np.asarray(eb); rel = np.asarray(rel, np.float64); S6 = np.asarray(sqrt_info).reshape(-1, 6, 6)
+    idx = np.asarray(idx, int); u_ego = np.asarray(u_ego, np.float64).reshape(-1, 3); S3 = np.asarray(S, np.float64).reshape(-1, 3, 3)
+
+    def blocks(x):
+        r_e, J0, J1 = edges_eval(x, ea, eb, rel, S6)
+        out = [(r_e, [(ea, J0), (eb, J1)])]
+        if len(idx):
+            r_g, Jg = priors_eval(x, idx, u_ego, S3)
+            out.append((r_g, [(idx, Jg)]))
+        return out
+    return blocks
 
 
 def gradient(poses, fixed, ea, eb, rel, sqrt_info, idx, u_ego, S):
     """J^T r over the free poses' tangents, [n_free, 6]."""
-    x = np.asarray(poses, np.float64); N = len(x)
-    free = np.nonzero(np.asarray(fixed) == 0)[0]; col = -np.ones(N, int); col[free] = np.arange(len(free)) * 6
-    r, J = _system(x, col, np.asarray(ea), np.asarray(eb), np.asarray(rel, np.float64), np.asarray(sqrt_info).reshape(-1, 6, 6),
-                   np.asarray(idx, int), np.asarray(u_ego, np.float64).reshape(-1, 3), np.asarray(S, np.float64).reshape(-1, 3, 3))
+    free, col = free_columns(fixed, 6)
+    r, J = assemble(_blocks_at(ea, eb, rel, sqrt_info, idx, u_ego, S)(np.asarray(poses, np.float64)), col, len(free), 6)
     return (J.T @ r).reshape(-1, 6)
 
 
 def solve_gravity(poses, fixed, ea, eb, rel, sqrt_info, idx, u_ego, S, iters=30, ftol=1e-12):
     """Gauss-Newton with a sparse direct solve over the edges (RelPoseFactorAD) and the gravity priors; returns (poses, costs).
     idx [G] pose index of each prior, u_ego [G,3] (ego_gravity), S [G,3,3]."""
-    x = np.array(poses, float); N = len(x)
-    free = np.nonzero(np.asarray(fixed) == 0)[0]; col = -np.ones(N, int); col[free] = np.arange(len(free)) * 6
-    ea = np.asarray(ea); eb = np.asarray(eb); rel = np.asarray(rel, float); S6 = np.asarray(sqrt_info).reshape(-1, 6, 6)
-    idx = np.asarray(idx, int); u_ego = np.asarray(u_ego, float).reshape(-1, 3); S3 = np.asarray(S, float).reshape(-1, 3, 3)
-    costs = []
-    for it in range(iters):
-        r_all, J = _system(x, col, ea, eb, rel, S6, idx, u_ego, S3)
-        c = 0.5 * float(r_all @ r_all); costs.append(c)
-        if it and abs(costs[-2] - c) <= ftol * max(c, 1e-300):
-            break
-        H = (J.T @ J).tocsc(); g = J.T @ r_all
-        dx = spla.spsolve(H + 1e-12 * sp.identity(H.shape[0], format="csc"), -g)
-        for i in free:
-            x[i] = synth.pose_plus(x[i], dx[col[i]:col[i] + 6])
-    return x, costs
+    return gauss_newton(poses, fixed, _blocks_at(ea, eb, rel, sqrt_info, idx, u_ego, S), iters, ftol)
 
 
 def tilt_errors(poses, gt):

@@ -14,9 +14,9 @@ import numpy as np
 import scipy.sparse as sp
 import scipy.sparse.linalg as spla
 
-from d2slam_b200 import synth
 from oracle import pgo4d_oracle as p4
 from oracle import pgo_gravity_oracle as pg
+from oracle import pgo_lsq
 from oracle import pgo_oracle as po
 
 
@@ -33,51 +33,23 @@ class Problem:
         self.pidx = np.zeros(0, int) if prior_idx is None else np.asarray(prior_idx, int)
         self.pu = None if prior_u is None else np.asarray(prior_u, np.float64).reshape(-1, 3)
         self.pS = None if prior_S is None else np.asarray(prior_S, np.float64).reshape(-1, 3, 3)
-        N = len(self.x0)
-        self.free = np.nonzero(~self.fixed)[0]
-        self.col = -np.ones(N, int); self.col[self.free] = np.arange(len(self.free)) * self.D
+        self.free, self.col = pgo_lsq.free_columns(self.fixed, self.D)
 
     def system(self, x):
         """residual r, sparse J over the free tangents, and d (the diagonal the damping scales)."""
-        D = self.D
-        ev = p4.edges_eval_4d if D == 4 else po.edges_eval
-        r_e, J0, J1 = ev(x, self.ea, self.eb, self.rel, self.S)
-        E = len(self.ea); nf = len(self.free) * D
-        rr, cc = np.meshgrid(np.arange(D), np.arange(D), indexing="ij")
-        rows, cols, vals = [], [], []
-        d = np.zeros(nf)
-        for blk, J in ((self.ea, J0), (self.eb, J1)):
-            keep = self.col[blk] >= 0
-            e_idx = np.nonzero(keep)[0]
-            c = self.col[blk[keep]]
-            rows.append((D * e_idx[:, None, None] + rr[None]).ravel()); cols.append((c[:, None, None] + cc[None]).ravel()); vals.append(J[keep].ravel())
-            np.add.at(d, (c[:, None] + np.arange(D)[None]).ravel(), (J[keep] ** 2).sum(axis=1).ravel())
-        r_all = r_e.ravel(); nrow = D * E
+        r_e, J0, J1 = (p4.edges_eval_4d if self.D == 4 else po.edges_eval)(x, self.ea, self.eb, self.rel, self.S)
+        blocks = [(r_e, [(self.ea, J0), (self.eb, J1)])]
         if len(self.pidx):
             r_g, Jg = pg.priors_eval(x, self.pidx, self.pu, self.pS)
-            keep = self.col[self.pidx] >= 0
-            g_idx = np.nonzero(keep)[0]; c = self.col[self.pidx[keep]]
-            r3, c6 = np.meshgrid(np.arange(3), np.arange(6), indexing="ij")
-            rows.append((nrow + 3 * g_idx[:, None, None] + r3[None]).ravel()); cols.append((c[:, None, None] + c6[None]).ravel()); vals.append(Jg[keep].ravel())
-            np.add.at(d, (c[:, None] + np.arange(6)[None]).ravel(), (Jg[keep] ** 2).sum(axis=1).ravel())
-            r_all = np.concatenate([r_all, r_g.ravel()]); nrow += 3 * len(self.pidx)
-        J = sp.csr_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(nrow, nf))
-        return r_all, J, d
+            blocks.append((r_g, [(self.pidx, Jg)]))
+        return pgo_lsq.assemble(blocks, self.col, len(self.free), self.D, diag=True)
 
     def cost(self, x):
         r = self.system(x)[0]
         return 0.5 * float(r @ r)
 
     def retract(self, x, dx):
-        y = x.copy(); D = self.D
-        dx = dx.reshape(-1, D)
-        if D == 4:
-            y[self.free, :3] += dx[:, :3]
-            y[self.free, 3] = po.normalize_angle(y[self.free, 3] + dx[:, 3])
-        else:
-            for k, i in enumerate(self.free):
-                y[i] = synth.pose_plus(x[i], dx[k])
-        return y
+        return pgo_lsq.retract(x, self.free, dx)
 
     def step(self, x, lam):
         """The exact step dx [N, D] (0 on fixed poses)."""

@@ -1,16 +1,15 @@
 """CPU oracle of the pose-graph path (TEST INFRASTRUCTURE: imported by tests/ and bench.py's cpu legs only).
 
 numpy restatement of D2Common::RelPoseFactorAD (d2common/include/d2common/solver/RelPoseFactor.hpp:68-135) and a
-Gauss-Newton / LM solve of the same least-squares problem with scipy's sparse direct solver (the reference hands the
+Gauss-Newton solve of the same least-squares problem with scipy's sparse direct solver (pgo_lsq; the reference hands the
 per-agent problems to ceres SPARSE_NORMAL_CHOLESKY + LM, d2pgo/test/d2pgo_test.cpp:95-99).  Factor level PINNED: edge_eval
 is compared with the reference's own RelPoseFactorAD functor compiled into oracle/_ref/libd2ref.so (doubles for the
 residual, dual numbers for its exact Jacobians; tests/test_ref_pin.py, tests/golden/ref_factors.npz); the minimiser is a
 restatement (same optimum, not ceres' iterates)."""
 import numpy as np
-import scipy.sparse as sp
-import scipy.sparse.linalg as spla
 
 from d2slam_b200 import synth
+from oracle.pgo_lsq import gauss_newton, normalize_angle
 
 
 def _skew(v):
@@ -19,16 +18,6 @@ def _skew(v):
 
 def _qmul(a, b):
     return synth.quat_mul(a, b)
-
-
-def _qinv(q):
-    return np.array([-q[0], -q[1], -q[2], q[3]]) / np.dot(q, q)
-
-
-def _qleft3(q):
-    if q[3] < 0:
-        q = -q
-    return q[3] * np.eye(3) + _skew(q[:3])
 
 
 def edge_eval(p0, p1, rel, S):
@@ -48,15 +37,10 @@ def edge_eval(p0, p1, rel, S):
     return r, S @ A0, S @ A1
 
 
-def normalize_angle(a):
-    """Utility::NormalizeAngle (utils.hpp:251-257)"""
-    return a - 2.0 * np.pi * np.floor((a + np.pi) / (2.0 * np.pi))
-
-
 def edge_eval_4d(pa, pb, rel_pos, rel_yaw, S):
     """RelPoseFactor4D (RelPoseFactor.hpp:216-227 + Utility::poseError4D utils.hpp:266-280), the reference's default PGO factor
     (pgo_pose_dof = PGO_POSE_4D): poses [x y z yaw]; r = S [p_meas - Rz(-yaw_a)(p_b - p_a) ; N(yaw_meas - N(yaw_b - yaw_a))] and its
-    Jacobians w.r.t. the two 4-vectors (the yaw manifold's tangent is the angle itself).  Oracle only: no device kernel yet."""
+    Jacobians w.r.t. the two 4-vectors (the yaw manifold's tangent is the angle itself)."""
     c, s_ = np.cos(-pa[3]), np.sin(-pa[3])
     Rz = np.array([[c, -s_, 0.0], [s_, c, 0.0], [0.0, 0.0, 1.0]]); dRz = np.array([[-s_, -c, 0.0], [c, -s_, 0.0], [0.0, 0.0, 0.0]])   # d Rz(t)/dt at t = -yaw_a
     v = pb[:3] - pa[:3]
@@ -105,31 +89,11 @@ def edges_eval(poses, ea, eb, rel, S):
     return r, np.einsum("eij,ejk->eik", S, A0), np.einsum("eij,ejk->eik", S, A1)
 
 
-def cost(poses, ea, eb, rel, S):
-    return 0.5 * sum(float(np.dot(*(2 * [edge_eval(poses[a], poses[b], rl, s)[0]]))) for a, b, rl, s in zip(ea, eb, rel, S))
-
-
 def solve(poses, fixed, ea, eb, rel, sqrt_info, iters=30, ftol=1e-12):
-    """Gauss-Newton with a sparse direct solve; returns (poses, costs)."""
-    x = np.array(poses, float); N = len(x); S = np.asarray(sqrt_info).reshape(-1, 6, 6)
-    free = np.nonzero(np.asarray(fixed) == 0)[0]; col = -np.ones(N, int); col[free] = np.arange(len(free)) * 6
-    costs = []
-    ea = np.asarray(ea); eb = np.asarray(eb); rel = np.asarray(rel, float)
-    E = len(ea); rr, cc = np.meshgrid(np.arange(6), np.arange(6), indexing="ij")
-    for it in range(iters):
-        r_e, J0, J1 = edges_eval(x, ea, eb, rel, S)                      # == edge_eval per edge (tests/test_pgo.py)
-        r_all = r_e.ravel()
-        rows, cols, vals = [], [], []
-        for blk, J in ((ea, J0), (eb, J1)):
-            keep = col[blk] >= 0
-            e_idx = np.nonzero(keep)[0]
-            rows.append((6 * e_idx[:, None, None] + rr[None]).ravel()); cols.append((col[blk[keep]][:, None, None] + cc[None]).ravel()); vals.append(J[keep].ravel())
-        J = sp.csr_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(6 * E, 6 * len(free)))
-        c = 0.5 * float(r_all @ r_all); costs.append(c)
-        if it and abs(costs[-2] - c) <= ftol * max(c, 1e-300):
-            break
-        H = (J.T @ J).tocsc(); g = J.T @ r_all
-        dx = spla.spsolve(H + 1e-12 * sp.identity(H.shape[0], format="csc"), -g)
-        for i in free:
-            x[i] = synth.pose_plus(x[i], dx[col[i]:col[i] + 6])
-    return x, costs
+    """Gauss-Newton with a sparse direct solve (pgo_lsq.gauss_newton); returns (poses, costs)."""
+    ea = np.asarray(ea); eb = np.asarray(eb); rel = np.asarray(rel, float); S = np.asarray(sqrt_info).reshape(-1, 6, 6)
+
+    def blocks(x):
+        r, J0, J1 = edges_eval(x, ea, eb, rel, S)                        # == edge_eval per edge (tests/test_pgo.py)
+        return [(r, [(ea, J0), (eb, J1)])]
+    return gauss_newton(poses, fixed, blocks, iters, ftol)
