@@ -1002,12 +1002,13 @@ static void pgo_cg_pose(d2pgo_handle *h, const PgoDev &d, int par, double tol2, 
   k_pgo_cg_pose<P, LOCAL, false><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
 }
 
-// kCgChunk CG iterations; ark: the proximal terms' damping pass.  The rotation rows (PgoRotRow) solve on one rank without
-// proximal terms, so only their single-rank kernels exist.
+// n CG iterations (n <= kCgChunk, the chunk starting at an iteration index that is a multiple of kCgChunk, so k & 1 is the
+// global parity); ark: the proximal terms' damping pass.  The rotation rows (PgoRotRow) solve on one rank without proximal
+// terms, so only their single-rank kernels exist.
 template <class P>
-static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr, const PgoArockDev &ak, double tol2, bool grav, bool ark) {
+static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr, const PgoArockDev &ak, double tol2, bool grav, bool ark, int n) {
   const int ge = (d.n_edge + 127) / 128;
-  for (int k = 0; k < kCgChunk; k++) {
+  for (int k = 0; k < n; k++) {
     const int par = k & 1;
     if (d.n_edge > 0) k_pgo_cg_edge<P><<<ge, 128, 0, h->stream>>>(d, par, tol2);
     if (!ark && !h->comm) {
@@ -1029,9 +1030,10 @@ static int pgo_cg_chunk(d2pgo_handle *h, const PgoDev &d, const PgoPriorDev &pr,
 }
 
 // (J^T J + lambda diag D) dx = -g at linearisation buffer `cur` by block-Jacobi preconditioned CG (J^T J is never formed), in
-// chunks of kCgChunk iterations up to max_it, until the convergence flag; *s holds the CG scalars after the last chunk.  On a
-// single rank a chunk is one launch of the buffer's captured graph.  The graph's kernel nodes hold the arguments they were
-// captured with (pointers, counts, weights, tol2), so it is captured again whenever any of those bytes differ.
+// chunks of kCgChunk iterations, the last one shortened so that at most max_it iterations run, until the convergence flag; *s
+// holds the CG scalars after the last chunk.  On a single rank a chunk is one launch of one of the buffer's two captured graphs
+// (full chunk, short last chunk).  A graph's kernel nodes hold the arguments they were captured with (pointers, counts,
+// weights, tol2) and its length, so it is captured again whenever any of those bytes differ.
 template <class P>
 static int pgo_pcg(d2pgo_handle *h, int cur, double lambda, double tol2, int max_it, bool grav, bool ark, PgoScalars *s) {
   const PgoDev d = pgo_view(h, cur);
@@ -1043,20 +1045,23 @@ static int pgo_pcg(d2pgo_handle *h, int cur, double lambda, double tol2, int max
   std::string args((const char *)&d, sizeof d);
   args.append((const char *)&pr, sizeof pr).append((const char *)&ak, sizeof ak).append((const char *)&tol2, sizeof tol2);
   args += (char)grav; args += (char)ark;
-  cudaGraphExec_t &graph = h->cg_graph[cur];
   for (int k = 0; k < max_it; k += kCgChunk) {
+    const int n = std::min(kCgChunk, max_it - k);
     if (h->comm) {
-      if (int rc = pgo_cg_chunk<P>(h, d, pr, ak, tol2, grav, ark)) return rc;
+      if (int rc = pgo_cg_chunk<P>(h, d, pr, ak, tol2, grav, ark, n)) return rc;
     } else {
-      if (!graph || h->cg_args[cur] != args) {
+      const int which = n < kCgChunk;
+      cudaGraphExec_t &graph = h->cg_graph[cur][which];
+      const std::string key = args + std::string((const char *)&n, sizeof n);
+      if (!graph || h->cg_args[cur][which] != key) {
         if (graph) { cudaGraphExecDestroy(graph); graph = nullptr; }
         cudaGraph_t g;
         PCK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-        pgo_cg_chunk<P>(h, d, pr, ak, tol2, grav, ark);
+        pgo_cg_chunk<P>(h, d, pr, ak, tol2, grav, ark, n);
         PCK(cudaStreamEndCapture(h->stream, &g));
         PCK(cudaGraphInstantiate(&graph, g, 0));
         cudaGraphDestroy(g);
-        h->cg_args[cur] = args;
+        h->cg_args[cur][which] = key;
       }
       PCK(cudaGraphLaunch(graph, h->stream));
     }
@@ -1498,6 +1503,39 @@ static int pgo_exact_step(d2pgo_handle *h, double lambda, bool ark, double *out)
   return 0;
 }
 
+// the iterations of the last pgo_pcg and the relative residual sqrt(r.r / b.b) of its last update, read from the device (with
+// max_it = 0 pgo_pcg reads nothing back): the r.r partials sit in the parity slot of the last iteration (cg_init: slot 1)
+static int pcg_last_residual(d2pgo_handle *h, int32_t *iters, double *residual) {
+  const PgoDev d = pgo_view(h, 0);
+  PgoScalars s;
+  PCK(cudaMemcpyAsync(&s, h->d_s.p, sizeof s, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
+  std::vector<double> part(d.nbp);
+  const int slot = s.iters == 0 ? 1 : (s.iters - 1) & 1;
+  PCK(cudaMemcpyAsync(part.data(), d.rr_part + (size_t)slot * d.nbp, (size_t)d.nbp * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
+  double rr = 0.0;
+  for (double v : part) rr += v;
+  *iters = s.iters;
+  *residual = s.bb > 0.0 ? std::sqrt(rr / s.bb) : 0.0;
+  return 0;
+}
+
+// one PCG step of d2pgo_solve at the current poses (buffer 0), its iteration count and last relative residual
+template <class P>
+static int pgo_pcg_step(d2pgo_handle *h, double lambda, int max_it, double tol, bool ark, double *out, int32_t *iters, double *residual) {
+  int rc;
+  if (!h->uploaded && (rc = pgo_upload(h))) return rc;
+  if (ark && (rc = arock_sync(h))) return rc;
+  const bool grav = !h->gp_pose.empty();
+  double cost;
+  if ((rc = pgo_linearize<P>(h, 0, 1, grav, ark, &cost))) return rc;
+  PgoScalars s; memset(&s, 0, sizeof s);
+  if ((rc = pgo_pcg<P>(h, 0, lambda, tol * tol, max_it, grav, ark, &s))) return rc;
+  PCK(cudaMemcpyAsync(out, h->d_dx.p, h->ids.size() * (size_t)P::D * 8, cudaMemcpyDeviceToHost, h->stream));
+  return pcg_last_residual(h, iters, residual);
+}
+
 extern "C" {
 
 int d2pgo_set_linear_solver(d2pgo_handle *h, int32_t kind) {
@@ -1539,6 +1577,22 @@ int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64
   if (h->arock) if (int rc = arock_check_poses(h, "debug_exact_step")) return rc;
   cudaSetDevice(h->cfg.device);
   return h->dof == 4 ? pgo_exact_step<PgoEdge4>(h, lambda, h->arock, dx_out) : pgo_exact_step<PgoEdge6>(h, lambda, h->arock, dx_out);
+}
+
+int d2pgo_debug_pcg_step(d2pgo_handle *h, double lambda, int32_t max_it, double tol, double *dx_out, int64_t out_doubles,
+                         int32_t *iters_out, double *residual_out) {
+  if (!h) return 1;
+  if (!dx_out || !iters_out || !residual_out || h->ids.empty()) { h->err = "debug_pcg_step: null argument or no poses"; return 1; }
+  if ((size_t)out_doubles < h->ids.size() * (size_t)h->dof) { h->err = "debug_pcg_step: buffer too small: " + std::to_string(h->ids.size() * h->dof) + " doubles needed"; return 2; }
+  if (!(lambda >= 0.0 && std::isfinite(lambda)) || !(tol >= 0.0 && std::isfinite(tol)) || max_it < 0) {
+    h->err = "debug_pcg_step: lambda and tol must be finite and non-negative, max_it non-negative";
+    return 2;
+  }
+  if (h->comm) { h->err = "debug_pcg_step: the handle has a communicator"; return 5; }
+  if (h->arock) if (int rc = arock_check_poses(h, "debug_pcg_step")) return rc;
+  cudaSetDevice(h->cfg.device);
+  return h->dof == 4 ? pgo_pcg_step<PgoEdge4>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out)
+                     : pgo_pcg_step<PgoEdge6>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out);
 }
 
 int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out, int32_t max_pairs, int32_t *n_pairs_out,
@@ -1592,16 +1646,7 @@ static int rot_solve_row(d2pgo_handle *h, double tol2, int max_it, int *iters, d
   PgoScalars s; memset(&s, 0, sizeof s);
   if ((rc = pgo_pcg<P>(h, 0, 0.0, tol2, max_it, false, false, &s))) return rc;
   k_pgo_retract<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_x[1].p);
-  // the residual of the last CG update: its r.r partials sit in the parity slot of the last iteration (cg_init: slot 1)
-  std::vector<double> part(d.nbp);
-  const int slot = s.iters == 0 ? 1 : (s.iters - 1) & 1;
-  PCK(cudaMemcpyAsync(part.data(), d.rr_part + (size_t)slot * d.nbp, (size_t)d.nbp * 8, cudaMemcpyDeviceToHost, h->stream));
-  PCK(cudaStreamSynchronize(h->stream));
-  double rr = 0.0;
-  for (double v : part) rr += v;
-  *iters = s.iters;
-  *residual = s.bb > 0.0 ? std::sqrt(rr / s.bb) : 0.0;
-  return 0;
+  return pcg_last_residual(h, iters, residual);
 }
 
 extern "C" {

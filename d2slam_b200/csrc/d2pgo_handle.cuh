@@ -45,8 +45,10 @@ struct d2pgo_handle {
   Buf<double> d_gp_u, d_gp_S, d_glin[2]; Buf<int> d_gp_pose, d_prior_of;
   Buf<double> d_x[2], d_rel, d_sinfo, d_lin[2], d_g[2], d_D[2], d_Minv, d_dx, d_r, d_z, d_p, d_Ap, d_cost, d_damp, d_t, d_part, d_cost_part;
   Buf<unsigned char> d_fixed; Buf<int> d_ea, d_eb, d_inc_ptr, d_inc; Buf<d2pgo_host::PgoScalars> d_s;
-  cudaGraphExec_t cg_graph[2] = {nullptr, nullptr};   // kCgChunk CG iterations on the linearisation buffer 0 / 1 (single rank)
-  std::string cg_args[2];                             // the bytes of the kernel arguments each graph was captured with
+  // single rank, per linearisation buffer 0 / 1: [0] a chunk of kCgChunk CG iterations, [1] the shorter last chunk that stops
+  // at pcg_max_iterations; cg_args: the bytes of the kernel arguments (and the chunk length) each graph was captured with
+  cudaGraphExec_t cg_graph[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};
+  std::string cg_args[2][2];
   bool uploaded = false;
   void *comm = nullptr; int rank = 0, nranks = 1;
   std::unique_ptr<d2pgo_host::PcmBufs, d2pgo_host::PcmBufsFree> pcm;   // d2pgo_pcm's device buffers, from its first call
@@ -65,7 +67,7 @@ struct d2pgo_handle {
   std::unique_ptr<d2pgo_chol::Numeric> chol;   // the sparse Cholesky's analysis and device state (d2pgo_chol.cu)
 
   ~d2pgo_handle() {   // the device buffers free themselves
-    for (cudaGraphExec_t g : cg_graph) if (g) cudaGraphExecDestroy(g);
+    for (auto &pair : cg_graph) for (cudaGraphExec_t g : pair) if (g) cudaGraphExecDestroy(g);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (own_stream) cudaStreamDestroy(stream);

@@ -102,7 +102,7 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors", "d2pgo_default_arock_config", "d2pgo_arock_enable",
                 "d2pgo_arock_receive", "d2pgo_arock_step", "d2pgo_arock_neighbours", "d2pgo_arock_duals", "d2pgo_debug_arock_terms",
                 "d2pgo_default_rot_init_config", "d2pgo_rot_init", "d2pgo_set_linear_solver", "d2pgo_cholesky_stats",
-                "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic", "d2pgo_debug_cholesky_system"]
+                "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic", "d2pgo_debug_cholesky_system", "d2pgo_debug_pcg_step"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -150,6 +150,15 @@ class PgoSolver:
         out = np.zeros((self.n_poses, D))
         self._chk(_lib().d2pgo_debug_exact_step(self.h, C.c_double(lam), _p(out), C.c_int64(out.size)), "debug_exact_step")
         return out
+
+    def debug_pcg_step(self, lam, max_iterations, tolerance):
+        """One PCG step (the default linear solver) for damping lam at the current poses, at most max_iterations iterations to
+        relative residual tolerance: (dx [N, D] (0 on fixed poses), iterations run, the last relative residual); poses unchanged."""
+        D = 4 if self.cfg.pose_dof == 4 else 6
+        out = np.zeros((self.n_poses, D)); it = C.c_int32(); res = C.c_double()
+        self._chk(_lib().d2pgo_debug_pcg_step(self.h, C.c_double(lam), C.c_int32(max_iterations), C.c_double(tolerance), _p(out),
+                                              C.c_int64(out.size), C.byref(it), C.byref(res)), "debug_pcg_step")
+        return out, it.value, res.value
 
     def debug_cholesky_system(self):
         """The system the last sparse-Cholesky step on this handle factored, as the device assembled it (include/d2pgo.h

@@ -260,7 +260,8 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
 
 /* ---- linear solver of the LM steps (the reference's ceres linear_solver_type)
  *   D2PGO_LINEAR_PCG             the default: (J^T J + lambda diag D) dx = -g by block-Jacobi PCG to pcg_tolerance, at most
- *                                pcg_max_iterations (a truncated step); the only kind with a communicator and for rot init
+ *                                pcg_max_iterations (a truncated step); the only kind with a communicator and for rot init.
+ *                                d2pgo_debug_pcg_step takes one such step alone
  *   D2PGO_LINEAR_SPARSE_CHOLESKY <- SPARSE_NORMAL_CHOLESKY, which d2pgo uses for every pose graph (d2pgo/src/d2pgo_node.cpp:
  *                                191-195, and the ARock local solves, :202): the exact step from a supernodal multifrontal
  *                                Cholesky of H = J^T J + lambda diag(D) + 1e-12 I over the free poses, H being exactly the
@@ -295,6 +296,12 @@ int d2pgo_cholesky_stats(d2pgo_handle *h, d2pgo_cholesky_info *out);
  * and solve for the given lambda; dx_out[N][D] (0 on fixed poses).  The poses do not move.  Returns 6 (dx_out still written)
  * when a pivot was not positive. */
 int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64_t out_doubles);
+/* parity hook: linearise at the current poses as d2pgo_debug_exact_step does and take one step of the PCG solver instead,
+ * at most max_it iterations to relative residual tol: dx_out[N][D] (0 on fixed poses), *iters_out the iterations run and
+ * *residual_out sqrt(r.r / b.b) of the last update (the CG recurrence; 0 when b = 0).  The poses do not move.  Returns 1 on
+ * a null argument, 2 on a small buffer, a negative max_it or a non-finite or negative lambda or tol, 5 with a communicator. */
+int d2pgo_debug_pcg_step(d2pgo_handle *h, double lambda, int32_t max_it, double tol, double *dx_out, int64_t out_doubles,
+                         int32_t *iters_out, double *residual_out);
 /* parity hook: the system the last sparse-Cholesky step on the handle (d2pgo_debug_exact_step or an LM iteration) assembled on
  * the device and factored, copied out (no other device work): diag_out[N][D*D] the damped diagonal block of each pose
  * (row-major, the factored lower triangle mirrored; 0 on fixed poses), b_out[N][D] the right-hand side -g (0 on fixed poses),

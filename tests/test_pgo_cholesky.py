@@ -207,24 +207,33 @@ def _coo_csr(trip, n):
     return sp.coo_matrix((vals, (rows, cols)), shape=(n, n)).tocsr()
 
 
-def assemble(s, g, dof, lam, with_priors=False, arock_poses=None, magnitude=False):
-    """(A, b, terms) of (J^T J + diag(lam d + 1e-12)) dx = -J^T r over the free poses (D rows per free pose, in pose order;
-    A scipy CSR) from the handle's own edge, gravity-prior and (arock_poses: the pose of each dual in table order)
-    proximal-term records; terms = the largest number of records touching one pose.  magnitude: the same sums over |J|
-    and |r| (b then holds +sum |J|^T |r|)."""
+def records(s, g, dof, with_priors=False, arock_poses=None):
+    """The handle's own edge, gravity-prior (one per pose) and (arock_poses: the pose of each dual in table order)
+    proximal-term records at the current poses, as factor groups (poses of each Jacobian slot, r [R, m], Jacobians [R, m, D]
+    per slot)"""
     D = dof; N = len(g["ids"])
-    f = np.abs if magnitude else (lambda v: v)
     rec = s.debug_edges()
-    factors = [((np.asarray(g["ea"]), np.asarray(g["eb"])), f(rec[:, :D]),
-                (f(rec[:, D:D + D * D].reshape(-1, D, D)), f(rec[:, D + D * D:].reshape(-1, D, D))))]
+    factors = [((np.asarray(g["ea"]), np.asarray(g["eb"])), rec[:, :D],
+                (rec[:, D:D + D * D].reshape(-1, D, D), rec[:, D + D * D:].reshape(-1, D, D)))]
     if with_priors:
         pr = s.debug_gravity_priors()
-        factors.append(((np.arange(N),), f(pr[:, :3]), (f(pr[:, 3:].reshape(-1, 3, 6)),)))
+        factors.append(((np.arange(N),), pr[:, :3], (pr[:, 3:].reshape(-1, 3, 6),)))
     if arock_poses is not None:
         tr = s.debug_arock_terms(len(arock_poses))
-        factors.append(((np.asarray(arock_poses),), f(tr[:, :D]), (f(tr[:, D:].reshape(-1, D, D)),)))
+        factors.append(((np.asarray(arock_poses),), tr[:, :D], (tr[:, D:].reshape(-1, D, D),)))
+    return factors
+
+
+def assemble(s, g, dof, lam, with_priors=False, arock_poses=None, magnitude=False, factors=None):
+    """(A, b, terms) of (J^T J + diag(lam d + 1e-12)) dx = -J^T r over the free poses (D rows per free pose, in pose order;
+    A scipy CSR) from the records (factors, or the handle's own: records()); terms = the largest number of records touching
+    one pose.  magnitude: the same sums over |J| and |r| (b then holds +sum |J|^T |r|)."""
+    D = dof; N = len(g["fixed"])
+    f = np.abs if magnitude else (lambda v: v)
+    factors = records(s, g, dof, with_priors, arock_poses) if factors is None else factors
     trip, gv, d, count = [], np.zeros(N * D), np.zeros(N * D), np.zeros(N, int)
     for poses, r, Js in factors:
+        r, Js = f(r), tuple(f(J) for J in Js)
         for pa, Ja in zip(poses, Js):
             idx = (pa[:, None] * D + np.arange(D)).ravel()
             gv += np.bincount(idx, np.einsum("eka,ek->ea", Ja, r).ravel(), N * D)
