@@ -768,6 +768,62 @@ __global__ void __launch_bounds__(128) k_rotinit_project(int n, const int *frame
   if (threadIdx.x == 0) chg_part[blockIdx.x] = chg;
 }
 
+// ---- distributed rotation initialisation (d2pgo_arock_rot_init_step; RotationInitARock<double>,
+// rotation_initialization_arock.hpp).  A dual prior w (r_f^k - (row k of Y_r)^T) = 0 is an edge from a fixed virtual node
+// (R_ab = I, S = w I3) whose value is row k of the dual's y_r; this kernel writes those values for row system k into the virtual
+// nodes x[j] of the dual priors j, dual[j] being the dual of prior j in table order.
+__global__ void k_rotinit_arock_targets(int n, int k, const int *dual, const double *yr, double *x) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  for (int c = 0; c < 3; c++) x[(size_t)j * 8 + c] = yr[(size_t)dual[j] * 9 + 3 * k + c];
+}
+
+// recoverRotationLLT (rotation_initialization_base.hpp:360-389) with is_multi set, per solved frame j: M from the three row
+// solutions, |R_state - M|_F / |R_state|_F into per-block partials, R_state = M unprojected (the value the dual update reads),
+// and, for frames this agent owns only, the attitude x[3..6] = quaternion of the projection of M.  Eigen's JacobiSVD of M = 0
+// gives U = V = I, so the zero matrix projects to I (a non-main agent's first step without gravity rows has b = 0, M = 0).
+__global__ void __launch_bounds__(128) k_rotinit_arock_project(int n, const int *frame, const unsigned char *owned, const double *m0,
+                                                               const double *m1, const double *m2, double *rstate, double *x, double *chg_part) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  __shared__ double red[40];
+  double chg = 0.0;
+  if (j < n) {
+    const size_t i = (size_t)frame[j];
+    double M[9], R[9];
+    for (int c = 0; c < 3; c++) { M[c] = m0[i * 8 + c]; M[3 + c] = m1[i * 8 + c]; M[6 + c] = m2[i * 8 + c]; }
+    double dd = 0.0, nn = 0.0;
+    bool zero = true;
+    for (int c = 0; c < 9; c++) {
+      const double s = rstate[i * 9 + c];
+      dd += (s - M[c]) * (s - M[c]); nn += s * s;
+      rstate[i * 9 + c] = M[c];
+      zero = zero && M[c] == 0.0;
+    }
+    chg = sqrt(dd) / sqrt(nn);
+    if (owned[j]) {
+      if (zero) for (int c = 0; c < 9; c++) R[c] = c % 4 == 0 ? 1.0 : 0.0;
+      else rotinit_project_svd(M, R);
+      const Q4 o = rotinit_quat(R);
+      x[i * 8 + 3] = o.x; x[i * 8 + 4] = o.y; x[i * 8 + 5] = o.z; x[i * 8 + 6] = o.w;
+    }
+  }
+  chg = block_sum(chg, red);
+  if (threadIdx.x == 0) chg_part[blockIdx.x] = chg;
+}
+
+// updateDualStates, vector branch (ARock.cpp:63-81), per dual k on frame pose[k]: y_l -= eta ((y_l + y_r) / 2 - x) with x the
+// frame's R_state (for a fixed frame, the rotation of its attitude when it entered), in the reference's order and rounding
+__global__ void k_rotinit_arock_update(int n, const int *pose, const double *rstate, const double *yr, double *yl, double eta) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const double *x = rstate + (size_t)pose[k] * 9;
+  for (int q = 0; q < 9; q++) {
+    const double l = yl[(size_t)k * 9 + q];
+    const double avg = __ddiv_rn(__dadd_rn(l, yr[(size_t)k * 9 + q]), 2.0);
+    yl[(size_t)k * 9 + q] = __dsub_rn(l, __dmul_rn(__dsub_rn(avg, x[q]), eta));
+  }
+}
+
 }  // namespace
 
 // the 6-DoF and the 4-DoF entry points each serve one kind of handle
@@ -789,6 +845,10 @@ static int pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const d
   h->gp_pose.clear(); h->gp_u.clear(); h->gp_S.clear();
   for (auto it = h->duals.begin(); it != h->duals.end();)   // ARock duals live on for the frames still present
     it = h->index.count(it->first.second) ? std::next(it) : h->duals.erase(it);
+  for (auto it = h->rot_duals.begin(); it != h->rot_duals.end();)   // and so do the rotation-initialisation duals and states
+    it = h->index.count(it->first.second) ? std::next(it) : h->rot_duals.erase(it);
+  for (auto it = h->rot_state.begin(); it != h->rot_state.end();)
+    it = h->index.count(it->first) ? std::next(it) : h->rot_state.erase(it);
   h->ak_n = -1;
   return 0;
 }
@@ -1633,12 +1693,11 @@ static int rot_find(std::vector<int> &uf, int i) {
   return i;
 }
 
-// one row system on the inner handle h (poses and edges already set; errors are reported there): upload, linearise at
-// x = 0 rows, one undamped Gauss-Newton step by the block-Jacobi PCG of d2pgo_solve, x + dx into h->d_x[1]
+// one row system on the inner handle h (poses and edges uploaded; errors are reported there): linearise at x = 0 rows, one
+// undamped Gauss-Newton step by the block-Jacobi PCG of d2pgo_solve, x + dx into h->d_x[1]
 static int rot_solve_row(d2pgo_handle *h, double tol2, int max_it, int *iters, double *residual) {
   typedef PgoRotRow P;
   int rc;
-  if ((rc = pgo_upload(h))) return rc;
   const PgoDev d = pgo_view(h, 0);
   const PgoPriorDev pr = pgo_prior_view(h, 0);
   if (d.n_edge > 0) k_pgo_lin<P><<<(d.n_edge + 127) / 128, 128, 0, h->stream>>>(d, h->d_cost_part.p, 1);
@@ -1647,6 +1706,81 @@ static int rot_solve_row(d2pgo_handle *h, double tol2, int max_it, int *iters, d
   if ((rc = pgo_pcg<P>(h, 0, 0.0, tol2, max_it, false, false, &s))) return rc;
   k_pgo_retract<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_x[1].p);
   return pcg_last_residual(h, iters, residual);
+}
+
+// the ego attitudes by pose index (gravity rows only): ego_of[i] = the entry of pose i in ego_ids, -1 = none
+static int rot_ego_index(d2pgo_handle *h, const char *what, int32_t n_ego, const int64_t *ego_ids, const double *ego_poses7, std::vector<int> &ego_of) {
+  ego_of.assign(h->ids.size(), -1);
+  for (int k = 0; k < n_ego; k++) {
+    const std::string which = std::string(what) + ": ego pose " + std::to_string(k) + " (id " + std::to_string(ego_ids[k]) + ")";
+    auto it = h->index.find(ego_ids[k]);
+    if (it == h->index.end()) return pgo_fail(h, 2, which + ": unknown pose id");
+    if (ego_of[it->second] >= 0) return pgo_fail(h, 2, which + ": duplicate id");
+    ego_of[it->second] = k;
+    if (!all_finite(ego_poses7 + (size_t)k * 7, 7)) return pgo_fail(h, 2, which + ": non-finite value");
+    const double *q = ego_poses7 + (size_t)k * 7 + 3;
+    if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return pgo_fail(h, 2, which + ": zero quaternion");
+  }
+  return 0;
+}
+
+// the frames the edges name (all of them: the reference's all_frames, :444-450), the edges that give rows, and the union-find
+// of free frames joined by the edges with both ends free
+struct RotEdges { std::vector<char> named; std::vector<int> uf, used; int dropped = 0; };
+static int rot_scan_edges(d2pgo_handle *h, const char *what, RotEdges &s) {
+  const int N = (int)h->ids.size(), E = (int)h->ea.size();
+  s.named.assign(N, 0); s.uf.resize(N); s.used.clear(); s.dropped = 0;
+  for (int i = 0; i < N; i++) s.uf[i] = i;
+  for (int e = 0; e < E; e++) {
+    const int a = h->ea[e], b = h->eb[e];
+    s.named[a] = s.named[b] = 1;
+    const bool fa = h->fixed[a] != 0, fb = h->fixed[b] != 0;
+    if (a == b || fb) { s.dropped++; continue; }   // self loop, both fixed, or b fixed with a free (the :84 quirk)
+    const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
+    if (!all_finite(q, 4) || !(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0) || !all_finite(S, 36))
+      return pgo_fail(h, 2, std::string(what) + ": edge " + std::to_string(e) + ": non-finite or zero relative rotation or square-root information");
+    if (fa && !all_finite(&h->poses[(size_t)a * 8 + 3], 4))
+      return pgo_fail(h, 2, std::string(what) + ": edge " + std::to_string(e) + ": non-finite attitude of its fixed frame");
+    s.used.push_back(e);
+    if (!fa) s.uf[rot_find(s.uf, a)] = rot_find(s.uf, b);
+  }
+  return 0;
+}
+
+// the inner handle of the row systems (dof 3, on h's stream) with the rows of the used edges: R_ab normalised, S = s I3 with
+// s = |S[3:6, 3:6]|_F; Rfix[N][9] the rotations of the fixed frames those edges start from
+static d2pgo_handle *rot_inner_edges(d2pgo_handle *h, const std::vector<int> &used, std::vector<double> &Rfix) {
+  if (!h->rot) { h->rot.reset(new d2pgo_handle()); h->rot->dof = 3; }
+  d2pgo_handle *r = h->rot.get();
+  r->cfg = h->cfg; r->stream = h->stream;   // borrowed: r->own_stream stays false
+  r->ea.clear(); r->eb.clear(); r->rel.clear(); r->sinfo.clear();
+  for (int e : used) {
+    r->ea.push_back(h->ea[e]); r->eb.push_back(h->eb[e]);
+    const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
+    const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    const double rel[8] = {0, 0, 0, q[0] / n, q[1] / n, q[2] / n, q[3] / n, 0};
+    r->rel.insert(r->rel.end(), rel, rel + 8);
+    double s2 = 0.0;   // |S[3:6, 3:6]|_F
+    for (int i = 3; i < 6; i++) for (int j = 3; j < 6; j++) s2 += S[i * 6 + j] * S[i * 6 + j];
+    const double s = std::sqrt(s2), Si[9] = {s, 0, 0, 0, s, 0, 0, 0, s};
+    r->sinfo.insert(r->sinfo.end(), Si, Si + 9);
+  }
+  Rfix.assign(h->ids.size() * 9, 0.0);
+  for (int e : used) if (h->fixed[h->ea[e]]) rot_quat_R(&h->poses[(size_t)h->ea[e] * 8 + 3], &Rfix[(size_t)h->ea[e] * 9]);
+  return r;
+}
+
+// row system k's gravity rows g (r_f^2 - R_ego^T e3), one per frame: an edge from the fixed virtual node base + j of r (its
+// poses already sized) holding R_ego^T e3, with R_ab = I, S = g I3
+static void rot_gravity_rows(d2pgo_handle *r, int base, const std::vector<int> &frames, const std::vector<int> &ego_of, const double *ego_poses7, double g) {
+  const double Si[9] = {g, 0, 0, 0, g, 0, 0, 0, g}, rel[8] = {0, 0, 0, 0, 0, 0, 1, 0};
+  for (size_t j = 0; j < frames.size(); j++) {
+    double Re[9];
+    rot_quat_R(ego_poses7 + (size_t)ego_of[frames[j]] * 7 + 3, Re);
+    for (int c = 0; c < 3; c++) r->poses[(base + j) * 8 + c] = Re[6 + c];   // R_ego^T e3 = third row of R_ego
+    r->ea.push_back(base + (int)j); r->eb.push_back(frames[j]);
+    r->rel.insert(r->rel.end(), rel, rel + 8); r->sinfo.insert(r->sinfo.end(), Si, Si + 9);
+  }
 }
 
 extern "C" {
@@ -1669,95 +1803,46 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
   if (!(std::isfinite(cfg->pcg_tolerance) && cfg->pcg_tolerance >= 0.0) || cfg->pcg_max_iterations < 0 ||
       (cfg->enable_gravity_prior && !std::isfinite(cfg->gravity_sqrt_info)))
     return pgo_fail(h, 2, "rot_init: non-finite or negative pcg_tolerance, gravity_sqrt_info or pcg_max_iterations");
-  const int N = (int)h->ids.size(), E = (int)h->ea.size();
+  const int N = (int)h->ids.size();
   const bool grav = cfg->enable_gravity_prior != 0;
-  // the ego attitudes by pose index (gravity rows only)
-  std::vector<int> ego_of(N, -1);
-  for (int k = 0; k < n_ego; k++) {
-    const std::string which = "ego pose " + std::to_string(k) + " (id " + std::to_string(ego_ids[k]) + ")";
-    auto it = h->index.find(ego_ids[k]);
-    if (it == h->index.end()) return pgo_fail(h, 2, "rot_init: " + which + ": unknown pose id");
-    if (ego_of[it->second] >= 0) return pgo_fail(h, 2, "rot_init: " + which + ": duplicate id");
-    ego_of[it->second] = k;
-    if (!all_finite(ego_poses7 + (size_t)k * 7, 7)) return pgo_fail(h, 2, "rot_init: " + which + ": non-finite value");
-    const double *q = ego_poses7 + (size_t)k * 7 + 3;
-    if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return pgo_fail(h, 2, "rot_init: " + which + ": zero quaternion");
-  }
-  // the frames the edges name (all of them: the reference's all_frames, :444-450), the edges that give rows, and the components
-  // of free frames joined by the edges with both ends free; an edge from a fixed frame anchors its free end's component
-  std::vector<char> named(N, 0), anchored(N, 0);
-  std::vector<int> uf(N), used;
-  for (int i = 0; i < N; i++) uf[i] = i;
-  int dropped = 0;
-  for (int e = 0; e < E; e++) {
-    const int a = h->ea[e], b = h->eb[e];
-    named[a] = named[b] = 1;
-    const bool fa = h->fixed[a] != 0, fb = h->fixed[b] != 0;
-    if (a == b || fb) { dropped++; continue; }   // self loop, both fixed, or b fixed with a free (the :84 quirk)
-    const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
-    if (!all_finite(q, 4) || !(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0) || !all_finite(S, 36))
-      return pgo_fail(h, 2, "rot_init: edge " + std::to_string(e) + ": non-finite or zero relative rotation or square-root information");
-    if (fa && !all_finite(&h->poses[(size_t)a * 8 + 3], 4))
-      return pgo_fail(h, 2, "rot_init: edge " + std::to_string(e) + ": non-finite attitude of its fixed frame");
-    used.push_back(e);
-    if (!fa) uf[rot_find(uf, a)] = rot_find(uf, b);
-  }
-  for (int e : used) if (h->fixed[h->ea[e]]) anchored[rot_find(uf, h->eb[e])] = 1;
+  std::vector<int> ego_of;
+  int rc;
+  if ((rc = rot_ego_index(h, "rot_init", n_ego, ego_ids, ego_poses7, ego_of))) return rc;
+  // an edge from a fixed frame anchors its free end's component
+  RotEdges s;
+  if ((rc = rot_scan_edges(h, "rot_init", s))) return rc;
+  std::vector<char> anchored(N, 0);
+  for (int e : s.used) if (h->fixed[h->ea[e]]) anchored[rot_find(s.uf, h->eb[e])] = 1;
   std::vector<int> frames;   // the free frames solved, ascending pose index
   for (int i = 0; i < N; i++) {
-    if (!named[i] || h->fixed[i]) continue;
-    if (!anchored[rot_find(uf, i)])
+    if (!s.named[i] || h->fixed[i]) continue;
+    if (!anchored[rot_find(s.uf, i)])
       return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": its component of free frames holds no fixed frame (A^T A is singular)");
     if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": non-finite attitude");
     if (grav && ego_of[i] < 0) return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": gravity rows are on and the frame has no ego pose");
     frames.push_back(i);
   }
   d2pgo_rot_init_report R; memset(&R, 0, sizeof R);
-  R.frames = (int)frames.size(); R.edges_used = (int)used.size(); R.edges_dropped = dropped;
+  R.frames = (int)frames.size(); R.edges_used = (int)s.used.size(); R.edges_dropped = s.dropped;
   cudaSetDevice(h->cfg.device);
   PCK(cudaEventRecord(h->ev0, h->stream));
   std::vector<double> poses = h->poses;
   if (!frames.empty()) {
     // the inner handle: nodes = the handle's poses, then (gravity) one fixed virtual node per solved frame holding R_ego^T e3
-    if (!h->rot) { h->rot.reset(new d2pgo_handle()); h->rot->dof = 3; }
-    d2pgo_handle *r = h->rot.get();
-    r->cfg = h->cfg; r->stream = h->stream;   // borrowed: r->own_stream stays false
-    const int G = grav ? (int)frames.size() : 0, Nn = N + G;
-    r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
-    for (int f : frames) r->fixed[f] = 0;
-    r->ea.clear(); r->eb.clear(); r->rel.clear(); r->sinfo.clear();
-    for (int e : used) {
-      r->ea.push_back(h->ea[e]); r->eb.push_back(h->eb[e]);
-      const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
-      const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-      const double rel[8] = {0, 0, 0, q[0] / n, q[1] / n, q[2] / n, q[3] / n, 0};
-      r->rel.insert(r->rel.end(), rel, rel + 8);
-      double s2 = 0.0;   // |S[3:6, 3:6]|_F
-      for (int i = 3; i < 6; i++) for (int j = 3; j < 6; j++) s2 += S[i * 6 + j] * S[i * 6 + j];
-      const double s = std::sqrt(s2), Si[9] = {s, 0, 0, 0, s, 0, 0, 0, s};
-      r->sinfo.insert(r->sinfo.end(), Si, Si + 9);
-    }
-    std::vector<double> Rfix((size_t)N * 9, 0.0);
-    for (int e : used) if (h->fixed[h->ea[e]]) rot_quat_R(&h->poses[(size_t)h->ea[e] * 8 + 3], &Rfix[(size_t)h->ea[e] * 9]);
+    std::vector<double> Rfix;
+    d2pgo_handle *r = rot_inner_edges(h, s.used, Rfix);
+    const int Nn = N + (grav ? (int)frames.size() : 0);
     Buf<double> sol[3];
     const double tol2 = cfg->pcg_tolerance * cfg->pcg_tolerance;
-    int rc = 0;
     for (int k = 0; k < 3 && !rc; k++) {
+      r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
+      for (int f : frames) r->fixed[f] = 0;
       r->poses.assign((size_t)Nn * 8, 0.0);
       for (int i = 0; i < N; i++) if (r->fixed[i]) for (int c = 0; c < 3; c++) r->poses[(size_t)i * 8 + c] = Rfix[(size_t)i * 9 + k * 3 + c];
-      if (k == 2 && G) {   // gravity rows g (r_f^2 - R_ego^T e3): an edge from the virtual node with R_ab = I, S = g I3
-        const double g = cfg->gravity_sqrt_info, Si[9] = {g, 0, 0, 0, g, 0, 0, 0, g}, rel[8] = {0, 0, 0, 0, 0, 0, 1, 0};
-        for (int j = 0; j < G; j++) {
-          double Re[9];
-          rot_quat_R(ego_poses7 + (size_t)ego_of[frames[j]] * 7 + 3, Re);
-          for (int c = 0; c < 3; c++) r->poses[(size_t)(N + j) * 8 + c] = Re[6 + c];   // R_ego^T e3 = third row of R_ego
-          r->ea.push_back(N + j); r->eb.push_back(frames[j]);
-          r->rel.insert(r->rel.end(), rel, rel + 8); r->sinfo.insert(r->sinfo.end(), Si, Si + 9);
-        }
-      }
-      if ((rc = rot_solve_row(r, tol2, cfg->pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) break;
-      if (sol[k].alloc((size_t)Nn * 8) != cudaSuccess ||
-          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, (size_t)Nn * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = pgo_fail(h, 100, "rot_init: device buffer for a row system"); break; }
+      if (k == 2 && grav) rot_gravity_rows(r, N, frames, ego_of, ego_poses7, cfg->gravity_sqrt_info);
+      if ((rc = pgo_upload(r)) || (rc = rot_solve_row(r, tol2, cfg->pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) break;
+      if (sol[k].alloc(r->ids.size() * 8) != cudaSuccess ||
+          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, r->ids.size() * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = pgo_fail(h, 100, "rot_init: device buffer for a row system"); break; }
     }
     if (rc && rc != 100) h->err = "rot_init: " + r->err;
     Buf<double> x, part; Buf<int> fr;
@@ -1784,6 +1869,276 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
   h->poses.swap(poses);   // commit: the solved attitudes; the next d2pgo_solve uploads them
   h->uploaded = false;
   if (report) *report = R;
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- distributed rotation initialisation host side (d2pgo_arock_rot_*)
+
+// w = |getSqrtInfoMatRot()|_F of a dual prior Swarm::PosePrior(f, Y_r, rho_rot_mat I3) (setDualStateFactors,
+// rotation_initialization_arock.hpp:52-57).  ASSUMED: the 3x3 argument is information whose Cholesky factor is the square root
+// sqrt(rho) I3, so w = sqrt(3 rho).
+static double rot_dual_weight(double rho_rot_mat) { return std::sqrt(3.0 * rho_rot_mat); }
+
+// what every d2pgo_arock_rot_* call needs: a 6-DoF handle in ARock mode; and a step or a receipt, one whose perturbation solve
+// has not started
+static int rot_arock_check(d2pgo_handle *h, const char *what, bool changes) {
+  if (h->dof != 6) return pgo_fail(h, 5, std::string(what) + ": the handle was created with pose_dof = 4; rotation initialisation acts on 6-DoF poses");
+  if (!h->arock) return pgo_fail(h, 5, std::string(what) + ": the handle is not in ARock mode (d2pgo_arock_enable)");
+  if (changes && !h->duals.empty()) return pgo_fail(h, 5, std::string(what) + ": the ARock pose dual table is not empty (rotation initialisation precedes the perturbation solve)");
+  return 0;
+}
+
+extern "C" {
+
+int d2pgo_default_arock_rot_init_config(d2pgo_arock_rot_init_config *c) {
+  if (!c) return 1;
+  memset(c, 0, sizeof *c);
+  c->enable_gravity_prior = 0; c->pcg_max_iterations = 20000; c->gravity_sqrt_info = 10.0; c->pcg_tolerance = 1e-12; c->rho_rot_mat = 0.1;
+  return 0;
+}
+
+int d2pgo_arock_rot_receive(d2pgo_handle *h, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int32_t dim,
+                            const double *duals, const double *poses7) {
+  if (!h) return 1;
+  if (int rc = rot_arock_check(h, "arock_rot_receive", true)) return rc;
+  if (n < 0 || (n > 0 && (!frame_ids || !duals || !poses7))) return pgo_fail(h, 1, "arock_rot_receive: null argument or negative count");
+  if (dim != 9) return pgo_fail(h, 2, "arock_rot_receive: duals of dimension " + std::to_string(dim) + " (a rotation dual is a 3x3 matrix, 9)");
+  if (sender == h->acfg.self_id) return pgo_fail(h, 2, "arock_rot_receive: a message from this agent itself (self_id " + std::to_string(sender) + ")");
+  if (!all_finite(duals, (size_t)n * 9) || !all_finite(poses7, (size_t)n * 7)) return pgo_fail(h, 2, "arock_rot_receive: non-finite dual or pose");
+  std::unordered_map<int64_t, int> seen;
+  for (int k = 0; k < n; k++) {
+    if (!seen.emplace(frame_ids[k], k).second) return pgo_fail(h, 2, "arock_rot_receive: frame id " + std::to_string(frame_ids[k]) + " twice in one message");
+    const double *q = poses7 + (size_t)k * 7 + 3;
+    if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return pgo_fail(h, 2, "arock_rot_receive: frame id " + std::to_string(frame_ids[k]) + ": zero quaternion");
+  }
+  // inputDPGOData (:216-235): the sender's frames take the sender's pose (position and attitude) and their attitude-init, now
+  for (int k = 0; k < n; k++) {
+    auto it = h->index.find(frame_ids[k]);
+    if (it == h->index.end()) continue;
+    auto o = h->owner.find(frame_ids[k]);
+    if (o == h->owner.end() || o->second != sender) continue;
+    const double *p = poses7 + (size_t)k * 7, *q = p + 3;
+    memcpy(&h->poses[(size_t)it->second * 8], p, 56);
+    const double s = 1.0 / std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    h->qinit[frame_ids[k]] = {q[0] * s, q[1] * s, q[2] * s, q[3] * s};
+    h->uploaded = false;
+  }
+  h->rot_inbox.push_back(d2pgo_handle::Msg{sender, target, std::vector<int64_t>(frame_ids, frame_ids + n), std::vector<double>(duals, duals + (size_t)n * 9)});
+  return 0;
+}
+
+int d2pgo_arock_rot_init_step(d2pgo_handle *h, const d2pgo_arock_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids,
+                              const double *ego_poses7, d2pgo_rot_init_report *report) {
+  if (!h) return 1;
+  if (!cfg || n_ego < 0 || (n_ego > 0 && (!ego_ids || !ego_poses7))) return pgo_fail(h, 1, "arock_rot_init_step: null argument or negative count");
+  int rc;
+  if ((rc = rot_arock_check(h, "arock_rot_init_step", true))) return rc;
+  if (h->ids.empty()) return pgo_fail(h, 1, "arock_rot_init_step: the handle has no poses");
+  if ((rc = arock_check_poses(h, "arock_rot_init_step"))) return rc;
+  if (!(std::isfinite(cfg->pcg_tolerance) && cfg->pcg_tolerance >= 0.0) || cfg->pcg_max_iterations < 0 ||
+      (cfg->enable_gravity_prior && !std::isfinite(cfg->gravity_sqrt_info)) || !(std::isfinite(cfg->rho_rot_mat) && cfg->rho_rot_mat >= 0.0))
+    return pgo_fail(h, 2, "arock_rot_init_step: non-finite or negative pcg_tolerance, gravity_sqrt_info, rho_rot_mat or pcg_max_iterations");
+  const int N = (int)h->ids.size(), self = h->acfg.self_id;
+  const bool grav = cfg->enable_gravity_prior != 0;
+  std::vector<int> ego_of;
+  if ((rc = rot_ego_index(h, "arock_rot_init_step", n_ego, ego_ids, ego_poses7, ego_of))) return rc;
+  RotEdges s;
+  if ((rc = rot_scan_edges(h, "arock_rot_init_step", s))) return rc;
+  // 1. receiveAll / processPGOData (:104-111, :142-182) on a copy of the table, messages in arrival order: a frame the problem
+  // estimates (an edge names it), if target == self or there is no dual (sender, f) yet: created with zeros if missing, y_r set,
+  // and y_l set too when it was just created
+  auto duals = h->rot_duals;
+  for (const auto &m : h->rot_inbox)
+    for (size_t k = 0; k < m.frames.size(); k++) {
+      auto it = h->index.find(m.frames[k]);
+      if (it == h->index.end() || !s.named[it->second]) continue;
+      const auto key = std::make_pair(m.sender, m.frames[k]);
+      auto d = duals.find(key);
+      if (m.target != self && d != duals.end()) continue;
+      const double *v = &m.duals[k * 9];
+      if (d == duals.end()) { d2pgo_handle::RotDual nd; memcpy(nd.yl, v, 72); memcpy(nd.yr, v, 72); duals.emplace(key, nd); }
+      else memcpy(d->second.yr, v, 72);
+    }
+  // 3. scanAndCreateDualStates (:79-102): every edge end another agent owns gets the dual (owner, f), zero, if it has none
+  for (size_t e = 0; e < h->ea.size(); e++)
+    for (int i : {h->ea[e], h->eb[e]}) {
+      const int32_t o = h->owner.at(h->ids[i]);
+      if (o == self) continue;
+      const auto key = std::make_pair(o, h->ids[i]);
+      if (!duals.count(key)) { d2pgo_handle::RotDual nd; memset(&nd, 0, sizeof nd); duals.emplace(key, nd); }
+    }
+  // 4. setDualStateFactors (:32-61): a prior per dual on a free frame; with the fixed-frame edge rows they anchor the components
+  std::vector<int> dual_pose, prior_dual;
+  std::vector<char> anchored(N, 0);
+  for (int e : s.used) if (h->fixed[h->ea[e]]) anchored[rot_find(s.uf, h->eb[e])] = 1;
+  for (const auto &kv : duals) {
+    const int i = h->index.at(kv.first.second);
+    if (!h->fixed[i]) { prior_dual.push_back((int)dual_pose.size()); anchored[rot_find(s.uf, i)] = 1; }
+    dual_pose.push_back(i);
+  }
+  std::vector<int> frames;   // the free frames solved, ascending pose index
+  std::vector<unsigned char> owned;
+  for (int i = 0; i < N; i++) {
+    if (!s.named[i]) continue;
+    const std::string fid = "arock_rot_init_step: frame id " + std::to_string(h->ids[i]);
+    if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return pgo_fail(h, 2, fid + ": non-finite attitude");
+    if (h->fixed[i]) continue;
+    if (!anchored[rot_find(s.uf, i)]) return pgo_fail(h, 2, fid + ": its component of free frames has no fixed-frame row and no dual prior (A^T A is singular)");
+    if (grav && ego_of[i] < 0) return pgo_fail(h, 2, fid + ": gravity rows are on and the frame has no ego pose");
+    frames.push_back(i); owned.push_back(h->owner.at(h->ids[i]) == self);
+  }
+  // R_state of every named frame: kept, or R(attitude) when the frame first enters a step (PGOState::addFrame)
+  std::vector<double> rstate((size_t)N * 9, 0.0);
+  for (int i = 0; i < N; i++) {
+    auto it = h->rot_state.find(h->ids[i]);
+    if (it != h->rot_state.end()) memcpy(&rstate[(size_t)i * 9], it->second.data(), 72);
+    else if (s.named[i]) rot_quat_R(&h->poses[(size_t)i * 8 + 3], &rstate[(size_t)i * 9]);
+  }
+  const int K = (int)duals.size(), P = (int)prior_dual.size(), F = (int)frames.size();
+  std::vector<double> yl((size_t)K * 9), yr((size_t)K * 9);
+  { size_t k = 0;
+    for (const auto &kv : duals) { memcpy(&yl[k * 9], kv.second.yl, 72); memcpy(&yr[k * 9], kv.second.yr, 72); k++; } }
+  d2pgo_rot_init_report R; memset(&R, 0, sizeof R);
+  R.frames = F; R.edges_used = (int)s.used.size(); R.edges_dropped = s.dropped;
+  cudaSetDevice(h->cfg.device);
+  PCK(cudaEventRecord(h->ev0, h->stream));
+  // the dual table and the rotation states to the device
+  PCK(h->d_rk_pose.alloc(K)); PCK(h->d_rk_prior.alloc(P)); PCK(h->d_rk_yl.alloc((size_t)K * 9)); PCK(h->d_rk_yr.alloc((size_t)K * 9));
+  PCK(h->d_rk_state.alloc((size_t)N * 9));
+  if (K) {
+    PCK(cudaMemcpyAsync(h->d_rk_pose.p, dual_pose.data(), (size_t)K * 4, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_rk_yl.p, yl.data(), (size_t)K * 72, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_rk_yr.p, yr.data(), (size_t)K * 72, cudaMemcpyHostToDevice, h->stream));
+  }
+  if (P) PCK(cudaMemcpyAsync(h->d_rk_prior.p, prior_dual.data(), (size_t)P * 4, cudaMemcpyHostToDevice, h->stream));
+  PCK(cudaMemcpyAsync(h->d_rk_state.p, rstate.data(), (size_t)N * 72, cudaMemcpyHostToDevice, h->stream));
+  std::vector<double> poses = h->poses;
+  double chg = 0.0;
+  if (F) {
+    // 5. solveLinearRot (base :178-213): nodes = the handle's poses, then one fixed virtual node per dual prior, then (k = 2,
+    // gravity) one per solved frame; rows = the used edges, the dual priors, the gravity rows
+    std::vector<double> Rfix;
+    d2pgo_handle *r = rot_inner_edges(h, s.used, Rfix);
+    const double w = rot_dual_weight(cfg->rho_rot_mat), Sw[9] = {w, 0, 0, 0, w, 0, 0, 0, w}, I[8] = {0, 0, 0, 0, 0, 0, 1, 0};
+    for (int j = 0; j < P; j++) {
+      r->ea.push_back(N + j); r->eb.push_back(dual_pose[prior_dual[j]]);
+      r->rel.insert(r->rel.end(), I, I + 8); r->sinfo.insert(r->sinfo.end(), Sw, Sw + 9);
+    }
+    const int Nn = N + P + (grav ? F : 0);
+    Buf<double> sol[3];
+    const double tol2 = cfg->pcg_tolerance * cfg->pcg_tolerance;
+    for (int k = 0; k < 3 && !rc; k++) {
+      r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
+      for (int f : frames) r->fixed[f] = 0;
+      r->poses.assign((size_t)Nn * 8, 0.0);
+      for (int i = 0; i < N; i++) if (r->fixed[i]) for (int c = 0; c < 3; c++) r->poses[(size_t)i * 8 + c] = Rfix[(size_t)i * 9 + k * 3 + c];
+      if (k == 2 && grav) rot_gravity_rows(r, N + P, frames, ego_of, ego_poses7, cfg->gravity_sqrt_info);
+      if ((rc = pgo_upload(r))) break;
+      if (P) k_rotinit_arock_targets<<<(P + 127) / 128, 128, 0, h->stream>>>(P, k, h->d_rk_prior.p, h->d_rk_yr.p, r->d_x[0].p + (size_t)N * 8);
+      if ((rc = rot_solve_row(r, tol2, cfg->pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) break;
+      if (sol[k].alloc(r->ids.size() * 8) != cudaSuccess ||
+          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, r->ids.size() * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = pgo_fail(h, 100, "arock_rot_init_step: device buffer for a row system"); break; }
+    }
+    if (rc && rc != 100) h->err = "arock_rot_init_step: " + r->err;
+    if (rc) return rc;
+    // 6. recoverRotationLLT: R_state = M, the owned frames' attitudes; state_changes = the mean over the free frames
+    Buf<double> x, part; Buf<int> fr; Buf<unsigned char> own;
+    const int nb = (F + 127) / 128;
+    PCK(x.alloc((size_t)N * 8)); PCK(part.alloc(nb)); PCK(fr.alloc(F)); PCK(own.alloc(F));
+    PCK(cudaMemcpyAsync(x.p, poses.data(), (size_t)N * 64, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(fr.p, frames.data(), (size_t)F * 4, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(own.p, owned.data(), (size_t)F, cudaMemcpyHostToDevice, h->stream));
+    k_rotinit_arock_project<<<nb, 128, 0, h->stream>>>(F, fr.p, own.p, sol[0].p, sol[1].p, sol[2].p, h->d_rk_state.p, x.p, part.p);
+    k_pgo_sum<<<1, 128, 0, h->stream>>>(part.p, nb, r->d_cost.p);
+    PCK(cudaGetLastError());
+    PCK(cudaMemcpyAsync(&chg, r->d_cost.p, 8, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaMemcpyAsync(poses.data(), x.p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream));
+  }
+  // 7. updateDualStates on every dual, at R_state
+  if (K) k_rotinit_arock_update<<<(K + 127) / 128, 128, 0, h->stream>>>(K, h->d_rk_pose.p, h->d_rk_state.p, h->d_rk_yr.p, h->d_rk_yl.p, h->acfg.eta_k);
+  PCK(cudaGetLastError());
+  if (K) PCK(cudaMemcpyAsync(yl.data(), h->d_rk_yl.p, (size_t)K * 72, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaMemcpyAsync(rstate.data(), h->d_rk_state.p, (size_t)N * 72, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaEventRecord(h->ev1, h->stream));
+  PCK(cudaEventSynchronize(h->ev1));
+  float ms = 0; cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+  R.device_ms = ms;
+  R.state_changes = F ? chg / F : 0.0;
+  // commit: the table, the states of the named frames, the owned frames' attitudes and their q_init (so that the first
+  // d2pgo_arock_step starts from theta = 0 at them); the inbox has been processed
+  { size_t k = 0;
+    for (auto &kv : duals) { memcpy(kv.second.yl, &yl[k * 9], 72); k++; } }
+  h->rot_duals.swap(duals);
+  h->rot_inbox.clear();
+  for (int i = 0; i < N; i++) if (s.named[i]) memcpy(h->rot_state[h->ids[i]].data(), &rstate[(size_t)i * 9], 72);
+  for (size_t j = 0; j < frames.size(); j++) {
+    if (!owned[j]) continue;
+    const double *q = &poses[(size_t)frames[j] * 8 + 3];
+    const double n = 1.0 / std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+    h->qinit[h->ids[frames[j]]] = {q[0] * n, q[1] * n, q[2] * n, q[3] * n};
+  }
+  h->poses.swap(poses);
+  h->uploaded = false; h->ak_n = -1;
+  if (report) *report = R;
+  return 0;
+}
+
+int d2pgo_arock_rot_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out) {
+  if (!h) return 1;
+  if (int rc = rot_arock_check(h, "arock_rot_neighbours", false)) return rc;
+  if (!n_out || max_n < 0 || (max_n > 0 && !ids_out)) return pgo_fail(h, 1, "arock_rot_neighbours: null argument or negative count");
+  std::vector<int32_t> nb;
+  for (const auto &kv : h->rot_duals) if (nb.empty() || nb.back() != kv.first.first) nb.push_back(kv.first.first);
+  *n_out = (int32_t)nb.size();
+  if ((int32_t)nb.size() > max_n) return pgo_fail(h, 2, "arock_rot_neighbours: room for " + std::to_string(max_n) + " ids, " + std::to_string(nb.size()) + " needed");
+  std::copy(nb.begin(), nb.end(), ids_out);
+  return 0;
+}
+
+int d2pgo_arock_rot_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t *n_out, int64_t *frame_ids, double *local9,
+                          double *remote9, double *poses7) {
+  if (!h) return 1;
+  if (int rc = rot_arock_check(h, "arock_rot_duals", false)) return rc;
+  if (!n_out || max_n < 0 || (max_n > 0 && (!frame_ids || !local9))) return pgo_fail(h, 1, "arock_rot_duals: null argument or negative count");
+  auto lo = h->rot_duals.lower_bound(std::make_pair(neighbour, INT64_MIN)), hi = h->rot_duals.upper_bound(std::make_pair(neighbour, INT64_MAX));
+  const int32_t cnt = (int32_t)std::distance(lo, hi);
+  *n_out = cnt;
+  if (cnt > max_n) return pgo_fail(h, 2, "arock_rot_duals: room for " + std::to_string(max_n) + " duals, " + std::to_string(cnt) + " needed");
+  int k = 0;
+  for (auto it = lo; it != hi; ++it, ++k) {
+    frame_ids[k] = it->first.second;
+    memcpy(local9 + (size_t)k * 9, it->second.yl, 72);
+    if (remote9) memcpy(remote9 + (size_t)k * 9, it->second.yr, 72);
+    if (poses7) memcpy(poses7 + (size_t)k * 7, &h->poses[(size_t)h->index.at(it->first.second) * 8], 56);
+  }
+  return 0;
+}
+
+int d2pgo_debug_arock_rot_state(d2pgo_handle *h, double *state9_out, uint8_t *flag_out, int32_t max_duals, int32_t *n_duals_out,
+                                int32_t *neighbour_out, int64_t *frame_out, double *local9_out, double *remote9_out) {
+  if (!h) return 1;
+  if (int rc = rot_arock_check(h, "debug_arock_rot_state", false)) return rc;
+  if (!state9_out || !flag_out || !n_duals_out || max_duals < 0 ||
+      (max_duals > 0 && (!neighbour_out || !frame_out || !local9_out || !remote9_out))) return pgo_fail(h, 1, "debug_arock_rot_state: null argument or negative count");
+  const size_t N = h->ids.size();
+  std::vector<char> named(N, 0);
+  for (size_t e = 0; e < h->ea.size(); e++) named[h->ea[e]] = named[h->eb[e]] = 1;
+  for (size_t i = 0; i < N; i++) {
+    auto it = h->rot_state.find(h->ids[i]);
+    for (int c = 0; c < 9; c++) state9_out[i * 9 + c] = it == h->rot_state.end() ? 0.0 : it->second[c];
+    flag_out[i] = !named[i] ? 0 : h->fixed[i] ? 2 : 1;
+  }
+  const int32_t K = (int32_t)h->rot_duals.size();
+  *n_duals_out = K;
+  if (K > max_duals) return pgo_fail(h, 2, "debug_arock_rot_state: room for " + std::to_string(max_duals) + " duals, " + std::to_string(K) + " needed");
+  int k = 0;
+  for (const auto &kv : h->rot_duals) {
+    neighbour_out[k] = kv.first.first; frame_out[k] = kv.first.second;
+    memcpy(local9_out + (size_t)k * 9, kv.second.yl, 72); memcpy(remote9_out + (size_t)k * 9, kv.second.yr, 72);
+    k++;
+  }
   return 0;
 }
 

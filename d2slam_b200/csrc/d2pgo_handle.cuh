@@ -62,6 +62,14 @@ struct d2pgo_handle {
   std::vector<Msg> inbox;
   Buf<int> d_ak_pose, d_ak_ptr, d_ak_of; Buf<double> d_ak_yr, d_ak_yl, d_ak_qinit, d_ak_lin[2], d_ak_coord;
   int ak_n = -1;                      // duals on the device, -1 = none synced
+  // distributed rotation initialisation (d2pgo_arock_rot_*): its own dual table keyed (neighbour, frame id) ascending, y_l and
+  // y_r being row-major 3x3 matrices, the messages received since the last step (duals [n][9]), each frame's rotation state
+  // R_state (row-major; R(attitude) when the frame first enters a step, then the last unprojected M), and the device copies
+  struct RotDual { double yl[9], yr[9]; };
+  std::map<std::pair<int32_t, int64_t>, RotDual> rot_duals;
+  std::vector<Msg> rot_inbox;
+  std::unordered_map<int64_t, std::array<double, 9>> rot_state;
+  Buf<int> d_rk_pose, d_rk_prior; Buf<double> d_rk_yl, d_rk_yr, d_rk_state;
   std::unique_ptr<d2pgo_handle> rot;  // d2pgo_rot_init's row systems (dof 3), kept between calls for their buffers
   int linear_solver = D2PGO_LINEAR_PCG;   // d2pgo_set_linear_solver
   std::unique_ptr<d2pgo_chol::Numeric> chol;   // the sparse Cholesky's analysis and device state (d2pgo_chol.cu)

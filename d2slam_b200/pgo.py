@@ -21,7 +21,9 @@ arock_split builds agent s's sub-graph the way D2PGO::solve_multi does, arock_ru
 
 Rotation initialisation (d2pgo's rotInitial, enable_rotation_initialization): `PgoSolver.rot_init` replaces the attitudes of the
 free frames by d2pgo's chordal relaxation from the handle's edges and fixed frames (include/d2pgo.h d2pgo_rot_init), before
-solve().
+solve().  In ARock mode the distributed form (RotationInitARock): `ArockAgent.rot_init_step` / `rot_messages` / `rot_receive`
+(include/d2pgo.h d2pgo_arock_rot_*), and arock_rot_init_run runs them on the synchronous schedule until rotInitial's
+convergence gate, before arock_run.
 
 Linear solver (the reference's ceres linear_solver_type): `PgoSolver(linear_solver="sparse_cholesky")` takes exact LM steps
 from a GPU supernodal sparse Cholesky (d2pgo's SPARSE_NORMAL_CHOLESKY; include/d2pgo.h d2pgo_set_linear_solver) instead of the
@@ -63,6 +65,11 @@ class RotInitReport(C.Structure):
                 ("residual", C.c_double * 3), ("state_changes", C.c_double), ("device_ms", C.c_double)]
 
 
+class ArockRotInitConfig(C.Structure):
+    _fields_ = [("enable_gravity_prior", C.c_int32), ("pcg_max_iterations", C.c_int32), ("gravity_sqrt_info", C.c_double),
+                ("pcg_tolerance", C.c_double), ("rho_rot_mat", C.c_double)]
+
+
 class CholeskyInfo(C.Structure):
     _fields_ = [("free_poses", C.c_int32), ("block_pairs", C.c_int32), ("nnz_L", C.c_int64), ("nnz_L_stored", C.c_int64),
                 ("supernodes", C.c_int32), ("levels", C.c_int32), ("supernodes_fundamental", C.c_int32), ("levels_fundamental", C.c_int32),
@@ -102,7 +109,9 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_add_gravity_priors", "d2pgo_debug_gravity_priors", "d2pgo_default_arock_config", "d2pgo_arock_enable",
                 "d2pgo_arock_receive", "d2pgo_arock_step", "d2pgo_arock_neighbours", "d2pgo_arock_duals", "d2pgo_debug_arock_terms",
                 "d2pgo_default_rot_init_config", "d2pgo_rot_init", "d2pgo_set_linear_solver", "d2pgo_cholesky_stats",
-                "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic", "d2pgo_debug_cholesky_system", "d2pgo_debug_pcg_step"]
+                "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic", "d2pgo_debug_cholesky_system", "d2pgo_debug_pcg_step",
+                "d2pgo_default_arock_rot_init_config", "d2pgo_arock_rot_init_step", "d2pgo_arock_rot_receive",
+                "d2pgo_arock_rot_neighbours", "d2pgo_arock_rot_duals", "d2pgo_debug_arock_rot_state"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -244,8 +253,7 @@ class PgoSolver:
         ego = np.zeros((0, 7)) if ego_poses7 is None else np.ascontiguousarray(np.asarray(ego_poses7, np.float64).reshape(-1, 7))
         r = RotInitReport()
         self._chk(_lib().d2pgo_rot_init(self.h, C.byref(c), C.c_int32(len(ids)), _p(ids), _p(ego), C.byref(r)), "rot_init")
-        return dict(frames=r.frames, edges_used=r.edges_used, edges_dropped=r.edges_dropped, pcg_iterations=list(r.pcg_iterations),
-                    residual=list(r.residual), state_changes=r.state_changes, device_ms=r.device_ms)
+        return _rot_report(r)
 
     def comm_init(self, unique_id, rank, nranks):
         uid = (C.c_uint8 * 128)(*unique_id)
@@ -346,12 +354,66 @@ class PgoSolver:
         self._chk(_lib().d2pgo_debug_arock_terms(self.h, _p(out), C.c_int64(out.size)), "debug_arock_terms")
         return out[:n_duals]
 
+    # ---- distributed rotation initialisation (include/d2pgo.h d2pgo_arock_rot_*)
+    def arock_rot_init_step(self, ego_ids=None, ego_poses7=None, **cfg):
+        """One RotationInitARock step on this ARock handle; cfg overrides ArockRotInitConfig fields (enable_gravity_prior,
+        pcg_max_iterations, gravity_sqrt_info, pcg_tolerance, rho_rot_mat).  Returns the report as a dict."""
+        c = ArockRotInitConfig()
+        _lib().d2pgo_default_arock_rot_init_config(C.byref(c))
+        for k, v in cfg.items():
+            setattr(c, k, v)
+        ids = np.zeros(0, np.int64) if ego_ids is None else np.ascontiguousarray(ego_ids, np.int64)
+        ego = np.zeros((0, 7)) if ego_poses7 is None else np.ascontiguousarray(np.asarray(ego_poses7, np.float64).reshape(-1, 7))
+        r = RotInitReport()
+        self._chk(_lib().d2pgo_arock_rot_init_step(self.h, C.byref(c), C.c_int32(len(ids)), _p(ids), _p(ego), C.byref(r)), "arock_rot_init_step")
+        return _rot_report(r)
+
+    def arock_rot_receive(self, sender, target, frame_ids, duals, poses7, dim=9):
+        f = np.ascontiguousarray(frame_ids, np.int64)
+        d = np.ascontiguousarray(np.asarray(duals, np.float64).reshape(len(f), -1)); p = np.ascontiguousarray(np.asarray(poses7, np.float64).reshape(len(f), 7))
+        self._chk(_lib().d2pgo_arock_rot_receive(self.h, C.c_int32(sender), C.c_int32(target), C.c_int32(len(f)), _p(f), C.c_int32(dim), _p(d), _p(p)),
+                  "arock_rot_receive")
+
+    def arock_rot_neighbours(self):
+        n = C.c_int32()
+        _lib().d2pgo_arock_rot_neighbours(self.h, 0, C.byref(n), None)
+        out = np.zeros(max(n.value, 1), np.int32)
+        self._chk(_lib().d2pgo_arock_rot_neighbours(self.h, C.c_int32(len(out)), C.byref(n), _p(out)), "arock_rot_neighbours")
+        return out[: n.value]
+
+    def arock_rot_duals(self, neighbour):
+        """(frame ids ascending, y_l [n, 9], y_r [n, 9], this handle's poses [n, 7]) of the rotation duals held with `neighbour`."""
+        n = C.c_int32()
+        _lib().d2pgo_arock_rot_duals(self.h, C.c_int32(neighbour), 0, C.byref(n), None, None, None, None)
+        m = max(n.value, 1)
+        f = np.zeros(m, np.int64); yl = np.zeros((m, 9)); yr = np.zeros((m, 9)); ps = np.zeros((m, 7))
+        self._chk(_lib().d2pgo_arock_rot_duals(self.h, C.c_int32(neighbour), C.c_int32(m), C.byref(n), _p(f), _p(yl), _p(yr), _p(ps)), "arock_rot_duals")
+        return f[: n.value], yl[: n.value], yr[: n.value], ps[: n.value]
+
+    def debug_arock_rot_state(self):
+        """dict(state [N, 3, 3] R_state per pose (0 before its first step), flag [N] 0 unnamed / 1 free / 2 fixed, and the rotation
+        dual table in table order: neighbour [K], frame [K], yl [K, 9], yr [K, 9])."""
+        N = self.n_poses
+        st = np.zeros((max(N, 1), 9)); fl = np.zeros(max(N, 1), np.uint8); n = C.c_int32()
+        _lib().d2pgo_debug_arock_rot_state(self.h, _p(st), _p(fl), 0, C.byref(n), None, None, None, None)
+        K = max(n.value, 1)
+        nb = np.zeros(K, np.int32); fr = np.zeros(K, np.int64); yl = np.zeros((K, 9)); yr = np.zeros((K, 9))
+        self._chk(_lib().d2pgo_debug_arock_rot_state(self.h, _p(st), _p(fl), C.c_int32(K), C.byref(n), _p(nb), _p(fr), _p(yl), _p(yr)),
+                  "debug_arock_rot_state")
+        k = n.value
+        return dict(state=st[:N].reshape(N, 3, 3), flag=fl[:N].copy(), neighbour=nb[:k], frame=fr[:k], yl=yl[:k], yr=yr[:k])
+
     def debug_pcm_clique(self, adj):
         """The device clique kernel alone on a symmetric boolean adjacency [n, n] -> boolean membership [n]."""
         words = pcm_pack_bits(adj)
         n = len(words); member = np.zeros(max(n, 1), np.uint8); size = C.c_int32()
         self._chk(_lib().d2pgo_debug_pcm_clique(self.h, C.c_int32(n), _p(words), _p(member), C.byref(size)), "debug_pcm_clique")
         return member[:n].astype(bool)
+
+
+def _rot_report(r):
+    return dict(frames=r.frames, edges_used=r.edges_used, edges_dropped=r.edges_dropped, pcg_iterations=list(r.pcg_iterations),
+                residual=list(r.residual), state_changes=r.state_changes, device_ms=r.device_ms)
 
 
 def pcm_pack_bits(adj):
@@ -697,7 +759,7 @@ class ArockAgent:
     solver_kw: PgoConfig fields (pose_dof is taken from the poses)."""
 
     def __init__(self, split, q_init=None, ego_poses=None, solver_kw=None, **cfg):
-        self.split = split; self.self_id = split["self_id"]
+        self.split = split; self.self_id = split["self_id"]; self.ego_poses = ego_poses
         self.dof = 4 if np.asarray(split["poses"]).shape[1] == 4 else 6
         self.s = PgoSolver(pose_dof=self.dof, **(solver_kw or {}))
         if self.dof == 4:
@@ -731,6 +793,24 @@ class ArockAgent:
         ids = self.split["ids"]
         return self.s.get_poses_4d(ids) if self.dof == 4 else self.s.get_poses(ids)
 
+    def rot_init_step(self, ego_poses7=None, **cfg):
+        """One distributed rotation-initialisation step (RotationInitARock; PgoSolver.arock_rot_init_step); 6-DoF only.
+        ego_poses7 [n, 7]: the ego poses of the sub-graph's frames for the gravity rows (None = the agent's ego_poses)."""
+        ego = self.ego_poses if ego_poses7 is None else ego_poses7
+        return self.s.arock_rot_init_step(None if ego is None else self.split["ids"], ego, **cfg)
+
+    def rot_messages(self):
+        """The rotation-initialisation broadcast: one (sender, target, frame ids, y_l [n, 9], poses [n, 7]) per neighbour."""
+        out = []
+        for n in self.s.arock_rot_neighbours():
+            f, yl, _, ps = self.s.arock_rot_duals(int(n))
+            out.append((self.self_id, int(n), f, yl, ps))
+        return out
+
+    def rot_receive(self, msg):
+        sender, target, frames, duals, poses = msg
+        self.s.arock_rot_receive(sender, target, frames, duals, poses)
+
     def close(self):
         self.s.close()
 
@@ -751,3 +831,37 @@ def arock_run(agents, rounds, after_round=None):
         if after_round is not None:
             after_round(r, agents, reps)
     return out
+
+
+def rot_init_converged(state_changes, rounds_run, eps=1e-2, min_rounds=10):
+    """D2PGO::rotInitial's gate (d2pgo.cpp:351-353): state_changes < eps with more than min_rounds solves before this one."""
+    return state_changes < eps and rounds_run - 1 > min_rounds
+
+
+def arock_rot_init_run(agents, max_rounds, eps=1e-2, min_rounds=10, after_round=None, **cfg):
+    """d2pgo's distributed rotation initialisation on the synchronous schedule of arock_run: every round, every agent that has
+    not converged steps (agent.rot_init_step(**cfg)), then every message of the round goes to every other agent.  An agent
+    stops stepping and broadcasting once rot_init_converged holds for its report (rotInitial's is_rot_init_convergence) but
+    keeps receiving.  after_round(r, agents, reports) after each round's delivery (None for an
+    agent that did not step).  Returns the 1-based round at which each agent converged, None where it did not within
+    max_rounds."""
+    done = [None] * len(agents)
+    for r in range(max_rounds):
+        reps = []
+        for i, a in enumerate(agents):
+            if done[i] is not None:
+                reps.append(None); continue
+            rep = a.rot_init_step(**cfg)
+            reps.append(rep)
+            if rot_init_converged(rep["state_changes"], r + 1, eps, min_rounds):
+                done[i] = r + 1
+        msgs = [m for a, rep in zip(agents, reps) if rep is not None for m in a.rot_messages()]
+        for a in agents:
+            for m in msgs:
+                if m[0] != a.self_id:
+                    a.rot_receive(m)
+        if after_round is not None:
+            after_round(r, agents, reps)
+        if all(d is not None for d in done):
+            break
+    return done

@@ -19,6 +19,8 @@
  *   d2pgo_add_gravity_priors      <- setupGravityPriorFactors (enable_gravity_prior): GravityPriorPerturbAD per frame
  *                                    (d2pgo/src/d2pgo.cpp:530-559, GravityPrior.hpp:8-46)
  *   d2pgo_arock_*                 <- ARockPGO, d2pgo's distributed pgo_mode 1 (ARock.cpp:24-314, ARockPGO.cpp:7-104; below)
+ *   d2pgo_arock_rot_*             <- RotationInitARock, the rotation initialisation d2pgo runs before the ARock solve
+ *                                    (rotation_initialization_arock.hpp:10-236; below)
  *
  * Scope note: the reference solves the multi-agent graph with ARock (dual updates around per-agent ceres problems,
  * ARock.cpp:140-328), which the d2pgo_arock_* entry points reproduce, one handle per agent.  BASELINE's config also asks for
@@ -257,6 +259,72 @@ int d2pgo_default_rot_init_config(d2pgo_rot_init_config *cfg);
  * the frames ego_ids, [x y z qx qy qz qw] (the attitude is normalised).  report may be NULL. */
 int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids,
                    const double *ego_poses7, d2pgo_rot_init_report *report);
+
+/* ---- distributed chordal rotation initialisation (d2pgo's rotInitial in pgo_mode 1: RotationInitARock<double>)
+ *   d2pgo_arock_rot_init_step  <- one RotationInitARock::solve with max_steps = 1, one pass of ARockBase::solve_arock
+ *                                 (d2pgo/src/rot_init/rotation_initialization_arock.hpp:195-205, d2common/src/solver/ARock.cpp:
+ *                                 140-190), as D2PGO::rotInitial runs it (d2pgo/src/d2pgo.cpp:336-361)
+ *   d2pgo_arock_rot_receive    <- RotationInitARock::inputDPGOData (:216-235); its duals are handled at the next step
+ *   d2pgo_arock_rot_neighbours,
+ *   d2pgo_arock_rot_duals      <- broadcastData (:113-140): one DPGO_ROT_MAT_DUAL message per neighbour of the table
+ * On a 6-DoF handle in ARock mode (d2pgo_arock_enable: self_id, owners, eta_k).  The unknowns are the rows r_f^k of M_f of
+ * every free frame an edge names, whoever owns it; only the handle's fixed flags fix frames (d2pgo fixes main_id's head frame,
+ * d2pgo.cpp:346-349).  The rotation dual table is the handle's own, apart from the pose dual table of d2pgo_arock_step: keyed
+ * (neighbour, frame id), ascending, y_l and y_r being 3x3 matrices stored row-major (9 doubles); d2pgo_set_poses keeps the
+ * duals of the frames still present.  Every named frame has a rotation state R_state: R(attitude) when the frame first enters
+ * a step, then the last unprojected M of that frame.  One step:
+ *   1. receiveAll / processPGOData (:104-111, :142-182): the queued messages in arrival order; for a frame an edge names, if
+ *      target == self_id or there is no dual (sender, frame) yet: the dual is created with zeros if missing, y_r = the value,
+ *      and y_l = the value too if it was just created;
+ *   2. the fixed-frame edge rows of d2pgo_rot_init (prepareSolverInIter :74-77, the :84 quirk included);
+ *   3. scanAndCreateDualStates (:79-102): every edge end another agent owns gets the dual (owner, frame), zero, if it has none;
+ *   4. setDualStateFactors (:32-61): per dual on a free frame, w (r_f^k - (row k of Y_r)^T) = 0, w = sqrt(3 rho_rot_mat)
+ *      (ASSUMED: PosePrior's 3x3 argument rho I3 is information whose Cholesky factor is the square root, so
+ *      |getSqrtInfoMatRot()|_F = sqrt(3 rho); and getRotMat() returns Y_r unprojected);
+ *   5. solveLinearRot (rotation_initialization_base.hpp:178-213): the three row systems of d2pgo_rot_init over the edge rows,
+ *      the fixed-frame rows and the dual priors, plus with enable_gravity_prior the gravity rows of every free frame, owned or
+ *      remote (:195-201), by the block-Jacobi PCG to pcg_tolerance;
+ *   6. recoverRotationLLT (:360-389) per free frame: state_changes += |R_state - M_f|_F / |R_state|_F, R_state = M_f; frames
+ *      this agent owns take the attitude of R_f = U diag(1, 1, det(U V^T)) V^T (the zero matrix projects to I, as Eigen's
+ *      JacobiSVD gives U = V = I there) and their ARock q_init becomes it; the report's state_changes is the mean;
+ *   7. updateDualStates, vector branch (ARock.cpp:63-81), every dual: y_l -= eta_k ((y_l + y_r) / 2 - R_state of its frame)
+ *      (for a fixed frame R_state is the rotation of its attitude when it entered).
+ * Receipt (d2pgo_arock_rot_receive): every frame of the message that the handle holds and the sender owns takes the sender's
+ * pose, position and attitude, and its q_init becomes that attitude; frames the handle does not hold are ignored.  So the first
+ * d2pgo_arock_step after rotation initialisation starts from theta = 0 at the attitudes it left.  D2PGO::rotInitial declares
+ * convergence once state_changes < rot_init_state_eps after more than 10 solves.  Binary64, no atomics, bitwise reproducible.
+ * Refusals keep nothing of the call and set d2pgo_last_error: 5 on a 4-DoF handle or a handle not in ARock mode, and for a
+ * step or a receipt once the pose dual table is non-empty (rotation initialisation precedes the perturbation solve); 2 on a component of free frames with
+ * no fixed-frame edge row and no dual prior (gravity rows anchor k = 2 only; the reference asserts there), when gravity rows
+ * are on and a free frame lacks an ego pose, on a dual dimension other than 9, a non-finite value, a zero quaternion, a frame
+ * twice in one message or a message from self_id; 1 on a null argument or a negative count.  d2pgo_rot_init keeps refusing
+ * ARock handles (5). */
+typedef struct d2pgo_arock_rot_init_config {
+  int32_t enable_gravity_prior;   /* RotInitConfig::enable_gravity_prior                                                   */
+  int32_t pcg_max_iterations;     /* per row system k (default 20000)                                                      */
+  double gravity_sqrt_info;       /* default 10                                                                            */
+  double pcg_tolerance;           /* relative residual per row system (default 1e-12)                                      */
+  double rho_rot_mat;             /* ARockSolverConfig::rho_rot_mat, default 0.1 (ARock.hpp:11); d2pgo_test_multi: 0.16      */
+} d2pgo_arock_rot_init_config;
+
+int d2pgo_default_arock_rot_init_config(d2pgo_arock_rot_init_config *cfg);
+/* one step; ego_poses7[n_ego][7] of ego_ids as for d2pgo_rot_init (every free frame an edge names, owned or remote, needs one
+ * with gravity rows on).  report may be NULL; its state_changes is 0 when there is no free frame. */
+int d2pgo_arock_rot_init_step(d2pgo_handle *h, const d2pgo_arock_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids,
+                              const double *ego_poses7, d2pgo_rot_init_report *report);
+/* one message: frames, duals[n][dim] (dim must be 9) and the sender's poses7[n][7] of those frames */
+int d2pgo_arock_rot_receive(d2pgo_handle *h, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int32_t dim,
+                            const double *duals, const double *poses7);
+/* the neighbours of the rotation dual table, ascending; *n_out = their number (2 if more than max_n) */
+int d2pgo_arock_rot_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out);
+/* the broadcast payload for one neighbour: frame ids ascending, y_l [n][9], (may be NULL) y_r [n][9] and this handle's current
+ * poses [n][7] of those frames; *n_out = the count (2 if more than max_n) */
+int d2pgo_arock_rot_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t *n_out, int64_t *frame_ids, double *local9,
+                          double *remote9, double *poses7);
+/* parity hook: per pose, state9_out[N][9] its R_state (0 before it entered a step) and flag_out[N] 0 = no edge names it,
+ * 1 = free, 2 = fixed; the rotation dual table in table order: *n_duals_out entries (2 if more than max_duals) */
+int d2pgo_debug_arock_rot_state(d2pgo_handle *h, double *state9_out, uint8_t *flag_out, int32_t max_duals, int32_t *n_duals_out,
+                                int32_t *neighbour_out, int64_t *frame_out, double *local9_out, double *remote9_out);
 
 /* ---- linear solver of the LM steps (the reference's ceres linear_solver_type)
  *   D2PGO_LINEAR_PCG             the default: (J^T J + lambda diag D) dx = -g by block-Jacobi PCG to pcg_tolerance, at most
