@@ -834,6 +834,11 @@ static int pgo_want_dof(d2pgo_handle *h, int dof, const char *what) {
   return 5;
 }
 
+// an ARock dual table without the duals of frames the handle no longer has
+template <class Duals> static void arock_keep_present(const d2pgo_handle *h, Duals &duals) {
+  for (auto it = duals.begin(); it != duals.end();) it = h->index.count(it->first.second) ? std::next(it) : duals.erase(it);
+}
+
 static int pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *poses, int width, const uint8_t *fixed, const char *what) {
   h->ids.assign(ids, ids + n); h->index.clear(); h->poses.assign((size_t)n * 8, 0.0); h->fixed.assign(n, 0);
   for (int i = 0; i < n; i++) {
@@ -843,10 +848,8 @@ static int pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const d
   }
   h->ea.clear(); h->eb.clear(); h->rel.clear(); h->sinfo.clear(); h->uploaded = false;
   h->gp_pose.clear(); h->gp_u.clear(); h->gp_S.clear();
-  for (auto it = h->duals.begin(); it != h->duals.end();)   // ARock duals live on for the frames still present
-    it = h->index.count(it->first.second) ? std::next(it) : h->duals.erase(it);
-  for (auto it = h->rot_duals.begin(); it != h->rot_duals.end();)   // and so do the rotation-initialisation duals and states
-    it = h->index.count(it->first.second) ? std::next(it) : h->rot_duals.erase(it);
+  arock_keep_present(h, h->pose_table.duals);   // ARock duals live on for the frames still present
+  arock_keep_present(h, h->rot_table.duals);    // and so do the rotation-initialisation duals and states
   for (auto it = h->rot_state.begin(); it != h->rot_state.end();)
     it = h->index.count(it->first) ? std::next(it) : h->rot_state.erase(it);
   h->ak_n = -1;
@@ -1334,17 +1337,92 @@ static std::vector<char> arock_in_problem(const d2pgo_handle *h) {
   return in;
 }
 
+// ---- the ARock dual tables (d2pgo_handle::pose_table, rot_table): what the pose and the rotation exchanges share
+using d2pgo_host::ArockDuals;
+using d2pgo_host::ArockTable;
+
+// a received message, before it is queued: counts and pointers, its dual width D, not from this agent, finite, no frame twice
+static int arock_receive_check(d2pgo_handle *h, const char *what, int D, int32_t sender, int32_t n, const int64_t *frame_ids,
+                               int32_t dim, const double *duals) {
+  const std::string w(what);
+  if (n < 0 || (n > 0 && (!frame_ids || !duals))) return pgo_fail(h, 1, w + ": null argument or negative count");
+  if (dim != D) return pgo_fail(h, 2, w + ": duals of dimension " + std::to_string(dim) + ", this exchange's duals have " + std::to_string(D));
+  if (sender == h->acfg.self_id) return pgo_fail(h, 2, w + ": a message from this agent itself (self_id " + std::to_string(sender) + ")");
+  if (!all_finite(duals, (size_t)n * dim)) return pgo_fail(h, 2, w + ": non-finite dual");
+  std::unordered_map<int64_t, int> seen;
+  for (int k = 0; k < n; k++) if (!seen.emplace(frame_ids[k], k).second) return pgo_fail(h, 2, w + ": frame id " + std::to_string(frame_ids[k]) + " twice in one message");
+  return 0;
+}
+
+template <int W> static void arock_queue(ArockTable<W> &t, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int D, const double *duals) {
+  t.inbox.push_back(d2pgo_host::ArockMsg{sender, target, std::vector<int64_t>(frame_ids, frame_ids + n), std::vector<double>(duals, duals + (size_t)n * D)});
+}
+
+// receiveAll / processPGOData (ARockPGO.cpp:13-70; rotation_initialization_arock.hpp:104-111, :142-182): t's messages applied to
+// duals in arrival order.  A frame counts only if the local problem contains it (in[pose index]); the message applies if
+// target == self or there is no dual (sender, f) yet: a new dual takes the value on both sides, an existing one on y_r only.
+template <int W>
+static void arock_apply_inbox(const d2pgo_handle *h, const ArockTable<W> &t, const std::vector<char> &in, int D, ArockDuals<W> &duals) {
+  for (const auto &m : t.inbox)
+    for (size_t k = 0; k < m.frames.size(); k++) {
+      auto it = h->index.find(m.frames[k]);
+      if (it == h->index.end() || !in[it->second]) continue;
+      const auto key = std::make_pair(m.sender, m.frames[k]);
+      auto d = duals.find(key);
+      if (m.target != h->acfg.self_id && d != duals.end()) continue;
+      const double *v = &m.duals[k * D];
+      if (d == duals.end()) { d2pgo_host::ArockDual<W> nd; memset(&nd, 0, sizeof nd); memcpy(nd.yl, v, D * 8); memcpy(nd.yr, v, D * 8); duals.emplace(key, nd); }
+      else memcpy(d->second.yr, v, D * 8);
+    }
+}
+
+// the duals [lo, hi) in table order: y_l [n][D] and (if not null) y_r [n][D]; and back, y_l only
+template <class It> static void arock_flatten(It lo, It hi, int D, double *yl, double *yr) {
+  for (size_t k = 0; lo != hi; ++lo, ++k) {
+    memcpy(yl + k * D, lo->second.yl, D * 8);
+    if (yr) memcpy(yr + k * D, lo->second.yr, D * 8);
+  }
+}
+template <int W> static void arock_set_yl(ArockDuals<W> &duals, int D, const double *yl) {
+  size_t k = 0;
+  for (auto &kv : duals) memcpy(kv.second.yl, yl + k++ * D, D * 8);
+}
+
+// the neighbours of the table, ascending
+template <int W> static int arock_neighbours(d2pgo_handle *h, const ArockTable<W> &t, const char *what, int32_t max_n, int32_t *n_out, int32_t *ids_out) {
+  if (!n_out || max_n < 0 || (max_n > 0 && !ids_out)) return pgo_fail(h, 1, std::string(what) + ": null argument or negative count");
+  std::vector<int32_t> nb;
+  for (const auto &kv : t.duals) if (nb.empty() || nb.back() != kv.first.first) nb.push_back(kv.first.first);
+  *n_out = (int32_t)nb.size();
+  if ((int32_t)nb.size() > max_n) return pgo_fail(h, 2, std::string(what) + ": room for " + std::to_string(max_n) + " ids, " + std::to_string(nb.size()) + " needed");
+  std::copy(nb.begin(), nb.end(), ids_out);
+  return 0;
+}
+
+// the broadcast payload for one neighbour: its frame ids ascending, y_l [n][D] and (if not null) y_r [n][D]
+template <int W>
+static int arock_export(d2pgo_handle *h, const ArockTable<W> &t, const char *what, int D, int32_t neighbour, int32_t max_n, int32_t *n_out,
+                        int64_t *frame_ids, double *local_out, double *remote_out) {
+  if (!n_out || max_n < 0 || (max_n > 0 && (!frame_ids || !local_out))) return pgo_fail(h, 1, std::string(what) + ": null argument or negative count");
+  auto lo = t.duals.lower_bound(std::make_pair(neighbour, INT64_MIN)), hi = t.duals.upper_bound(std::make_pair(neighbour, INT64_MAX));
+  const int32_t cnt = (int32_t)std::distance(lo, hi);
+  *n_out = cnt;
+  if (cnt > max_n) return pgo_fail(h, 2, std::string(what) + ": room for " + std::to_string(max_n) + " duals, " + std::to_string(cnt) + " needed");
+  int k = 0;
+  for (auto it = lo; it != hi; ++it) frame_ids[k++] = it->first.second;
+  arock_flatten(lo, hi, D, local_out, remote_out);
+  return 0;
+}
+
 // the dual table, in table order, to the device: pose of each dual, the pose -> duals CSR, y_r, y_l, q_init
 static int arock_sync(d2pgo_handle *h) {
-  const size_t N = h->ids.size(), K = h->duals.size(), D = h->dof;
+  const auto &duals = h->pose_table.duals;
+  const size_t N = h->ids.size(), K = duals.size(), D = h->dof;
   std::vector<int> pose(K), ptr(N + 1, 0), of(K);
   std::vector<double> yr(K * D), yl(K * D), qi(N * 4, 0.0);
   size_t k = 0;
-  for (const auto &kv : h->duals) {
-    pose[k] = h->index.at(kv.first.second); ptr[pose[k] + 1]++;
-    for (size_t q = 0; q < D; q++) { yr[k * D + q] = kv.second.yr[q]; yl[k * D + q] = kv.second.yl[q]; }
-    k++;
-  }
+  for (const auto &kv : duals) { pose[k] = h->index.at(kv.first.second); ptr[pose[k] + 1]++; k++; }
+  arock_flatten(duals.begin(), duals.end(), (int)D, yl.data(), yr.data());
   for (size_t i = 0; i < N; i++) ptr[i + 1] += ptr[i];
   { std::vector<int> fill(ptr.begin(), ptr.end() - 1);
     for (size_t j = 0; j < K; j++) of[fill[pose[j]]++] = (int)j; }
@@ -1424,13 +1502,8 @@ int d2pgo_arock_enable(d2pgo_handle *h, const d2pgo_arock_config *cfg, int32_t n
 int d2pgo_arock_receive(d2pgo_handle *h, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int32_t dim, const double *duals) {
   if (!h) return 1;
   if (!h->arock) return pgo_fail(h, 5, "arock_receive: the handle is not in ARock mode (d2pgo_arock_enable)");
-  if (n < 0 || (n > 0 && (!frame_ids || !duals))) return pgo_fail(h, 1, "arock_receive: null argument or negative count");
-  if (dim != h->dof) return pgo_fail(h, 2, "arock_receive: duals of dimension " + std::to_string(dim) + " on a handle with pose_dof = " + std::to_string(h->dof));
-  if (sender == h->acfg.self_id) return pgo_fail(h, 2, "arock_receive: a message from this agent itself (self_id " + std::to_string(sender) + ")");
-  if (!all_finite(duals, (size_t)n * dim)) return pgo_fail(h, 2, "arock_receive: non-finite dual");
-  std::unordered_map<int64_t, int> seen;
-  for (int k = 0; k < n; k++) if (!seen.emplace(frame_ids[k], k).second) return pgo_fail(h, 2, "arock_receive: frame id " + std::to_string(frame_ids[k]) + " twice in one message");
-  h->inbox.push_back(d2pgo_handle::Msg{sender, target, std::vector<int64_t>(frame_ids, frame_ids + n), std::vector<double>(duals, duals + (size_t)n * dim)});
+  if (int rc = arock_receive_check(h, "arock_receive", h->dof, sender, n, frame_ids, dim, duals)) return rc;
+  arock_queue(h->pose_table, sender, target, n, frame_ids, h->dof, duals);
   return 0;
 }
 
@@ -1443,19 +1516,10 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
   const int D = h->dof, self = h->acfg.self_id;
   const std::vector<char> in = arock_in_problem(h);
-  // 1. receiveAll / processPGOData (ARockPGO.cpp:13-70), messages in arrival order
-  for (const auto &m : h->inbox)
-    for (size_t k = 0; k < m.frames.size(); k++) {
-      auto it = h->index.find(m.frames[k]);
-      if (it == h->index.end() || !in[it->second]) continue;
-      const auto key = std::make_pair(m.sender, m.frames[k]);
-      auto d = h->duals.find(key);
-      if (m.target != self && d != h->duals.end()) continue;
-      const double *v = &m.duals[k * D];
-      if (d == h->duals.end()) { d2pgo_handle::Dual nd; memset(&nd, 0, sizeof nd); memcpy(nd.yl, v, D * 8); memcpy(nd.yr, v, D * 8); h->duals.emplace(key, nd); }
-      else memcpy(d->second.yr, v, D * 8);
-    }
-  h->inbox.clear();
+  auto &duals = h->pose_table.duals;
+  // 1. receiveAll / processPGOData, on the live table
+  arock_apply_inbox(h, h->pose_table, in, D, duals);
+  h->pose_table.inbox.clear();
   // 2. scanAndCreateDualStates (ARock.cpp:192-208): a dual for every frame of another agent, from x(f) or zero.  The q_init
   // table goes to the device first (arock_sync) so that the coordinates can be taken there.
   if ((rc = arock_sync(h))) return rc;
@@ -1466,10 +1530,10 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
     const int32_t o = h->owner.at(h->ids[i]);
     if (!in[i] || o == self) continue;
     const auto key = std::make_pair(o, h->ids[i]);
-    if (h->duals.count(key)) continue;
-    d2pgo_handle::Dual nd; memset(&nd, 0, sizeof nd);
+    if (duals.count(key)) continue;
+    d2pgo_host::ArockDual<6> nd; memset(&nd, 0, sizeof nd);
     if (!h->acfg.dual_state_init_to_zero) { memcpy(nd.yl, &coord[i * D], D * 8); memcpy(nd.yr, &coord[i * D], D * 8); }
-    h->duals.emplace(key, nd); created = true;
+    duals.emplace(key, nd); created = true;
   }
   // 3. setDualStateFactors + solveLocalStep: the LM solve with the proximal terms towards y_r
   if (created && (rc = arock_sync(h))) return rc;
@@ -1484,8 +1548,7 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
     std::vector<double> yl((size_t)ak.n_dual * D);
     PCK(cudaMemcpyAsync(yl.data(), h->d_ak_yl.p, yl.size() * 8, cudaMemcpyDeviceToHost, h->stream));
     PCK(cudaStreamSynchronize(h->stream));
-    size_t k = 0;
-    for (auto &kv : h->duals) { memcpy(kv.second.yl, &yl[k * D], D * 8); k++; }
+    arock_set_yl(duals, D, yl.data());
   }
   return 0;
 }
@@ -1493,37 +1556,19 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
 int d2pgo_arock_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out) {
   if (!h) return 1;
   if (!h->arock) return pgo_fail(h, 5, "arock_neighbours: the handle is not in ARock mode (d2pgo_arock_enable)");
-  if (!n_out || max_n < 0 || (max_n > 0 && !ids_out)) return pgo_fail(h, 1, "arock_neighbours: null argument or negative count");
-  std::vector<int32_t> nb;
-  for (const auto &kv : h->duals) if (nb.empty() || nb.back() != kv.first.first) nb.push_back(kv.first.first);
-  *n_out = (int32_t)nb.size();
-  if ((int32_t)nb.size() > max_n) return pgo_fail(h, 2, "arock_neighbours: room for " + std::to_string(max_n) + " ids, " + std::to_string(nb.size()) + " needed");
-  std::copy(nb.begin(), nb.end(), ids_out);
-  return 0;
+  return arock_neighbours(h, h->pose_table, "arock_neighbours", max_n, n_out, ids_out);
 }
 
 int d2pgo_arock_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t *n_out, int64_t *frame_ids, double *local_out, double *remote_out) {
   if (!h) return 1;
   if (!h->arock) return pgo_fail(h, 5, "arock_duals: the handle is not in ARock mode (d2pgo_arock_enable)");
-  if (!n_out || max_n < 0 || (max_n > 0 && (!frame_ids || !local_out))) return pgo_fail(h, 1, "arock_duals: null argument or negative count");
-  const int D = h->dof;
-  auto lo = h->duals.lower_bound(std::make_pair(neighbour, INT64_MIN)), hi = h->duals.upper_bound(std::make_pair(neighbour, INT64_MAX));
-  const int32_t cnt = (int32_t)std::distance(lo, hi);
-  *n_out = cnt;
-  if (cnt > max_n) return pgo_fail(h, 2, "arock_duals: room for " + std::to_string(max_n) + " duals, " + std::to_string(cnt) + " needed");
-  int k = 0;
-  for (auto it = lo; it != hi; ++it, ++k) {
-    frame_ids[k] = it->first.second;
-    memcpy(local_out + (size_t)k * D, it->second.yl, D * 8);
-    if (remote_out) memcpy(remote_out + (size_t)k * D, it->second.yr, D * 8);
-  }
-  return 0;
+  return arock_export(h, h->pose_table, "arock_duals", h->dof, neighbour, max_n, n_out, frame_ids, local_out, remote_out);
 }
 
 int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
   if (!h) return 1;
   if (int rc = arock_check_poses(h, "debug_arock_terms")) return rc;
-  const size_t K = h->duals.size(), D = h->dof, W = D + D * D;
+  const size_t K = h->pose_table.duals.size(), D = h->dof, W = D + D * D;
   if ((size_t)out_doubles < K * W) return pgo_fail(h, 2, "debug_arock_terms: buffer too small: " + std::to_string(K * W) + " doubles needed");
   if (!out && K) return pgo_fail(h, 1, "debug_arock_terms: null argument");
   if (!K) return 0;
@@ -1708,27 +1753,31 @@ static int rot_solve_row(d2pgo_handle *h, double tol2, int max_it, int *iters, d
   return pcg_last_residual(h, iters, residual);
 }
 
-// the ego attitudes by pose index (gravity rows only): ego_of[i] = the entry of pose i in ego_ids, -1 = none
-static int rot_ego_index(d2pgo_handle *h, const char *what, int32_t n_ego, const int64_t *ego_ids, const double *ego_poses7, std::vector<int> &ego_of) {
-  ego_of.assign(h->ids.size(), -1);
+// the rotation initialisation problem both entry points solve: ego_of[i] = the entry of pose i in ego_ids (gravity rows only),
+// -1 = none; the frames the edges name (all of them: the reference's all_frames, :444-450); the edges that give rows; the
+// union-find of free frames joined by the edges with both ends free, and which of its components are anchored
+struct RotProblem { std::vector<int> ego_of, uf, used; std::vector<char> named, anchored; int dropped = 0; };
+
+// the checks of the settings both configs share, the ego attitudes and the edges; an edge from a fixed frame anchors its free
+// end's component
+static int rot_problem(d2pgo_handle *h, const char *what, const d2pgo_rot_init_config &cfg, int32_t n_ego, const int64_t *ego_ids,
+                       const double *ego_poses7, RotProblem &s) {
+  const std::string w(what);
+  if (!(std::isfinite(cfg.pcg_tolerance) && cfg.pcg_tolerance >= 0.0) || cfg.pcg_max_iterations < 0 ||
+      (cfg.enable_gravity_prior && !std::isfinite(cfg.gravity_sqrt_info)))
+    return pgo_fail(h, 2, w + ": non-finite or negative pcg_tolerance, gravity_sqrt_info or pcg_max_iterations");
+  const int N = (int)h->ids.size(), E = (int)h->ea.size();
+  s.ego_of.assign(N, -1);
   for (int k = 0; k < n_ego; k++) {
-    const std::string which = std::string(what) + ": ego pose " + std::to_string(k) + " (id " + std::to_string(ego_ids[k]) + ")";
+    const std::string which = w + ": ego pose " + std::to_string(k) + " (id " + std::to_string(ego_ids[k]) + ")";
     auto it = h->index.find(ego_ids[k]);
     if (it == h->index.end()) return pgo_fail(h, 2, which + ": unknown pose id");
-    if (ego_of[it->second] >= 0) return pgo_fail(h, 2, which + ": duplicate id");
-    ego_of[it->second] = k;
+    if (s.ego_of[it->second] >= 0) return pgo_fail(h, 2, which + ": duplicate id");
+    s.ego_of[it->second] = k;
     if (!all_finite(ego_poses7 + (size_t)k * 7, 7)) return pgo_fail(h, 2, which + ": non-finite value");
     const double *q = ego_poses7 + (size_t)k * 7 + 3;
     if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return pgo_fail(h, 2, which + ": zero quaternion");
   }
-  return 0;
-}
-
-// the frames the edges name (all of them: the reference's all_frames, :444-450), the edges that give rows, and the union-find
-// of free frames joined by the edges with both ends free
-struct RotEdges { std::vector<char> named; std::vector<int> uf, used; int dropped = 0; };
-static int rot_scan_edges(d2pgo_handle *h, const char *what, RotEdges &s) {
-  const int N = (int)h->ids.size(), E = (int)h->ea.size();
   s.named.assign(N, 0); s.uf.resize(N); s.used.clear(); s.dropped = 0;
   for (int i = 0; i < N; i++) s.uf[i] = i;
   for (int e = 0; e < E; e++) {
@@ -1738,11 +1787,27 @@ static int rot_scan_edges(d2pgo_handle *h, const char *what, RotEdges &s) {
     if (a == b || fb) { s.dropped++; continue; }   // self loop, both fixed, or b fixed with a free (the :84 quirk)
     const double *q = &h->rel[(size_t)e * 8 + 3], *S = &h->sinfo[(size_t)e * 36];
     if (!all_finite(q, 4) || !(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0) || !all_finite(S, 36))
-      return pgo_fail(h, 2, std::string(what) + ": edge " + std::to_string(e) + ": non-finite or zero relative rotation or square-root information");
+      return pgo_fail(h, 2, w + ": edge " + std::to_string(e) + ": non-finite or zero relative rotation or square-root information");
     if (fa && !all_finite(&h->poses[(size_t)a * 8 + 3], 4))
-      return pgo_fail(h, 2, std::string(what) + ": edge " + std::to_string(e) + ": non-finite attitude of its fixed frame");
+      return pgo_fail(h, 2, w + ": edge " + std::to_string(e) + ": non-finite attitude of its fixed frame");
     s.used.push_back(e);
     if (!fa) s.uf[rot_find(s.uf, a)] = rot_find(s.uf, b);
+  }
+  s.anchored.assign(N, 0);
+  for (int e : s.used) if (h->fixed[h->ea[e]]) s.anchored[rot_find(s.uf, h->eb[e])] = 1;
+  return 0;
+}
+
+// the free frames solved, ascending pose index: every free frame an edge names, refused if its attitude is not finite, its
+// component is not anchored or, with gravity rows, it has no ego pose
+static int rot_frames(d2pgo_handle *h, const char *what, RotProblem &s, bool grav, std::vector<int> &frames) {
+  for (int i = 0; i < (int)h->ids.size(); i++) {
+    if (!s.named[i] || h->fixed[i]) continue;
+    const std::string fid = std::string(what) + ": frame id " + std::to_string(h->ids[i]);
+    if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return pgo_fail(h, 2, fid + ": non-finite attitude");
+    if (!s.anchored[rot_find(s.uf, i)]) return pgo_fail(h, 2, fid + ": its component of free frames is not anchored (A^T A is singular)");
+    if (grav && s.ego_of[i] < 0) return pgo_fail(h, 2, fid + ": gravity rows are on and the frame has no ego pose");
+    frames.push_back(i);
   }
   return 0;
 }
@@ -1770,17 +1835,81 @@ static d2pgo_handle *rot_inner_edges(d2pgo_handle *h, const std::vector<int> &us
   return r;
 }
 
-// row system k's gravity rows g (r_f^2 - R_ego^T e3), one per frame: an edge from the fixed virtual node base + j of r (its
-// poses already sized) holding R_ego^T e3, with R_ab = I, S = g I3
-static void rot_gravity_rows(d2pgo_handle *r, int base, const std::vector<int> &frames, const std::vector<int> &ego_of, const double *ego_poses7, double g) {
-  const double Si[9] = {g, 0, 0, 0, g, 0, 0, 0, g}, rel[8] = {0, 0, 0, 0, 0, 0, 1, 0};
-  for (size_t j = 0; j < frames.size(); j++) {
-    double Re[9];
-    rot_quat_R(ego_poses7 + (size_t)ego_of[frames[j]] * 7 + 3, Re);
-    for (int c = 0; c < 3; c++) r->poses[(base + j) * 8 + c] = Re[6 + c];   // R_ego^T e3 = third row of R_ego
-    r->ea.push_back(base + (int)j); r->eb.push_back(frames[j]);
+// rows from the fixed virtual nodes base + j of r (its poses already sized) to the frames to[j], with R_ab = I, S = w I3
+static void rot_unit_rows(d2pgo_handle *r, int base, const std::vector<int> &to, double w) {
+  const double Si[9] = {w, 0, 0, 0, w, 0, 0, 0, w}, rel[8] = {0, 0, 0, 0, 0, 0, 1, 0};
+  for (size_t j = 0; j < to.size(); j++) {
+    r->ea.push_back(base + (int)j); r->eb.push_back(to[j]);
     r->rel.insert(r->rel.end(), rel, rel + 8); r->sinfo.insert(r->sinfo.end(), Si, Si + 9);
   }
+}
+
+// solveLinearRot (rotation_initialization_base.hpp:178-213): the three row systems on the inner handle.  Nodes: the handle's
+// poses, then one fixed virtual node per dual prior, then (k = 2, gravity rows) one per solved frame.  Rows: the used edges;
+// the dual priors, one to each frame of prior_pose with weight w, whose virtual node k_rotinit_arock_targets sets to row k of
+// y_r of the dual d_prior[j] in d_yr; on k = 2 the gravity rows g (r_f^2 - R_ego^T e3), the virtual node holding R_ego^T e3.
+// sol[k] = the solution of row system k ([nodes][8]); the per-row CG counts and residuals go to R.
+static int rot_solve_rows(d2pgo_handle *h, const d2pgo_rot_init_config &cfg, const RotProblem &s, const std::vector<int> &frames,
+                          const double *ego_poses7, const std::vector<int> &prior_pose, double w, const int *d_prior,
+                          const double *d_yr, Buf<double> (&sol)[3], d2pgo_rot_init_report &R) {
+  const int N = (int)h->ids.size(), P = (int)prior_pose.size();
+  const bool grav = cfg.enable_gravity_prior != 0;
+  std::vector<double> Rfix;
+  d2pgo_handle *r = rot_inner_edges(h, s.used, Rfix);
+  rot_unit_rows(r, N, prior_pose, w);
+  const int Nn = N + P + (grav ? (int)frames.size() : 0);
+  const double tol2 = cfg.pcg_tolerance * cfg.pcg_tolerance;
+  for (int k = 0; k < 3; k++) {
+    r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
+    for (int f : frames) r->fixed[f] = 0;
+    r->poses.assign((size_t)Nn * 8, 0.0);
+    for (int i = 0; i < N; i++) if (r->fixed[i]) for (int c = 0; c < 3; c++) r->poses[(size_t)i * 8 + c] = Rfix[(size_t)i * 9 + k * 3 + c];
+    if (k == 2 && grav) {
+      for (size_t j = 0; j < frames.size(); j++) {
+        double Re[9];
+        rot_quat_R(ego_poses7 + (size_t)s.ego_of[frames[j]] * 7 + 3, Re);
+        for (int c = 0; c < 3; c++) r->poses[(N + P + j) * 8 + c] = Re[6 + c];   // R_ego^T e3 = third row of R_ego
+      }
+      rot_unit_rows(r, N + P, frames, cfg.gravity_sqrt_info);
+    }
+    int rc;
+    if ((rc = pgo_upload(r))) return pgo_fail(h, rc, r->err);
+    if (P) k_rotinit_arock_targets<<<(P + 127) / 128, 128, 0, h->stream>>>(P, k, d_prior, d_yr, r->d_x[0].p + (size_t)N * 8);
+    if ((rc = rot_solve_row(r, tol2, cfg.pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) return pgo_fail(h, rc, r->err);
+    PCK(sol[k].alloc((size_t)Nn * 8));
+    PCK(cudaMemcpyAsync(sol[k].p, r->d_x[1].p, (size_t)Nn * 64, cudaMemcpyDeviceToDevice, h->stream));
+  }
+  return 0;
+}
+
+// the projection onto SO(3) of the F solved frames: project(fr, x, part, nb) launches the caller's kernel on the frame indices
+// fr, the poses x ([N][8], from and back to poses) and nb per-block partials of the state changes; their mean over the frames
+// goes to *state_changes
+template <class Project>
+static int rot_project(d2pgo_handle *h, const std::vector<int> &frames, std::vector<double> &poses, double *state_changes, Project project) {
+  const int N = (int)h->ids.size(), F = (int)frames.size(), nb = (F + 127) / 128;
+  Buf<double> x, part; Buf<int> fr;
+  PCK(x.alloc((size_t)N * 8)); PCK(part.alloc(nb)); PCK(fr.alloc(F));
+  PCK(cudaMemcpyAsync(x.p, poses.data(), (size_t)N * 64, cudaMemcpyHostToDevice, h->stream));
+  PCK(cudaMemcpyAsync(fr.p, frames.data(), (size_t)F * 4, cudaMemcpyHostToDevice, h->stream));
+  project(fr.p, x.p, part.p, nb);
+  k_pgo_sum<<<1, 128, 0, h->stream>>>(part.p, nb, h->rot->d_cost.p);
+  PCK(cudaGetLastError());
+  double chg = 0.0;
+  PCK(cudaMemcpyAsync(&chg, h->rot->d_cost.p, 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaMemcpyAsync(poses.data(), x.p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));
+  *state_changes = chg / F;
+  return 0;
+}
+
+// the device time since h->ev0, once the stream has drained
+static int rot_device_ms(d2pgo_handle *h, double *ms_out) {
+  PCK(cudaEventRecord(h->ev1, h->stream));
+  PCK(cudaEventSynchronize(h->ev1));
+  float ms = 0; cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+  *ms_out = ms;
+  return 0;
 }
 
 extern "C" {
@@ -1800,72 +1929,28 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
   if (h->comm) return pgo_fail(h, 5, "rot_init: a communicator is attached (edge-sharded rotation initialisation is not supported)");
   if (h->arock) return pgo_fail(h, 5, "rot_init: the handle is in ARock mode (d2pgo runs the distributed RotationInitARock there)");
   if (h->ids.empty()) return pgo_fail(h, 1, "rot_init: the handle has no poses");
-  if (!(std::isfinite(cfg->pcg_tolerance) && cfg->pcg_tolerance >= 0.0) || cfg->pcg_max_iterations < 0 ||
-      (cfg->enable_gravity_prior && !std::isfinite(cfg->gravity_sqrt_info)))
-    return pgo_fail(h, 2, "rot_init: non-finite or negative pcg_tolerance, gravity_sqrt_info or pcg_max_iterations");
-  const int N = (int)h->ids.size();
-  const bool grav = cfg->enable_gravity_prior != 0;
-  std::vector<int> ego_of;
+  RotProblem s;
+  std::vector<int> frames;
   int rc;
-  if ((rc = rot_ego_index(h, "rot_init", n_ego, ego_ids, ego_poses7, ego_of))) return rc;
-  // an edge from a fixed frame anchors its free end's component
-  RotEdges s;
-  if ((rc = rot_scan_edges(h, "rot_init", s))) return rc;
-  std::vector<char> anchored(N, 0);
-  for (int e : s.used) if (h->fixed[h->ea[e]]) anchored[rot_find(s.uf, h->eb[e])] = 1;
-  std::vector<int> frames;   // the free frames solved, ascending pose index
-  for (int i = 0; i < N; i++) {
-    if (!s.named[i] || h->fixed[i]) continue;
-    if (!anchored[rot_find(s.uf, i)])
-      return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": its component of free frames holds no fixed frame (A^T A is singular)");
-    if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": non-finite attitude");
-    if (grav && ego_of[i] < 0) return pgo_fail(h, 2, "rot_init: frame id " + std::to_string(h->ids[i]) + ": gravity rows are on and the frame has no ego pose");
-    frames.push_back(i);
-  }
+  if ((rc = rot_problem(h, "rot_init", *cfg, n_ego, ego_ids, ego_poses7, s))) return rc;
+  if ((rc = rot_frames(h, "rot_init", s, cfg->enable_gravity_prior != 0, frames))) return rc;
   d2pgo_rot_init_report R; memset(&R, 0, sizeof R);
   R.frames = (int)frames.size(); R.edges_used = (int)s.used.size(); R.edges_dropped = s.dropped;
-  cudaSetDevice(h->cfg.device);
-  PCK(cudaEventRecord(h->ev0, h->stream));
   std::vector<double> poses = h->poses;
-  if (!frames.empty()) {
-    // the inner handle: nodes = the handle's poses, then (gravity) one fixed virtual node per solved frame holding R_ego^T e3
-    std::vector<double> Rfix;
-    d2pgo_handle *r = rot_inner_edges(h, s.used, Rfix);
-    const int Nn = N + (grav ? (int)frames.size() : 0);
-    Buf<double> sol[3];
-    const double tol2 = cfg->pcg_tolerance * cfg->pcg_tolerance;
-    for (int k = 0; k < 3 && !rc; k++) {
-      r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
-      for (int f : frames) r->fixed[f] = 0;
-      r->poses.assign((size_t)Nn * 8, 0.0);
-      for (int i = 0; i < N; i++) if (r->fixed[i]) for (int c = 0; c < 3; c++) r->poses[(size_t)i * 8 + c] = Rfix[(size_t)i * 9 + k * 3 + c];
-      if (k == 2 && grav) rot_gravity_rows(r, N, frames, ego_of, ego_poses7, cfg->gravity_sqrt_info);
-      if ((rc = pgo_upload(r)) || (rc = rot_solve_row(r, tol2, cfg->pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) break;
-      if (sol[k].alloc(r->ids.size() * 8) != cudaSuccess ||
-          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, r->ids.size() * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = pgo_fail(h, 100, "rot_init: device buffer for a row system"); break; }
+  cudaSetDevice(h->cfg.device);
+  auto device = [&]() -> int {
+    PCK(cudaEventRecord(h->ev0, h->stream));
+    if (!frames.empty()) {
+      Buf<double> sol[3];
+      if ((rc = rot_solve_rows(h, *cfg, s, frames, ego_poses7, {}, 0.0, nullptr, nullptr, sol, R))) return rc;
+      auto project = [&](const int *fr, double *x, double *part, int nb) {
+        k_rotinit_project<<<nb, 128, 0, h->stream>>>((int)frames.size(), fr, sol[0].p, sol[1].p, sol[2].p, x, part);
+      };
+      if ((rc = rot_project(h, frames, poses, &R.state_changes, project))) return rc;
     }
-    if (rc && rc != 100) h->err = "rot_init: " + r->err;
-    Buf<double> x, part; Buf<int> fr;
-    const int F = (int)frames.size(), nb = (F + 127) / 128;
-    if (!rc && (x.alloc((size_t)N * 8) != cudaSuccess || part.alloc(nb) != cudaSuccess || fr.alloc(F) != cudaSuccess)) rc = pgo_fail(h, 100, "rot_init: device buffers");
-    if (!rc) {
-      double chg = 0.0;
-      cudaMemcpyAsync(x.p, poses.data(), (size_t)N * 64, cudaMemcpyHostToDevice, h->stream);
-      cudaMemcpyAsync(fr.p, frames.data(), (size_t)F * 4, cudaMemcpyHostToDevice, h->stream);
-      k_rotinit_project<<<nb, 128, 0, h->stream>>>(F, fr.p, sol[0].p, sol[1].p, sol[2].p, x.p, part.p);
-      k_pgo_sum<<<1, 128, 0, h->stream>>>(part.p, nb, r->d_cost.p);
-      cudaMemcpyAsync(&chg, r->d_cost.p, 8, cudaMemcpyDeviceToHost, h->stream);
-      cudaMemcpyAsync(poses.data(), x.p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream);
-      const cudaError_t e = cudaStreamSynchronize(h->stream);
-      if (e != cudaSuccess) rc = pgo_fail(h, 100 + (int)e, std::string("rot_init: projection: ") + cudaGetErrorString(e));
-      R.state_changes = chg / F;
-    }
-    if (rc) return rc;
-  }
-  PCK(cudaEventRecord(h->ev1, h->stream));
-  PCK(cudaEventSynchronize(h->ev1));
-  float ms = 0; cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  R.device_ms = ms;
+    return rot_device_ms(h, &R.device_ms);
+  };
+  if ((rc = device())) return pgo_fail(h, rc, "rot_init: " + h->err);
   h->poses.swap(poses);   // commit: the solved attitudes; the next d2pgo_solve uploads them
   h->uploaded = false;
   if (report) *report = R;
@@ -1886,7 +1971,7 @@ static double rot_dual_weight(double rho_rot_mat) { return std::sqrt(3.0 * rho_r
 static int rot_arock_check(d2pgo_handle *h, const char *what, bool changes) {
   if (h->dof != 6) return pgo_fail(h, 5, std::string(what) + ": the handle was created with pose_dof = 4; rotation initialisation acts on 6-DoF poses");
   if (!h->arock) return pgo_fail(h, 5, std::string(what) + ": the handle is not in ARock mode (d2pgo_arock_enable)");
-  if (changes && !h->duals.empty()) return pgo_fail(h, 5, std::string(what) + ": the ARock pose dual table is not empty (rotation initialisation precedes the perturbation solve)");
+  if (changes && !h->pose_table.duals.empty()) return pgo_fail(h, 5, std::string(what) + ": the ARock pose dual table is not empty (rotation initialisation precedes the perturbation solve)");
   return 0;
 }
 
@@ -1902,14 +1987,12 @@ int d2pgo_default_arock_rot_init_config(d2pgo_arock_rot_init_config *c) {
 int d2pgo_arock_rot_receive(d2pgo_handle *h, int32_t sender, int32_t target, int32_t n, const int64_t *frame_ids, int32_t dim,
                             const double *duals, const double *poses7) {
   if (!h) return 1;
-  if (int rc = rot_arock_check(h, "arock_rot_receive", true)) return rc;
-  if (n < 0 || (n > 0 && (!frame_ids || !duals || !poses7))) return pgo_fail(h, 1, "arock_rot_receive: null argument or negative count");
-  if (dim != 9) return pgo_fail(h, 2, "arock_rot_receive: duals of dimension " + std::to_string(dim) + " (a rotation dual is a 3x3 matrix, 9)");
-  if (sender == h->acfg.self_id) return pgo_fail(h, 2, "arock_rot_receive: a message from this agent itself (self_id " + std::to_string(sender) + ")");
-  if (!all_finite(duals, (size_t)n * 9) || !all_finite(poses7, (size_t)n * 7)) return pgo_fail(h, 2, "arock_rot_receive: non-finite dual or pose");
-  std::unordered_map<int64_t, int> seen;
+  int rc;
+  if ((rc = rot_arock_check(h, "arock_rot_receive", true))) return rc;
+  if (n > 0 && !poses7) return pgo_fail(h, 1, "arock_rot_receive: null argument or negative count");
+  if ((rc = arock_receive_check(h, "arock_rot_receive", 9, sender, n, frame_ids, dim, duals))) return rc;
+  if (!all_finite(poses7, (size_t)n * 7)) return pgo_fail(h, 2, "arock_rot_receive: non-finite pose");
   for (int k = 0; k < n; k++) {
-    if (!seen.emplace(frame_ids[k], k).second) return pgo_fail(h, 2, "arock_rot_receive: frame id " + std::to_string(frame_ids[k]) + " twice in one message");
     const double *q = poses7 + (size_t)k * 7 + 3;
     if (!(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3] > 0.0)) return pgo_fail(h, 2, "arock_rot_receive: frame id " + std::to_string(frame_ids[k]) + ": zero quaternion");
   }
@@ -1925,7 +2008,7 @@ int d2pgo_arock_rot_receive(d2pgo_handle *h, int32_t sender, int32_t target, int
     h->qinit[frame_ids[k]] = {q[0] * s, q[1] * s, q[2] * s, q[3] * s};
     h->uploaded = false;
   }
-  h->rot_inbox.push_back(d2pgo_handle::Msg{sender, target, std::vector<int64_t>(frame_ids, frame_ids + n), std::vector<double>(duals, duals + (size_t)n * 9)});
+  arock_queue(h->rot_table, sender, target, n, frame_ids, 9, duals);
   return 0;
 }
 
@@ -1937,58 +2020,38 @@ int d2pgo_arock_rot_init_step(d2pgo_handle *h, const d2pgo_arock_rot_init_config
   if ((rc = rot_arock_check(h, "arock_rot_init_step", true))) return rc;
   if (h->ids.empty()) return pgo_fail(h, 1, "arock_rot_init_step: the handle has no poses");
   if ((rc = arock_check_poses(h, "arock_rot_init_step"))) return rc;
-  if (!(std::isfinite(cfg->pcg_tolerance) && cfg->pcg_tolerance >= 0.0) || cfg->pcg_max_iterations < 0 ||
-      (cfg->enable_gravity_prior && !std::isfinite(cfg->gravity_sqrt_info)) || !(std::isfinite(cfg->rho_rot_mat) && cfg->rho_rot_mat >= 0.0))
-    return pgo_fail(h, 2, "arock_rot_init_step: non-finite or negative pcg_tolerance, gravity_sqrt_info, rho_rot_mat or pcg_max_iterations");
+  d2pgo_rot_init_config rcfg;   // the fields the two configs share
+  rcfg.enable_gravity_prior = cfg->enable_gravity_prior; rcfg.pcg_max_iterations = cfg->pcg_max_iterations;
+  rcfg.gravity_sqrt_info = cfg->gravity_sqrt_info; rcfg.pcg_tolerance = cfg->pcg_tolerance;
+  RotProblem s;
+  if ((rc = rot_problem(h, "arock_rot_init_step", rcfg, n_ego, ego_ids, ego_poses7, s))) return rc;
+  if (!(std::isfinite(cfg->rho_rot_mat) && cfg->rho_rot_mat >= 0.0)) return pgo_fail(h, 2, "arock_rot_init_step: non-finite or negative rho_rot_mat");
   const int N = (int)h->ids.size(), self = h->acfg.self_id;
-  const bool grav = cfg->enable_gravity_prior != 0;
-  std::vector<int> ego_of;
-  if ((rc = rot_ego_index(h, "arock_rot_init_step", n_ego, ego_ids, ego_poses7, ego_of))) return rc;
-  RotEdges s;
-  if ((rc = rot_scan_edges(h, "arock_rot_init_step", s))) return rc;
-  // 1. receiveAll / processPGOData (:104-111, :142-182) on a copy of the table, messages in arrival order: a frame the problem
-  // estimates (an edge names it), if target == self or there is no dual (sender, f) yet: created with zeros if missing, y_r set,
-  // and y_l set too when it was just created
-  auto duals = h->rot_duals;
-  for (const auto &m : h->rot_inbox)
-    for (size_t k = 0; k < m.frames.size(); k++) {
-      auto it = h->index.find(m.frames[k]);
-      if (it == h->index.end() || !s.named[it->second]) continue;
-      const auto key = std::make_pair(m.sender, m.frames[k]);
-      auto d = duals.find(key);
-      if (m.target != self && d != duals.end()) continue;
-      const double *v = &m.duals[k * 9];
-      if (d == duals.end()) { d2pgo_handle::RotDual nd; memcpy(nd.yl, v, 72); memcpy(nd.yr, v, 72); duals.emplace(key, nd); }
-      else memcpy(d->second.yr, v, 72);
-    }
+  // 1. receiveAll / processPGOData on a copy of the table, for the frames the problem estimates (an edge names them)
+  auto duals = h->rot_table.duals;
+  arock_apply_inbox(h, h->rot_table, s.named, 9, duals);
   // 3. scanAndCreateDualStates (:79-102): every edge end another agent owns gets the dual (owner, f), zero, if it has none
   for (size_t e = 0; e < h->ea.size(); e++)
     for (int i : {h->ea[e], h->eb[e]}) {
       const int32_t o = h->owner.at(h->ids[i]);
       if (o == self) continue;
       const auto key = std::make_pair(o, h->ids[i]);
-      if (!duals.count(key)) { d2pgo_handle::RotDual nd; memset(&nd, 0, sizeof nd); duals.emplace(key, nd); }
+      if (!duals.count(key)) { d2pgo_host::ArockDual<9> nd; memset(&nd, 0, sizeof nd); duals.emplace(key, nd); }
     }
   // 4. setDualStateFactors (:32-61): a prior per dual on a free frame; with the fixed-frame edge rows they anchor the components
-  std::vector<int> dual_pose, prior_dual;
-  std::vector<char> anchored(N, 0);
-  for (int e : s.used) if (h->fixed[h->ea[e]]) anchored[rot_find(s.uf, h->eb[e])] = 1;
+  std::vector<int> dual_pose, prior_dual, prior_pose;
   for (const auto &kv : duals) {
     const int i = h->index.at(kv.first.second);
-    if (!h->fixed[i]) { prior_dual.push_back((int)dual_pose.size()); anchored[rot_find(s.uf, i)] = 1; }
+    if (!h->fixed[i]) { prior_dual.push_back((int)dual_pose.size()); prior_pose.push_back(i); s.anchored[rot_find(s.uf, i)] = 1; }
     dual_pose.push_back(i);
   }
-  std::vector<int> frames;   // the free frames solved, ascending pose index
+  for (int i = 0; i < N; i++)
+    if (s.named[i] && h->fixed[i] && !all_finite(&h->poses[(size_t)i * 8 + 3], 4))
+      return pgo_fail(h, 2, "arock_rot_init_step: frame id " + std::to_string(h->ids[i]) + ": non-finite attitude");
+  std::vector<int> frames;
+  if ((rc = rot_frames(h, "arock_rot_init_step", s, rcfg.enable_gravity_prior != 0, frames))) return rc;
   std::vector<unsigned char> owned;
-  for (int i = 0; i < N; i++) {
-    if (!s.named[i]) continue;
-    const std::string fid = "arock_rot_init_step: frame id " + std::to_string(h->ids[i]);
-    if (!all_finite(&h->poses[(size_t)i * 8 + 3], 4)) return pgo_fail(h, 2, fid + ": non-finite attitude");
-    if (h->fixed[i]) continue;
-    if (!anchored[rot_find(s.uf, i)]) return pgo_fail(h, 2, fid + ": its component of free frames has no fixed-frame row and no dual prior (A^T A is singular)");
-    if (grav && ego_of[i] < 0) return pgo_fail(h, 2, fid + ": gravity rows are on and the frame has no ego pose");
-    frames.push_back(i); owned.push_back(h->owner.at(h->ids[i]) == self);
-  }
+  for (int i : frames) owned.push_back(h->owner.at(h->ids[i]) == self);
   // R_state of every named frame: kept, or R(attitude) when the frame first enters a step (PGOState::addFrame)
   std::vector<double> rstate((size_t)N * 9, 0.0);
   for (int i = 0; i < N; i++) {
@@ -1998,80 +2061,49 @@ int d2pgo_arock_rot_init_step(d2pgo_handle *h, const d2pgo_arock_rot_init_config
   }
   const int K = (int)duals.size(), P = (int)prior_dual.size(), F = (int)frames.size();
   std::vector<double> yl((size_t)K * 9), yr((size_t)K * 9);
-  { size_t k = 0;
-    for (const auto &kv : duals) { memcpy(&yl[k * 9], kv.second.yl, 72); memcpy(&yr[k * 9], kv.second.yr, 72); k++; } }
+  arock_flatten(duals.begin(), duals.end(), 9, yl.data(), yr.data());
   d2pgo_rot_init_report R; memset(&R, 0, sizeof R);
   R.frames = F; R.edges_used = (int)s.used.size(); R.edges_dropped = s.dropped;
-  cudaSetDevice(h->cfg.device);
-  PCK(cudaEventRecord(h->ev0, h->stream));
-  // the dual table and the rotation states to the device
-  PCK(h->d_rk_pose.alloc(K)); PCK(h->d_rk_prior.alloc(P)); PCK(h->d_rk_yl.alloc((size_t)K * 9)); PCK(h->d_rk_yr.alloc((size_t)K * 9));
-  PCK(h->d_rk_state.alloc((size_t)N * 9));
-  if (K) {
-    PCK(cudaMemcpyAsync(h->d_rk_pose.p, dual_pose.data(), (size_t)K * 4, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(h->d_rk_yl.p, yl.data(), (size_t)K * 72, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(h->d_rk_yr.p, yr.data(), (size_t)K * 72, cudaMemcpyHostToDevice, h->stream));
-  }
-  if (P) PCK(cudaMemcpyAsync(h->d_rk_prior.p, prior_dual.data(), (size_t)P * 4, cudaMemcpyHostToDevice, h->stream));
-  PCK(cudaMemcpyAsync(h->d_rk_state.p, rstate.data(), (size_t)N * 72, cudaMemcpyHostToDevice, h->stream));
   std::vector<double> poses = h->poses;
-  double chg = 0.0;
-  if (F) {
-    // 5. solveLinearRot (base :178-213): nodes = the handle's poses, then one fixed virtual node per dual prior, then (k = 2,
-    // gravity) one per solved frame; rows = the used edges, the dual priors, the gravity rows
-    std::vector<double> Rfix;
-    d2pgo_handle *r = rot_inner_edges(h, s.used, Rfix);
-    const double w = rot_dual_weight(cfg->rho_rot_mat), Sw[9] = {w, 0, 0, 0, w, 0, 0, 0, w}, I[8] = {0, 0, 0, 0, 0, 0, 1, 0};
-    for (int j = 0; j < P; j++) {
-      r->ea.push_back(N + j); r->eb.push_back(dual_pose[prior_dual[j]]);
-      r->rel.insert(r->rel.end(), I, I + 8); r->sinfo.insert(r->sinfo.end(), Sw, Sw + 9);
+  cudaSetDevice(h->cfg.device);
+  auto device = [&]() -> int {
+    PCK(cudaEventRecord(h->ev0, h->stream));
+    // the dual table and the rotation states to the device
+    PCK(h->d_rk_pose.alloc(K)); PCK(h->d_rk_prior.alloc(P)); PCK(h->d_rk_yl.alloc((size_t)K * 9)); PCK(h->d_rk_yr.alloc((size_t)K * 9));
+    PCK(h->d_rk_state.alloc((size_t)N * 9));
+    if (K) {
+      PCK(cudaMemcpyAsync(h->d_rk_pose.p, dual_pose.data(), (size_t)K * 4, cudaMemcpyHostToDevice, h->stream));
+      PCK(cudaMemcpyAsync(h->d_rk_yl.p, yl.data(), (size_t)K * 72, cudaMemcpyHostToDevice, h->stream));
+      PCK(cudaMemcpyAsync(h->d_rk_yr.p, yr.data(), (size_t)K * 72, cudaMemcpyHostToDevice, h->stream));
     }
-    const int Nn = N + P + (grav ? F : 0);
-    Buf<double> sol[3];
-    const double tol2 = cfg->pcg_tolerance * cfg->pcg_tolerance;
-    for (int k = 0; k < 3 && !rc; k++) {
-      r->ids.assign(Nn, 0); r->fixed.assign(Nn, 1);
-      for (int f : frames) r->fixed[f] = 0;
-      r->poses.assign((size_t)Nn * 8, 0.0);
-      for (int i = 0; i < N; i++) if (r->fixed[i]) for (int c = 0; c < 3; c++) r->poses[(size_t)i * 8 + c] = Rfix[(size_t)i * 9 + k * 3 + c];
-      if (k == 2 && grav) rot_gravity_rows(r, N + P, frames, ego_of, ego_poses7, cfg->gravity_sqrt_info);
-      if ((rc = pgo_upload(r))) break;
-      if (P) k_rotinit_arock_targets<<<(P + 127) / 128, 128, 0, h->stream>>>(P, k, h->d_rk_prior.p, h->d_rk_yr.p, r->d_x[0].p + (size_t)N * 8);
-      if ((rc = rot_solve_row(r, tol2, cfg->pcg_max_iterations, &R.pcg_iterations[k], &R.residual[k]))) break;
-      if (sol[k].alloc(r->ids.size() * 8) != cudaSuccess ||
-          cudaMemcpyAsync(sol[k].p, r->d_x[1].p, r->ids.size() * 64, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) { rc = pgo_fail(h, 100, "arock_rot_init_step: device buffer for a row system"); break; }
+    if (P) PCK(cudaMemcpyAsync(h->d_rk_prior.p, prior_dual.data(), (size_t)P * 4, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemcpyAsync(h->d_rk_state.p, rstate.data(), (size_t)N * 72, cudaMemcpyHostToDevice, h->stream));
+    if (F) {
+      // 5. solveLinearRot, with the dual priors
+      Buf<double> sol[3];
+      if ((rc = rot_solve_rows(h, rcfg, s, frames, ego_poses7, prior_pose, rot_dual_weight(cfg->rho_rot_mat), h->d_rk_prior.p, h->d_rk_yr.p, sol, R))) return rc;
+      // 6. recoverRotationLLT: R_state = M, the owned frames' attitudes; state_changes = the mean over the free frames
+      Buf<unsigned char> own;
+      PCK(own.alloc(F));
+      PCK(cudaMemcpyAsync(own.p, owned.data(), (size_t)F, cudaMemcpyHostToDevice, h->stream));
+      auto project = [&](const int *fr, double *x, double *part, int nb) {
+        k_rotinit_arock_project<<<nb, 128, 0, h->stream>>>(F, fr, own.p, sol[0].p, sol[1].p, sol[2].p, h->d_rk_state.p, x, part);
+      };
+      if ((rc = rot_project(h, frames, poses, &R.state_changes, project))) return rc;
     }
-    if (rc && rc != 100) h->err = "arock_rot_init_step: " + r->err;
-    if (rc) return rc;
-    // 6. recoverRotationLLT: R_state = M, the owned frames' attitudes; state_changes = the mean over the free frames
-    Buf<double> x, part; Buf<int> fr; Buf<unsigned char> own;
-    const int nb = (F + 127) / 128;
-    PCK(x.alloc((size_t)N * 8)); PCK(part.alloc(nb)); PCK(fr.alloc(F)); PCK(own.alloc(F));
-    PCK(cudaMemcpyAsync(x.p, poses.data(), (size_t)N * 64, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(fr.p, frames.data(), (size_t)F * 4, cudaMemcpyHostToDevice, h->stream));
-    PCK(cudaMemcpyAsync(own.p, owned.data(), (size_t)F, cudaMemcpyHostToDevice, h->stream));
-    k_rotinit_arock_project<<<nb, 128, 0, h->stream>>>(F, fr.p, own.p, sol[0].p, sol[1].p, sol[2].p, h->d_rk_state.p, x.p, part.p);
-    k_pgo_sum<<<1, 128, 0, h->stream>>>(part.p, nb, r->d_cost.p);
+    // 7. updateDualStates on every dual, at R_state
+    if (K) k_rotinit_arock_update<<<(K + 127) / 128, 128, 0, h->stream>>>(K, h->d_rk_pose.p, h->d_rk_state.p, h->d_rk_yr.p, h->d_rk_yl.p, h->acfg.eta_k);
     PCK(cudaGetLastError());
-    PCK(cudaMemcpyAsync(&chg, r->d_cost.p, 8, cudaMemcpyDeviceToHost, h->stream));
-    PCK(cudaMemcpyAsync(poses.data(), x.p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream));
-  }
-  // 7. updateDualStates on every dual, at R_state
-  if (K) k_rotinit_arock_update<<<(K + 127) / 128, 128, 0, h->stream>>>(K, h->d_rk_pose.p, h->d_rk_state.p, h->d_rk_yr.p, h->d_rk_yl.p, h->acfg.eta_k);
-  PCK(cudaGetLastError());
-  if (K) PCK(cudaMemcpyAsync(yl.data(), h->d_rk_yl.p, (size_t)K * 72, cudaMemcpyDeviceToHost, h->stream));
-  PCK(cudaMemcpyAsync(rstate.data(), h->d_rk_state.p, (size_t)N * 72, cudaMemcpyDeviceToHost, h->stream));
-  PCK(cudaEventRecord(h->ev1, h->stream));
-  PCK(cudaEventSynchronize(h->ev1));
-  float ms = 0; cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  R.device_ms = ms;
-  R.state_changes = F ? chg / F : 0.0;
+    if (K) PCK(cudaMemcpyAsync(yl.data(), h->d_rk_yl.p, (size_t)K * 72, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaMemcpyAsync(rstate.data(), h->d_rk_state.p, (size_t)N * 72, cudaMemcpyDeviceToHost, h->stream));
+    return rot_device_ms(h, &R.device_ms);
+  };
+  if ((rc = device())) return pgo_fail(h, rc, "arock_rot_init_step: " + h->err);
   // commit: the table, the states of the named frames, the owned frames' attitudes and their q_init (so that the first
   // d2pgo_arock_step starts from theta = 0 at them); the inbox has been processed
-  { size_t k = 0;
-    for (auto &kv : duals) { memcpy(kv.second.yl, &yl[k * 9], 72); k++; } }
-  h->rot_duals.swap(duals);
-  h->rot_inbox.clear();
+  arock_set_yl(duals, 9, yl.data());
+  h->rot_table.duals.swap(duals);
+  h->rot_table.inbox.clear();
   for (int i = 0; i < N; i++) if (s.named[i]) memcpy(h->rot_state[h->ids[i]].data(), &rstate[(size_t)i * 9], 72);
   for (size_t j = 0; j < frames.size(); j++) {
     if (!owned[j]) continue;
@@ -2088,31 +2120,16 @@ int d2pgo_arock_rot_init_step(d2pgo_handle *h, const d2pgo_arock_rot_init_config
 int d2pgo_arock_rot_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out) {
   if (!h) return 1;
   if (int rc = rot_arock_check(h, "arock_rot_neighbours", false)) return rc;
-  if (!n_out || max_n < 0 || (max_n > 0 && !ids_out)) return pgo_fail(h, 1, "arock_rot_neighbours: null argument or negative count");
-  std::vector<int32_t> nb;
-  for (const auto &kv : h->rot_duals) if (nb.empty() || nb.back() != kv.first.first) nb.push_back(kv.first.first);
-  *n_out = (int32_t)nb.size();
-  if ((int32_t)nb.size() > max_n) return pgo_fail(h, 2, "arock_rot_neighbours: room for " + std::to_string(max_n) + " ids, " + std::to_string(nb.size()) + " needed");
-  std::copy(nb.begin(), nb.end(), ids_out);
-  return 0;
+  return arock_neighbours(h, h->rot_table, "arock_rot_neighbours", max_n, n_out, ids_out);
 }
 
 int d2pgo_arock_rot_duals(d2pgo_handle *h, int32_t neighbour, int32_t max_n, int32_t *n_out, int64_t *frame_ids, double *local9,
                           double *remote9, double *poses7) {
   if (!h) return 1;
-  if (int rc = rot_arock_check(h, "arock_rot_duals", false)) return rc;
-  if (!n_out || max_n < 0 || (max_n > 0 && (!frame_ids || !local9))) return pgo_fail(h, 1, "arock_rot_duals: null argument or negative count");
-  auto lo = h->rot_duals.lower_bound(std::make_pair(neighbour, INT64_MIN)), hi = h->rot_duals.upper_bound(std::make_pair(neighbour, INT64_MAX));
-  const int32_t cnt = (int32_t)std::distance(lo, hi);
-  *n_out = cnt;
-  if (cnt > max_n) return pgo_fail(h, 2, "arock_rot_duals: room for " + std::to_string(max_n) + " duals, " + std::to_string(cnt) + " needed");
-  int k = 0;
-  for (auto it = lo; it != hi; ++it, ++k) {
-    frame_ids[k] = it->first.second;
-    memcpy(local9 + (size_t)k * 9, it->second.yl, 72);
-    if (remote9) memcpy(remote9 + (size_t)k * 9, it->second.yr, 72);
-    if (poses7) memcpy(poses7 + (size_t)k * 7, &h->poses[(size_t)h->index.at(it->first.second) * 8], 56);
-  }
+  int rc;
+  if ((rc = rot_arock_check(h, "arock_rot_duals", false))) return rc;
+  if ((rc = arock_export(h, h->rot_table, "arock_rot_duals", 9, neighbour, max_n, n_out, frame_ids, local9, remote9))) return rc;
+  if (poses7) for (int k = 0; k < *n_out; k++) memcpy(poses7 + (size_t)k * 7, &h->poses[(size_t)h->index.at(frame_ids[k]) * 8], 56);
   return 0;
 }
 
@@ -2130,15 +2147,13 @@ int d2pgo_debug_arock_rot_state(d2pgo_handle *h, double *state9_out, uint8_t *fl
     for (int c = 0; c < 9; c++) state9_out[i * 9 + c] = it == h->rot_state.end() ? 0.0 : it->second[c];
     flag_out[i] = !named[i] ? 0 : h->fixed[i] ? 2 : 1;
   }
-  const int32_t K = (int32_t)h->rot_duals.size();
+  const auto &duals = h->rot_table.duals;
+  const int32_t K = (int32_t)duals.size();
   *n_duals_out = K;
   if (K > max_duals) return pgo_fail(h, 2, "debug_arock_rot_state: room for " + std::to_string(max_duals) + " duals, " + std::to_string(K) + " needed");
   int k = 0;
-  for (const auto &kv : h->rot_duals) {
-    neighbour_out[k] = kv.first.first; frame_out[k] = kv.first.second;
-    memcpy(local9_out + (size_t)k * 9, kv.second.yl, 72); memcpy(remote9_out + (size_t)k * 9, kv.second.yr, 72);
-    k++;
-  }
+  for (const auto &kv : duals) { neighbour_out[k] = kv.first.first; frame_out[k] = kv.first.second; k++; }
+  arock_flatten(duals.begin(), duals.end(), 9, local9_out, remote9_out);
   return 0;
 }
 

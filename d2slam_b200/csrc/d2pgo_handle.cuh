@@ -25,6 +25,14 @@ struct PgoScalars {      // device-resident CG state that is not a per-block par
   int done, iters;
 };
 
+// an ARock dual table: the duals keyed (neighbour, frame id) in ascending order, y_l and y_r of up to W doubles each (the
+// exchange's width: the pose table's is the pose dof, 4 or 6; the rotation table's 9, a row-major 3x3 matrix), and the
+// messages received since the last step (duals [n][width])
+template <int W> struct ArockDual { double yl[W], yr[W]; };
+template <int W> using ArockDuals = std::map<std::pair<int32_t, int64_t>, ArockDual<W>>;
+struct ArockMsg { int32_t sender, target; std::vector<int64_t> frames; std::vector<double> duals; };
+template <int W> struct ArockTable { ArockDuals<W> duals; std::vector<ArockMsg> inbox; };
+
 struct PcmBufs;                                               // d2pgo_pcm.cu
 struct PcmBufsFree { void operator()(PcmBufs *p) const; };    // defined beside PcmBufs
 
@@ -52,25 +60,19 @@ struct d2pgo_handle {
   bool uploaded = false;
   void *comm = nullptr; int rank = 0, nranks = 1;
   std::unique_ptr<d2pgo_host::PcmBufs, d2pgo_host::PcmBufsFree> pcm;   // d2pgo_pcm's device buffers, from its first call
-  // ARock (d2pgo_arock_enable): owner agent and 6-DoF q_init per pose id, the dual table keyed (neighbour, frame id) in
-  // ascending order, the messages received since the last step, and the device copy of the table (in table order)
+  // ARock (d2pgo_arock_enable): owner agent and 6-DoF q_init per pose id, the pose dual table, and the device copy of the table
+  // (in table order)
   bool arock = false; d2pgo_arock_config acfg = {};
   std::unordered_map<int64_t, int32_t> owner; std::unordered_map<int64_t, std::array<double, 4>> qinit;
-  struct Dual { double yl[6], yr[6]; };
-  struct Msg { int32_t sender, target; std::vector<int64_t> frames; std::vector<double> duals; };
-  std::map<std::pair<int32_t, int64_t>, Dual> duals;
-  std::vector<Msg> inbox;
+  d2pgo_host::ArockTable<6> pose_table;
   Buf<int> d_ak_pose, d_ak_ptr, d_ak_of; Buf<double> d_ak_yr, d_ak_yl, d_ak_qinit, d_ak_lin[2], d_ak_coord;
   int ak_n = -1;                      // duals on the device, -1 = none synced
-  // distributed rotation initialisation (d2pgo_arock_rot_*): its own dual table keyed (neighbour, frame id) ascending, y_l and
-  // y_r being row-major 3x3 matrices, the messages received since the last step (duals [n][9]), each frame's rotation state
-  // R_state (row-major; R(attitude) when the frame first enters a step, then the last unprojected M), and the device copies
-  struct RotDual { double yl[9], yr[9]; };
-  std::map<std::pair<int32_t, int64_t>, RotDual> rot_duals;
-  std::vector<Msg> rot_inbox;
+  // distributed rotation initialisation (d2pgo_arock_rot_*): its own dual table, each frame's rotation state R_state
+  // (row-major; R(attitude) when the frame first enters a step, then the last unprojected M), and the device copies
+  d2pgo_host::ArockTable<9> rot_table;
   std::unordered_map<int64_t, std::array<double, 9>> rot_state;
   Buf<int> d_rk_pose, d_rk_prior; Buf<double> d_rk_yl, d_rk_yr, d_rk_state;
-  std::unique_ptr<d2pgo_handle> rot;  // d2pgo_rot_init's row systems (dof 3), kept between calls for their buffers
+  std::unique_ptr<d2pgo_handle> rot;  // the row systems (dof 3) of both rotation initialisations, kept between calls for their buffers
   int linear_solver = D2PGO_LINEAR_PCG;   // d2pgo_set_linear_solver
   std::unique_ptr<d2pgo_chol::Numeric> chol;   // the sparse Cholesky's analysis and device state (d2pgo_chol.cu)
 

@@ -245,14 +245,17 @@ class PgoSolver:
         no edge names are kept.  cfg overrides RotInitConfig fields (enable_gravity_prior, pcg_max_iterations,
         gravity_sqrt_info, pcg_tolerance); with enable_gravity_prior every free frame an edge names needs an ego pose
         [x y z qx qy qz qw] in ego_ids / ego_poses7.  6-DoF only.  Returns the report as a dict."""
-        c = RotInitConfig()
-        _lib().d2pgo_default_rot_init_config(C.byref(c))
+        return self._rot_init_call("rot_init", RotInitConfig(), _lib().d2pgo_default_rot_init_config, ego_ids, ego_poses7, cfg)
+
+    def _rot_init_call(self, name, c, default, ego_ids, ego_poses7, cfg):
+        """d2pgo_<name>(h, &c, n_ego, ego_ids, ego_poses7, &report), c filled by default(&c) and then cfg's overrides."""
+        default(C.byref(c))
         for k, v in cfg.items():
             setattr(c, k, v)
         ids = np.zeros(0, np.int64) if ego_ids is None else np.ascontiguousarray(ego_ids, np.int64)
         ego = np.zeros((0, 7)) if ego_poses7 is None else np.ascontiguousarray(np.asarray(ego_poses7, np.float64).reshape(-1, 7))
         r = RotInitReport()
-        self._chk(_lib().d2pgo_rot_init(self.h, C.byref(c), C.c_int32(len(ids)), _p(ids), _p(ego), C.byref(r)), "rot_init")
+        self._chk(getattr(_lib(), f"d2pgo_{name}")(self.h, C.byref(c), C.c_int32(len(ids)), _p(ids), _p(ego), C.byref(r)), name)
         return _rot_report(r)
 
     def comm_init(self, unique_id, rank, nranks):
@@ -358,15 +361,8 @@ class PgoSolver:
     def arock_rot_init_step(self, ego_ids=None, ego_poses7=None, **cfg):
         """One RotationInitARock step on this ARock handle; cfg overrides ArockRotInitConfig fields (enable_gravity_prior,
         pcg_max_iterations, gravity_sqrt_info, pcg_tolerance, rho_rot_mat).  Returns the report as a dict."""
-        c = ArockRotInitConfig()
-        _lib().d2pgo_default_arock_rot_init_config(C.byref(c))
-        for k, v in cfg.items():
-            setattr(c, k, v)
-        ids = np.zeros(0, np.int64) if ego_ids is None else np.ascontiguousarray(ego_ids, np.int64)
-        ego = np.zeros((0, 7)) if ego_poses7 is None else np.ascontiguousarray(np.asarray(ego_poses7, np.float64).reshape(-1, 7))
-        r = RotInitReport()
-        self._chk(_lib().d2pgo_arock_rot_init_step(self.h, C.byref(c), C.c_int32(len(ids)), _p(ids), _p(ego), C.byref(r)), "arock_rot_init_step")
-        return _rot_report(r)
+        return self._rot_init_call("arock_rot_init_step", ArockRotInitConfig(), _lib().d2pgo_default_arock_rot_init_config, ego_ids,
+                                   ego_poses7, cfg)
 
     def arock_rot_receive(self, sender, target, frame_ids, duals, poses7, dim=9):
         f = np.ascontiguousarray(frame_ids, np.int64)

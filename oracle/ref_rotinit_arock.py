@@ -1,32 +1,17 @@
 """ctypes front-end of oracle/_ref/libd2ref_rotinit_arock.so: the REFERENCE's own distributed rotation initialisation
 (RotationInitARock<double> in d2pgo/src/rot_init/rotation_initialization_arock.hpp on ARockBase, d2common/src/solver/ARock.cpp)
-compiled unmodified by oracle/Makefile.rotinit_arock against the stand-in headers of oracle/_shim.
+compiled unmodified by oracle/Makefile.ref against the stand-in headers of oracle/_shim.
 
 TEST INFRASTRUCTURE ONLY: used by tests/test_pgo_rotinit_arock.py (oracle/pgo_rotinit_arock_oracle.py == reference) and by
 tests/golden/make_ref_rotinit_arock_golden.py.  Nothing under d2slam_b200/ imports it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle.ref import _HERE, REF_ROOT, Pin, _p
+from oracle.ref import Pin, _p
 
-
-class _Pin(Pin):
-    """Pin, built by its own makefile"""
-
-    def build(self, force=False):
-        so = self.so_path()
-        if self._buildable():
-            subprocess.check_call(["make", "-C", _HERE, "-f", "Makefile.rotinit_arock", "-s", f"REF={REF_ROOT}", f"_ref/{self.name}"] + (["-B"] if force else []))
-        if not os.path.exists(so):
-            raise RuntimeError(f"oracle/_ref/{self.name} missing and the reference tree is not present to build it")
-        return so
-
-
-_PIN = _Pin("libd2ref_rotinit_arock.so", "d2pgo")
+_PIN = Pin("libd2ref_rotinit_arock.so", "d2pgo")
 so_path, available, build, lib = _PIN.so_path, _PIN.available, _PIN.build, _PIN.lib
 
 

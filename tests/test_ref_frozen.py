@@ -1,6 +1,6 @@
 """Every reference pin library still computes its frozen golden file, bit for bit.
 
-All five libraries of oracle/Makefile.ref are built against the one stand-in tree oracle/_shim, so an edit made there for one
+All six libraries of oracle/Makefile.ref are built against the one stand-in tree oracle/_shim, so an edit made there for one
 pin can change what another computes.  This test reruns each tests/golden/make_ref_*_golden.py generator through the live
 library and compares every array with the committed tests/golden/ref_*.npz: same keys, dtype, shape and bytes.  The one
 exception is the reference Marginalizer's output in ref_factors.npz (marg*_refs / _x0 / _J / _e0): it orders the kept blocks
@@ -15,7 +15,7 @@ import sys
 import numpy as np
 import pytest
 
-from oracle import ref, ref_arock, ref_gravity, ref_pcm, ref_rotinit
+from oracle import ref, ref_arock, ref_gravity, ref_pcm, ref_rotinit, ref_rotinit_arock
 
 import test_ref_pin as trp
 
@@ -30,6 +30,7 @@ PINS = {
     "ref_gravity": ("make_ref_gravity_golden", ref_gravity),
     "ref_arock": ("make_ref_arock_golden", ref_arock),
     "ref_rotinit": ("make_ref_rotinit_golden", ref_rotinit),
+    "ref_rotinit_arock": ("make_ref_rotinit_arock_golden", ref_rotinit_arock),
     "ref_lin_edges": ("make_ref_lin_edges_golden", ref),
 }
 MARG = re.compile(r"marg(\d+)_(refs|x0|J|e0)")
