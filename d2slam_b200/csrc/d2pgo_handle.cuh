@@ -35,6 +35,8 @@ template <int W> struct ArockTable { ArockDuals<W> duals; std::vector<ArockMsg> 
 
 struct PcmBufs;                                               // d2pgo_pcm.cu
 struct PcmBufsFree { void operator()(PcmBufs *p) const; };    // defined beside PcmBufs
+struct PcmStream;                                             // d2pgo_pcm.cu
+struct PcmStreamFree { void operator()(PcmStream *p) const; };
 
 }  // namespace d2pgo_host
 
@@ -60,6 +62,7 @@ struct d2pgo_handle {
   bool uploaded = false;
   void *comm = nullptr; int rank = 0, nranks = 1;
   std::unique_ptr<d2pgo_host::PcmBufs, d2pgo_host::PcmBufsFree> pcm;   // d2pgo_pcm's device buffers, from its first call
+  std::unique_ptr<d2pgo_host::PcmStream, d2pgo_host::PcmStreamFree> pcm_stream;   // the PCM stream, from d2pgo_pcm_stream_reset
   // ARock (d2pgo_arock_enable): owner agent and 6-DoF q_init per pose id, the pose dual table, and the device copy of the table
   // (in table order)
   bool arock = false; d2pgo_arock_config acfg = {};

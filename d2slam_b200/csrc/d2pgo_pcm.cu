@@ -194,10 +194,11 @@ __global__ void k_pcm_degree(int G, const int *g_loop, const long long *g_word, 
 }
 
 // FMC's greedy from seed s under the running maximum m (findCliqueHeu.cpp:146-239): C = N(s) & {deg >= m}; repeat
-// v = max C, C &= N(v).  One warp; C in shared memory, word k owned by lane k % 32.  Returns the clique size 1 + picks, or 0
-// once the clique can no longer exceed m (1 + picks + |C| <= m): such a seed is never taken, so stopping early changes nothing.
-D2BA_DEV int pcm_greedy(int s, int m, const unsigned *rows, int W, const unsigned *degmask, unsigned *C, int lane, long long *rounds, unsigned char *member) {
-  for (int k = lane; k < W; k += 32) C[k] = rows[(size_t)s * W + k] & degmask[k];
+// v = max C, C &= N(v).  One warp; rows `pitch` words apart; C in shared memory, word k owned by lane k % 32.  Returns the
+// clique size 1 + picks, or 0 once the clique can no longer exceed m (1 + picks + |C| <= m): such a seed is never taken, so
+// stopping early changes nothing.
+template <typename Pitch> D2BA_DEV int pcm_greedy(int s, int m, const unsigned *rows, Pitch pitch, int W, const unsigned *degmask, unsigned *C, int lane, long long *rounds, unsigned char *member) {
+  for (int k = lane; k < W; k += 32) C[k] = rows[(size_t)s * pitch + k] & degmask[k];
   if (member && lane == 0) member[s] = 1;
   int picks = 0;
   for (;;) {
@@ -209,7 +210,7 @@ D2BA_DEV int pcm_greedy(int s, int m, const unsigned *rows, int W, const unsigne
     if (cnt == 0) return 1 + picks;
     if (member && lane == 0) member[hi] = 1;
     picks++; (*rounds)++;
-    for (int k = lane; k < W; k += 32) C[k] &= rows[(size_t)hi * W + k];
+    for (int k = lane; k < W; k += 32) C[k] &= rows[(size_t)hi * pitch + k];
   }
 }
 
@@ -241,7 +242,7 @@ __global__ void __launch_bounds__(kPcmWarps * 32) k_pcm_clique(const int *g_loop
   for (int s0 = 0; s0 < L;) {
     const int m = s_m, s = s0 + warp;
     int size = 0;
-    if (s < L && !(m > deg[s])) size = pcm_greedy(s, m, rows, W, degmask, C, lane, &rounds, nullptr);   // Pruning 1
+    if (s < L && !(m > deg[s])) size = pcm_greedy(s, m, rows, W, W, degmask, C, lane, &rounds, nullptr);   // Pruning 1
     if (lane == 0) s_size[warp] = size;
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -257,7 +258,7 @@ __global__ void __launch_bounds__(kPcmWarps * 32) k_pcm_clique(const int *g_loop
   if (s_best >= 0) {
     pcm_degmask(degmask, deg, L, W, s_best_m);
     __syncthreads();
-    if (warp == 0) { long long dummy = 0; pcm_greedy(s_best, s_best_m, rows, W, degmask, C, lane, &dummy, inlier + base); }
+    if (warp == 0) { long long dummy = 0; pcm_greedy(s_best, s_best_m, rows, W, W, degmask, C, lane, &dummy, inlier + base); }
   }
   s_part[threadIdx.x] = lane == 0 ? rounds : 0;   // every lane of a warp counted the same rounds
   __syncthreads();
@@ -270,11 +271,117 @@ __global__ void __launch_bounds__(kPcmWarps * 32) k_pcm_clique(const int *g_loop
   if (threadIdx.x == 0) { long long t = 0; for (int k = 0; k < kPcmWarps * 32; k++) t += s_part[k]; stats[2 * g] = t; stats[2 * g + 1] = r; }
 }
 
+// one clique search of k_pcm_clique_jobs: a group's rows (row pitch `pitch` words), its degrees and its member flags.  Seeds are
+// s_lo .. L-1 and the running maximum starts at m0: s_lo = 0, m0 = -1 is FMC maxCliqueHeu, as k_pcm_clique; s_lo = L0 (the first
+// new vertex), m0 = the group's clique size is maxCliqueHeuIncremental's search (findCliqueHeuInc.cpp:32-96).
+struct PcmCliqueJob { const unsigned *rows; int *deg; unsigned char *member; long long pitch; int L, s_lo, m0; };
+
+// k_pcm_clique on a job table (the PCM stream, d2pgo_debug_pcm_clique_inc), one CTA per job, with the same rounds.  When a seed
+// commits, the member flags [0, L) are replaced by its clique, rebuilt at the end under the m it was found with; otherwise they
+// stay.  stats[j] = {sum of degrees, greedy rounds}.
+__global__ void __launch_bounds__(kPcmWarps * 32) k_pcm_clique_jobs(const PcmCliqueJob *jobs, long long *stats) {
+  extern __shared__ unsigned pcm_smem[];
+  __shared__ int s_size[kPcmWarps], s_m, s_best, s_best_m, s_next;
+  __shared__ long long s_part[kPcmWarps * 32];
+  const PcmCliqueJob J = jobs[blockIdx.x];
+  const int L = J.L, W = (L + 31) >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned *rows = J.rows;
+  const int *deg = J.deg;
+  unsigned *degmask = pcm_smem, *C = pcm_smem + W * (1 + warp);
+  long long rounds = 0, dsum = 0;
+  for (int k = threadIdx.x; k < L; k += blockDim.x) dsum += deg[k];
+  if (threadIdx.x == 0) { s_m = J.m0; s_best = -1; s_best_m = -1; }
+  pcm_degmask(degmask, deg, L, W, J.m0);
+  __syncthreads();
+  for (int s0 = J.s_lo; s0 < L;) {
+    const int m = s_m, s = s0 + warp;
+    int size = 0;
+    if (s < L && !(m > deg[s])) size = pcm_greedy(s, m, rows, J.pitch, W, degmask, C, lane, &rounds, nullptr);   // Pruning 1
+    if (lane == 0) s_size[warp] = size;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      s_next = s0 + kPcmWarps;
+      for (int w = 0; w < kPcmWarps; w++)
+        if (s_size[w] > m) { s_best = s0 + w; s_best_m = m; s_m = s_size[w]; s_next = s0 + w + 1; break; }
+    }
+    __syncthreads();
+    if (s_m != m) { pcm_degmask(degmask, deg, L, W, s_m); __syncthreads(); }
+    s0 = s_next;
+    __syncthreads();
+  }
+  if (s_best >= 0) {
+    for (int k = threadIdx.x; k < L; k += blockDim.x) J.member[k] = 0;
+    pcm_degmask(degmask, deg, L, W, s_best_m);
+    __syncthreads();
+    if (warp == 0) { long long dummy = 0; pcm_greedy(s_best, s_best_m, rows, J.pitch, W, degmask, C, lane, &dummy, J.member); }
+  }
+  s_part[threadIdx.x] = lane == 0 ? rounds : 0;   // every lane of a warp counted the same rounds
+  __syncthreads();
+  if (threadIdx.x == 0) { long long r = 0; for (int k = 0; k < kPcmWarps * 32; k++) r += s_part[k]; s_part[0] = r; }
+  __syncthreads();
+  const long long r = s_part[0];
+  __syncthreads();
+  s_part[threadIdx.x] = dsum;
+  __syncthreads();
+  if (threadIdx.x == 0) { long long t = 0; for (int k = 0; k < kPcmWarps * 32; k++) t += s_part[k]; stats[2 * blockIdx.x] = t; stats[2 * blockIdx.x + 1] = r; }
+}
+
+// ---- the PCM stream (d2pgo_pcm_stream): a group's adjacency is [cap][pitch] words with cap = 32 pitch rows; its rows 0 .. L0-1
+// are the loops of earlier calls, L0 .. L-1 the loops new in this call.  slot[r] = the stream's loop index of row r.
+struct PcmPairJob { unsigned *adj; const int *slot; double *smd; long long pitch; int L0, L; };
+
+// one warp per adjacency word that a call changes: every word of the new rows, and the words of the old rows that cover columns
+// >= L0.  Same cell rule and ballot as k_pcm_pairs; an old row's bits below column L0 are kept.  The smd of new row i against
+// j < i is kept at smd[i (i - 1) / 2 - L0 (L0 - 1) / 2 + j] for d2pgo_debug_pcm_stream_smd.
+__global__ void __launch_bounds__(256) k_pcm_stream_pairs(PcmDev d, const PcmPairJob *jobs, const long long *job_word, int n_jobs, long long n_words) {
+  const long long t = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (t >= n_words) return;
+  const int g = pcm_group_of(job_word, n_jobs, t);
+  const PcmPairJob &J = jobs[g];
+  const int L0 = J.L0, L = J.L, W = (L + 31) >> 5;
+  long long local = t - job_word[g];
+  const long long n_new = (long long)(L - L0) * W;
+  int i, w;
+  unsigned keep = 0;
+  if (local < n_new) { i = L0 + (int)(local / W); w = (int)(local % W); }
+  else {
+    local -= n_new;
+    const int w0 = L0 >> 5, Wo = W - w0;
+    i = (int)(local / Wo); w = w0 + (int)(local % Wo);
+    if (w == w0) keep = (1u << (L0 & 31)) - 1u;
+  }
+  const int j = w * 32 + lane;
+  bool ok = false;
+  if (j < L && j != i && j >= (i < L0 ? L0 : 0)) {
+    const double s = pcm_smd(d, J.slot[max(i, j)], J.slot[min(i, j)]);
+    ok = s < d.thr;
+    if (j < i) J.smd[(long long)i * (i - 1) / 2 - (long long)L0 * (L0 - 1) / 2 + j] = s;
+  }
+  const unsigned word = __ballot_sync(0xffffffffu, ok);
+  if (lane == 0) { unsigned *p = J.adj + i * J.pitch + w; *p = (*p & keep) | word; }
+}
+
+// thread per row of the jobs' groups: degree = popcount of the row (row_off: prefix sums of the jobs' L)
+__global__ void k_pcm_stream_degree(const PcmCliqueJob *jobs, const int *row_off, int n_jobs) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= row_off[n_jobs]) return;
+  int lo = 0, hi = n_jobs - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (row_off[mid] <= e) lo = mid; else hi = mid - 1; }
+  const PcmCliqueJob &J = jobs[lo];
+  const int r = e - row_off[lo], W = (J.L + 31) >> 5;
+  const unsigned *row = J.rows + r * J.pitch;
+  int c = 0;
+  for (int k = 0; k < W; k++) c += __popc(row[k]);
+  J.deg[r] = c;
+}
+
 }  // namespace
 
 struct d2pgo_host::PcmBufs {
   Buf<int> g_loop, fa, fb, src, traj_ptr, traj, deg; Buf<long long> g_word, g_smd, stats; Buf<unsigned char> flip, inlier;
-  Buf<double> rel_in, sqrt_in, rel, cov, ego, path, smd; Buf<unsigned> adj;
+  Buf<double> rel_in, sqrt_in, rel, cov, ego, path, smd; Buf<unsigned> adj; Buf<PcmCliqueJob> jobs;   // jobs: d2pgo_debug_pcm_clique_inc
   long long n_smd = -1;   // tested pairs of the last d2pgo_pcm call (-1: none yet)
   cudaEvent_t ev_pair = nullptr;
   ~PcmBufs() { if (ev_pair) cudaEventDestroy(ev_pair); }
@@ -291,6 +398,47 @@ static int pcm_run_clique(d2pgo_handle *h, int G, int n, int max_w) {
   PCK(cudaGetLastError());
   return 0;
 }
+
+// ---- the PCM stream's state (d2pgo_pcm_stream): frames, loops and per-group consistency graphs that stay on the device
+namespace {
+
+// grow b to hold at least `need` elements (capacity doubles), keeping the first `used`; new elements are zeroed
+template <typename T> cudaError_t pcm_grow(d2pgo_host::Buf<T> &b, size_t used, size_t need, cudaStream_t st) {
+  if (b.p && need <= b.n) return cudaSuccess;
+  d2pgo_host::Buf<T> nb;
+  cudaError_t e = nb.alloc(std::max(need, 2 * b.n));
+  if (e == cudaSuccess) e = cudaMemsetAsync(nb.p, 0, nb.n * sizeof(T), st);
+  if (e == cudaSuccess && used) e = cudaMemcpyAsync(nb.p, b.p, used * sizeof(T), cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);   // the old array is freed below
+  if (e != cudaSuccess) return e;
+  std::swap(b.p, nb.p); std::swap(b.n, nb.n);
+  return cudaSuccess;
+}
+
+struct PcmStreamGroup {   // one drone pair: L loops (rows), an adjacency of cap = 32 pitch rows, the clique's member flags
+  int32_t lo, hi;
+  int L = 0, pitch = 0, size = 0;
+  long long dsum = 0;                    // sum of the degrees after the last call that touched the group
+  d2pgo_host::Buf<unsigned> adj; d2pgo_host::Buf<int> slot, deg; d2pgo_host::Buf<unsigned char> member;
+  std::vector<unsigned char> member_h;   // host copy of member [L]
+};
+
+}  // namespace
+
+struct d2pgo_host::PcmStream {
+  bool ready = false; int incremental = 0, is4 = 0; double thr = 0, pos_cov = 0, yaw_cov = 0;
+  std::unordered_map<int64_t, int> fidx; std::vector<int32_t> f_agent;   // keyframe id -> frame index; frame -> drone
+  std::unordered_map<int32_t, int> drone_of; std::vector<std::vector<int>> trajs;
+  std::unordered_map<int64_t, int> loop_of; std::vector<int> l_group, l_row;   // loop id -> loop index; loop -> group, row
+  std::unordered_map<uint64_t, int> gid; std::vector<std::unique_ptr<PcmStreamGroup>> groups;
+  Buf<double> ego, path, rel, cov, rel_in, sqrt_in, smd; Buf<int> fa, fb, src, traj_ptr, traj, row_off; Buf<unsigned char> flip;
+  Buf<PcmPairJob> pjobs; Buf<long long> pword, stats; Buf<PcmCliqueJob> cjobs;
+  long long n_smd = -1;   // pairs tested by the last stream call (-1: none yet)
+  cudaEvent_t ev_pair = nullptr;
+  ~PcmStream() { if (ev_pair) cudaEventDestroy(ev_pair); }
+};
+
+void d2pgo_host::PcmStreamFree::operator()(PcmStream *p) const { delete p; }
 
 extern "C" {
 
@@ -445,6 +593,262 @@ int d2pgo_debug_pcm_clique(d2pgo_handle *h, int32_t n, const uint32_t *adj, uint
   int c = 0;
   for (int k = 0; k < n; k++) c += member_out[k];
   if (size_out) *size_out = c;
+  return 0;
+}
+
+int d2pgo_debug_pcm_clique_inc(d2pgo_handle *h, int32_t n, const uint32_t *adj, int32_t n_new, int32_t prev_size, uint8_t *member_out, int32_t *size_out) {
+  if (!h) return 1;
+  if (n < 0 || (n && (!adj || !member_out))) return pgo_fail(h, 1, "debug_pcm_clique_inc: null argument or negative count");
+  if (n > kPcmMaxGroup) return pgo_fail(h, 4, "debug_pcm_clique_inc: at most " + std::to_string(kPcmMaxGroup) + " vertices are supported");
+  if (n_new < 0 || n_new > n || prev_size < 0) return pgo_fail(h, 2, "debug_pcm_clique_inc: n_new must lie in [0, n] and prev_size be non-negative");
+  cudaSetDevice(h->cfg.device);
+  if (!h->pcm) h->pcm.reset(new PcmBufs());
+  PcmBufs &P = *h->pcm;
+  const long long W = (n + 31) / 32;
+  const int g_loop[2] = {0, n}; const long long g_word[2] = {0, n * W};
+  P.n_smd = -1;   // the buffers below are shared with d2pgo_pcm
+  PCK(P.g_loop.alloc(2)); PCK(P.g_word.alloc(2)); PCK(P.adj.alloc(n * W)); PCK(P.deg.alloc(n)); PCK(P.inlier.alloc(n)); PCK(P.stats.alloc(2)); PCK(P.jobs.alloc(1));
+  const PcmCliqueJob job{P.adj.p, P.deg.p, P.inlier.p, (long long)W, n, n - n_new, prev_size};
+  PCK(cudaMemcpyAsync(P.g_loop.p, g_loop, 8, cudaMemcpyHostToDevice, h->stream));
+  PCK(cudaMemcpyAsync(P.g_word.p, g_word, 16, cudaMemcpyHostToDevice, h->stream));
+  PCK(cudaMemcpyAsync(P.jobs.p, &job, sizeof job, cudaMemcpyHostToDevice, h->stream));
+  if (n) {
+    PCK(cudaMemcpyAsync(P.adj.p, adj, (size_t)(n * W) * 4, cudaMemcpyHostToDevice, h->stream));
+    PCK(cudaMemsetAsync(P.inlier.p, 0, n, h->stream));   // the flags stay 0 when no seed beats prev_size
+    k_pcm_degree<<<(n + 255) / 256, 256, 0, h->stream>>>(1, P.g_loop.p, P.g_word.p, P.adj.p, P.deg.p);
+    k_pcm_clique_jobs<<<1, kPcmWarps * 32, (size_t)(1 + kPcmWarps) * std::max(W, 1LL) * 4, h->stream>>>(P.jobs.p, P.stats.p);
+    PCK(cudaGetLastError());
+    PCK(cudaMemcpyAsync(member_out, P.inlier.p, n, cudaMemcpyDeviceToHost, h->stream));
+  }
+  PCK(cudaStreamSynchronize(h->stream));
+  int c = 0;
+  for (int k = 0; k < n; k++) c += member_out[k];
+  if (size_out) *size_out = c > 0 ? c : prev_size;   // FMC's return: the clique that beat prev_size, else prev_size
+  return 0;
+}
+
+int d2pgo_pcm_stream_reset(d2pgo_handle *h, const d2pgo_pcm_config *cfg, int32_t incremental) {
+  if (!h) return 1;
+  if (!cfg) return pgo_fail(h, 1, "pcm_stream_reset: null argument");
+  const double thr = (double)(float)cfg->pcm_thres;   // a float in the reference, as in d2pgo_pcm
+  if (!(std::isfinite(thr) && thr > 0.0)) return pgo_fail(h, 2, "pcm_stream_reset: pcm_thres must be finite and positive");
+  if (!(std::isfinite(cfg->pos_covariance_per_meter) && cfg->pos_covariance_per_meter >= 0.0 && std::isfinite(cfg->yaw_covariance_per_meter) && cfg->yaw_covariance_per_meter >= 0.0))
+    return pgo_fail(h, 2, "pcm_stream_reset: covariance rates must be finite and non-negative");
+  if (incremental != 0 && incremental != 1) return pgo_fail(h, 2, "pcm_stream_reset: incremental must be 0 or 1");
+  cudaSetDevice(h->cfg.device);
+  h->pcm_stream.reset(new d2pgo_host::PcmStream());
+  d2pgo_host::PcmStream &S = *h->pcm_stream;
+  S.ready = true; S.incremental = incremental; S.is4 = h->dof == 4; S.thr = thr;
+  S.pos_cov = cfg->pos_covariance_per_meter; S.yaw_cov = cfg->yaw_covariance_per_meter;
+  PCK(cudaEventCreate(&S.ev_pair));
+  return 0;
+}
+
+int d2pgo_pcm_stream(d2pgo_handle *h, int32_t n_frames, const int64_t *frame_ids, const int32_t *frame_agent, const double *ego_poses7, int32_t n_loops,
+                     const int64_t *loop_ids, const int64_t *kf_a, const int64_t *kf_b, const double *rel7, const double *sqrt_info36, uint8_t *inlier_out,
+                     d2pgo_pcm_stream_report *rep) {
+  if (!h) return 1;
+  if (n_frames < 0 || n_loops < 0 || (n_frames && (!frame_ids || !frame_agent || !ego_poses7)) ||
+      (n_loops && (!loop_ids || !kf_a || !kf_b || !rel7 || !sqrt_info36 || !inlier_out)))
+    return pgo_fail(h, 1, "pcm_stream: null argument or negative count");
+  if (!h->pcm_stream || !h->pcm_stream->ready) return pgo_fail(h, 5, "pcm_stream: no d2pgo_pcm_stream_reset on this handle");
+  d2pgo_host::PcmStream &S = *h->pcm_stream;
+  // ---- checks: nothing of the call is kept until all of them pass
+  std::unordered_map<int64_t, int32_t> fnew;   // keyframes first seen in this call -> drone
+  std::vector<int> fadd;                       // their positions in the call, in the order given
+  for (int f = 0; f < n_frames; f++) {
+    auto old = S.fidx.find(frame_ids[f]);
+    const int32_t had = old != S.fidx.end() ? S.f_agent[old->second] : (fnew.count(frame_ids[f]) ? fnew[frame_ids[f]] : frame_agent[f]);
+    if (had != frame_agent[f])
+      return pgo_fail(h, 3, "pcm_stream: keyframe id " + std::to_string(frame_ids[f]) + " was given with drone " + std::to_string(had) + " and now with drone " + std::to_string(frame_agent[f]));
+    if (old != S.fidx.end() || fnew.count(frame_ids[f])) continue;
+    for (int k = 0; k < 7; k++)
+      if (!std::isfinite(ego_poses7[(size_t)f * 7 + k])) return pgo_fail(h, 2, "pcm_stream: non-finite ego pose of keyframe id " + std::to_string(frame_ids[f]));
+    fnew.emplace(frame_ids[f], frame_agent[f]); fadd.push_back(f);
+  }
+  auto agent_of = [&](int64_t id, int32_t *a) {
+    auto it = S.fidx.find(id);
+    if (it != S.fidx.end()) { *a = S.f_agent[it->second]; return true; }
+    auto jt = fnew.find(id);
+    if (jt != fnew.end()) { *a = jt->second; return true; }
+    return false;
+  };
+  std::unordered_map<int64_t, int> seen;       // loop id -> position in the call
+  std::vector<int> ladd;                       // new loops: positions in the call
+  std::unordered_map<uint64_t, int> gnew_size; // loops per group after the call, for the groups that get new loops
+  for (int e = 0; e < n_loops; e++) {
+    if (!seen.emplace(loop_ids[e], e).second) return pgo_fail(h, 3, "pcm_stream: loop id " + std::to_string(loop_ids[e]) + " appears twice in one call");
+    if (S.loop_of.count(loop_ids[e])) continue;
+    int32_t x, y;
+    if (!agent_of(kf_a[e], &x) || !agent_of(kf_b[e], &y))
+      return pgo_fail(h, 3, "pcm_stream: loop id " + std::to_string(loop_ids[e]) + " names unknown keyframe id " + std::to_string(agent_of(kf_a[e], &x) ? kf_b[e] : kf_a[e]));
+    for (int k = 0; k < 7; k++)
+      if (!std::isfinite(rel7[(size_t)e * 7 + k])) return pgo_fail(h, 2, "pcm_stream: non-finite relative pose of loop id " + std::to_string(loop_ids[e]));
+    for (int k = 0; k < 36; k++)
+      if (!std::isfinite(sqrt_info36[(size_t)e * 36 + k])) return pgo_fail(h, 2, "pcm_stream: non-finite sqrt_info of loop id " + std::to_string(loop_ids[e]));
+    const uint64_t key = (uint64_t)(uint32_t)std::min(x, y) << 32 | (uint32_t)std::max(x, y);
+    auto it = gnew_size.find(key);
+    if (it == gnew_size.end()) { auto g = S.gid.find(key); it = gnew_size.emplace(key, g == S.gid.end() ? 0 : S.groups[g->second]->L).first; }
+    if (++it->second > kPcmMaxGroup)
+      return pgo_fail(h, 4, "pcm_stream: the group of drones " + std::to_string(std::min(x, y)) + " and " + std::to_string(std::max(x, y)) + " would hold " +
+                                std::to_string(it->second) + " loops; at most " + std::to_string(kPcmMaxGroup) + " are supported");
+    ladd.push_back(e);
+  }
+  cudaSetDevice(h->cfg.device);
+  cudaStream_t st = h->stream;
+  // ---- frames: appended to their drone's trajectory; ego poses [F][8] stay on the device
+  const int F0 = (int)S.f_agent.size(), F = F0 + (int)fadd.size();
+  if (!fadd.empty()) {
+    PCK(pcm_grow(S.ego, (size_t)F0 * 8, (size_t)F * 8, st)); PCK(pcm_grow(S.path, F0, F, st));
+    std::vector<double> ego(fadd.size() * 8, 0.0);
+    for (size_t k = 0; k < fadd.size(); k++) {
+      const int f = fadd[k];
+      memcpy(&ego[k * 8], ego_poses7 + (size_t)f * 7, 56);
+      S.fidx.emplace(frame_ids[f], F0 + (int)k); S.f_agent.push_back(frame_agent[f]);
+      auto it = S.drone_of.emplace(frame_agent[f], (int)S.trajs.size());
+      if (it.second) S.trajs.emplace_back();
+      S.trajs[it.first->second].push_back(F0 + (int)k);
+    }
+    PCK(cudaMemcpyAsync(S.ego.p + (size_t)F0 * 8, ego.data(), ego.size() * 8, cudaMemcpyHostToDevice, st));
+    std::vector<int> traj_ptr(1, 0), traj;
+    for (auto &t : S.trajs) { traj.insert(traj.end(), t.begin(), t.end()); traj_ptr.push_back((int)traj.size()); }
+    PCK(S.traj_ptr.alloc(traj_ptr.size())); PCK(S.traj.alloc(traj.size()));
+    PCK(cudaMemcpyAsync(S.traj_ptr.p, traj_ptr.data(), traj_ptr.size() * 4, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(S.traj.p, traj.data(), traj.size() * 4, cudaMemcpyHostToDevice, st));
+  }
+  // ---- new loops: constants by loop index, rows of their group (groups numbered by their first loop)
+  const int n0 = (int)S.l_group.size(), nn = (int)ladd.size(), n1 = n0 + nn;
+  std::vector<int> touched, L0_of;   // group indices in ascending order, and their sizes before the call
+  std::vector<int> sfa(nn), sfb(nn), iota(nn);
+  std::vector<unsigned char> sflip(nn);
+  std::vector<double> rin((size_t)nn * 7), sqi((size_t)nn * 36);
+  std::vector<std::vector<int>> gslots;   // per touched group: the loop indices of its new rows
+  std::unordered_map<int, int> tpos;
+  for (int k = 0; k < nn; k++) {
+    const int e = ladd[k];
+    const int a = S.fidx.at(kf_a[e]), b = S.fidx.at(kf_b[e]);
+    const int32_t x = S.f_agent[a], y = S.f_agent[b];
+    const uint64_t key = (uint64_t)(uint32_t)std::min(x, y) << 32 | (uint32_t)std::max(x, y);
+    auto g = S.gid.emplace(key, (int)S.groups.size());
+    if (g.second) { S.groups.emplace_back(new PcmStreamGroup()); S.groups.back()->lo = std::min(x, y); S.groups.back()->hi = std::max(x, y); }
+    const int gi = g.first->second;
+    auto t = tpos.emplace(gi, (int)touched.size());
+    if (t.second) { touched.push_back(gi); L0_of.push_back(S.groups[gi]->L); gslots.emplace_back(); }
+    S.loop_of.emplace(loop_ids[e], n0 + k); S.l_group.push_back(gi); S.l_row.push_back(S.groups[gi]->L++);
+    gslots[t.first->second].push_back(n0 + k);
+    sfa[k] = a; sfb[k] = b; sflip[k] = x > y; iota[k] = k;
+    memcpy(&rin[(size_t)k * 7], rel7 + (size_t)e * 7, 56); memcpy(&sqi[(size_t)k * 36], sqrt_info36 + (size_t)e * 36, 288);
+  }
+  if (nn) {
+    PCK(pcm_grow(S.fa, n0, n1, st)); PCK(pcm_grow(S.fb, n0, n1, st)); PCK(pcm_grow(S.flip, n0, n1, st));
+    PCK(pcm_grow(S.rel, (size_t)n0 * 8, (size_t)n1 * 8, st)); PCK(pcm_grow(S.cov, (size_t)n0 * 21, (size_t)n1 * 21, st));
+    PCK(S.rel_in.alloc((size_t)nn * 7)); PCK(S.sqrt_in.alloc((size_t)nn * 36)); PCK(S.src.alloc(nn));
+    PCK(cudaMemcpyAsync(S.fa.p + n0, sfa.data(), nn * 4, cudaMemcpyHostToDevice, st)); PCK(cudaMemcpyAsync(S.fb.p + n0, sfb.data(), nn * 4, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(S.flip.p + n0, sflip.data(), nn, cudaMemcpyHostToDevice, st)); PCK(cudaMemcpyAsync(S.src.p, iota.data(), nn * 4, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(S.rel_in.p, rin.data(), rin.size() * 8, cudaMemcpyHostToDevice, st)); PCK(cudaMemcpyAsync(S.sqrt_in.p, sqi.data(), sqi.size() * 8, cudaMemcpyHostToDevice, st));
+  }
+  // touched groups in the order of their first loop; each grows its adjacency (pitch doubling, rows copied to the new pitch)
+  std::vector<int> order(touched.size());
+  for (size_t k = 0; k < order.size(); k++) order[k] = (int)k;
+  std::sort(order.begin(), order.end(), [&](int u, int v) { return touched[u] < touched[v]; });
+  const int T = (int)touched.size();
+  std::vector<PcmPairJob> pj(T); std::vector<PcmCliqueJob> cj(T);
+  std::vector<long long> pword(T + 1, 0), smd_off(T + 1, 0); std::vector<int> row_off(T + 1, 0);
+  int max_w = 1;
+  for (int k = 0; k < T; k++) {
+    const int u = order[k];
+    PcmStreamGroup &G = *S.groups[touched[u]];
+    const int L0 = L0_of[u], L = G.L;
+    if (32 * G.pitch < L) {
+      int p = std::max(G.pitch, 1);
+      while (32 * p < L) p *= 2;
+      d2pgo_host::Buf<unsigned> na;
+      PCK(na.alloc((size_t)32 * p * p));
+      if (L0) PCK(cudaMemcpy2DAsync(na.p, (size_t)p * 4, G.adj.p, (size_t)G.pitch * 4, (size_t)G.pitch * 4, L0, cudaMemcpyDeviceToDevice, st));
+      PCK(cudaStreamSynchronize(st));
+      std::swap(G.adj.p, na.p); std::swap(G.adj.n, na.n);
+      PCK(pcm_grow(G.slot, L0, (size_t)32 * p, st)); PCK(pcm_grow(G.deg, L0, (size_t)32 * p, st)); PCK(pcm_grow(G.member, L0, (size_t)32 * p, st));
+      G.pitch = p;
+    }
+    PCK(cudaMemcpyAsync(G.slot.p + L0, gslots[u].data(), (L - L0) * 4, cudaMemcpyHostToDevice, st));
+    const long long W = (L + 31) / 32;
+    max_w = std::max(max_w, (int)W);
+    pj[k] = PcmPairJob{G.adj.p, G.slot.p, nullptr, G.pitch, L0, L};
+    cj[k] = PcmCliqueJob{G.adj.p, G.deg.p, G.member.p, G.pitch, L, S.incremental ? L0 : 0, S.incremental ? G.size : -1};
+    pword[k + 1] = pword[k] + (L - L0) * W + (long long)L0 * (W - (L0 >> 5));
+    smd_off[k + 1] = smd_off[k] + (long long)L * (L - 1) / 2 - (long long)L0 * (L0 - 1) / 2;
+    row_off[k + 1] = row_off[k] + L;
+  }
+  PCK(S.smd.alloc(smd_off[T]));
+  for (int k = 0; k < T; k++) pj[k].smd = S.smd.p + smd_off[k];
+  PCK(S.pjobs.alloc(T)); PCK(S.cjobs.alloc(T)); PCK(S.pword.alloc(T + 1)); PCK(S.row_off.alloc(T + 1)); PCK(S.stats.alloc(2 * (size_t)T));
+  if (T) {
+    PCK(cudaMemcpyAsync(S.pjobs.p, pj.data(), T * sizeof(PcmPairJob), cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(S.cjobs.p, cj.data(), T * sizeof(PcmCliqueJob), cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(S.pword.p, pword.data(), (T + 1) * 8, cudaMemcpyHostToDevice, st));
+    PCK(cudaMemcpyAsync(S.row_off.p, row_off.data(), (T + 1) * 4, cudaMemcpyHostToDevice, st));
+  }
+  // ---- device: path lengths over the whole trajectories (appending frames leaves an earlier frame's value unchanged: the warp
+  // scan of k_pcm_path adds lane k's prefix from lanes <= k only, and the carry from whole earlier chunks), loop constants of the
+  // new loops, the changed adjacency words, degrees and cliques of the touched groups
+  PcmDev d;
+  memset(&d, 0, sizeof d);
+  d.fa = S.fa.p; d.fb = S.fb.p; d.flip = S.flip.p; d.rel = S.rel.p; d.cov = S.cov.p; d.ego = S.ego.p; d.path = S.path.p;
+  d.is4 = S.is4; d.thr = S.thr; d.pos_cov = S.pos_cov; d.yaw_cov = S.yaw_cov;
+  PCK(cudaEventRecord(h->ev0, st));
+  if (!S.trajs.empty()) k_pcm_path<<<((int)S.trajs.size() * 32 + 255) / 256, 256, 0, st>>>((int)S.trajs.size(), S.traj_ptr.p, S.traj.p, S.ego.p, S.path.p);
+  if (nn) k_pcm_loop<<<(nn + 127) / 128, 128, 0, st>>>(nn, S.src.p, S.rel_in.p, S.sqrt_in.p, S.rel.p + (size_t)n0 * 8, S.cov.p + (size_t)n0 * 21);
+  if (pword[T]) k_pcm_stream_pairs<<<(unsigned)((pword[T] * 32 + 255) / 256), 256, 0, st>>>(d, S.pjobs.p, S.pword.p, T, pword[T]);
+  PCK(cudaGetLastError());
+  PCK(cudaEventRecord(S.ev_pair, st));
+  if (T) {
+    k_pcm_stream_degree<<<(row_off[T] + 255) / 256, 256, 0, st>>>(S.cjobs.p, S.row_off.p, T);
+    k_pcm_clique_jobs<<<T, kPcmWarps * 32, (size_t)(1 + kPcmWarps) * max_w * 4, st>>>(S.cjobs.p, S.stats.p);
+  }
+  PCK(cudaGetLastError());
+  PCK(cudaEventRecord(h->ev1, st));
+  std::vector<long long> stats(2 * (size_t)T);
+  for (int k = 0; k < T; k++) {
+    PcmStreamGroup &G = *S.groups[touched[order[k]]];
+    G.member_h.resize(G.L);
+    PCK(cudaMemcpyAsync(G.member_h.data(), G.member.p, G.L, cudaMemcpyDeviceToHost, st));
+  }
+  if (T) PCK(cudaMemcpyAsync(stats.data(), S.stats.p, 16 * (size_t)T, cudaMemcpyDeviceToHost, st));
+  PCK(cudaStreamSynchronize(st));
+  d2pgo_pcm_stream_report R; memset(&R, 0, sizeof R);
+  for (int k = 0; k < T; k++) {
+    PcmStreamGroup &G = *S.groups[touched[order[k]]];
+    int c = 0;
+    for (unsigned char m : G.member_h) c += m;
+    G.size = c;
+    R.consistent_pairs += (stats[2 * k] - G.dsum) / 2; G.dsum = stats[2 * k];
+    R.clique_rounds += stats[2 * k + 1];
+  }
+  // every group the call names has been through the clique, so each loop's pair has an inlier set (:96-111): membership decides
+  for (int e = 0; e < n_loops; e++) {
+    const int l = S.loop_of.at(loop_ids[e]);
+    inlier_out[e] = S.groups[S.l_group[l]]->member_h[S.l_row[l]];
+    R.inliers += inlier_out[e];
+  }
+  R.new_loops = nn; R.total_loops = n1; R.groups = (int32_t)S.groups.size(); R.groups_touched = T; R.pairs_tested = smd_off[T];
+  float ms = 0, mp = 0;
+  cudaEventElapsedTime(&ms, h->ev0, h->ev1); cudaEventElapsedTime(&mp, h->ev0, S.ev_pair);
+  R.device_ms = ms; R.pair_ms = mp; R.clique_ms = ms - mp;
+  S.n_smd = smd_off[T];
+  if (rep) *rep = R;
+  return 0;
+}
+
+int d2pgo_debug_pcm_stream_smd(d2pgo_handle *h, double *out, int64_t out_doubles) {
+  if (!h) return 1;
+  if (!h->pcm_stream || h->pcm_stream->n_smd < 0) return pgo_fail(h, 2, "debug_pcm_stream_smd: no successful d2pgo_pcm_stream call since the last reset");
+  const d2pgo_host::PcmStream &S = *h->pcm_stream;
+  if (out_doubles < S.n_smd) return pgo_fail(h, 2, "debug_pcm_stream_smd: buffer too small: " + std::to_string(S.n_smd) + " doubles needed");
+  cudaSetDevice(h->cfg.device);
+  if (S.n_smd) {
+    PCK(cudaMemcpyAsync(out, S.smd.p, (size_t)S.n_smd * 8, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaStreamSynchronize(h->stream));
+  }
   return 0;
 }
 

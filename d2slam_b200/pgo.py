@@ -103,6 +103,12 @@ class PcmReport(C.Structure):
                 ("clique_rounds", C.c_int64), ("device_ms", C.c_double), ("pair_ms", C.c_double), ("clique_ms", C.c_double)]
 
 
+class PcmStreamReport(C.Structure):
+    _fields_ = [("new_loops", C.c_int32), ("total_loops", C.c_int32), ("groups", C.c_int32), ("groups_touched", C.c_int32), ("inliers", C.c_int32),
+                ("pairs_tested", C.c_int64), ("consistent_pairs", C.c_int64), ("clique_rounds", C.c_int64), ("device_ms", C.c_double),
+                ("pair_ms", C.c_double), ("clique_ms", C.c_double)]
+
+
 PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_last_error", "d2pgo_set_poses", "d2pgo_add_edges",
                 "d2pgo_comm_init", "d2pgo_solve", "d2pgo_get_poses", "d2pgo_debug_edges", "d2pgo_set_poses_4d", "d2pgo_add_edges_4d",
                 "d2pgo_get_poses_4d", "d2pgo_default_pcm_config", "d2pgo_pcm", "d2pgo_debug_pcm_smd", "d2pgo_debug_pcm_clique",
@@ -111,7 +117,8 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_default_rot_init_config", "d2pgo_rot_init", "d2pgo_set_linear_solver", "d2pgo_cholesky_stats",
                 "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic", "d2pgo_debug_cholesky_system", "d2pgo_debug_pcg_step",
                 "d2pgo_default_arock_rot_init_config", "d2pgo_arock_rot_init_step", "d2pgo_arock_rot_receive",
-                "d2pgo_arock_rot_neighbours", "d2pgo_arock_rot_duals", "d2pgo_debug_arock_rot_state"]
+                "d2pgo_arock_rot_neighbours", "d2pgo_arock_rot_duals", "d2pgo_debug_arock_rot_state", "d2pgo_pcm_stream_reset",
+                "d2pgo_pcm_stream", "d2pgo_debug_pcm_stream_smd", "d2pgo_debug_pcm_clique_inc"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -306,6 +313,46 @@ class PgoSolver:
         out = np.zeros(max(int(self.pcm_report.pairs_tested), 1))
         self._chk(_lib().d2pgo_debug_pcm_smd(self.h, _p(out), C.c_int64(out.size)), "debug_pcm_smd")
         return out[: int(self.pcm_report.pairs_tested)]
+
+    # ---- PCM as a stream (include/d2pgo.h d2pgo_pcm_stream*)
+    def pcm_stream_reset(self, incremental=0, **cfg):
+        """Start a new PCM stream on this handle (forgets every frame, loop and clique); incremental 0 = maxCliqueHeu on the
+        groups that get new loops, 1 = the incremental clique.  cfg overrides PcmConfig fields as for pcm()."""
+        c = PcmConfig()
+        _lib().d2pgo_default_pcm_config(C.byref(c))
+        for k, v in cfg.items():
+            setattr(c, k, v)
+        self._chk(_lib().d2pgo_pcm_stream_reset(self.h, C.byref(c), C.c_int32(incremental)), "pcm_stream_reset")
+        self.pcm_stream_report = None
+
+    def pcm_stream(self, frame_ids, frame_agent, ego_poses7, loop_ids, kf_a, kf_b, rel7, sqrt_info36):
+        """One call of the stream: the keyframes new since the last call, and the call's loops keyed by loop_ids (ids seen before
+        are not tested again).  Boolean inlier mask over the call's loops; the report is kept in self.pcm_stream_report."""
+        fid = np.ascontiguousarray(frame_ids, np.int64); fag = np.ascontiguousarray(frame_agent, np.int32)
+        ego = np.ascontiguousarray(ego_poses7, np.float64).reshape(-1, 7)
+        lid = np.ascontiguousarray(loop_ids, np.int64); ka = np.ascontiguousarray(kf_a, np.int64); kb = np.ascontiguousarray(kf_b, np.int64)
+        rel = np.ascontiguousarray(rel7, np.float64).reshape(-1, 7); si = np.ascontiguousarray(sqrt_info36, np.float64).reshape(-1, 36)
+        out = np.zeros(max(len(lid), 1), np.uint8); r = PcmStreamReport()
+        self._chk(_lib().d2pgo_pcm_stream(self.h, C.c_int32(len(fid)), _p(fid), _p(fag), _p(ego), C.c_int32(len(lid)), _p(lid), _p(ka), _p(kb), _p(rel),
+                                          _p(si), _p(out), C.byref(r)), "pcm_stream")
+        self.pcm_stream_report = r
+        return out[: len(lid)].astype(bool)
+
+    def debug_pcm_stream_smd(self):
+        """smd of the pairs tested by the last pcm_stream() call: groups in order of their first loop, new rows i ascending, j < i."""
+        n = int(self.pcm_stream_report.pairs_tested)
+        out = np.zeros(max(n, 1))
+        self._chk(_lib().d2pgo_debug_pcm_stream_smd(self.h, _p(out), C.c_int64(out.size)), "debug_pcm_stream_smd")
+        return out[:n]
+
+    def debug_pcm_clique_inc(self, adj, n_new, prev_size):
+        """The incremental clique kernel alone on a symmetric boolean adjacency [n, n] whose last n_new vertices are new ->
+        (boolean membership [n] of the clique found, all False when no seed beats prev_size; FMC's return value)."""
+        words = pcm_pack_bits(adj)
+        n = len(words); member = np.zeros(max(n, 1), np.uint8); size = C.c_int32()
+        self._chk(_lib().d2pgo_debug_pcm_clique_inc(self.h, C.c_int32(n), _p(words if n else np.zeros(1, np.uint32)), C.c_int32(n_new), C.c_int32(prev_size),
+                                                    _p(member), C.byref(size)), "debug_pcm_clique_inc")
+        return member[:n].astype(bool), size.value
 
     # ---- ARock (include/d2pgo.h d2pgo_arock_*)
     @property
@@ -609,6 +656,28 @@ def make_pcm_case(g, outlier_frac=0.05, seed=0):
     return dict(frame_ids=ids, frame_agent=agent, ego=ego, kf_a=np.asarray(g["id_a"][n_odo:]), kf_b=np.asarray(g["id_b"][n_odo:]), rel=rel,
                 rel_bad=rel_bad, sqrt_info=np.asarray(g["sqrt_info"][n_odo:]), outlier=bad, bad_dt=d * np.linalg.norm(rel_bad[bad, :3] - rel[bad, :3], axis=1, keepdims=True),
                 bad_yaw=yaw, n_odo=n_odo)
+
+
+def pcm_arrival_steps(case, n_steps):
+    """Splits a make_pcm_case input into arrival batches, as a PCM stream would receive it: each drone's keyframes are revealed
+    in trajectory order, spread evenly over n_steps steps, and a loop arrives in the first step in which both its keyframes
+    exist (loops of one step in input order).  -> list of (frame indices, loop indices) per step; steps may be empty."""
+    agent = np.asarray(case["frame_agent"])
+    step = np.zeros(len(agent), np.int64)
+    for a in np.unique(agent):
+        f = np.nonzero(agent == a)[0]
+        step[f] = np.arange(len(f)) * n_steps // len(f)
+    fidx = {int(f): k for k, f in enumerate(np.asarray(case["frame_ids"]).tolist())}
+    la = np.array([fidx[int(k)] for k in np.asarray(case["kf_a"])], np.int64); lb = np.array([fidx[int(k)] for k in np.asarray(case["kf_b"])], np.int64)
+    lstep = np.maximum(step[la], step[lb]) if len(la) else np.zeros(0, np.int64)
+    return [(np.nonzero(step == t)[0], np.nonzero(lstep == t)[0]) for t in range(n_steps)]
+
+
+def pcm_stream_args(case, frames, loops, rel_key="rel_bad"):
+    """The arguments of PgoSolver.pcm_stream for frame and loop indices of a make_pcm_case input (loop id = its index)."""
+    return (np.asarray(case["frame_ids"])[frames], np.asarray(case["frame_agent"])[frames], np.asarray(case["ego"])[frames], np.asarray(loops, np.int64),
+            np.asarray(case["kf_a"])[loops], np.asarray(case["kf_b"])[loops], np.asarray(case[rel_key])[loops],
+            np.asarray(case["sqrt_info"]).reshape(-1, 36)[loops])
 
 
 # ------------------------------------------------------------------------------------------------ gravity priors

@@ -16,6 +16,7 @@
  *   d2pgo_get_poses_4d            <- syncFromState: the optimised [x y z yaw] blocks
  *   d2pgo_pcm                     <- SwarmLocalOutlierRejection::OutlierRejectionLoopEdges (enable_pcm), the loops it keeps
  *                                    being those setupLoopFactors receives (d2pgo/src/d2pgo.cpp:177-186, :276-282)
+ *   d2pgo_pcm_stream[_reset]      <- the same object kept across solves: only the loops new in each call are tested (below)
  *   d2pgo_add_gravity_priors      <- setupGravityPriorFactors (enable_gravity_prior): GravityPriorPerturbAD per frame
  *                                    (d2pgo/src/d2pgo.cpp:530-559, GravityPrior.hpp:8-46)
  *   d2pgo_arock_*                 <- ARockPGO, d2pgo's distributed pgo_mode 1 (ARock.cpp:24-314, ARockPGO.cpp:7-104; below)
@@ -152,6 +153,53 @@ int d2pgo_pcm(d2pgo_handle *h, const d2pgo_pcm_config *cfg, int32_t n_frames, co
  * self loops, adj[n][ceil(n / 32)] words, bit j of row i = word j / 32, bit j % 32: member_out[n], size_out = clique size. */
 int d2pgo_debug_pcm_smd(d2pgo_handle *h, double *out, int64_t out_doubles);
 int d2pgo_debug_pcm_clique(d2pgo_handle *h, int32_t n, const uint32_t *adj, uint8_t *member_out, int32_t *size_out);
+
+/* ---- PCM as a stream: the stateful object the reference node keeps between solves
+ *   d2pgo_pcm_stream_reset  <- a new SwarmLocalOutlierRejection (redundant = true, is_4dof = (pose_dof == 4)) over empty
+ *                              trajectories (d2pgo/src/swarm_outlier_rejection/swarm_outlier_rejection.cpp:20-30)
+ *   d2pgo_pcm_stream        <- one OutlierRejectionLoopEdges call with available_loops = the loops given
+ *                              (swarm_outlier_rejection.cpp:46-120; D2PGO::solve_single / solve_multi pass every loop they
+ *                              hold on each call, d2pgo/src/d2pgo.cpp:170-186), after the keyframes new since the last call
+ *                              were pushed to their drones' trajectories
+ *   incremental = 0         <- incremental_pcm = false: FMC::maxCliqueHeu on each group that got new loops (:287-301)
+ *   incremental = 1         <- incremental_pcm = true (the d2pgo_config.h default): FMC::maxCliqueHeuIncremental's search
+ *                              (d2pgo/third_party/fast_max-clique_finder/src/findCliqueHeuInc.cpp:32-96, :269-281)
+ * A loop is tested only the first time its id appears, against every earlier loop of its group (edge1 = the new loop), with
+ * d2pgo_pcm's consistency test; the consistency graph stays on the device between calls.  Only groups that got new loops run
+ * the clique again; the others keep their inlier sets.  Mode 0 gives, after any split of an input into calls, the mask and
+ * the smd d2pgo_pcm gives on the concatenated input.  Mode 1 seeds only the new vertices, starts from m = the group's clique
+ * size, and replaces the group's set when a seed's clique beats m.
+ * Declared deviation (mode 1): the reference copies FMC's candidate buffer v_i_S into the result (findCliqueHeuInc.cpp:92-94),
+ * which is not the clique; here the set is the clique the search found, seed and picks, and its size is FMC's return value.
+ * inlier_out[n_loops] = the call's loops that are in their group's set (:96-111; every group the stream holds has a set).
+ * The stream is independent of d2pgo_pcm's buffers: calls to the two may interleave.  Deterministic, no atomics.
+ * Refusals keep nothing of the call (the stream is as before it) and set d2pgo_last_error: 5 before any reset; 3 on a loop
+ * naming an unknown keyframe, a loop id twice in one call, or a keyframe id given again with another drone; 2 on a non-finite
+ * ego pose, relative pose or sqrt_info of a new frame or loop; 4 on a group growing past 32768 loops; 1 on a null argument. */
+typedef struct d2pgo_pcm_stream_report {
+  int32_t new_loops, total_loops;    /* loops first seen in this call; loops in the stream                              */
+  int32_t groups, groups_touched;    /* drone pairs in the stream; those that got new loops                             */
+  int32_t inliers;                   /* over the loops passed to this call                                              */
+  int64_t pairs_tested, consistent_pairs, clique_rounds;   /* this call only                                           */
+  double device_ms, pair_ms, clique_ms;
+} d2pgo_pcm_stream_report;
+
+/* forgets every frame, loop and clique.  cfg as for d2pgo_pcm; incremental 0 or 1 (above). */
+int d2pgo_pcm_stream_reset(d2pgo_handle *h, const d2pgo_pcm_config *cfg, int32_t incremental);
+/* frames: keyframes new since the last call, appended to their drone's trajectory in the order given (a keyframe id already in
+ * the stream is ignored when it names the same drone).  loops: the call's available_loops keyed by loop_ids; an id seen
+ * before is not tested again and its other fields are ignored. */
+int d2pgo_pcm_stream(d2pgo_handle *h, int32_t n_frames, const int64_t *frame_ids, const int32_t *frame_agent, const double *ego_poses7,
+                     int32_t n_loops, const int64_t *loop_ids, const int64_t *kf_a, const int64_t *kf_b, const double *rel7,
+                     const double *sqrt_info36, uint8_t *inlier_out, d2pgo_pcm_stream_report *report);
+/* parity hooks.  The smd of the pairs tested by the last stream call (report.pairs_tested doubles): groups in order of their
+ * first loop, new rows i ascending, j < i ascending.  The incremental clique kernel alone on a caller-given adjacency (as
+ * d2pgo_debug_pcm_clique) whose last n_new vertices are new, under the bound prev_size: member_out = the clique found when a
+ * seed beats prev_size, else all 0; size_out = FMC::maxCliqueHeuIncremental's return value (n_new = n, prev_size = 0 is
+ * maxCliqueHeu). */
+int d2pgo_debug_pcm_stream_smd(d2pgo_handle *h, double *out, int64_t out_doubles);
+int d2pgo_debug_pcm_clique_inc(d2pgo_handle *h, int32_t n, const uint32_t *adj, int32_t n_new, int32_t prev_size, uint8_t *member_out,
+                               int32_t *size_out);
 
 /* ---- ARock distributed mode (d2pgo's pgo_mode 1: PGO_MODE_DISTRIBUTED_AROCK)
  *   d2pgo_arock_enable     <- ARockPGO construction with ARockSolverConfig (d2common/include/d2common/solver/ARock.hpp:6-19)
