@@ -18,6 +18,7 @@
 
 #include "d2ba_math.cuh"
 #include "d2pgo_handle.cuh"
+#include "d2pgo_lm.cuh"
 
 namespace d2ba {
 // NCCL through the dlopen'ed entry points of d2ba_host.cu
@@ -1029,22 +1030,29 @@ static PgoArockDev pgo_arock_view(d2pgo_handle *h, int cur) {
 // cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks.  grav: the
 // gravity priors of this rank (6-DoF only; their cost partials follow the edges', their terms enter g and D after each pose's
 // edges).  ark: the ARock proximal terms of the synced dual table (cost partials last, g and D after the edges and priors).
+// the kernels of one linearisation of buffer b on stream st, the total cost into *cost_dev
 template <class P>
-static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, bool grav, bool ark, double *cost) {
+static void pgo_linearize_enqueue(d2pgo_handle *h, cudaStream_t st, int b, int want_jac, bool grav, bool ark, double *cost_dev) {
   constexpr int D = P::D;
   PgoDev d = pgo_view(h, b);
   const PgoPriorDev pr = pgo_prior_view(h, b);
   const PgoArockDev ak = pgo_arock_view(h, b);
-  const size_t N = h->ids.size();
   const int nbe = (d.n_edge + 127) / 128, nbg = grav ? (pr.n_prior + 127) / 128 : 0, nbk = ark ? (ak.n_dual + 127) / 128 : 0;
-  if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, h->stream>>>(d, h->d_cost_part.p, want_jac);
-  if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, h->stream>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
-  if (nbk > 0) k_pgo_arock_lin<D><<<nbk, 128, 0, h->stream>>>(d, h->d_cost_part.p + nbe + nbg, ak);
-  k_pgo_sum<<<1, 128, 0, h->stream>>>(h->d_cost_part.p, nbe + nbg + nbk, h->d_cost.p);
+  if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, st>>>(d, h->d_cost_part.p, want_jac);
+  if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, st>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
+  if (nbk > 0) k_pgo_arock_lin<D><<<nbk, 128, 0, st>>>(d, h->d_cost_part.p + nbe + nbg, ak);
+  k_pgo_sum<<<1, 128, 0, st>>>(h->d_cost_part.p, nbe + nbg + nbk, cost_dev);
   if (want_jac && grav) {
-    if constexpr (D == 6) k_pgo_gD<P, true><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
-  } else if (want_jac) k_pgo_gD<P, false><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
-  if (want_jac && nbk > 0) k_pgo_arock_gD<D><<<d.nbp, 128, 0, h->stream>>>(d, h->d_g[b].p, h->d_D[b].p, ak);
+    if constexpr (D == 6) k_pgo_gD<P, true><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+  } else if (want_jac) k_pgo_gD<P, false><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+  if (want_jac && nbk > 0) k_pgo_arock_gD<D><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, ak);
+}
+
+template <class P>
+static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, bool grav, bool ark, double *cost) {
+  constexpr int D = P::D;
+  const size_t N = h->ids.size();
+  pgo_linearize_enqueue<P>(h, h->stream, b, want_jac, grav, ark, h->d_cost.p);
   if (h->comm) {
     if (nccl_allreduce_f64(h->comm, h->d_cost.p, 1, h->stream)) { h->err = "ncclAllReduce(cost) failed"; return 40; }
     if (want_jac && (nccl_allreduce_f64(h->comm, h->d_g[b].p, N * D, h->stream) || nccl_allreduce_f64(h->comm, h->d_D[b].p, N * D * D, h->stream))) { h->err = "ncclAllReduce(g, D) failed"; return 40; }
@@ -1225,12 +1233,174 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   return 0;
 }
 
+// ---- the ceres minimiser's host side: refusals, the graph of one solve, and the solve.  The graph:
+//   k_lm_start, linearisation of x0 (buffer 0), k_lm_scale, k_lm_xnorm, then WHILE(loop) {
+//     k_lm_begin; IF(go) { factor + solve (k_chol_diag_lm's damping), k_lm_model, k_lm_mid;
+//                          IF(eval) { x1 = x0 [+] dx, cost of buffer 1 into d_cost[1] }; k_lm_end;
+//                          IF(accept) { x0 <- x1 (N x 64 bytes), linearisation of x0 into d_cost[0], k_lm_xnorm } } }
+// Accepting copies the candidate's poses into buffer 0 and relinearises there (as ceres evaluates the Jacobian at the new x),
+// so the kernels' buffer pointers are fixed and the graph serves every solve of the same buffers.
+static int lm_refuse(d2pgo_handle *h, const char *what) {
+  if (h->minimizer != D2PGO_MINIMIZER_CERES_LM) return 0;
+  if (h->comm) return pgo_fail(h, 5, std::string(what) + ": the ceres minimiser has no edge-sharded form (the handle has a communicator)");
+  if (h->linear_solver != D2PGO_LINEAR_SPARSE_CHOLESKY)
+    return pgo_fail(h, 5, std::string(what) + ": the ceres minimiser takes exact steps from the sparse Cholesky (d2pgo_set_linear_solver(h, D2PGO_LINEAR_SPARSE_CHOLESKY) first)");
+  if (!h->driver_version && cudaDriverGetVersion(&h->driver_version) != cudaSuccess) h->driver_version = 0;
+  if (h->driver_version < 12040)
+    return pgo_fail(h, 3, std::string(what) + ": the ceres minimiser runs as one CUDA graph with conditional nodes, which needs a driver for CUDA 12.4 or newer (this one: " +
+                              std::to_string(h->driver_version) + ")");
+  return 0;
+}
+
+// appends a conditional node on the handle `c` after the work captured so far on st; *body = the graph it runs
+static cudaError_t lm_cond(cudaStream_t st, cudaGraphConditionalHandle c, cudaGraphConditionalNodeType type, cudaGraph_t *body) {
+  cudaStreamCaptureStatus cs;
+  cudaGraph_t g;
+  const cudaGraphNode_t *deps = nullptr;
+  size_t nd = 0;
+  cudaError_t e = cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, &deps, &nd);
+  if (e != cudaSuccess) return e;
+  cudaGraphNodeParams p = {cudaGraphNodeTypeConditional};
+  p.conditional.handle = c; p.conditional.type = type; p.conditional.size = 1;
+  cudaGraphNode_t node;
+  if ((e = cudaGraphAddNode(&node, g, deps, nd, &p)) != cudaSuccess) return e;
+  *body = p.conditional.phGraph_out[0];
+  return cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies);
+}
+
+template <class P>
+static int lm_build(d2pgo_handle *h, bool grav, bool ark, cudaStream_t *cs) {
+  constexpr int D = P::D;
+  const PgoDev d0 = pgo_view(h, 0), d1 = pgo_view(h, 1);
+  const PgoPriorDev pr = pgo_prior_view(h, 0);
+  const PgoArockDev ak = pgo_arock_view(h, 0);
+  const int nbp = d0.nbp, nbe = (d0.n_edge + 127) / 128, nbg = grav ? (pr.n_prior + 127) / 128 : 0, nbk = ark ? (ak.n_dual + 127) / 128 : 0;
+  const int nbm = nbe + nbg + nbk + nbp;
+  const d2pgo_lm::View v{D, d0.n_pose, d0.n_edge, grav ? pr.n_prior : 0, ark ? ak.n_dual : 0, d0.x, h->d_g[0].p, d0.dx, d0.lin, pr.lin, ak.lin,
+                         d0.fixed, d0.ea, d0.eb, pr.pose, ak.pose};
+  LmState *s = h->d_lm.p;
+  double *xpart = h->d_lm_part.p, *mpart = xpart + 2 * (size_t)nbp, *cost = h->d_cost.p;
+  d2pgo_minimizer_iteration *trace = h->d_lm_trace.p;
+  const d2pgo_chol::Lin in{h->d_lin[0].p, h->d_D[0].p, h->d_g[0].p, h->d_fixed.p, h->d_ea.p, h->d_eb.p, h->d_dx.p};
+  const d2pgo_chol::LmDamping dm{h->d_lm_scale.p, &s->radius};
+  cudaGraph_t top = nullptr, body, go_g, eval_g, acc_g;
+  cudaGraphConditionalHandle loop, go, eval, acc;
+  PCK(cudaGraphCreate(&top, 0));
+  std::unique_ptr<CUgraph_st, cudaError_t (*)(cudaGraph_t)> own(top, cudaGraphDestroy);
+  const cudaStreamCaptureMode mode = cudaStreamCaptureModeThreadLocal;
+  PCK(cudaGraphConditionalHandleCreate(&loop, top, 1, cudaGraphCondAssignDefault));
+  PCK(cudaStreamBeginCaptureToGraph(cs[0], top, nullptr, nullptr, 0, mode));
+  d2pgo_lm::start(cs[0], s);
+  pgo_linearize_enqueue<P>(h, cs[0], 0, 1, grav, ark, cost);
+  d2pgo_lm::scale(cs[0], v, h->d_D[0].p, s, h->d_lm_scale.p);
+  d2pgo_lm::xnorm(cs[0], v, xpart);
+  PCK(lm_cond(cs[0], loop, cudaGraphCondTypeWhile, &body));
+  PCK(cudaStreamEndCapture(cs[0], &top));
+  PCK(cudaGraphConditionalHandleCreate(&go, body, 0, 0));
+  PCK(cudaStreamBeginCaptureToGraph(cs[1], body, nullptr, nullptr, 0, mode));
+  d2pgo_lm::begin(cs[1], s, cost, xpart, nbp, loop, go);
+  PCK(lm_cond(cs[1], go, cudaGraphCondTypeIf, &go_g));
+  PCK(cudaStreamEndCapture(cs[1], &body));
+  PCK(cudaGraphConditionalHandleCreate(&eval, go_g, 0, 0));
+  PCK(cudaGraphConditionalHandleCreate(&acc, go_g, 0, 0));
+  PCK(cudaStreamBeginCaptureToGraph(cs[2], go_g, nullptr, nullptr, 0, mode));
+  if (int rc = h->chol->enqueue_lm(cs[2], in, dm, h->err)) { cudaStreamEndCapture(cs[2], &go_g); return rc; }
+  d2pgo_lm::model(cs[2], v, nbe, nbg, nbk, mpart);
+  d2pgo_lm::mid(cs[2], s, h->chol->d_fail, mpart, nbm, trace, eval);
+  PCK(lm_cond(cs[2], eval, cudaGraphCondTypeIf, &eval_g));
+  d2pgo_lm::end(cs[2], s, cost, trace, acc);
+  PCK(lm_cond(cs[2], acc, cudaGraphCondTypeIf, &acc_g));
+  PCK(cudaStreamEndCapture(cs[2], &go_g));
+  PCK(cudaStreamBeginCaptureToGraph(cs[3], eval_g, nullptr, nullptr, 0, mode));
+  k_pgo_retract<P><<<nbp, 128, 0, cs[3]>>>(d0, h->d_x[1].p);
+  pgo_linearize_enqueue<P>(h, cs[3], 1, 0, grav, ark, cost + 1);
+  PCK(cudaStreamEndCapture(cs[3], &eval_g));
+  PCK(cudaStreamBeginCaptureToGraph(cs[3], acc_g, nullptr, nullptr, 0, mode));
+  PCK(cudaMemcpyAsync(h->d_x[0].p, d1.x, (size_t)d0.n_pose * 64, cudaMemcpyDeviceToDevice, cs[3]));
+  pgo_linearize_enqueue<P>(h, cs[3], 0, 1, grav, ark, cost);
+  d2pgo_lm::xnorm(cs[3], v, xpart);
+  PCK(cudaStreamEndCapture(cs[3], &acc_g));
+  PCK(cudaGetLastError());
+  if (h->lm_graph) { cudaGraphExecDestroy(h->lm_graph); h->lm_graph = nullptr; }
+  PCK(cudaGraphInstantiate(&h->lm_graph, top, 0));
+  return 0;
+}
+
+constexpr int kLmTraceCap = 16384;   // trace records kept per solve (the first iterations)
+
+// ceres' TrustRegionMinimizer with LevenbergMarquardtStrategy (d2pgo_set_minimizer): one graph launch, one synchronisation
+template <class P>
+static int pgo_solve_ceres(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
+  int rc, syncs = 1;
+  if ((rc = pgo_chol_prepare(h))) return rc;
+  if (!h->uploaded) { if ((rc = pgo_upload(h))) return rc; syncs++; }
+  if (!h->chol->dev_ready) { if ((rc = h->chol->upload(h->stream, h->err))) return rc; syncs++; }
+  const bool grav = !h->gp_pose.empty();
+  const d2pgo_ceres_lm_config &c = h->lm_cfg;
+  const int N = (int)h->ids.size(), D = P::D, nbp = (N + 127) / 128;
+  const int nbm = (int)(h->ea.size() + 127) / 128 + (grav ? (int)(h->gp_pose.size() + 127) / 128 : 0) + (ark ? (std::max(h->ak_n, 0) + 127) / 128 : 0) + nbp;
+  const int cap = std::max(1, std::min(c.max_num_iterations, kLmTraceCap));
+  PCK(h->d_lm.alloc(1)); PCK(h->d_lm_scale.alloc((size_t)N * D)); PCK(h->d_lm_part.alloc(2 * (size_t)nbp + 3 * (size_t)nbm));
+  PCK(h->d_lm_trace.alloc(cap));
+  // the graph holds every pointer and count its kernels were captured with: rebuilt when any of those bytes differ
+  std::string key;
+  auto put = [&key](const void *p, size_t n) { key.append((const char *)p, n); };
+  for (int b = 0; b < 2; b++) {
+    const PgoDev d = pgo_view(h, b); const PgoPriorDev pr = pgo_prior_view(h, b); const PgoArockDev ak = pgo_arock_view(h, b);
+    put(&d, sizeof d); put(&pr, sizeof pr); put(&ak, sizeof ak);
+  }
+  const void *ptrs[7] = {h->d_lm.p, h->d_lm_scale.p, h->d_lm_part.p, h->d_lm_trace.p, h->d_cost.p, h->d_cost_part.p, h->chol.get()};
+  const int gen[4] = {h->chol->generation, grav, ark, 0};
+  put(ptrs, sizeof ptrs); put(gen, sizeof gen);
+  if (!h->lm_graph || h->lm_key != key) {
+    cudaStream_t cs[4] = {h->stream, nullptr, nullptr, nullptr};
+    for (int k = 1; k < 4; k++) PCK(cudaStreamCreateWithFlags(&cs[k], cudaStreamNonBlocking));
+    rc = lm_build<P>(h, grav, ark, cs);
+    for (int k = 1; k < 4; k++) cudaStreamDestroy(cs[k]);
+    if (rc) { h->lm_key.clear(); return rc; }
+    h->lm_key = key;
+  }
+  LmState st;
+  memset(&st, 0, sizeof st);
+  st.radius0 = c.initial_trust_region_radius; st.max_radius = c.max_trust_region_radius; st.min_radius = c.min_trust_region_radius;
+  st.min_diag = c.min_lm_diagonal; st.max_diag = c.max_lm_diagonal; st.min_rel_dec = c.min_relative_decrease;
+  st.ftol = c.function_tolerance; st.gtol = c.gradient_tolerance; st.ptol = c.parameter_tolerance; st.budget_s = c.max_solver_time_in_seconds;
+  st.max_iter = c.max_num_iterations; st.max_invalid = c.max_num_consecutive_invalid_steps; st.jacobi = c.jacobi_scaling; st.trace_cap = cap;
+  PCK(cudaMemcpyAsync(h->d_lm.p, &st, sizeof st, cudaMemcpyHostToDevice, h->stream));
+  PCK(cudaEventRecord(h->ev0, h->stream));
+  PCK(cudaGraphLaunch(h->lm_graph, h->stream));
+  PCK(cudaEventRecord(h->ev1, h->stream));
+  PCK(cudaMemcpyAsync(h->poses.data(), h->d_x[0].p, (size_t)N * 64, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaMemcpyAsync(&st, h->d_lm.p, sizeof st, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaStreamSynchronize(h->stream));   // the solve's one synchronisation
+  float ms = 0; cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+  d2pgo_minimizer_summary &m = h->lm_report;
+  memset(&m, 0, sizeof m);
+  m.termination_type = st.type; m.reason = st.reason; m.successful_steps = st.ok; m.unsuccessful_steps = st.bad; m.host_syncs = syncs;
+  m.final_radius = st.radius; m.elapsed_s = (double)(st.t_end - st.t0) * 1e-9; m.initial_cost = st.cost0; m.final_cost = st.cost;
+  h->lm_ran = true; h->lm_trace_n = std::min(st.iter, cap);
+  h->chol->factorizations = st.iter; h->chol->failed = st.pivot_fail; h->chol->factor_ms = h->chol->solve_ms = 0.0;
+  d2pgo_report R; memset(&R, 0, sizeof R);
+  R.iterations = st.ok + st.bad; R.accepted = st.ok; R.converged = st.type == D2PGO_TERMINATION_CONVERGENCE;
+  R.initial_cost = st.cost0; R.final_cost = st.cost; R.device_ms = ms;
+  if (rep) *rep = R;
+  return 0;
+}
+
+// the handle's minimiser (d2pgo_set_minimizer); its refusals (lm_refuse) come before any state changes, in the callers
+template <class P>
+static int pgo_minimize(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
+  h->lm_ran = false;
+  return h->minimizer == D2PGO_MINIMIZER_CERES_LM ? pgo_solve_ceres<P>(h, rep, ark) : pgo_solve<P>(h, rep, ark);
+}
+
 extern "C" {
 
 int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h || h->ids.empty()) return 1;
+  if (int rc = lm_refuse(h, "solve")) return rc;
   cudaSetDevice(h->cfg.device);
-  return h->dof == 4 ? pgo_solve<PgoEdge4>(h, rep, false) : pgo_solve<PgoEdge6>(h, rep, false);
+  return h->dof == 4 ? pgo_minimize<PgoEdge4>(h, rep, false) : pgo_minimize<PgoEdge6>(h, rep, false);
 }
 
 int d2pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out) {
@@ -1511,6 +1681,7 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h) return 1;
   if (h->ids.empty()) return pgo_fail(h, 1, "arock_step: no poses");
   if (int rc = arock_check_poses(h, "arock_step")) return rc;
+  if (int rc = lm_refuse(h, "arock_step")) return rc;
   cudaSetDevice(h->cfg.device);
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
@@ -1537,7 +1708,7 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
   }
   // 3. setDualStateFactors + solveLocalStep: the LM solve with the proximal terms towards y_r
   if (created && (rc = arock_sync(h))) return rc;
-  if ((rc = D == 4 ? pgo_solve<PgoEdge4>(h, rep, true) : pgo_solve<PgoEdge6>(h, rep, true))) return rc;
+  if ((rc = D == 4 ? pgo_minimize<PgoEdge4>(h, rep, true) : pgo_minimize<PgoEdge6>(h, rep, true))) return rc;
   // 4. updateDualStates at the solved poses, which pgo_solve leaves in buffer 0
   const PgoArockDev ak = pgo_arock_view(h, 0);
   if (ak.n_dual > 0) {
@@ -2154,6 +2325,63 @@ int d2pgo_debug_arock_rot_state(d2pgo_handle *h, double *state9_out, uint8_t *fl
   int k = 0;
   for (const auto &kv : duals) { neighbour_out[k] = kv.first.first; frame_out[k] = kv.first.second; k++; }
   arock_flatten(duals.begin(), duals.end(), 9, local9_out, remote9_out);
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- minimiser selection and its reports (include/d2pgo.h d2pgo_set_minimizer)
+extern "C" {
+
+int d2pgo_default_ceres_lm_config(d2pgo_ceres_lm_config *c) {
+  if (!c) return 1;
+  memset(c, 0, sizeof *c);
+  c->max_num_iterations = 50; c->max_num_consecutive_invalid_steps = 5; c->jacobi_scaling = 1;
+  c->max_solver_time_in_seconds = 0.0; c->initial_trust_region_radius = 1e4; c->max_trust_region_radius = 1e16;
+  c->min_trust_region_radius = 1e-32; c->min_relative_decrease = 1e-3; c->min_lm_diagonal = 1e-6; c->max_lm_diagonal = 1e32;
+  c->function_tolerance = 1e-6; c->gradient_tolerance = 1e-10; c->parameter_tolerance = 1e-8;
+  return 0;
+}
+
+int d2pgo_set_minimizer(d2pgo_handle *h, int32_t kind, const d2pgo_ceres_lm_config *cfg) {
+  if (!h) return 1;
+  if (kind == D2PGO_MINIMIZER_RESTATED) { h->minimizer = kind; return 0; }
+  if (kind != D2PGO_MINIMIZER_CERES_LM)
+    return pgo_fail(h, 2, "set_minimizer: unknown kind " + std::to_string(kind) + " (0 = the restated LM loop, 1 = ceres LM)");
+  d2pgo_ceres_lm_config c;
+  if (cfg) c = *cfg; else d2pgo_default_ceres_lm_config(&c);
+  const double v[10] = {c.max_solver_time_in_seconds, c.initial_trust_region_radius, c.max_trust_region_radius, c.min_trust_region_radius,
+                        c.min_relative_decrease, c.min_lm_diagonal, c.max_lm_diagonal, c.function_tolerance, c.gradient_tolerance, c.parameter_tolerance};
+  for (double x : v)
+    if (!(std::isfinite(x) && x >= 0.0)) return pgo_fail(h, 2, "set_minimizer: every real field must be finite and non-negative");
+  if (c.max_num_iterations < 0 || c.max_num_consecutive_invalid_steps < 0 || (c.jacobi_scaling != 0 && c.jacobi_scaling != 1))
+    return pgo_fail(h, 2, "set_minimizer: max_num_iterations and max_num_consecutive_invalid_steps must be >= 0, jacobi_scaling 0 or 1");
+  if (!(c.min_trust_region_radius > 0.0 && c.min_trust_region_radius <= c.initial_trust_region_radius &&
+        c.initial_trust_region_radius <= c.max_trust_region_radius))
+    return pgo_fail(h, 2, "set_minimizer: need 0 < min_trust_region_radius <= initial_trust_region_radius <= max_trust_region_radius");
+  if (!(c.min_lm_diagonal > 0.0 && c.min_lm_diagonal <= c.max_lm_diagonal))
+    return pgo_fail(h, 2, "set_minimizer: need 0 < min_lm_diagonal <= max_lm_diagonal");
+  h->minimizer = kind; h->lm_cfg = c;
+  return 0;
+}
+
+int d2pgo_minimizer_report(d2pgo_handle *h, d2pgo_minimizer_summary *out) {
+  if (!h || !out) return 1;
+  if (!h->lm_ran) return pgo_fail(h, 5, "minimizer_report: the last solve or ARock step did not run the ceres minimiser");
+  *out = h->lm_report;
+  return 0;
+}
+
+int d2pgo_debug_minimizer_trace(d2pgo_handle *h, int32_t max, int32_t *n_out, d2pgo_minimizer_iteration *out) {
+  if (!h || !n_out || (max > 0 && !out)) return 1;
+  if (!h->lm_ran) return pgo_fail(h, 5, "debug_minimizer_trace: the last solve or ARock step did not run the ceres minimiser");
+  *n_out = h->lm_trace_n;
+  if (max < h->lm_trace_n) return pgo_fail(h, 2, "debug_minimizer_trace: " + std::to_string(h->lm_trace_n) + " records, room for " + std::to_string(max));
+  cudaSetDevice(h->cfg.device);
+  if (h->lm_trace_n > 0) {
+    PCK(cudaMemcpyAsync(out, h->d_lm_trace.p, (size_t)h->lm_trace_n * sizeof *out, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaStreamSynchronize(h->stream));
+  }
   return 0;
 }
 

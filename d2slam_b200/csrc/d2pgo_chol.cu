@@ -382,6 +382,36 @@ __global__ void __launch_bounds__(128) k_chol_diag(Dev c) {
   for (int k = 0; k < D; k++) c.b[(size_t)j * D + k] = -c.g[(size_t)i * D + k];
 }
 
+// k_chol_diag with ceres' Levenberg-Marquardt damping (d2pgo_set_minimizer's CERES_LM) in place of lambda diag(D) + 1e-12:
+// mu_k = clamp(s_k^2 D_kk, min_diag, max_diag) / (radius s_k^2), s the Jacobi scale, par = {radius, min_diag, max_diag}
+// in device memory (the minimiser's control kernel moves the radius between factorisations)
+template <int D>
+__global__ void __launch_bounds__(128) k_chol_diag_lm(Dev c, const double *scale, const double *par) {
+  constexpr int DD = D * D;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= c.n_free) return;
+  const int i = c.perm[j];
+  const size_t E = (size_t)c.n_edge;
+  double A[DD];
+  for (int k = 0; k < DD; k++) A[k] = c.Dg[(size_t)i * DD + k];
+  for (int q = c.self_ptr[j]; q < c.self_ptr[j + 1]; q++) {
+    const int e = c.self_edge[q];
+    const double *J0 = c.lin + (size_t)D * E + e, *J1 = J0 + (size_t)DD * E;
+    for (int k = 0; k < D; k++) {
+      double j0[D], j1[D];
+      for (int a = 0; a < D; a++) { j0[a] = J0[(size_t)(k * D + a) * E]; j1[a] = J1[(size_t)(k * D + a) * E]; }
+      for (int a = 0; a < D; a++) for (int b = 0; b < D; b++) A[a * D + b] += j0[a] * j1[b] + j1[a] * j0[b];
+    }
+  }
+  const double radius = par[0], lo = par[1], hi = par[2];
+  for (int k = 0; k < D; k++) {
+    const double s2 = scale[(size_t)i * D + k] * scale[(size_t)i * D + k];
+    A[k * (D + 1)] += fmin(fmax(s2 * c.Dg[(size_t)i * DD + k * (D + 1)], lo), hi) / (radius * s2);
+  }
+  for (int k = 0; k < DD; k++) c.diagH[(size_t)j * DD + k] = A[k];
+  for (int k = 0; k < D; k++) c.b[(size_t)j * D + k] = -c.g[(size_t)i * D + k];
+}
+
 struct Front { int s, f, W, M; double *F; };
 template <int D>
 __device__ Front front_of(const Dev &c, int s) {
@@ -538,10 +568,14 @@ __global__ void k_chol_scatter(Dev c) {   // dx per pose from x in column order;
   for (int k = 0; k < D; k++) c.dx[(size_t)i * D + k] = j < 0 ? 0.0 : c.x[(size_t)j * D + k];
 }
 
+// lm: the damping of k_chol_diag_lm (or null: k_chol_diag's)
 template <int D>
-void launch_factor(const Dev &c, const Symbolic &S, cudaStream_t st) {
+void launch_factor(const Dev &c, const Symbolic &S, cudaStream_t st, const LmDamping *lm = nullptr) {
   if (c.n_pair > 0) k_chol_pairs<D><<<(c.n_pair + 127) / 128, 128, 0, st>>>(c);
-  if (c.n_free > 0) k_chol_diag<D><<<(c.n_free + 127) / 128, 128, 0, st>>>(c);
+  if (c.n_free > 0) {
+    if (lm) k_chol_diag_lm<D><<<(c.n_free + 127) / 128, 128, 0, st>>>(c, lm->scale, lm->par);
+    else k_chol_diag<D><<<(c.n_free + 127) / 128, 128, 0, st>>>(c);
+  }
   for (size_t l = 0; l + 1 < S.lvl_ptr.size(); l++) {
     int m = 0;   // the level's largest front sets its shared memory
     for (int k = S.lvl_ptr[l]; k < S.lvl_ptr[l + 1]; k++) m = std::max(m, S.idx_ptr[S.lvl_sn[k] + 1] - S.idx_ptr[S.lvl_sn[k]]);
@@ -603,22 +637,44 @@ int Numeric::upload(cudaStream_t st, std::string &err) {
   for (auto &e : ev) CCK(cudaEventCreate(&e));
   CCK(cudaFuncSetAttribute(k_chol_factor<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)factor_smem(kMaxFront)));
   CCK(cudaFuncSetAttribute(k_chol_factor<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)factor_smem(kMaxFront)));
+  static int uploads = 0;   // process-wide, so that a new Numeric never repeats an old one's generation
   dev_ready = true;
+  generation = ++uploads;
+  return 0;
+}
+
+namespace {
+// the kernels' view of n's tables and arenas with the linearisation buffers `in`
+Dev dev_of(const Numeric &n, const Lin &in) {
+  const Symbolic &S = n.sym;
+  const int *d_i = n.d_i;
+  Dev c;
+  memset(&c, 0, sizeof c);
+  c.n_pose = S.n_pose; c.n_free = S.n_free; c.n_edge = S.n_edge; c.n_pair = S.n_pairs;
+  c.lin = in.lin; c.Dg = in.Dg; c.g = in.g; c.fixed = in.fixed; c.ea = in.ea; c.eb = in.eb; c.dx = in.dx;
+  c.perm = d_i + n.o_perm; c.col_of = d_i + n.o_col_of; c.pair_lo = d_i + n.o_pair_lo; c.pair_ptr = d_i + n.o_pair_ptr; c.pair_edge = d_i + n.o_pair_edge;
+  c.self_ptr = d_i + n.o_self_ptr; c.self_edge = d_i + n.o_self_edge; c.sn_first = d_i + n.o_sn_first; c.sn_width = d_i + n.o_sn_width;
+  c.idx_ptr = d_i + n.o_idx_ptr; c.idx = d_i + n.o_idx; c.relmap = d_i + n.o_relmap; c.ch_ptr = d_i + n.o_ch_ptr; c.ch = d_i + n.o_ch;
+  c.po_ptr = d_i + n.o_po_ptr; c.po_pair = d_i + n.o_po_pair; c.po_row = d_i + n.o_po_row; c.po_col = d_i + n.o_po_col; c.po_tr = d_i + n.o_po_tr;
+  c.lvl_sn = d_i + n.o_lvl_sn; c.sn_off = n.d_off; c.sn_uoff = n.d_off + S.sn_off.size();
+  c.pairH = n.d_pairH; c.diagH = n.d_diagH; c.front = n.d_front; c.uvec = n.d_uvec; c.b = n.d_b; c.y = n.d_y; c.x = n.d_x; c.lambda = n.d_lambda;
+  c.fail = n.d_fail;
+  return c;
+}
+}  // namespace
+
+int Numeric::enqueue_lm(cudaStream_t st, const Lin &in, const LmDamping &lm, std::string &err) {
+  const Dev c = dev_of(*this, in);
+  CCK(cudaMemsetAsync(d_fail, 0, 4, st));
+  if (sym.D == 6) { launch_factor<6>(c, sym, st, &lm); launch_solve<6>(c, sym, st); }
+  else { launch_factor<4>(c, sym, st, &lm); launch_solve<4>(c, sym, st); }
+  CCK(cudaGetLastError());
   return 0;
 }
 
 int Numeric::step(cudaStream_t st, int par, const Lin &in, double lambda, bool *failed_out, std::string &err) {
   const Symbolic &S = sym;
-  Dev c;
-  memset(&c, 0, sizeof c);
-  c.n_pose = S.n_pose; c.n_free = S.n_free; c.n_edge = S.n_edge; c.n_pair = S.n_pairs;
-  c.lin = in.lin; c.Dg = in.Dg; c.g = in.g; c.fixed = in.fixed; c.ea = in.ea; c.eb = in.eb; c.dx = in.dx;
-  c.perm = d_i + o_perm; c.col_of = d_i + o_col_of; c.pair_lo = d_i + o_pair_lo; c.pair_ptr = d_i + o_pair_ptr; c.pair_edge = d_i + o_pair_edge;
-  c.self_ptr = d_i + o_self_ptr; c.self_edge = d_i + o_self_edge; c.sn_first = d_i + o_sn_first; c.sn_width = d_i + o_sn_width;
-  c.idx_ptr = d_i + o_idx_ptr; c.idx = d_i + o_idx; c.relmap = d_i + o_relmap; c.ch_ptr = d_i + o_ch_ptr; c.ch = d_i + o_ch;
-  c.po_ptr = d_i + o_po_ptr; c.po_pair = d_i + o_po_pair; c.po_row = d_i + o_po_row; c.po_col = d_i + o_po_col; c.po_tr = d_i + o_po_tr;
-  c.lvl_sn = d_i + o_lvl_sn; c.sn_off = d_off; c.sn_uoff = d_off + S.sn_off.size();
-  c.pairH = d_pairH; c.diagH = d_diagH; c.front = d_front; c.uvec = d_uvec; c.b = d_b; c.y = d_y; c.x = d_x; c.lambda = d_lambda; c.fail = d_fail;
+  const Dev c = dev_of(*this, in);
   if (memcmp(&gkey[par], &in, sizeof in)) {   // capture this parity's two graphs for these buffers
     if (gfac[par]) cudaGraphExecDestroy(gfac[par]);
     if (gsol[par]) cudaGraphExecDestroy(gsol[par]);

@@ -51,6 +51,10 @@ struct Lin {
   double *dx;                   // [N][D] output
 };
 
+// the damping of a ceres Levenberg-Marquardt step (d2pgo_set_minimizer): scale [N][D] the Jacobi scale s, par -> {radius,
+// min_lm_diagonal, max_lm_diagonal}, both in device memory
+struct LmDamping { const double *scale, *par; };
+
 struct Numeric {
   Symbolic sym;
   bool dev_ready = false;
@@ -68,6 +72,7 @@ struct Numeric {
   bool has_system = false;      // d_pairH / d_diagH / d_b hold the system of a step on these buffers
   // counters of the last solve
   int factorizations = 0, failed = 0; double factor_ms = 0.0, solve_ms = 0.0;
+  int generation = 0;           // set by every upload, unique in the process: graphs that captured other buffers are stale
 
   ~Numeric() { release(); }
   void release();
@@ -77,6 +82,9 @@ struct Numeric {
   // (H + damping) dx = -g at the buffers `in` (parity `par` picks the captured graphs): *failed = a non-positive or non-finite
   // pivot.  Synchronises the stream.
   int step(cudaStream_t st, int par, const Lin &in, double lambda, bool *failed, std::string &err);
+  // the same factorisation and solve with the damping of lm, enqueued on `st` (not launched, not synchronised: for capture
+  // into the minimiser's graph); the pivot flag is left in d_fail
+  int enqueue_lm(cudaStream_t st, const Lin &in, const LmDamping &lm, std::string &err);
   // copies of the last step's assembled system by pose index (has_system): diag[n_pose][D*D] (lower triangle as factored,
   // mirrored; 0 on fixed poses), b[n_pose][D] (0 on fixed poses), the first max_pairs pairs' pose indices pair_ab[][2] (lo, hi)
   // and blocks pair_H[][D*D] (sum J_lo^T J_hi).  Synchronises the stream.

@@ -33,6 +33,17 @@ template <int W> using ArockDuals = std::map<std::pair<int32_t, int64_t>, ArockD
 struct ArockMsg { int32_t sender, target; std::vector<int64_t> frames; std::vector<double> duals; };
 template <int W> struct ArockTable { ArockDuals<W> duals; std::vector<ArockMsg> inbox; };
 
+// the ceres minimiser's device state (d2pgo_set_minimizer): its config and its trust region, written by the one-thread control
+// kernels of d2pgo.cu only
+struct LmState {
+  double radius, min_diag, max_diag;   // in this order: the Cholesky's damping reads them (d2pgo_chol::LmDamping::par)
+  double radius0, max_radius, min_radius, min_rel_dec, ftol, gtol, ptol, budget_s;
+  int max_iter, max_invalid, jacobi, trace_cap;
+  double decrease_factor, cost, cost0, x_norm, model, step_norm;
+  unsigned long long t0, t_end;        // %globaltimer at the first device work and at the last decision
+  int iter, ok, bad, invalid_run, pivot_fail, pending_grad, done, type, reason, cand;
+};
+
 struct PcmBufs;                                               // d2pgo_pcm.cu
 struct PcmBufsFree { void operator()(PcmBufs *p) const; };    // defined beside PcmBufs
 struct PcmStream;                                             // d2pgo_pcm.cu
@@ -78,8 +89,16 @@ struct d2pgo_handle {
   std::unique_ptr<d2pgo_handle> rot;  // the row systems (dof 3) of both rotation initialisations, kept between calls for their buffers
   int linear_solver = D2PGO_LINEAR_PCG;   // d2pgo_set_linear_solver
   std::unique_ptr<d2pgo_chol::Numeric> chol;   // the sparse Cholesky's analysis and device state (d2pgo_chol.cu)
+  // d2pgo_set_minimizer: the kind and ceres LM's config; its device state, Jacobi scale, per-block partials and trace; the
+  // graph of one whole solve and the bytes it was built from; the last solve's report (lm_ran: that solve was ceres LM)
+  int minimizer = D2PGO_MINIMIZER_RESTATED; d2pgo_ceres_lm_config lm_cfg = {};
+  Buf<d2pgo_host::LmState> d_lm; Buf<double> d_lm_scale, d_lm_part; Buf<d2pgo_minimizer_iteration> d_lm_trace;
+  cudaGraphExec_t lm_graph = nullptr; std::string lm_key;
+  bool lm_ran = false; d2pgo_minimizer_summary lm_report = {}; int lm_trace_n = 0;
+  int driver_version = 0;
 
   ~d2pgo_handle() {   // the device buffers free themselves
+    if (lm_graph) cudaGraphExecDestroy(lm_graph);
     for (auto &pair : cg_graph) for (cudaGraphExec_t g : pair) if (g) cudaGraphExecDestroy(g);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);

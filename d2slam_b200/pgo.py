@@ -28,7 +28,12 @@ convergence gate, before arock_run.
 Linear solver (the reference's ceres linear_solver_type): `PgoSolver(linear_solver="sparse_cholesky")` takes exact LM steps
 from a GPU supernodal sparse Cholesky (d2pgo's SPARSE_NORMAL_CHOLESKY; include/d2pgo.h d2pgo_set_linear_solver) instead of the
 default truncated block-Jacobi PCG ("pcg"); cholesky_stats() reports the factor's structure and timings, cholesky_symbolic() runs
-the host analysis alone."""
+the host analysis alone.
+
+Minimiser (the reference's ceres minimizer_type and time budget): `PgoSolver.set_minimizer("ceres_lm", **cfg)` on a
+sparse-Cholesky handle solves with ceres' Levenberg-Marquardt trust region as d2pgo runs it (include/d2pgo.h
+d2pgo_set_minimizer; cfg overrides CeresLmConfig fields, e.g. max_solver_time_in_seconds), decided on the device in one graph
+launch; minimizer_report() and debug_minimizer_trace() report the last solve.  "restated" is the default LM loop."""
 import ctypes as C
 
 import numpy as np
@@ -80,6 +85,39 @@ class CholeskyInfo(C.Structure):
 LINEAR_SOLVERS = {"pcg": 0, "sparse_cholesky": 1}
 
 
+class CeresLmConfig(C.Structure):
+    _fields_ = [("max_num_iterations", C.c_int32), ("max_num_consecutive_invalid_steps", C.c_int32), ("jacobi_scaling", C.c_int32),
+                ("pad_", C.c_int32), ("max_solver_time_in_seconds", C.c_double), ("initial_trust_region_radius", C.c_double),
+                ("max_trust_region_radius", C.c_double), ("min_trust_region_radius", C.c_double), ("min_relative_decrease", C.c_double),
+                ("min_lm_diagonal", C.c_double), ("max_lm_diagonal", C.c_double), ("function_tolerance", C.c_double),
+                ("gradient_tolerance", C.c_double), ("parameter_tolerance", C.c_double)]
+
+
+class MinimizerSummary(C.Structure):
+    _fields_ = [("termination_type", C.c_int32), ("reason", C.c_int32), ("successful_steps", C.c_int32), ("unsuccessful_steps", C.c_int32),
+                ("host_syncs", C.c_int32), ("pad_", C.c_int32), ("final_radius", C.c_double), ("elapsed_s", C.c_double),
+                ("initial_cost", C.c_double), ("final_cost", C.c_double)]
+
+
+class MinimizerIteration(C.Structure):
+    _fields_ = [("cost", C.c_double), ("candidate_cost", C.c_double), ("model_cost_change", C.c_double), ("relative_decrease", C.c_double),
+                ("step_norm", C.c_double), ("radius", C.c_double), ("decrease_factor", C.c_double), ("kind", C.c_int32), ("pad_", C.c_int32)]
+
+
+MINIMIZERS = {"restated": 0, "ceres_lm": 1}
+TERMINATIONS = {0: "CONVERGENCE", 1: "NO_CONVERGENCE", 2: "FAILURE"}
+STOP_REASONS = {1: "gradient", 2: "parameter", 3: "function", 4: "min_radius", 5: "max_iterations", 6: "time", 7: "invalid_steps"}
+STEP_KINDS = {0: "accepted", 1: "rejected", 2: "invalid", 3: "converged"}
+TRACE_CAP = 16384   # trace records the library keeps per solve
+
+
+def default_ceres_lm_config():
+    """ceres' defaults as the library states them (d2pgo_default_ceres_lm_config), as a dict."""
+    c = CeresLmConfig()
+    _lib().d2pgo_default_ceres_lm_config(C.byref(c))
+    return {k: getattr(c, k) for k, _ in CeresLmConfig._fields_ if k != "pad_"}
+
+
 def _info_dict(r):
     return {k: getattr(r, k) for k, _ in CholeskyInfo._fields_}
 
@@ -118,7 +156,8 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_debug_exact_step", "d2pgo_cholesky_symbolic", "d2pgo_debug_cholesky_system", "d2pgo_debug_pcg_step",
                 "d2pgo_default_arock_rot_init_config", "d2pgo_arock_rot_init_step", "d2pgo_arock_rot_receive",
                 "d2pgo_arock_rot_neighbours", "d2pgo_arock_rot_duals", "d2pgo_debug_arock_rot_state", "d2pgo_pcm_stream_reset",
-                "d2pgo_pcm_stream", "d2pgo_debug_pcm_stream_smd", "d2pgo_debug_pcm_clique_inc"]
+                "d2pgo_pcm_stream", "d2pgo_debug_pcm_stream_smd", "d2pgo_debug_pcm_clique_inc",
+                "d2pgo_default_ceres_lm_config", "d2pgo_set_minimizer", "d2pgo_minimizer_report", "d2pgo_debug_minimizer_trace"]
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -186,6 +225,40 @@ class PgoSolver:
         ab = np.zeros((max(P, 1), 2), np.int32); H = np.zeros((max(P, 1), D, D)); n = C.c_int32()
         self._chk(_lib().d2pgo_debug_cholesky_system(self.h, _p(diag), _p(b), C.c_int32(P), C.byref(n), _p(ab), _p(H)), "debug_cholesky_system")
         return dict(diag=diag, b=b, pairs=ab[: n.value], pair_blocks=H[: n.value])
+
+    def set_minimizer(self, kind, **cfg):
+        """"restated" (the default LM loop) or "ceres_lm" (include/d2pgo.h d2pgo_set_minimizer): cfg overrides CeresLmConfig
+        fields of ceres' defaults; ints pass through."""
+        k = MINIMIZERS.get(kind, kind) if isinstance(kind, str) else int(kind)
+        if isinstance(k, str):
+            raise ValueError(f"unknown minimizer {kind!r}: {sorted(MINIMIZERS)}")
+        c = CeresLmConfig()
+        _lib().d2pgo_default_ceres_lm_config(C.byref(c))
+        for name, v in cfg.items():
+            if name not in dict(CeresLmConfig._fields_):
+                raise KeyError(name)
+            setattr(c, name, v)
+        self._chk(_lib().d2pgo_set_minimizer(self.h, C.c_int32(k), C.byref(c)), "set_minimizer")
+
+    def minimizer_report(self):
+        """The ceres minimiser's report of the last solve or ARock step, as a dict (termination and reason as names)."""
+        r = MinimizerSummary()
+        self._chk(_lib().d2pgo_minimizer_report(self.h, C.byref(r)), "minimizer_report")
+        out = {k: getattr(r, k) for k, _ in MinimizerSummary._fields_ if k != "pad_"}
+        out["termination"] = TERMINATIONS.get(r.termination_type, r.termination_type)
+        out["stop"] = STOP_REASONS.get(r.reason, r.reason)
+        return out
+
+    def debug_minimizer_trace(self):
+        """Per iteration of the last ceres solve: dict of arrays cost, candidate_cost, model_cost_change, relative_decrease,
+        step_norm, radius, decrease_factor (after the update) and kind (0 accepted, 1 rejected, 2 invalid, 3 converged)."""
+        rep = self.minimizer_report()
+        n_max = min(rep["successful_steps"] + rep["unsuccessful_steps"], TRACE_CAP)
+        buf = (MinimizerIteration * max(n_max, 1))()
+        n = C.c_int32()
+        self._chk(_lib().d2pgo_debug_minimizer_trace(self.h, C.c_int32(n_max), C.byref(n), buf), "debug_minimizer_trace")
+        names = [k for k, _ in MinimizerIteration._fields_ if k != "pad_"]
+        return {k: np.array([getattr(buf[i], k) for i in range(n.value)], np.int32 if k == "kind" else np.float64) for k in names}
 
     def _chk(self, rc, what):
         if rc:

@@ -433,6 +433,96 @@ int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out
 int d2pgo_cholesky_symbolic(int32_t n, const uint8_t *fixed, int32_t n_edges, const int32_t *ea, const int32_t *eb, int32_t dof,
                             int32_t *perm_out, int32_t *sn_ptr_out, int32_t *sn_parent_out, d2pgo_cholesky_info *info);
 
+/* ---- minimiser of d2pgo_solve and of d2pgo_arock_step's local solve
+ *   D2PGO_MINIMIZER_RESTATED  the default: the LM loop above (lambda / 3 on accept, x 4 on reject, one relative-decrease test,
+ *                             no time budget; the host reads the cost after every linearisation).  The only kind for PCG and
+ *                             for a handle with a communicator.
+ *   D2PGO_MINIMIZER_CERES_LM  <- ceres 2.1's TrustRegionMinimizer + LevenbergMarquardtStrategy, as every shipped d2pgo
+ *                             configuration runs it: SPARSE_NORMAL_CHOLESKY + LEVENBERG_MARQUARDT with max_solver_time_in_seconds
+ *                             = pgo_solver_time (d2pgo/src/d2pgo_node.cpp:190-197; 0.5 or 1.0 s in config/quadcam/*.yaml; the
+ *                             test driver d2pgo/test/d2pgo_test.cpp:95-103 uses 0.1 s and 50 iterations), and the ARock local
+ *                             solves the same (ARock.cpp:317, d2pgo_node.cpp:202).  With s_k = 1 / (1 + |J_:,k|) from the
+ *                             first linearisation (1 without jacobi_scaling), each iteration solves
+ *                               (J^T J + diag(mu)) dx = -g,  mu_k = clamp(s_k^2 H_kk, min_lm_diagonal, max_lm_diagonal) / (radius s_k^2)
+ *                             over the free poses with the sparse Cholesky (H_kk from the block diagonal; a self loop's cross
+ *                             terms are in J^T J, not in H_kk), model m = -(r.J dx + |J dx|^2 / 2), rho = (C - C+) / m; accept
+ *                             if rho > min_relative_decrease: radius = min(radius / max(1/3, 1 - (2 rho - 1)^3), max radius),
+ *                             decrease factor 2; else radius /= decrease factor, decrease factor *= 2.  A non-positive or
+ *                             non-finite pivot, m <= 0 or a non-finite step is an invalid step (rejected; FAILURE after more
+ *                             than max_num_consecutive_invalid_steps in a row).  Stops, in this order: gradient (max over the
+ *                             free poses' ambient components of |x - x [+] (-g)| <= gradient_tolerance, at the start and after
+ *                             every accepted step), iterations (the count of accepted and rejected steps reaches
+ *                             max_num_iterations), time (max_solver_time_in_seconds > 0 reached on the device's %globaltimer,
+ *                             measured from the solve's first device work, not from the call), parameter (|dx| <=
+ *                             parameter_tolerance (|x| + parameter_tolerance), |x| over the free poses' ambient components),
+ *                             function (|C - C+| <= function_tolerance C), min radius (radius < min_trust_region_radius after a
+ *                             rejection).  A parameter or function stop returns x, not the candidate; that last iteration counts
+ *                             as unsuccessful.  ASSUMED (restated from upstream ceres, which is not in the reference tree): the
+ *                             Jacobi scale computed once at x0, the gradient test's ambient form, FAILURE after more than 5
+ *                             invalid steps, m <= 0 invalid, the parameter and function tests returning x and their order
+ *                             (parameter, function, acceptance).  Edges, gravity priors and ARock proximal terms enter as in
+ *                             the restated loop.  Needs D2PGO_LINEAR_SPARSE_CHOLESKY and no communicator: otherwise d2pgo_solve
+ *                             and d2pgo_arock_step return 5 and do nothing.  The whole solve is one CUDA graph (the iterations
+ *                             under a conditional WHILE node, one-thread control kernels deciding on the device) and one host
+ *                             synchronisation; it needs a driver for CUDA 12.4 or newer (3 otherwise).
+ * d2pgo_report of such a solve: iterations = successful + unsuccessful steps, accepted = successful, converged = (termination
+ * type CONVERGENCE), pcg_iterations 0, the costs and device_ms (SolverWrapper.cpp:38-49's mapping of ceres' summary).  The
+ * Cholesky counters of d2pgo_cholesky_stats count one factorisation per iteration and no device times. */
+enum { D2PGO_MINIMIZER_RESTATED = 0, D2PGO_MINIMIZER_CERES_LM = 1 };
+enum { D2PGO_TERMINATION_CONVERGENCE = 0, D2PGO_TERMINATION_NO_CONVERGENCE = 1, D2PGO_TERMINATION_FAILURE = 2 };
+enum { D2PGO_STOP_GRADIENT = 1, D2PGO_STOP_PARAMETER = 2, D2PGO_STOP_FUNCTION = 3, D2PGO_STOP_MIN_RADIUS = 4,
+       D2PGO_STOP_MAX_ITERATIONS = 5, D2PGO_STOP_TIME = 6, D2PGO_STOP_INVALID_STEPS = 7 };
+enum { D2PGO_STEP_ACCEPTED = 0, D2PGO_STEP_REJECTED = 1, D2PGO_STEP_INVALID = 2, D2PGO_STEP_CONVERGED = 3 };
+
+typedef struct d2pgo_ceres_lm_config {   /* ceres::Solver::Options fields; defaults are ceres' */
+  int32_t max_num_iterations;            /* 50                                                      */
+  int32_t max_num_consecutive_invalid_steps;   /* 5                                                 */
+  int32_t jacobi_scaling;                /* 1 (0 or 1)                                              */
+  int32_t pad_;
+  double max_solver_time_in_seconds;     /* 0 = no budget                                           */
+  double initial_trust_region_radius;    /* 1e4                                                     */
+  double max_trust_region_radius;        /* 1e16                                                    */
+  double min_trust_region_radius;        /* 1e-32                                                   */
+  double min_relative_decrease;          /* 1e-3                                                    */
+  double min_lm_diagonal, max_lm_diagonal;   /* 1e-6, 1e32                                          */
+  double function_tolerance;             /* 1e-6                                                    */
+  double gradient_tolerance;             /* 1e-10                                                   */
+  double parameter_tolerance;            /* 1e-8                                                    */
+} d2pgo_ceres_lm_config;
+
+typedef struct d2pgo_minimizer_summary {   /* the last ceres-LM solve or ARock step                   */
+  int32_t termination_type;              /* D2PGO_TERMINATION_*                                     */
+  int32_t reason;                        /* D2PGO_STOP_*                                            */
+  int32_t successful_steps, unsuccessful_steps;
+  int32_t host_syncs;                    /* stream synchronisations of the call: 1, plus 1 for uploading a graph changed
+                                            since the last solve and 1 for the Cholesky's first upload of a structure    */
+  int32_t pad_;
+  double final_radius;
+  double elapsed_s;                      /* device seconds on %globaltimer, first device work to the last decision        */
+  double initial_cost, final_cost;
+} d2pgo_minimizer_summary;
+
+typedef struct d2pgo_minimizer_iteration {   /* one iteration of the trace                               */
+  double cost, candidate_cost;           /* C at x, C+ (NaN when no candidate was evaluated)        */
+  double model_cost_change;              /* m                                                       */
+  double relative_decrease;              /* rho (NaN when no candidate was evaluated)               */
+  double step_norm;                      /* |dx|                                                    */
+  double radius, decrease_factor;        /* after the iteration's update                            */
+  int32_t kind;                          /* D2PGO_STEP_*                                            */
+  int32_t pad_;
+} d2pgo_minimizer_iteration;
+
+int d2pgo_default_ceres_lm_config(d2pgo_ceres_lm_config *cfg);
+/* kind D2PGO_MINIMIZER_RESTATED (cfg ignored) or D2PGO_MINIMIZER_CERES_LM (cfg NULL = the defaults).  Returns 2 on an unknown
+ * kind or a config field that is non-finite, negative or inconsistent (min radius <= initial radius <= max radius, radii > 0,
+ * 0 < min_lm_diagonal <= max_lm_diagonal, jacobi_scaling 0 or 1); a refusal keeps nothing.  It may change between solves. */
+int d2pgo_set_minimizer(d2pgo_handle *h, int32_t kind, const d2pgo_ceres_lm_config *cfg);
+/* the report of the last d2pgo_solve / d2pgo_arock_step; 5 when that call did not run the ceres minimiser */
+int d2pgo_minimizer_report(d2pgo_handle *h, d2pgo_minimizer_summary *out);
+/* parity hook: the per-iteration records of that call (the first 16384 iterations), copied from the device.  *n_out = the
+ * records held; returns 2 (with *n_out set) when max < *n_out, 5 as d2pgo_minimizer_report does */
+int d2pgo_debug_minimizer_trace(d2pgo_handle *h, int32_t max, int32_t *n_out, d2pgo_minimizer_iteration *out);
+
 #ifdef __cplusplus
 }
 #endif
