@@ -256,6 +256,7 @@ struct d2ba_handle {
   bool no_sb_elim = false;       // D2BA_NO_SB_ELIM=1: keep the dense Cholesky of the whole reduced system (A/B switch for tests / profiling)
   bool rec128 = false;           // D2BA_REC128=1: 128-byte records and k_lm_gather16 in every window that would use 96-byte ones (A/B switch)
   bool no_fused_solve = false;   // D2BA_NO_FUSED_SOLVE=1: the separate Schur / Cholesky / back-substitution / step kernels everywhere (A/B switch)
+  unsigned long long *solve_ts = nullptr;   // d2ba_debug_solve_phases: k_solve_small's phase timestamps of this iteration
   double host_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // wall-clock phases of the last d2ba_finalize (d2ba_debug_host_times)
   double solve_ms[4] = {0, 0, 0, 0};             // host wall-clock of the last solve: enqueue, wait for the device, write-back
   std::atomic<long long> h2d_bytes_add;          // bytes d2ba_add_proj put on the copy stream since the last reset
@@ -1497,7 +1498,8 @@ static int upload_state(d2ba_handle *h) {
 }
 
 // Points of the iteration sequence at which d2ba_debug_kernel_times records an event, in enqueue order.
-enum IterMark { kMkGather, kMkSbElim, kMkSchur, kMkLeafElimEnd, kMkChol, kMkSbBack, kMkLeafBack, kMkStep, kMkLin, kMkProj, kMkControl, kMkEnd, kNumMarks };
+enum IterMark { kMkGather, kMkSbElim, kMkSchur, kMkLeafElimEnd, kMkChol, kMkSbBack, kMkLeafBack, kMkStep, kMkSolveSmallEnd, kMkLin, kMkProj, kMkControl, kMkEnd,
+                kNumMarks };
 // `ev` (nullptr outside d2ba_debug_kernel_times): one event per IterMark, recorded on the solver stream, and one lane only
 static void iter_mark(d2ba_handle *h, cudaEvent_t *ev, IterMark m) { if (ev) cudaEventRecord(ev[m], h->stream); }
 
@@ -1531,9 +1533,9 @@ static void enqueue_solve_reduced(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
   iter_mark(h, ev, kMkLeafBack); launch_leaf_back(h->dev, h->ls, h->stream);
 }
 // the step: k_solve_small does the whole reduced-system solve and the step of its windows, k_step the others'
-static void enqueue_step(d2ba_handle *h) {
-  launch_solve_small(h->dev, h->ls, h->stream);
-  launch_step(h->dev, h->ls, h->stream);
+static void enqueue_step(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
+  launch_solve_small(h->dev, h->ls, h->solve_ts, h->stream);
+  iter_mark(h, ev, kMkSolveSmallEnd); launch_step(h->dev, h->ls, h->stream);
 }
 
 static void enqueue_iteration(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
@@ -1546,7 +1548,7 @@ static void enqueue_iteration(d2ba_handle *h, cudaEvent_t *ev = nullptr) {
   else launch_sb_elim(h->dev, h->ls, h->stream);   // Y rows into Wt: the Schur kernels subtract them too
   iter_mark(h, ev, kMkSchur); enqueue_schur(h, ev);
   iter_mark(h, ev, kMkChol); enqueue_solve_reduced(h, ev);
-  iter_mark(h, ev, kMkStep); enqueue_step(h);
+  iter_mark(h, ev, kMkStep); enqueue_step(h, ev);
   iter_mark(h, ev, kMkLin); enqueue_linearize(h, 0, ev);
   iter_mark(h, ev, kMkControl); launch_control(h->dev, 0, h->stream);
   iter_mark(h, ev, kMkEnd);
@@ -2070,8 +2072,8 @@ int d2ba_debug_solve_occupancy(d2ba_handle *h, int32_t *ctas_per_sm) {
 // chol bucket.  Used by bench.py for the roofline of the dominant kernel.  k_solve_small (the whole reduced-system
 // solve and step of the windows with fused_solve) is timed in the step bucket; the schur, chol and back-substitution
 // buckets then hold only the other windows' kernels.
-int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
-  if (!h) return 1;
+// The fixed-iteration solve of the timed debug entries up to its first iteration: linearised at the uploaded state.
+static int begin_timed_iterations(d2ba_handle *h, int iters) {
   cudaSetDevice(h->cfg.device);
   if (!h->finalized) { int rc = d2ba_finalize(h); if (rc) return rc; }
   if (h->state_dirty) { int rc = upload_state(h); if (rc) return rc; }
@@ -2082,6 +2084,12 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
   if (h->ls.any_admm) { int rc = consensus_exchange(h); if (rc) return rc; }
   enqueue_linearize(h, 1);
   launch_control(h->dev, 1, h->stream);
+  return 0;
+}
+
+int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
+  if (!h) return 1;
+  { int rc = begin_timed_iterations(h, iters); if (rc) return rc; }
   cudaEvent_t ev[kNumMarks];
   for (cudaEvent_t &e : ev) cudaEventCreate(&e);
   // ms_out[i] sums the span between two marks ([7] is the iteration count)
@@ -2096,6 +2104,33 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out) {
   }
   ms_out[7] = iters;
   for (cudaEvent_t e : ev) cudaEventDestroy(e);
+  CK(cudaGetLastError());
+  h->state_dirty = true;
+  return 0;
+}
+
+// Phase timestamps of k_solve_small over `iters` fixed iterations (the timestamped instantiation in place of the plain one).
+int d2ba_debug_solve_phases(d2ba_handle *h, int32_t iters, int64_t *ts_out, double *ms_out) {
+  if (!h || iters < 1 || !ts_out || !ms_out) return 1;
+  if (!h->finalized) return fail(h, 1, "solve_phases: the handle must be finalized (ts_out is sized by its window count)");
+  { int rc = begin_timed_iterations(h, iters); if (rc) return rc; }
+  const size_t per = (size_t)5 * h->dev.n_win;
+  DBuf<unsigned long long> d_ts;
+  CK(d_ts.alloc(per * iters));
+  cudaError_t ce = cudaMemsetAsync(d_ts.p, 0, per * iters * 8, h->stream);
+  cudaEvent_t ev[kNumMarks];
+  for (cudaEvent_t &e : ev) cudaEventCreate(&e);
+  for (int it = 0; it < iters && ce == cudaSuccess; it++) {
+    h->solve_ts = d_ts.p + per * it;
+    enqueue_iteration(h, ev);
+    h->solve_ts = nullptr;
+    ce = cudaStreamSynchronize(h->stream);
+    float ms = 0; cudaEventElapsedTime(&ms, ev[kMkStep], ev[kMkSolveSmallEnd]); ms_out[it] = ms;
+  }
+  for (cudaEvent_t e : ev) cudaEventDestroy(e);
+  if (ce == cudaSuccess) ce = cudaMemcpy(ts_out, d_ts.p, per * iters * 8, cudaMemcpyDeviceToHost);
+  d_ts.release();
+  CK(ce);
   CK(cudaGetLastError());
   h->state_dirty = true;
   return 0;

@@ -2143,10 +2143,12 @@ __global__ void __launch_bounds__(kSeThreads, 4) k_sb_elim(Dev d) {
 }
 
 // Speed-bias part of the Gauss-Newton step: L_kk^T x_k = z_k - Y_k x_p - E'_k^T x_{k+1}, blocks from the last to the
-// first.  One CTA per window: all warps form v = Y x_p (coalesced, many loads in flight) and stage the small blocks,
+// first.  One CTA per window: all warps form v = Y x_p (coalesced, 3 RW loads per lane in flight) and stage the small blocks,
 // warp 0 then runs the short recursion out of shared memory.
 constexpr int kSbBackThreads = 256;
-// Body shared by k_sb_back and k_solve_small (gn_c holds the pose part of the step).
+// Body shared by k_sb_back and k_solve_small (gn_c holds the pose part of the step).  RW: rows of Y per warp at a time
+// (8 in k_solve_small, whose other phases set the register budget; 4 in k_sb_back, which keeps its occupancy).
+template <int RW>
 D2BA_DEV void sb_back_body(const Dev &d, int wi, double *sm) {
   const WinDesc &w = d.win[wi];
   const int c0 = w.hub0, nh = w.n_lc - c0, nlc = w.n_lc, nb = w.n_sbe, ldy = w.ldw;   // Y lives in the hub columns [hub0, n_lc] of its rows
@@ -2159,18 +2161,39 @@ D2BA_DEV void sb_back_body(const Dev &d, int wi, double *sm) {
   for (int c = tid; c < nh; c += nt) xp[c] = -gn[c0 + c];
   for (int e = tid; e < nb * 171; e += nt) cp_async8(LE + e, LEg + e);   // needed only by the recursion: lands during the products
   __syncthreads();
-  for (int r0 = warp * 4; r0 < 9 * nb; r0 += nwarp * 4) {
-    double s_[4] = {0.0, 0.0, 0.0, 0.0};
+  // v = Y x_p, RW rows per warp at a time: every load of the RW rows (3 column chunks of 32 per step of 96 columns) and
+  // their z entries (column n_lc, lanes 0..RW-1) is issued before the first product, so a warp waits for one round trip per
+  // step, not one per row and chunk.  Each row's sum runs over its columns in ascending order per lane, as one row at a
+  // time would.
+  const int nrow = 9 * nb;
+  for (int r0 = warp * RW; r0 < nrow; r0 += nwarp * RW) {
+    const double z = (lane < RW && r0 + lane < nrow) ? Yg[(size_t)(r0 + lane) * ldy + nlc] : 0.0;
+    double s_[RW];
 #pragma unroll
-    for (int q = 0; q < 4; q++) {
-      if (r0 + q >= 9 * nb) break;
-      const double *yr = Yg + (size_t)(r0 + q) * ldy + c0;
-      for (int c = lane; c < nh; c += 32) s_[q] += yr[c] * xp[c];
+    for (int q = 0; q < RW; q++) s_[q] = 0.0;
+    for (int cb = 0; cb < nh; cb += 96) {
+      double v[3][RW];
+#pragma unroll
+      for (int u = 0; u < 3; u++)
+#pragma unroll
+        for (int q = 0; q < RW; q++) {
+          const int c = cb + lane + 32 * u;
+          v[u][q] = (c < nh && r0 + q < nrow) ? Yg[(size_t)(r0 + q) * ldy + c0 + c] : 0.0;
+        }
+#pragma unroll
+      for (int u = 0; u < 3; u++) {
+        const int c = cb + lane + 32 * u;
+        if (c < nh) {
+          const double x = xp[c];
+#pragma unroll
+          for (int q = 0; q < RW; q++) if (r0 + q < nrow) s_[q] += v[u][q] * x;
+        }
+      }
     }
 #pragma unroll
-    for (int q = 0; q < 4; q++) {
-      const double t = warp_sum(s_[q]);
-      if (lane == 0 && r0 + q < 9 * nb) rhs[r0 + q] = Yg[(size_t)(r0 + q) * ldy + nlc] - t;
+    for (int q = 0; q < RW; q++) {
+      const double t = warp_sum(s_[q]);   // (the same in every lane)
+      if (lane == q && r0 + q < nrow) rhs[r0 + q] = z - t;
     }
   }
   cp_async_wait_all();
@@ -2213,7 +2236,7 @@ __global__ void __launch_bounds__(kSbBackThreads) k_sb_back(Dev d) {
   const Ctl *ctl = d.ctl + wi;
   if (ctl->done || ctl->reuse || ctl->chol_fail) return;
   extern __shared__ double sm[];
-  sb_back_body(d, wi, sm);
+  sb_back_body<4>(d, wi, sm);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2455,8 +2478,10 @@ __global__ void k_zero_leaf_rows(Dev d) {
 // ------------------------------------------------------------------------------------------------
 // Step kernel: one CTA per window.
 constexpr int kStepThreads = 256;
-// Body shared by k_step and k_solve_small; sm holds 40 + 3 max_nc doubles.
-template <bool LEAF>   // LEAF: windows with leaves (block-sparse landmark rows); the other instantiation handles the dense rows
+// Body shared by k_step and k_solve_small; sm holds 40 + 3 max_nc doubles.  PIPE (dense rows): the next step's rows are
+// loaded before this step's warp sums (k_solve_small); without it (k_step: 3 CTAs of 256 threads per SM leave 80
+// registers) each half of a step's rows is loaded right before its products.
+template <bool LEAF, bool PIPE = false>   // LEAF: windows with leaves (block-sparse landmark rows); the other instantiation handles the dense rows
 D2BA_DEV void step_body(const Dev &d, int wi, double *sm, int max_nc) {
   const WinDesc &w = d.win[wi];
   Ctl *ctl = d.ctl + wi;
@@ -2482,58 +2507,93 @@ D2BA_DEV void step_body(const Dev &d, int wi, double *sm, int max_nc) {
     if (ctl->chol_fail) { if (tid == 0) ctl->step_valid = 0; return; }
     // landmark back-substitution and the landmark part of the Cauchy / dogleg dot products
     const double *Wt = d.Wt + w.offW;
+    const int ldw = w.ldw;
     double s_gg = 0, s_uHu = 0, s_nn = 0, s_gdn = 0;
-    for (int l0 = warp * 8; l0 < nl; l0 += nw * 8) {
+    // per-landmark scalars of the batch l0 .. l0 + 7 on lanes 0..7: 1 / Hll, g~ (column n_lc of the row), Hll, g_l, D_l^2, w.u
+    double di = 0, gt = 0, hq = 0, gq = 0, dq = 0, wq = 0;
+    auto load_scalars = [&](int l0) {
+      const int l = l0 + lane;
+      if (lane < 8 && l < nl) { di = dinv[l]; gt = Wt[(size_t)l * ldw + nlc]; hq = hl[l]; gq = glv[l]; dq = D2l[l]; wq = wuv[l]; }
+    };
+    // the warp sums of the batch's 8 row products, then the landmark step and its share of the dot products on lanes 0..7
+    auto finish = [&](int l0, double (&a)[8]) {
+#pragma unroll
+      for (int q = 0; q < 8; q++) a[q] = warp_sum(a[q]);
+      if (LEAF) load_scalars(l0);
+      if (lane < 8 && l0 + lane < nl) {
+        const int l = l0 + lane;
+        double aq = a[0];
+#pragma unroll
+        for (int q = 1; q < 8; q++) if (lane == q) aq = a[q];
+        const double gnl = -di * (gt + aq);
+        gn_l[l] = gnl;
+        const double ul = gq / dq;
+        s_gg += gq * ul;
+        s_uHu += 2.0 * ul * wq + hq * ul * ul;
+        s_nn += gnl * gnl * dq;
+        s_gdn += gq * gnl;
+      }
+    };
+    if (!LEAF) {
+      // dense rows (single-drone window), in steps of 8 rows x 3 column chunks of 32.  One load round trip per step: a
+      // batch's scalars go out with its first rows, and with PIPE the next step's rows are requested before this step's
+      // warp sums and scalar work.  Every row product is formed in the same order either way.
+      double v[3][8];
+      auto load_rows = [&](int l0, int cb, int q0, int q1) {
+#pragma unroll
+        for (int u = 0; u < 3; u++)
+#pragma unroll
+          for (int q = q0; q < q1; q++) {
+            const int c = cb + lane + 32 * u;
+            v[u][q] = (c < nlc && l0 + q < nl) ? Wt[(size_t)(l0 + q) * ldw + c] : 0.0;
+          }
+      };
+      int l0 = warp * 8, cb = 0;   // the step v holds: rows l0.., columns cb + lane + 32 u
+      if (l0 < nl) { if (PIPE) load_rows(l0, cb, 0, 8); load_scalars(l0); }
       double a[8];
 #pragma unroll
       for (int q = 0; q < 8; q++) a[q] = 0.0;
-      if (!LEAF) {
-        // dense rows (single-drone window): 4 rows x 3 column chunks = 12 independent loads in flight before the first use
-        for (int c0 = lane; c0 < nlc; c0 += 96) {
+      while (l0 < nl) {
+        if (cb + lane < nlc) {   // (a lane past the last column chunk adds nothing)
           double dc[3];
 #pragma unroll
-          for (int u = 0; u < 3; u++) dc[u] = c0 + 32 * u < nlc ? dcs[c0 + 32 * u] : 0.0;
+          for (int u = 0; u < 3; u++) dc[u] = cb + lane + 32 * u < nlc ? dcs[cb + lane + 32 * u] : 0.0;
 #pragma unroll
           for (int qh = 0; qh < 8; qh += 4) {
-            const double *r0 = Wt + (size_t)(l0 + qh) * w.ldw;
-            double v[3][4];
+            if (!PIPE) load_rows(l0, cb, qh, qh + 4);
 #pragma unroll
             for (int u = 0; u < 3; u++)
 #pragma unroll
-              for (int q = 0; q < 4; q++) v[u][q] = (c0 + 32 * u < nlc && l0 + qh + q < nl) ? r0[(size_t)q * w.ldw + c0 + 32 * u] : 0.0;
-#pragma unroll
-            for (int u = 0; u < 3; u++)
-#pragma unroll
-              for (int q = 0; q < 4; q++) a[qh + q] = fma(v[u][q], dc[u], a[qh + q]);
+              for (int q = 0; q < 4; q++) a[qh + q] = fma(v[u][qh + q], dc[u], a[qh + q]);
           }
         }
-      } else {
+        int l1 = l0, c1 = cb + 96;
+        if (c1 >= nlc) { l1 = l0 + nw * 8; c1 = 0; }
+        if (PIPE && l1 < nl) load_rows(l1, c1, 0, 8);
+        if (l1 != l0) {
+          finish(l0, a);
+#pragma unroll
+          for (int q = 0; q < 8; q++) a[q] = 0.0;
+          if (l1 < nl) load_scalars(l1);
+        }
+        l0 = l1; cb = c1;
+      }
+    } else {
+      for (int l0 = warp * 8; l0 < nl; l0 += nw * 8) {
+        double a[8];
+#pragma unroll
+        for (int q = 0; q < 8; q++) a[q] = 0.0;
 #pragma unroll
         for (int q = 0; q < 8; q++) {
           if (l0 + q < nl) {
-            const double *row = Wt + (size_t)(l0 + q) * w.ldw;
+            const double *row = Wt + (size_t)(l0 + q) * ldw;
             for (unsigned long long m = d.lm_mask[w.offlm + l0 + q]; m; m &= m - 1) {   // only the column tiles the row has entries in
               const int c = (__ffsll((long long)m) - 1) * 32 + lane;
               if (c < nlc) a[q] += row[c] * dcs[c];
             }
           }
         }
-      }
-#pragma unroll
-      for (int q = 0; q < 8; q++) a[q] = warp_sum(a[q]);
-      if (lane < 8 && l0 + lane < nl) {
-        const int l = l0 + lane;
-        double aq = a[0];
-#pragma unroll
-        for (int q = 1; q < 8; q++) if (lane == q) aq = a[q];
-        const double di = dinv[l], gt = Wt[(size_t)l * w.ldw + nlc];
-        const double gnl = -di * (gt + aq);
-        gn_l[l] = gnl;
-        const double h = hl[l], g = glv[l], dl2 = D2l[l], ul = g / dl2;
-        s_gg += g * ul;
-        s_uHu += 2.0 * ul * wuv[l] + h * ul * ul;
-        s_nn += gnl * gnl * dl2;
-        s_gdn += g * gnl;
+        finish(l0, a);
       }
     }
     for (int j = tid; j < n; j += nt) { s_nn += dcs[j] * dcs[j] * D2[j]; s_gdn += gcv[j] * dcs[j]; }
@@ -2639,7 +2699,10 @@ __global__ void __launch_bounds__(kStepThreads, LEAF ? 4 : 3) k_step(Dev d, int 
 //   (4) landmark back substitution, dogleg, model change, retraction into the candidate buffers.
 // A rejected step (reuse), a finished window and a failed speed-bias elimination skip (1)-(3), as the separate kernels do.
 // 4 warps and <= 56 KB of shared memory: 4 CTAs per SM, so the 528 windows of 132 SMs run in one wave.
-__global__ void __launch_bounds__(kSolveThreads, 4) k_solve_small(Dev d) {
+// TS (d2ba_debug_solve_phases only): thread 0 stores %globaltimer at the start of phases (1)-(4) and at the end into
+// ts[5 wi ..]; a skipped phase gets the start time of the next.
+template <bool TS>
+__global__ void __launch_bounds__(kSolveThreads, 4) k_solve_small(Dev d, unsigned long long *ts) {
   const int wi = blockIdx.x;
   const WinDesc &w = d.win[wi];
   if (!w.fused_solve) return;
@@ -2647,18 +2710,25 @@ __global__ void __launch_bounds__(kSolveThreads, 4) k_solve_small(Dev d) {
   if (ctl->done) return;
   extern __shared__ __align__(16) double sm[];
   __shared__ double red[40];
+  auto stamp = [&](int k) { if (TS && threadIdx.x == 0) ts[5 * wi + k] = globaltimer_ns(); };
+  stamp(0);
   if (!ctl->reuse && !ctl->chol_fail) {
     const double uhu = schur_small_body<kSolveThreads, kSolveMaxB>(d, wi, sm, red, sm, chol_smem_ld(w.n_lc));
     // k_sb_elim has added its share already and nothing else writes the window's uHu_cam now: a plain add
     if (threadIdx.x == 0) ctl->uHu_cam += uhu;
     __syncthreads();
-    if (!chol_smem_body(d, wi, sm, true)) {
+    stamp(1);
+    const bool fail = chol_smem_body(d, wi, sm, true);
+    stamp(2);
+    if (!fail) {
       __syncthreads();   // gn_c (pose part) and the shared memory of phase 2
-      sb_back_body(d, wi, sm);
+      sb_back_body<8>(d, wi, sm);
     }
     __syncthreads();
-  }
-  step_body<false>(d, wi, sm, w.n_c);
+  } else { stamp(1); stamp(2); }
+  stamp(3);
+  step_body<false, true>(d, wi, sm, w.n_c);
+  stamp(4);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3025,7 +3095,8 @@ const char *configure_launches(const LaunchSummary &L) {
   if (raise_smem_limit(k_leaf_elim, L.leaf_smem)) return "cudaFuncSetAttribute(k_leaf_elim) failed";
   if (raise_smem_limit(k_leaf_back, L.leafb_smem)) return "cudaFuncSetAttribute(k_leaf_back) failed";
   if (L.max_n_smem > 0 && raise_smem_limit(k_chol_smem, chol_smem_bytes(L.max_n_smem))) return "cudaFuncSetAttribute(k_chol_smem) failed";
-  if (raise_smem_limit(k_solve_small, L.fused_smem)) return "cudaFuncSetAttribute(k_solve_small) failed";
+  if (raise_smem_limit(k_solve_small<false>, L.fused_smem) || raise_smem_limit(k_solve_small<true>, L.fused_smem))
+    return "cudaFuncSetAttribute(k_solve_small) failed";
   return nullptr;
 }
 
@@ -3094,10 +3165,14 @@ void launch_sb_back(const Dev &d, const LaunchSummary &L, cudaStream_t s) { if (
 void launch_leaf_back(const Dev &d, const LaunchSummary &L, cudaStream_t s) {
   if (L.n_leaf_total > 0) k_leaf_back<<<L.n_leaf_total, kLeafBackThreads, L.leafb_smem, s>>>(d);
 }
-void launch_solve_small(const Dev &d, const LaunchSummary &L, cudaStream_t s) { if (L.n_fused > 0) k_solve_small<<<d.n_win, kSolveThreads, L.fused_smem, s>>>(d); }
+void launch_solve_small(const Dev &d, const LaunchSummary &L, unsigned long long *phase_ts, cudaStream_t s) {
+  if (L.n_fused == 0) return;
+  if (phase_ts) k_solve_small<true><<<d.n_win, kSolveThreads, L.fused_smem, s>>>(d, phase_ts);
+  else k_solve_small<false><<<d.n_win, kSolveThreads, L.fused_smem, s>>>(d, nullptr);
+}
 int solve_small_occupancy(size_t smem) {
   int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_solve_small, kSolveThreads, smem) != cudaSuccess) return -1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_solve_small<false>, kSolveThreads, smem) != cudaSuccess) return -1;
   return n;
 }
 void launch_step(const Dev &d, const LaunchSummary &L, cudaStream_t s) {

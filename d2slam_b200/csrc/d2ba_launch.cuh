@@ -100,7 +100,8 @@ void launch_chol_smem(const Dev &d, const LaunchSummary &L, cudaStream_t s);
 void launch_chol(const Dev &d, const LaunchSummary &L, cudaStream_t s);
 void launch_sb_back(const Dev &d, const LaunchSummary &L, cudaStream_t s);
 void launch_leaf_back(const Dev &d, const LaunchSummary &L, cudaStream_t s);
-void launch_solve_small(const Dev &d, const LaunchSummary &L, cudaStream_t s);
+// phase_ts: nullptr, or 5 timestamps per window (d2ba_debug_solve_phases: the timestamped instantiation)
+void launch_solve_small(const Dev &d, const LaunchSummary &L, unsigned long long *phase_ts, cudaStream_t s);
 int solve_small_occupancy(size_t smem);   // CTAs per SM, -1 if the query fails
 void launch_step(const Dev &d, const LaunchSummary &L, cudaStream_t s);
 void launch_control(const Dev &d, int init, cudaStream_t s);

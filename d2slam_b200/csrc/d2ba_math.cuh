@@ -166,6 +166,11 @@ D2BA_DEV void bulk_g2s(void *dst, const void *src, unsigned bytes, unsigned long
                "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+D2BA_DEV unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 D2BA_DEV void mbar_wait(unsigned long long *bar, unsigned parity) {
   unsigned ok;
   do {

@@ -50,7 +50,7 @@ EXPORTED = [
     "d2ba_set_consensus", "d2ba_comm_unique_id", "d2ba_comm_init", "d2ba_consensus_buffer", "d2ba_finalize",
     "d2ba_solve", "d2ba_solve_fixed", "d2ba_get_blocks", "d2ba_num_windows", "d2ba_marginalize",
     "d2ba_debug_linearize", "d2ba_debug_get", "d2ba_debug_kernel_times", "d2ba_debug_host_times",
-    "d2ba_debug_solve_occupancy",
+    "d2ba_debug_solve_occupancy", "d2ba_debug_solve_phases",
 ]
 
 
@@ -178,6 +178,15 @@ class Solver:
         n = C.c_int32()
         self._chk(lib().d2ba_debug_solve_occupancy(self.h, C.byref(n)), "solve_occupancy")
         return n.value
+
+    def solve_phases(self, iters):
+        """Phase timestamps of the one-kernel solve over ``iters`` fixed iterations from the uploaded state:
+        (ts [iters, windows, 5] int64 ns, launch_ms [iters]); see d2ba_debug_solve_phases in include/d2ba.h."""
+        n = self.num_windows()
+        ts = np.zeros((iters, n, 5), dtype=np.int64)
+        ms = np.zeros(iters)
+        self._chk(lib().d2ba_debug_solve_phases(self.h, C.c_int32(iters), abi.ptr(ts), abi.ptr(ms)), "solve_phases")
+        return ts, ms
 
     def kernel_times(self, iters):
         out = np.zeros(12)

@@ -317,6 +317,14 @@ int d2ba_debug_kernel_times(d2ba_handle *h, int32_t iters, double *ms_out /* [12
 /* CTAs per SM of the one-kernel solve at this handle's shared-memory size (cudaOccupancyMaxActiveBlocksPerMultiprocessor);
  * 0 when no window of the finalized handle takes that path. */
 int d2ba_debug_solve_occupancy(d2ba_handle *h, int32_t *ctas_per_sm);
+/* Phase timestamps of the one-kernel solve: runs `iters` fixed iterations from the uploaded state (as
+ * d2ba_debug_kernel_times does) with a timestamped k_solve_small, whose first thread stores %globaltimer (ns) at the
+ * start of (1) Schur complement, (2) Cholesky, (3) speed-bias back substitution, (4) landmark back substitution + step,
+ * and at the end.  ts_out[(it * n + w) * 5 + k] for iteration it and window w of the n = d2ba_num_windows windows
+ * (iters * n * 5 entries); a skipped phase (rejected step) has the start time of the next, and windows outside that
+ * path or already finished stay 0.  ms_out[it] is the device time of that iteration's k_solve_small launch (CUDA
+ * events).  Needs a finalized handle. */
+int d2ba_debug_solve_phases(d2ba_handle *h, int32_t iters, int64_t *ts_out, double *ms_out /* [iters] */);
 /* Host wall-clock (ms) of the phases of the last d2ba_finalize: [plan (pair-major order, groups, jobs), prefix sums +
  * staging resize, staging fill, upload enqueue, error check, read-back buffers, device ms of the uploads, device ms of tile build + prep kernels], followed by
  * the thread-summed ms spent inside d2ba_add_proj since the last d2ba_reset: [id lookup, stamp scan, staging copy,
