@@ -6,9 +6,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.environ.get("D2BA_OUT") or os.path.join(HERE, "libd2ba.so")
-SOURCES = ["d2ba_kernels.cu", "d2ba_host.cu", "d2ba_margin.cu", "d2pgo.cu", "d2pgo_pcm.cu", "d2pgo_chol.cu", "d2pgo_lm.cu"]
+SOURCES = ["d2ba_kernels.cu", "d2ba_host.cu", "d2ba_margin.cu", "d2pgo.cu", "d2pgo_pcm.cu", "d2pgo_chol.cu", "d2pgo_lm.cu", "d2pgo_chart.cu"]
 EXTRA_DEPS = ["d2ba_harness.cpp"]
-HEADERS = ["d2ba_types.cuh", "d2ba_math.cuh", "d2ba_proj.cuh", "d2ba_launch.cuh", "d2pgo_chol.cuh", "d2pgo_handle.cuh", "d2pgo_lm.cuh", os.path.join("..", "..", "include", "d2ba.h"), os.path.join("..", "..", "include", "d2pgo.h")]
+HEADERS = ["d2ba_types.cuh", "d2ba_math.cuh", "d2ba_proj.cuh", "d2ba_launch.cuh", "d2pgo_chol.cuh", "d2pgo_handle.cuh", "d2pgo_lm.cuh", "d2pgo_chart.cuh", os.path.join("..", "..", "include", "d2ba.h"), os.path.join("..", "..", "include", "d2pgo.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 

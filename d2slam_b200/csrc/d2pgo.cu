@@ -18,6 +18,7 @@
 
 #include "d2ba_math.cuh"
 #include "d2pgo_handle.cuh"
+#include "d2pgo_chart.cuh"
 #include "d2pgo_lm.cuh"
 
 namespace d2ba {
@@ -158,6 +159,11 @@ D2BA_DEV void pgo_gravity_eval(const double *x, const double *ue, const double *
   const double K[9] = {0.0, -u[2], u[1], u[2], 0.0, -u[0], -u[1], u[0], 0.0};   // [u]x
   for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) J[i * 3 + j] = S[i] * K[j] + S[3 + i] * K[3 + j] + S[6 + i] * K[6 + j];
 }
+
+// the perturbation chart's policy (d2pgo_set_chart): pose records [p, theta, 0, 0], the retraction x + dx.  A tag for the host
+// templates only: its factor, prior, proximal, retraction and dual-update kernels live in d2pgo_chart.cu, and every kernel here that reads only D runs
+// its PgoEdge6 instantiation (PgoKern)
+struct PgoChart6 { static constexpr int D = 6; };
 
 // Fixed-order sum of n per-block partials, the same value in every thread of every block (so that all blocks -- and all
 // ranks, which hold identical vectors -- take the same branch without a single-thread "decide" kernel in between).
@@ -880,6 +886,79 @@ static int pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double 
   return 0;
 }
 
+// ---- the perturbation chart, host side (d2pgo_set_chart)
+static bool all_finite(const double *v, size_t n) {
+  for (size_t k = 0; k < n; k++) if (!std::isfinite(v[k])) return false;
+  return true;
+}
+
+// a q_init as the chart keeps it: finite, non-zero, normalised (false otherwise)
+static bool chart_unit(const double *q, double *out) {
+  const double s2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  if (!all_finite(q, 4) || !(s2 > 0.0)) return false;
+  const double s = 1.0 / std::sqrt(s2);
+  for (int k = 0; k < 4; k++) out[k] = q[k] * s;
+  return true;
+}
+
+// normalise(q_init (x) quatfromRotationVector(theta)) of a chart record [p, theta, 0, 0] (postPerturbSolve, d2pgo.cpp:616-628;
+// the normalisation is Swarm::Pose's, ASSUMED)
+static void chart_attitude(const double *x, const double *qi, double *q) {
+  const double *th = x + 3;
+  const double n = std::sqrt(th[0] * th[0] + th[1] * th[1] + th[2] * th[2]);
+  double d[4];   // x y z w
+  if (n < 1e-2) { d[0] = th[0] / 2.0; d[1] = th[1] / 2.0; d[2] = th[2] / 2.0; d[3] = 1.0; }
+  else { const double s = std::sin(n / 2.0); for (int k = 0; k < 3; k++) d[k] = th[k] / n * s; d[3] = std::cos(n / 2.0); }
+  const double o[4] = {qi[3] * d[0] + qi[0] * d[3] + qi[1] * d[2] - qi[2] * d[1], qi[3] * d[1] - qi[0] * d[2] + qi[1] * d[3] + qi[2] * d[0],
+                       qi[3] * d[2] + qi[0] * d[1] - qi[1] * d[0] + qi[2] * d[3], qi[3] * d[3] - qi[0] * d[0] - qi[1] * d[1] - qi[2] * d[2]};
+  chart_unit(o, q);
+}
+
+// the pose records in the retraction's layout [p, q, 0]: the chart's attitudes composed and normalised
+static std::vector<double> chart_poses(const d2pgo_handle *h) {
+  std::vector<double> out(h->poses.size(), 0.0);
+  for (size_t i = 0; i < h->ids.size(); i++) {
+    memcpy(&out[i * 8], &h->poses[i * 8], 24);
+    chart_attitude(&h->poses[i * 8], &h->chart_qinit[i * 4], &out[i * 8 + 3]);
+  }
+  return out;
+}
+
+static int chart_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out) {
+  if (n < 0 || (n > 0 && (!ids || !out))) return pgo_fail(h, 1, "get_poses: null argument or negative count");
+  for (int k = 0; k < n; k++) {
+    auto it = h->index.find(ids[k]);
+    if (it == h->index.end()) return pgo_fail(h, 2, "get_poses: unknown id");
+    const size_t i = (size_t)it->second;
+    memcpy(out + (size_t)k * 7, &h->poses[i * 8], 24);
+    chart_attitude(&h->poses[i * 8], &h->chart_qinit[i * 4], out + (size_t)k * 7 + 3);
+  }
+  return 0;
+}
+
+// d2pgo_set_poses on a chart handle: ids already present keep their [p, theta] and q_init, new ids start at [p, 0] with q_init
+// = their normalised attitude (PGOState::addFrame)
+static int chart_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *poses7, const uint8_t *fixed) {
+  std::vector<double> x((size_t)n * 7, 0.0), qi((size_t)n * 4);
+  std::unordered_map<int64_t, int> seen;
+  for (int k = 0; k < n; k++) {
+    if (!seen.emplace(ids[k], k).second) return pgo_fail(h, 2, "set_poses: duplicate pose id");
+    auto it = h->index.find(ids[k]);
+    if (it != h->index.end()) {
+      memcpy(&x[(size_t)k * 7], &h->poses[(size_t)it->second * 8], 48);
+      memcpy(&qi[(size_t)k * 4], &h->chart_qinit[(size_t)it->second * 4], 32);
+      continue;
+    }
+    const double *p = poses7 + (size_t)k * 7;
+    if (!all_finite(p, 7) || !chart_unit(p + 3, &qi[(size_t)k * 4]))
+      return pgo_fail(h, 2, "set_poses: pose id " + std::to_string(ids[k]) + ": non-finite value or zero quaternion (the perturbation chart takes its q_init from it)");
+    memcpy(&x[(size_t)k * 7], p, 24);
+  }
+  if (int rc = pgo_set_poses(h, n, ids, x.data(), 7, fixed, "set_poses")) return rc;
+  h->chart_qinit.swap(qi);
+  return 0;
+}
+
 extern "C" {
 
 int d2pgo_default_config(d2pgo_config *c) {
@@ -922,6 +1001,7 @@ const char *d2pgo_last_error(const d2pgo_handle *h) { return h ? h->err.c_str() 
 int d2pgo_set_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *poses7, const uint8_t *fixed) {
   if (!h || n <= 0) return 1;
   if (int rc = pgo_want_dof(h, 6, "set_poses")) return rc;
+  if (h->chart) return chart_set_poses(h, n, ids, poses7, fixed);
   return pgo_set_poses(h, n, ids, poses7, 7, fixed, "set_poses");
 }
 
@@ -946,6 +1026,7 @@ int d2pgo_add_edges_4d(d2pgo_handle *h, int32_t n, const int64_t *id_a, const in
 int d2pgo_comm_init(d2pgo_handle *h, const uint8_t unique_id[128], int32_t rank, int32_t nranks) {
   if (!h) return 1;
   if (h->arock) { h->err = "comm_init: the handle is in ARock mode (each agent solves its own sub-graph; edge sharding splits one graph)"; return 5; }
+  if (h->chart) { h->err = "comm_init: the handle is in the perturbation chart, which has no edge-sharded form (d2pgo_set_chart(h, D2PGO_CHART_RETRACTION, ...) first)"; return 5; }
   if (h->linear_solver == D2PGO_LINEAR_SPARSE_CHOLESKY) { h->err = "comm_init: the handle solves with the sparse Cholesky, which has no edge-sharded form (d2pgo_set_linear_solver PCG first)"; return 5; }
   cudaSetDevice(h->cfg.device);
   if (nccl_comm_init(&h->comm, unique_id, rank, nranks, h->err)) return 3;
@@ -997,6 +1078,10 @@ static int pgo_upload(d2pgo_handle *h) {
     PCK(cudaMemcpyAsync(h->d_gp_S.p, h->gp_S.data(), G * 72, cudaMemcpyHostToDevice, h->stream));
     PCK(cudaMemcpyAsync(h->d_prior_of.p, prior_of.data(), N * 4, cudaMemcpyHostToDevice, h->stream));
   }
+  if (h->chart == D2PGO_CHART_PERTURB) {
+    PCK(h->d_qinit.alloc(N * 4));
+    PCK(cudaMemcpyAsync(h->d_qinit.p, h->chart_qinit.data(), N * 32, cudaMemcpyHostToDevice, h->stream));
+  }
   PCK(cudaStreamSynchronize(h->stream));   // ptr / inc / prior_of go out of scope
   h->uploaded = true;
   return 0;
@@ -1027,6 +1112,9 @@ static PgoArockDev pgo_arock_view(d2pgo_handle *h, int cur) {
   return a;
 }
 
+// the kernels that only read P::D (gradient, block diagonal, CG) serve both 6-DoF charts: their PgoEdge6 instantiations
+template <class P> using PgoKern = typename std::conditional<std::is_same<P, PgoChart6>::value, PgoEdge6, P>::type;
+
 // cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks.  grav: the
 // gravity priors of this rank (6-DoF only; their cost partials follow the edges', their terms enter g and D after each pose's
 // edges).  ark: the ARock proximal terms of the synced dual table (cost partials last, g and D after the edges and priors).
@@ -1034,18 +1122,34 @@ static PgoArockDev pgo_arock_view(d2pgo_handle *h, int cur) {
 template <class P>
 static void pgo_linearize_enqueue(d2pgo_handle *h, cudaStream_t st, int b, int want_jac, bool grav, bool ark, double *cost_dev) {
   constexpr int D = P::D;
+  constexpr bool chart = std::is_same<P, PgoChart6>::value;
+  using K = PgoKern<P>;
   PgoDev d = pgo_view(h, b);
   const PgoPriorDev pr = pgo_prior_view(h, b);
   const PgoArockDev ak = pgo_arock_view(h, b);
   const int nbe = (d.n_edge + 127) / 128, nbg = grav ? (pr.n_prior + 127) / 128 : 0, nbk = ark ? (ak.n_dual + 127) / 128 : 0;
-  if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, st>>>(d, h->d_cost_part.p, want_jac);
-  if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, st>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
-  if (nbk > 0) k_pgo_arock_lin<D><<<nbk, 128, 0, st>>>(d, h->d_cost_part.p + nbe + nbg, ak);
+  if constexpr (chart) {
+    if (d.n_edge > 0) d2pgo_chart::edges(st, d.n_edge, d.ea, d.eb, d.x, h->d_qinit.p, d.rel, d.sinfo, d.lin, h->d_cost_part.p, want_jac);
+    if (nbg > 0) d2pgo_chart::priors(st, pr.n_prior, pr.pose, pr.u, pr.S, d.x, h->d_qinit.p, pr.lin, h->d_cost_part.p + nbe, want_jac);
+  } else {
+    if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, st>>>(d, h->d_cost_part.p, want_jac);
+    if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, st>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
+  }
+  if constexpr (chart) {
+    if (nbk > 0) d2pgo_chart::arock_lin(st, ak.n_dual, ak.pose, d.x, ak.yr, ak.wT, ak.wR, ak.lin, h->d_cost_part.p + nbe + nbg);
+  } else if (nbk > 0) k_pgo_arock_lin<D><<<nbk, 128, 0, st>>>(d, h->d_cost_part.p + nbe + nbg, ak);
   k_pgo_sum<<<1, 128, 0, st>>>(h->d_cost_part.p, nbe + nbg + nbk, cost_dev);
   if (want_jac && grav) {
-    if constexpr (D == 6) k_pgo_gD<P, true><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
-  } else if (want_jac) k_pgo_gD<P, false><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+    if constexpr (D == 6) k_pgo_gD<K, true><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+  } else if (want_jac) k_pgo_gD<K, false><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
   if (want_jac && nbk > 0) k_pgo_arock_gD<D><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, ak);
+}
+
+// candidate poses x (+) dx of linearisation view d into x_out
+template <class P>
+static void pgo_retract_enqueue(cudaStream_t st, const PgoDev &d, double *x_out) {
+  if constexpr (std::is_same<P, PgoChart6>::value) d2pgo_chart::retract(st, d.n_pose, d.x, d.fixed, d.dx, x_out);
+  else k_pgo_retract<P><<<d.nbp, 128, 0, st>>>(d, x_out);
 }
 
 template <class P>
@@ -1207,9 +1311,9 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
         if (lambda > 1e8) break;
         continue;
       }
-    } else if ((rc = pgo_pcg<P>(h, cur, lambda, tol2, h->cfg.pcg_max_iterations, grav, ark, &s))) return rc;
+    } else if ((rc = pgo_pcg<PgoKern<P>>(h, cur, lambda, tol2, h->cfg.pcg_max_iterations, grav, ark, &s))) return rc;
     const PgoDev d = pgo_view(h, cur);
-    k_pgo_retract<P><<<d.nbp, 128, 0, h->stream>>>(d, h->d_x[1 - cur].p);
+    pgo_retract_enqueue<P>(h->stream, d, h->d_x[1 - cur].p);
     double cand = 0;
     if ((rc = pgo_linearize<P>(h, 1 - cur, 1, grav, ark, &cand))) return rc;
     R.pcg_iterations += s.iters; R.iterations++;
@@ -1293,7 +1397,9 @@ static int lm_build(d2pgo_handle *h, bool grav, bool ark, cudaStream_t *cs) {
   d2pgo_lm::start(cs[0], s);
   pgo_linearize_enqueue<P>(h, cs[0], 0, 1, grav, ark, cost);
   d2pgo_lm::scale(cs[0], v, h->d_D[0].p, s, h->d_lm_scale.p);
-  d2pgo_lm::xnorm(cs[0], v, xpart);
+  // the gradient and parameter tests' norms: of the ambient 7-vectors, or of the chart's Euclidean 6-vectors
+  const auto xnorm = std::is_same<P, PgoChart6>::value ? d2pgo_lm::xnorm_chart : d2pgo_lm::xnorm;
+  xnorm(cs[0], v, xpart);
   PCK(lm_cond(cs[0], loop, cudaGraphCondTypeWhile, &body));
   PCK(cudaStreamEndCapture(cs[0], &top));
   PCK(cudaGraphConditionalHandleCreate(&go, body, 0, 0));
@@ -1312,13 +1418,13 @@ static int lm_build(d2pgo_handle *h, bool grav, bool ark, cudaStream_t *cs) {
   PCK(lm_cond(cs[2], acc, cudaGraphCondTypeIf, &acc_g));
   PCK(cudaStreamEndCapture(cs[2], &go_g));
   PCK(cudaStreamBeginCaptureToGraph(cs[3], eval_g, nullptr, nullptr, 0, mode));
-  k_pgo_retract<P><<<nbp, 128, 0, cs[3]>>>(d0, h->d_x[1].p);
+  pgo_retract_enqueue<P>(cs[3], d0, h->d_x[1].p);
   pgo_linearize_enqueue<P>(h, cs[3], 1, 0, grav, ark, cost + 1);
   PCK(cudaStreamEndCapture(cs[3], &eval_g));
   PCK(cudaStreamBeginCaptureToGraph(cs[3], acc_g, nullptr, nullptr, 0, mode));
   PCK(cudaMemcpyAsync(h->d_x[0].p, d1.x, (size_t)d0.n_pose * 64, cudaMemcpyDeviceToDevice, cs[3]));
   pgo_linearize_enqueue<P>(h, cs[3], 0, 1, grav, ark, cost);
-  d2pgo_lm::xnorm(cs[3], v, xpart);
+  xnorm(cs[3], v, xpart);
   PCK(cudaStreamEndCapture(cs[3], &acc_g));
   PCK(cudaGetLastError());
   if (h->lm_graph) { cudaGraphExecDestroy(h->lm_graph); h->lm_graph = nullptr; }
@@ -1349,8 +1455,8 @@ static int pgo_solve_ceres(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
     const PgoDev d = pgo_view(h, b); const PgoPriorDev pr = pgo_prior_view(h, b); const PgoArockDev ak = pgo_arock_view(h, b);
     put(&d, sizeof d); put(&pr, sizeof pr); put(&ak, sizeof ak);
   }
-  const void *ptrs[7] = {h->d_lm.p, h->d_lm_scale.p, h->d_lm_part.p, h->d_lm_trace.p, h->d_cost.p, h->d_cost_part.p, h->chol.get()};
-  const int gen[4] = {h->chol->generation, grav, ark, 0};
+  const void *ptrs[8] = {h->d_lm.p, h->d_lm_scale.p, h->d_lm_part.p, h->d_lm_trace.p, h->d_cost.p, h->d_cost_part.p, h->chol.get(), h->d_qinit.p};
+  const int gen[4] = {h->chol->generation, grav, ark, h->chart};
   put(ptrs, sizeof ptrs); put(gen, sizeof gen);
   if (!h->lm_graph || h->lm_key != key) {
     cudaStream_t cs[4] = {h->stream, nullptr, nullptr, nullptr};
@@ -1400,12 +1506,14 @@ int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h || h->ids.empty()) return 1;
   if (int rc = lm_refuse(h, "solve")) return rc;
   cudaSetDevice(h->cfg.device);
-  return h->dof == 4 ? pgo_minimize<PgoEdge4>(h, rep, false) : pgo_minimize<PgoEdge6>(h, rep, false);
+  if (h->dof == 4) return pgo_minimize<PgoEdge4>(h, rep, false);
+  return h->chart ? pgo_minimize<PgoChart6>(h, rep, false) : pgo_minimize<PgoEdge6>(h, rep, false);
 }
 
 int d2pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out) {
   if (!h) return 1;
   if (int rc = pgo_want_dof(h, 6, "get_poses")) return rc;
+  if (h->chart) return chart_get_poses(h, n, ids, out);
   return pgo_get_poses(h, n, ids, out, 7, "get_poses");
 }
 
@@ -1423,7 +1531,9 @@ int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles) {
   const size_t E = h->ea.size(), W = (size_t)h->dof + 2 * (size_t)h->dof * h->dof;   // 78 (6-DoF) or 36 (4-DoF) per edge
   if ((size_t)out_doubles < E * W) { h->err = "debug_edges: buffer too small"; return 2; }
   double cost;
-  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4>(h, 0, 1, false, false, &cost) : pgo_linearize<PgoEdge6>(h, 0, 1, false, false, &cost))) return rc;
+  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4>(h, 0, 1, false, false, &cost)
+            : h->chart  ? pgo_linearize<PgoChart6>(h, 0, 1, false, false, &cost)
+                        : pgo_linearize<PgoEdge6>(h, 0, 1, false, false, &cost))) return rc;
   std::vector<double> tmp(E * W);
   PCK(cudaMemcpyAsync(tmp.data(), h->d_lin[0].p, E * W * 8, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
@@ -1479,7 +1589,7 @@ int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
   double cost;
-  if ((rc = pgo_linearize<PgoEdge6>(h, 0, 1, true, false, &cost))) return rc;
+  if ((rc = h->chart ? pgo_linearize<PgoChart6>(h, 0, 1, true, false, &cost) : pgo_linearize<PgoEdge6>(h, 0, 1, true, false, &cost))) return rc;
   std::vector<double> tmp(G * 12);
   PCK(cudaMemcpyAsync(tmp.data(), h->d_glin[0].p, G * 12 * 8, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
@@ -1494,10 +1604,6 @@ int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles
 }  // extern "C"
 
 // ---- ARock host side
-static bool all_finite(const double *v, size_t n) {
-  for (size_t k = 0; k < n; k++) if (!std::isfinite(v[k])) return false;
-  return true;
-}
 
 // poses the local problem uses: those an edge or a gravity prior touches (ARockSolver::all_estimating_params)
 static std::vector<char> arock_in_problem(const d2pgo_handle *h) {
@@ -1615,6 +1721,14 @@ static int arock_sync(d2pgo_handle *h) {
 // every pose at d_x[0] in dual coordinates, [N][D] on the host
 static int arock_coords(d2pgo_handle *h, std::vector<double> &out) {
   const size_t N = h->ids.size(), D = h->dof;
+  if (h->chart) {   // the chart's dual coordinates are the state [p, theta] itself
+    std::vector<double> x(N * 8);
+    PCK(cudaMemcpyAsync(x.data(), h->d_x[0].p, N * 64, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaStreamSynchronize(h->stream));
+    out.resize(N * 6);
+    for (size_t i = 0; i < N; i++) memcpy(&out[i * 6], &x[i * 8], 48);
+    return 0;
+  }
   PCK(h->d_ak_coord.alloc(N * D));
   const int nb = (int)((N + 127) / 128);
   if (D == 6) k_pgo_arock_coord<6><<<nb, 128, 0, h->stream>>>((int)N, h->d_x[0].p, h->d_ak_qinit.p, h->d_ak_coord.p);
@@ -1655,7 +1769,7 @@ int d2pgo_arock_enable(d2pgo_handle *h, const d2pgo_arock_config *cfg, int32_t n
   for (int k = 0; k < n; k++) {
     auto it = h->index.find(ids[k]);
     if (it == h->index.end()) return pgo_fail(h, 2, "arock_enable: unknown pose id " + std::to_string(ids[k]));
-    const double *src = q_init4 ? q_init4 + (size_t)k * 4 : &h->poses[(size_t)it->second * 8 + 3];
+    const double *src = q_init4 ? q_init4 + (size_t)k * 4 : h->chart ? &h->chart_qinit[(size_t)it->second * 4] : &h->poses[(size_t)it->second * 8 + 3];
     if (h->dof == 6) {
       const double s2 = src[0] * src[0] + src[1] * src[1] + src[2] * src[2] + src[3] * src[3];
       if (!all_finite(src, 4) || !(s2 > 0.0)) return pgo_fail(h, 2, "arock_enable: pose id " + std::to_string(ids[k]) + ": non-finite or zero q_init");
@@ -1708,12 +1822,13 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
   }
   // 3. setDualStateFactors + solveLocalStep: the LM solve with the proximal terms towards y_r
   if (created && (rc = arock_sync(h))) return rc;
-  if ((rc = D == 4 ? pgo_minimize<PgoEdge4>(h, rep, true) : pgo_minimize<PgoEdge6>(h, rep, true))) return rc;
+  if ((rc = D == 4 ? pgo_minimize<PgoEdge4>(h, rep, true) : h->chart ? pgo_minimize<PgoChart6>(h, rep, true) : pgo_minimize<PgoEdge6>(h, rep, true))) return rc;
   // 4. updateDualStates at the solved poses, which pgo_solve leaves in buffer 0
   const PgoArockDev ak = pgo_arock_view(h, 0);
   if (ak.n_dual > 0) {
     const int nb = (ak.n_dual + 127) / 128;
-    if (D == 6) k_pgo_arock_update<6><<<nb, 128, 0, h->stream>>>(h->d_x[0].p, ak);
+    if (h->chart) d2pgo_chart::arock_update(h->stream, ak.n_dual, ak.pose, h->d_x[0].p, ak.yr, ak.yl, ak.eta);
+    else if (D == 6) k_pgo_arock_update<6><<<nb, 128, 0, h->stream>>>(h->d_x[0].p, ak);
     else k_pgo_arock_update<4><<<nb, 128, 0, h->stream>>>(h->d_x[0].p, ak);
     PCK(cudaGetLastError());
     std::vector<double> yl((size_t)ak.n_dual * D);
@@ -1750,7 +1865,8 @@ int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
   const PgoDev d = pgo_view(h, 0);
   const PgoArockDev ak = pgo_arock_view(h, 0);
   const int nb = (int)((K + 127) / 128);
-  if (D == 6) k_pgo_arock_lin<6><<<nb, 128, 0, h->stream>>>(d, h->d_cost_part.p, ak);
+  if (h->chart) d2pgo_chart::arock_lin(h->stream, ak.n_dual, ak.pose, d.x, ak.yr, ak.wT, ak.wR, ak.lin, h->d_cost_part.p);
+  else if (D == 6) k_pgo_arock_lin<6><<<nb, 128, 0, h->stream>>>(d, h->d_cost_part.p, ak);
   else k_pgo_arock_lin<4><<<nb, 128, 0, h->stream>>>(d, h->d_cost_part.p, ak);
   PCK(cudaGetLastError());
   std::vector<double> tmp(K * W);
@@ -1807,7 +1923,7 @@ static int pgo_pcg_step(d2pgo_handle *h, double lambda, int max_it, double tol, 
   double cost;
   if ((rc = pgo_linearize<P>(h, 0, 1, grav, ark, &cost))) return rc;
   PgoScalars s; memset(&s, 0, sizeof s);
-  if ((rc = pgo_pcg<P>(h, 0, lambda, tol * tol, max_it, grav, ark, &s))) return rc;
+  if ((rc = pgo_pcg<PgoKern<P>>(h, 0, lambda, tol * tol, max_it, grav, ark, &s))) return rc;
   PCK(cudaMemcpyAsync(out, h->d_dx.p, h->ids.size() * (size_t)P::D * 8, cudaMemcpyDeviceToHost, h->stream));
   return pcg_last_residual(h, iters, residual);
 }
@@ -1852,7 +1968,8 @@ int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64
   if (h->comm) { h->err = "debug_exact_step: the handle has a communicator"; return 5; }
   if (h->arock) if (int rc = arock_check_poses(h, "debug_exact_step")) return rc;
   cudaSetDevice(h->cfg.device);
-  return h->dof == 4 ? pgo_exact_step<PgoEdge4>(h, lambda, h->arock, dx_out) : pgo_exact_step<PgoEdge6>(h, lambda, h->arock, dx_out);
+  if (h->dof == 4) return pgo_exact_step<PgoEdge4>(h, lambda, h->arock, dx_out);
+  return h->chart ? pgo_exact_step<PgoChart6>(h, lambda, h->arock, dx_out) : pgo_exact_step<PgoEdge6>(h, lambda, h->arock, dx_out);
 }
 
 int d2pgo_debug_pcg_step(d2pgo_handle *h, double lambda, int32_t max_it, double tol, double *dx_out, int64_t out_doubles,
@@ -1867,8 +1984,9 @@ int d2pgo_debug_pcg_step(d2pgo_handle *h, double lambda, int32_t max_it, double 
   if (h->comm) { h->err = "debug_pcg_step: the handle has a communicator"; return 5; }
   if (h->arock) if (int rc = arock_check_poses(h, "debug_pcg_step")) return rc;
   cudaSetDevice(h->cfg.device);
-  return h->dof == 4 ? pgo_pcg_step<PgoEdge4>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out)
-                     : pgo_pcg_step<PgoEdge6>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out);
+  if (h->dof == 4) return pgo_pcg_step<PgoEdge4>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out);
+  return h->chart ? pgo_pcg_step<PgoChart6>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out)
+                  : pgo_pcg_step<PgoEdge6>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out);
 }
 
 int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out, int32_t max_pairs, int32_t *n_pairs_out,
@@ -2092,8 +2210,8 @@ int d2pgo_default_rot_init_config(d2pgo_rot_init_config *c) {
   return 0;
 }
 
-int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids, const double *ego_poses7,
-                   d2pgo_rot_init_report *report) {
+static int rot_init_run(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids, const double *ego_poses7,
+                        d2pgo_rot_init_report *report) {
   if (!h) return 1;
   if (!cfg || n_ego < 0 || (n_ego > 0 && (!ego_ids || !ego_poses7))) return pgo_fail(h, 1, "rot_init: null argument or negative count");
   if (h->dof != 6) return pgo_fail(h, 5, "rot_init: the handle was created with pose_dof = 4; rotation initialisation acts on 6-DoF poses");
@@ -2128,6 +2246,21 @@ int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_
   return 0;
 }
 
+// on a chart handle the initialisation runs on the composed attitudes; each frame's q_init then becomes its attitude after it --
+// the solved frames' the initialised one, every other frame's its current one (recoverRotationLLT, :360-389) --, and p and theta
+// keep every bit
+int d2pgo_rot_init(d2pgo_handle *h, const d2pgo_rot_init_config *cfg, int32_t n_ego, const int64_t *ego_ids, const double *ego_poses7,
+                   d2pgo_rot_init_report *report) {
+  if (!h || !h->chart) return rot_init_run(h, cfg, n_ego, ego_ids, ego_poses7, report);
+  std::vector<double> state = chart_poses(h);
+  state.swap(h->poses);
+  const int rc = rot_init_run(h, cfg, n_ego, ego_ids, ego_poses7, report);
+  if (!rc) for (size_t i = 0; i < h->ids.size(); i++) chart_unit(&h->poses[i * 8 + 3], &h->chart_qinit[i * 4]);
+  h->poses.swap(state);
+  h->uploaded = false;
+  return rc;
+}
+
 }  // extern "C"
 
 // ---- distributed rotation initialisation host side (d2pgo_arock_rot_*)
@@ -2160,6 +2293,7 @@ int d2pgo_arock_rot_receive(d2pgo_handle *h, int32_t sender, int32_t target, int
   if (!h) return 1;
   int rc;
   if ((rc = rot_arock_check(h, "arock_rot_receive", true))) return rc;
+  if (h->chart) return pgo_fail(h, 5, "arock_rot_receive: the handle is in the perturbation chart; the distributed rotation initialisation precedes it (d2pgo_set_chart after it takes its attitudes as q_init)");
   if (n > 0 && !poses7) return pgo_fail(h, 1, "arock_rot_receive: null argument or negative count");
   if ((rc = arock_receive_check(h, "arock_rot_receive", 9, sender, n, frame_ids, dim, duals))) return rc;
   if (!all_finite(poses7, (size_t)n * 7)) return pgo_fail(h, 2, "arock_rot_receive: non-finite pose");
@@ -2189,6 +2323,7 @@ int d2pgo_arock_rot_init_step(d2pgo_handle *h, const d2pgo_arock_rot_init_config
   if (!cfg || n_ego < 0 || (n_ego > 0 && (!ego_ids || !ego_poses7))) return pgo_fail(h, 1, "arock_rot_init_step: null argument or negative count");
   int rc;
   if ((rc = rot_arock_check(h, "arock_rot_init_step", true))) return rc;
+  if (h->chart) return pgo_fail(h, 5, "arock_rot_init_step: the handle is in the perturbation chart; the distributed rotation initialisation precedes it (d2pgo_set_chart after it takes its attitudes as q_init)");
   if (h->ids.empty()) return pgo_fail(h, 1, "arock_rot_init_step: the handle has no poses");
   if ((rc = arock_check_poses(h, "arock_rot_init_step"))) return rc;
   d2pgo_rot_init_config rcfg;   // the fields the two configs share
@@ -2381,6 +2516,75 @@ int d2pgo_debug_minimizer_trace(d2pgo_handle *h, int32_t max, int32_t *n_out, d2
   if (h->lm_trace_n > 0) {
     PCK(cudaMemcpyAsync(out, h->d_lm_trace.p, (size_t)h->lm_trace_n * sizeof *out, cudaMemcpyDeviceToHost, h->stream));
     PCK(cudaStreamSynchronize(h->stream));
+  }
+  return 0;
+}
+
+}  // extern "C"
+
+// ---- the perturbation chart's entry points (include/d2pgo.h d2pgo_set_chart)
+extern "C" {
+
+int d2pgo_set_chart(d2pgo_handle *h, int32_t chart, int32_t n, const int64_t *ids, const double *q_init4) {
+  if (!h) return 1;
+  if (chart != D2PGO_CHART_RETRACTION && chart != D2PGO_CHART_PERTURB)
+    return pgo_fail(h, 2, "set_chart: unknown chart " + std::to_string(chart) + " (0 = retraction, 1 = perturbation)");
+  if (h->dof != 6) return pgo_fail(h, 5, "set_chart: the handle was created with pose_dof = 4; d2pgo builds RelPoseFactor4D there in either mode");
+  if (h->comm) return pgo_fail(h, 5, "set_chart: the handle has a communicator; the perturbation chart has no edge-sharded form");
+  if (h->arock && !h->pose_table.duals.empty())
+    return pgo_fail(h, 5, "set_chart: the handle's ARock duals are held in the other chart's coordinates (enter the chart before the first d2pgo_arock_step)");
+  if (n < 0 || (n > 0 && !ids)) return pgo_fail(h, 1, "set_chart: null argument or negative count");
+  for (int k = 0; k < n; k++)
+    if (!h->index.count(ids[k])) return pgo_fail(h, 2, "set_chart: unknown pose id " + std::to_string(ids[k]));
+  // the attitudes as they stand, then every validation before anything changes
+  std::vector<double> cur = h->chart ? chart_poses(h) : h->poses;
+  const size_t N = h->ids.size();
+  std::vector<double> qi(N * 4);
+  for (size_t i = 0; i < N; i++)
+    if (!chart_unit(&cur[i * 8 + 3], &qi[i * 4])) return pgo_fail(h, 2, "set_chart: pose id " + std::to_string(h->ids[i]) + ": non-finite or zero attitude");
+  if (chart == D2PGO_CHART_PERTURB && q_init4)
+    for (int k = 0; k < n; k++) {
+      auto it = h->index.find(ids[k]);
+      if (!chart_unit(q_init4 + (size_t)k * 4, &qi[(size_t)it->second * 4]))
+        return pgo_fail(h, 2, "set_chart: pose id " + std::to_string(ids[k]) + ": non-finite or zero q_init");
+    }
+  if (chart == D2PGO_CHART_PERTURB) {   // PGOState::addFrame: x = [p, 0]
+    for (size_t i = 0; i < N; i++) for (int k = 3; k < 8; k++) cur[i * 8 + k] = 0.0;
+    h->chart_qinit.swap(qi);
+  } else {
+    h->chart_qinit.clear();
+  }
+  h->poses.swap(cur);
+  h->chart = chart;
+  h->uploaded = false;
+  return 0;
+}
+
+int d2pgo_set_perturb(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *x6) {
+  if (!h) return 1;
+  if (!h->chart) return pgo_fail(h, 5, "set_perturb: the handle is not in the perturbation chart (d2pgo_set_chart)");
+  if (n < 0 || (n > 0 && (!ids || !x6))) return pgo_fail(h, 1, "set_perturb: null argument or negative count");
+  std::vector<int> idx(n);
+  for (int k = 0; k < n; k++) {
+    auto it = h->index.find(ids[k]);
+    if (it == h->index.end()) return pgo_fail(h, 2, "set_perturb: unknown pose id " + std::to_string(ids[k]));
+    if (!all_finite(x6 + (size_t)k * 6, 6)) return pgo_fail(h, 2, "set_perturb: pose id " + std::to_string(ids[k]) + ": non-finite value");
+    idx[k] = it->second;
+  }
+  for (int k = 0; k < n; k++) memcpy(&h->poses[(size_t)idx[k] * 8], x6 + (size_t)k * 6, 48);
+  if (n > 0) h->uploaded = false;
+  return 0;
+}
+
+int d2pgo_get_perturb(d2pgo_handle *h, int32_t n, const int64_t *ids, double *x6_out, double *q_init4_out) {
+  if (!h) return 1;
+  if (!h->chart) return pgo_fail(h, 5, "get_perturb: the handle is not in the perturbation chart (d2pgo_set_chart)");
+  if (n < 0 || (n > 0 && (!ids || !x6_out))) return pgo_fail(h, 1, "get_perturb: null argument or negative count");
+  for (int k = 0; k < n; k++) {
+    auto it = h->index.find(ids[k]);
+    if (it == h->index.end()) return pgo_fail(h, 2, "get_perturb: unknown pose id " + std::to_string(ids[k]));
+    memcpy(x6_out + (size_t)k * 6, &h->poses[(size_t)it->second * 8], 48);
+    if (q_init4_out) memcpy(q_init4_out + (size_t)k * 4, &h->chart_qinit[(size_t)it->second * 4], 32);
   }
   return 0;
 }

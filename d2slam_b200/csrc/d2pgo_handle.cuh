@@ -95,6 +95,9 @@ struct d2pgo_handle {
   Buf<d2pgo_host::LmState> d_lm; Buf<double> d_lm_scale, d_lm_part; Buf<d2pgo_minimizer_iteration> d_lm_trace;
   cudaGraphExec_t lm_graph = nullptr; std::string lm_key;
   bool lm_ran = false; d2pgo_minimizer_summary lm_report = {}; int lm_trace_n = 0;
+  // d2pgo_set_chart: in the perturbation chart the pose records hold [p, theta, 0, 0] and chart_qinit [N][4] (unit, xyzw) the
+  // attitude each theta is taken from; d_qinit is its device copy, uploaded with the poses
+  int chart = D2PGO_CHART_RETRACTION; std::vector<double> chart_qinit; Buf<double> d_qinit;
   int driver_version = 0;
 
   ~d2pgo_handle() {   // the device buffers free themselves

@@ -68,6 +68,21 @@ __global__ void __launch_bounds__(128) k_lm_xnorm(View v, double *part) {
   if (threadIdx.x == 0) { part[blockIdx.x] = xx; part[gridDim.x + blockIdx.x] = gm; }
 }
 
+// k_lm_xnorm in the perturbation chart (d2pgo_set_chart): the state [p, theta] has no manifold, so |x|^2 and the gradient
+// test's max |x - (x + (-g))| run over the six Euclidean components of each free pose
+__global__ void __launch_bounds__(128) k_lm_xnorm_chart(View v, double *part) {
+  __shared__ double red[40];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  double xx = 0.0, gm = 0.0;
+  if (i < v.n_pose && !v.fixed[i]) {
+    const double *x = v.x + (size_t)i * 8;
+    for (int k = 0; k < 6; k++) { xx += x[k] * x[k]; gm = fmax(gm, fabs(x[k] - (x[k] + -v.g[(size_t)i * 6 + k]))); }
+  }
+  xx = block_sum(xx, red);
+  gm = block_max(gm, red);
+  if (threadIdx.x == 0) { part[blockIdx.x] = xx; part[gridDim.x + blockIdx.x] = gm; }
+}
+
 // the model terms of the step dx: partials of r.(J dx) and |J dx|^2 over the edges (blocks [0, nbe)), the gravity priors (next
 // nbg), the proximal terms (next nbk), and of |dx|^2 over the poses (the rest); part = [3][gridDim.x]
 template <int D>
@@ -229,6 +244,8 @@ void xnorm(cudaStream_t st, const View &v, double *part) {
   if (v.D == 6) k_lm_xnorm<6><<<nb, 128, 0, st>>>(v, part);
   else k_lm_xnorm<4><<<nb, 128, 0, st>>>(v, part);
 }
+
+void xnorm_chart(cudaStream_t st, const View &v, double *part) { k_lm_xnorm_chart<<<(v.n_pose + 127) / 128, 128, 0, st>>>(v, part); }
 
 void model(cudaStream_t st, const View &v, int nbe, int nbg, int nbk, double *part) {
   const int nb = nbe + nbg + nbk + (v.n_pose + 127) / 128;

@@ -18,6 +18,7 @@ struct View {
 void start(cudaStream_t st, d2pgo_host::LmState *s);   // the clock, the trust region and the counters
 void scale(cudaStream_t st, const View &v, const double *Dg, const d2pgo_host::LmState *s, double *scale);   // Jacobi scale
 void xnorm(cudaStream_t st, const View &v, double *part);   // partials of |x|^2 and of the gradient test, [2][(N + 127) / 128]
+void xnorm_chart(cudaStream_t st, const View &v, double *part);   // the same in the perturbation chart (6-DoF)
 // partials of r.(J dx), |J dx|^2 and |dx|^2, [3][nbe + nbg + nbk + (N + 127) / 128]
 void model(cudaStream_t st, const View &v, int nbe, int nbg, int nbk, double *part);
 // the one-thread decisions: the top of an iteration, after the step, after the candidate's cost

@@ -33,7 +33,11 @@ the host analysis alone.
 Minimiser (the reference's ceres minimizer_type and time budget): `PgoSolver.set_minimizer("ceres_lm", **cfg)` on a
 sparse-Cholesky handle solves with ceres' Levenberg-Marquardt trust region as d2pgo runs it (include/d2pgo.h
 d2pgo_set_minimizer; cfg overrides CeresLmConfig fields, e.g. max_solver_time_in_seconds), decided on the device in one graph
-launch; minimizer_report() and debug_minimizer_trace() report the last solve.  "restated" is the default LM loop."""
+launch; minimizer_report() and debug_minimizer_trace() report the last solve.  "restated" is the default LM loop.
+
+Perturbation chart (d2pgo's perturb_mode, every 6-DoF node): `PgoSolver.set_chart("perturb")` solves for the 6-vectors
+[p, theta] with q = q_init (x) quatfromRotationVector(theta), kept across solves (include/d2pgo.h d2pgo_set_chart);
+get_perturb / set_perturb read and write that state."""
 import ctypes as C
 
 import numpy as np
@@ -157,7 +161,9 @@ PGO_EXPORTED = ["d2pgo_default_config", "d2pgo_create", "d2pgo_destroy", "d2pgo_
                 "d2pgo_default_arock_rot_init_config", "d2pgo_arock_rot_init_step", "d2pgo_arock_rot_receive",
                 "d2pgo_arock_rot_neighbours", "d2pgo_arock_rot_duals", "d2pgo_debug_arock_rot_state", "d2pgo_pcm_stream_reset",
                 "d2pgo_pcm_stream", "d2pgo_debug_pcm_stream_smd", "d2pgo_debug_pcm_clique_inc",
-                "d2pgo_default_ceres_lm_config", "d2pgo_set_minimizer", "d2pgo_minimizer_report", "d2pgo_debug_minimizer_trace"]
+                "d2pgo_default_ceres_lm_config", "d2pgo_set_minimizer", "d2pgo_minimizer_report", "d2pgo_debug_minimizer_trace",
+                "d2pgo_set_chart", "d2pgo_set_perturb", "d2pgo_get_perturb"]
+CHARTS = {"retraction": 0, "perturb": 1}
 GRAVITY_SQRT_INFO = 10.0   # d2pgo's gravity_sqrt_info (RotInitConfig, d2pgo_config.h:13; the shipped configs)
 _CREATE_ERRORS = {2: "pose_dof must be 0 or 6 (6-DoF poses) or 4 ([x y z yaw] poses)", 3: "no CUDA device (there is no CPU fallback)",
                   4: "bad device index"}
@@ -259,6 +265,27 @@ class PgoSolver:
         self._chk(_lib().d2pgo_debug_minimizer_trace(self.h, C.c_int32(n_max), C.byref(n), buf), "debug_minimizer_trace")
         names = [k for k, _ in MinimizerIteration._fields_ if k != "pad_"]
         return {k: np.array([getattr(buf[i], k) for i in range(n.value)], np.int32 if k == "kind" else np.float64) for k in names}
+
+    def set_chart(self, chart, ids=None, q_init=None):
+        """"perturb" solves in d2pgo's perturbation chart (include/d2pgo.h d2pgo_set_chart): every pose's state becomes [p, 0]
+        with q_init its current attitude, or q_init [n, 4] (xyzw) for the listed ids; "retraction" (the default) leaves it."""
+        k = CHARTS.get(chart, chart) if isinstance(chart, str) else int(chart)
+        if isinstance(k, str):
+            raise ValueError(f"unknown chart {chart!r}: {sorted(CHARTS)}")
+        ids = np.zeros(0, np.int64) if ids is None else np.ascontiguousarray(ids, np.int64)
+        q = None if q_init is None else np.ascontiguousarray(np.asarray(q_init, np.float64).reshape(-1, 4))
+        self._chk(_lib().d2pgo_set_chart(self.h, C.c_int32(k), C.c_int32(len(ids)), _p(ids), _p(q)), "set_chart")
+
+    def set_perturb(self, ids, x6):
+        """The chart states [p, theta] of the listed poses."""
+        ids = np.ascontiguousarray(ids, np.int64); x = np.ascontiguousarray(np.asarray(x6, np.float64).reshape(-1, 6))
+        self._chk(_lib().d2pgo_set_perturb(self.h, C.c_int32(len(ids)), _p(ids), _p(x)), "set_perturb")
+
+    def get_perturb(self, ids):
+        """(x [n, 6] = [p, theta], q_init [n, 4]) of the listed poses of a chart handle."""
+        ids = np.ascontiguousarray(ids, np.int64); x = np.zeros((len(ids), 6)); q = np.zeros((len(ids), 4))
+        self._chk(_lib().d2pgo_get_perturb(self.h, C.c_int32(len(ids)), _p(ids), _p(x), _p(q)), "get_perturb")
+        return x, q
 
     def _chk(self, rc, what):
         if rc:

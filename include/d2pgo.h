@@ -215,6 +215,8 @@ int d2pgo_debug_pcm_clique_inc(d2pgo_handle *h, int32_t n, const uint32_t *adj, 
  *   4-DoF handles: [x y z yaw] (POSE_4D);
  *   6-DoF handles: [p ; theta] with R = R(q_init) Exp(theta), theta = Log(q_init^-1 q) the principal log (POSE_PERTURB_6D,
  *                  d2pgo/src/pgostate.hpp:35-46; the node's perturb_mode).  q_init is the frame's attitude when it was added.
+ *   6-DoF handles in the perturbation chart (d2pgo_set_chart): the state [p ; theta] itself, with the chart's proximal term
+ *                  below.
  * One step:
  *   1. the received messages in arrival order: for a frame the local problem uses (an edge or a gravity prior touches it),
  *      if target == self_id or there is no dual (sender, frame) yet: create it with y_l = y_r = the value, or else set y_r;
@@ -522,6 +524,55 @@ int d2pgo_minimizer_report(d2pgo_handle *h, d2pgo_minimizer_summary *out);
 /* parity hook: the per-iteration records of that call (the first 16384 iterations), copied from the device.  *n_out = the
  * records held; returns 2 (with *n_out set) when max < *n_out, 5 as d2pgo_minimizer_report does */
 int d2pgo_debug_minimizer_trace(d2pgo_handle *h, int32_t max, int32_t *n_out, d2pgo_minimizer_iteration *out);
+
+/* ---- perturbation chart of the 6-DoF solve (d2pgo's perturb_mode, which d2pgo_node sets for every 6-DoF graph,
+ *      d2pgo/src/d2pgo_node.cpp:216)
+ *   d2pgo_set_chart     <- PGOState::addFrame's POSE_PERTURB_6D block (d2pgo/src/pgostate.hpp:25-50, BaseParamResInfo.cpp:4-9)
+ *   d2pgo_get_poses     <- postPerturbSolve (d2pgo/src/d2pgo.cpp:616-628)
+ * In the chart the state of pose f is the Euclidean 6-vector x_f = [p_f, theta_f] (no manifold) and its attitude is
+ *     q_f = q_init,f (x) quatfromRotationVector(theta_f),   quatfromRotationVector(t) = [t / 2, 1] (unnormalised) if |t| < 1e-2,
+ *                                                           else the exact exponential   (utils.hpp:39-55; [x y z w])
+ * The factors are RelPoseFactorPerturbAD (RelPoseFactor.hpp:138-195) and GravityPriorPerturbAD (GravityPrior.hpp:8-46), as
+ * written: p_ab = q_a.conjugate() applied to p_b - p_a by Eigen's _transformVector (not a rotation for a non-unit q_a),
+ * dq = q_meas (q_a.conjugate() q_b).conjugate(), r = S [p_ab - p_meas ; 2 vec(dq)]; the prior's R_a = q_a.toRotationMatrix()
+ * (Eigen's polynomial, exact for unit q only), r = S^T (R_a.row(2) - R_ego.row(2))^T.  The state is kept across solves: each
+ * solve starts from the last [p, theta] (postPerturbSolve leaves theta, its reset being commented out).
+ *   Entering (chart = D2PGO_CHART_PERTURB): every pose gets x = [p, 0] and q_init = its current attitude, normalised, or for the
+ *     listed ids the given q_init4[n][4] (xyzw, normalised here; with q_init4 NULL every pose takes its current attitude and the
+ *     ids, which must still be poses of the handle, select nothing).  Entering again restarts from the current attitudes.
+ *     D2PGO_CHART_RETRACTION leaves it: the poses become d2pgo_get_poses'.
+ *   Fixed poses keep their 6-vector (setStateProperties, d2pgo.cpp:602-610).
+ *   d2pgo_set_poses keeps x and q_init of the ids already present (their given pose is ignored); new ids start as on entry.
+ *     It still removes every edge and gravity prior, as on any handle.  This is how the node's state grows between solves.
+ *   d2pgo_get_poses returns [p, normalise(q_init (x) quatfromRotationVector(theta))] (ASSUMED: Swarm::Pose normalises the
+ *     attitude postPerturbSolve gives it; that type is not in the reference tree).  d2pgo_get_perturb returns the raw state.
+ *   d2pgo_rot_init runs on those attitudes; afterwards every pose's q_init is its attitude: the rotation-initialised one for the
+ *     frames it solves, the current one for the others (recoverRotationLLT, rotation_initialization_base.hpp:360-389); p and
+ *     theta keep every bit.
+ *   d2pgo_debug_edges / d2pgo_debug_gravity_priors / d2pgo_debug_exact_step / d2pgo_debug_pcg_step report and solve in
+ *     [dp, dtheta] of the 6-vector, in the same layouts.
+ *   Both minimisers and both linear solvers run in the chart; only the linearisation and the retraction (x <- x + dx) change.
+ *   ceres LM: the Jacobi scale is of the 6-vector Jacobian's columns, the gradient test max |x - (x + (-g))| and |x| of the
+ *     parameter test run over the free poses' [p, theta] (ASSUMED as for the retraction chart), and the solve's graph is built
+ *     again when the chart changes.
+ *   ARock (d2pgo_arock_*; ARockPGO runs in perturb mode, ARockPGO.cpp:21-23): the dual coordinates are the state x = [p, theta]
+ *     itself (no log map, the ARock q_init of d2pgo_arock_enable is not read), the proximal NormalPrior is
+ *     r = diag(sqrt(rho_T) I3, sqrt(rho_theta) I3) (x - y_r) with that diagonal as its constant Jacobian (ARock.cpp:284-291;
+ *     d2pgo_debug_arock_terms reports it), and updateDualStates acts on x.  An ARock handle enters or leaves the chart only
+ *     while its pose dual table is empty (its duals are coordinates of one chart), and a chart handle refuses the distributed
+ *     rotation initialisation (d2pgo_arock_rot_init_step / d2pgo_arock_rot_receive: 5), which d2pgo runs before the perturbation
+ *     solve: enter the chart after it, and each q_init is the attitude it left.
+ * Not in the chart: 4-DoF handles (d2pgo has no perturbation chart there) and handles with a communicator (the edge-sharded path).
+ * Refusals keep nothing of the call and set d2pgo_last_error: 5 on a 4-DoF handle, with a communicator attached (and
+ * d2pgo_comm_init returns 5 on a chart handle) or on an ARock handle holding duals; 2 on an unknown chart or id, a non-finite value
+ * or a zero q_init (d2pgo_set_poses: a new id's zero quaternion); 1 on a null argument or n < 0.  d2pgo_set_perturb and
+ * d2pgo_get_perturb return 5 on a handle not in the chart. */
+enum { D2PGO_CHART_RETRACTION = 0, D2PGO_CHART_PERTURB = 1 };
+int d2pgo_set_chart(d2pgo_handle *h, int32_t chart, int32_t n, const int64_t *ids, const double *q_init4);
+/* x6[n][6] = [p, theta] of the listed poses */
+int d2pgo_set_perturb(d2pgo_handle *h, int32_t n, const int64_t *ids, const double *x6);
+/* x6_out[n][6] = [p, theta]; q_init4_out[n][4] (may be NULL) their q_init */
+int d2pgo_get_perturb(d2pgo_handle *h, int32_t n, const int64_t *ids, double *x6_out, double *q_init4_out);
 
 #ifdef __cplusplus
 }
