@@ -160,11 +160,6 @@ D2BA_DEV void pgo_gravity_eval(const double *x, const double *ue, const double *
   for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) J[i * 3 + j] = S[i] * K[j] + S[3 + i] * K[3 + j] + S[6 + i] * K[6 + j];
 }
 
-// the perturbation chart's policy (d2pgo_set_chart): pose records [p, theta, 0, 0], the retraction x + dx.  A tag for the host
-// templates only: its factor, prior, proximal, retraction and dual-update kernels live in d2pgo_chart.cu, and every kernel here that reads only D runs
-// its PgoEdge6 instantiation (PgoKern)
-struct PgoChart6 { static constexpr int D = 6; };
-
 // Fixed-order sum of n per-block partials, the same value in every thread of every block (so that all blocks -- and all
 // ranks, which hold identical vectors -- take the same branch without a single-thread "decide" kernel in between).
 D2BA_DEV double total_of(const double *part, int n, double *red) {
@@ -831,6 +826,61 @@ __global__ void k_rotinit_arock_update(int n, const int *pose, const double *rst
   }
 }
 
+// ---- the host policy of each pose parameterisation, picked once per call by with_policy: Kern, the kernel policy of the kernels
+// that read only D; the kernels that linearise, retract and update the ARock duals; the dual coordinates; the ceres minimiser's
+// norms; whether the ARock q_init table holds h->qinit.  The retraction of 6-DoF (K = PgoEdge6) or 4-DoF poses: this file's kernels
+template <class K> struct PgoRetraction {
+  using Kern = K;
+  static constexpr int D = K::D;
+  static constexpr bool arock_qinit = D == 6;   // the 6-DoF dual coordinates [p ; theta] are taken from q_init
+  static constexpr auto xnorm = d2pgo_lm::xnorm;
+  static void lin_edges(const d2pgo_handle *, cudaStream_t st, const PgoDev &d, double *part, int want_jac) { k_pgo_lin<K><<<(d.n_edge + 127) / 128, 128, 0, st>>>(d, part, want_jac); }
+  static void lin_priors(const d2pgo_handle *, cudaStream_t st, const PgoDev &d, const PgoPriorDev &pr, double *part, int want_jac) {
+    k_pgo_prior_lin<<<(pr.n_prior + 127) / 128, 128, 0, st>>>(d, part, want_jac, pr);
+  }
+  static void lin_arock(cudaStream_t st, const PgoDev &d, const PgoArockDev &ak, double *part) { k_pgo_arock_lin<D><<<(ak.n_dual + 127) / 128, 128, 0, st>>>(d, part, ak); }
+  static void retract(cudaStream_t st, const PgoDev &d, double *x_out) { k_pgo_retract<K><<<d.nbp, 128, 0, st>>>(d, x_out); }
+  static void arock_update(cudaStream_t st, const double *x, const PgoArockDev &ak) { k_pgo_arock_update<D><<<(ak.n_dual + 127) / 128, 128, 0, st>>>(x, ak); }
+  static int arock_coords(d2pgo_handle *h, std::vector<double> &out) {
+    const size_t N = h->ids.size();
+    PCK(h->d_ak_coord.alloc(N * D));
+    k_pgo_arock_coord<D><<<(int)((N + 127) / 128), 128, 0, h->stream>>>((int)N, h->d_x[0].p, h->d_ak_qinit.p, h->d_ak_coord.p);
+    PCK(cudaGetLastError());
+    out.resize(N * D);
+    PCK(cudaMemcpyAsync(out.data(), h->d_ak_coord.p, N * D * 8, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaStreamSynchronize(h->stream));
+    return 0;
+  }
+};
+
+// the perturbation chart (d2pgo_set_chart), records [p, theta, 0, 0] with q_init h->d_qinit: the kernels of d2pgo_chart.cu
+struct PgoChart6 {
+  using Kern = PgoEdge6;
+  static constexpr int D = 6;
+  static constexpr bool arock_qinit = true;   // as on every 6-DoF handle, though no chart kernel reads it
+  static constexpr auto xnorm = d2pgo_lm::xnorm_chart;
+  static void lin_edges(const d2pgo_handle *h, cudaStream_t st, const PgoDev &d, double *part, int want_jac) {
+    d2pgo_chart::edges(st, d.n_edge, d.ea, d.eb, d.x, h->d_qinit.p, d.rel, d.sinfo, d.lin, part, want_jac);
+  }
+  static void lin_priors(const d2pgo_handle *h, cudaStream_t st, const PgoDev &d, const PgoPriorDev &pr, double *part, int want_jac) {
+    d2pgo_chart::priors(st, pr.n_prior, pr.pose, pr.u, pr.S, d.x, h->d_qinit.p, pr.lin, part, want_jac);
+  }
+  static void lin_arock(cudaStream_t st, const PgoDev &d, const PgoArockDev &ak, double *part) { d2pgo_chart::arock_lin(st, ak.n_dual, ak.pose, d.x, ak.yr, ak.wT, ak.wR, ak.lin, part); }
+  static void retract(cudaStream_t st, const PgoDev &d, double *x_out) { d2pgo_chart::retract(st, d.n_pose, d.x, d.fixed, d.dx, x_out); }
+  static void arock_update(cudaStream_t st, const double *x, const PgoArockDev &ak) { d2pgo_chart::arock_update(st, ak.n_dual, ak.pose, x, ak.yr, ak.yl, ak.eta); }
+  static int arock_coords(d2pgo_handle *h, std::vector<double> &out) {   // the dual coordinates are the state [p, theta] itself
+    const size_t N = h->ids.size();
+    std::vector<double> x(N * 8);
+    PCK(cudaMemcpyAsync(x.data(), h->d_x[0].p, N * 64, cudaMemcpyDeviceToHost, h->stream));
+    PCK(cudaStreamSynchronize(h->stream));
+    out.resize(N * 6);
+    for (size_t i = 0; i < N; i++) memcpy(&out[i * 6], &x[i * 8], 48);
+    return 0;
+  }
+};
+
+template <class K> constexpr bool kPriorKern = K::D == 6;   // k_pgo_gD and k_pgo_cg_pose have gravity-prior instantiations
+
 }  // namespace
 
 // the 6-DoF and the 4-DoF entry points each serve one kind of handle
@@ -1112,51 +1162,36 @@ static PgoArockDev pgo_arock_view(d2pgo_handle *h, int cur) {
   return a;
 }
 
-// the kernels that only read P::D (gradient, block diagonal, CG) serve both 6-DoF charts: their PgoEdge6 instantiations
-template <class P> using PgoKern = typename std::conditional<std::is_same<P, PgoChart6>::value, PgoEdge6, P>::type;
+template <class F> static int with_policy(d2pgo_handle *h, F &&f) {   // f(the policy of the handle's parameterisation)
+  return h->dof == 4 ? f(PgoRetraction<PgoEdge4>()) : h->chart ? f(PgoChart6()) : f(PgoRetraction<PgoEdge6>());
+}
 
 // cost (+ lin records, gradient, block diagonal of buffer `b`) at pose buffer `b`; all-reduced across the ranks.  grav: the
 // gravity priors of this rank (6-DoF only; their cost partials follow the edges', their terms enter g and D after each pose's
 // edges).  ark: the ARock proximal terms of the synced dual table (cost partials last, g and D after the edges and priors).
 // the kernels of one linearisation of buffer b on stream st, the total cost into *cost_dev
-template <class P>
+template <class H>
 static void pgo_linearize_enqueue(d2pgo_handle *h, cudaStream_t st, int b, int want_jac, bool grav, bool ark, double *cost_dev) {
-  constexpr int D = P::D;
-  constexpr bool chart = std::is_same<P, PgoChart6>::value;
-  using K = PgoKern<P>;
+  using K = typename H::Kern;
   PgoDev d = pgo_view(h, b);
   const PgoPriorDev pr = pgo_prior_view(h, b);
   const PgoArockDev ak = pgo_arock_view(h, b);
   const int nbe = (d.n_edge + 127) / 128, nbg = grav ? (pr.n_prior + 127) / 128 : 0, nbk = ark ? (ak.n_dual + 127) / 128 : 0;
-  if constexpr (chart) {
-    if (d.n_edge > 0) d2pgo_chart::edges(st, d.n_edge, d.ea, d.eb, d.x, h->d_qinit.p, d.rel, d.sinfo, d.lin, h->d_cost_part.p, want_jac);
-    if (nbg > 0) d2pgo_chart::priors(st, pr.n_prior, pr.pose, pr.u, pr.S, d.x, h->d_qinit.p, pr.lin, h->d_cost_part.p + nbe, want_jac);
-  } else {
-    if (d.n_edge > 0) k_pgo_lin<P><<<nbe, 128, 0, st>>>(d, h->d_cost_part.p, want_jac);
-    if (nbg > 0) k_pgo_prior_lin<<<nbg, 128, 0, st>>>(d, h->d_cost_part.p + nbe, want_jac, pr);
-  }
-  if constexpr (chart) {
-    if (nbk > 0) d2pgo_chart::arock_lin(st, ak.n_dual, ak.pose, d.x, ak.yr, ak.wT, ak.wR, ak.lin, h->d_cost_part.p + nbe + nbg);
-  } else if (nbk > 0) k_pgo_arock_lin<D><<<nbk, 128, 0, st>>>(d, h->d_cost_part.p + nbe + nbg, ak);
+  if (d.n_edge > 0) H::lin_edges(h, st, d, h->d_cost_part.p, want_jac);
+  if (nbg > 0) H::lin_priors(h, st, d, pr, h->d_cost_part.p + nbe, want_jac);
+  if (nbk > 0) H::lin_arock(st, d, ak, h->d_cost_part.p + nbe + nbg);
   k_pgo_sum<<<1, 128, 0, st>>>(h->d_cost_part.p, nbe + nbg + nbk, cost_dev);
   if (want_jac && grav) {
-    if constexpr (D == 6) k_pgo_gD<K, true><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
+    if constexpr (kPriorKern<K>) k_pgo_gD<K, true><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
   } else if (want_jac) k_pgo_gD<K, false><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, pr);
-  if (want_jac && nbk > 0) k_pgo_arock_gD<D><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, ak);
+  if (want_jac && nbk > 0) k_pgo_arock_gD<H::D><<<d.nbp, 128, 0, st>>>(d, h->d_g[b].p, h->d_D[b].p, ak);
 }
 
-// candidate poses x (+) dx of linearisation view d into x_out
-template <class P>
-static void pgo_retract_enqueue(cudaStream_t st, const PgoDev &d, double *x_out) {
-  if constexpr (std::is_same<P, PgoChart6>::value) d2pgo_chart::retract(st, d.n_pose, d.x, d.fixed, d.dx, x_out);
-  else k_pgo_retract<P><<<d.nbp, 128, 0, st>>>(d, x_out);
-}
-
-template <class P>
+template <class H>
 static int pgo_linearize(d2pgo_handle *h, int b, int want_jac, bool grav, bool ark, double *cost) {
-  constexpr int D = P::D;
+  constexpr int D = H::D;
   const size_t N = h->ids.size();
-  pgo_linearize_enqueue<P>(h, h->stream, b, want_jac, grav, ark, h->d_cost.p);
+  pgo_linearize_enqueue<H>(h, h->stream, b, want_jac, grav, ark, h->d_cost.p);
   if (h->comm) {
     if (nccl_allreduce_f64(h->comm, h->d_cost.p, 1, h->stream)) { h->err = "ncclAllReduce(cost) failed"; return 40; }
     if (want_jac && (nccl_allreduce_f64(h->comm, h->d_g[b].p, N * D, h->stream) || nccl_allreduce_f64(h->comm, h->d_D[b].p, N * D * D, h->stream))) { h->err = "ncclAllReduce(g, D) failed"; return 40; }
@@ -1171,7 +1206,7 @@ constexpr int kCgChunk = 16;   // CG iterations between two looks at the converg
 // the pose pass of one CG iteration, with the gravity priors' terms when grav (6-DoF only)
 template <class P, bool LOCAL>
 static void pgo_cg_pose(d2pgo_handle *h, const PgoDev &d, int par, double tol2, const PgoPriorDev &pr, bool grav) {
-  if constexpr (P::D == 6) {
+  if constexpr (kPriorKern<P>) {
     if (grav) { k_pgo_cg_pose<P, LOCAL, true><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr); return; }
   }
   k_pgo_cg_pose<P, LOCAL, false><<<d.nbp, 128, 0, h->stream>>>(d, par, tol2, pr);
@@ -1281,9 +1316,9 @@ static int pgo_chol_step(d2pgo_handle *h, int cur, double lambda, bool *failed) 
   return c.step(h->stream, cur, in, lambda, failed, h->err);
 }
 
-// the LM loop, shared by both pose parameterisations (P = PgoEdge6 / PgoEdge4), with the handle's gravity priors and, when
-// ark, the ARock proximal terms of the synced dual table
-template <class P>
+// the LM loop in the pose parameterisation H, with the handle's gravity priors and, when ark, the ARock proximal terms of the
+// synced dual table
+template <class H>
 static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   int rc;
   const bool chol = h->linear_solver == D2PGO_LINEAR_SPARSE_CHOLESKY, grav = !h->gp_pose.empty();
@@ -1297,7 +1332,7 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   PCK(cudaEventRecord(h->ev0, h->stream));
   int cur = 0;                    // buffer (poses, lin records, g, D) of the accepted point
   double cost = 0, lambda = h->cfg.lambda0;
-  if ((rc = pgo_linearize<P>(h, cur, 1, grav, ark, &cost))) return rc;
+  if ((rc = pgo_linearize<H>(h, cur, 1, grav, ark, &cost))) return rc;
   R.initial_cost = cost;
   const double tol2 = h->cfg.pcg_tolerance * h->cfg.pcg_tolerance;
   for (int it = 0; it < h->cfg.max_iterations; it++) {
@@ -1311,11 +1346,10 @@ static int pgo_solve(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
         if (lambda > 1e8) break;
         continue;
       }
-    } else if ((rc = pgo_pcg<PgoKern<P>>(h, cur, lambda, tol2, h->cfg.pcg_max_iterations, grav, ark, &s))) return rc;
-    const PgoDev d = pgo_view(h, cur);
-    pgo_retract_enqueue<P>(h->stream, d, h->d_x[1 - cur].p);
+    } else if ((rc = pgo_pcg<typename H::Kern>(h, cur, lambda, tol2, h->cfg.pcg_max_iterations, grav, ark, &s))) return rc;
+    H::retract(h->stream, pgo_view(h, cur), h->d_x[1 - cur].p);
     double cand = 0;
-    if ((rc = pgo_linearize<P>(h, 1 - cur, 1, grav, ark, &cand))) return rc;
+    if ((rc = pgo_linearize<H>(h, 1 - cur, 1, grav, ark, &cand))) return rc;
     R.pcg_iterations += s.iters; R.iterations++;
     if (cand < cost && isfinite(cand)) {
       const double rel_dec = (cost - cand) / (cost > 0 ? cost : 1.0);
@@ -1372,15 +1406,14 @@ static cudaError_t lm_cond(cudaStream_t st, cudaGraphConditionalHandle c, cudaGr
   return cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies);
 }
 
-template <class P>
+template <class H>
 static int lm_build(d2pgo_handle *h, bool grav, bool ark, cudaStream_t *cs) {
-  constexpr int D = P::D;
   const PgoDev d0 = pgo_view(h, 0), d1 = pgo_view(h, 1);
   const PgoPriorDev pr = pgo_prior_view(h, 0);
   const PgoArockDev ak = pgo_arock_view(h, 0);
   const int nbp = d0.nbp, nbe = (d0.n_edge + 127) / 128, nbg = grav ? (pr.n_prior + 127) / 128 : 0, nbk = ark ? (ak.n_dual + 127) / 128 : 0;
   const int nbm = nbe + nbg + nbk + nbp;
-  const d2pgo_lm::View v{D, d0.n_pose, d0.n_edge, grav ? pr.n_prior : 0, ark ? ak.n_dual : 0, d0.x, h->d_g[0].p, d0.dx, d0.lin, pr.lin, ak.lin,
+  const d2pgo_lm::View v{H::D, d0.n_pose, d0.n_edge, grav ? pr.n_prior : 0, ark ? ak.n_dual : 0, d0.x, h->d_g[0].p, d0.dx, d0.lin, pr.lin, ak.lin,
                          d0.fixed, d0.ea, d0.eb, pr.pose, ak.pose};
   LmState *s = h->d_lm.p;
   double *xpart = h->d_lm_part.p, *mpart = xpart + 2 * (size_t)nbp, *cost = h->d_cost.p;
@@ -1395,11 +1428,9 @@ static int lm_build(d2pgo_handle *h, bool grav, bool ark, cudaStream_t *cs) {
   PCK(cudaGraphConditionalHandleCreate(&loop, top, 1, cudaGraphCondAssignDefault));
   PCK(cudaStreamBeginCaptureToGraph(cs[0], top, nullptr, nullptr, 0, mode));
   d2pgo_lm::start(cs[0], s);
-  pgo_linearize_enqueue<P>(h, cs[0], 0, 1, grav, ark, cost);
+  pgo_linearize_enqueue<H>(h, cs[0], 0, 1, grav, ark, cost);
   d2pgo_lm::scale(cs[0], v, h->d_D[0].p, s, h->d_lm_scale.p);
-  // the gradient and parameter tests' norms: of the ambient 7-vectors, or of the chart's Euclidean 6-vectors
-  const auto xnorm = std::is_same<P, PgoChart6>::value ? d2pgo_lm::xnorm_chart : d2pgo_lm::xnorm;
-  xnorm(cs[0], v, xpart);
+  H::xnorm(cs[0], v, xpart);
   PCK(lm_cond(cs[0], loop, cudaGraphCondTypeWhile, &body));
   PCK(cudaStreamEndCapture(cs[0], &top));
   PCK(cudaGraphConditionalHandleCreate(&go, body, 0, 0));
@@ -1418,13 +1449,13 @@ static int lm_build(d2pgo_handle *h, bool grav, bool ark, cudaStream_t *cs) {
   PCK(lm_cond(cs[2], acc, cudaGraphCondTypeIf, &acc_g));
   PCK(cudaStreamEndCapture(cs[2], &go_g));
   PCK(cudaStreamBeginCaptureToGraph(cs[3], eval_g, nullptr, nullptr, 0, mode));
-  pgo_retract_enqueue<P>(cs[3], d0, h->d_x[1].p);
-  pgo_linearize_enqueue<P>(h, cs[3], 1, 0, grav, ark, cost + 1);
+  H::retract(cs[3], d0, h->d_x[1].p);
+  pgo_linearize_enqueue<H>(h, cs[3], 1, 0, grav, ark, cost + 1);
   PCK(cudaStreamEndCapture(cs[3], &eval_g));
   PCK(cudaStreamBeginCaptureToGraph(cs[3], acc_g, nullptr, nullptr, 0, mode));
   PCK(cudaMemcpyAsync(h->d_x[0].p, d1.x, (size_t)d0.n_pose * 64, cudaMemcpyDeviceToDevice, cs[3]));
-  pgo_linearize_enqueue<P>(h, cs[3], 0, 1, grav, ark, cost);
-  xnorm(cs[3], v, xpart);
+  pgo_linearize_enqueue<H>(h, cs[3], 0, 1, grav, ark, cost);
+  H::xnorm(cs[3], v, xpart);
   PCK(cudaStreamEndCapture(cs[3], &acc_g));
   PCK(cudaGetLastError());
   if (h->lm_graph) { cudaGraphExecDestroy(h->lm_graph); h->lm_graph = nullptr; }
@@ -1435,7 +1466,7 @@ static int lm_build(d2pgo_handle *h, bool grav, bool ark, cudaStream_t *cs) {
 constexpr int kLmTraceCap = 16384;   // trace records kept per solve (the first iterations)
 
 // ceres' TrustRegionMinimizer with LevenbergMarquardtStrategy (d2pgo_set_minimizer): one graph launch, one synchronisation
-template <class P>
+template <class H>
 static int pgo_solve_ceres(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   int rc, syncs = 1;
   if ((rc = pgo_chol_prepare(h))) return rc;
@@ -1443,7 +1474,7 @@ static int pgo_solve_ceres(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   if (!h->chol->dev_ready) { if ((rc = h->chol->upload(h->stream, h->err))) return rc; syncs++; }
   const bool grav = !h->gp_pose.empty();
   const d2pgo_ceres_lm_config &c = h->lm_cfg;
-  const int N = (int)h->ids.size(), D = P::D, nbp = (N + 127) / 128;
+  const int N = (int)h->ids.size(), D = H::D, nbp = (N + 127) / 128;
   const int nbm = (int)(h->ea.size() + 127) / 128 + (grav ? (int)(h->gp_pose.size() + 127) / 128 : 0) + (ark ? (std::max(h->ak_n, 0) + 127) / 128 : 0) + nbp;
   const int cap = std::max(1, std::min(c.max_num_iterations, kLmTraceCap));
   PCK(h->d_lm.alloc(1)); PCK(h->d_lm_scale.alloc((size_t)N * D)); PCK(h->d_lm_part.alloc(2 * (size_t)nbp + 3 * (size_t)nbm));
@@ -1461,7 +1492,7 @@ static int pgo_solve_ceres(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   if (!h->lm_graph || h->lm_key != key) {
     cudaStream_t cs[4] = {h->stream, nullptr, nullptr, nullptr};
     for (int k = 1; k < 4; k++) PCK(cudaStreamCreateWithFlags(&cs[k], cudaStreamNonBlocking));
-    rc = lm_build<P>(h, grav, ark, cs);
+    rc = lm_build<H>(h, grav, ark, cs);
     for (int k = 1; k < 4; k++) cudaStreamDestroy(cs[k]);
     if (rc) { h->lm_key.clear(); return rc; }
     h->lm_key = key;
@@ -1494,10 +1525,10 @@ static int pgo_solve_ceres(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
 }
 
 // the handle's minimiser (d2pgo_set_minimizer); its refusals (lm_refuse) come before any state changes, in the callers
-template <class P>
+template <class H>
 static int pgo_minimize(d2pgo_handle *h, d2pgo_report *rep, bool ark) {
   h->lm_ran = false;
-  return h->minimizer == D2PGO_MINIMIZER_CERES_LM ? pgo_solve_ceres<P>(h, rep, ark) : pgo_solve<P>(h, rep, ark);
+  return h->minimizer == D2PGO_MINIMIZER_CERES_LM ? pgo_solve_ceres<H>(h, rep, ark) : pgo_solve<H>(h, rep, ark);
 }
 
 extern "C" {
@@ -1506,8 +1537,7 @@ int d2pgo_solve(d2pgo_handle *h, d2pgo_report *rep) {
   if (!h || h->ids.empty()) return 1;
   if (int rc = lm_refuse(h, "solve")) return rc;
   cudaSetDevice(h->cfg.device);
-  if (h->dof == 4) return pgo_minimize<PgoEdge4>(h, rep, false);
-  return h->chart ? pgo_minimize<PgoChart6>(h, rep, false) : pgo_minimize<PgoEdge6>(h, rep, false);
+  return with_policy(h, [&](auto pol) { return pgo_minimize<decltype(pol)>(h, rep, false); });
 }
 
 int d2pgo_get_poses(d2pgo_handle *h, int32_t n, const int64_t *ids, double *out) {
@@ -1531,9 +1561,7 @@ int d2pgo_debug_edges(d2pgo_handle *h, double *out, int64_t out_doubles) {
   const size_t E = h->ea.size(), W = (size_t)h->dof + 2 * (size_t)h->dof * h->dof;   // 78 (6-DoF) or 36 (4-DoF) per edge
   if ((size_t)out_doubles < E * W) { h->err = "debug_edges: buffer too small"; return 2; }
   double cost;
-  if ((rc = h->dof == 4 ? pgo_linearize<PgoEdge4>(h, 0, 1, false, false, &cost)
-            : h->chart  ? pgo_linearize<PgoChart6>(h, 0, 1, false, false, &cost)
-                        : pgo_linearize<PgoEdge6>(h, 0, 1, false, false, &cost))) return rc;
+  if ((rc = with_policy(h, [&](auto pol) { return pgo_linearize<decltype(pol)>(h, 0, 1, false, false, &cost); }))) return rc;
   std::vector<double> tmp(E * W);
   PCK(cudaMemcpyAsync(tmp.data(), h->d_lin[0].p, E * W * 8, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
@@ -1589,7 +1617,7 @@ int d2pgo_debug_gravity_priors(d2pgo_handle *h, double *out, int64_t out_doubles
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
   double cost;
-  if ((rc = h->chart ? pgo_linearize<PgoChart6>(h, 0, 1, true, false, &cost) : pgo_linearize<PgoEdge6>(h, 0, 1, true, false, &cost))) return rc;
+  if ((rc = with_policy(h, [&](auto pol) { return pgo_linearize<decltype(pol)>(h, 0, 1, true, false, &cost); }))) return rc;
   std::vector<double> tmp(G * 12);
   PCK(cudaMemcpyAsync(tmp.data(), h->d_glin[0].p, G * 12 * 8, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
@@ -1691,9 +1719,10 @@ static int arock_export(d2pgo_handle *h, const ArockTable<W> &t, const char *wha
 }
 
 // the dual table, in table order, to the device: pose of each dual, the pose -> duals CSR, y_r, y_l, q_init
+template <class H>
 static int arock_sync(d2pgo_handle *h) {
   const auto &duals = h->pose_table.duals;
-  const size_t N = h->ids.size(), K = duals.size(), D = h->dof;
+  const size_t N = h->ids.size(), K = duals.size(), D = H::D;
   std::vector<int> pose(K), ptr(N + 1, 0), of(K);
   std::vector<double> yr(K * D), yl(K * D), qi(N * 4, 0.0);
   size_t k = 0;
@@ -1702,7 +1731,7 @@ static int arock_sync(d2pgo_handle *h) {
   for (size_t i = 0; i < N; i++) ptr[i + 1] += ptr[i];
   { std::vector<int> fill(ptr.begin(), ptr.end() - 1);
     for (size_t j = 0; j < K; j++) of[fill[pose[j]]++] = (int)j; }
-  if (D == 6) for (size_t i = 0; i < N; i++) memcpy(&qi[i * 4], h->qinit.at(h->ids[i]).data(), 32);
+  if (H::arock_qinit) for (size_t i = 0; i < N; i++) memcpy(&qi[i * 4], h->qinit.at(h->ids[i]).data(), 32);
   PCK(h->d_ak_pose.alloc(K)); PCK(h->d_ak_of.alloc(K)); PCK(h->d_ak_ptr.alloc(N + 1)); PCK(h->d_ak_yr.alloc(K * D)); PCK(h->d_ak_yl.alloc(K * D));
   PCK(h->d_ak_qinit.alloc(N * 4)); PCK(h->d_ak_lin[0].alloc(K * (D + D * D))); PCK(h->d_ak_lin[1].alloc(K * (D + D * D)));
   if (K) {
@@ -1716,28 +1745,6 @@ static int arock_sync(d2pgo_handle *h) {
   PCK(cudaStreamSynchronize(h->stream));
   h->ak_n = (int)K;
   return pgo_alloc_cost_part(h);
-}
-
-// every pose at d_x[0] in dual coordinates, [N][D] on the host
-static int arock_coords(d2pgo_handle *h, std::vector<double> &out) {
-  const size_t N = h->ids.size(), D = h->dof;
-  if (h->chart) {   // the chart's dual coordinates are the state [p, theta] itself
-    std::vector<double> x(N * 8);
-    PCK(cudaMemcpyAsync(x.data(), h->d_x[0].p, N * 64, cudaMemcpyDeviceToHost, h->stream));
-    PCK(cudaStreamSynchronize(h->stream));
-    out.resize(N * 6);
-    for (size_t i = 0; i < N; i++) memcpy(&out[i * 6], &x[i * 8], 48);
-    return 0;
-  }
-  PCK(h->d_ak_coord.alloc(N * D));
-  const int nb = (int)((N + 127) / 128);
-  if (D == 6) k_pgo_arock_coord<6><<<nb, 128, 0, h->stream>>>((int)N, h->d_x[0].p, h->d_ak_qinit.p, h->d_ak_coord.p);
-  else k_pgo_arock_coord<4><<<nb, 128, 0, h->stream>>>((int)N, h->d_x[0].p, h->d_ak_qinit.p, h->d_ak_coord.p);
-  PCK(cudaGetLastError());
-  out.resize(N * D);
-  PCK(cudaMemcpyAsync(out.data(), h->d_ak_coord.p, N * D * 8, cudaMemcpyDeviceToHost, h->stream));
-  PCK(cudaStreamSynchronize(h->stream));
-  return 0;
 }
 
 // every pose needs an owner (and, 6-DoF, a q_init) before the table can be built
@@ -1770,12 +1777,8 @@ int d2pgo_arock_enable(d2pgo_handle *h, const d2pgo_arock_config *cfg, int32_t n
     auto it = h->index.find(ids[k]);
     if (it == h->index.end()) return pgo_fail(h, 2, "arock_enable: unknown pose id " + std::to_string(ids[k]));
     const double *src = q_init4 ? q_init4 + (size_t)k * 4 : h->chart ? &h->chart_qinit[(size_t)it->second * 4] : &h->poses[(size_t)it->second * 8 + 3];
-    if (h->dof == 6) {
-      const double s2 = src[0] * src[0] + src[1] * src[1] + src[2] * src[2] + src[3] * src[3];
-      if (!all_finite(src, 4) || !(s2 > 0.0)) return pgo_fail(h, 2, "arock_enable: pose id " + std::to_string(ids[k]) + ": non-finite or zero q_init");
-      const double s = 1.0 / std::sqrt(s2);
-      q[k] = {src[0] * s, src[1] * s, src[2] * s, src[3] * s};
-    }
+    if (h->dof == 6 && !chart_unit(src, q[k].data()))
+      return pgo_fail(h, 2, "arock_enable: pose id " + std::to_string(ids[k]) + ": non-finite or zero q_init");
   }
   h->arock = true; h->acfg = *cfg;
   for (int k = 0; k < n; k++) { h->owner[ids[k]] = owner[k]; if (h->dof == 6) h->qinit[ids[k]] = q[k]; }
@@ -1797,46 +1800,46 @@ int d2pgo_arock_step(d2pgo_handle *h, d2pgo_report *rep) {
   if (int rc = arock_check_poses(h, "arock_step")) return rc;
   if (int rc = lm_refuse(h, "arock_step")) return rc;
   cudaSetDevice(h->cfg.device);
-  int rc;
-  if (!h->uploaded && (rc = pgo_upload(h))) return rc;
-  const int D = h->dof, self = h->acfg.self_id;
-  const std::vector<char> in = arock_in_problem(h);
-  auto &duals = h->pose_table.duals;
-  // 1. receiveAll / processPGOData, on the live table
-  arock_apply_inbox(h, h->pose_table, in, D, duals);
-  h->pose_table.inbox.clear();
-  // 2. scanAndCreateDualStates (ARock.cpp:192-208): a dual for every frame of another agent, from x(f) or zero.  The q_init
-  // table goes to the device first (arock_sync) so that the coordinates can be taken there.
-  if ((rc = arock_sync(h))) return rc;
-  std::vector<double> coord;
-  if (!h->acfg.dual_state_init_to_zero && (rc = arock_coords(h, coord))) return rc;
-  bool created = false;
-  for (size_t i = 0; i < h->ids.size(); i++) {
-    const int32_t o = h->owner.at(h->ids[i]);
-    if (!in[i] || o == self) continue;
-    const auto key = std::make_pair(o, h->ids[i]);
-    if (duals.count(key)) continue;
-    d2pgo_host::ArockDual<6> nd; memset(&nd, 0, sizeof nd);
-    if (!h->acfg.dual_state_init_to_zero) { memcpy(nd.yl, &coord[i * D], D * 8); memcpy(nd.yr, &coord[i * D], D * 8); }
-    duals.emplace(key, nd); created = true;
-  }
-  // 3. setDualStateFactors + solveLocalStep: the LM solve with the proximal terms towards y_r
-  if (created && (rc = arock_sync(h))) return rc;
-  if ((rc = D == 4 ? pgo_minimize<PgoEdge4>(h, rep, true) : h->chart ? pgo_minimize<PgoChart6>(h, rep, true) : pgo_minimize<PgoEdge6>(h, rep, true))) return rc;
-  // 4. updateDualStates at the solved poses, which pgo_solve leaves in buffer 0
-  const PgoArockDev ak = pgo_arock_view(h, 0);
-  if (ak.n_dual > 0) {
-    const int nb = (ak.n_dual + 127) / 128;
-    if (h->chart) d2pgo_chart::arock_update(h->stream, ak.n_dual, ak.pose, h->d_x[0].p, ak.yr, ak.yl, ak.eta);
-    else if (D == 6) k_pgo_arock_update<6><<<nb, 128, 0, h->stream>>>(h->d_x[0].p, ak);
-    else k_pgo_arock_update<4><<<nb, 128, 0, h->stream>>>(h->d_x[0].p, ak);
-    PCK(cudaGetLastError());
-    std::vector<double> yl((size_t)ak.n_dual * D);
-    PCK(cudaMemcpyAsync(yl.data(), h->d_ak_yl.p, yl.size() * 8, cudaMemcpyDeviceToHost, h->stream));
-    PCK(cudaStreamSynchronize(h->stream));
-    arock_set_yl(duals, D, yl.data());
-  }
-  return 0;
+  return with_policy(h, [&](auto pol) -> int {   // one policy for the dual coordinates, the solve and the dual update
+    using H = decltype(pol);
+    int rc;
+    if (!h->uploaded && (rc = pgo_upload(h))) return rc;
+    const int D = H::D, self = h->acfg.self_id;
+    const std::vector<char> in = arock_in_problem(h);
+    auto &duals = h->pose_table.duals;
+    // 1. receiveAll / processPGOData, on the live table
+    arock_apply_inbox(h, h->pose_table, in, D, duals);
+    h->pose_table.inbox.clear();
+    // 2. scanAndCreateDualStates (ARock.cpp:192-208): a dual for every frame of another agent, from x(f) or zero.  The q_init
+    // table goes to the device first (arock_sync) so that the coordinates can be taken there.
+    if ((rc = arock_sync<H>(h))) return rc;
+    std::vector<double> coord;
+    if (!h->acfg.dual_state_init_to_zero && (rc = H::arock_coords(h, coord))) return rc;
+    bool created = false;
+    for (size_t i = 0; i < h->ids.size(); i++) {
+      const int32_t o = h->owner.at(h->ids[i]);
+      if (!in[i] || o == self) continue;
+      const auto key = std::make_pair(o, h->ids[i]);
+      if (duals.count(key)) continue;
+      d2pgo_host::ArockDual<6> nd; memset(&nd, 0, sizeof nd);
+      if (!h->acfg.dual_state_init_to_zero) { memcpy(nd.yl, &coord[i * D], D * 8); memcpy(nd.yr, &coord[i * D], D * 8); }
+      duals.emplace(key, nd); created = true;
+    }
+    // 3. setDualStateFactors + solveLocalStep: the LM solve with the proximal terms towards y_r
+    if (created && (rc = arock_sync<H>(h))) return rc;
+    if ((rc = pgo_minimize<H>(h, rep, true))) return rc;
+    // 4. updateDualStates at the solved poses, which pgo_solve leaves in buffer 0
+    const PgoArockDev ak = pgo_arock_view(h, 0);
+    if (ak.n_dual > 0) {
+      H::arock_update(h->stream, h->d_x[0].p, ak);
+      PCK(cudaGetLastError());
+      std::vector<double> yl((size_t)ak.n_dual * D);
+      PCK(cudaMemcpyAsync(yl.data(), h->d_ak_yl.p, yl.size() * 8, cudaMemcpyDeviceToHost, h->stream));
+      PCK(cudaStreamSynchronize(h->stream));
+      arock_set_yl(duals, D, yl.data());
+    }
+    return 0;
+  });
 }
 
 int d2pgo_arock_neighbours(d2pgo_handle *h, int32_t max_n, int32_t *n_out, int32_t *ids_out) {
@@ -1861,16 +1864,15 @@ int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
   cudaSetDevice(h->cfg.device);
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
-  if ((rc = arock_sync(h))) return rc;
-  const PgoDev d = pgo_view(h, 0);
-  const PgoArockDev ak = pgo_arock_view(h, 0);
-  const int nb = (int)((K + 127) / 128);
-  if (h->chart) d2pgo_chart::arock_lin(h->stream, ak.n_dual, ak.pose, d.x, ak.yr, ak.wT, ak.wR, ak.lin, h->d_cost_part.p);
-  else if (D == 6) k_pgo_arock_lin<6><<<nb, 128, 0, h->stream>>>(d, h->d_cost_part.p, ak);
-  else k_pgo_arock_lin<4><<<nb, 128, 0, h->stream>>>(d, h->d_cost_part.p, ak);
+  if ((rc = with_policy(h, [h](auto pol) {
+        using H = decltype(pol);
+        if (int e = arock_sync<H>(h)) return e;
+        H::lin_arock(h->stream, pgo_view(h, 0), pgo_arock_view(h, 0), h->d_cost_part.p);
+        return 0;
+      }))) return rc;
   PCK(cudaGetLastError());
   std::vector<double> tmp(K * W);
-  PCK(cudaMemcpyAsync(tmp.data(), ak.lin, K * W * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaMemcpyAsync(tmp.data(), h->d_ak_lin[0].p, K * W * 8, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
   for (size_t k = 0; k < K; k++) for (size_t q = 0; q < W; q++) out[k * W + q] = tmp[q * K + k];   // device layout is field-major
   return 0;
@@ -1879,17 +1881,17 @@ int d2pgo_debug_arock_terms(d2pgo_handle *h, double *out, int64_t out_doubles) {
 }  // extern "C"
 
 // ---- sparse Cholesky (d2pgo_set_linear_solver) host side
-template <class P>
+template <class H>
 static int pgo_exact_step(d2pgo_handle *h, double lambda, bool ark, double *out) {
   int rc;
   if ((rc = pgo_chol_prepare(h))) return rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
-  if (ark && (rc = arock_sync(h))) return rc;
+  if (ark && (rc = arock_sync<H>(h))) return rc;
   double cost;
-  if ((rc = pgo_linearize<P>(h, 0, 1, !h->gp_pose.empty(), ark, &cost))) return rc;
+  if ((rc = pgo_linearize<H>(h, 0, 1, !h->gp_pose.empty(), ark, &cost))) return rc;
   bool failed = false;
   if ((rc = pgo_chol_step(h, 0, lambda, &failed))) return rc;
-  PCK(cudaMemcpyAsync(out, h->d_dx.p, h->ids.size() * (size_t)P::D * 8, cudaMemcpyDeviceToHost, h->stream));
+  PCK(cudaMemcpyAsync(out, h->d_dx.p, h->ids.size() * (size_t)H::D * 8, cudaMemcpyDeviceToHost, h->stream));
   PCK(cudaStreamSynchronize(h->stream));
   if (failed) { h->err = "debug_exact_step: the factorisation met a non-positive or non-finite pivot"; return 6; }
   return 0;
@@ -1914,17 +1916,17 @@ static int pcg_last_residual(d2pgo_handle *h, int32_t *iters, double *residual) 
 }
 
 // one PCG step of d2pgo_solve at the current poses (buffer 0), its iteration count and last relative residual
-template <class P>
+template <class H>
 static int pgo_pcg_step(d2pgo_handle *h, double lambda, int max_it, double tol, bool ark, double *out, int32_t *iters, double *residual) {
   int rc;
   if (!h->uploaded && (rc = pgo_upload(h))) return rc;
-  if (ark && (rc = arock_sync(h))) return rc;
+  if (ark && (rc = arock_sync<H>(h))) return rc;
   const bool grav = !h->gp_pose.empty();
   double cost;
-  if ((rc = pgo_linearize<P>(h, 0, 1, grav, ark, &cost))) return rc;
+  if ((rc = pgo_linearize<H>(h, 0, 1, grav, ark, &cost))) return rc;
   PgoScalars s; memset(&s, 0, sizeof s);
-  if ((rc = pgo_pcg<PgoKern<P>>(h, 0, lambda, tol * tol, max_it, grav, ark, &s))) return rc;
-  PCK(cudaMemcpyAsync(out, h->d_dx.p, h->ids.size() * (size_t)P::D * 8, cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = pgo_pcg<typename H::Kern>(h, 0, lambda, tol * tol, max_it, grav, ark, &s))) return rc;
+  PCK(cudaMemcpyAsync(out, h->d_dx.p, h->ids.size() * (size_t)H::D * 8, cudaMemcpyDeviceToHost, h->stream));
   return pcg_last_residual(h, iters, residual);
 }
 
@@ -1968,8 +1970,7 @@ int d2pgo_debug_exact_step(d2pgo_handle *h, double lambda, double *dx_out, int64
   if (h->comm) { h->err = "debug_exact_step: the handle has a communicator"; return 5; }
   if (h->arock) if (int rc = arock_check_poses(h, "debug_exact_step")) return rc;
   cudaSetDevice(h->cfg.device);
-  if (h->dof == 4) return pgo_exact_step<PgoEdge4>(h, lambda, h->arock, dx_out);
-  return h->chart ? pgo_exact_step<PgoChart6>(h, lambda, h->arock, dx_out) : pgo_exact_step<PgoEdge6>(h, lambda, h->arock, dx_out);
+  return with_policy(h, [&](auto pol) { return pgo_exact_step<decltype(pol)>(h, lambda, h->arock, dx_out); });
 }
 
 int d2pgo_debug_pcg_step(d2pgo_handle *h, double lambda, int32_t max_it, double tol, double *dx_out, int64_t out_doubles,
@@ -1984,9 +1985,7 @@ int d2pgo_debug_pcg_step(d2pgo_handle *h, double lambda, int32_t max_it, double 
   if (h->comm) { h->err = "debug_pcg_step: the handle has a communicator"; return 5; }
   if (h->arock) if (int rc = arock_check_poses(h, "debug_pcg_step")) return rc;
   cudaSetDevice(h->cfg.device);
-  if (h->dof == 4) return pgo_pcg_step<PgoEdge4>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out);
-  return h->chart ? pgo_pcg_step<PgoChart6>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out)
-                  : pgo_pcg_step<PgoEdge6>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out);
+  return with_policy(h, [&](auto pol) { return pgo_pcg_step<decltype(pol)>(h, lambda, max_it, tol, h->arock, dx_out, iters_out, residual_out); });
 }
 
 int d2pgo_debug_cholesky_system(d2pgo_handle *h, double *diag_out, double *b_out, int32_t max_pairs, int32_t *n_pairs_out,

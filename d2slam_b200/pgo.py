@@ -192,6 +192,11 @@ class PgoSolver:
         if linear_solver != "pcg":
             self.set_linear_solver(linear_solver)
 
+    @property
+    def dim(self):
+        """The size D of a pose's tangent: 4 with pose_dof = 4, else 6."""
+        return 4 if self.cfg.pose_dof == 4 else 6
+
     def set_linear_solver(self, kind):
         """"pcg" (the default) or "sparse_cholesky" (include/d2pgo.h d2pgo_set_linear_solver); ints pass through."""
         k = LINEAR_SOLVERS.get(kind, kind) if isinstance(kind, str) else int(kind)
@@ -207,16 +212,14 @@ class PgoSolver:
 
     def debug_exact_step(self, lam):
         """The sparse Cholesky's step dx [N, D] for damping lam at the current poses (0 on fixed poses); poses unchanged."""
-        D = 4 if self.cfg.pose_dof == 4 else 6
-        out = np.zeros((self.n_poses, D))
+        out = np.zeros((self.n_poses, self.dim))
         self._chk(_lib().d2pgo_debug_exact_step(self.h, C.c_double(lam), _p(out), C.c_int64(out.size)), "debug_exact_step")
         return out
 
     def debug_pcg_step(self, lam, max_iterations, tolerance):
         """One PCG step (the default linear solver) for damping lam at the current poses, at most max_iterations iterations to
         relative residual tolerance: (dx [N, D] (0 on fixed poses), iterations run, the last relative residual); poses unchanged."""
-        D = 4 if self.cfg.pose_dof == 4 else 6
-        out = np.zeros((self.n_poses, D)); it = C.c_int32(); res = C.c_double()
+        out = np.zeros((self.n_poses, self.dim)); it = C.c_int32(); res = C.c_double()
         self._chk(_lib().d2pgo_debug_pcg_step(self.h, C.c_double(lam), C.c_int32(max_iterations), C.c_double(tolerance), _p(out),
                                               C.c_int64(out.size), C.byref(it), C.byref(res)), "debug_pcg_step")
         return out, it.value, res.value
@@ -225,7 +228,7 @@ class PgoSolver:
         """The system the last sparse-Cholesky step on this handle factored, as the device assembled it (include/d2pgo.h
         d2pgo_debug_cholesky_system): dict(diag [N, D, D] damped diagonal blocks, b [N, D] = -g (both 0 on fixed poses),
         pairs [P, 2] pose indices a < b of each distinct free pair, pair_blocks [P, D, D] H_ab)."""
-        D = 4 if self.cfg.pose_dof == 4 else 6
+        D = self.dim
         P = self.cholesky_stats()["block_pairs"]
         diag = np.zeros((self.n_poses, D, D)); b = np.zeros((self.n_poses, D))
         ab = np.zeros((max(P, 1), 2), np.int32); H = np.zeros((max(P, 1), D, D)); n = C.c_int32()
@@ -386,7 +389,8 @@ class PgoSolver:
 
     def debug_edges(self):
         """Per local edge: r | J_a | J_b at the current poses, 78 doubles (6-DoF) or 36 (pose_dof = 4)."""
-        out = np.zeros((max(self.n_edges, 1), 36 if self.cfg.pose_dof == 4 else 78))
+        D = self.dim
+        out = np.zeros((max(self.n_edges, 1), D + 2 * D * D))
         self._chk(_lib().d2pgo_debug_edges(self.h, _p(out), C.c_int64(out.size)), "debug_edges")
         return out[: self.n_edges]
 
@@ -455,10 +459,6 @@ class PgoSolver:
         return member[:n].astype(bool), size.value
 
     # ---- ARock (include/d2pgo.h d2pgo_arock_*)
-    @property
-    def dim(self):
-        return 4 if self.cfg.pose_dof == 4 else 6
-
     def arock_enable(self, ids, owner, q_init=None, **cfg):
         """ARock mode: owner agent per pose id, 6-DoF q_init [n, 4] (None = the attitudes given to set_poses); cfg overrides
         ArockConfig fields (self_id, dual_state_init_to_zero, rho_frame_T, rho_frame_theta, eta_k)."""
